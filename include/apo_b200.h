@@ -228,6 +228,7 @@ int apo_record_unpack16(const apo_record16 *in, uint64_t n, apo_record *out);
 #define APO_SCORE_CORPUS  0x1u   /* also run the 6-pattern scan over the corpus */
 #define APO_SCORE_RECIP   0x2u   /* finalReward = ws * (1/tw) from a LUT instead of ws / tw (<= 1 ulp apart) */
 #define APO_SCORE_TIMING  0x4u   /* record the per-stage CUDA events of apo_timing also for a small call */
+#define APO_SCORE_CANDIDATES 0x8u /* also build the per-candidate breakdown (apo_candidate_reports) */
 typedef struct apo_score_opts {
 	uint32_t K;          /* beam width (top-K), 0..min(C, 16384) */
 	uint32_t source;     /* APO_SRC_* */
@@ -320,6 +321,33 @@ int apo_last_timing(const apo_engine *e, apo_timing *out);
  * and the count; 4*C int64 words.  Order-independent, hence identical for any grid,
  * shard or rank count. */
 int apo_debug_partials(apo_engine *e, int64_t *out, uint32_t C);
+
+/* ---- per-candidate breakdown: why candidate c scored what it scored ------------------
+ * The corpus report (APO:498-625) answered per candidate, over the evaluations of c that the
+ * scoring call read (every window of a session, absolute record positions).  Built by a scoring
+ * call that sets APO_SCORE_CANDIDATES: apo_score, apo_score_finish (every apo_score_accumulate of
+ * the session must set it too) or any apo_score_host*.  Feedback tally of an evaluation: Form R /
+ * R16 from the feedback field (1 good, 2 bad, else none, whether or not VALID is set, as the
+ * corpus scan counts); Form D / Q / P / T from d0 = user_feedback (TCS:677-679): 1 good, -1 bad,
+ * anything else (absent included) none.  dim[i] covers the evaluations with a non-null
+ * finalReward in which dimension i is present: sum = exact integer sum of rint(v * 2^52) rounded
+ * once to binary64 (v = the fp32 value widened for Form D / Q / P / T, the TCS:668-763 binary64
+ * value for Form R / R16), avg = sum / count and the flags of APO:575/591/802/819, by the code
+ * that fills apo_corpus_report.dim.  A Form R candidate row therefore has the breakdown that the
+ * corpus report of that row has on every shared field.  Single rank only: APO_E_STATE on a handle
+ * after apo_comm_init with more than one rank (apo_comm_init with nranks == 1 leaves the handle
+ * single-rank, with no communicator, so the breakdown stays available). */
+typedef struct apo_candidate_report {
+	uint64_t total, good, bad, none;   /* evaluations of c in the scored window(s); tallies as APO:509-516 */
+	double   goodRate;                 /* good / (good + bad), 0 when both are 0 (APO:546-547) */
+	uint64_t withReward;               /* == counts[c] */
+	double   rewardSum, avgReward;     /* avgReward == scores[c] bit for bit; NaN (not -inf) when withReward == 0 */
+	apo_dimstat dim[APO_NDIM];         /* same rules and rounding as apo_corpus_report.dim */
+	int64_t  badExamples[3];           /* first 3 record indices (ascending) whose tally is 'bad'; -1 = none */
+} apo_candidate_report;
+/* Breakdown of candidates [c0, c0 + n) from the last scoring call.  APO_E_STATE when that call did
+ * not set APO_SCORE_CANDIDATES (or failed), APO_E_ARG when the range exceeds its C. */
+int apo_candidate_reports(apo_engine *e, uint32_t c0, uint32_t n, apo_candidate_report *out);
 
 /* ---- multi-GPU: the record axis is sharded across ranks (one process per GPU, or one handle per GPU inside one
  * process); the packed int64 partial vectors of the shards are joined INSIDE the scoring launch: the finalising CTA

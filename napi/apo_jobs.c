@@ -110,6 +110,14 @@ int apo_job_validate(apo_job *j)
 		if (j->corpus_bytes && !j->corpus) return bad(j, "corpus buffer missing");
 	}
 	if (j->K > 16384) return bad(j, "K exceeds the supported beam width 16384");
+	if (j->flags & APO_SCORE_CANDIDATES) {
+		if (j->kind != APO_JOB_SCORE_RESIDENT && j->kind != APO_JOB_SCORE_HOST && j->kind != APO_JOB_SCORE_HOST_RECORDS &&
+		    j->kind != APO_JOB_SCORE_HOST_TUPLES)
+			return bad(j, "the per-candidate breakdown belongs to a scoring call");
+		if (j->C == 0) return bad(j, "C must be > 0 for the per-candidate breakdown");
+		if (!fits(j->C, sizeof(apo_candidate_report), 1, APO_JOB_CANDIDATES_MAX_BYTES))
+			return bad(j, "the per-candidate breakdown of C candidates exceeds 4 GiB");
+	}
 	return APO_OK;
 }
 
@@ -120,7 +128,10 @@ int apo_job_prepare(apo_job *j)
 		 * caller passes C (the count it uploaded); the ABI re-checks K <= C against the loaded shape */
 		const uint32_t C = j->C ? j->C : 1, K = j->K ? j->K : 1;
 		j->scores = (double *)malloc(8u * (size_t)C); j->counts = (uint64_t *)malloc(8u * (size_t)C); j->topk = (int32_t *)malloc(4u * (size_t)K);
-		if (!j->scores || !j->counts || !j->topk) { apo_job_release(j); j->rc = APO_E_NOMEM; snprintf(j->err, sizeof j->err, "out of host memory"); return APO_E_NOMEM; }
+		if (j->flags & APO_SCORE_CANDIDATES) j->candidates = (apo_candidate_report *)malloc(sizeof(apo_candidate_report) * (size_t)C);
+		if (!j->scores || !j->counts || !j->topk || ((j->flags & APO_SCORE_CANDIDATES) && !j->candidates)) {
+			apo_job_release(j); j->rc = APO_E_NOMEM; snprintf(j->err, sizeof j->err, "out of host memory"); return APO_E_NOMEM;
+		}
 	} else if (j->kind == APO_JOB_REWARD_BATCH) {
 		const uint64_t n = j->buf_bytes / sizeof(apo_record);
 		j->n_out = n;
@@ -133,8 +144,8 @@ int apo_job_prepare(apo_job *j)
 
 void apo_job_release(apo_job *j)
 {
-	free(j->scores); free(j->counts); free(j->topk); free(j->dims_out); free(j->masks_out); free(j->finals_out);
-	j->scores = NULL; j->counts = NULL; j->topk = NULL; j->dims_out = NULL; j->masks_out = NULL; j->finals_out = NULL;
+	free(j->scores); free(j->counts); free(j->topk); free(j->dims_out); free(j->masks_out); free(j->finals_out); free(j->candidates);
+	j->scores = NULL; j->counts = NULL; j->topk = NULL; j->dims_out = NULL; j->masks_out = NULL; j->finals_out = NULL; j->candidates = NULL;
 }
 
 static void execute(apo_serial *s, apo_job *j)
@@ -191,6 +202,7 @@ static void execute(apo_serial *s, apo_job *j)
 	default:
 		j->rc = APO_E_ARG;
 	}
+	if (j->rc == APO_OK && j->candidates) j->rc = apo_candidate_reports(e, 0, j->C, j->candidates);
 	if (j->rc != APO_OK) snprintf(j->err, sizeof j->err, "%s", apo_last_error(e));
 }
 

@@ -145,8 +145,7 @@ class APOService:
                 if tot:
                     byMode[name] = {"total": tot, "good": g, "bad": b, "goodRate": float(rep.byModeGoodRate[m])}
             avgReward = None if rew.withReward == 0 else float(rew.avgReward)
-            rewardByDimension = {DIM_NAMES[i]: {"sum": float(rew.dim[i].sum), "count": int(rew.dim[i].count), "avg": float(rew.dim[i].avg)}
-                                 for i in range(9) if rew.dim[i].count}
+            rewardByDimension = self._rewardByDimension(rew)
         else:
             rep = rew = None
             good = bad = none = 0
@@ -168,13 +167,7 @@ class APOService:
                                "assistantMessagePreview": self._example_detail(p, t), "feedback": t["summary"]["userFeedback"]})
                 patterns.append({"id": str(uuid.uuid4()), "description": text, "frequency": int(q.count),
                                  "severity": SEVERITY[q.severity], "relatedCategory": cat, "examples": ex})
-            for i, name in enumerate(DIM_NAMES):                            # APO:574-596
-                d = rew.dim[i]
-                if d.count and d.low_flag:
-                    patterns.append({"id": str(uuid.uuid4()),
-                                     "description": f"{name} dimension reward signal consistently low (avg: {js_to_fixed(d.avg, 3)})",
-                                     "frequency": int(d.count), "severity": SEVERITY[d.low_severity],
-                                     "relatedCategory": DIM_CATEGORY.get(name, "core_behavior"), "examples": []})
+            patterns.extend(self._dimensionPatterns(rew))
 
         suggestions = self._generateLocalSuggestions(goodRate, patterns, byMode, avgReward, rew)
         report = {"id": str(uuid.uuid4()), "generatedAt": now,
@@ -187,6 +180,41 @@ class APOService:
         if suggestions:
             self._fire(self._suggestionListeners, suggestions)
         return report
+
+    @staticmethod
+    def _rewardByDimension(rew):
+        """APO:556-568 from a corpus report or a candidate report (same apo_dimstat fields)."""
+        return {DIM_NAMES[i]: {"sum": float(rew.dim[i].sum), "count": int(rew.dim[i].count), "avg": float(rew.dim[i].avg)}
+                for i in range(9) if rew.dim[i].count}
+
+    @staticmethod
+    def _dimensionPatterns(rew):
+        """APO:574-596: the dimension-low patterns of a corpus report or a candidate report."""
+        out = []
+        for i, name in enumerate(DIM_NAMES):
+            d = rew.dim[i]
+            if d.count and d.low_flag:
+                out.append({"id": str(uuid.uuid4()),
+                            "description": f"{name} dimension reward signal consistently low (avg: {js_to_fixed(d.avg, 3)})",
+                            "frequency": int(d.count), "severity": SEVERITY[d.low_severity],
+                            "relatedCategory": DIM_CATEGORY.get(name, "core_behavior"), "examples": []})
+        return out
+
+    def candidateReport(self, res, c):
+        """The report of one beam candidate, shaped like _buildReport's, from a ScoreResult scored with the per-candidate
+        breakdown (evaluateBeam(..., reports=True)): feedback tallies and goodRate of its rollouts, avgReward (== its score),
+        rewardByDimension, the dimension-low patterns and the suggestions they raise (the rules of APO:574-596, 800-827, by
+        the code _buildReport uses), and badExamples = the first three rollout indices with 'bad' feedback.  Pure: it
+        neither records the suggestions nor fires events nor touches storage."""
+        r = res.candidates[c]
+        goodRate = float(r.goodRate)
+        avgReward = None if r.withReward == 0 else float(r.avgReward)
+        patterns = self._dimensionPatterns(r)
+        return {"candidate": int(c), "totalRollouts": int(r.total), "goodFeedbackCount": int(r.good), "badFeedbackCount": int(r.bad),
+                "noFeedbackCount": int(r.none), "goodRate": goodRate, "avgReward": avgReward,
+                "rewardByDimension": self._rewardByDimension(r), "patterns": patterns,
+                "suggestions": self._generateLocalSuggestions(goodRate, patterns, {}, avgReward, r),
+                "badExamples": [int(x) for x in r.badExamples if x >= 0]}
 
     @staticmethod
     def _example_detail(p, t):
@@ -239,20 +267,22 @@ class APOService:
         return out
 
     # ---- beam evaluation: the step the reference delegates to its backend --------------------------------
-    def evaluateBeam(self, candidates, dims=None, rollouts=None):
+    def evaluateBeam(self, candidates, dims=None, rollouts=None, reports=False):
         """Score a beam of VersionedPromptTemplate candidates on their rollout outcomes and keep the
         top `beamWidth` (score desc, ties -> lower index), then apply the APO:1138-1166 update with the
         strict `>` adoption rule (APO:1159).  dims: float32 [C][T][9] (NaN = absent) or rollouts:
-        apo_record [C][T]."""
+        apo_record [C][T].  reports=True also builds the per-candidate breakdown (res.candidates, see
+        candidateReport)."""
         try:
             C = len(candidates)
             K = min(self._config["beamWidth"], C)
+            extra = {"candidates": True} if reports else {}
             if dims is not None:
                 self._engine.dims_upload(np.ascontiguousarray(dims, np.float32))
-                res = self._engine.score(C, K, source=SRC_DIMS)
+                res = self._engine.score(C, K, source=SRC_DIMS, **extra)
             else:
                 self._engine.rollouts_upload(rollouts)
-                res = self._engine.score(C, K, source=SRC_ROLLOUTS)
+                res = self._engine.score(C, K, source=SRC_ROLLOUTS, **extra)
             beam = []
             for c in res.topk:
                 tpl = dict(candidates[int(c)])
@@ -266,25 +296,32 @@ class APOService:
             print("[APO] Beam evaluation failed:", e)
             return None
 
-    def runBeamSearch(self, seedPrompt, proposeCandidates, rolloutDims, rounds=None):
+    def runBeamSearch(self, seedPrompt, proposeCandidates, rolloutDims, rounds=None, withReports=False):
         """Client-side round driver (SURVEY 8f rank 3) around the GPU top-K: each round expands every beam
         member into `branchFactor` children through the caller's `proposeCandidates(parent, n) -> [content]`
         hook (the LLM critique/edit step of APO:918-988 lives there), scores parents + children on
         `rolloutDims(candidates) -> float32 [C][T][9]`, keeps the top `beamWidth` and applies the
-        APO:1138-1166 update.  Returns the final beam state."""
+        APO:1138-1166 update.  withReports=True calls `proposeCandidates(parent, n, report)` instead, with the
+        candidateReport of the parent from the round that scored it (None for the unscored seed), so that the
+        critique can name what the parent lost on.  Returns the final beam state."""
         rounds = rounds or self._config["beamRounds"]
         beam = [{"version": "v0", "content": seedPrompt, "score": None, "createdAt": time.time() * 1000.0}]
         counter = 0
+        reports = {}                                                         # version -> candidateReport of its last scoring
         for _ in range(rounds):
             cands = list(beam)
             for parent in beam:
-                for content in proposeCandidates(parent, self._config["branchFactor"]):
+                proposed = (proposeCandidates(parent, self._config["branchFactor"], reports.get(parent["version"])) if withReports
+                            else proposeCandidates(parent, self._config["branchFactor"]))
+                for content in proposed:
                     counter += 1
                     cands.append({"version": f"v{counter}", "content": content, "score": None,
                                   "parentVersion": parent["version"], "createdAt": time.time() * 1000.0})
-            res = self.evaluateBeam(cands, dims=rolloutDims(cands))
+            res = self.evaluateBeam(cands, dims=rolloutDims(cands), reports=withReports)
             if res is None:
                 break
+            if withReports:
+                reports = {cands[int(c)]["version"]: self.candidateReport(res, int(c)) for c in res.topk}
             beam = self._beamState["beam"]
             self._beamState["versionCounter"] = counter
         return self.getBeamState()

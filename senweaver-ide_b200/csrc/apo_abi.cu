@@ -134,6 +134,14 @@ struct apo_engine {
 	size_t k1_used = 0;
 	uint32_t score_C = 0; bool scoring = false;
 	apo_timing timing{};
+	// per-candidate breakdown (APO_SCORE_CANDIDATES, csrc/apo_cand.cu): its own integers, never part of the accumulator vector
+	DevBuf<long long> cand_acc;              // [C][CB_INT] integers | [C][3] first-three 'bad' slots
+	DevBuf<apo_candidate_report> cand_rep;   // reports of the last flagged call
+	DevBuf<float> cand_book;                 // Form T: [8][16] code -> fp32 value of the dictionary's codebook
+	uint32_t cand_C = 0;
+	bool cand_armed = false;                 // cand_acc zeroed for this call / session
+	bool cand_every = true;                  // every accumulate of the session so far set the flag
+	bool cand_ready = false;                 // cand_rep holds the breakdown of the last scoring call
 };
 
 namespace {
@@ -477,6 +485,7 @@ int begin_score(apo_engine *e, uint32_t C, bool whole = false) {
 	e->acc_clean_words = 0;                         // from here on the block is in use
 	e->partials_src = e->nranks > 1 ? e->acc_joined.p : e->acc.p;
 	e->last_C = C; e->score_C = C; e->scoring = true; e->k1_used = 0;
+	e->cand_armed = false; e->cand_every = true; e->cand_ready = false;
 	e->timing = apo_timing{};
 	if (e->timing_on) CK(cudaEventRecord(e->ev[0], e->stream));
 	return APO_OK;
@@ -573,6 +582,83 @@ int launch_k1_resident(apo_engine *e, const apo_score_opts *o, uint32_t cand_off
 	CK(apo::run_reward9(P, row, (int)o->variant, (o->flags & APO_SCORE_RECIP) != 0, e->sm_count, e->stream));
 	if ((rc = record_k1_event(e, 1))) return rc;
 	e->timing.launches++;
+	return APO_OK;
+}
+
+// ---- per-candidate breakdown (APO_SCORE_CANDIDATES)
+bool wants_cand(const apo_score_opts *o) { return (o->flags & APO_SCORE_CANDIDATES) != 0; }
+
+int cand_check(apo_engine *e) {
+	if (e->nranks > 1)
+		return fail(e, APO_E_STATE, "APO_SCORE_CANDIDATES is single-rank only: the per-candidate breakdown is not joined across the %d ranks of this handle", e->nranks);
+	return APO_OK;
+}
+
+// zero the breakdown of C candidates (first flagged launch of a call or session)
+int cand_arm(apo_engine *e, uint32_t C) {
+	const uint64_t words = (uint64_t)C * (apo::CB_INT + 3);
+	CK(e->cand_acc.reserve(words));
+	CK(cudaMemsetAsync(e->cand_acc.p, 0, words * 8, e->stream));
+	e->cand_armed = true;
+	return APO_OK;
+}
+
+apo::CandParams cand_params(apo_engine *e, uint32_t C, uint64_t T, uint64_t idx_base, uint32_t cand_offset, uint64_t pitch_evals) {
+	apo::CandParams P{};
+	P.C = C; P.T = T; P.idx_base = idx_base; P.pitch_evals = pitch_evals; P.lut = e->d_lut.p;
+	P.ints = e->cand_acc.p + (uint64_t)apo::CB_INT * cand_offset;
+	P.ex = (unsigned long long *)(e->cand_acc.p + (uint64_t)apo::CB_INT * e->score_C) + 3ull * cand_offset;
+	return P;
+}
+
+int cand_launch(apo_engine *e, const apo::CandParams &P, int source) {
+	CK(apo::run_cand_breakdown(P, source, e->sm_count, e->stream));
+	e->timing.launches++;
+	return APO_OK;
+}
+
+// Form T dictionary codebook -> [8][16] fp32 values (4-bit codes, csrc/apo_tuple.cu)
+int cand_upload_tbook(apo_engine *e, const uint32_t *codebook) {
+	uint32_t tab[8 * 16];
+	for (int j = 0; j < 8; j++) for (int k = 0; k < 16; k++) tab[16 * j + k] = codebook[256 * j + k];
+	CK(e->cand_book.reserve(8 * 16));
+	CK(cudaMemcpyAsync(e->cand_book.p, tab, sizeof tab, cudaMemcpyHostToDevice, e->stream));   // pageable source: consumed when this returns
+	return APO_OK;
+}
+
+// breakdown of the loaded source over [first, first+count) into candidates [cand_offset, ...)
+int launch_cand_resident(apo_engine *e, const apo_score_opts *o, uint32_t cand_offset, uint64_t first, uint64_t count) {
+	if (!count) return APO_OK;
+	if (o->source == APO_SRC_TUPLES) {
+		int rc = cand_upload_tbook(e, e->tup_book);
+		if (rc) return rc;
+		apo::CandParams P = cand_params(e, e->tup_C, count, first, cand_offset, e->tup_pitch);
+		P.tl = e->tup_l.p + first; P.th = e->tup_h.p + first; P.tb_pc = e->tup_pc.p; P.tb_pd = e->tup_pd.p; P.n_tuples = e->tup_n;
+		P.tbook = e->cand_book.p; P.d2book = e->tup_d2.p;
+		return cand_launch(e, P, apo::CAND_T);
+	}
+	if (o->source == APO_SRC_ROLLOUTS) {
+		apo::CandParams P = cand_params(e, e->roll_C, count, first, cand_offset, e->roll_pitch);
+		P.rows = e->roll.p + first * e->roll_row;
+		return cand_launch(e, P, e->roll_row == 32 ? apo::CAND_REC32 : apo::CAND_REC16);
+	}
+	apo::CandParams P = cand_params(e, e->dims_C, count, first, cand_offset, e->dims_pitch);
+	if (e->compact) {
+		P.q8 = e->q8.p + first; P.d2 = e->qd2.p + first; P.li = e->qli.p + first; P.cbf = e->d_cbf.p;
+		return cand_launch(e, P, apo::CAND_Q);
+	}
+	P.rows = (const uint8_t *)(e->dims_ptr + first * APO_NDIM);
+	return cand_launch(e, P, apo::CAND_DIMS);
+}
+
+// integers -> apo_candidate_report[C]; after the scoring call has completed (its partials are final)
+int cand_finish(apo_engine *e, uint32_t C) {
+	CK(e->cand_rep.reserve(C ? C : 1));
+	const long long *partials = e->partials_src ? e->partials_src : e->acc.p;
+	CK(apo::run_cand_report(e->cand_acc.p, (const unsigned long long *)(e->cand_acc.p + (uint64_t)apo::CB_INT * C), partials, C, e->cand_rep.p, e->stream));
+	e->timing.launches++;
+	CK(cudaStreamSynchronize(e->stream));
+	e->cand_C = C; e->cand_ready = true;
 	return APO_OK;
 }
 
@@ -841,6 +927,7 @@ extern "C" void apo_destroy(apo_engine *e) {
 	e->d_lut.release(); e->corpus.release(); e->dims.release(); e->roll.release(); e->acc.release(); e->acc_joined.release(); e->acc_snapshot.release(); e->misc.release();
 	e->result.release(); e->keys.release(); e->sel_key.release(); e->sel_idx.release();
 	e->tups_pc.release(); e->tups_pd.release(); e->tups_d2.release();
+	e->cand_acc.release(); e->cand_rep.release(); e->cand_book.release();
 	e->tup_l.release(); e->tup_h.release(); e->tup_pc.release(); e->tup_pd.release(); e->tup_bad.release(); e->tup_d2.release(); e->tup_ptab.release(); e->tup_val.release();
 	e->win[0].release(); e->win[1].release(); e->batch_in.release(); e->batch_out.release(); e->batch_mask.release();
 	if (e->h_result) cudaFreeHost(e->h_result);
@@ -1202,28 +1289,47 @@ extern "C" int apo_score_accumulate(apo_engine *e, const apo_score_opts *o, uint
 	if (o->first % 4) return fail(e, APO_E_ARG, "window start must be a multiple of 4");
 	if (o->first > T || (o->count && o->first + o->count > T)) return fail(e, APO_E_ARG, "window outside [0,%llu)", (unsigned long long)T);
 	first = o->first; count = o->count ? o->count : T - o->first;
+	const bool cand = wants_cand(o);
+	if (cand && (rc = cand_check(e))) return rc;
 	CK(cudaSetDevice(e->device));
-	return launch_k1_resident(e, o, cand_offset, first, count);
+	if ((rc = launch_k1_resident(e, o, cand_offset, first, count))) return rc;
+	if (!cand) { e->cand_every = false; return APO_OK; }
+	if (!e->cand_every) return APO_OK;                  // an earlier accumulate of the session did not set the flag: finish refuses
+	if (!e->cand_armed && (rc = cand_arm(e, e->score_C))) return rc;
+	return launch_cand_resident(e, o, cand_offset, first, count);
 }
 
 extern "C" int apo_score_finish(apo_engine *e, const apo_score_opts *o, double *scores, uint64_t *counts, int32_t *topk,
                                 apo_corpus_report *report) {
 	if (!e) return APO_E_ARG;
+	e->cand_ready = false;                              // a failed finish leaves no breakdown behind either
 	if (!o) return fail(e, APO_E_ARG, "opts is NULL");
 	if (!e->scoring) return fail(e, APO_E_STATE, "apo_score_begin has not been called");
 	if (o->K > e->score_C) return fail(e, APO_E_ARG, "K=%u exceeds the number of candidates C=%u", o->K, e->score_C);
 	if (o->K > kMaxK) return fail(e, APO_E_ARG, "K=%u exceeds the supported beam width %u", o->K, kMaxK);
+	const bool cand = wants_cand(o);
+	int rc;
+	if (cand) {
+		if ((rc = cand_check(e))) return rc;
+		if (!e->cand_every)
+			return fail(e, APO_E_STATE, "APO_SCORE_CANDIDATES: every apo_score_accumulate of the session must set the flag for a breakdown");
+	}
 	CK(cudaSetDevice(e->device));
+	if (cand && !e->cand_armed && (rc = cand_arm(e, e->score_C))) return rc;   // nothing accumulated yet: an empty breakdown
 	if (peer_join_active(e, e->score_C)) e->join_epoch++;
-	return finish_score(e, o, e->score_C, scores, counts, topk, report);
+	if ((rc = finish_score(e, o, e->score_C, scores, counts, topk, report))) return rc;
+	return cand ? cand_finish(e, e->score_C) : APO_OK;
 }
 
 extern "C" int apo_score(apo_engine *e, const apo_score_opts *o, double *scores, uint64_t *counts, int32_t *topk, apo_corpus_report *report) {
 	if (!e) return APO_E_ARG;
+	e->cand_ready = false;                              // a failed call leaves no breakdown behind either
 	uint32_t C = 0; uint64_t T = 0, first = 0, count = 0;
 	int rc = source_shape(e, o, &C, &T);
 	if (rc) return rc;
 	if ((rc = check_opts(e, o, C, T, &first, &count))) return rc;
+	const bool cand = wants_cand(o);
+	if (cand && (rc = cand_check(e))) return rc;
 	CK(cudaSetDevice(e->device));
 	if ((rc = ensure_scratch(e, C, o->K))) return rc;
 	const bool tup = o->source == APO_SRC_TUPLES;      // gather-and-add kernel: stand-alone corpus scan + tail
@@ -1248,23 +1354,29 @@ extern "C" int apo_score(apo_engine *e, const apo_score_opts *o, double *scores,
 	const bool tail_only = !tup && !wants_corpus(e, o) && one_launch && count > 0 && !e->env_no_fuse;
 	if (fuse || tail_only) {
 		if ((rc = begin_score(e, C, true))) return rc;
+		if (cand && (rc = cand_arm(e, C))) return rc;
 		apo::FinalizeParams F = make_fin(e, C, o->K, fuse ? 1 : 0);
 		const bool self_clean = one_launch;          // the finalising CTA is in this launch: it can leave the block zeroed
 		if (self_clean) { F.clean_ptr = e->acc.p; F.clean_words = (uint32_t)(acc_words(C, e->nranks) + ARM_WORDS); F.snapshot = e->acc_snapshot.p; }
 		apo::K2Params k2 = make_k2(e, C, F);
 		if (tail_only) { k2.T = 0; k2.recs = nullptr; }
 		if ((rc = launch_k1_resident(e, o, 0, first, count, &k2))) return rc;
+		if (cand && (rc = launch_cand_resident(e, o, 0, first, count))) return rc;
 		rc = finish_score(e, o, C, scores, counts, topk, report, true);
 		if (rc == APO_OK && self_clean) {
 			e->acc_clean_words = F.clean_words;
 			if (e->nranks == 1) e->partials_src = e->acc_snapshot.p;
 		}
+		if (rc == APO_OK && cand) rc = cand_finish(e, C);
 		return rc;
 	} else {
 		if ((rc = begin_score(e, C))) return rc;
+		if (cand && (rc = cand_arm(e, C))) return rc;
 		if ((rc = launch_k1_resident(e, o, 0, first, count))) return rc;
+		if (cand && (rc = launch_cand_resident(e, o, 0, first, count))) return rc;
 	}
-	return finish_score(e, o, C, scores, counts, topk, report, fuse || tail_only);
+	if ((rc = finish_score(e, o, C, scores, counts, topk, report, fuse || tail_only))) return rc;
+	return cand ? cand_finish(e, C) : APO_OK;
 }
 
 namespace {
@@ -1273,13 +1385,16 @@ namespace {
 int score_host_rows_impl(apo_engine *e, const apo_score_opts *o, const uint8_t *rows, uint32_t row, uint32_t C, uint64_t T,
                          double *scores, uint64_t *counts, int32_t *topk, apo_corpus_report *report) {
 	if (!e) return APO_E_ARG;
+	e->cand_ready = false;
 	if (!o) return fail(e, APO_E_ARG, "opts is NULL");
 	if (!rows || C == 0) return fail(e, APO_E_ARG, "input is NULL or C == 0");
 	if (o->K > C) return fail(e, APO_E_ARG, "K=%u exceeds the number of candidates C=%u", o->K, C);
 	if (o->K > kMaxK) return fail(e, APO_E_ARG, "K=%u exceeds the supported beam width %u", o->K, kMaxK);
 	if (o->first || o->count) return fail(e, APO_E_ARG, "windows are not supported by the host-streaming calls");
-	CK(cudaSetDevice(e->device));
+	const bool cand = wants_cand(o);
 	int rc;
+	if (cand && (rc = cand_check(e))) return rc;
+	CK(cudaSetDevice(e->device));
 	if ((rc = ensure_scratch(e, C, o->K))) return rc;
 	// window of ~256 MB per buffer, a multiple of the K1 tile so chunks never split a tile
 	const int tile = apo::k1_tile_evals((int)row, (int)o->variant);
@@ -1296,6 +1411,7 @@ int score_host_rows_impl(apo_engine *e, const apo_score_opts *o, const uint8_t *
 	choose_timing(e, o, (uint64_t)C * T * row);
 	if (peer_join_active(e, C)) e->join_epoch++;
 	if ((rc = begin_score(e, C))) return rc;
+	if (cand && (rc = cand_arm(e, C))) return rc;
 	const bool recip = (o->flags & APO_SCORE_RECIP) != 0;
 	int nchunk = 0;
 	for (uint64_t t0 = 0; t0 < T; t0 += Tc, nchunk++) {
@@ -1324,9 +1440,15 @@ int score_host_rows_impl(apo_engine *e, const apo_score_opts *o, const uint8_t *
 		CK(apo::run_reward9(P, (int)row, (int)o->variant, recip, e->sm_count, e->stream));
 		if ((rc = record_k1_event(e, 1))) return rc;
 		e->timing.launches++;
+		if (cand) {
+			apo::CandParams B = cand_params(e, C, n, t0, 0, Tc);
+			B.rows = e->win[b].p;
+			if ((rc = cand_launch(e, B, row == 36 ? apo::CAND_DIMS : row == 32 ? apo::CAND_REC32 : apo::CAND_REC16))) return rc;
+		}
 		CK(cudaEventRecord(e->win_free[b], e->stream));
 	}
-	return finish_score(e, o, C, scores, counts, topk, report);
+	if ((rc = finish_score(e, o, C, scores, counts, topk, report))) return rc;
+	return cand ? cand_finish(e, C) : APO_OK;
 }
 
 int score_host_rows(apo_engine *e, const apo_score_opts *o, const uint8_t *rows, uint32_t row, uint32_t C, uint64_t T,
@@ -1437,13 +1559,16 @@ int score_host_compact_impl(apo_engine *e, const apo_score_opts *o, const uint64
                             const uint32_t *codebook, uint32_t C, uint64_t T, double *scores, uint64_t *counts, int32_t *topk,
                             apo_corpus_report *report) {
 	const bool packed = pc != nullptr;
+	e->cand_ready = false;
 	if (!o) return fail(e, APO_E_ARG, "opts is NULL");
 	if (!codebook || C == 0 || (packed ? (!pd || !d2book) : (!q8 || !d2 || !li))) return fail(e, APO_E_ARG, "input is NULL or C == 0");
 	if (o->K > C) return fail(e, APO_E_ARG, "K=%u exceeds the number of candidates C=%u", o->K, C);
 	if (o->K > kMaxK) return fail(e, APO_E_ARG, "K=%u exceeds the supported beam width %u", o->K, kMaxK);
 	if (o->first || o->count) return fail(e, APO_E_ARG, "windows are not supported by the host-streaming calls");
-	CK(cudaSetDevice(e->device));
+	const bool cand = wants_cand(o);
 	int rc;
+	if (cand && (rc = cand_check(e))) return rc;
+	CK(cudaSetDevice(e->device));
 	if ((rc = ensure_scratch(e, C, o->K))) return rc;
 	// the lookup tables of K1q follow the codebook of THIS call; a resident Form Q tensor keeps its own and gets it back when the
 	// call returns, on every path (Restore)
@@ -1472,6 +1597,7 @@ int score_host_compact_impl(apo_engine *e, const apo_score_opts *o, const uint64
 	choose_timing(e, o, (uint64_t)C * T * wire);
 	if (peer_join_active(e, C)) e->join_epoch++;
 	if ((rc = begin_score(e, C))) return rc;
+	if (cand && (rc = cand_arm(e, C))) return rc;
 	int nchunk = 0;
 	for (uint64_t t0 = 0; t0 < T; t0 += Tc, nchunk++) {
 		const int b = nchunk & 1;
@@ -1509,9 +1635,15 @@ int score_host_compact_impl(apo_engine *e, const apo_score_opts *o, const uint64
 		CK(apo::run_reward9q(Q, qv, (o->flags & APO_SCORE_RECIP) != 0, e->sm_count, e->stream));
 		if ((rc = record_k1_event(e, 1))) return rc;
 		e->timing.launches++;
+		if (cand) {
+			apo::CandParams B = cand_params(e, C, n, t0, 0, Tc);
+			B.q8 = wq; B.d2 = wd; B.li = wl; B.cbf = e->d_cbf.p;           // the tables of this call's codebook (upload_ptab above)
+			if ((rc = cand_launch(e, B, apo::CAND_Q))) return rc;
+		}
 		CK(cudaEventRecord(e->win_free[b], e->stream));
 	}
-	return finish_score(e, o, C, scores, counts, topk, report);
+	if ((rc = finish_score(e, o, C, scores, counts, topk, report))) return rc;
+	return cand ? cand_finish(e, C) : APO_OK;
 }
 }  // namespace
 
@@ -1549,12 +1681,15 @@ int tuples_args(apo_engine *e, const uint16_t *tl, const uint8_t *th, const uint
 int score_host_tuples_impl(apo_engine *e, const apo_score_opts *o, const uint16_t *tl, const uint8_t *th, const uint32_t *tb_pc,
                            const uint16_t *tb_pd, uint32_t n_tuples, const uint32_t *codebook, const uint32_t *d2book, uint32_t C, uint64_t T,
                            double *scores, uint64_t *counts, int32_t *topk, apo_corpus_report *report) {
+	e->cand_ready = false;
 	if (!o) return fail(e, APO_E_ARG, "opts is NULL");
 	int rc;
 	if ((rc = tuples_args(e, tl, th, tb_pc, tb_pd, n_tuples, codebook, d2book, C, T))) return rc;
 	if (o->K > C) return fail(e, APO_E_ARG, "K=%u exceeds the number of candidates C=%u", o->K, C);
 	if (o->K > kMaxK) return fail(e, APO_E_ARG, "K=%u exceeds the supported beam width %u", o->K, kMaxK);
 	if (o->first || o->count) return fail(e, APO_E_ARG, "windows are not supported by the host-streaming calls");
+	const bool cand = wants_cand(o);
+	if (cand && (rc = cand_check(e))) return rc;
 	CK(cudaSetDevice(e->device));
 	if ((rc = ensure_scratch(e, C, o->K))) return rc;
 	const int tile = apo::kt_tile_evals();
@@ -1569,6 +1704,7 @@ int score_host_tuples_impl(apo_engine *e, const apo_score_opts *o, const uint16_
 	choose_timing(e, o, (uint64_t)C * T * 3);
 	if (peer_join_active(e, C)) e->join_epoch++;
 	if ((rc = begin_score(e, C))) return rc;
+	if (cand && ((rc = cand_arm(e, C)) || (rc = cand_upload_tbook(e, codebook)))) return rc;
 	if (n_tuples) {
 		CK(cudaMemcpyAsync(e->tups_pc.p, tb_pc, (uint64_t)n_tuples * 4, cudaMemcpyHostToDevice, e->stream));
 		CK(cudaMemcpyAsync(e->tups_pd.p, tb_pd, (uint64_t)n_tuples * 2, cudaMemcpyHostToDevice, e->stream));
@@ -1593,9 +1729,16 @@ int score_host_tuples_impl(apo_engine *e, const apo_score_opts *o, const uint16_
 		CK(apo::run_reward9t(P, e->sm_count, e->stream));
 		if ((rc = record_k1_event(e, 1))) return rc;
 		e->timing.launches++;
+		if (cand) {
+			apo::CandParams B = cand_params(e, C, n, t0, 0, Tc);
+			B.tl = wl; B.th = wh; B.tb_pc = e->tups_pc.p; B.tb_pd = e->tups_pd.p; B.n_tuples = n_tuples;
+			B.tbook = e->cand_book.p; B.d2book = e->tups_d2.p;
+			if ((rc = cand_launch(e, B, apo::CAND_T))) return rc;
+		}
 		CK(cudaEventRecord(e->win_free[b], e->stream));
 	}
-	return finish_score(e, o, C, scores, counts, topk, report);
+	if ((rc = finish_score(e, o, C, scores, counts, topk, report))) return rc;
+	return cand ? cand_finish(e, C) : APO_OK;
 }
 }  // namespace
 
@@ -1669,6 +1812,18 @@ extern "C" int apo_debug_partials(apo_engine *e, int64_t *out, uint32_t C) {
 	if (C != e->last_C || !e->acc.p) return fail(e, APO_E_STATE, "no scoring call with C=%u to read back", C);
 	CK(cudaSetDevice(e->device));
 	CK(cudaMemcpyAsync(out, e->partials_src ? e->partials_src : e->acc.p, 8ull * ACC_PER_CAND * C, cudaMemcpyDeviceToHost, e->stream));
+	CK(cudaStreamSynchronize(e->stream));
+	return APO_OK;
+}
+
+extern "C" int apo_candidate_reports(apo_engine *e, uint32_t c0, uint32_t n, apo_candidate_report *out) {
+	if (!e) return APO_E_ARG;
+	if (!e->cand_ready) return fail(e, APO_E_STATE, "the last scoring call did not set APO_SCORE_CANDIDATES");
+	if ((uint64_t)c0 + n > e->cand_C) return fail(e, APO_E_ARG, "candidates [%u,%llu) exceed C=%u", c0, (unsigned long long)c0 + n, e->cand_C);
+	if (n == 0) return APO_OK;
+	if (!out) return fail(e, APO_E_ARG, "out is NULL");
+	CK(cudaSetDevice(e->device));
+	CK(cudaMemcpyAsync(out, e->cand_rep.p + c0, (uint64_t)n * sizeof(apo_candidate_report), cudaMemcpyDeviceToHost, e->stream));
 	CK(cudaStreamSynchronize(e->stream));
 	return APO_OK;
 }

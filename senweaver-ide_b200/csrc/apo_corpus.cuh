@@ -258,6 +258,31 @@ __device__ __forceinline__ unsigned long long score_key(double s) {
 	return (b >> 63) ? ~b : (b | 0x8000000000000000ull);     // ascending order-preserving map
 }
 
+// The numeric rules of a report, shared by the corpus report (build_report) and the per-candidate breakdown
+// (csrc/apo_cand.cu k_cand_report) so that the two cannot drift apart.
+// good / (good + bad), 0 when both are 0 (APO:546-547, APO:541-544)
+__device__ __forceinline__ double report_good_rate(uint64_t good, uint64_t bad) {
+	const uint64_t twf = good + bad;
+	return twf > 0 ? __ddiv_rn((double)good, (double)twf) : 0.0;
+}
+// rewardSum / withReward, NaN (null) when nothing carried a reward (APO:550-553)
+__device__ __forceinline__ double report_avg_reward(double rsum, uint64_t nrew) {
+	return nrew > 0 ? __ddiv_rn(rsum, (double)nrew) : __longlong_as_double(0x7ff8000000000000ll);
+}
+// rewardByDimension entry from its exact (l0, l1, l2, count) words: APO:556-568 + rules APO:575,591,802,819
+__device__ __forceinline__ apo_dimstat report_dimstat(const long long l[4]) {
+	apo_dimstat D;
+	D.sum = limbs_to_double(l);
+	D.count = (uint64_t)l[3];
+	D.avg = D.count > 0 ? __ddiv_rn(D.sum, (double)D.count) : 0.0;                       // APO:567
+	D.low_flag = (D.count >= 5 && D.avg < -0.3) ? 1 : 0;                                 // APO:575
+	D.low_severity = D.avg < -0.5 ? 2 : 1;                                               // APO:591
+	D.sugg_flag = (D.count >= 3 && D.avg < 0.0) ? 1 : 0;                                 // APO:802
+	D.sugg_priority = D.avg < -0.5 ? 2 : 1;                                              // APO:819
+	for (int k = 0; k < 4; k++) D.pad[k] = 0;
+	return D;
+}
+
 // APO:498-625 / TCS:596-626 from the joined corpus block.  Block-wide: thread 0 the tallies, threads 1..9 one
 // dimension each, threads 10..15 one pattern each (a single thread walking all of it costs ~10 us of serial latency).
 static __device__ void build_report(const FinalizeParams &F, const long long *corp_g) {
@@ -267,38 +292,27 @@ static __device__ void build_report(const FinalizeParams &F, const long long *co
 		R.total = (uint64_t)__ldcg(corp_g + CORP_NREC);
 		const uint64_t good = (uint64_t)__ldcg(corp_g + CORP_TALLY), bad = (uint64_t)__ldcg(corp_g + CORP_TALLY + 1);
 		R.good = good; R.bad = bad; R.none = (uint64_t)__ldcg(corp_g + CORP_TALLY + 2);
-		const uint64_t twf = good + bad;
-		R.goodRate = twf > 0 ? __ddiv_rn((double)good, (double)twf) : 0.0;                       // APO:546-547
+		R.goodRate = report_good_rate(good, bad);                                                // APO:546-547
 		for (int m = 0; m < APO_NMODE; m++) {
 			uint64_t v[3];
 			for (int k = 0; k < 3; k++) { v[k] = (uint64_t)__ldcg(corp_g + CORP_MODE + 3 * m + k); R.byMode[m][k] = v[k]; }
-			const uint64_t tot = v[1] + v[2];
-			R.byModeGoodRate[m] = tot > 0 ? __ddiv_rn((double)v[1], (double)tot) : 0.0;         // APO:541-544
+			R.byModeGoodRate[m] = report_good_rate(v[1], v[2]);                                  // APO:541-544
 		}
 		long long l[4];
 		for (int q = 0; q < 4; q++) l[q] = __ldcg(corp_g + CORP_REWARD + q);
 		const uint64_t nrew = (uint64_t)l[3];
 		const double rsum = limbs_to_double(l);
 		R.withReward = nrew; R.rewardSum = rsum;
-		R.avgReward = nrew > 0 ? __ddiv_rn(rsum, (double)nrew) : __longlong_as_double(0x7ff8000000000000ll);
+		R.avgReward = report_avg_reward(rsum, nrew);
 		const uint64_t tc = (uint64_t)__ldcg(corp_g + CORP_TOOL), ts = (uint64_t)__ldcg(corp_g + CORP_TOOL + 1);
 		R.toolCalls = tc; R.toolSucc = ts; R.toolFail = (uint64_t)__ldcg(corp_g + CORP_TOOL + 2);
 		R.toolSuccessRate = tc > 0 ? __ddiv_rn((double)ts, (double)tc)                          // TCS:624
 		                           : __longlong_as_double(0x7ff8000000000000ll);
 	} else if (tid <= APO_NDIM) {
 		const int i = tid - 1;
-		apo_dimstat D;
 		long long l[4];
 		for (int q = 0; q < 4; q++) l[q] = __ldcg(corp_g + CORP_DIM + 4 * i + q);
-		D.sum = limbs_to_double(l);
-		D.count = (uint64_t)l[3];
-		D.avg = D.count > 0 ? __ddiv_rn(D.sum, (double)D.count) : 0.0;                       // APO:567
-		D.low_flag = (D.count >= 5 && D.avg < -0.3) ? 1 : 0;                                 // APO:575
-		D.low_severity = D.avg < -0.5 ? 2 : 1;                                               // APO:591
-		D.sugg_flag = (D.count >= 3 && D.avg < 0.0) ? 1 : 0;                                 // APO:802
-		D.sugg_priority = D.avg < -0.5 ? 2 : 1;                                              // APO:819
-		for (int k = 0; k < 4; k++) D.pad[k] = 0;
-		R.dim[i] = D;
+		R.dim[i] = report_dimstat(l);
 	} else if (tid <= APO_NDIM + APO_NPAT) {
 		const int p = tid - 1 - APO_NDIM;
 		const uint64_t minc[APO_NPAT] = {2, 2, 3, 2, 2, 2};                                      // APO:645,671,695,715,736,756

@@ -177,6 +177,39 @@ int kt_tile_evals();
 cudaError_t run_tuple_values(const TupleValParams &P, bool recip, cudaStream_t st);
 cudaError_t run_reward9t(KtParams P, int sm_count, cudaStream_t st);
 
+// ---- per-candidate breakdown (csrc/apo_cand.cu): a second pass over the evaluations a scoring call reads.
+// Own integer buffer, never part of the scoring accumulator vector: [C][CB_INT] words (a later cross-rank join is one
+// integer sum of this part) followed by the first-three 'bad' slots [nranks][C][3] (inverted indices as ex_insert keeps them).
+constexpr int CB_DIM = 0;        // 9 x (l0, l1, l2, count): exact sum of rint(v * 2^52) over non-null evaluations where dim i is present
+constexpr int CB_TALLY = 36;     // total, good, bad
+constexpr int CB_INT = 39;
+enum CandSource { CAND_DIMS = 0, CAND_REC32 = 1, CAND_REC16 = 2, CAND_Q = 3, CAND_T = 4 };
+struct CandParams {
+	uint32_t C;
+	uint64_t T;                     // evaluations per candidate in this launch
+	uint64_t idx_base;              // record position of evaluation 0 of this launch (window start / streamed chunk start)
+	uint64_t pitch_evals;           // candidate row pitch in evaluations
+	const uint8_t *rows;            // Form D (36 B) / R (32 B) / R16 (16 B): evaluation 0 of candidate 0
+	const unsigned long long *q8;   // Form Q planes
+	const float *d2;
+	const unsigned short *li;
+	const float *cbf;               // Form Q: [8][256] code -> fp32 value
+	const unsigned short *tl;       // Form T planes + dictionary
+	const unsigned char *th;
+	const uint32_t *tb_pc;
+	const unsigned short *tb_pd;
+	uint32_t n_tuples;
+	const float *tbook;             // Form T: [8][16] 4-bit code -> fp32 value
+	const float *d2book;            // Form T: [4096] tool_success_rate values
+	const double *lut;              // natural-mask LUT [512] total weight (<= 0: finalReward null)
+	long long *ints;                // [C][CB_INT] of candidate 0 of this launch
+	unsigned long long *ex;         // [C][3] of candidate 0 of this launch
+};
+cudaError_t run_cand_breakdown(const CandParams &P, int source, int sm_count, cudaStream_t st);
+// ints / ex: the whole buffer; partials: the scoring call's candidate accumulators (4 words per candidate)
+cudaError_t run_cand_report(const long long *ints, const unsigned long long *ex, const long long *partials, uint32_t C,
+                            apo_candidate_report *out, cudaStream_t st);
+
 int k1_tile_evals(int row, int variant);
 cudaError_t run_reward9(K1Params P, int row, int variant, bool recip, int sm_count, cudaStream_t st);
 cudaError_t run_detect6(const K2Params &P, int sm_count, cudaStream_t st);

@@ -20,7 +20,7 @@
 import { VSBuffer } from '../../../../base/common/buffer.js';
 import { ApoResidentQuery, ApoScoreBlocks, ApoTupleBuffers, IApoScoringService } from '../common/apoScoringService.js';
 
-type Blocks = { scores: ArrayBuffer; counts: ArrayBuffer; topk: ArrayBuffer; report: ArrayBuffer };
+type Blocks = { scores: ArrayBuffer; counts: ArrayBuffer; topk: ArrayBuffer; report: ArrayBuffer; candidates?: ArrayBuffer };
 
 interface ApoAddon {
 	create(device: number): unknown | null;             // null when no H100 / library: never throws
@@ -30,11 +30,12 @@ interface ApoAddon {
 	corpusUpload(handle: unknown, records: ArrayBuffer, idxBase: number): Promise<void>;
 	corpusUploadJson(handle: unknown, utf8: ArrayBuffer, idxBase: number): Promise<number>;
 	scoreResident(handle: unknown, query: ApoResidentQuery): Promise<Blocks>;
-	score(handle: unknown, dims: ArrayBuffer, C: number, T: number, corpus: ArrayBuffer | null, K: number): Promise<Blocks>;
-	scoreHostRecords(handle: unknown, records: ArrayBuffer, rowBytes: number, C: number, T: number, corpus: ArrayBuffer | null, K: number): Promise<Blocks>;
+	score(handle: unknown, dims: ArrayBuffer, C: number, T: number, corpus: ArrayBuffer | null, K: number, candidates?: boolean): Promise<Blocks>;
+	scoreHostRecords(handle: unknown, records: ArrayBuffer, rowBytes: number, C: number, T: number, corpus: ArrayBuffer | null, K: number,
+		candidates?: boolean): Promise<Blocks>;
 	/** Form D -> Form T on worker threads of the addon (no GPU): 3 bytes per evaluation instead of 36; null = not categorical. */
 	encodeTuples(dims: ArrayBuffer, C: number, T: number, nthreads?: number): Promise<ApoTuples | null>;
-	scoreHostTuples(handle: unknown, tuples: ApoTuples, C: number, T: number, corpus: ArrayBuffer | null, K: number): Promise<Blocks>;
+	scoreHostTuples(handle: unknown, tuples: ApoTuples, C: number, T: number, corpus: ArrayBuffer | null, K: number, candidates?: boolean): Promise<Blocks>;
 	rewardBatch(handle: unknown, records: ArrayBuffer): Promise<{ dims: ArrayBuffer; masks: ArrayBuffer; finals: ArrayBuffer }>;
 	recordsFromJson(utf8: ArrayBuffer): ArrayBuffer | null;
 }
@@ -50,10 +51,12 @@ function ab(buf: VSBuffer): ArrayBuffer {
 }
 
 function wrapBlocks(r: Blocks): ApoScoreBlocks {
-	return {
+	const out: ApoScoreBlocks = {
 		scores: VSBuffer.wrap(new Uint8Array(r.scores)), counts: VSBuffer.wrap(new Uint8Array(r.counts)),
 		topk: VSBuffer.wrap(new Uint8Array(r.topk)), report: VSBuffer.wrap(new Uint8Array(r.report)),
 	};
+	if (r.candidates) { out.candidates = VSBuffer.wrap(new Uint8Array(r.candidates)); }     // apo_candidate_report[C]
+	return out;
 }
 
 interface PendingReward {
@@ -162,8 +165,8 @@ export class ApoScoringMainService implements IApoScoringService {
 	}
 
 	// ---- one-shot path ------------------------------------------------------------------------
-	async score(dims: VSBuffer, C: number, T: number, corpus: VSBuffer | undefined, K: number): Promise<ApoScoreBlocks> {
-		return wrapBlocks(await (await this._need()).score(this._handle, ab(dims), C, T, corpus ? ab(corpus) : null, K));
+	async score(dims: VSBuffer, C: number, T: number, corpus: VSBuffer | undefined, K: number, candidates?: boolean): Promise<ApoScoreBlocks> {
+		return wrapBlocks(await (await this._need()).score(this._handle, ab(dims), C, T, corpus ? ab(corpus) : null, K, !!candidates));
 	}
 
 	/** fp32 evaluations -> Form T (3 bytes per evaluation + the dictionary of distinct evaluations); undefined when the tensor is not
@@ -178,12 +181,13 @@ export class ApoScoringMainService implements IApoScoringService {
 	}
 
 	/** Same result as score() on the tensor the tuples were encoded from; 12x fewer bytes over IPC and PCIe. */
-	async scoreTuples(t: ApoTupleBuffers, C: number, T: number, corpus: VSBuffer | undefined, K: number): Promise<ApoScoreBlocks> {
+	async scoreTuples(t: ApoTupleBuffers, C: number, T: number, corpus: VSBuffer | undefined, K: number, candidates?: boolean): Promise<ApoScoreBlocks> {
 		const raw: ApoTuples = { tl: ab(t.tl), th: ab(t.th), tbookPc: ab(t.tbookPc), tbookPd: ab(t.tbookPd), codebook: ab(t.codebook), d2book: ab(t.d2book), nTuples: t.nTuples };
-		return wrapBlocks(await (await this._need()).scoreHostTuples(this._handle, raw, C, T, corpus ? ab(corpus) : null, K));
+		return wrapBlocks(await (await this._need()).scoreHostTuples(this._handle, raw, C, T, corpus ? ab(corpus) : null, K, !!candidates));
 	}
 
-	async scoreHostRecords(records: VSBuffer, rowBytes: 32 | 16, C: number, T: number, corpus: VSBuffer | undefined, K: number): Promise<ApoScoreBlocks> {
-		return wrapBlocks(await (await this._need()).scoreHostRecords(this._handle, ab(records), rowBytes, C, T, corpus ? ab(corpus) : null, K));
+	async scoreHostRecords(records: VSBuffer, rowBytes: 32 | 16, C: number, T: number, corpus: VSBuffer | undefined, K: number,
+		candidates?: boolean): Promise<ApoScoreBlocks> {
+		return wrapBlocks(await (await this._need()).scoreHostRecords(this._handle, ab(records), rowBytes, C, T, corpus ? ab(corpus) : null, K, !!candidates));
 	}
 }

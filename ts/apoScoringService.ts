@@ -24,6 +24,7 @@ export interface ApoScoreBlocks {
 	counts: VSBuffer;   // uint64[C]
 	topk: VSBuffer;     // int32[K]    score desc, ties -> lower index
 	report: VSBuffer;   // struct apo_corpus_report (784 bytes)
+	candidates?: VSBuffer;   // apo_candidate_report[C] (376 bytes each, candidateReportCodec.ts); only when the call asked for it
 }
 
 /** Form T of a float32[C][T][9] tensor (include/apo_b200.h): tl uint16[C][T] | th uint8[C][T] = the 24-bit dictionary index of every
@@ -39,6 +40,7 @@ export interface ApoResidentQuery {
 	K: number;              // beam width (APOConfig.beamWidth, APO:288)
 	source?: 0 | 1;         // 0 = dims (Form D / Form Q), 1 = per-(candidate, trace) records
 	corpus?: 0 | 1;         // also build the corpus report from the uploaded corpus
+	candidates?: 0 | 1;     // also build the per-candidate breakdown (ApoScoreBlocks.candidates)
 	first?: number;         // window [first, first + count) of the trace axis; count 0 = to the end
 	count?: number;
 }
@@ -66,14 +68,15 @@ export interface IApoScoringService {
 	scoreResident(query: ApoResidentQuery): Promise<ApoScoreBlocks>;
 
 	// ---- one-shot path: host buffers streamed through the device, nothing stays resident
-	/** dims: float32[C][T][9] (pass C = 1, T = 4 of NaN for report-only calls). */
-	score(dims: VSBuffer, C: number, T: number, corpus: VSBuffer | undefined, K: number): Promise<ApoScoreBlocks>;
+	/** dims: float32[C][T][9] (pass C = 1, T = 4 of NaN for report-only calls).
+	 *  candidates: also return the per-candidate breakdown (ApoScoreBlocks.candidates), here and on the other one-shot calls. */
+	score(dims: VSBuffer, C: number, T: number, corpus: VSBuffer | undefined, K: number, candidates?: boolean): Promise<ApoScoreBlocks>;
 	/** [C][T] trace records (the IDE's own representation): 2.2x fewer PCIe bytes than fp32 dims with 16-byte rows. */
-	scoreHostRecords(records: VSBuffer, rowBytes: 32 | 16, C: number, T: number, corpus: VSBuffer | undefined, K: number): Promise<ApoScoreBlocks>;
+	scoreHostRecords(records: VSBuffer, rowBytes: 32 | 16, C: number, T: number, corpus: VSBuffer | undefined, K: number, candidates?: boolean): Promise<ApoScoreBlocks>;
 	/** fp32 evaluations -> Form T (include/apo_b200.h): a 24-bit dictionary index per evaluation (3 bytes instead of 36) + the
 	 *  dictionary of distinct evaluations.  For evaluations that are scored more than once, kept, or moved between processes. */
 	encodeTuples(dims: VSBuffer, C: number, T: number): Promise<ApoTupleBuffers | undefined>;
-	scoreTuples(tuples: ApoTupleBuffers, C: number, T: number, corpus: VSBuffer | undefined, K: number): Promise<ApoScoreBlocks>;
+	scoreTuples(tuples: ApoTupleBuffers, C: number, T: number, corpus: VSBuffer | undefined, K: number, candidates?: boolean): Promise<ApoScoreBlocks>;
 }
 
 export const IApoScoringService = createDecorator<IApoScoringService>('senweaverApoScoringService');
@@ -95,12 +98,16 @@ export class ApoScoringService implements IApoScoringService {
 	corpusUpload(records: VSBuffer, idxBase?: number) { return this._proxy.corpusUpload(records, idxBase); }
 	corpusUploadJson(persisted: string, idxBase?: number) { return this._proxy.corpusUploadJson(persisted, idxBase); }
 	scoreResident(query: ApoResidentQuery) { return this._proxy.scoreResident(query); }
-	score(dims: VSBuffer, C: number, T: number, corpus: VSBuffer | undefined, K: number) { return this._proxy.score(dims, C, T, corpus, K); }
-	scoreHostRecords(records: VSBuffer, rowBytes: 32 | 16, C: number, T: number, corpus: VSBuffer | undefined, K: number) {
-		return this._proxy.scoreHostRecords(records, rowBytes, C, T, corpus, K);
+	score(dims: VSBuffer, C: number, T: number, corpus: VSBuffer | undefined, K: number, candidates?: boolean) {
+		return this._proxy.score(dims, C, T, corpus, K, candidates);
+	}
+	scoreHostRecords(records: VSBuffer, rowBytes: 32 | 16, C: number, T: number, corpus: VSBuffer | undefined, K: number, candidates?: boolean) {
+		return this._proxy.scoreHostRecords(records, rowBytes, C, T, corpus, K, candidates);
 	}
 	encodeTuples(dims: VSBuffer, C: number, T: number) { return this._proxy.encodeTuples(dims, C, T); }
-	scoreTuples(tuples: ApoTupleBuffers, C: number, T: number, corpus: VSBuffer | undefined, K: number) { return this._proxy.scoreTuples(tuples, C, T, corpus, K); }
+	scoreTuples(tuples: ApoTupleBuffers, C: number, T: number, corpus: VSBuffer | undefined, K: number, candidates?: boolean) {
+		return this._proxy.scoreTuples(tuples, C, T, corpus, K, candidates);
+	}
 }
 
 registerSingleton(IApoScoringService, ApoScoringService, InstantiationType.Delayed);

@@ -1,0 +1,75 @@
+/*---------------------------------------------------------------------------------------------
+ *  NEW FILE for src/vs/workbench/contrib/senweaver/common/candidateReportCodec.ts
+ *
+ *  Decoder of the per-candidate breakdown (ApoScoreBlocks.candidates): apo_candidate_report[C] of
+ *  include/apo_b200.h, the numbers _buildReport computes for the corpus (APO:498-625) answered for
+ *  every beam candidate — feedback tallies, goodRate, avgReward (== the candidate's score),
+ *  rewardByDimension with the dim-low / suggestion flags (APO:575/591/802/819), and the first three
+ *  rollouts of the candidate whose feedback was 'bad'.  The beam loop's critique step
+ *  (_buildTextualGradientPrompt, APO:918-962) can name what a parent lost on from this.
+ *
+ *  The byte offsets below are pinned to the C struct by tests/test_napi_candidates.py.
+ *--------------------------------------------------------------------------------------------*/
+import { VSBuffer } from '../../../../base/common/buffer.js';
+import { DIM_NAMES } from './traceRecordCodec.js';
+
+const CANDIDATE_REPORT_BYTES = 376;
+const OFF_TOTAL = 0;
+const OFF_GOOD = 8;
+const OFF_BAD = 16;
+const OFF_NONE = 24;
+const OFF_GOOD_RATE = 32;
+const OFF_WITH_REWARD = 40;
+const OFF_REWARD_SUM = 48;
+const OFF_AVG_REWARD = 56;
+const OFF_DIM = 64;
+const DIMSTAT_BYTES = 32;
+const OFF_BAD_EXAMPLES = 352;
+// inside one apo_dimstat (sum at 0)
+const DIM_COUNT = 8;
+const DIM_AVG = 16;
+const DIM_LOW_FLAG = 24;
+const DIM_LOW_SEVERITY = 25;
+const DIM_SUGG_FLAG = 26;
+const DIM_SUGG_PRIORITY = 27;
+
+export interface CandidateReportNumbers {
+	candidate: number;
+	total: number; goodFeedbackCount: number; badFeedbackCount: number; noFeedbackCount: number; goodRate: number;
+	withReward: number; rewardSum: number; avgReward: number | null;
+	rewardByDimension: Record<string, { sum: number; count: number; avg: number; low: 'medium' | 'high' | null; suggest: 'medium' | 'high' | null }>;
+	badExamples: number[];                 // rollout indices (the candidate's record axis), ascending
+}
+
+const u64 = (v: DataView, o: number) => Number(v.getBigUint64(o, true));
+
+/** Number of reports in a candidates block. */
+export function candidateReportCount(buf: VSBuffer): number {
+	return Math.floor(buf.byteLength / CANDIDATE_REPORT_BYTES);
+}
+
+/** Report c of a candidates block (ApoScoreBlocks.candidates). */
+export function decodeCandidateReport(buf: VSBuffer, c: number): CandidateReportNumbers {
+	const base = c * CANDIDATE_REPORT_BYTES;
+	if (c < 0 || base + CANDIDATE_REPORT_BYTES > buf.byteLength) { throw new RangeError(`candidate ${c} outside the block`); }
+	const v = new DataView(buf.buffer.buffer, buf.buffer.byteOffset + base, CANDIDATE_REPORT_BYTES);
+	const rewardByDimension: CandidateReportNumbers['rewardByDimension'] = {};
+	DIM_NAMES.forEach((name, i) => {
+		const o = OFF_DIM + DIMSTAT_BYTES * i, count = u64(v, o + DIM_COUNT);
+		if (count) {
+			rewardByDimension[name] = {
+				sum: v.getFloat64(o, true), count, avg: v.getFloat64(o + DIM_AVG, true),
+				low: v.getUint8(o + DIM_LOW_FLAG) ? (v.getUint8(o + DIM_LOW_SEVERITY) === 2 ? 'high' : 'medium') : null,      // APO:575, 591
+				suggest: v.getUint8(o + DIM_SUGG_FLAG) ? (v.getUint8(o + DIM_SUGG_PRIORITY) === 2 ? 'high' : 'medium') : null, // APO:802, 819
+			};
+		}
+	});
+	const badExamples = [0, 1, 2].map(k => Number(v.getBigInt64(OFF_BAD_EXAMPLES + 8 * k, true))).filter(x => x >= 0);
+	const withReward = u64(v, OFF_WITH_REWARD);
+	return {
+		candidate: c, total: u64(v, OFF_TOTAL), goodFeedbackCount: u64(v, OFF_GOOD), badFeedbackCount: u64(v, OFF_BAD),
+		noFeedbackCount: u64(v, OFF_NONE), goodRate: v.getFloat64(OFF_GOOD_RATE, true), withReward,
+		rewardSum: v.getFloat64(OFF_REWARD_SUM, true), avgReward: withReward ? v.getFloat64(OFF_AVG_REWARD, true) : null,
+		rewardByDimension, badExamples,
+	};
+}
