@@ -3,7 +3,12 @@ same process, alternating, on the configs[2] workload (256 x 5 M) resident as Fo
 Form R16 rollouts.  Every leg carries a parity block: the full breakdown of 8 candidates spread over C, over the whole
 record axis, against the CPU oracle's generator path (integers, first-three examples and every binary64 field).
 
-    python examples/candidates_cost.py [--steps 10] [--out FILE.json]
+The rollout legs (R16, and R = the same rollouts as 32-byte records) also time the step with the per-candidate corpus
+reports (APO_SCORE_CANDIDATE_CORPUS), alternating plain / candidates / candidate_corpus, and add a second parity block: the
+corpus report of the same 8 candidates against the CPU oracle's report of their generated rows (integers, flags, examples
+and severities exactly; binary64 sums to 1e-12, the oracle merging per-thread slices).
+
+    python examples/candidates_cost.py [--steps 10] [--legs D,Q,T,R16,R] [--out FILE.json]
 
 Prints one JSON object; the card name and power limit are read in the same run (nvidia-smi query)."""
 import argparse
@@ -61,6 +66,52 @@ def leg(eng, C, K, steps, score_kw, ref, picks):
                        "bad_examples": [list(r.candidates[c].badExamples) for c in picks]}}
 
 
+def same_corpus(r, ref):
+    """apo_corpus_report against oracle.report (the comparison of tests/test_gpu_parity.py check_report)"""
+    close = lambda a, b: abs(a - b) <= 1e-12 * max(1.0, abs(b))
+    if (r.total, r.good, r.bad, r.none, r.withReward) != (ref.total, ref.good, ref.bad, ref.none, ref.withReward):
+        return False
+    if r.goodRate != ref.goodRate or any(list(r.byMode[m]) != list(ref.byMode[m]) or r.byModeGoodRate[m] != ref.byModeGoodRate[m]
+                                         for m in range(5)):
+        return False
+    if ref.withReward and not close(r.avgReward, ref.avgReward):
+        return False
+    for i in range(9):
+        a, b = r.dim[i], ref.dim[i]
+        if a.count != b.count or not close(a.sum, b.sum) or not close(a.avg, b.avg) or (a.low_flag, a.sugg_flag) != (b.low_flag, b.sugg_flag):
+            return False
+    for p in range(6):
+        a, b = r.pat[p], ref.pat[p]
+        if (a.count, a.flag, list(a.examples)) != (b.count, b.flag, list(b.examples)) or (b.flag and a.severity != b.severity):
+            return False
+    return (r.toolCalls, r.toolSucc, r.toolFail) == (ref.toolCalls, ref.toolSucc, ref.toolFail)
+
+
+def corpus_leg(eng, C, K, steps, score_kw, ref, picks, ref_corpus):
+    """plain / candidates / candidate_corpus steps, alternating, with both parity blocks"""
+    kinds = {"plain": {}, "candidates": {"candidates": True}, "candidate_corpus": {"candidate_corpus": True}}
+    times = {k: [] for k in kinds}
+    for _ in range(2):                                          # warm every shape
+        for kw in kinds.values():
+            eng.score(C, K, **kw, **score_kw)
+    last = {}
+    for _ in range(steps):
+        for k, kw in kinds.items():
+            t0 = time.perf_counter(); last[k] = eng.score(C, K, **kw, **score_kw); times[k].append(time.perf_counter() - t0)
+    med = {k: float(np.median(v)) * 1e3 for k, v in times.items()}
+    ok = [same(last["candidates"].candidates[c], d) for c, d in zip(picks, ref)]
+    ok_c = [same_corpus(last["candidate_corpus"].candidate_corpus[c], d) for c, d in zip(picks, ref_corpus)]
+    cc = last["candidate_corpus"].candidate_corpus
+    return {"plain_ms_median": round(med["plain"], 3), "candidates_ms_median": round(med["candidates"], 3),
+            "candidate_corpus_ms_median": round(med["candidate_corpus"], 3),
+            "candidates_ratio": round(med["candidates"] / med["plain"], 3),
+            "candidate_corpus_ratio": round(med["candidate_corpus"] / med["plain"], 3),
+            "min_ms": {k: round(min(v) * 1e3, 3) for k, v in times.items()},
+            "parity": {"candidates": picks, "equal": all(ok), "per_candidate": ok},
+            "parity_corpus": {"candidates": picks, "equal": all(ok_c), "per_candidate": ok_c,
+                              "pattern_counts": [[int(cc[c].pat[p].count) for p in range(6)] for c in picks]}}
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--steps", type=int, default=10)
@@ -69,6 +120,7 @@ def main():
     args = ap.parse_args()
     import importlib
     pkg = importlib.import_module("senweaver-ide_b200")
+    import oracle
     from oracle import candidates as oc
     legs = args.legs.split(",")
     out = {"card": card(), "steps": args.steps, "timing": "host clock around each synchronous apo_score call"}
@@ -96,12 +148,17 @@ def main():
                 eng.tuples_upload(tl, th, tbook, book, d2book)
                 del tl, th
                 out["form_t_256x5M"] = leg(eng, C, K, args.steps, {"source": pkg.SRC_TUPLES}, ref, picks)
-        if "R16" in legs:
+        if {"R16", "R"} & set(legs):
             Cr = 128
             picks_r = [int(x) for x in np.linspace(0, Cr - 1, 8).round()]
             ref_r = oc.cand_generated(seed, picks_r, 0, T, 300, nthreads=nth, records=True)
-            eng.rollouts16_generate(seed, 0, Cr, 0, T, 300)
-            out["form_r16_128x5M"] = leg(eng, Cr, K, args.steps, {"source": pkg.SRC_ROLLOUTS}, ref_r, picks_r)
+            ref_rc = [oracle.report(oracle.gen_records(seed, oracle.STREAM_ROLLOUT, c, 1, 0, T, 300, nth), nthreads=nth) for c in picks_r]
+            if "R16" in legs:
+                eng.rollouts16_generate(seed, 0, Cr, 0, T, 300)
+                out["form_r16_128x5M"] = corpus_leg(eng, Cr, K, args.steps, {"source": pkg.SRC_ROLLOUTS}, ref_r, picks_r, ref_rc)
+            if "R" in legs:
+                eng.rollouts_generate(seed, 0, Cr, 0, T, 300)
+                out["form_r_128x5M"] = corpus_leg(eng, Cr, K, args.steps, {"source": pkg.SRC_ROLLOUTS}, ref_r, picks_r, ref_rc)
     finally:
         eng.close()
     out["card_after"] = card()

@@ -229,6 +229,7 @@ int apo_record_unpack16(const apo_record16 *in, uint64_t n, apo_record *out);
 #define APO_SCORE_RECIP   0x2u   /* finalReward = ws * (1/tw) from a LUT instead of ws / tw (<= 1 ulp apart) */
 #define APO_SCORE_TIMING  0x4u   /* record the per-stage CUDA events of apo_timing also for a small call */
 #define APO_SCORE_CANDIDATES 0x8u /* also build the per-candidate breakdown (apo_candidate_reports) */
+#define APO_SCORE_CANDIDATE_CORPUS 0x10u /* also build the corpus report of every candidate's rollout records (apo_candidate_corpus_reports) */
 typedef struct apo_score_opts {
 	uint32_t K;          /* beam width (top-K), 0..min(C, 16384) */
 	uint32_t source;     /* APO_SRC_* */
@@ -348,6 +349,19 @@ typedef struct apo_candidate_report {
 /* Breakdown of candidates [c0, c0 + n) from the last scoring call.  APO_E_STATE when that call did
  * not set APO_SCORE_CANDIDATES (or failed), APO_E_ARG when the range exceeds its C. */
 int apo_candidate_reports(apo_engine *e, uint32_t c0, uint32_t n, apo_candidate_report *out);
+/* Per-candidate corpus report (record sources only): the whole apo_corpus_report of each candidate's scored rollout records.
+ * Built by a scoring call that sets APO_SCORE_CANDIDATE_CORPUS (independent of APO_SCORE_CANDIDATES; either or both may be
+ * set): apo_score with source APO_SRC_ROLLOUTS (Form R or R16), apo_score_finish (every apo_score_accumulate of the session
+ * must set it too) and apo_score_host_records (32- and 16-byte rows).  out[c] is byte for byte the report that apo_score with
+ * APO_SCORE_CORPUS produces when candidate c's scored records are the corpus: tallies, goodRate, byMode / byModeGoodRate,
+ * withReward / rewardSum / avgReward, dim[9] with its flags, pat[6] with count, flag, severity and examples (no pattern
+ * counts when no record is 'bad', APO:641), tool totals and toolSuccessRate.  Example indices are absolute record positions
+ * (they include the window's first); a session covers the union of its windows.  Form D / Q / P / T carry none of the record
+ * fields the patterns read: APO_E_ARG on those sources and on apo_score_host, apo_score_host_compact, apo_score_host_packed
+ * and apo_score_host_tuples.  Single rank only, as the breakdown (APO_E_STATE on a handle with more than one rank).
+ * Reports of candidates [c0, c0 + n) of the last scoring call: APO_E_STATE when that call did not set the flag (or failed),
+ * APO_E_ARG when the range exceeds its C. */
+int apo_candidate_corpus_reports(apo_engine *e, uint32_t c0, uint32_t n, apo_corpus_report *out);
 
 /* ---- multi-GPU: the record axis is sharded across ranks (one process per GPU, or one handle per GPU inside one
  * process); the packed int64 partial vectors of the shards are joined INSIDE the scoring launch: the finalising CTA

@@ -118,6 +118,13 @@ int apo_job_validate(apo_job *j)
 		if (!fits(j->C, sizeof(apo_candidate_report), 1, APO_JOB_CANDIDATES_MAX_BYTES))
 			return bad(j, "the per-candidate breakdown of C candidates exceeds 4 GiB");
 	}
+	if (j->flags & APO_SCORE_CANDIDATE_CORPUS) {
+		if (!((j->kind == APO_JOB_SCORE_RESIDENT && j->source == APO_SRC_ROLLOUTS) || j->kind == APO_JOB_SCORE_HOST_RECORDS))
+			return bad(j, "the per-candidate corpus reports belong to a scoring call over rollout records");
+		if (j->C == 0) return bad(j, "C must be > 0 for the per-candidate corpus reports");
+		if (!fits(j->C, sizeof(apo_corpus_report), 1, APO_JOB_CANDIDATE_CORPUS_MAX_BYTES))
+			return bad(j, "the per-candidate corpus reports of C candidates exceed 4 GiB");
+	}
 	return APO_OK;
 }
 
@@ -129,7 +136,9 @@ int apo_job_prepare(apo_job *j)
 		const uint32_t C = j->C ? j->C : 1, K = j->K ? j->K : 1;
 		j->scores = (double *)malloc(8u * (size_t)C); j->counts = (uint64_t *)malloc(8u * (size_t)C); j->topk = (int32_t *)malloc(4u * (size_t)K);
 		if (j->flags & APO_SCORE_CANDIDATES) j->candidates = (apo_candidate_report *)malloc(sizeof(apo_candidate_report) * (size_t)C);
-		if (!j->scores || !j->counts || !j->topk || ((j->flags & APO_SCORE_CANDIDATES) && !j->candidates)) {
+		if (j->flags & APO_SCORE_CANDIDATE_CORPUS) j->candidate_corpus = (apo_corpus_report *)malloc(sizeof(apo_corpus_report) * (size_t)C);
+		if (!j->scores || !j->counts || !j->topk || ((j->flags & APO_SCORE_CANDIDATES) && !j->candidates) ||
+		    ((j->flags & APO_SCORE_CANDIDATE_CORPUS) && !j->candidate_corpus)) {
 			apo_job_release(j); j->rc = APO_E_NOMEM; snprintf(j->err, sizeof j->err, "out of host memory"); return APO_E_NOMEM;
 		}
 	} else if (j->kind == APO_JOB_REWARD_BATCH) {
@@ -145,7 +154,9 @@ int apo_job_prepare(apo_job *j)
 void apo_job_release(apo_job *j)
 {
 	free(j->scores); free(j->counts); free(j->topk); free(j->dims_out); free(j->masks_out); free(j->finals_out); free(j->candidates);
+	free(j->candidate_corpus);
 	j->scores = NULL; j->counts = NULL; j->topk = NULL; j->dims_out = NULL; j->masks_out = NULL; j->finals_out = NULL; j->candidates = NULL;
+	j->candidate_corpus = NULL;
 }
 
 static void execute(apo_serial *s, apo_job *j)
@@ -203,6 +214,7 @@ static void execute(apo_serial *s, apo_job *j)
 		j->rc = APO_E_ARG;
 	}
 	if (j->rc == APO_OK && j->candidates) j->rc = apo_candidate_reports(e, 0, j->C, j->candidates);
+	if (j->rc == APO_OK && j->candidate_corpus) j->rc = apo_candidate_corpus_reports(e, 0, j->C, j->candidate_corpus);
 	if (j->rc != APO_OK) snprintf(j->err, sizeof j->err, "%s", apo_last_error(e));
 }
 

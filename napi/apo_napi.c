@@ -25,15 +25,17 @@
  *   rolloutsUpload(h, recs:ArrayBuffer, rowBytes 32|16, C, T)               -> Promise<void>
  *   corpusUpload(h, recs:ArrayBuffer apo_record[T], idxBase)                -> Promise<void>
  *   corpusUploadJson(h, utf8:ArrayBuffer, idxBase)                          -> Promise<number>   (records)
- *   scoreResident(h, {C, K, source, corpus, first, count, candidates})      -> Promise<blocks>   ... scored many times
+ *   scoreResident(h, {C, K, source, corpus, first, count, candidates, candidateCorpus}) -> Promise<blocks>   ... scored many times
  *   score(h, dims, C, T, corpus|null, K, candidates?)                       -> Promise<blocks>   host streaming, Form D
- *   scoreHostRecords(h, recs, rowBytes, C, T, corpus|null, K, candidates?)  -> Promise<blocks>   host streaming, trace records
+ *   scoreHostRecords(h, recs, rowBytes, C, T, corpus|null, K, candidates?, candidateCorpus?) -> Promise<blocks>   host streaming, trace records
  *   scoreHostTuples(h, {tl, th, ...}, C, T, corpus|null, K, candidates?)    -> Promise<blocks>   host streaming, Form T
  *   rewardBatch(h, recs:ArrayBuffer apo_record[n])                          -> Promise<{dims,masks,finals}>
  *   commUniqueId() -> ArrayBuffer(128) | null     commInit(h, nranks, rank, id) -> Promise<void>
  *   recordsFromJson(utf8) -> ArrayBuffer | null   allocPinned(bytes) -> ArrayBuffer | null      (host-only helpers)
  *   blocks = {scores:ArrayBuffer f64[C], counts:ArrayBuffer u64[C], topk:ArrayBuffer i32[K], report:ArrayBuffer,
- *             candidates?:ArrayBuffer apo_candidate_report[C] (only when the call asked for the per-candidate breakdown)}
+ *             candidates?:ArrayBuffer apo_candidate_report[C] (only when the call asked for the per-candidate breakdown),
+ *             candidateCorpus?:ArrayBuffer apo_corpus_report[C] (only when a call over rollout records asked for the per-candidate
+ *             corpus reports)}
  */
 #include <stdint.h>
 #include <stdio.h>
@@ -135,6 +137,8 @@ static napi_value blocks_of(napi_env env, const apo_job *j)
 	if ((v = copy_out(env, j->topk, 4u * (size_t)K))) napi_set_named_property(env, out, "topk", v);
 	if ((v = copy_out(env, &j->report, sizeof j->report))) napi_set_named_property(env, out, "report", v);
 	if (j->candidates && (v = copy_out(env, j->candidates, sizeof(apo_candidate_report) * (size_t)C))) napi_set_named_property(env, out, "candidates", v);
+	if (j->candidate_corpus && (v = copy_out(env, j->candidate_corpus, sizeof(apo_corpus_report) * (size_t)C)))
+		napi_set_named_property(env, out, "candidateCorpus", v);
 	return out;
 }
 
@@ -315,7 +319,7 @@ static int opt_bool_arg(napi_env env, napi_value v, int *out)
 	return 1;
 }
 
-/* scoreResident(h, {C, K, source?, corpus?, first?, count?, candidates?}): scores what dimsUpload / rolloutsUpload / corpusUpload left
+/* scoreResident(h, {C, K, source?, corpus?, first?, count?, candidates?, candidateCorpus?}): scores what dimsUpload / rolloutsUpload / corpusUpload left
  * resident — "uploaded once, scored many times" (SURVEY 8b ownership row); nothing crosses PCIe but the result block. */
 static napi_value ScoreResident(napi_env env, napi_callback_info info)
 {
@@ -323,25 +327,25 @@ static napi_value ScoreResident(napi_env env, napi_callback_info info)
 	call_t *c = argc >= 1 ? new_call(env, argv[0], APO_JOB_SCORE_RESIDENT) : NULL;
 	if (!c) return reject_now(env, "scoreResident: invalid handle");
 	napi_valuetype t;
-	uint32_t corpus = 0, cands = 0;
+	uint32_t corpus = 0, cands = 0, ccorp = 0;
 	if (argc < 2 || napi_typeof(env, argv[1], &t) != napi_ok || t != napi_object ||
 	    !opt_u32(env, argv[1], "C", &c->job.C) || !opt_u32(env, argv[1], "K", &c->job.K) || !opt_u32(env, argv[1], "source", &c->job.source) ||
 	    !opt_u32(env, argv[1], "corpus", &corpus) || !opt_u64(env, argv[1], "first", &c->job.first) || !opt_u64(env, argv[1], "count", &c->job.count) ||
-	    !opt_u32(env, argv[1], "candidates", &cands) || cands > 1)
-		arg_error(c, "scoreResident(handle, {C:uint32, K:uint32, source?:0|1|2, corpus?:0|1, first?:uint53, count?:uint53, candidates?:0|1})");
+	    !opt_u32(env, argv[1], "candidates", &cands) || cands > 1 || !opt_u32(env, argv[1], "candidateCorpus", &ccorp) || ccorp > 1)
+		arg_error(c, "scoreResident(handle, {C:uint32, K:uint32, source?:0|1|2, corpus?:0|1, first?:uint53, count?:uint53, candidates?:0|1, candidateCorpus?:0|1})");
 	if (c->job.C == 0) arg_error(c, "scoreResident: C (the number of uploaded candidates) is required");
 	if (c->job.K > c->job.C) arg_error(c, "scoreResident: K exceeds C");
-	c->job.flags = (corpus ? APO_SCORE_CORPUS : 0) | (cands ? APO_SCORE_CANDIDATES : 0);
+	c->job.flags = (corpus ? APO_SCORE_CORPUS : 0) | (cands ? APO_SCORE_CANDIDATES : 0) | (ccorp ? APO_SCORE_CANDIDATE_CORPUS : 0);
 	return submit(env, c, argv[0], NULL, NULL, "apo_score");
 }
 
 static napi_value score_host_common(napi_env env, napi_callback_info info, apo_job_kind kind)
 {
 	const int rec = kind == APO_JOB_SCORE_HOST_RECORDS;
-	ARGS(8)
+	ARGS(9)
 	call_t *c = argc >= 1 ? new_call(env, argv[0], kind) : NULL;
 	if (!c) return reject_now(env, "score: invalid handle");
-	int cands = 0;
+	int cands = 0, ccorp = 0;
 	const size_t base = rec ? 3 : 2;              /* index of C */
 	const size_t need = base + 4;                 /* ..., C, T, corpus, K */
 	int ok = argc >= need && get_buffer(env, argv[1], &c->job.buf, &c->job.buf_bytes);
@@ -353,8 +357,9 @@ static napi_value score_host_common(napi_env env, napi_callback_info info, apo_j
 		corpus = ok ? argv[base + 2] : NULL;
 	}
 	if (ok && argc > need) ok = opt_bool_arg(env, argv[need], &cands);
-	c->job.flags = cands ? APO_SCORE_CANDIDATES : 0;
-	if (!ok) arg_error(c, rec ? "scoreHostRecords(handle, recs:ArrayBuffer, rowBytes:32|16, C:uint32, T:uint53, corpus:ArrayBuffer|null, K:uint32, candidates?:boolean)"
+	if (ok && rec && argc > need + 1) ok = opt_bool_arg(env, argv[need + 1], &ccorp);     /* trace records only */
+	c->job.flags = (cands ? APO_SCORE_CANDIDATES : 0) | (ccorp ? APO_SCORE_CANDIDATE_CORPUS : 0);
+	if (!ok) arg_error(c, rec ? "scoreHostRecords(handle, recs:ArrayBuffer, rowBytes:32|16, C:uint32, T:uint53, corpus:ArrayBuffer|null, K:uint32, candidates?:boolean, candidateCorpus?:boolean)"
 	                          : "score(handle, dims:ArrayBuffer, C:uint32, T:uint53, corpus:ArrayBuffer|null, K:uint32, candidates?:boolean)");
 	return submit(env, c, argv[0], c->job.buf ? argv[1] : NULL, corpus, rec ? "apo_score_host_records" : "apo_score_host");
 }

@@ -139,11 +139,7 @@ class APOService:
             rep, rew = self._corpus_report(traces)
             good, bad, none = int(rep.good), int(rep.bad), int(rep.none)
             goodRate = float(rep.goodRate)
-            byMode = {}
-            for m, name in enumerate(MODE_NAMES):
-                tot, g, b = (int(x) for x in rep.byMode[m])
-                if tot:
-                    byMode[name] = {"total": tot, "good": g, "bad": b, "goodRate": float(rep.byModeGoodRate[m])}
+            byMode = self._byMode(rep)
             avgReward = None if rew.withReward == 0 else float(rew.avgReward)
             rewardByDimension = self._rewardByDimension(rew)
         else:
@@ -153,20 +149,11 @@ class APOService:
 
         patterns = []
         if rep is not None:
-            for p in range(6):                                              # APO:643-770
-                q = rep.pat[p]
-                if not q.flag:
-                    continue
-                text, cat = PATTERN_TEXT[p]
-                ex = []
-                for gi in q.examples:
-                    if gi < 0:
-                        continue
-                    t = traces[int(gi)]
-                    ex.append({"threadId": t["threadId"], "userMessagePreview": _first_preview(t, "user_message"),
-                               "assistantMessagePreview": self._example_detail(p, t), "feedback": t["summary"]["userFeedback"]})
-                patterns.append({"id": str(uuid.uuid4()), "description": text, "frequency": int(q.count),
-                                 "severity": SEVERITY[q.severity], "relatedCategory": cat, "examples": ex})
+            def example(p, gi):
+                t = traces[gi]
+                return {"threadId": t["threadId"], "userMessagePreview": _first_preview(t, "user_message"),
+                        "assistantMessagePreview": self._example_detail(p, t), "feedback": t["summary"]["userFeedback"]}
+            patterns = self._emittedPatterns(rep, example)
             patterns.extend(self._dimensionPatterns(rew))
 
         suggestions = self._generateLocalSuggestions(goodRate, patterns, byMode, avgReward, rew)
@@ -180,6 +167,31 @@ class APOService:
         if suggestions:
             self._fire(self._suggestionListeners, suggestions)
         return report
+
+    @staticmethod
+    def _byMode(rep):
+        """APO:519-544: per-mode tallies of a corpus report, modes without records left out."""
+        byMode = {}
+        for m, name in enumerate(MODE_NAMES):
+            tot, g, b = (int(x) for x in rep.byMode[m])
+            if tot:
+                byMode[name] = {"total": tot, "good": g, "bad": b, "goodRate": float(rep.byModeGoodRate[m])}
+        return byMode
+
+    @staticmethod
+    def _emittedPatterns(rep, example):
+        """APO:643-770: the emitted problem patterns of a corpus report; example(p, index) shapes one of its first three
+        matching records."""
+        patterns = []
+        for p in range(6):
+            q = rep.pat[p]
+            if not q.flag:
+                continue
+            text, cat = PATTERN_TEXT[p]
+            ex = [example(p, int(gi)) for gi in q.examples if gi >= 0]
+            patterns.append({"id": str(uuid.uuid4()), "description": text, "frequency": int(q.count),
+                             "severity": SEVERITY[q.severity], "relatedCategory": cat, "examples": ex})
+        return patterns
 
     @staticmethod
     def _rewardByDimension(rew):
@@ -204,17 +216,30 @@ class APOService:
         """The report of one beam candidate, shaped like _buildReport's, from a ScoreResult scored with the per-candidate
         breakdown (evaluateBeam(..., reports=True)): feedback tallies and goodRate of its rollouts, avgReward (== its score),
         rewardByDimension, the dimension-low patterns and the suggestions they raise (the rules of APO:574-596, 800-827, by
-        the code _buildReport uses), and badExamples = the first three rollout indices with 'bad' feedback.  Pure: it
-        neither records the suggestions nor fires events nor touches storage."""
-        r = res.candidates[c]
+        the code _buildReport uses), and badExamples = the first three rollout indices with 'bad' feedback.
+        When the result also carries the candidate's corpus report (rollout records scored with candidate_corpus=True,
+        evaluateBeam(..., patterns=True)), the report adds byMode, the six problem patterns of APO:643-770 (examples = rollout
+        indices) ahead of the dimension-low ones, and toolStats (TCS:603-624); its suggestions then follow the pattern and
+        mode rules of APO:830-859 as well.  Pure: it neither records the suggestions nor fires events nor touches storage."""
+        cc = res.candidate_corpus[c] if getattr(res, "candidate_corpus", None) is not None else None
+        r = res.candidates[c] if res.candidates is not None else cc
         goodRate = float(r.goodRate)
         avgReward = None if r.withReward == 0 else float(r.avgReward)
-        patterns = self._dimensionPatterns(r)
-        return {"candidate": int(c), "totalRollouts": int(r.total), "goodFeedbackCount": int(r.good), "badFeedbackCount": int(r.bad),
-                "noFeedbackCount": int(r.none), "goodRate": goodRate, "avgReward": avgReward,
-                "rewardByDimension": self._rewardByDimension(r), "patterns": patterns,
-                "suggestions": self._generateLocalSuggestions(goodRate, patterns, {}, avgReward, r),
-                "badExamples": [int(x) for x in r.badExamples if x >= 0]}
+        byMode = self._byMode(cc) if cc is not None else {}
+        patterns = self._emittedPatterns(cc, lambda p, gi: gi) if cc is not None else []
+        patterns.extend(self._dimensionPatterns(r))
+        out = {"candidate": int(c), "totalRollouts": int(r.total), "goodFeedbackCount": int(r.good), "badFeedbackCount": int(r.bad),
+               "noFeedbackCount": int(r.none), "goodRate": goodRate, "avgReward": avgReward,
+               "rewardByDimension": self._rewardByDimension(r), "patterns": patterns,
+               "suggestions": self._generateLocalSuggestions(goodRate, patterns, byMode, avgReward, r)}
+        if res.candidates is not None:
+            out["badExamples"] = [int(x) for x in r.badExamples if x >= 0]
+        if cc is not None:
+            out["byMode"] = byMode
+            out["toolStats"] = {"totalToolCalls": int(cc.toolCalls), "totalToolSucceeded": int(cc.toolSucc),
+                                "totalToolFailed": int(cc.toolFail),
+                                "toolSuccessRate": None if cc.toolCalls == 0 else float(cc.toolSuccessRate)}
+        return out
 
     @staticmethod
     def _example_detail(p, t):
@@ -267,16 +292,19 @@ class APOService:
         return out
 
     # ---- beam evaluation: the step the reference delegates to its backend --------------------------------
-    def evaluateBeam(self, candidates, dims=None, rollouts=None, reports=False):
+    def evaluateBeam(self, candidates, dims=None, rollouts=None, reports=False, patterns=False):
         """Score a beam of VersionedPromptTemplate candidates on their rollout outcomes and keep the
         top `beamWidth` (score desc, ties -> lower index), then apply the APO:1138-1166 update with the
         strict `>` adoption rule (APO:1159).  dims: float32 [C][T][9] (NaN = absent) or rollouts:
         apo_record [C][T].  reports=True also builds the per-candidate breakdown (res.candidates, see
-        candidateReport)."""
+        candidateReport); with rollouts, reports=True and patterns=True also build every candidate's corpus
+        report (res.candidate_corpus: problem patterns, per-mode tallies, tool totals)."""
         try:
             C = len(candidates)
             K = min(self._config["beamWidth"], C)
             extra = {"candidates": True} if reports else {}
+            if reports and patterns and rollouts is not None:
+                extra["candidate_corpus"] = True
             if dims is not None:
                 self._engine.dims_upload(np.ascontiguousarray(dims, np.float32))
                 res = self._engine.score(C, K, source=SRC_DIMS, **extra)
@@ -296,14 +324,18 @@ class APOService:
             print("[APO] Beam evaluation failed:", e)
             return None
 
-    def runBeamSearch(self, seedPrompt, proposeCandidates, rolloutDims, rounds=None, withReports=False):
+    def runBeamSearch(self, seedPrompt, proposeCandidates, rolloutDims=None, rounds=None, withReports=False, rolloutRecords=None):
         """Client-side round driver (SURVEY 8f rank 3) around the GPU top-K: each round expands every beam
         member into `branchFactor` children through the caller's `proposeCandidates(parent, n) -> [content]`
         hook (the LLM critique/edit step of APO:918-988 lives there), scores parents + children on
-        `rolloutDims(candidates) -> float32 [C][T][9]`, keeps the top `beamWidth` and applies the
-        APO:1138-1166 update.  withReports=True calls `proposeCandidates(parent, n, report)` instead, with the
-        candidateReport of the parent from the round that scored it (None for the unscored seed), so that the
-        critique can name what the parent lost on.  Returns the final beam state."""
+        `rolloutDims(candidates) -> float32 [C][T][9]` or `rolloutRecords(candidates) -> apo_record [C][T]` (exactly
+        one of the two), keeps the top `beamWidth` and applies the APO:1138-1166 update.  withReports=True calls
+        `proposeCandidates(parent, n, report)` instead, with the candidateReport of the parent from the round that
+        scored it (None for the unscored seed), so that the critique can name what the parent lost on; with
+        rolloutRecords that report also carries the parent's problem patterns, byMode and toolStats.  Returns the
+        final beam state."""
+        if (rolloutDims is None) == (rolloutRecords is None):
+            raise ValueError("runBeamSearch needs exactly one of rolloutDims / rolloutRecords")
         rounds = rounds or self._config["beamRounds"]
         beam = [{"version": "v0", "content": seedPrompt, "score": None, "createdAt": time.time() * 1000.0}]
         counter = 0
@@ -317,7 +349,10 @@ class APOService:
                     counter += 1
                     cands.append({"version": f"v{counter}", "content": content, "score": None,
                                   "parentVersion": parent["version"], "createdAt": time.time() * 1000.0})
-            res = self.evaluateBeam(cands, dims=rolloutDims(cands), reports=withReports)
+            if rolloutRecords is not None:
+                res = self.evaluateBeam(cands, rollouts=rolloutRecords(cands), reports=withReports, patterns=withReports)
+            else:
+                res = self.evaluateBeam(cands, dims=rolloutDims(cands), reports=withReports)
             if res is None:
                 break
             if withReports:

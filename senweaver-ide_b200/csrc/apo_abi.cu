@@ -142,6 +142,11 @@ struct apo_engine {
 	bool cand_armed = false;                 // cand_acc zeroed for this call / session
 	bool cand_every = true;                  // every accumulate of the session so far set the flag
 	bool cand_ready = false;                 // cand_rep holds the breakdown of the last scoring call
+	// per-candidate corpus report (APO_SCORE_CANDIDATE_CORPUS, csrc/apo_cand.cu k_cand_corpus): its own blocks, as cand_acc
+	DevBuf<long long> ccorp_acc;             // [C][CC_WORDS] corpus blocks | [C][CC_WORDS] scratch of the report kernel
+	DevBuf<apo_corpus_report> ccorp_rep;     // reports of the last flagged call
+	uint32_t ccorp_C = 0;
+	bool ccorp_armed = false, ccorp_every = true, ccorp_ready = false;   // as cand_armed / cand_every / cand_ready
 };
 
 namespace {
@@ -486,6 +491,7 @@ int begin_score(apo_engine *e, uint32_t C, bool whole = false) {
 	e->partials_src = e->nranks > 1 ? e->acc_joined.p : e->acc.p;
 	e->last_C = C; e->score_C = C; e->scoring = true; e->k1_used = 0;
 	e->cand_armed = false; e->cand_every = true; e->cand_ready = false;
+	e->ccorp_armed = false; e->ccorp_every = true; e->ccorp_ready = false;
 	e->timing = apo_timing{};
 	if (e->timing_on) CK(cudaEventRecord(e->ev[0], e->stream));
 	return APO_OK;
@@ -659,6 +665,56 @@ int cand_finish(apo_engine *e, uint32_t C) {
 	e->timing.launches++;
 	CK(cudaStreamSynchronize(e->stream));
 	e->cand_C = C; e->cand_ready = true;
+	return APO_OK;
+}
+
+// ---- per-candidate corpus report (APO_SCORE_CANDIDATE_CORPUS)
+bool wants_ccorp(const apo_score_opts *o) { return (o->flags & APO_SCORE_CANDIDATE_CORPUS) != 0; }
+
+// records: the call reads trace records (Form R / R16); the other forms carry only the nine reward values
+int ccorp_check(apo_engine *e, bool records) {
+	if (!records)
+		return fail(e, APO_E_ARG, "APO_SCORE_CANDIDATE_CORPUS needs rollout records (Form R / R16): this source holds reward values only, "
+		                          "without the fields the patterns, modes and tool totals read");
+	if (e->nranks > 1)
+		return fail(e, APO_E_STATE, "APO_SCORE_CANDIDATE_CORPUS is single-rank only: the per-candidate corpus reports are not joined across the %d ranks of this handle", e->nranks);
+	return APO_OK;
+}
+
+// zero the corpus blocks of C candidates (first flagged launch of a call or session)
+int ccorp_arm(apo_engine *e, uint32_t C) {
+	const uint64_t words = (uint64_t)C * apo::CC_WORDS;
+	CK(e->ccorp_acc.reserve(2 * words));                 // blocks | report scratch
+	CK(cudaMemsetAsync(e->ccorp_acc.p, 0, words * 8, e->stream));
+	e->ccorp_armed = true;
+	return APO_OK;
+}
+
+// corpus scan of C candidate rows of T records (row bytes 32 / 16) into candidates [cand_offset, ...); idx_base = position of record 0
+int ccorp_launch(apo_engine *e, const uint8_t *rows, uint32_t row, uint32_t C, uint64_t T, uint64_t pitch_evals, uint64_t idx_base,
+                 uint32_t cand_offset) {
+	if (!T) return APO_OK;
+	apo::CandCorpusParams P{};
+	P.C = C; P.T = T; P.idx_base = idx_base; P.pitch_evals = pitch_evals; P.rows = rows;
+	P.lut = e->d_lut.p; P.w2 = e->W.w[2];
+	P.blk = e->ccorp_acc.p + (uint64_t)apo::CC_WORDS * cand_offset;
+	CK(apo::run_cand_corpus(P, (int)row, e->sm_count, e->stream));
+	e->timing.launches++;
+	return APO_OK;
+}
+
+// the resident rollouts over [first, first+count) into candidates [cand_offset, ...)
+int launch_ccorp_resident(apo_engine *e, uint32_t cand_offset, uint64_t first, uint64_t count) {
+	return ccorp_launch(e, e->roll.p + first * e->roll_row, e->roll_row, e->roll_C, count, e->roll_pitch, first, cand_offset);
+}
+
+// blocks -> apo_corpus_report[C]
+int ccorp_finish(apo_engine *e, uint32_t C) {
+	CK(e->ccorp_rep.reserve(C ? C : 1));
+	CK(apo::run_cand_corpus_report(e->ccorp_acc.p, C, e->ccorp_rep.p, e->stream));
+	e->timing.launches++;
+	CK(cudaStreamSynchronize(e->stream));
+	e->ccorp_C = C; e->ccorp_ready = true;
 	return APO_OK;
 }
 
@@ -927,7 +983,7 @@ extern "C" void apo_destroy(apo_engine *e) {
 	e->d_lut.release(); e->corpus.release(); e->dims.release(); e->roll.release(); e->acc.release(); e->acc_joined.release(); e->acc_snapshot.release(); e->misc.release();
 	e->result.release(); e->keys.release(); e->sel_key.release(); e->sel_idx.release();
 	e->tups_pc.release(); e->tups_pd.release(); e->tups_d2.release();
-	e->cand_acc.release(); e->cand_rep.release(); e->cand_book.release();
+	e->cand_acc.release(); e->cand_rep.release(); e->cand_book.release(); e->ccorp_acc.release(); e->ccorp_rep.release();
 	e->tup_l.release(); e->tup_h.release(); e->tup_pc.release(); e->tup_pd.release(); e->tup_bad.release(); e->tup_d2.release(); e->tup_ptab.release(); e->tup_val.release();
 	e->win[0].release(); e->win[1].release(); e->batch_in.release(); e->batch_out.release(); e->batch_mask.release();
 	if (e->h_result) cudaFreeHost(e->h_result);
@@ -1289,10 +1345,16 @@ extern "C" int apo_score_accumulate(apo_engine *e, const apo_score_opts *o, uint
 	if (o->first % 4) return fail(e, APO_E_ARG, "window start must be a multiple of 4");
 	if (o->first > T || (o->count && o->first + o->count > T)) return fail(e, APO_E_ARG, "window outside [0,%llu)", (unsigned long long)T);
 	first = o->first; count = o->count ? o->count : T - o->first;
-	const bool cand = wants_cand(o);
+	const bool cand = wants_cand(o), ccorp = wants_ccorp(o);
 	if (cand && (rc = cand_check(e))) return rc;
+	if (ccorp && (rc = ccorp_check(e, o->source == APO_SRC_ROLLOUTS))) return rc;
 	CK(cudaSetDevice(e->device));
 	if ((rc = launch_k1_resident(e, o, cand_offset, first, count))) return rc;
+	if (!ccorp) e->ccorp_every = false;
+	else if (e->ccorp_every) {                          // an earlier accumulate of the session did not set the flag: finish refuses
+		if (!e->ccorp_armed && (rc = ccorp_arm(e, e->score_C))) return rc;
+		if ((rc = launch_ccorp_resident(e, cand_offset, first, count))) return rc;
+	}
 	if (!cand) { e->cand_every = false; return APO_OK; }
 	if (!e->cand_every) return APO_OK;                  // an earlier accumulate of the session did not set the flag: finish refuses
 	if (!e->cand_armed && (rc = cand_arm(e, e->score_C))) return rc;
@@ -1303,33 +1365,43 @@ extern "C" int apo_score_finish(apo_engine *e, const apo_score_opts *o, double *
                                 apo_corpus_report *report) {
 	if (!e) return APO_E_ARG;
 	e->cand_ready = false;                              // a failed finish leaves no breakdown behind either
+	e->ccorp_ready = false;
 	if (!o) return fail(e, APO_E_ARG, "opts is NULL");
 	if (!e->scoring) return fail(e, APO_E_STATE, "apo_score_begin has not been called");
 	if (o->K > e->score_C) return fail(e, APO_E_ARG, "K=%u exceeds the number of candidates C=%u", o->K, e->score_C);
 	if (o->K > kMaxK) return fail(e, APO_E_ARG, "K=%u exceeds the supported beam width %u", o->K, kMaxK);
-	const bool cand = wants_cand(o);
+	const bool cand = wants_cand(o), ccorp = wants_ccorp(o);
 	int rc;
 	if (cand) {
 		if ((rc = cand_check(e))) return rc;
 		if (!e->cand_every)
 			return fail(e, APO_E_STATE, "APO_SCORE_CANDIDATES: every apo_score_accumulate of the session must set the flag for a breakdown");
 	}
+	if (ccorp) {
+		if ((rc = ccorp_check(e, true))) return rc;     // the accumulate calls refused every other source
+		if (!e->ccorp_every)
+			return fail(e, APO_E_STATE, "APO_SCORE_CANDIDATE_CORPUS: every apo_score_accumulate of the session must set the flag for the reports");
+	}
 	CK(cudaSetDevice(e->device));
 	if (cand && !e->cand_armed && (rc = cand_arm(e, e->score_C))) return rc;   // nothing accumulated yet: an empty breakdown
+	if (ccorp && !e->ccorp_armed && (rc = ccorp_arm(e, e->score_C))) return rc;
 	if (peer_join_active(e, e->score_C)) e->join_epoch++;
 	if ((rc = finish_score(e, o, e->score_C, scores, counts, topk, report))) return rc;
-	return cand ? cand_finish(e, e->score_C) : APO_OK;
+	if (cand && (rc = cand_finish(e, e->score_C))) return rc;
+	return ccorp ? ccorp_finish(e, e->score_C) : APO_OK;
 }
 
 extern "C" int apo_score(apo_engine *e, const apo_score_opts *o, double *scores, uint64_t *counts, int32_t *topk, apo_corpus_report *report) {
 	if (!e) return APO_E_ARG;
 	e->cand_ready = false;                              // a failed call leaves no breakdown behind either
+	e->ccorp_ready = false;
 	uint32_t C = 0; uint64_t T = 0, first = 0, count = 0;
 	int rc = source_shape(e, o, &C, &T);
 	if (rc) return rc;
 	if ((rc = check_opts(e, o, C, T, &first, &count))) return rc;
-	const bool cand = wants_cand(o);
+	const bool cand = wants_cand(o), ccorp = wants_ccorp(o);
 	if (cand && (rc = cand_check(e))) return rc;
+	if (ccorp && (rc = ccorp_check(e, o->source == APO_SRC_ROLLOUTS))) return rc;
 	CK(cudaSetDevice(e->device));
 	if ((rc = ensure_scratch(e, C, o->K))) return rc;
 	const bool tup = o->source == APO_SRC_TUPLES;      // gather-and-add kernel: stand-alone corpus scan + tail
@@ -1355,6 +1427,7 @@ extern "C" int apo_score(apo_engine *e, const apo_score_opts *o, double *scores,
 	if (fuse || tail_only) {
 		if ((rc = begin_score(e, C, true))) return rc;
 		if (cand && (rc = cand_arm(e, C))) return rc;
+		if (ccorp && (rc = ccorp_arm(e, C))) return rc;
 		apo::FinalizeParams F = make_fin(e, C, o->K, fuse ? 1 : 0);
 		const bool self_clean = one_launch;          // the finalising CTA is in this launch: it can leave the block zeroed
 		if (self_clean) { F.clean_ptr = e->acc.p; F.clean_words = (uint32_t)(acc_words(C, e->nranks) + ARM_WORDS); F.snapshot = e->acc_snapshot.p; }
@@ -1362,21 +1435,26 @@ extern "C" int apo_score(apo_engine *e, const apo_score_opts *o, double *scores,
 		if (tail_only) { k2.T = 0; k2.recs = nullptr; }
 		if ((rc = launch_k1_resident(e, o, 0, first, count, &k2))) return rc;
 		if (cand && (rc = launch_cand_resident(e, o, 0, first, count))) return rc;
+		if (ccorp && (rc = launch_ccorp_resident(e, 0, first, count))) return rc;
 		rc = finish_score(e, o, C, scores, counts, topk, report, true);
 		if (rc == APO_OK && self_clean) {
 			e->acc_clean_words = F.clean_words;
 			if (e->nranks == 1) e->partials_src = e->acc_snapshot.p;
 		}
 		if (rc == APO_OK && cand) rc = cand_finish(e, C);
+		if (rc == APO_OK && ccorp) rc = ccorp_finish(e, C);
 		return rc;
 	} else {
 		if ((rc = begin_score(e, C))) return rc;
 		if (cand && (rc = cand_arm(e, C))) return rc;
+		if (ccorp && (rc = ccorp_arm(e, C))) return rc;
 		if ((rc = launch_k1_resident(e, o, 0, first, count))) return rc;
 		if (cand && (rc = launch_cand_resident(e, o, 0, first, count))) return rc;
+		if (ccorp && (rc = launch_ccorp_resident(e, 0, first, count))) return rc;
 	}
 	if ((rc = finish_score(e, o, C, scores, counts, topk, report, fuse || tail_only))) return rc;
-	return cand ? cand_finish(e, C) : APO_OK;
+	if (cand && (rc = cand_finish(e, C))) return rc;
+	return ccorp ? ccorp_finish(e, C) : APO_OK;
 }
 
 namespace {
@@ -1386,14 +1464,16 @@ int score_host_rows_impl(apo_engine *e, const apo_score_opts *o, const uint8_t *
                          double *scores, uint64_t *counts, int32_t *topk, apo_corpus_report *report) {
 	if (!e) return APO_E_ARG;
 	e->cand_ready = false;
+	e->ccorp_ready = false;
 	if (!o) return fail(e, APO_E_ARG, "opts is NULL");
 	if (!rows || C == 0) return fail(e, APO_E_ARG, "input is NULL or C == 0");
 	if (o->K > C) return fail(e, APO_E_ARG, "K=%u exceeds the number of candidates C=%u", o->K, C);
 	if (o->K > kMaxK) return fail(e, APO_E_ARG, "K=%u exceeds the supported beam width %u", o->K, kMaxK);
 	if (o->first || o->count) return fail(e, APO_E_ARG, "windows are not supported by the host-streaming calls");
-	const bool cand = wants_cand(o);
+	const bool cand = wants_cand(o), ccorp = wants_ccorp(o);
 	int rc;
 	if (cand && (rc = cand_check(e))) return rc;
+	if (ccorp && (rc = ccorp_check(e, row != 36))) return rc;
 	CK(cudaSetDevice(e->device));
 	if ((rc = ensure_scratch(e, C, o->K))) return rc;
 	// window of ~256 MB per buffer, a multiple of the K1 tile so chunks never split a tile
@@ -1412,6 +1492,7 @@ int score_host_rows_impl(apo_engine *e, const apo_score_opts *o, const uint8_t *
 	if (peer_join_active(e, C)) e->join_epoch++;
 	if ((rc = begin_score(e, C))) return rc;
 	if (cand && (rc = cand_arm(e, C))) return rc;
+	if (ccorp && (rc = ccorp_arm(e, C))) return rc;
 	const bool recip = (o->flags & APO_SCORE_RECIP) != 0;
 	int nchunk = 0;
 	for (uint64_t t0 = 0; t0 < T; t0 += Tc, nchunk++) {
@@ -1445,10 +1526,12 @@ int score_host_rows_impl(apo_engine *e, const apo_score_opts *o, const uint8_t *
 			B.rows = e->win[b].p;
 			if ((rc = cand_launch(e, B, row == 36 ? apo::CAND_DIMS : row == 32 ? apo::CAND_REC32 : apo::CAND_REC16))) return rc;
 		}
+		if (ccorp && (rc = ccorp_launch(e, e->win[b].p, row, C, n, Tc, t0, 0))) return rc;   // before the window is released
 		CK(cudaEventRecord(e->win_free[b], e->stream));
 	}
 	if ((rc = finish_score(e, o, C, scores, counts, topk, report))) return rc;
-	return cand ? cand_finish(e, C) : APO_OK;
+	if (cand && (rc = cand_finish(e, C))) return rc;
+	return ccorp ? ccorp_finish(e, C) : APO_OK;
 }
 
 int score_host_rows(apo_engine *e, const apo_score_opts *o, const uint8_t *rows, uint32_t row, uint32_t C, uint64_t T,
@@ -1560,7 +1643,9 @@ int score_host_compact_impl(apo_engine *e, const apo_score_opts *o, const uint64
                             apo_corpus_report *report) {
 	const bool packed = pc != nullptr;
 	e->cand_ready = false;
+	e->ccorp_ready = false;
 	if (!o) return fail(e, APO_E_ARG, "opts is NULL");
+	if (wants_ccorp(o)) return ccorp_check(e, false);
 	if (!codebook || C == 0 || (packed ? (!pd || !d2book) : (!q8 || !d2 || !li))) return fail(e, APO_E_ARG, "input is NULL or C == 0");
 	if (o->K > C) return fail(e, APO_E_ARG, "K=%u exceeds the number of candidates C=%u", o->K, C);
 	if (o->K > kMaxK) return fail(e, APO_E_ARG, "K=%u exceeds the supported beam width %u", o->K, kMaxK);
@@ -1682,7 +1767,9 @@ int score_host_tuples_impl(apo_engine *e, const apo_score_opts *o, const uint16_
                            const uint16_t *tb_pd, uint32_t n_tuples, const uint32_t *codebook, const uint32_t *d2book, uint32_t C, uint64_t T,
                            double *scores, uint64_t *counts, int32_t *topk, apo_corpus_report *report) {
 	e->cand_ready = false;
+	e->ccorp_ready = false;
 	if (!o) return fail(e, APO_E_ARG, "opts is NULL");
+	if (wants_ccorp(o)) return ccorp_check(e, false);
 	int rc;
 	if ((rc = tuples_args(e, tl, th, tb_pc, tb_pd, n_tuples, codebook, d2book, C, T))) return rc;
 	if (o->K > C) return fail(e, APO_E_ARG, "K=%u exceeds the number of candidates C=%u", o->K, C);
@@ -1824,6 +1911,18 @@ extern "C" int apo_candidate_reports(apo_engine *e, uint32_t c0, uint32_t n, apo
 	if (!out) return fail(e, APO_E_ARG, "out is NULL");
 	CK(cudaSetDevice(e->device));
 	CK(cudaMemcpyAsync(out, e->cand_rep.p + c0, (uint64_t)n * sizeof(apo_candidate_report), cudaMemcpyDeviceToHost, e->stream));
+	CK(cudaStreamSynchronize(e->stream));
+	return APO_OK;
+}
+
+extern "C" int apo_candidate_corpus_reports(apo_engine *e, uint32_t c0, uint32_t n, apo_corpus_report *out) {
+	if (!e) return APO_E_ARG;
+	if (!e->ccorp_ready) return fail(e, APO_E_STATE, "the last scoring call did not set APO_SCORE_CANDIDATE_CORPUS");
+	if ((uint64_t)c0 + n > e->ccorp_C) return fail(e, APO_E_ARG, "candidates [%u,%llu) exceed C=%u", c0, (unsigned long long)c0 + n, e->ccorp_C);
+	if (n == 0) return APO_OK;
+	if (!out) return fail(e, APO_E_ARG, "out is NULL");
+	CK(cudaSetDevice(e->device));
+	CK(cudaMemcpyAsync(out, e->ccorp_rep.p + c0, (uint64_t)n * sizeof(apo_corpus_report), cudaMemcpyDeviceToHost, e->stream));
 	CK(cudaStreamSynchronize(e->stream));
 	return APO_OK;
 }

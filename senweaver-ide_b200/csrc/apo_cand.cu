@@ -11,6 +11,9 @@
 // path it mirrors: fp32 rows (Form D), codes + codebook (Form Q, and Form P after k_unpack_p), dictionary entry ->
 // codebook / d2book (Form T), records -> reward_dims (Form R / R16).  Validity is the scoring kernels' rule: total weight
 // of the presence mask > 0 (LUT), and for records also the VALID flag.
+//
+// For record sources a second feature (APO_SCORE_CANDIDATE_CORPUS, k_cand_corpus below) goes further: the whole corpus
+// report of every candidate's records — patterns, per-mode tallies and tool totals included — by the corpus scan's own code.
 #include "apo_device.cuh"
 #include "apo_format.h"
 #include "apo_kernels.h"
@@ -287,6 +290,139 @@ cudaError_t run_cand_report(const long long *ints, const unsigned long long *ex,
                             apo_candidate_report *out, cudaStream_t st) {
 	if (C == 0) return cudaSuccess;
 	k_cand_report<<<(C + 255) / 256, 256, 0, st>>>(ints, ex, partials, C, out);
+	return cudaGetLastError();
+}
+
+// ================================================================ per-candidate corpus report (APO_SCORE_CANDIDATE_CORPUS)
+//   k_cand_corpus<ROW>      the corpus scan (scan_record / scan_flush of apo_corpus.cuh) over the records of every candidate
+//                           that a scoring call reads, into one corpus block per candidate
+//   k_cand_corpus_report    corpus block -> apo_corpus_report with build_report, the code of the corpus report itself
+static_assert(CC_WORDS == CORP_FIXED + APO_NPAT * 3, "one rank's corpus block with its example slots");
+constexpr int CC_THREADS = 256;
+constexpr int CC_WARPS = CC_THREADS / 32;
+constexpr int CC_GROUPS = 32;                               // records per lane in a warp tile (one candidate)
+constexpr int CC_TILE = 32 * CC_GROUPS;
+constexpr uint32_t CC_RUN_TILES = K2_CHUNK / CC_GROUPS;     // the packed ScanAcc fields hold K2_CHUNK records per lane
+static_assert(K2_CHUNK % CC_GROUPS == 0, "a chunk is a whole number of tiles");
+
+// Warps walk candidate-major tiles as k_cand_breakdown does.  A warp flushes its ScanAcc into the candidate's block when the
+// candidate changes and after every CC_RUN_TILES tiles; its pattern examples collect in the warp's own 18 shared slots and
+// are merged into the candidate's slots at every flush (ex_insert, gated on the third slot).
+template <int ROW>
+__global__ void __launch_bounds__(CC_THREADS)
+k_cand_corpus(const CandCorpusParams P, uint32_t tiles_per_cand, uint64_t total_tiles) {
+	__shared__ double s_cat[CAT_WORDS];
+	__shared__ double2 s_lut[512];                          // {total weight, reciprocal} per (natural) presence mask
+	__shared__ unsigned long long s_ex[CC_WARPS][APO_NPAT * 3];
+	const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+	if (tid < CAT_WORDS) s_cat[tid] = P.lut[1024 + tid];
+	for (int i = tid; i < 512; i += CC_THREADS) s_lut[i] = make_double2(P.lut[i], P.lut[512 + i]);
+	if (lane < APO_NPAT * 3) s_ex[warp][lane] = 0ull;
+	__syncthreads();
+	const uint64_t nwarps = (uint64_t)gridDim.x * CC_WARPS;
+	const uint64_t gw = (uint64_t)blockIdx.x * CC_WARPS + warp;
+	const uint64_t lo = total_tiles * gw / nwarps, hi = total_tiles * (gw + 1) / nwarps;
+	if (lo >= hi) return;
+	unsigned long long *ex = s_ex[warp];
+	constexpr int U = ROW == 32 ? 2 : 4;                   // records in flight per lane
+	ScanAcc A;
+	A.zero();
+	uint32_t nrec = 0, run = 0;
+
+	auto flush = [&](uint32_t c) {
+		long long *corp = P.blk + (uint64_t)c * CC_WORDS;
+		scan_flush(A, corp, lane);
+		const uint32_t n = warp_sum_u32(nrec);              // CORP_NREC: corpus_tail writes it for the corpus, the pass counts here
+		if (lane == 0 && n) atomicAdd((unsigned long long *)corp + CORP_NREC, (unsigned long long)n);
+		__syncwarp();
+		if (lane < APO_NPAT * 3) {
+			const unsigned long long v = ex[lane];
+			unsigned long long *slots = (unsigned long long *)corp + CORP_EX + 3 * (lane / 3);
+			if (v != 0ull && v > *((volatile unsigned long long *)&slots[2])) ex_insert(slots, v);
+			ex[lane] = 0ull;
+		}
+		__syncwarp();
+		A.zero();
+		nrec = 0; run = 0;
+	};
+
+	uint32_t cur = (uint32_t)(lo / tiles_per_cand);
+	for (uint64_t tile = lo; tile < hi; tile++) {
+		const uint32_t c = (uint32_t)(tile / tiles_per_cand), j = (uint32_t)(tile - (uint64_t)c * tiles_per_cand);
+		if (c != cur || run == CC_RUN_TILES) { flush(cur); cur = c; }
+		run++;
+		const uint64_t t0 = (uint64_t)j * CC_TILE;
+		const uint4 *row = reinterpret_cast<const uint4 *>(P.rows + (uint64_t)c * P.pitch_evals * ROW);
+		for (int g0 = 0; g0 < CC_GROUPS; g0 += U) {
+			if (t0 + (uint64_t)g0 * 32 >= P.T) break;                           // warp-uniform: the rest of the tile is past the row end
+			uint4 q[U][ROW / 16];
+#pragma unroll
+			for (int u = 0; u < U; u++) {
+				const uint64_t t = t0 + (uint64_t)(g0 + u) * 32 + lane;
+				if (t < P.T) {
+#pragma unroll
+					for (int k = 0; k < ROW / 16; k++) q[u][k] = __ldg(row + t * (ROW / 16) + k);
+				}
+			}
+#pragma unroll
+			for (int u = 0; u < U; u++) {
+				const uint64_t t = t0 + (uint64_t)(g0 + u) * 32 + lane;
+				if (t < P.T) {
+					apo_record r;
+					if constexpr (ROW == 32) { memcpy(&r, q[u], sizeof r); }
+					else { apo_record16 p; memcpy(&p, q[u], sizeof p); r = unpack16(p); }
+					scan_record<false>(A, r, P.idx_base + t, ex, s_cat, s_lut, P.w2);
+					nrec++;
+				}
+			}
+		}
+	}
+	flush(cur);
+}
+
+template <int ROW>
+static cudaError_t launch_cand_corpus(const CandCorpusParams &P, int sm_count, cudaStream_t st) {
+	const uint32_t tiles_per_cand = (uint32_t)((P.T + CC_TILE - 1) / CC_TILE);
+	const uint64_t total_tiles = (uint64_t)tiles_per_cand * P.C;
+	if (total_tiles == 0) return cudaSuccess;
+	int per_sm = 0;
+	cudaError_t err = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_cand_corpus<ROW>, CC_THREADS, 0);
+	if (err != cudaSuccess) return err;
+	uint64_t grid = (uint64_t)sm_count * (uint64_t)(per_sm > 0 ? per_sm : 1);
+	const uint64_t need = (total_tiles + CC_WARPS - 1) / CC_WARPS;
+	if (grid > need) grid = need;
+	k_cand_corpus<ROW><<<(unsigned)grid, CC_THREADS, 0, st>>>(P, tiles_per_cand, total_tiles);
+	return cudaGetLastError();
+}
+
+cudaError_t run_cand_corpus(const CandCorpusParams &P, int row, int sm_count, cudaStream_t st) {
+	if (row == 32) return launch_cand_corpus<32>(P, sm_count, st);
+	if (row == 16) return launch_cand_corpus<16>(P, sm_count, st);
+	return cudaErrorInvalidValue;
+}
+
+// one warp per candidate: the block is copied to the scratch with its example slots as the corpus block holds them (index + 1,
+// 0 = none), so that the accumulating block stays intact for later windows of a session; then build_report at one rank.
+__global__ void __launch_bounds__(32)
+k_cand_corpus_report(const long long *blk, long long *scratch, apo_corpus_report *out) {
+	const uint32_t c = blockIdx.x;
+	const long long *src = blk + (uint64_t)c * CC_WORDS;
+	long long *corp = scratch + (uint64_t)c * CC_WORDS;
+	for (int i = threadIdx.x; i < CC_WORDS; i += 32) {
+		const long long v = src[i];
+		const unsigned long long k = (unsigned long long)v;
+		corp[i] = i < CORP_EX ? v : (k == 0ull ? 0ll : (long long)(~k + 1));
+	}
+	__syncthreads();                                        // build_report reads through L2 what this block wrote (as corpus_tail)
+	FinalizeParams F{};
+	F.nranks = 1;
+	F.report = out + c;
+	build_report(F, corp);
+}
+
+cudaError_t run_cand_corpus_report(long long *blk, uint32_t C, apo_corpus_report *out, cudaStream_t st) {
+	if (C == 0) return cudaSuccess;
+	k_cand_corpus_report<<<C, 32, 0, st>>>(blk, blk + (uint64_t)C * CC_WORDS, out);
 	return cudaGetLastError();
 }
 

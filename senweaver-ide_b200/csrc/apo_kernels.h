@@ -210,6 +210,25 @@ cudaError_t run_cand_breakdown(const CandParams &P, int source, int sm_count, cu
 cudaError_t run_cand_report(const long long *ints, const unsigned long long *ex, const long long *partials, uint32_t C,
                             apo_candidate_report *out, cudaStream_t st);
 
+// ---- per-candidate corpus report (csrc/apo_cand.cu): the corpus scan run over every candidate's rollout records (Form R / R16).
+// Own buffer, never part of the scoring accumulator vector: [C][CC_WORDS] blocks in the corpus-block layout (apo_device.cuh
+// CORP_*), whose CORP_NREC the pass accumulates itself and whose 18 CORP_EX words hold the first-three slots as inverted
+// indices (ex_insert keys, 0 = empty), followed by [C][CC_WORDS] scratch where the report kernel converts them to index + 1.
+constexpr int CC_WORDS = 68 + 18;   // CORP_FIXED + one rank's 18 example slots
+struct CandCorpusParams {
+	uint32_t C;
+	uint64_t T;                     // records per candidate in this launch
+	uint64_t idx_base;              // record position of record 0 of this launch (window start / streamed chunk start)
+	uint64_t pitch_evals;           // candidate row pitch in records
+	const uint8_t *rows;            // Form R (32 B) / R16 (16 B): record 0 of candidate 0
+	const double *lut;              // as K1Params::lut (total weight | reciprocal | categorical product table)
+	double w2;
+	long long *blk;                 // [C][CC_WORDS] of candidate 0 of this launch
+};
+cudaError_t run_cand_corpus(const CandCorpusParams &P, int row, int sm_count, cudaStream_t st);
+// blk: the whole buffer ([C][CC_WORDS] blocks, then the scratch)
+cudaError_t run_cand_corpus_report(long long *blk, uint32_t C, apo_corpus_report *out, cudaStream_t st);
+
 int k1_tile_evals(int row, int variant);
 cudaError_t run_reward9(K1Params P, int row, int variant, bool recip, int sm_count, cudaStream_t st);
 cudaError_t run_detect6(const K2Params &P, int sm_count, cudaStream_t st);

@@ -20,6 +20,7 @@ NDIM, NPAT, NMODE = 9, 6, 5
 SRC_DIMS, SRC_ROLLOUTS, SRC_TUPLES = 0, 1, 2
 TUPLES_MAX = 0xFFFFFF
 SCORE_CORPUS, SCORE_RECIP, SCORE_TIMING, SCORE_CANDIDATES = 0x1, 0x2, 0x4, 0x8
+SCORE_CANDIDATE_CORPUS = 0x10
 TUNE_NO_FUSE, TUNE_FORCE_FUSE, TUNE_NO_STAGING, TUNE_NCCL_JOIN = 0x1, 0x2, 0x4, 0x8
 F_ERRORS, F_ENDED, F_VALID, F_FAILSPAN = 0x01, 0x02, 0x08, 0x10
 UNIQUE_ID_BYTES = 128
@@ -100,7 +101,7 @@ ABI_SYMBOLS = (
     "apo_score_begin", "apo_score_accumulate", "apo_score_finish", "apo_score_host", "apo_score_host_records", "apo_score_host_compact", "apo_compact_encode_host",
     "apo_dims_compact_download", "apo_dims_codebook", "apo_packed_encode_host", "apo_score_host_packed", "apo_dims_packed_download", "apo_dims_d2book",
     "apo_tuple_encode_host", "apo_score_host_tuples", "apo_tuples_upload", "apo_host_alloc", "apo_host_free",
-    "apo_last_timing", "apo_debug_partials", "apo_candidate_reports", "apo_comm_unique_id", "apo_comm_init", "apo_comm_destroy", "apo_comm_join_mode",
+    "apo_last_timing", "apo_debug_partials", "apo_candidate_reports", "apo_candidate_corpus_reports", "apo_comm_unique_id", "apo_comm_init", "apo_comm_destroy", "apo_comm_join_mode",
 )
 
 
@@ -183,6 +184,7 @@ def load_library() -> C.CDLL:
     L.apo_last_timing.argtypes = [vp, C.POINTER(Timing)]
     L.apo_debug_partials.argtypes = [vp, vp, u32]
     L.apo_candidate_reports.argtypes = [vp, u32, u32, vp]
+    L.apo_candidate_corpus_reports.argtypes = [vp, u32, u32, vp]
     L.apo_comm_unique_id.argtypes = [vp]
     L.apo_comm_init.argtypes = [vp, i32, i32, vp]
     L.apo_comm_destroy.argtypes = [vp]
@@ -249,11 +251,12 @@ def records_from_json(text: str | bytes) -> np.ndarray:
 
 
 class ScoreResult:
-    __slots__ = ("scores", "counts", "topk", "report", "timing", "candidates")
+    __slots__ = ("scores", "counts", "topk", "report", "timing", "candidates", "candidate_corpus")
 
-    def __init__(self, scores, counts, topk, report, timing, candidates=None):
+    def __init__(self, scores, counts, topk, report, timing, candidates=None, candidate_corpus=None):
         self.scores, self.counts, self.topk, self.report, self.timing = scores, counts, topk, report, timing
         self.candidates = candidates        # CandidateReport array [C] when the call asked for the breakdown, else None
+        self.candidate_corpus = candidate_corpus   # CorpusReport array [C] when the call asked for the per-candidate corpus reports
 
 
 class Engine:
@@ -393,26 +396,40 @@ class Engine:
         return out
 
     def score_host_records(self, recs: np.ndarray, K: int, corpus: bool = False, recip: bool = False, variant: int = 0,
-                           candidates: bool = False) -> ScoreResult:
+                           candidates: bool = False, candidate_corpus: bool = False) -> ScoreResult:
         """recs: C-contiguous [C][T] of RECORD_DTYPE (32 B) or RECORD16_DTYPE (16 B) in host memory."""
         assert recs.flags.c_contiguous and recs.ndim == 2 and recs.dtype.itemsize in (32, 16)
         Cn, T = recs.shape
-        o = self._opts(K, SRC_ROLLOUTS, corpus, recip, variant, 0, 0, candidates=candidates)
+        o = self._opts(K, SRC_ROLLOUTS, corpus, recip, variant, 0, 0, candidates=candidates, candidate_corpus=candidate_corpus)
         scores = np.empty(Cn, np.float64)
         counts = np.empty(Cn, np.uint64)
         topk = np.empty(K, np.int32)
         rep = CorpusReport() if corpus else None
         self._ck(self._L.apo_score_host_records(self._h, C.byref(o), _p(recs), recs.dtype.itemsize, Cn, T, _p(scores), _p(counts),
                                                 _p(topk), C.byref(rep) if rep is not None else None))
-        return ScoreResult(scores, counts, topk, rep, self.last_timing(), self._cands(Cn, candidates))
+        return ScoreResult(scores, counts, topk, rep, self.last_timing(), self._cands(Cn, candidates),
+                           self._ccorp(Cn, candidate_corpus))
 
     # -- scoring
-    def _opts(self, K, source, corpus, recip, variant, first, count, timing=False, candidates=False) -> ScoreOpts:
+    def _opts(self, K, source, corpus, recip, variant, first, count, timing=False, candidates=False,
+              candidate_corpus=False) -> ScoreOpts:
         return ScoreOpts(K, source, (SCORE_CORPUS if corpus else 0) | (SCORE_RECIP if recip else 0) | (SCORE_TIMING if timing else 0)
-                         | (SCORE_CANDIDATES if candidates else 0), variant, first, count)
+                         | (SCORE_CANDIDATES if candidates else 0) | (SCORE_CANDIDATE_CORPUS if candidate_corpus else 0),
+                         variant, first, count)
 
     def _cands(self, Cn: int, wanted: bool):
         return self.candidate_reports(0, Cn) if wanted else None
+
+    def _ccorp(self, Cn: int, wanted: bool):
+        return self.candidate_corpus_reports(0, Cn) if wanted else None
+
+    def candidate_corpus_reports(self, c0: int, n: int):
+        """apo_candidate_corpus_reports: CorpusReport[n] of candidates [c0, c0+n) from the last scoring call, which must have
+        set candidate_corpus=True (ApoError APO_E_STATE otherwise).  Report c is the corpus report of candidate c's scored
+        rollout records (example indices are absolute record positions)."""
+        out = (CorpusReport * n)()
+        self._ck(self._L.apo_candidate_corpus_reports(self._h, c0, n, out if n else None))
+        return out
 
     def candidate_reports(self, c0: int, n: int):
         """apo_candidate_reports: CandidateReport[n] of candidates [c0, c0+n) from the last scoring call, which must have set
@@ -422,8 +439,9 @@ class Engine:
         return out
 
     def score(self, Cn: int, K: int, source: int = SRC_DIMS, corpus: bool = False, recip: bool = False,
-              variant: int = 0, first: int = 0, count: int = 0, timing: bool = False, candidates: bool = False) -> ScoreResult:
-        o = self._opts(K, source, corpus, recip, variant, first, count, timing, candidates)
+              variant: int = 0, first: int = 0, count: int = 0, timing: bool = False, candidates: bool = False,
+              candidate_corpus: bool = False) -> ScoreResult:
+        o = self._opts(K, source, corpus, recip, variant, first, count, timing, candidates, candidate_corpus)
         scores = np.empty(Cn, np.float64)
         counts = np.empty(Cn, np.uint64)
         topk = np.empty(K, np.int32)
@@ -434,26 +452,28 @@ class Engine:
         if rc != 0:
             self._ck(rc)
         L.apo_last_timing(self._h, C.byref(t))
-        return ScoreResult(scores, counts, topk, rep, t, self._cands(Cn, candidates))
+        return ScoreResult(scores, counts, topk, rep, t, self._cands(Cn, candidates), self._ccorp(Cn, candidate_corpus))
 
     # chunked form: begin / accumulate (per candidate chunk or record window) / finish
     def score_begin(self, C_total: int):
         self._ck(self._L.apo_score_begin(self._h, C_total))
 
     def score_accumulate(self, cand_offset: int = 0, source: int = SRC_DIMS, recip: bool = False, variant: int = 0,
-                         first: int = 0, count: int = 0, candidates: bool = False):
-        o = self._opts(0, source, False, recip, variant, first, count, candidates=candidates)
+                         first: int = 0, count: int = 0, candidates: bool = False, candidate_corpus: bool = False):
+        o = self._opts(0, source, False, recip, variant, first, count, candidates=candidates, candidate_corpus=candidate_corpus)
         self._ck(self._L.apo_score_accumulate(self._h, C.byref(o), cand_offset))
 
-    def score_finish(self, C_total: int, K: int, corpus: bool = False, candidates: bool = False) -> ScoreResult:
-        o = self._opts(K, SRC_DIMS, corpus, False, 0, 0, 0, candidates=candidates)
+    def score_finish(self, C_total: int, K: int, corpus: bool = False, candidates: bool = False,
+                     candidate_corpus: bool = False) -> ScoreResult:
+        o = self._opts(K, SRC_DIMS, corpus, False, 0, 0, 0, candidates=candidates, candidate_corpus=candidate_corpus)
         scores = np.empty(C_total, np.float64)
         counts = np.empty(C_total, np.uint64)
         topk = np.empty(K, np.int32)
         rep = CorpusReport() if corpus else None
         self._ck(self._L.apo_score_finish(self._h, C.byref(o), _p(scores), _p(counts), _p(topk),
                                           C.byref(rep) if rep is not None else None))
-        return ScoreResult(scores, counts, topk, rep, self.last_timing(), self._cands(C_total, candidates))
+        return ScoreResult(scores, counts, topk, rep, self.last_timing(), self._cands(C_total, candidates),
+                           self._ccorp(C_total, candidate_corpus))
 
     def score_host(self, dims: np.ndarray, K: int, corpus: bool = False, recip: bool = False, variant: int = 0,
                    candidates: bool = False) -> ScoreResult:

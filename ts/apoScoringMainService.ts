@@ -20,7 +20,7 @@
 import { VSBuffer } from '../../../../base/common/buffer.js';
 import { ApoResidentQuery, ApoScoreBlocks, ApoTupleBuffers, IApoScoringService } from '../common/apoScoringService.js';
 
-type Blocks = { scores: ArrayBuffer; counts: ArrayBuffer; topk: ArrayBuffer; report: ArrayBuffer; candidates?: ArrayBuffer };
+type Blocks = { scores: ArrayBuffer; counts: ArrayBuffer; topk: ArrayBuffer; report: ArrayBuffer; candidates?: ArrayBuffer; candidateCorpus?: ArrayBuffer };
 
 interface ApoAddon {
 	create(device: number): unknown | null;             // null when no H100 / library: never throws
@@ -32,7 +32,7 @@ interface ApoAddon {
 	scoreResident(handle: unknown, query: ApoResidentQuery): Promise<Blocks>;
 	score(handle: unknown, dims: ArrayBuffer, C: number, T: number, corpus: ArrayBuffer | null, K: number, candidates?: boolean): Promise<Blocks>;
 	scoreHostRecords(handle: unknown, records: ArrayBuffer, rowBytes: number, C: number, T: number, corpus: ArrayBuffer | null, K: number,
-		candidates?: boolean): Promise<Blocks>;
+		candidates?: boolean, candidateCorpus?: boolean): Promise<Blocks>;
 	/** Form D -> Form T on worker threads of the addon (no GPU): 3 bytes per evaluation instead of 36; null = not categorical. */
 	encodeTuples(dims: ArrayBuffer, C: number, T: number, nthreads?: number): Promise<ApoTuples | null>;
 	scoreHostTuples(handle: unknown, tuples: ApoTuples, C: number, T: number, corpus: ArrayBuffer | null, K: number, candidates?: boolean): Promise<Blocks>;
@@ -56,6 +56,7 @@ function wrapBlocks(r: Blocks): ApoScoreBlocks {
 		topk: VSBuffer.wrap(new Uint8Array(r.topk)), report: VSBuffer.wrap(new Uint8Array(r.report)),
 	};
 	if (r.candidates) { out.candidates = VSBuffer.wrap(new Uint8Array(r.candidates)); }     // apo_candidate_report[C]
+	if (r.candidateCorpus) { out.candidateCorpus = VSBuffer.wrap(new Uint8Array(r.candidateCorpus)); }     // apo_corpus_report[C]
 	return out;
 }
 
@@ -187,7 +188,8 @@ export class ApoScoringMainService implements IApoScoringService {
 	}
 
 	async scoreHostRecords(records: VSBuffer, rowBytes: 32 | 16, C: number, T: number, corpus: VSBuffer | undefined, K: number,
-		candidates?: boolean): Promise<ApoScoreBlocks> {
-		return wrapBlocks(await (await this._need()).scoreHostRecords(this._handle, ab(records), rowBytes, C, T, corpus ? ab(corpus) : null, K, !!candidates));
+		candidates?: boolean, candidateCorpus?: boolean): Promise<ApoScoreBlocks> {
+		return wrapBlocks(await (await this._need()).scoreHostRecords(this._handle, ab(records), rowBytes, C, T, corpus ? ab(corpus) : null, K, !!candidates,
+			!!candidateCorpus));
 	}
 }

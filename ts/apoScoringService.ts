@@ -25,6 +25,7 @@ export interface ApoScoreBlocks {
 	topk: VSBuffer;     // int32[K]    score desc, ties -> lower index
 	report: VSBuffer;   // struct apo_corpus_report (784 bytes)
 	candidates?: VSBuffer;   // apo_candidate_report[C] (376 bytes each, candidateReportCodec.ts); only when the call asked for it
+	candidateCorpus?: VSBuffer;   // apo_corpus_report[C] (784 bytes each, decodeCandidateCorpusReport); rollout records only, when asked for
 }
 
 /** Form T of a float32[C][T][9] tensor (include/apo_b200.h): tl uint16[C][T] | th uint8[C][T] = the 24-bit dictionary index of every
@@ -41,6 +42,7 @@ export interface ApoResidentQuery {
 	source?: 0 | 1;         // 0 = dims (Form D / Form Q), 1 = per-(candidate, trace) records
 	corpus?: 0 | 1;         // also build the corpus report from the uploaded corpus
 	candidates?: 0 | 1;     // also build the per-candidate breakdown (ApoScoreBlocks.candidates)
+	candidateCorpus?: 0 | 1;   // source 1 only: also build every candidate's corpus report (ApoScoreBlocks.candidateCorpus)
 	first?: number;         // window [first, first + count) of the trace axis; count 0 = to the end
 	count?: number;
 }
@@ -71,8 +73,10 @@ export interface IApoScoringService {
 	/** dims: float32[C][T][9] (pass C = 1, T = 4 of NaN for report-only calls).
 	 *  candidates: also return the per-candidate breakdown (ApoScoreBlocks.candidates), here and on the other one-shot calls. */
 	score(dims: VSBuffer, C: number, T: number, corpus: VSBuffer | undefined, K: number, candidates?: boolean): Promise<ApoScoreBlocks>;
-	/** [C][T] trace records (the IDE's own representation): 2.2x fewer PCIe bytes than fp32 dims with 16-byte rows. */
-	scoreHostRecords(records: VSBuffer, rowBytes: 32 | 16, C: number, T: number, corpus: VSBuffer | undefined, K: number, candidates?: boolean): Promise<ApoScoreBlocks>;
+	/** [C][T] trace records (the IDE's own representation): 2.2x fewer PCIe bytes than fp32 dims with 16-byte rows.
+	 *  candidateCorpus: also return the corpus report of every candidate's records (ApoScoreBlocks.candidateCorpus). */
+	scoreHostRecords(records: VSBuffer, rowBytes: 32 | 16, C: number, T: number, corpus: VSBuffer | undefined, K: number, candidates?: boolean,
+		candidateCorpus?: boolean): Promise<ApoScoreBlocks>;
 	/** fp32 evaluations -> Form T (include/apo_b200.h): a 24-bit dictionary index per evaluation (3 bytes instead of 36) + the
 	 *  dictionary of distinct evaluations.  For evaluations that are scored more than once, kept, or moved between processes. */
 	encodeTuples(dims: VSBuffer, C: number, T: number): Promise<ApoTupleBuffers | undefined>;
@@ -101,8 +105,9 @@ export class ApoScoringService implements IApoScoringService {
 	score(dims: VSBuffer, C: number, T: number, corpus: VSBuffer | undefined, K: number, candidates?: boolean) {
 		return this._proxy.score(dims, C, T, corpus, K, candidates);
 	}
-	scoreHostRecords(records: VSBuffer, rowBytes: 32 | 16, C: number, T: number, corpus: VSBuffer | undefined, K: number, candidates?: boolean) {
-		return this._proxy.scoreHostRecords(records, rowBytes, C, T, corpus, K, candidates);
+	scoreHostRecords(records: VSBuffer, rowBytes: 32 | 16, C: number, T: number, corpus: VSBuffer | undefined, K: number, candidates?: boolean,
+		candidateCorpus?: boolean) {
+		return this._proxy.scoreHostRecords(records, rowBytes, C, T, corpus, K, candidates, candidateCorpus);
 	}
 	encodeTuples(dims: VSBuffer, C: number, T: number) { return this._proxy.encodeTuples(dims, C, T); }
 	scoreTuples(tuples: ApoTupleBuffers, C: number, T: number, corpus: VSBuffer | undefined, K: number, candidates?: boolean) {

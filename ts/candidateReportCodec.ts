@@ -8,10 +8,14 @@
  *  rollouts of the candidate whose feedback was 'bad'.  The beam loop's critique step
  *  (_buildTextualGradientPrompt, APO:918-962) can name what a parent lost on from this.
  *
- *  The byte offsets below are pinned to the C struct by tests/test_napi_candidates.py.
+ *  Also the decoder of the per-candidate corpus reports (ApoScoreBlocks.candidateCorpus): apo_corpus_report[C], the whole
+ *  corpus report of each candidate's rollout records (problem patterns, byMode, tool totals included), decoded by
+ *  traceRecordCodec's decodeCorpusReport.
+ *
+ *  The byte offsets below are pinned to the C structs by tests/test_napi_candidates.py and tests/test_candidate_corpus_cpu.py.
  *--------------------------------------------------------------------------------------------*/
 import { VSBuffer } from '../../../../base/common/buffer.js';
-import { DIM_NAMES } from './traceRecordCodec.js';
+import { CorpusReportNumbers, DIM_NAMES, decodeCorpusReport } from './traceRecordCodec.js';
 
 const CANDIDATE_REPORT_BYTES = 376;
 const OFF_TOTAL = 0;
@@ -72,4 +76,19 @@ export function decodeCandidateReport(buf: VSBuffer, c: number): CandidateReport
 		rewardSum: v.getFloat64(OFF_REWARD_SUM, true), avgReward: withReward ? v.getFloat64(OFF_AVG_REWARD, true) : null,
 		rewardByDimension, badExamples,
 	};
+}
+
+const CORPUS_REPORT_BYTES = 784;         // sizeof(apo_corpus_report)
+
+/** Number of reports in a candidateCorpus block. */
+export function candidateCorpusReportCount(buf: VSBuffer): number {
+	return Math.floor(buf.byteLength / CORPUS_REPORT_BYTES);
+}
+
+/** Corpus report of candidate c from a candidateCorpus block (ApoScoreBlocks.candidateCorpus); pattern examples are rollout
+ *  indices (absolute positions on the candidate's record axis). */
+export function decodeCandidateCorpusReport(buf: VSBuffer, c: number): CorpusReportNumbers {
+	const base = c * CORPUS_REPORT_BYTES;
+	if (c < 0 || base + CORPUS_REPORT_BYTES > buf.byteLength) { throw new RangeError(`candidate ${c} outside the block`); }
+	return decodeCorpusReport(buf.slice(base, base + CORPUS_REPORT_BYTES));
 }
