@@ -85,6 +85,37 @@ assert e.debug_partials(3) == orc.score_dims_fx(dt)
 e.tuples_upload(tl, th, tbook, bkt, d2t)
 e.score(3, 2, source=pkg.SRC_TUPLES, first=8, count=8192 + 100)
 assert e.debug_partials(3) == orc.score_dims_fx(dt[:, 8:8192 + 108])
+# per-candidate breakdown (k_cand_breakdown + k_cand_report) on every record source, and the per-candidate corpus reports
+# (k_cand_corpus + k_cand_corpus_report) on the two that carry record fields
+from oracle import candidates as oc  # noqa: E402
+oc.build()
+dref = [(d["bad"], d["badExamples"]) for d in oc.cand_dims(dt)]
+for run in (lambda: e.score(3, 1, source=pkg.SRC_TUPLES, candidates=True),
+            lambda: e.score_host_tuples(tl, th, tbook, bkt, d2t, 1, candidates=True),
+            lambda: e.score_host_packed(pt, pdt, bkt, d2t, 1, candidates=True),
+            lambda: e.score_host(dt, 1, candidates=True)):
+    assert [(b.bad, list(b.badExamples)) for b in run().candidates] == dref
+e.dims_upload(dt)
+assert [(b.bad, list(b.badExamples)) for b in e.score(3, 1, candidates=True).candidates] == dref
+e.dims_upload_compact(dt)
+assert [(b.bad, list(b.badExamples)) for b in e.score(3, 1, candidates=True).candidates] == dref
+rref = [(d["bad"], d["badExamples"]) for d in oc.cand_records(roll)]
+e.rollouts_upload(roll)
+assert [(b.bad, list(b.badExamples)) for b in e.score(C, 2, source=1, candidates=True).candidates] == rref
+cc = e.score(C, 2, source=1, candidate_corpus=True).candidate_corpus
+assert [bytes(x) for x in e.score_host_records(roll, 2, candidate_corpus=True).candidate_corpus] == [bytes(x) for x in cc]
+assert [(b.bad, list(b.badExamples)) for b in e.score_host_records(roll, 2, candidates=True).candidates] == rref
+for c in range(C):
+    rc = orc.report(roll[c])
+    assert cc[c].bad == rc.bad and [list(cc[c].pat[p].examples) for p in range(6)] == [list(rc.pat[p].examples) for p in range(6)]
+r16 = pkg.pack16(roll)
+rref = [(d["bad"], d["badExamples"]) for d in oc.cand_records(orc.unpack16(r16))]
+e.rollouts16_upload(r16)
+assert [(b.bad, list(b.badExamples)) for b in e.score(C, 2, source=1, candidates=True).candidates] == rref
+assert [(b.bad, list(b.badExamples)) for b in e.score_host_records(r16, 2, candidates=True).candidates] == rref
+cc = e.score(C, 2, source=1, candidate_corpus=True).candidate_corpus
+assert [bytes(x) for x in e.score_host_records(r16, 2, candidate_corpus=True).candidate_corpus] == [bytes(x) for x in cc]
+assert [cc[c].pat[1].count for c in range(C)] == [orc.report(orc.unpack16(r16[c])).pat[1].count for c in range(C)]
 for Cn in ((3, 1500, 3000) if not os.environ.get("SMOKE_NO_MANY_CANDIDATES") else ()):       # counting top-K (<= 2048 keys in shared memory) and the radix select
     e.dims_generate(seed, 0, Cn, 0, 64, 300)
     r = e.score(Cn, min(Cn, 40))
