@@ -269,7 +269,8 @@ int apo_score_host_records(apo_engine *e, const apo_score_opts *o, const void *r
  * per evaluation instead of 36) + the codebook (8 x 256 fp32 bit patterns, 0xFFFFFFFF = unused) that assigns the codes.
  * apo_compact_encode_host builds them from Form D on the host (two passes on nthreads threads; APO_E_STATE when a coded
  * dimension has more than 255 distinct values); apo_dims_compact_download / apo_dims_codebook export a resident Form Q
- * tensor.  Results are bit-identical to scoring the Form D tensor. */
+ * tensor.  Results are bit-identical to scoring the Form D tensor.  The codebook must be the one that assigned the planes'
+ * codes: this call has no per-evaluation pass to check them, and a code naming an empty slot is scored as a present 0.0. */
 int apo_compact_encode_host(const float *dims, uint32_t C, uint64_t T, uint64_t *q8, float *d2, uint16_t *li,
                             uint32_t *codebook /* [8*256] */, int nthreads);
 int apo_dims_compact_download(apo_engine *e, uint64_t *q8, float *d2, uint16_t *li, uint32_t c, uint64_t first, uint64_t n);
@@ -281,7 +282,9 @@ int apo_score_host_compact(apo_engine *e, const apo_score_opts *o, const uint64_
  * 0,1,3,4,5,6,7,8; 15 = absent), pd = 12-bit index of the tool_success_rate value into d2book (4095 = absent), both [C][T].
  * Needs <= 15 distinct values per coded dimension and <= 4095 distinct tool_success_rate values (APO_E_STATE otherwise:
  * fall back to Form Q / Form D); dims produced by TCS:668-763 always qualify.  The device expands every window to Form Q
- * (k_unpack_p) right behind its H2D copy and scores it with K1q: same integers, 2.3x fewer PCIe bytes than Form Q. */
+ * (k_unpack_p) right behind its H2D copy and scores it with K1q: same integers, 2.3x fewer PCIe bytes than Form Q.
+ * Both codebooks travel with the planes (empty slots 0xFFFFFFFF): an evaluation whose code names an empty or NaN codebook
+ * slot, or whose tool_success_rate index names an empty or NaN d2book slot, fails the call with APO_E_ARG. */
 int apo_packed_encode_host(const float *dims, uint32_t C, uint64_t T, uint32_t *pc, uint16_t *pd,
                            uint32_t *codebook /* [8*256] */, uint32_t *d2book /* [4096] fp32 bit patterns */, int nthreads);
 /* Export of a resident Form Q tensor in Form P (rows of candidate c) and the tool_success_rate table that goes with it
@@ -300,7 +303,9 @@ int apo_score_host_packed(apo_engine *e, const apo_score_opts *o, const uint32_t
  * receives the number of distinct evaluations; APO_E_STATE when that exceeds cap (<= 16777215 = APO_TUPLES_MAX) — keep Form P then.
  * apo_score_host_tuples streams the planes from host memory (as apo_score_host_packed does for Form P);
  * apo_tuples_upload makes them resident: apo_score / apo_score_accumulate with source APO_SRC_TUPLES then read 3 B per evaluation.
- * An index >= n_tuples in the planes, or an entry whose finalReward is not within (-2, 2), fails the call with APO_E_ARG. */
+ * An index >= n_tuples in the planes, or a dictionary entry whose finalReward is not within (-2, 2) or that names an empty or
+ * NaN slot of the codebook or of d2book, fails the call with APO_E_ARG.  Entries are checked whether or not an evaluation
+ * names them. */
 #define APO_TUPLES_MAX 16777215u
 int apo_tuple_encode_host(const uint32_t *pc, const uint16_t *pd, uint32_t C, uint64_t T, uint16_t *tl, uint8_t *th,
                           uint32_t *tbook_pc, uint16_t *tbook_pd, uint32_t cap, uint32_t *n_tuples, int nthreads);

@@ -97,6 +97,7 @@ struct apo_engine {
 	// Form Q (compact) copy of the evaluations: replaces dims/dims_ptr when `compact` is set
 	DevBuf<unsigned long long> q8; DevBuf<float> qd2; DevBuf<unsigned short> qli; DevBuf<uint32_t> qbook;   // qbook: [8][256] codebook + [8] overflow flags
 	DevBuf<double> d_ptab, d_pair; DevBuf<float> stage, d_cbf, d_d2book, d_d2stream; uint32_t q_n0 = 0, q_n1 = 0; bool q_pair_ok = false;
+	DevBuf<uint32_t> unpack_bad;                              // k_unpack_p: an evaluation named an empty or NaN codebook slot
 	uint32_t qbook_host[8 * 256]; bool compact = false;
 	uint32_t d2book_host[4096]; uint32_t d2book_n = ~0u;       // Form P export of the resident tensor (~0 = not built yet)
 	DevBuf<uint8_t> roll; uint32_t roll_C = 0, roll_row = 32; uint64_t roll_T = 0, roll_pitch = 0;   // Form R (32 B) or R16 (16 B) rows
@@ -233,14 +234,15 @@ int upload_luts(apo_engine *e) {
 	return APO_OK;
 }
 
-// value*weight per code for the eight coded dimensions (csrc/apo_compact.cu); table 0 = fl(0 + d0*w0)
-std::vector<double> make_ptab(const uint32_t *book, const apo::Weights &W) {
+// value*weight per code for the eight coded dimensions (csrc/apo_compact.cu); table 0 = fl(0 + d0*w0).  Empty slots hold
+// `empty`: +0.0 for K1q, NaN for k_tuple_values, which refuses an entry that names one.  Slot 255 (absent) is +0.0.
+std::vector<double> make_ptab(const uint32_t *book, const apo::Weights &W, double empty = 0.0) {
 	static const int dim_of[8] = {0, 1, 3, 4, 5, 6, 7, 8};
 	std::vector<double> tab(8 * 256, 0.0);
 	for (int j = 0; j < 8; j++)
 		for (int c = 0; c < 255; c++) {
 			const uint32_t bits = book[256 * j + c];
-			if (bits == 0xFFFFFFFFu) continue;
+			if (bits == 0xFFFFFFFFu) { tab[256 * j + c] = empty; continue; }
 			float f; memcpy(&f, &bits, 4);
 			volatile double p = (double)f * W.w[dim_of[j]];             // TCS:781 value * weight
 			if (j == 0) { volatile double z = 0.0; p = z + p; }          // weightedSum = 0 + first product
@@ -509,7 +511,7 @@ int record_k1_event(apo_engine *e, int which) {
 
 // Form T: finalReward of every dictionary entry for the current weights (device work on e->stream, no synchronisation)
 int tuples_values(apo_engine *e, const uint32_t *book_host, const uint32_t *d_pc, const unsigned short *d_pd, uint32_t n, const float *d_d2, bool recip) {
-	const std::vector<double> tab = make_ptab(book_host, e->W);
+	const std::vector<double> tab = make_ptab(book_host, e->W, std::nan(""));
 	CK(e->tup_ptab.reserve(8 * 256));
 	CK(e->tup_val.reserve((uint64_t)n + 1));
 	CK(e->tup_bad.reserve(1));
@@ -979,7 +981,7 @@ extern "C" void apo_destroy(apo_engine *e) {
 	peer_teardown(e);
 	if (e->comm && g_nccl.CommDestroy) g_nccl.CommDestroy(e->comm);
 	if (e->zc_host) cudaFreeHost(e->zc_host);
-	e->q8.release(); e->qd2.release(); e->qli.release(); e->qbook.release(); e->d_ptab.release(); e->d_pair.release(); e->d_cbf.release(); e->d_d2book.release(); e->d_d2stream.release(); e->stage.release();
+	e->q8.release(); e->qd2.release(); e->qli.release(); e->qbook.release(); e->d_ptab.release(); e->d_pair.release(); e->d_cbf.release(); e->d_d2book.release(); e->d_d2stream.release(); e->unpack_bad.release(); e->stage.release();
 	e->d_lut.release(); e->corpus.release(); e->dims.release(); e->roll.release(); e->acc.release(); e->acc_joined.release(); e->acc_snapshot.release(); e->misc.release();
 	e->result.release(); e->keys.release(); e->sel_key.release(); e->sel_idx.release();
 	e->tups_pc.release(); e->tups_pd.release(); e->tups_d2.release();
@@ -1675,9 +1677,17 @@ int score_host_compact_impl(apo_engine *e, const apo_score_opts *o, const uint64
 	if (Tc < (uint64_t)tile) Tc = tile;
 	if (Tc > round_up(T ? T : 1, tile)) Tc = round_up(T ? T : 1, tile);
 	for (int i = 0; i < 2; i++) CK(e->win[i].reserve((uint64_t)C * Tc * (packed ? 20 : 14)));
+	uint64_t code_ok[2] = {0, 0};      // Form P: bit 16 j + c set when code c of coded dimension j names a value (not empty, not NaN)
 	if (packed) {
+		for (int j = 0; j < 8; j++)
+			for (int c = 0; c < 15; c++) {
+				const uint32_t bits = codebook[256 * j + c];
+				if ((bits & 0x7FFFFFFFu) <= 0x7F800000u) code_ok[j >> 2] |= 1ull << (16 * (j & 3) + c);
+			}
 		CK(e->d_d2stream.reserve(4096));
-		CK(cudaMemcpyAsync(e->d_d2stream.p, d2book, 4096 * 4, cudaMemcpyHostToDevice, e->stream));   // bit patterns: unused slots are NaNs nobody reads
+		CK(e->unpack_bad.reserve(1));
+		CK(cudaMemcpyAsync(e->d_d2stream.p, d2book, 4096 * 4, cudaMemcpyHostToDevice, e->stream));   // bit patterns: empty slots are NaNs, flagged if named
+		CK(cudaMemsetAsync(e->unpack_bad.p, 0, 4, e->stream));
 	}
 	choose_timing(e, o, (uint64_t)C * T * wire);
 	if (peer_join_active(e, C)) e->join_epoch++;
@@ -1705,7 +1715,7 @@ int score_host_compact_impl(apo_engine *e, const apo_score_opts *o, const uint64
 		CK(cudaEventRecord(e->win_ready[b], e->copy_stream));
 		CK(cudaStreamWaitEvent(e->stream, e->win_ready[b], 0));
 		if (packed) {
-			CK(apo::run_unpack_p(wpc, wpd, Tc, C, n, e->d_d2stream.p, wq, wd, wl, Tc, e->stream));
+			CK(apo::run_unpack_p(wpc, wpd, Tc, C, n, e->d_d2stream.p, code_ok[0], code_ok[1], e->unpack_bad.p, wq, wd, wl, Tc, e->stream));
 			e->timing.launches++;
 		}
 		apo::KqParams Q{};
@@ -1728,6 +1738,12 @@ int score_host_compact_impl(apo_engine *e, const apo_score_opts *o, const uint64
 		CK(cudaEventRecord(e->win_free[b], e->stream));
 	}
 	if ((rc = finish_score(e, o, C, scores, counts, topk, report))) return rc;
+	if (packed) {                                                  // finish_score has synchronised the stream
+		uint32_t bad = 0;
+		CK(cudaMemcpyAsync(&bad, e->unpack_bad.p, 4, cudaMemcpyDeviceToHost, e->stream));
+		CK(cudaStreamSynchronize(e->stream));
+		if (bad) return fail(e, APO_E_ARG, "an evaluation names an empty or NaN slot of the codebook or of d2book");
+	}
 	return cand ? cand_finish(e, C) : APO_OK;
 }
 }  // namespace

@@ -128,11 +128,12 @@ cudaError_t run_recode(unsigned long long *q8, float *d2, unsigned short *li, ui
 // fp32 table (4095 = absent; <= 4095 distinct ratios).  Expansion runs at HBM speed right behind the H2D copy of a window.
 __global__ void __launch_bounds__(256)
 k_unpack_p(const uint32_t *pc, const unsigned short *pd, uint64_t pitch_in, uint32_t C, uint64_t T, const float *d2book,
-           unsigned long long *q8, float *d2, unsigned short *li, uint64_t pitch_out) {
+           uint64_t ok_lo, uint64_t ok_hi, uint32_t *bad, unsigned long long *q8, float *d2, unsigned short *li, uint64_t pitch_out) {
 	// d2book is read through the read-only path: a tensor uses a few hundred of its 4096 entries, which stay in L1
 	// (staging the 16 KB table in shared memory per block cost more than the block's own 256 evaluations)
 	const uint32_t c = blockIdx.y;
 	if (c >= C) return;
+	bool named_empty = false;                // a code whose codebook slot is empty or NaN (ok bit 16 j + code clear), or a NaN d2
 	for (uint64_t t = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; t < T; t += (uint64_t)gridDim.x * blockDim.x) {
 		const uint32_t w = pc[(uint64_t)c * pitch_in + t];
 		const uint32_t k2 = pd[(uint64_t)c * pitch_in + t] & 4095u;
@@ -144,29 +145,34 @@ k_unpack_p(const uint32_t *pc, const unsigned short *pd, uint64_t pitch_in, uint
 			const uint32_t code = nib == 15u ? 255u : nib;
 			q |= (unsigned long long)code << (8 * j);
 			mask |= (nib != 15u ? 1u : 0u) << (j < 2 ? j : j + 1);
+			if (nib != 15u && !(((j < 4 ? ok_lo : ok_hi) >> (16 * (j & 3) + nib)) & 1u)) named_empty = true;
 		}
 		const bool p2 = k2 != 4095u;
 		mask |= (p2 ? 1u : 0u) << 2;
 		const uint64_t o = (uint64_t)c * pitch_out + t;
 		q8[o] = q;
-		d2[o] = p2 ? __ldg(d2book + k2) : 0.0f;
+		const float v2 = p2 ? __ldg(d2book + k2) : 0.0f;
+		if (!(v2 == v2)) named_empty = true;
+		d2[o] = v2;
 		// The empty asm keeps the index computation in 32-bit registers.  Narrowed to 16-bit operations (the store is 16 bits
 		// wide), ptxas for sm_90a dropped the dimension-2 presence bit, and K1q then renormalised without tool_success_rate.
 		uint32_t idx = lut_index(mask);
 		asm("" : "+r"(idx));
 		li[o] = (unsigned short)idx;
 	}
+	if (named_empty) atomicOr(bad, 1u);
 }
 
 cudaError_t run_unpack_p(const uint32_t *pc, const unsigned short *pd, uint64_t pitch_in, uint32_t C, uint64_t T, const float *d2book,
-                         unsigned long long *q8, float *d2, unsigned short *li, uint64_t pitch_out, cudaStream_t st) {
+                         uint64_t ok_lo, uint64_t ok_hi, uint32_t *bad, unsigned long long *q8, float *d2, unsigned short *li,
+                         uint64_t pitch_out, cudaStream_t st) {
 	if (C == 0 || T == 0) return cudaSuccess;
 	uint64_t gx = (T + 1023) / 1024;                              // four evaluations per thread and row
 	if (gx > 132ull * 8) gx = 132ull * 8;
 	for (uint32_t cb = 0; cb < C; cb += 32768) {
 		const uint32_t cn = C - cb < 32768 ? C - cb : 32768;
 		k_unpack_p<<<dim3((unsigned)gx, cn), 256, 0, st>>>(pc + (uint64_t)cb * pitch_in, pd + (uint64_t)cb * pitch_in, pitch_in, cn, T, d2book,
-		                                                 q8 + (uint64_t)cb * pitch_out, d2 + (uint64_t)cb * pitch_out, li + (uint64_t)cb * pitch_out, pitch_out);
+		                                                 ok_lo, ok_hi, bad, q8 + (uint64_t)cb * pitch_out, d2 + (uint64_t)cb * pitch_out, li + (uint64_t)cb * pitch_out, pitch_out);
 	}
 	return cudaGetLastError();
 }

@@ -137,8 +137,11 @@ cudaError_t run_reward9q(KqParams P, int variant, bool recip, int sm_count, cuda
 cudaError_t run_transcode(const float *dims, uint64_t pitch_in, uint32_t C, uint64_t T, unsigned long long *q8, float *d2,
                           uint64_t pitch_out, uint32_t *codebook, uint32_t *overflow, cudaStream_t st);
 cudaError_t run_recode(unsigned long long *q8, float *d2, unsigned short *li, uint64_t n, const uint8_t *remap, cudaStream_t st);
+// ok_lo / ok_hi: bit 16 j + c set when code c of coded dimension j names a value; *bad |= 1 when an evaluation names a slot
+// that does not (empty or NaN), or a NaN tool_success_rate slot
 cudaError_t run_unpack_p(const uint32_t *pc, const unsigned short *pd, uint64_t pitch_in, uint32_t C, uint64_t T, const float *d2book,
-                         unsigned long long *q8, float *d2, unsigned short *li, uint64_t pitch_out, cudaStream_t st);
+                         uint64_t ok_lo, uint64_t ok_hi, uint32_t *bad, unsigned long long *q8, float *d2, unsigned short *li,
+                         uint64_t pitch_out, cudaStream_t st);
 cudaError_t run_collect_d2(const float *d2, const unsigned short *li, uint64_t n, uint32_t *table, uint32_t *count, cudaStream_t st);
 cudaError_t run_pack_p(const unsigned long long *q8, const float *d2, const unsigned short *li, uint64_t n, const uint32_t *d2book, uint32_t nbook,
                        uint32_t *pc, unsigned short *pd, uint32_t *bad, cudaStream_t st);
@@ -166,12 +169,12 @@ struct TupleValParams {
 	const uint32_t *tb_pc;          // [n] Form P code word of the entry (eight 4-bit codes, 15 = absent)
 	const unsigned short *tb_pd;    // [n] 12-bit tool_success_rate index (4095 = absent)
 	uint32_t n;
-	const double *ptab;             // [8][256] as KqParams::ptab
+	const double *ptab;             // [8][256] as KqParams::ptab, but NaN in empty slots
 	const double *lut;              // as K1Params::lut
 	const float *d2book;            // [4096]
 	double w2;
 	long long *tval;                // [n + 1] out
-	uint32_t *bad;                  // bit 1: an entry is not representable (|reward| >= 2, NaN tool_success_rate)
+	uint32_t *bad;                  // bit 1: an entry is not representable (|reward| >= 2, or it names an empty or NaN slot of a codebook)
 };
 int kt_tile_evals();
 cudaError_t run_tuple_values(const TupleValParams &P, bool recip, cudaStream_t st);

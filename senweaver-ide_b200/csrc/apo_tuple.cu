@@ -29,7 +29,7 @@ k_tuple_values(const TupleValParams P) {
 #pragma unroll
 	for (int j = 0; j < 8; j++) {
 		const uint32_t nib = (w >> (4 * j)) & 15u;
-		code[j] = nib == 15u ? 255u : nib;                          // product table slot 255 holds +0.0
+		code[j] = nib == 15u ? 255u : nib;                          // product table slot 255 holds +0.0, empty slots NaN
 		mask |= (nib != 15u ? 1u : 0u) << (j < 2 ? j : j + 1);
 	}
 	const bool p2 = k2 != 4095u;
@@ -45,8 +45,9 @@ k_tuple_values(const TupleValParams P) {
 	const double v = div_lut<RECIP>(ws, t);
 	const long long fx = to_fx(v);
 	const bool counted = t.x > 0.0;
+	// ws is NaN when the entry names an empty or NaN slot of either codebook (the product table holds NaN there).
 	// K1t adds up to 16 entries before it splits value and count: |fx| < 2^53 keeps their sum below the count field
-	if (!(d2f == d2f) || !(v == v) || fx >= (1ll << 53) || fx <= -(1ll << 53)) atomicOr(P.bad, 2u);
+	if (!(ws == ws) || !(v == v) || fx >= (1ll << 53) || fx <= -(1ll << 53)) atomicOr(P.bad, 2u);
 	P.tval[i] = fx + ((long long)(counted ? 1 : 0) << KT_VALID_SHIFT);
 }
 

@@ -85,6 +85,19 @@ assert e.debug_partials(3) == orc.score_dims_fx(dt)
 e.tuples_upload(tl, th, tbook, bkt, d2t)
 e.score(3, 2, source=pkg.SRC_TUPLES, first=8, count=8192 + 100)
 assert e.debug_partials(3) == orc.score_dims_fx(dt[:, 8:8192 + 108])
+# Form T, hand-built (tests/tuple_fixtures.py): the largest dictionary (2^24 - 1 entries), indices with every high byte
+sys.path.insert(0, os.path.join(ROOT, "tests"))
+import tuple_fixtures as tfx  # noqa: E402
+tbx, bkx, d2x = tfx.dictionary(tfx.TUPLES_MAX), tfx.codebook(), tfx.d2book()
+ix = tfx.hi_byte_groups(tfx.TUPLES_MAX, 2, 2 * 8192 + 77)
+assert len(np.unique(ix >> 16)) == 256
+wx = tfx.expected(ix, *tfx.entry_fx(tbx, bkx, d2x))
+e.score_host_tuples(*tfx.planes(ix), tbx, bkx, d2x, 1)
+assert e.debug_partials(2) == wx
+e.tuples_upload(*tfx.planes(ix), tbx, bkx, d2x)
+e.score(2, 1, source=pkg.SRC_TUPLES)
+assert e.debug_partials(2) == wx
+e.tuples_upload(tl, th, tbook, bkt, d2t)                          # the generated tensor again, for the breakdown below
 # per-candidate breakdown (k_cand_breakdown + k_cand_report) on every record source, and the per-candidate corpus reports
 # (k_cand_corpus + k_cand_corpus_report) on the two that carry record fields
 from oracle import candidates as oc  # noqa: E402
