@@ -16,7 +16,6 @@
 #include <utility>
 #include <thread>
 #include <vector>
-#include <vector>
 
 #include "../../include/apo_b200.h"
 #include "apo_format.h"
@@ -31,6 +30,7 @@ std::string g_create_error;
 
 // TCS:766-776 in push order d0..d8
 const double kDefaultWeights[APO_NDIM] = {0.25, 0.18, 0.12, 0.08, 0.05, 0.05, 0.08, 0.08, 0.11};
+const int kCodedDim[8] = {0, 1, 3, 4, 5, 6, 7, 8};   // push-order dimension of coded dimension j (Form Q / P / T; d2 is not coded)
 
 // ---- NCCL through dlopen: the library loads (and every single-GPU path works) without it
 struct NcclId { char b[APO_UNIQUE_ID_BYTES]; };
@@ -237,14 +237,13 @@ int upload_luts(apo_engine *e) {
 // value*weight per code for the eight coded dimensions (csrc/apo_compact.cu); table 0 = fl(0 + d0*w0).  Empty slots hold
 // `empty`: +0.0 for K1q, NaN for k_tuple_values, which refuses an entry that names one.  Slot 255 (absent) is +0.0.
 std::vector<double> make_ptab(const uint32_t *book, const apo::Weights &W, double empty = 0.0) {
-	static const int dim_of[8] = {0, 1, 3, 4, 5, 6, 7, 8};
 	std::vector<double> tab(8 * 256, 0.0);
 	for (int j = 0; j < 8; j++)
 		for (int c = 0; c < 255; c++) {
 			const uint32_t bits = book[256 * j + c];
 			if (bits == 0xFFFFFFFFu) { tab[256 * j + c] = empty; continue; }
 			float f; memcpy(&f, &bits, 4);
-			volatile double p = (double)f * W.w[dim_of[j]];             // TCS:781 value * weight
+			volatile double p = (double)f * W.w[kCodedDim[j]];          // TCS:781 value * weight
 			if (j == 0) { volatile double z = 0.0; p = z + p; }          // weightedSum = 0 + first product
 			tab[256 * j + c] = p;
 		}
@@ -537,57 +536,108 @@ int tuples_check(apo_engine *e) {
 	return APO_OK;
 }
 
-// one K1 launch over [first, first+count) of the loaded source into candidates [cand_offset, ...)
-int launch_k1_resident(apo_engine *e, const apo_score_opts *o, uint32_t cand_offset, uint64_t first, uint64_t count,
-                       const apo::K2Params *fused = nullptr) {
-	const bool raw = o->source == APO_SRC_ROLLOUTS;
-	const uint32_t C = raw ? e->roll_C : e->dims_C;
-	int rc;
+// ---- the evaluations one launch reads: a resident tensor (or a window of it), or one window of a host-streaming call
+using Form = apo::CandSource;   // the five layouts: CAND_DIMS (Form D), CAND_REC32 / CAND_REC16 (Form R / R16), CAND_Q, CAND_T
+
+struct Evals {
+	Form form = apo::CAND_DIMS;
+	int variant = 0;                          // kernel variant (Form Q: after the fall-back to the product tables)
+	uint32_t C = 0;
+	uint64_t count = 0;                       // evaluations per candidate
+	uint64_t pitch_evals = 0;                 // candidate row pitch
+	uint64_t idx_base = 0;                    // record position of evaluation 0: the window start or the streamed chunk start
+	const uint8_t *rows = nullptr;            // Form D / R / R16: evaluation 0 of candidate 0
+	const unsigned long long *q8 = nullptr;   // Form Q planes
+	const float *d2 = nullptr;
+	const unsigned short *li = nullptr;
+	const unsigned short *tl = nullptr;       // Form T planes + dictionary
+	const unsigned char *th = nullptr;
+	const uint32_t *tb_pc = nullptr;
+	const unsigned short *tb_pd = nullptr;
+	uint32_t n_tuples = 0;
+	const float *d2book = nullptr;
+	const uint32_t *codebook = nullptr;       // resident Form T: every launch rebuilds this codebook's tables (NULL: built once per call)
+
+	bool records() const { return form == apo::CAND_REC32 || form == apo::CAND_REC16; }
+	uint32_t row() const { return form == apo::CAND_DIMS ? 36 : form == apo::CAND_REC32 ? 32 : 16; }
+	uint32_t bytes() const { return form == apo::CAND_T ? 3 : form == apo::CAND_Q ? 14 : row(); }   // read per evaluation
+	uint64_t tile() const {                   // evaluations per tile of the scoring kernel
+		return (uint64_t)(form == apo::CAND_T ? apo::kt_tile_evals() : form == apo::CAND_Q ? apo::kq_tile_evals(variant)
+		                                                                                   : apo::k1_tile_evals((int)row(), variant));
+	}
+};
+
+// the whole tensor loaded for o->source (count = all its evaluations)
+int resident_evals(apo_engine *e, const apo_score_opts *o, Evals *ev) {
+	if (!o) return fail(e, APO_E_ARG, "opts is NULL");
+	if (o->source > APO_SRC_TUPLES) return fail(e, APO_E_ARG, "unknown source %u", o->source);
+	Evals &v = *ev;
+	v = Evals{};
+	v.variant = (int)o->variant;
 	if (o->source == APO_SRC_TUPLES) {
-		if (!count) return APO_OK;
-		if (first % 8) return fail(e, APO_E_ARG, "window start must be a multiple of 8 for Form T");
-		if ((rc = tuples_values(e, e->tup_book, e->tup_pc.p, e->tup_pd.p, e->tup_n, e->tup_d2.p, (o->flags & APO_SCORE_RECIP) != 0))) return rc;
-		apo::KtParams P{};
-		P.tl = e->tup_l.p + first; P.th = e->tup_h.p + first; P.pitch_evals = e->tup_pitch; P.C = e->tup_C; P.T = count;
-		P.acc = e->acc.p + (uint64_t)ACC_PER_CAND * cand_offset; P.tval = e->tup_val.p; P.n_tuples = e->tup_n; P.bad = e->tup_bad.p;
-		if ((rc = record_k1_event(e, 0))) return rc;
-		CK(apo::run_reward9t(P, e->sm_count, e->stream));
-		if ((rc = record_k1_event(e, 1))) return rc;
-		e->timing.launches++;
-		return APO_OK;
-	}
-	if (!raw && e->compact) {
-		if (!count) return APO_OK;
-		if (first % 8) return fail(e, APO_E_ARG, "window start must be a multiple of 8 for the compact layout");
-		apo::KqParams Q{};
-		Q.q8 = e->q8.p + first; Q.d2 = e->qd2.p + first; Q.li = e->qli.p + first; Q.pitch_evals = e->dims_pitch; Q.C = C; Q.T = count;
-		Q.acc = e->acc.p + (uint64_t)ACC_PER_CAND * cand_offset; Q.lut = e->d_lut.p; Q.ptab = e->d_ptab.p; Q.w2 = e->W.w[2];
-		Q.pair = e->d_pair.p; Q.cbf = e->d_cbf.p; Q.n0 = e->q_n0; Q.n1 = e->q_n1;
-		{
-			static const int dim_of[8] = {0, 1, 3, 4, 5, 6, 7, 8};
-			for (int j = 0; j < 8; j++) Q.wq[j] = e->W.w[dim_of[j]];
+		if (e->tup_l.p == nullptr || e->tup_C == 0) return fail(e, APO_E_STATE, "no tuples loaded");
+		v.form = apo::CAND_T; v.C = e->tup_C; v.count = e->tup_T; v.pitch_evals = e->tup_pitch;
+		v.tl = e->tup_l.p; v.th = e->tup_h.p;
+		v.tb_pc = e->tup_pc.p; v.tb_pd = e->tup_pd.p; v.n_tuples = e->tup_n; v.d2book = e->tup_d2.p; v.codebook = e->tup_book;
+	} else if (o->source == APO_SRC_ROLLOUTS) {
+		if (e->roll.p == nullptr || e->roll_C == 0) return fail(e, APO_E_STATE, "no rollouts loaded");
+		v.form = e->roll_row == 32 ? apo::CAND_REC32 : apo::CAND_REC16; v.C = e->roll_C; v.count = e->roll_T; v.pitch_evals = e->roll_pitch;
+		v.rows = e->roll.p;
+	} else {
+		if ((e->dims_ptr == nullptr && !e->compact) || e->dims_C == 0) return fail(e, APO_E_STATE, "no dims loaded");
+		v.C = e->dims_C; v.count = e->dims_T; v.pitch_evals = e->dims_pitch;
+		if (e->compact) {
+			v.form = apo::CAND_Q; v.q8 = e->q8.p; v.d2 = e->qd2.p; v.li = e->qli.p;
+			if ((v.variant == 0 || v.variant >= 5) && !e->q_pair_ok) v.variant = 4;   // prefix table would not fit: product tables only
+		} else {
+			v.rows = (const uint8_t *)e->dims_ptr;
 		}
-		int qvariant = (int)o->variant;
-		if ((qvariant == 0 || qvariant >= 5) && !e->q_pair_ok) qvariant = 4;   // prefix table would not fit: product tables only
-		if (fused) { Q.corpus_on = 1; Q.corpus = *fused; }
-		if ((rc = record_k1_event(e, 0))) return rc;
-		CK(apo::run_reward9q(Q, qvariant, (o->flags & APO_SCORE_RECIP) != 0, e->sm_count, e->stream));
-		if ((rc = record_k1_event(e, 1))) return rc;
-		e->timing.launches++;
-		return APO_OK;
 	}
-	apo::K1Params P{};
-	const int row = raw ? (int)e->roll_row : 36;
-	const uint64_t pitch = raw ? e->roll_pitch : e->dims_pitch;
-	P.base = (raw ? (const uint8_t *)e->roll.p : (const uint8_t *)e->dims_ptr) + first * row;
-	P.pitch_bytes = pitch * row;
-	P.C = C; P.T = count; P.acc = e->acc.p + (uint64_t)ACC_PER_CAND * cand_offset;
-	P.lut = e->d_lut.p;
-	P.W = e->W;
-	if (fused) { P.corpus_on = 1; P.corpus = *fused; }
-	if (!count) return APO_OK;
+	return APO_OK;
+}
+
+// ev narrowed to o's window, which check_window has placed inside it
+int resident_window(apo_engine *e, const apo_score_opts *o, Evals *ev) {
+	const uint64_t first = o->first;
+	ev->count = o->count ? o->count : ev->count - first;
+	if (ev->count && first % 8 && ev->form == apo::CAND_T) return fail(e, APO_E_ARG, "window start must be a multiple of 8 for Form T");
+	if (ev->count && first % 8 && ev->form == apo::CAND_Q) return fail(e, APO_E_ARG, "window start must be a multiple of 8 for the compact layout");
+	ev->idx_base = first;
+	if (ev->rows) ev->rows += first * ev->row();
+	if (ev->q8) { ev->q8 += first; ev->d2 += first; ev->li += first; }
+	if (ev->tl) { ev->tl += first; ev->th += first; }
+	return APO_OK;
+}
+
+// one scoring launch (K1 / K1q / K1t) over ev into candidates [cand_offset, ...); fused: the corpus scan and the tail ride on it
+int launch_score(apo_engine *e, const apo_score_opts *o, const Evals &ev, uint32_t cand_offset, const apo::K2Params *fused = nullptr) {
+	if (!ev.count) return APO_OK;
+	const bool recip = (o->flags & APO_SCORE_RECIP) != 0;
+	long long *acc = e->acc.p + (uint64_t)ACC_PER_CAND * cand_offset;
+	int rc;
+	if (ev.codebook && (rc = tuples_values(e, ev.codebook, ev.tb_pc, ev.tb_pd, ev.n_tuples, ev.d2book, recip))) return rc;
 	if ((rc = record_k1_event(e, 0))) return rc;
-	CK(apo::run_reward9(P, row, (int)o->variant, (o->flags & APO_SCORE_RECIP) != 0, e->sm_count, e->stream));
+	if (ev.form == apo::CAND_T) {
+		apo::KtParams P{};
+		P.tl = ev.tl; P.th = ev.th; P.pitch_evals = ev.pitch_evals; P.C = ev.C; P.T = ev.count;
+		P.acc = acc; P.tval = e->tup_val.p; P.n_tuples = ev.n_tuples; P.bad = e->tup_bad.p;
+		CK(apo::run_reward9t(P, e->sm_count, e->stream));
+	} else if (ev.form == apo::CAND_Q) {
+		apo::KqParams Q{};
+		Q.q8 = ev.q8; Q.d2 = ev.d2; Q.li = ev.li; Q.pitch_evals = ev.pitch_evals; Q.C = ev.C; Q.T = ev.count;
+		Q.acc = acc; Q.lut = e->d_lut.p; Q.ptab = e->d_ptab.p; Q.w2 = e->W.w[2];
+		Q.pair = e->d_pair.p; Q.cbf = e->d_cbf.p; Q.n0 = e->q_n0; Q.n1 = e->q_n1;
+		for (int j = 0; j < 8; j++) Q.wq[j] = e->W.w[kCodedDim[j]];
+		if (fused) { Q.corpus_on = 1; Q.corpus = *fused; }
+		CK(apo::run_reward9q(Q, ev.variant, recip, e->sm_count, e->stream));
+	} else {
+		apo::K1Params P{};
+		P.base = ev.rows; P.pitch_bytes = ev.pitch_evals * ev.row(); P.C = ev.C; P.T = ev.count; P.acc = acc;
+		P.lut = e->d_lut.p;
+		P.W = e->W;
+		if (fused) { P.corpus_on = 1; P.corpus = *fused; }
+		CK(apo::run_reward9(P, (int)ev.row(), ev.variant, recip, e->sm_count, e->stream));
+	}
 	if ((rc = record_k1_event(e, 1))) return rc;
 	e->timing.launches++;
 	return APO_OK;
@@ -611,20 +661,6 @@ int cand_arm(apo_engine *e, uint32_t C) {
 	return APO_OK;
 }
 
-apo::CandParams cand_params(apo_engine *e, uint32_t C, uint64_t T, uint64_t idx_base, uint32_t cand_offset, uint64_t pitch_evals) {
-	apo::CandParams P{};
-	P.C = C; P.T = T; P.idx_base = idx_base; P.pitch_evals = pitch_evals; P.lut = e->d_lut.p;
-	P.ints = e->cand_acc.p + (uint64_t)apo::CB_INT * cand_offset;
-	P.ex = (unsigned long long *)(e->cand_acc.p + (uint64_t)apo::CB_INT * e->score_C) + 3ull * cand_offset;
-	return P;
-}
-
-int cand_launch(apo_engine *e, const apo::CandParams &P, int source) {
-	CK(apo::run_cand_breakdown(P, source, e->sm_count, e->stream));
-	e->timing.launches++;
-	return APO_OK;
-}
-
 // Form T dictionary codebook -> [8][16] fp32 values (4-bit codes, csrc/apo_tuple.cu)
 int cand_upload_tbook(apo_engine *e, const uint32_t *codebook) {
 	uint32_t tab[8 * 16];
@@ -634,29 +670,21 @@ int cand_upload_tbook(apo_engine *e, const uint32_t *codebook) {
 	return APO_OK;
 }
 
-// breakdown of the loaded source over [first, first+count) into candidates [cand_offset, ...)
-int launch_cand_resident(apo_engine *e, const apo_score_opts *o, uint32_t cand_offset, uint64_t first, uint64_t count) {
-	if (!count) return APO_OK;
-	if (o->source == APO_SRC_TUPLES) {
-		int rc = cand_upload_tbook(e, e->tup_book);
-		if (rc) return rc;
-		apo::CandParams P = cand_params(e, e->tup_C, count, first, cand_offset, e->tup_pitch);
-		P.tl = e->tup_l.p + first; P.th = e->tup_h.p + first; P.tb_pc = e->tup_pc.p; P.tb_pd = e->tup_pd.p; P.n_tuples = e->tup_n;
-		P.tbook = e->cand_book.p; P.d2book = e->tup_d2.p;
-		return cand_launch(e, P, apo::CAND_T);
-	}
-	if (o->source == APO_SRC_ROLLOUTS) {
-		apo::CandParams P = cand_params(e, e->roll_C, count, first, cand_offset, e->roll_pitch);
-		P.rows = e->roll.p + first * e->roll_row;
-		return cand_launch(e, P, e->roll_row == 32 ? apo::CAND_REC32 : apo::CAND_REC16);
-	}
-	apo::CandParams P = cand_params(e, e->dims_C, count, first, cand_offset, e->dims_pitch);
-	if (e->compact) {
-		P.q8 = e->q8.p + first; P.d2 = e->qd2.p + first; P.li = e->qli.p + first; P.cbf = e->d_cbf.p;
-		return cand_launch(e, P, apo::CAND_Q);
-	}
-	P.rows = (const uint8_t *)(e->dims_ptr + first * APO_NDIM);
-	return cand_launch(e, P, apo::CAND_DIMS);
+// the breakdown pass over ev into candidates [cand_offset, ...)
+int launch_cand(apo_engine *e, const Evals &ev, uint32_t cand_offset) {
+	if (!ev.count) return APO_OK;
+	if (ev.codebook) { const int rc = cand_upload_tbook(e, ev.codebook); if (rc) return rc; }
+	apo::CandParams P{};
+	P.C = ev.C; P.T = ev.count; P.idx_base = ev.idx_base; P.pitch_evals = ev.pitch_evals; P.lut = e->d_lut.p;
+	P.ints = e->cand_acc.p + (uint64_t)apo::CB_INT * cand_offset;
+	P.ex = (unsigned long long *)(e->cand_acc.p + (uint64_t)apo::CB_INT * e->score_C) + 3ull * cand_offset;
+	P.rows = ev.rows; P.q8 = ev.q8; P.d2 = ev.d2; P.li = ev.li;
+	P.tl = ev.tl; P.th = ev.th; P.tb_pc = ev.tb_pc; P.tb_pd = ev.tb_pd; P.n_tuples = ev.n_tuples; P.d2book = ev.d2book;
+	if (ev.form == apo::CAND_Q) P.cbf = e->d_cbf.p;           // the tables of the codebook this call scores with (upload_ptab)
+	if (ev.form == apo::CAND_T) P.tbook = e->cand_book.p;
+	CK(apo::run_cand_breakdown(P, ev.form, e->sm_count, e->stream));
+	e->timing.launches++;
+	return APO_OK;
 }
 
 // integers -> apo_candidate_report[C]; after the scoring call has completed (its partials are final)
@@ -692,22 +720,16 @@ int ccorp_arm(apo_engine *e, uint32_t C) {
 	return APO_OK;
 }
 
-// corpus scan of C candidate rows of T records (row bytes 32 / 16) into candidates [cand_offset, ...); idx_base = position of record 0
-int ccorp_launch(apo_engine *e, const uint8_t *rows, uint32_t row, uint32_t C, uint64_t T, uint64_t pitch_evals, uint64_t idx_base,
-                 uint32_t cand_offset) {
-	if (!T) return APO_OK;
+// corpus scan of ev's trace records (Form R / R16) into candidates [cand_offset, ...)
+int launch_ccorp(apo_engine *e, const Evals &ev, uint32_t cand_offset) {
+	if (!ev.count) return APO_OK;
 	apo::CandCorpusParams P{};
-	P.C = C; P.T = T; P.idx_base = idx_base; P.pitch_evals = pitch_evals; P.rows = rows;
+	P.C = ev.C; P.T = ev.count; P.idx_base = ev.idx_base; P.pitch_evals = ev.pitch_evals; P.rows = ev.rows;
 	P.lut = e->d_lut.p; P.w2 = e->W.w[2];
 	P.blk = e->ccorp_acc.p + (uint64_t)apo::CC_WORDS * cand_offset;
-	CK(apo::run_cand_corpus(P, (int)row, e->sm_count, e->stream));
+	CK(apo::run_cand_corpus(P, (int)ev.row(), e->sm_count, e->stream));
 	e->timing.launches++;
 	return APO_OK;
-}
-
-// the resident rollouts over [first, first+count) into candidates [cand_offset, ...)
-int launch_ccorp_resident(apo_engine *e, uint32_t cand_offset, uint64_t first, uint64_t count) {
-	return ccorp_launch(e, e->roll.p + first * e->roll_row, e->roll_row, e->roll_C, count, e->roll_pitch, first, cand_offset);
 }
 
 // blocks -> apo_corpus_report[C]
@@ -740,17 +762,21 @@ apo::K2Params make_k2(apo_engine *e, uint32_t C, const apo::FinalizeParams &F) {
 	return P;
 }
 
-// fused_corpus: the scoring kernel already ran the corpus scan and the finalisation
+// The end of every scoring call: the result, then the per-candidate reports it asked for.  fused_corpus: the scoring kernel
+// already ran the corpus scan; at one rank or with the peer join its last CTA also finalised and left the accumulator block
+// zeroed (apo_score sets FinalizeParams::clean_ptr).  unpacked: Form P, whose k_unpack_p flags evaluations naming empty slots.
 int finish_score(apo_engine *e, const apo_score_opts *o, uint32_t C, double *scores, uint64_t *counts, int32_t *topk,
-                 apo_corpus_report *report, bool fused_corpus = false) {
+                 apo_corpus_report *report, bool fused_corpus = false, bool unpacked = false) {
 	const uint32_t K = o->K;
 	const bool with_corpus = wants_corpus(e, o);
 	const bool tm = e->timing_on;
 	apo::FinalizeParams F = make_fin(e, C, K, with_corpus ? 1 : 0);
 	const bool peer = F.join.nranks > 1;
-	if (!fused_corpus) { int rc = arm_corpus(e, C); if (rc) return rc; }
+	int rc;
+	if (!fused_corpus && (rc = arm_corpus(e, C))) return rc;
 	if (tm) CK(cudaEventRecord(e->ev[1], e->stream));
-	bool finalized = fused_corpus && (e->nranks == 1 || peer);
+	const bool self_clean = fused_corpus && (e->nranks == 1 || peer);
+	bool finalized = self_clean;
 	if (with_corpus && !fused_corpus) {
 		const apo::K2Params P = make_k2(e, C, F);
 		CK(apo::run_detect6(P, e->sm_count, e->stream));
@@ -778,6 +804,10 @@ int finish_score(apo_engine *e, const apo_score_opts *o, uint32_t C, double *sco
 	if (meta.status != 0)
 		return fail(e, APO_E_NCCL, "peer-memory join timed out after %.0f ms: a rank did not reach the join of call %llu", meta.join_wait_us * 1e-3,
 		            (unsigned long long)e->join_epoch);
+	if (self_clean) {
+		e->acc_clean_words = acc_words(C, e->nranks) + ARM_WORDS;
+		if (e->nranks == 1) e->partials_src = e->acc_snapshot.p;
+	}
 	if (scores) memcpy(scores, e->h_result + L.off_scores, 8ull * C);
 	if (counts) memcpy(counts, e->h_result + L.off_counts, 8ull * C);
 	if (topk && K) memcpy(topk, e->h_result + L.off_topk, 4ull * (K < C ? K : C));
@@ -798,24 +828,56 @@ int finish_score(apo_engine *e, const apo_score_opts *o, uint32_t C, double *sco
 		cudaEventElapsedTime(&ms, e->ev[3], e->ev[4]); e->timing.finalize_ms = ms;
 		cudaEventElapsedTime(&ms, e->ev[0], e->ev[4]); e->timing.total_ms = ms;
 	}
-	if (e->tup_used) return tuples_check(e);
-	return APO_OK;
+	if (e->tup_used && (rc = tuples_check(e))) return rc;
+	if (unpacked) {                                                // the stream is synchronised
+		uint32_t bad = 0;
+		CK(cudaMemcpyAsync(&bad, e->unpack_bad.p, 4, cudaMemcpyDeviceToHost, e->stream));
+		CK(cudaStreamSynchronize(e->stream));
+		if (bad) return fail(e, APO_E_ARG, "an evaluation names an empty or NaN slot of the codebook or of d2book");
+	}
+	if (wants_cand(o) && (rc = cand_finish(e, C))) return rc;
+	return wants_ccorp(o) ? ccorp_finish(e, C) : APO_OK;
 }
 
-// per-stage CUDA events cost ~1 us each on the host: record them for calls that stream enough for it not to matter, or on request
-void choose_timing(apo_engine *e, const apo_score_opts *o, uint64_t bytes) {
-	e->timing_on = (o->flags & APO_SCORE_TIMING) != 0 || bytes >= kTimingMinBytes;
-}
-
-int check_opts(apo_engine *e, const apo_score_opts *o, uint32_t C, uint64_t T, uint64_t *first, uint64_t *count) {
-	if (!o) return fail(e, APO_E_ARG, "opts is NULL");
-	if (o->K > C) return fail(e, APO_E_ARG, "K=%u exceeds the number of candidates C=%u", o->K, C);
-	if (o->K > kMaxK) return fail(e, APO_E_ARG, "K=%u exceeds the supported beam width %u", o->K, kMaxK);
+// o's window against the T evaluations loaded
+int check_window(apo_engine *e, const apo_score_opts *o, uint64_t T) {
 	if (o->first % 4) return fail(e, APO_E_ARG, "window start must be a multiple of 4");
 	if (o->first > T || (o->count && o->first + o->count > T)) return fail(e, APO_E_ARG, "window outside [0,%llu)", (unsigned long long)T);
-	*first = o->first;
-	*count = o->count ? o->count : T - o->first;
 	return APO_OK;
+}
+
+// score_check's T for the host-streaming calls (they take no window) and for apo_score_finish (each accumulate checked its own)
+constexpr uint64_t kStreamed = ~0ull, kSession = ~0ull - 1;
+
+// The refusals apo_score, apo_score_finish and the host-streaming calls share, once each has checked its source, in this
+// order: beam width, window (inside the T evaluations loaded), per-candidate passes (records: the source holds trace
+// records); then the device and the scratch of C candidates.
+int score_check(apo_engine *e, const apo_score_opts *o, uint32_t C, uint64_t T, bool records) {
+	if (o->K > C) return fail(e, APO_E_ARG, "K=%u exceeds the number of candidates C=%u", o->K, C);
+	if (o->K > kMaxK) return fail(e, APO_E_ARG, "K=%u exceeds the supported beam width %u", o->K, kMaxK);
+	int rc;
+	if (T == kStreamed) {
+		if (o->first || o->count) return fail(e, APO_E_ARG, "windows are not supported by the host-streaming calls");
+	} else if (T != kSession && (rc = check_window(e, o, T))) {
+		return rc;
+	}
+	if (wants_cand(o) && (rc = cand_check(e))) return rc;
+	if (wants_ccorp(o) && (rc = ccorp_check(e, records))) return rc;
+	CK(cudaSetDevice(e->device));
+	return T == kSession ? APO_OK : ensure_scratch(e, C, o->K);     // a session's scratch was sized by apo_score_begin
+}
+
+// The start of the launches: for a new call (begin) the timing choice over `bytes` streamed and the zeroed accumulators (whole:
+// a one-shot call's corpus block too, begin_score); then the join epoch, and the per-candidate passes armed unless an
+// accumulate of the session has armed them.
+int score_arm(apo_engine *e, const apo_score_opts *o, uint32_t C, bool begin, uint64_t bytes = 0, bool whole = false) {
+	// per-stage CUDA events cost ~1 us each on the host: record them for calls that stream enough for it not to matter, or on request
+	if (begin) e->timing_on = (o->flags & APO_SCORE_TIMING) != 0 || bytes >= kTimingMinBytes;
+	if (peer_join_active(e, C)) e->join_epoch++;          // counts joined calls only: consecutive joins alternate between the two export slots
+	int rc;
+	if (begin && (rc = begin_score(e, C, whole))) return rc;
+	if (wants_cand(o) && !e->cand_armed && (rc = cand_arm(e, C))) return rc;
+	return wants_ccorp(o) && !e->ccorp_armed ? ccorp_arm(e, C) : APO_OK;
 }
 
 }  // namespace
@@ -1311,22 +1373,6 @@ extern "C" int apo_record_unpack16(const apo_record16 *in, uint64_t n, apo_recor
 }
 
 // =============================================================================== scoring
-static int source_shape(apo_engine *e, const apo_score_opts *o, uint32_t *C, uint64_t *T) {
-	if (!o) return fail(e, APO_E_ARG, "opts is NULL");
-	if (o->source > APO_SRC_TUPLES) return fail(e, APO_E_ARG, "unknown source %u", o->source);
-	if (o->source == APO_SRC_TUPLES) {
-		if (e->tup_l.p == nullptr || e->tup_C == 0) return fail(e, APO_E_STATE, "no tuples loaded");
-		*C = e->tup_C; *T = e->tup_T;
-		return APO_OK;
-	}
-	const bool raw = o->source == APO_SRC_ROLLOUTS;
-	if (raw ? (e->roll.p == nullptr || e->roll_C == 0) : ((e->dims_ptr == nullptr && !e->compact) || e->dims_C == 0))
-		return fail(e, APO_E_STATE, "no %s loaded", raw ? "rollouts" : "dims");
-	*C = raw ? e->roll_C : e->dims_C;
-	*T = raw ? e->roll_T : e->dims_T;
-	return APO_OK;
-}
-
 extern "C" int apo_score_begin(apo_engine *e, uint32_t C_total) {
 	if (!e) return APO_E_ARG;
 	if (C_total == 0) return fail(e, APO_E_ARG, "C_total is 0");
@@ -1340,209 +1386,244 @@ extern "C" int apo_score_begin(apo_engine *e, uint32_t C_total) {
 extern "C" int apo_score_accumulate(apo_engine *e, const apo_score_opts *o, uint32_t cand_offset) {
 	if (!e) return APO_E_ARG;
 	if (!e->scoring) return fail(e, APO_E_STATE, "apo_score_begin has not been called");
-	uint32_t C = 0; uint64_t T = 0, first = 0, count = 0;
-	int rc = source_shape(e, o, &C, &T);
+	Evals ev;
+	int rc = resident_evals(e, o, &ev);
 	if (rc) return rc;
-	if ((uint64_t)cand_offset + C > e->score_C) return fail(e, APO_E_ARG, "candidates [%u,%u) exceed C_total=%u", cand_offset, cand_offset + C, e->score_C);
-	if (o->first % 4) return fail(e, APO_E_ARG, "window start must be a multiple of 4");
-	if (o->first > T || (o->count && o->first + o->count > T)) return fail(e, APO_E_ARG, "window outside [0,%llu)", (unsigned long long)T);
-	first = o->first; count = o->count ? o->count : T - o->first;
+	if ((uint64_t)cand_offset + ev.C > e->score_C) return fail(e, APO_E_ARG, "candidates [%u,%u) exceed C_total=%u", cand_offset, cand_offset + ev.C, e->score_C);
+	if ((rc = check_window(e, o, ev.count))) return rc;
 	const bool cand = wants_cand(o), ccorp = wants_ccorp(o);
 	if (cand && (rc = cand_check(e))) return rc;
-	if (ccorp && (rc = ccorp_check(e, o->source == APO_SRC_ROLLOUTS))) return rc;
+	if (ccorp && (rc = ccorp_check(e, ev.records()))) return rc;
 	CK(cudaSetDevice(e->device));
-	if ((rc = launch_k1_resident(e, o, cand_offset, first, count))) return rc;
+	if ((rc = resident_window(e, o, &ev)) || (rc = launch_score(e, o, ev, cand_offset))) return rc;
 	if (!ccorp) e->ccorp_every = false;
 	else if (e->ccorp_every) {                          // an earlier accumulate of the session did not set the flag: finish refuses
 		if (!e->ccorp_armed && (rc = ccorp_arm(e, e->score_C))) return rc;
-		if ((rc = launch_ccorp_resident(e, cand_offset, first, count))) return rc;
+		if ((rc = launch_ccorp(e, ev, cand_offset))) return rc;
 	}
 	if (!cand) { e->cand_every = false; return APO_OK; }
 	if (!e->cand_every) return APO_OK;                  // an earlier accumulate of the session did not set the flag: finish refuses
 	if (!e->cand_armed && (rc = cand_arm(e, e->score_C))) return rc;
-	return launch_cand_resident(e, o, cand_offset, first, count);
+	return launch_cand(e, ev, cand_offset);
 }
 
 extern "C" int apo_score_finish(apo_engine *e, const apo_score_opts *o, double *scores, uint64_t *counts, int32_t *topk,
                                 apo_corpus_report *report) {
 	if (!e) return APO_E_ARG;
-	e->cand_ready = false;                              // a failed finish leaves no breakdown behind either
-	e->ccorp_ready = false;
+	e->cand_ready = e->ccorp_ready = false;             // a failed finish leaves no breakdown behind either
 	if (!o) return fail(e, APO_E_ARG, "opts is NULL");
 	if (!e->scoring) return fail(e, APO_E_STATE, "apo_score_begin has not been called");
-	if (o->K > e->score_C) return fail(e, APO_E_ARG, "K=%u exceeds the number of candidates C=%u", o->K, e->score_C);
-	if (o->K > kMaxK) return fail(e, APO_E_ARG, "K=%u exceeds the supported beam width %u", o->K, kMaxK);
-	const bool cand = wants_cand(o), ccorp = wants_ccorp(o);
-	int rc;
-	if (cand) {
-		if ((rc = cand_check(e))) return rc;
-		if (!e->cand_every)
-			return fail(e, APO_E_STATE, "APO_SCORE_CANDIDATES: every apo_score_accumulate of the session must set the flag for a breakdown");
-	}
-	if (ccorp) {
-		if ((rc = ccorp_check(e, true))) return rc;     // the accumulate calls refused every other source
-		if (!e->ccorp_every)
-			return fail(e, APO_E_STATE, "APO_SCORE_CANDIDATE_CORPUS: every apo_score_accumulate of the session must set the flag for the reports");
-	}
-	CK(cudaSetDevice(e->device));
-	if (cand && !e->cand_armed && (rc = cand_arm(e, e->score_C))) return rc;   // nothing accumulated yet: an empty breakdown
-	if (ccorp && !e->ccorp_armed && (rc = ccorp_arm(e, e->score_C))) return rc;
-	if (peer_join_active(e, e->score_C)) e->join_epoch++;
-	if ((rc = finish_score(e, o, e->score_C, scores, counts, topk, report))) return rc;
-	if (cand && (rc = cand_finish(e, e->score_C))) return rc;
-	return ccorp ? ccorp_finish(e, e->score_C) : APO_OK;
+	int rc = score_check(e, o, e->score_C, kSession, true);      // the accumulate calls refused every other source
+	if (rc) return rc;
+	if (wants_cand(o) && !e->cand_every)
+		return fail(e, APO_E_STATE, "APO_SCORE_CANDIDATES: every apo_score_accumulate of the session must set the flag for a breakdown");
+	if (wants_ccorp(o) && !e->ccorp_every)
+		return fail(e, APO_E_STATE, "APO_SCORE_CANDIDATE_CORPUS: every apo_score_accumulate of the session must set the flag for the reports");
+	if ((rc = score_arm(e, o, e->score_C, false))) return rc;   // nothing accumulated yet: an empty breakdown
+	return finish_score(e, o, e->score_C, scores, counts, topk, report);
 }
 
 extern "C" int apo_score(apo_engine *e, const apo_score_opts *o, double *scores, uint64_t *counts, int32_t *topk, apo_corpus_report *report) {
 	if (!e) return APO_E_ARG;
-	e->cand_ready = false;                              // a failed call leaves no breakdown behind either
-	e->ccorp_ready = false;
-	uint32_t C = 0; uint64_t T = 0, first = 0, count = 0;
-	int rc = source_shape(e, o, &C, &T);
+	e->cand_ready = e->ccorp_ready = false;             // a failed call leaves no breakdown behind either
+	Evals ev;
+	int rc = resident_evals(e, o, &ev);
 	if (rc) return rc;
-	if ((rc = check_opts(e, o, C, T, &first, &count))) return rc;
-	const bool cand = wants_cand(o), ccorp = wants_ccorp(o);
-	if (cand && (rc = cand_check(e))) return rc;
-	if (ccorp && (rc = ccorp_check(e, o->source == APO_SRC_ROLLOUTS))) return rc;
-	CK(cudaSetDevice(e->device));
-	if ((rc = ensure_scratch(e, C, o->K))) return rc;
-	const bool tup = o->source == APO_SRC_TUPLES;      // gather-and-add kernel: stand-alone corpus scan + tail
-	const double row_bytes = tup ? 3.0 : o->source == APO_SRC_ROLLOUTS ? (double)e->roll_row : (e->compact ? 14.0 : 36.0);
-	const double stream_bytes = (double)C * (double)count * row_bytes;
-	choose_timing(e, o, (uint64_t)stream_bytes);
-	if (peer_join_active(e, C)) e->join_epoch++;          // counts joined calls only: consecutive joins alternate between the two export slots
+	const uint32_t C = ev.C;
+	if ((rc = score_check(e, o, C, ev.count, ev.records())) || (rc = resident_window(e, o, &ev))) return rc;
+	const bool tup = ev.form == apo::CAND_T;            // gather-and-add kernel: stand-alone corpus scan + tail
+	const double stream_bytes = (double)C * (double)ev.count * ev.bytes();
 	// One launch per call: the corpus scan (K2) rides on an extra warp of every scoring CTA and the last CTA finalises (K3,
 	// after the peer-memory join when the record axis is sharded) ... when the scan can hide behind the evaluation stream.
 	// Both rates are derived from the device at apo_create.
-	const double k1_ms = stream_bytes / (o->source == APO_SRC_DIMS && e->compact ? e->stream_q_bytes_per_ms : e->stream_bytes_per_ms);
+	const double k1_ms = stream_bytes / (ev.form == apo::CAND_Q ? e->stream_q_bytes_per_ms : e->stream_bytes_per_ms);
 	const double scan_ms = (double)e->corpus_T * e->scan_ms_per_record;
 	const bool one_launch = e->nranks == 1 || peer_join_active(e, C);
 	// ... or when it is tiny anyway (the IDE's real corpora, <= 1000 traces): at most 16 records per lane of the corpus warps,
 	// a few microseconds, against a second launch
-	const int tile_evals = tup ? apo::kt_tile_evals() : (o->source == APO_SRC_DIMS && e->compact) ? apo::kq_tile_evals((int)o->variant) : apo::k1_tile_evals((int)row_bytes, (int)o->variant);
-	const uint64_t tiles = (uint64_t)C * ((count + (uint64_t)tile_evals - 1) / (uint64_t)tile_evals);
+	const uint64_t tiles = (uint64_t)C * ((ev.count + ev.tile() - 1) / ev.tile());
 	const uint64_t ctas = tiles < (uint64_t)e->sm_count ? tiles : (uint64_t)e->sm_count;
 	const bool small_scan = e->corpus_T <= 16ull * 32ull * ctas;
-	const bool fuse = !tup && wants_corpus(e, o) && count > 0 && !e->env_no_fuse && (k1_ms > 1.3 * scan_ms || small_scan || e->env_force_fuse);
+	const bool fuse = !tup && wants_corpus(e, o) && ev.count > 0 && !e->env_no_fuse && (k1_ms > 1.3 * scan_ms || small_scan || e->env_force_fuse);
 	// without a corpus request the same tail still saves the K3 launch: an empty scan, then the last CTA finalises
-	const bool tail_only = !tup && !wants_corpus(e, o) && one_launch && count > 0 && !e->env_no_fuse;
-	if (fuse || tail_only) {
-		if ((rc = begin_score(e, C, true))) return rc;
-		if (cand && (rc = cand_arm(e, C))) return rc;
-		if (ccorp && (rc = ccorp_arm(e, C))) return rc;
+	const bool tail_only = !tup && !wants_corpus(e, o) && one_launch && ev.count > 0 && !e->env_no_fuse;
+	const bool fused = fuse || tail_only;
+	if ((rc = score_arm(e, o, C, true, (uint64_t)stream_bytes, fused))) return rc;
+	apo::K2Params k2{};
+	if (fused) {
 		apo::FinalizeParams F = make_fin(e, C, o->K, fuse ? 1 : 0);
-		const bool self_clean = one_launch;          // the finalising CTA is in this launch: it can leave the block zeroed
-		if (self_clean) { F.clean_ptr = e->acc.p; F.clean_words = (uint32_t)(acc_words(C, e->nranks) + ARM_WORDS); F.snapshot = e->acc_snapshot.p; }
-		apo::K2Params k2 = make_k2(e, C, F);
+		// the finalising CTA is in this launch: it can leave the block zeroed (finish_score records that it did)
+		if (one_launch) { F.clean_ptr = e->acc.p; F.clean_words = (uint32_t)(acc_words(C, e->nranks) + ARM_WORDS); F.snapshot = e->acc_snapshot.p; }
+		k2 = make_k2(e, C, F);
 		if (tail_only) { k2.T = 0; k2.recs = nullptr; }
-		if ((rc = launch_k1_resident(e, o, 0, first, count, &k2))) return rc;
-		if (cand && (rc = launch_cand_resident(e, o, 0, first, count))) return rc;
-		if (ccorp && (rc = launch_ccorp_resident(e, 0, first, count))) return rc;
-		rc = finish_score(e, o, C, scores, counts, topk, report, true);
-		if (rc == APO_OK && self_clean) {
-			e->acc_clean_words = F.clean_words;
-			if (e->nranks == 1) e->partials_src = e->acc_snapshot.p;
-		}
-		if (rc == APO_OK && cand) rc = cand_finish(e, C);
-		if (rc == APO_OK && ccorp) rc = ccorp_finish(e, C);
-		return rc;
-	} else {
-		if ((rc = begin_score(e, C))) return rc;
-		if (cand && (rc = cand_arm(e, C))) return rc;
-		if (ccorp && (rc = ccorp_arm(e, C))) return rc;
-		if ((rc = launch_k1_resident(e, o, 0, first, count))) return rc;
-		if (cand && (rc = launch_cand_resident(e, o, 0, first, count))) return rc;
-		if (ccorp && (rc = launch_ccorp_resident(e, 0, first, count))) return rc;
 	}
-	if ((rc = finish_score(e, o, C, scores, counts, topk, report, fuse || tail_only))) return rc;
-	if (cand && (rc = cand_finish(e, C))) return rc;
-	return ccorp ? ccorp_finish(e, C) : APO_OK;
+	if ((rc = launch_score(e, o, ev, 0, fused ? &k2 : nullptr))) return rc;
+	if (wants_cand(o) && (rc = launch_cand(e, ev, 0))) return rc;
+	if (wants_ccorp(o) && (rc = launch_ccorp(e, ev, 0))) return rc;
+	return finish_score(e, o, C, scores, counts, topk, report, fused);
 }
 
 namespace {
-// Streams host rows [C][T] (row bytes 36 = Form D, 32 = Form R, 16 = Form R16) through two device
-// windows: the H2D copy of chunk i+1 (copy stream) overlaps K1 on chunk i (compute stream).
-int score_host_rows_impl(apo_engine *e, const apo_score_opts *o, const uint8_t *rows, uint32_t row, uint32_t C, uint64_t T,
-                         double *scores, uint64_t *counts, int32_t *topk, apo_corpus_report *report) {
-	if (!e) return APO_E_ARG;
-	e->cand_ready = false;
-	e->ccorp_ready = false;
+int tuples_args(apo_engine *e, const uint16_t *tl, const uint8_t *th, const uint32_t *tb_pc, const uint16_t *tb_pd, uint32_t n,
+                const uint32_t *codebook, const uint32_t *d2book, uint32_t C, uint64_t T) {
+	if (C == 0) return fail(e, APO_E_ARG, "C == 0");
+	if (!codebook || !d2book || (n && (!tb_pc || !tb_pd)) || (T && (!tl || !th))) return fail(e, APO_E_ARG, "input is NULL");
+	if (n > APO_TUPLES_MAX) return fail(e, APO_E_ARG, "n_tuples=%u exceeds %u", n, APO_TUPLES_MAX);
+	if (T && n == 0) return fail(e, APO_E_ARG, "evaluations without a dictionary");
+	return APO_OK;
+}
+
+// A tensor [C][T] in the caller's memory for the host-streaming calls: the planes of one layout, each [C][T] at `bytes` per
+// evaluation.  D / R / R16: the rows; Q: q8, d2, li; P: pc, pd; T: tl, th.
+struct HostTensor {
+	Form form;                                   // what the scoring kernel reads (Form P: Form Q, which k_unpack_p expands it into)
+	uint32_t C;
+	uint64_t T;
+	struct { const void *p; uint32_t bytes; } plane[3];
+	int planes;
+	bool packed = false;                         // Form P
+	const uint32_t *codebook = nullptr;          // Form Q / P / T
+	const uint32_t *d2book = nullptr;            // Form P / T
+	const uint32_t *tb_pc = nullptr;             // Form T: the dictionary
+	const uint16_t *tb_pd = nullptr;
+	uint32_t n_tuples = 0;
+};
+
+// Streams a host tensor through two device windows of ~256 MB: the H2D copy of chunk i+1 (copy stream) overlaps the scoring
+// kernel and the per-candidate passes on chunk i (compute stream).  A window holds the planes one after the other, [C][Tc] each.
+int stream_host(apo_engine *e, const apo_score_opts *o, const HostTensor &h, double *scores, uint64_t *counts, int32_t *topk,
+                apo_corpus_report *report) {
+	const uint32_t C = h.C;
+	const uint64_t T = h.T;
+	e->cand_ready = e->ccorp_ready = false;
 	if (!o) return fail(e, APO_E_ARG, "opts is NULL");
-	if (!rows || C == 0) return fail(e, APO_E_ARG, "input is NULL or C == 0");
-	if (o->K > C) return fail(e, APO_E_ARG, "K=%u exceeds the number of candidates C=%u", o->K, C);
-	if (o->K > kMaxK) return fail(e, APO_E_ARG, "K=%u exceeds the supported beam width %u", o->K, kMaxK);
-	if (o->first || o->count) return fail(e, APO_E_ARG, "windows are not supported by the host-streaming calls");
-	const bool cand = wants_cand(o), ccorp = wants_ccorp(o);
+	const bool rows = h.form != apo::CAND_Q && h.form != apo::CAND_T;
+	if (!rows && wants_ccorp(o)) return ccorp_check(e, false);   // the wire formats refuse it before they look at their inputs
 	int rc;
-	if (cand && (rc = cand_check(e))) return rc;
-	if (ccorp && (rc = ccorp_check(e, row != 36))) return rc;
-	CK(cudaSetDevice(e->device));
-	if ((rc = ensure_scratch(e, C, o->K))) return rc;
-	// window of ~256 MB per buffer, a multiple of the K1 tile so chunks never split a tile
-	const int tile = apo::k1_tile_evals((int)row, (int)o->variant);
-	uint64_t Tc = (256ull << 20) / ((uint64_t)C * row);
+	if (h.form == apo::CAND_T) {
+		if ((rc = tuples_args(e, (const uint16_t *)h.plane[0].p, (const uint8_t *)h.plane[1].p, h.tb_pc, h.tb_pd, h.n_tuples, h.codebook,
+		                      h.d2book, C, T)))
+			return rc;
+	} else {
+		bool missing = C == 0 || (h.form == apo::CAND_Q && !h.codebook) || (h.packed && !h.d2book);
+		for (int k = 0; k < h.planes; k++) missing |= h.plane[k].p == nullptr;
+		if (missing) return fail(e, APO_E_ARG, "input is NULL or C == 0");
+	}
+	Evals ev;
+	ev.form = h.form; ev.C = C; ev.variant = (int)o->variant;
+	if ((rc = score_check(e, o, C, kStreamed, ev.records()))) return rc;
+	// Form Q / P: the lookup tables of K1q follow the codebook of THIS call; a resident Form Q tensor keeps its own and gets it
+	// back when the call returns, on every path (Restore)
+	struct Restore {
+		apo_engine *e; uint32_t saved[8 * 256]; bool armed = false;
+		~Restore() { if (armed) { memcpy(e->qbook_host, saved, sizeof saved); upload_ptab(e); } }
+	} restore{e};
+	if (h.form == apo::CAND_Q) {
+		const bool same_book = memcmp(e->qbook_host, h.codebook, sizeof e->qbook_host) == 0 && e->d_ptab.p != nullptr;
+		if (!same_book) {
+			if (e->compact) { memcpy(restore.saved, e->qbook_host, sizeof restore.saved); restore.armed = true; }
+			memcpy(e->qbook_host, h.codebook, sizeof e->qbook_host);
+			if ((rc = upload_ptab(e))) return rc;
+		}
+		ev.variant = e->q_pair_ok ? 0 : 4;
+	}
+	uint64_t wire = 0;                                             // bytes per evaluation over PCIe
+	for (int k = 0; k < h.planes; k++) wire += h.plane[k].bytes;
+	const uint64_t dev = h.packed ? 14 + wire : wire;             // per window evaluation: Form P also holds the Form Q planes
+	// window of ~256 MB per buffer, a multiple of the scoring kernel's tile so chunks never split a tile
+	const uint64_t tile = ev.tile();
+	uint64_t Tc = (256ull << 20) / ((uint64_t)C * wire);
 	Tc = Tc / tile * tile;
-	if (Tc < (uint64_t)tile) Tc = tile;
+	if (Tc < tile) Tc = tile;
 	if (Tc > round_up(T ? T : 1, tile)) Tc = round_up(T ? T : 1, tile);
-	for (int i = 0; i < 2; i++) CK(e->win[i].reserve((uint64_t)C * Tc * row));
-	// pageable callers (malloc / ArrayBuffer / numpy): the driver would stage such copies through one small internal
-	// buffer on the calling thread; instead gather each chunk into pinned memory with a few host threads while the
+	for (int i = 0; i < 2; i++) CK(e->win[i].reserve((uint64_t)C * Tc * dev));
+	// pageable callers (malloc / ArrayBuffer / numpy) of the row formats: the driver would stage such copies through one small
+	// internal buffer on the calling thread; instead gather each chunk into pinned memory with a few host threads while the
 	// previous chunk is on the wire.  Pinned or registered callers (apo_host_alloc) are read in place.
-	const bool staged = T > 0 && is_pageable(rows) && !e->env_no_staging;
-	if (staged && (rc = ensure_stage(e, (uint64_t)C * Tc * row))) return rc;
-	choose_timing(e, o, (uint64_t)C * T * row);
-	if (peer_join_active(e, C)) e->join_epoch++;
-	if ((rc = begin_score(e, C))) return rc;
-	if (cand && (rc = cand_arm(e, C))) return rc;
-	if (ccorp && (rc = ccorp_arm(e, C))) return rc;
-	const bool recip = (o->flags & APO_SCORE_RECIP) != 0;
+	const bool staged = rows && T > 0 && is_pageable(h.plane[0].p) && !e->env_no_staging;
+	if (staged && (rc = ensure_stage(e, (uint64_t)C * Tc * wire))) return rc;
+	uint64_t code_ok[2] = {0, 0};      // Form P: bit 16 j + c set when code c of coded dimension j names a value (not empty, not NaN)
+	if (h.packed) {
+		for (int j = 0; j < 8; j++)
+			for (int c = 0; c < 15; c++) {
+				const uint32_t bits = h.codebook[256 * j + c];
+				if ((bits & 0x7FFFFFFFu) <= 0x7F800000u) code_ok[j >> 2] |= 1ull << (16 * (j & 3) + c);
+			}
+		CK(e->d_d2stream.reserve(4096));
+		CK(e->unpack_bad.reserve(1));
+		CK(cudaMemcpyAsync(e->d_d2stream.p, h.d2book, 4096 * 4, cudaMemcpyHostToDevice, e->stream));   // bit patterns: empty slots are NaNs, flagged if named
+		CK(cudaMemsetAsync(e->unpack_bad.p, 0, 4, e->stream));
+	}
+	if (h.form == apo::CAND_T) {
+		CK(e->tups_pc.reserve(h.n_tuples ? h.n_tuples : 1));
+		CK(e->tups_pd.reserve(h.n_tuples ? h.n_tuples : 1));
+		CK(e->tups_d2.reserve(4096));
+	}
+	if ((rc = score_arm(e, o, C, true, (uint64_t)C * T * wire))) return rc;
+	if (h.form == apo::CAND_T) {                                   // the dictionary and its values, once for the whole call
+		if (wants_cand(o) && (rc = cand_upload_tbook(e, h.codebook))) return rc;
+		if (h.n_tuples) {
+			CK(cudaMemcpyAsync(e->tups_pc.p, h.tb_pc, (uint64_t)h.n_tuples * 4, cudaMemcpyHostToDevice, e->stream));
+			CK(cudaMemcpyAsync(e->tups_pd.p, h.tb_pd, (uint64_t)h.n_tuples * 2, cudaMemcpyHostToDevice, e->stream));
+		}
+		CK(cudaMemcpyAsync(e->tups_d2.p, h.d2book, 4096 * 4, cudaMemcpyHostToDevice, e->stream));   // bit patterns: unused slots are NaNs, flagged if an entry names one
+		ev.tb_pc = e->tups_pc.p; ev.tb_pd = e->tups_pd.p; ev.n_tuples = h.n_tuples; ev.d2book = e->tups_d2.p;
+		if ((rc = tuples_values(e, h.codebook, ev.tb_pc, ev.tb_pd, ev.n_tuples, ev.d2book, (o->flags & APO_SCORE_RECIP) != 0))) return rc;
+	}
+	const uint64_t CTc = (uint64_t)C * Tc;
+	ev.pitch_evals = Tc;
 	int nchunk = 0;
 	for (uint64_t t0 = 0; t0 < T; t0 += Tc, nchunk++) {
 		const int b = nchunk & 1;
 		const uint64_t n = T - t0 < Tc ? T - t0 : Tc;
-		const uint8_t *src = rows + t0 * row;
-		size_t spitch = T * row;
-		if (staged) {
-			if (nchunk >= 2) CK(cudaEventSynchronize(e->stage_done[b]));      // the copy that read this staging buffer has finished
-			parallel_rows_copy(e->h_stage[b], Tc * row, src, spitch, n * row, C);
-			src = e->h_stage[b]; spitch = Tc * row;
-		}
+		uint8_t *w = e->win[b].p;
 		if (nchunk >= 2) CK(cudaStreamWaitEvent(e->copy_stream, e->win_free[b], 0));
-		if ((rc = copy_rows_h2d(e, e->win[b].p, Tc * row, src, spitch, n * row, C, e->copy_stream))) { cudaStreamSynchronize(e->copy_stream); return rc; }
+		uint8_t *dst = w + CTc * (dev - wire);                      // Form P: behind the Form Q planes
+		for (int k = 0; k < h.planes; k++) {
+			const uint64_t pb = h.plane[k].bytes;
+			const uint8_t *src = (const uint8_t *)h.plane[k].p + t0 * pb;
+			size_t spitch = T * pb;
+			if (staged) {
+				if (nchunk >= 2) CK(cudaEventSynchronize(e->stage_done[b]));      // the copy that read this staging buffer has finished
+				parallel_rows_copy(e->h_stage[b], Tc * pb, src, spitch, n * pb, C);
+				src = e->h_stage[b]; spitch = Tc * pb;
+			}
+			if ((rc = copy_rows_h2d(e, dst, Tc * pb, src, spitch, n * pb, C, e->copy_stream))) return rc;
+			dst += CTc * pb;
+		}
 		if (staged) CK(cudaEventRecord(e->stage_done[b], e->copy_stream));
 		CK(cudaEventRecord(e->win_ready[b], e->copy_stream));
 		CK(cudaStreamWaitEvent(e->stream, e->win_ready[b], 0));
-		if (row != 36) {                                               // trace records: make sure the window carries the duration class
-			CK(apo::run_fill_durclass(e->win[b].p, row, (uint64_t)C * Tc, e->stream));
+		ev.count = n; ev.idx_base = t0;
+		if (rows) ev.rows = w;
+		if (h.form == apo::CAND_Q) { ev.q8 = (const unsigned long long *)w; ev.d2 = (const float *)(w + CTc * 8); ev.li = (const unsigned short *)(w + CTc * 12); }
+		if (h.form == apo::CAND_T) { ev.tl = (const unsigned short *)w; ev.th = w + CTc * 2; }
+		if (ev.records()) {                                            // trace records: make sure the window carries the duration class
+			CK(apo::run_fill_durclass(w, ev.row(), CTc, e->stream));
 			e->timing.launches++;
 		}
-		apo::K1Params P{};
-		P.base = e->win[b].p; P.pitch_bytes = Tc * row; P.C = C; P.T = n; P.acc = e->acc.p;
-		P.lut = e->d_lut.p; P.W = e->W;
-		if ((rc = record_k1_event(e, 0))) return rc;
-		CK(apo::run_reward9(P, (int)row, (int)o->variant, recip, e->sm_count, e->stream));
-		if ((rc = record_k1_event(e, 1))) return rc;
-		e->timing.launches++;
-		if (cand) {
-			apo::CandParams B = cand_params(e, C, n, t0, 0, Tc);
-			B.rows = e->win[b].p;
-			if ((rc = cand_launch(e, B, row == 36 ? apo::CAND_DIMS : row == 32 ? apo::CAND_REC32 : apo::CAND_REC16))) return rc;
+		if (h.packed) {
+			CK(apo::run_unpack_p((const uint32_t *)(w + CTc * 14), (const unsigned short *)(w + CTc * 18), Tc, C, n, e->d_d2stream.p, code_ok[0],
+			                     code_ok[1], e->unpack_bad.p, (unsigned long long *)w, (float *)(w + CTc * 8), (unsigned short *)(w + CTc * 12), Tc, e->stream));
+			e->timing.launches++;
 		}
-		if (ccorp && (rc = ccorp_launch(e, e->win[b].p, row, C, n, Tc, t0, 0))) return rc;   // before the window is released
+		if ((rc = launch_score(e, o, ev, 0))) return rc;
+		if (wants_cand(o) && (rc = launch_cand(e, ev, 0))) return rc;
+		if (wants_ccorp(o) && (rc = launch_ccorp(e, ev, 0))) return rc;   // before the window is released
 		CK(cudaEventRecord(e->win_free[b], e->stream));
 	}
-	if ((rc = finish_score(e, o, C, scores, counts, topk, report))) return rc;
-	if (cand && (rc = cand_finish(e, C))) return rc;
-	return ccorp ? ccorp_finish(e, C) : APO_OK;
+	return finish_score(e, o, C, scores, counts, topk, report, false, h.packed);
 }
 
-int score_host_rows(apo_engine *e, const apo_score_opts *o, const uint8_t *rows, uint32_t row, uint32_t C, uint64_t T,
-                    double *scores, uint64_t *counts, int32_t *topk, apo_corpus_report *report) {
-	const int rc = score_host_rows_impl(e, o, rows, row, C, T, scores, counts, topk, report);
-	if (rc && e) {
+int score_host(apo_engine *e, const apo_score_opts *o, const HostTensor &h, double *scores, uint64_t *counts, int32_t *topk,
+               apo_corpus_report *report) {
+	if (!e) return APO_E_ARG;
+	const int rc = stream_host(e, o, h, scores, counts, topk, report);
+	if (rc) {
 		// a failure in the middle of the chunk loop: nothing may still be reading the caller's memory when we return
 		cudaStreamSynchronize(e->copy_stream);
 		cudaStreamSynchronize(e->stream);
+		if (h.form == apo::CAND_T) e->tup_used = false;
 	}
 	return rc;
 }
@@ -1634,224 +1715,31 @@ extern "C" int apo_dims_packed_download(apo_engine *e, uint32_t *pc, uint16_t *p
 	return APO_OK;
 }
 
-namespace {
-// Streams the three Form Q planes [C][T] (8 + 4 + 2 bytes per evaluation) through two device windows, H2D of chunk i+1
-// overlapped with K1q on chunk i — the host-streaming call for callers that hold the compact wire format (14 B / evaluation
-// over PCIe instead of 36).
-// Form P (pc / pd / d2book non-NULL): 6 B per evaluation cross PCIe and k_unpack_p expands each window to Form Q on the device.
-int score_host_compact_impl(apo_engine *e, const apo_score_opts *o, const uint64_t *q8, const float *d2, const uint16_t *li,
-                            const uint32_t *pc, const uint16_t *pd, const uint32_t *d2book,
-                            const uint32_t *codebook, uint32_t C, uint64_t T, double *scores, uint64_t *counts, int32_t *topk,
-                            apo_corpus_report *report) {
-	const bool packed = pc != nullptr;
-	e->cand_ready = false;
-	e->ccorp_ready = false;
-	if (!o) return fail(e, APO_E_ARG, "opts is NULL");
-	if (wants_ccorp(o)) return ccorp_check(e, false);
-	if (!codebook || C == 0 || (packed ? (!pd || !d2book) : (!q8 || !d2 || !li))) return fail(e, APO_E_ARG, "input is NULL or C == 0");
-	if (o->K > C) return fail(e, APO_E_ARG, "K=%u exceeds the number of candidates C=%u", o->K, C);
-	if (o->K > kMaxK) return fail(e, APO_E_ARG, "K=%u exceeds the supported beam width %u", o->K, kMaxK);
-	if (o->first || o->count) return fail(e, APO_E_ARG, "windows are not supported by the host-streaming calls");
-	const bool cand = wants_cand(o);
-	int rc;
-	if (cand && (rc = cand_check(e))) return rc;
-	CK(cudaSetDevice(e->device));
-	if ((rc = ensure_scratch(e, C, o->K))) return rc;
-	// the lookup tables of K1q follow the codebook of THIS call; a resident Form Q tensor keeps its own and gets it back when the
-	// call returns, on every path (Restore)
-	struct Restore {
-		apo_engine *e; uint32_t saved[8 * 256]; bool armed = false;
-		~Restore() { if (armed) { memcpy(e->qbook_host, saved, sizeof saved); upload_ptab(e); } }
-	} restore{e};
-	const bool same_book = memcmp(e->qbook_host, codebook, sizeof e->qbook_host) == 0 && e->d_ptab.p != nullptr;
-	if (!same_book) {
-		if (e->compact) { memcpy(restore.saved, e->qbook_host, sizeof restore.saved); restore.armed = true; }
-		memcpy(e->qbook_host, codebook, sizeof e->qbook_host);
-		if ((rc = upload_ptab(e))) return rc;
-	}
-	const int qv = e->q_pair_ok ? 0 : 4;
-	const int tile = apo::kq_tile_evals(qv);
-	const uint64_t wire = packed ? 6 : 14;
-	uint64_t Tc = (256ull << 20) / ((uint64_t)C * wire);
-	Tc = Tc / tile * tile;
-	if (Tc < (uint64_t)tile) Tc = tile;
-	if (Tc > round_up(T ? T : 1, tile)) Tc = round_up(T ? T : 1, tile);
-	for (int i = 0; i < 2; i++) CK(e->win[i].reserve((uint64_t)C * Tc * (packed ? 20 : 14)));
-	uint64_t code_ok[2] = {0, 0};      // Form P: bit 16 j + c set when code c of coded dimension j names a value (not empty, not NaN)
-	if (packed) {
-		for (int j = 0; j < 8; j++)
-			for (int c = 0; c < 15; c++) {
-				const uint32_t bits = codebook[256 * j + c];
-				if ((bits & 0x7FFFFFFFu) <= 0x7F800000u) code_ok[j >> 2] |= 1ull << (16 * (j & 3) + c);
-			}
-		CK(e->d_d2stream.reserve(4096));
-		CK(e->unpack_bad.reserve(1));
-		CK(cudaMemcpyAsync(e->d_d2stream.p, d2book, 4096 * 4, cudaMemcpyHostToDevice, e->stream));   // bit patterns: empty slots are NaNs, flagged if named
-		CK(cudaMemsetAsync(e->unpack_bad.p, 0, 4, e->stream));
-	}
-	choose_timing(e, o, (uint64_t)C * T * wire);
-	if (peer_join_active(e, C)) e->join_epoch++;
-	if ((rc = begin_score(e, C))) return rc;
-	if (cand && (rc = cand_arm(e, C))) return rc;
-	int nchunk = 0;
-	for (uint64_t t0 = 0; t0 < T; t0 += Tc, nchunk++) {
-		const int b = nchunk & 1;
-		const uint64_t n = T - t0 < Tc ? T - t0 : Tc;
-		uint8_t *w = e->win[b].p;
-		unsigned long long *wq = (unsigned long long *)w;
-		float *wd = (float *)(w + (uint64_t)C * Tc * 8);
-		unsigned short *wl = (unsigned short *)(w + (uint64_t)C * Tc * 12);
-		uint32_t *wpc = (uint32_t *)(w + (uint64_t)C * Tc * 14);
-		unsigned short *wpd = (unsigned short *)(w + (uint64_t)C * Tc * 18);
-		if (nchunk >= 2) CK(cudaStreamWaitEvent(e->copy_stream, e->win_free[b], 0));
-		if (packed) {
-			if ((rc = copy_rows_h2d(e, wpc, Tc * 4, pc + t0, T * 4, n * 4, C, e->copy_stream))) return rc;
-			if ((rc = copy_rows_h2d(e, wpd, Tc * 2, pd + t0, T * 2, n * 2, C, e->copy_stream))) return rc;
-		} else {
-			if ((rc = copy_rows_h2d(e, wq, Tc * 8, q8 + t0, T * 8, n * 8, C, e->copy_stream))) return rc;
-			if ((rc = copy_rows_h2d(e, wd, Tc * 4, d2 + t0, T * 4, n * 4, C, e->copy_stream))) return rc;
-			if ((rc = copy_rows_h2d(e, wl, Tc * 2, li + t0, T * 2, n * 2, C, e->copy_stream))) return rc;
-		}
-		CK(cudaEventRecord(e->win_ready[b], e->copy_stream));
-		CK(cudaStreamWaitEvent(e->stream, e->win_ready[b], 0));
-		if (packed) {
-			CK(apo::run_unpack_p(wpc, wpd, Tc, C, n, e->d_d2stream.p, code_ok[0], code_ok[1], e->unpack_bad.p, wq, wd, wl, Tc, e->stream));
-			e->timing.launches++;
-		}
-		apo::KqParams Q{};
-		Q.q8 = wq; Q.d2 = wd; Q.li = wl; Q.pitch_evals = Tc; Q.C = C; Q.T = n;
-		Q.acc = e->acc.p; Q.lut = e->d_lut.p; Q.ptab = e->d_ptab.p; Q.w2 = e->W.w[2];
-		Q.pair = e->d_pair.p; Q.cbf = e->d_cbf.p; Q.n0 = e->q_n0; Q.n1 = e->q_n1;
-		{
-			static const int dim_of[8] = {0, 1, 3, 4, 5, 6, 7, 8};
-			for (int j = 0; j < 8; j++) Q.wq[j] = e->W.w[dim_of[j]];
-		}
-		if ((rc = record_k1_event(e, 0))) return rc;
-		CK(apo::run_reward9q(Q, qv, (o->flags & APO_SCORE_RECIP) != 0, e->sm_count, e->stream));
-		if ((rc = record_k1_event(e, 1))) return rc;
-		e->timing.launches++;
-		if (cand) {
-			apo::CandParams B = cand_params(e, C, n, t0, 0, Tc);
-			B.q8 = wq; B.d2 = wd; B.li = wl; B.cbf = e->d_cbf.p;           // the tables of this call's codebook (upload_ptab above)
-			if ((rc = cand_launch(e, B, apo::CAND_Q))) return rc;
-		}
-		CK(cudaEventRecord(e->win_free[b], e->stream));
-	}
-	if ((rc = finish_score(e, o, C, scores, counts, topk, report))) return rc;
-	if (packed) {                                                  // finish_score has synchronised the stream
-		uint32_t bad = 0;
-		CK(cudaMemcpyAsync(&bad, e->unpack_bad.p, 4, cudaMemcpyDeviceToHost, e->stream));
-		CK(cudaStreamSynchronize(e->stream));
-		if (bad) return fail(e, APO_E_ARG, "an evaluation names an empty or NaN slot of the codebook or of d2book");
-	}
-	return cand ? cand_finish(e, C) : APO_OK;
-}
-}  // namespace
-
+// Form Q planes (8 + 4 + 2 B per evaluation) for callers that hold the compact wire format: 14 B / evaluation over PCIe instead of 36
 extern "C" int apo_score_host_compact(apo_engine *e, const apo_score_opts *o, const uint64_t *q8, const float *d2, const uint16_t *li,
                                       const uint32_t *codebook, uint32_t C, uint64_t T, double *scores, uint64_t *counts,
                                       int32_t *topk, apo_corpus_report *report) {
-	if (!e) return APO_E_ARG;
-	const int rc = score_host_compact_impl(e, o, q8, d2, li, nullptr, nullptr, nullptr, codebook, C, T, scores, counts, topk, report);
-	if (rc) { cudaStreamSynchronize(e->copy_stream); cudaStreamSynchronize(e->stream); }
-	return rc;
+	HostTensor h{apo::CAND_Q, C, T, {{q8, 8}, {d2, 4}, {li, 2}}, 3};
+	h.codebook = codebook;
+	return score_host(e, o, h, scores, counts, topk, report);
 }
 
+// Form P: 6 B per evaluation cross PCIe and k_unpack_p expands each window to Form Q on the device
 extern "C" int apo_score_host_packed(apo_engine *e, const apo_score_opts *o, const uint32_t *pc, const uint16_t *pd, const uint32_t *codebook,
                                      const uint32_t *d2book, uint32_t C, uint64_t T, double *scores, uint64_t *counts, int32_t *topk,
                                      apo_corpus_report *report) {
 	if (!e) return APO_E_ARG;
 	if (!pc) return fail(e, APO_E_ARG, "input is NULL");
-	const int rc = score_host_compact_impl(e, o, nullptr, nullptr, nullptr, pc, pd, d2book, codebook, C, T, scores, counts, topk, report);
-	if (rc) { cudaStreamSynchronize(e->copy_stream); cudaStreamSynchronize(e->stream); }
-	return rc;
+	HostTensor h{apo::CAND_Q, C, T, {{pc, 4}, {pd, 2}}, 2, true, codebook, d2book};
+	return score_host(e, o, h, scores, counts, topk, report);
 }
 
 // =============================================================================== Form T (dictionary indices, 3 B / evaluation)
-namespace {
-int tuples_args(apo_engine *e, const uint16_t *tl, const uint8_t *th, const uint32_t *tb_pc, const uint16_t *tb_pd, uint32_t n,
-                const uint32_t *codebook, const uint32_t *d2book, uint32_t C, uint64_t T) {
-	if (C == 0) return fail(e, APO_E_ARG, "C == 0");
-	if (!codebook || !d2book || (n && (!tb_pc || !tb_pd)) || (T && (!tl || !th))) return fail(e, APO_E_ARG, "input is NULL");
-	if (n > APO_TUPLES_MAX) return fail(e, APO_E_ARG, "n_tuples=%u exceeds %u", n, APO_TUPLES_MAX);
-	if (T && n == 0) return fail(e, APO_E_ARG, "evaluations without a dictionary");
-	return APO_OK;
-}
-
-// Streams the two index planes [C][T] through two device windows, H2D of chunk i+1 overlapped with K1t on chunk i.
-int score_host_tuples_impl(apo_engine *e, const apo_score_opts *o, const uint16_t *tl, const uint8_t *th, const uint32_t *tb_pc,
-                           const uint16_t *tb_pd, uint32_t n_tuples, const uint32_t *codebook, const uint32_t *d2book, uint32_t C, uint64_t T,
-                           double *scores, uint64_t *counts, int32_t *topk, apo_corpus_report *report) {
-	e->cand_ready = false;
-	e->ccorp_ready = false;
-	if (!o) return fail(e, APO_E_ARG, "opts is NULL");
-	if (wants_ccorp(o)) return ccorp_check(e, false);
-	int rc;
-	if ((rc = tuples_args(e, tl, th, tb_pc, tb_pd, n_tuples, codebook, d2book, C, T))) return rc;
-	if (o->K > C) return fail(e, APO_E_ARG, "K=%u exceeds the number of candidates C=%u", o->K, C);
-	if (o->K > kMaxK) return fail(e, APO_E_ARG, "K=%u exceeds the supported beam width %u", o->K, kMaxK);
-	if (o->first || o->count) return fail(e, APO_E_ARG, "windows are not supported by the host-streaming calls");
-	const bool cand = wants_cand(o);
-	if (cand && (rc = cand_check(e))) return rc;
-	CK(cudaSetDevice(e->device));
-	if ((rc = ensure_scratch(e, C, o->K))) return rc;
-	const int tile = apo::kt_tile_evals();
-	uint64_t Tc = (256ull << 20) / ((uint64_t)C * 3);
-	Tc = Tc / tile * tile;
-	if (Tc < (uint64_t)tile) Tc = tile;
-	if (Tc > round_up(T ? T : 1, tile)) Tc = round_up(T ? T : 1, tile);
-	for (int i = 0; i < 2; i++) CK(e->win[i].reserve((uint64_t)C * Tc * 3));
-	CK(e->tups_pc.reserve(n_tuples ? n_tuples : 1));
-	CK(e->tups_pd.reserve(n_tuples ? n_tuples : 1));
-	CK(e->tups_d2.reserve(4096));
-	choose_timing(e, o, (uint64_t)C * T * 3);
-	if (peer_join_active(e, C)) e->join_epoch++;
-	if ((rc = begin_score(e, C))) return rc;
-	if (cand && ((rc = cand_arm(e, C)) || (rc = cand_upload_tbook(e, codebook)))) return rc;
-	if (n_tuples) {
-		CK(cudaMemcpyAsync(e->tups_pc.p, tb_pc, (uint64_t)n_tuples * 4, cudaMemcpyHostToDevice, e->stream));
-		CK(cudaMemcpyAsync(e->tups_pd.p, tb_pd, (uint64_t)n_tuples * 2, cudaMemcpyHostToDevice, e->stream));
-	}
-	CK(cudaMemcpyAsync(e->tups_d2.p, d2book, 4096 * 4, cudaMemcpyHostToDevice, e->stream));   // bit patterns: unused slots are NaNs, flagged if an entry names one
-	if ((rc = tuples_values(e, codebook, e->tups_pc.p, e->tups_pd.p, n_tuples, e->tups_d2.p, (o->flags & APO_SCORE_RECIP) != 0))) return rc;
-	int nchunk = 0;
-	for (uint64_t t0 = 0; t0 < T; t0 += Tc, nchunk++) {
-		const int b = nchunk & 1;
-		const uint64_t n = T - t0 < Tc ? T - t0 : Tc;
-		unsigned short *wl = (unsigned short *)e->win[b].p;
-		unsigned char *wh = e->win[b].p + (uint64_t)C * Tc * 2;
-		if (nchunk >= 2) CK(cudaStreamWaitEvent(e->copy_stream, e->win_free[b], 0));
-		if ((rc = copy_rows_h2d(e, wl, Tc * 2, tl + t0, T * 2, n * 2, C, e->copy_stream))) return rc;
-		if ((rc = copy_rows_h2d(e, wh, Tc, th + t0, T, n, C, e->copy_stream))) return rc;
-		CK(cudaEventRecord(e->win_ready[b], e->copy_stream));
-		CK(cudaStreamWaitEvent(e->stream, e->win_ready[b], 0));
-		apo::KtParams P{};
-		P.tl = wl; P.th = wh; P.pitch_evals = Tc; P.C = C; P.T = n; P.acc = e->acc.p;
-		P.tval = e->tup_val.p; P.n_tuples = n_tuples; P.bad = e->tup_bad.p;
-		if ((rc = record_k1_event(e, 0))) return rc;
-		CK(apo::run_reward9t(P, e->sm_count, e->stream));
-		if ((rc = record_k1_event(e, 1))) return rc;
-		e->timing.launches++;
-		if (cand) {
-			apo::CandParams B = cand_params(e, C, n, t0, 0, Tc);
-			B.tl = wl; B.th = wh; B.tb_pc = e->tups_pc.p; B.tb_pd = e->tups_pd.p; B.n_tuples = n_tuples;
-			B.tbook = e->cand_book.p; B.d2book = e->tups_d2.p;
-			if ((rc = cand_launch(e, B, apo::CAND_T))) return rc;
-		}
-		CK(cudaEventRecord(e->win_free[b], e->stream));
-	}
-	if ((rc = finish_score(e, o, C, scores, counts, topk, report))) return rc;
-	return cand ? cand_finish(e, C) : APO_OK;
-}
-}  // namespace
-
 extern "C" int apo_score_host_tuples(apo_engine *e, const apo_score_opts *o, const uint16_t *tl, const uint8_t *th, const uint32_t *tbook_pc,
                                      const uint16_t *tbook_pd, uint32_t n_tuples, const uint32_t *codebook, const uint32_t *d2book,
                                      uint32_t C, uint64_t T, double *scores, uint64_t *counts, int32_t *topk, apo_corpus_report *report) {
-	if (!e) return APO_E_ARG;
-	const int rc = score_host_tuples_impl(e, o, tl, th, tbook_pc, tbook_pd, n_tuples, codebook, d2book, C, T, scores, counts, topk, report);
-	if (rc) { cudaStreamSynchronize(e->copy_stream); cudaStreamSynchronize(e->stream); e->tup_used = false; }
-	return rc;
+	const HostTensor h{apo::CAND_T, C, T, {{tl, 2}, {th, 1}}, 2, false, codebook, d2book, tbook_pc, tbook_pd, n_tuples};
+	return score_host(e, o, h, scores, counts, topk, report);
 }
 
 extern "C" int apo_tuples_upload(apo_engine *e, const uint16_t *tl, const uint8_t *th, const uint32_t *tbook_pc, const uint16_t *tbook_pd,
@@ -1895,13 +1783,13 @@ extern "C" int apo_host_free(void *p) {
 
 extern "C" int apo_score_host(apo_engine *e, const apo_score_opts *o, const float *dims, uint32_t C, uint64_t T,
                               double *scores, uint64_t *counts, int32_t *topk, apo_corpus_report *report) {
-	return score_host_rows(e, o, (const uint8_t *)dims, 36, C, T, scores, counts, topk, report);
+	return score_host(e, o, {apo::CAND_DIMS, C, T, {{dims, 36}}, 1}, scores, counts, topk, report);
 }
 
 extern "C" int apo_score_host_records(apo_engine *e, const apo_score_opts *o, const void *recs, uint32_t row_bytes, uint32_t C, uint64_t T,
                                       double *scores, uint64_t *counts, int32_t *topk, apo_corpus_report *report) {
 	if (row_bytes != 32 && row_bytes != 16) return fail(e, APO_E_ARG, "row_bytes must be 32 (apo_record) or 16 (apo_record16)");
-	return score_host_rows(e, o, (const uint8_t *)recs, row_bytes, C, T, scores, counts, topk, report);
+	return score_host(e, o, {row_bytes == 32 ? apo::CAND_REC32 : apo::CAND_REC16, C, T, {{recs, row_bytes}}, 1}, scores, counts, topk, report);
 }
 
 extern "C" int apo_last_timing(const apo_engine *e, apo_timing *out) {
