@@ -178,8 +178,10 @@ int64_t apo_records_from_json(const char *json, uint64_t len, apo_record *out, u
 int apo_corpus_upload_json(apo_engine *e, const char *json, uint64_t len, uint64_t idx_base, uint64_t *n_records);
 
 /* ---- candidate x record evaluations ------------------------------------------------
- * Form D: fp32 dims[C][T][9], NaN = dimension absent, all-NaN = finalReward null.  Values are
- * expected within +-512 (the reference range is [-1,1], TCS:36): sums are exact fixed point.
+ * Form D: fp32 dims[C][T][9], NaN = dimension absent, all-NaN = finalReward null.  Domain: every
+ * evaluation's finalReward within [-512, 512) (the reference range is [-1,1], TCS:36), so that the
+ * sums are exact fixed point; a Form D / Q / P evaluation outside it (a finalReward of 512 or more,
+ * below -512, +-inf) fails the scoring call with APO_E_ARG.
  * Form R: one apo_record per (candidate, record); dims derived on device (TCS:668-763). */
 int apo_dims_upload(apo_engine *e, const float *dims, uint32_t C, uint64_t T);
 int apo_dims_generate(apo_engine *e, uint64_t seed, uint32_t c0, uint32_t C, uint64_t t0, uint64_t T,

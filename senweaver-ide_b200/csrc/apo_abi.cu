@@ -116,6 +116,9 @@ struct apo_engine {
 	DevBuf<uint8_t> result;              // scores | counts | topk | report
 	DevBuf<unsigned long long> keys, sel_key; DevBuf<int32_t> sel_idx;
 	uint8_t *h_result = nullptr; uint64_t h_result_cap = 0;
+	// page-locked, device-mapped word K1 (Form D) and K1q set when an evaluation's finalReward is outside [-512, 512): cleared
+	// when a call or session begins, read after its synchronise (no extra copy or launch per call)
+	volatile uint32_t *h_domain = nullptr;
 	DevBuf<uint8_t> win[2]; cudaEvent_t win_free[2] = {nullptr, nullptr}, win_ready[2] = {nullptr, nullptr};
 	uint8_t *h_stage[2] = {nullptr, nullptr}; uint64_t h_stage_cap = 0; cudaEvent_t stage_done[2] = {nullptr, nullptr};   // pinned staging of pageable callers
 	DevBuf<apo_record> batch_in; DevBuf<double> batch_out; DevBuf<uint32_t> batch_mask;
@@ -489,6 +492,7 @@ int begin_score(apo_engine *e, uint32_t C, bool whole = false) {
 	const uint64_t words = whole ? acc_words(C, e->nranks) + ARM_WORDS : (uint64_t)ACC_PER_CAND * C;
 	if (!(whole && e->acc_clean_words >= words)) CK(cudaMemsetAsync(e->acc.p, 0, words * 8, e->stream));
 	e->acc_clean_words = 0;                         // from here on the block is in use
+	*e->h_domain = 0u;                              // the previous call has been synchronised: no kernel writes it now
 	e->partials_src = e->nranks > 1 ? e->acc_joined.p : e->acc.p;
 	e->last_C = C; e->score_C = C; e->scoring = true; e->k1_used = 0;
 	e->cand_armed = false; e->cand_every = true; e->cand_ready = false;
@@ -628,6 +632,7 @@ int launch_score(apo_engine *e, const apo_score_opts *o, const Evals &ev, uint32
 		Q.acc = acc; Q.lut = e->d_lut.p; Q.ptab = e->d_ptab.p; Q.w2 = e->W.w[2];
 		Q.pair = e->d_pair.p; Q.cbf = e->d_cbf.p; Q.n0 = e->q_n0; Q.n1 = e->q_n1;
 		for (int j = 0; j < 8; j++) Q.wq[j] = e->W.w[kCodedDim[j]];
+		Q.bad = (uint32_t *)e->h_domain;
 		if (fused) { Q.corpus_on = 1; Q.corpus = *fused; }
 		CK(apo::run_reward9q(Q, ev.variant, recip, e->sm_count, e->stream));
 	} else {
@@ -635,6 +640,7 @@ int launch_score(apo_engine *e, const apo_score_opts *o, const Evals &ev, uint32
 		P.base = ev.rows; P.pitch_bytes = ev.pitch_evals * ev.row(); P.C = ev.C; P.T = ev.count; P.acc = acc;
 		P.lut = e->d_lut.p;
 		P.W = e->W;
+		P.bad = (uint32_t *)e->h_domain;
 		if (fused) { P.corpus_on = 1; P.corpus = *fused; }
 		CK(apo::run_reward9(P, (int)ev.row(), ev.variant, recip, e->sm_count, e->stream));
 	}
@@ -804,6 +810,8 @@ int finish_score(apo_engine *e, const apo_score_opts *o, uint32_t C, double *sco
 	if (meta.status != 0)
 		return fail(e, APO_E_NCCL, "peer-memory join timed out after %.0f ms: a rank did not reach the join of call %llu", meta.join_wait_us * 1e-3,
 		            (unsigned long long)e->join_epoch);
+	if (*e->h_domain)
+		return fail(e, APO_E_ARG, "an evaluation's finalReward is outside [-512, 512) (a dimension beyond +-512, +-inf): outside the exact fixed-point domain");
 	if (self_clean) {
 		e->acc_clean_words = acc_words(C, e->nranks) + ARM_WORDS;
 		if (e->nranks == 1) e->partials_src = e->acc_snapshot.p;
@@ -1029,6 +1037,8 @@ extern "C" int apo_create(int device, apo_engine **out) {
 		if ((c = cudaEventCreateWithFlags(&e->win_ready[i], cudaEventDisableTiming)) != cudaSuccess) return bail("cudaEventCreate", c);
 		if ((c = cudaEventCreateWithFlags(&e->stage_done[i], cudaEventDisableTiming)) != cudaSuccess) return bail("cudaEventCreate", c);
 	}
+	if ((c = cudaMallocHost((void **)&e->h_domain, sizeof(uint32_t))) != cudaSuccess) return bail("cudaMallocHost", c);
+	*e->h_domain = 0u;
 	memcpy(e->W.w, kDefaultWeights, sizeof kDefaultWeights);
 	build_luts(e);
 	if (upload_luts(e) != APO_OK) { g_create_error = e->err; apo_destroy(e); return APO_E_CUDA; }
@@ -1051,6 +1061,7 @@ extern "C" void apo_destroy(apo_engine *e) {
 	e->tup_l.release(); e->tup_h.release(); e->tup_pc.release(); e->tup_pd.release(); e->tup_bad.release(); e->tup_d2.release(); e->tup_ptab.release(); e->tup_val.release();
 	e->win[0].release(); e->win[1].release(); e->batch_in.release(); e->batch_out.release(); e->batch_mask.release();
 	if (e->h_result) cudaFreeHost(e->h_result);
+	if (e->h_domain) cudaFreeHost((void *)e->h_domain);
 	for (auto &ev : e->ev) if (ev) cudaEventDestroy(ev);
 	for (auto &ev : e->k1_ev) cudaEventDestroy(ev);
 	for (int i = 0; i < 2; i++) { if (e->win_free[i]) cudaEventDestroy(e->win_free[i]); if (e->win_ready[i]) cudaEventDestroy(e->win_ready[i]); }

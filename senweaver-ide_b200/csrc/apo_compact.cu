@@ -409,6 +409,7 @@ k_reward9q(const KqParams P) {
 	Acc128 acc; acc.zero();
 	uint32_t cnt = 0;
 	int cur = -1;
+	uint32_t dom = 0;                                     // fx_domain_acc of every evaluation
 	const double w2 = P.w2;
 	double wq[8];
 #pragma unroll
@@ -452,10 +453,10 @@ k_reward9q(const KqParams P) {
 				long long x4 = 0;
 				if (!generic) {
 #pragma unroll
-					for (int k = 0; k < 4; k++) x4 += to_fx(div_fast<RECIP>(ws4[k], t4[k]));
+					for (int k = 0; k < 4; k++) { const long long x = to_fx(div_fast<RECIP>(ws4[k], t4[k])); fx_domain_acc(dom, x); x4 += x; }
 				} else {
 #pragma unroll
-					for (int k = 0; k < 4; k++) x4 += to_fx(div_lut<RECIP>(ws4[k], t4[k]));
+					for (int k = 0; k < 4; k++) { const long long x = to_fx(div_lut<RECIP>(ws4[k], t4[k])); fx_domain_acc(dom, x); x4 += x; }
 				}
 				acc.add(x4);
 			}
@@ -465,7 +466,9 @@ k_reward9q(const KqParams P) {
 				if (e < n) {
 					double ws; double2 t; uint32_t ok;
 					evalq(sq[e], sd[e], sl[e], ws, t, ok);
-					acc.add(to_fx(div_lut<RECIP>(ws, t)));
+					const long long x = to_fx(div_lut<RECIP>(ws, t));
+					fx_domain_acc(dom, x);
+					acc.add(x);
 					cnt += ok;
 				}
 			}
@@ -474,6 +477,7 @@ k_reward9q(const KqParams P) {
 		if (lane == 0) mbar_arrive(&empty[s]);
 	}
 	if (cur >= 0) flush(cur);
+	if (fx_out_of_domain(dom)) *P.bad = 1u;               // read by the host after the call's synchronise
 	}
 	if (P.corpus_on) corpus_tail(P.corpus, s_ex, s_last, reinterpret_cast<unsigned long long *>(smem), 2048u);     // block-wide; stage 0 is free: scratch
 }

@@ -160,6 +160,7 @@ k_reward9(const K1Params P) {
 	Acc128 acc; acc.zero();
 	uint32_t cnt = 0;
 	int cur = -1;
+	uint32_t dom = 0;                                     // Form D: fx_domain_acc of every evaluation
 	const Weights W = P.W;
 	auto flush = [&](int c) {
 		long long *dst = P.acc + (uint64_t)ACC_PER_CAND * c;
@@ -202,13 +203,13 @@ k_reward9(const K1Params P) {
 				// one uniform check for the (rare) flagged masks keeps the four divisions branch-free
 				const bool generic = !RECIP && ((__double2hiint(t4[0].y) | __double2hiint(t4[1].y) |
 				                                 __double2hiint(t4[2].y) | __double2hiint(t4[3].y)) < 0);
-				long long x4 = 0;                         // |fr| <= 512 -> |x| < 2^61: four terms fit int64
+				long long x4 = 0;                         // -512 <= fr < 512 -> four terms fit int64 (else flagged)
 				if (!generic) {
 #pragma unroll
-					for (int k = 0; k < 4; k++) x4 += to_fx(div_fast<RECIP>(ws4[k], t4[k]));
+					for (int k = 0; k < 4; k++) { const long long x = to_fx(div_fast<RECIP>(ws4[k], t4[k])); fx_domain_acc(dom, x); x4 += x; }
 				} else {
 #pragma unroll
-					for (int k = 0; k < 4; k++) x4 += to_fx(div_lut<RECIP>(ws4[k], t4[k]));
+					for (int k = 0; k < 4; k++) { const long long x = to_fx(div_lut<RECIP>(ws4[k], t4[k])); fx_domain_acc(dom, x); x4 += x; }
 				}
 				acc.add(x4);
 			} else if (e0 < n) {
@@ -226,6 +227,7 @@ k_reward9(const K1Params P) {
 						for (int i = 0; i < APO_NDIM; i++) v[i] = f[9 * k + i];
 						uint32_t ok;
 						const long long x = eval_dims<RECIP>(v, W, s_lut, ok);
+						fx_domain_acc(dom, x);
 						acc.add(x);
 						cnt += ok;
 					}
@@ -283,6 +285,7 @@ k_reward9(const K1Params P) {
 		if (lane == 0) mbar_arrive(&empty[s]);
 	}
 	if (cur >= 0) flush(cur);
+	if (ROW == 36 && fx_out_of_domain(dom)) *P.bad = 1u;                    // read by the host after the call's synchronise
 	}
 	// block-wide: every warp arrives here; the stage buffers are free by now (every tile was consumed) and serve as scratch
 	if (P.corpus_on) corpus_tail(P.corpus, s_ex, s_last, reinterpret_cast<unsigned long long *>(smem), 2048u);

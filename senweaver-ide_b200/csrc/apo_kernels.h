@@ -88,6 +88,7 @@ struct K1Params {
 	Weights W;
 	int corpus_on;              // run the corpus scan (K2) on one extra warp per CTA and the K2 tail in this launch
 	K2Params corpus;
+	uint32_t *bad;              // Form D: set to 1 when an evaluation's finalReward is outside [-512, 512) (fx_out_of_domain)
 };
 
 
@@ -113,6 +114,7 @@ struct KqParams {
 	double wq[8];                   // weight of coded dimension j (push order 0,1,3..8)
 	int corpus_on;                  // as K1Params
 	K2Params corpus;
+	uint32_t *bad;                  // as K1Params
 };
 // ---- categorical product table layout (built by apo_abi.cu build_luts, read by the kernels)
 constexpr int CAT_D01 = 0;    // [fb + 3*err + 6*ended] -> fl(fl(0 + d0*w0) + d1*w1)      (12)
