@@ -138,11 +138,12 @@ int  apo_set_stream(apo_engine *e, uint64_t cuda_stream);
 /* Replace the TCS:766-776 weights (default = reference values). */
 int  apo_set_weights(apo_engine *e, const double w[APO_NDIM]);
 /* Experiment / test switches of one handle (initial value: the environment variables APO_NO_FUSE, APO_FORCE_FUSE,
- * APO_NO_STAGING, APO_JOIN_NCCL read once at apo_create).  Results are identical for every setting. */
+ * APO_NO_STAGING, APO_JOIN_NCCL, APO_NO_TWIN read once at apo_create).  Results are identical for every setting. */
 #define APO_TUNE_NO_FUSE     0x1u  /* corpus scan / finalisation as stand-alone launches                         */
 #define APO_TUNE_FORCE_FUSE  0x2u  /* corpus scan inside the scoring launch even when it cannot hide behind it   */
 #define APO_TUNE_NO_STAGING  0x4u  /* pageable host buffers straight to cudaMemcpy (no threaded pinned staging)  */
 #define APO_TUNE_NCCL_JOIN   0x8u  /* join shards with ncclAllReduce + k_finalize instead of the peer-memory join */
+#define APO_TUNE_NO_TWIN     0x10u /* no Form Q copy of a loaded Form D tensor is built or read: resident Form D runs K1 */
 int  apo_set_tuning(apo_engine *e, uint32_t flags);
 int  apo_get_weights(const apo_engine *e, double w[APO_NDIM]);
 
@@ -182,7 +183,14 @@ int apo_corpus_upload_json(apo_engine *e, const char *json, uint64_t len, uint64
  * evaluation's finalReward within [-512, 512) (the reference range is [-1,1], TCS:36), so that the
  * sums are exact fixed point; a Form D / Q / P evaluation outside it (a finalReward of 512 or more,
  * below -512, +-inf) fails the scoring call with APO_E_ARG.
- * Form R: one apo_record per (candidate, record); dims derived on device (TCS:668-763). */
+ * Form R: one apo_record per (candidate, record); dims derived on device (TCS:668-763).
+ * apo_dims_upload and apo_dims_generate also build a Form Q copy of the tensor (see below) when its evaluations are
+ * categorical and at least 4 GiB of device memory stays free beside the copy; otherwise, quietly, they keep Form D alone.
+ * Resident Form D calls with variant 0 and a window starting on a multiple of 8 then read the copy through K1q (14 B
+ * instead of 36 B per evaluation); other variants and windows read the fp32 tensor through K1.  The results are the same
+ * either way.  The fp32 tensor stays loaded (apo_dims_layout 1, apo_dims_download); the copy goes with the next load or
+ * attach, and whenever an engine allocation would otherwise fail for lack of device memory.  apo_dims_attach never
+ * builds one: the caller owns that memory and may change it. */
 int apo_dims_upload(apo_engine *e, const float *dims, uint32_t C, uint64_t T);
 int apo_dims_generate(apo_engine *e, uint64_t seed, uint32_t c0, uint32_t C, uint64_t t0, uint64_t T,
                       uint32_t agent_permille);
@@ -190,7 +198,8 @@ int apo_dims_download(apo_engine *e, float *out, uint32_t c, uint64_t first, uin
 /* Form Q — compact resident layout (csrc/apo_compact.cu): 8 one-byte codebook indices + the
  * fp32 tool_success_rate + a 2-byte presence index per evaluation (14 B instead of 36 B), lossless.  Available when every
  * dimension except d2 takes <= 255 distinct values (true for dims produced by TCS:668-763).
- * apo_dims_compact transcodes the loaded Form D in place (the fp32 copy is released);
+ * apo_dims_compact transcodes the loaded Form D in place (the fp32 copy is released; when the Form Q copy
+ * built at load is held, it becomes the tensor without a second transcode);
  * the *_compact generate/upload variants never materialise the full fp32 tensor.  When the data
  * is not categorical they return APO_E_STATE: apo_dims_compact keeps the loaded Form D usable, the
  * streaming variants leave nothing loaded.  Scores, counts, top-K and the integer partial sums are

@@ -94,11 +94,12 @@ struct apo_engine {
 
 	DevBuf<apo_record> corpus; uint64_t corpus_T = 0, corpus_base = 0;
 	DevBuf<float> dims; const float *dims_ptr = nullptr; uint32_t dims_C = 0; uint64_t dims_T = 0, dims_pitch = 0;
-	// Form Q (compact) copy of the evaluations: replaces dims/dims_ptr when `compact` is set
+	// Form Q (compact) copy of the evaluations: replaces dims/dims_ptr when `compact` is set; when `twin` is set it sits beside
+	// the engine's own fp32 tensor (built at load, a cache that is released whenever device memory runs short: see reserve)
 	DevBuf<unsigned long long> q8; DevBuf<float> qd2; DevBuf<unsigned short> qli; DevBuf<uint32_t> qbook;   // qbook: [8][256] codebook + [8] overflow flags
 	DevBuf<double> d_ptab, d_pair; DevBuf<float> stage, d_cbf, d_d2book, d_d2stream; uint32_t q_n0 = 0, q_n1 = 0; bool q_pair_ok = false;
 	DevBuf<uint32_t> unpack_bad;                              // k_unpack_p: an evaluation named an empty or NaN codebook slot
-	uint32_t qbook_host[8 * 256]; bool compact = false;
+	uint32_t qbook_host[8 * 256]; bool compact = false, twin = false;
 	uint32_t d2book_host[4096]; uint32_t d2book_n = ~0u;       // Form P export of the resident tensor (~0 = not built yet)
 	DevBuf<uint8_t> roll; uint32_t roll_C = 0, roll_row = 32; uint64_t roll_T = 0, roll_pitch = 0;   // Form R (32 B) or R16 (16 B) rows
 	// Form T (csrc/apo_tuple.cu): resident index planes + dictionary; per call: product table of its codebook, table values
@@ -128,7 +129,7 @@ struct apo_engine {
 	uint8_t *peer_block = nullptr; uint64_t peer_slot_words = 0; bool peer_ok = false;
 	void *peer_base[apo::PEER_MAX] = {nullptr}; bool peer_ipc[apo::PEER_MAX] = {false};
 	unsigned long long join_epoch = 0;
-	bool env_no_fuse = false, env_force_fuse = false, env_no_staging = false, env_nccl_join = false;   // apo_set_tuning
+	bool env_no_fuse = false, env_force_fuse = false, env_no_staging = false, env_nccl_join = false, env_no_twin = false;   // apo_set_tuning
 	double stream_bytes_per_ms = 7.4e9, stream_q_bytes_per_ms = 5.0e9, scan_ms_per_record = 3.35e-7;   // fuse heuristic, derived from the device at apo_create
 	size_t mem_pitch_max = 0;
 	uint8_t *zc_host = nullptr; uint64_t zc_cap = 0;   // zero-copy block of the single-trace path
@@ -166,6 +167,26 @@ int fail(apo_engine *e, int code, const char *fmt, ...) {
 		cudaError_t _c = (call);                                                                    \
 		if (_c != cudaSuccess) return fail(e, APO_E_CUDA, "%s: %s (%s:%d)", #call, cudaGetErrorString(_c), __FILE__, __LINE__); \
 	} while (0)
+
+void drop_twin(apo_engine *e) {
+	if (!e->twin) return;
+	e->q8.release(); e->qd2.release(); e->qli.release();
+	e->twin = false;
+}
+
+// Every engine buffer grows through here.  The Form Q copy of the fp32 tensor is a cache: an allocation that fails for lack
+// of device memory while it is held releases it and is tried once more, so holding it never fails a call that would succeed
+// without it.  Launches already queued may still read the copy: they finish first.  A resident call picks the evaluations
+// it reads (route_twin) only after its last allocation before its launches.
+template <class T>
+cudaError_t reserve(apo_engine *e, DevBuf<T> &b, uint64_t n) {
+	cudaError_t c = b.reserve(n);
+	if (c != cudaErrorMemoryAllocation || !e->twin) return c;
+	cudaGetLastError();
+	if ((c = cudaStreamSynchronize(e->stream)) != cudaSuccess) return c;
+	drop_twin(e);
+	return b.reserve(n);
+}
 
 void build_luts(apo_engine *e) {
 	for (uint32_t m = 0; m < 512; m++) {
@@ -229,7 +250,7 @@ void build_luts(apo_engine *e) {
 }
 
 int upload_luts(apo_engine *e) {
-	CK(e->d_lut.reserve(1024 + apo::CAT_WORDS));
+	CK(reserve(e, e->d_lut, 1024 + apo::CAT_WORDS));
 	CK(cudaMemcpyAsync(e->d_lut.p + 1024, e->lut_cat, apo::CAT_WORDS * 8, cudaMemcpyHostToDevice, e->stream));
 	CK(cudaMemcpyAsync(e->d_lut.p, e->lut_tw, 512 * 8, cudaMemcpyHostToDevice, e->stream));
 	CK(cudaMemcpyAsync(e->d_lut.p + 512, e->lut_rc, 512 * 8, cudaMemcpyHostToDevice, e->stream));
@@ -255,7 +276,7 @@ std::vector<double> make_ptab(const uint32_t *book, const apo::Weights &W, doubl
 
 int upload_ptab(apo_engine *e) {
 	const std::vector<double> tab = make_ptab(e->qbook_host, e->W);
-	CK(e->d_ptab.reserve(8 * 256));
+	CK(reserve(e, e->d_ptab, 8 * 256));
 	CK(cudaMemcpyAsync(e->d_ptab.p, tab.data(), 8 * 256 * 8, cudaMemcpyHostToDevice, e->stream));
 	// tables of the mixed-lookup variants: fp32 values per code, and the exact two-term prefix of dimensions 0 and 1
 	std::vector<float> cbf(8 * 256, 0.0f);
@@ -277,8 +298,8 @@ int upload_ptab(apo_engine *e) {
 				s = s + tab[256 + (b < used[1] ? b : 255)];               // + d1*w1 (TCS:781, second push)
 				pair[a * (used[1] + 1) + b] = s;
 			}
-	CK(e->d_cbf.reserve(8 * 256));
-	CK(e->d_pair.reserve(apo::KQ_PAIR_MAX));
+	CK(reserve(e, e->d_cbf, 8 * 256));
+	CK(reserve(e, e->d_pair, apo::KQ_PAIR_MAX));
 	CK(cudaMemcpyAsync(e->d_cbf.p, cbf.data(), 8 * 256 * 4, cudaMemcpyHostToDevice, e->stream));
 	CK(cudaMemcpyAsync(e->d_pair.p, pair.data(), apo::KQ_PAIR_MAX * 8, cudaMemcpyHostToDevice, e->stream));
 	CK(cudaStreamSynchronize(e->stream));
@@ -286,10 +307,10 @@ int upload_ptab(apo_engine *e) {
 }
 
 int compact_begin(apo_engine *e, uint32_t C, uint64_t pitch) {
-	CK(e->q8.reserve((uint64_t)(C ? C : 1) * pitch));
-	CK(e->qd2.reserve((uint64_t)(C ? C : 1) * pitch));
-	CK(e->qli.reserve((uint64_t)(C ? C : 1) * pitch));
-	CK(e->qbook.reserve(8 * 256 + 8));
+	CK(reserve(e, e->q8, (uint64_t)(C ? C : 1) * pitch));
+	CK(reserve(e, e->qd2, (uint64_t)(C ? C : 1) * pitch));
+	CK(reserve(e, e->qli, (uint64_t)(C ? C : 1) * pitch));
+	CK(reserve(e, e->qbook, 8 * 256 + 8));
 	CK(cudaMemsetAsync(e->qbook.p, 0xFF, 8 * 256 * 4, e->stream));
 	CK(cudaMemsetAsync(e->qbook.p + 8 * 256, 0, 8 * 4, e->stream));
 	// pad evaluations of every row: all codes 255 + NaN = finalReward null
@@ -298,14 +319,16 @@ int compact_begin(apo_engine *e, uint32_t C, uint64_t pitch) {
 	return APO_OK;
 }
 
-// returns APO_E_STATE when a coded dimension has more than 255 distinct values
-int compact_finish(apo_engine *e, uint32_t C, uint64_t T, uint64_t pitch) {
+// returns APO_E_STATE when a coded dimension has more than 255 distinct values (twin: without an error text).  twin: the planes
+// become the Form Q copy of the engine's fp32 tensor, which stays loaded; otherwise they replace it.
+int compact_finish(apo_engine *e, uint32_t C, uint64_t T, uint64_t pitch, bool twin = false) {
 	uint32_t host[8 * 256 + 8];
 	CK(cudaMemcpyAsync(host, e->qbook.p, sizeof host, cudaMemcpyDeviceToHost, e->stream));
 	CK(cudaStreamSynchronize(e->stream));
 	for (int j = 0; j < 8; j++)
 		if (host[8 * 256 + j]) {
 			e->q8.release(); e->qd2.release(); e->qli.release();
+			if (twin) return APO_E_STATE;
 			return fail(e, APO_E_STATE, "evaluations are not categorical: coded dimension %d has more than 255 distinct values; Form D is kept", j < 2 ? j : j + 1);
 		}
 	// hash-slot codes -> dense codes ordered by value (deterministic, bank-conflict-free table reads)
@@ -324,7 +347,7 @@ int compact_finish(apo_engine *e, uint32_t C, uint64_t T, uint64_t pitch) {
 		for (int c = 0; c < 256; c++) { remap[256 * j + c] = 255; dense[256 * j + c] = 0xFFFFFFFFu; }
 		for (size_t r = 0; r < used.size(); r++) { remap[256 * j + used[r].second] = (uint8_t)r; dense[256 * j + r] = host[256 * j + used[r].second]; }
 	}
-	CK(e->stage.reserve(1024));
+	CK(reserve(e, e->stage, 1024));
 	CK(cudaMemcpyAsync(e->stage.p, remap, sizeof remap, cudaMemcpyHostToDevice, e->stream));
 	CK(apo::run_recode(e->q8.p, e->qd2.p, e->qli.p, (uint64_t)C * pitch, (const uint8_t *)e->stage.p, e->stream));
 	CK(cudaMemcpyAsync(e->qbook.p, dense, sizeof dense, cudaMemcpyHostToDevice, e->stream));
@@ -332,9 +355,33 @@ int compact_finish(apo_engine *e, uint32_t C, uint64_t T, uint64_t pitch) {
 	memcpy(e->qbook_host, dense, sizeof e->qbook_host);
 	int rc = upload_ptab(e);
 	if (rc) return rc;
-	e->compact = true; e->dims_C = C; e->dims_T = T; e->dims_pitch = pitch; e->dims_ptr = nullptr;
+	if (twin) e->twin = true;
+	else { e->compact = true; e->dims_C = C; e->dims_T = T; e->dims_pitch = pitch; e->dims_ptr = nullptr; }
 	e->d2book_n = ~0u;
 	return APO_OK;
+}
+
+// After apo_dims_upload / apo_dims_generate: the Form Q copy of the engine's fp32 tensor, which resident Form D calls read
+// through K1q (route_twin) at 14 instead of 36 bytes per evaluation.  Built when the evaluations are categorical and at least
+// kTwinHeadroom of device memory stays free beside it; otherwise Form D is kept alone, without an error.
+constexpr uint64_t kTwinHeadroom = 4ull << 30;
+int build_twin(apo_engine *e) {
+	const uint32_t C = e->dims_C;
+	const uint64_t T = e->dims_T, pitch = e->dims_pitch, n = (uint64_t)C * pitch;
+	if (e->env_no_twin || C == 0 || T == 0) return APO_OK;
+	size_t free_bytes = 0, total_bytes = 0;
+	CK(cudaMemGetInfo(&free_bytes, &total_bytes));
+	if ((uint64_t)free_bytes < n * 14 + kTwinHeadroom) return APO_OK;
+	if (e->q8.reserve(n) != cudaSuccess || e->qd2.reserve(n) != cudaSuccess || e->qli.reserve(n) != cudaSuccess) {
+		cudaGetLastError();                                 // another user of the device took the room since cudaMemGetInfo
+		e->q8.release(); e->qd2.release(); e->qli.release();
+		return APO_OK;
+	}
+	int rc = compact_begin(e, C, pitch);
+	if (rc) return rc;
+	CK(apo::run_transcode(e->dims_ptr, pitch, C, T, e->q8.p, e->qd2.p, pitch, e->qbook.p, e->qbook.p + 8 * 256, e->stream));
+	rc = compact_finish(e, C, T, pitch, true);
+	return rc == APO_E_STATE ? APO_OK : rc;
 }
 
 // true when the driver does not know the pointer: ordinary pageable host memory (malloc, JS ArrayBuffer, numpy)
@@ -434,14 +481,14 @@ constexpr uint64_t ARM_WORDS = 19;                  // 18 example slots + ticket
 
 int ensure_scratch(apo_engine *e, uint32_t C, uint32_t K) {
 	if (acc_words(C, e->nranks) + ARM_WORDS > e->acc.cap) e->acc_clean_words = 0;      // a fresh allocation is not zeroed
-	CK(e->acc.reserve(acc_words(C, e->nranks) + ARM_WORDS));
-	CK(e->acc_snapshot.reserve((uint64_t)ACC_PER_CAND * (C ? C : 1)));
+	CK(reserve(e, e->acc, acc_words(C, e->nranks) + ARM_WORDS));
+	CK(reserve(e, e->acc_snapshot, (uint64_t)ACC_PER_CAND * (C ? C : 1)));
 	const ResultLayout L = result_layout(C, K);
-	CK(e->result.reserve(L.bytes));
-	CK(e->keys.reserve(C ? C : 1));
-	CK(e->sel_key.reserve(K ? K : 1));
-	CK(e->sel_idx.reserve(K ? K : 1));
-	if (e->nranks > 1) CK(e->acc_joined.reserve(acc_words(C, e->nranks)));
+	CK(reserve(e, e->result, L.bytes));
+	CK(reserve(e, e->keys, C ? C : 1));
+	CK(reserve(e, e->sel_key, K ? K : 1));
+	CK(reserve(e, e->sel_idx, K ? K : 1));
+	if (e->nranks > 1) CK(reserve(e, e->acc_joined, acc_words(C, e->nranks)));
 	if (e->h_result_cap < L.bytes) {
 		if (e->h_result) cudaFreeHost(e->h_result);
 		e->h_result = nullptr; e->h_result_cap = 0;
@@ -515,9 +562,9 @@ int record_k1_event(apo_engine *e, int which) {
 // Form T: finalReward of every dictionary entry for the current weights (device work on e->stream, no synchronisation)
 int tuples_values(apo_engine *e, const uint32_t *book_host, const uint32_t *d_pc, const unsigned short *d_pd, uint32_t n, const float *d_d2, bool recip) {
 	const std::vector<double> tab = make_ptab(book_host, e->W, std::nan(""));
-	CK(e->tup_ptab.reserve(8 * 256));
-	CK(e->tup_val.reserve((uint64_t)n + 1));
-	CK(e->tup_bad.reserve(1));
+	CK(reserve(e, e->tup_ptab, 8 * 256));
+	CK(reserve(e, e->tup_val, (uint64_t)n + 1));
+	CK(reserve(e, e->tup_bad, 1));
 	CK(cudaMemcpyAsync(e->tup_ptab.p, tab.data(), 8 * 256 * 8, cudaMemcpyHostToDevice, e->stream));   // pageable source: consumed when this returns
 	if (!e->tup_used) CK(cudaMemsetAsync(e->tup_bad.p, 0, 4, e->stream));       // a session keeps the flags of its earlier launches
 	apo::TupleValParams V{};
@@ -613,6 +660,16 @@ int resident_window(apo_engine *e, const apo_score_opts *o, Evals *ev) {
 	return APO_OK;
 }
 
+// A resident Form D call reads the Form Q copy through K1q instead when one is held, the variant is the default (1-4 name K1
+// tile shapes) and the window starts on K1q's 8-evaluation grid.  Before resident_window, after the call's last allocation
+// before its launches (reserve may release the copy).
+void route_twin(const apo_engine *e, const apo_score_opts *o, Evals *ev) {
+	if (ev->form != apo::CAND_DIMS || !e->twin || e->env_no_twin || o->variant != 0 || o->first % 8) return;
+	ev->form = apo::CAND_Q; ev->rows = nullptr;
+	ev->q8 = e->q8.p; ev->d2 = e->qd2.p; ev->li = e->qli.p;
+	ev->variant = e->q_pair_ok ? 0 : 4;                      // as resident_evals for a compact tensor
+}
+
 // one scoring launch (K1 / K1q / K1t) over ev into candidates [cand_offset, ...); fused: the corpus scan and the tail ride on it
 int launch_score(apo_engine *e, const apo_score_opts *o, const Evals &ev, uint32_t cand_offset, const apo::K2Params *fused = nullptr) {
 	if (!ev.count) return APO_OK;
@@ -661,7 +718,7 @@ int cand_check(apo_engine *e) {
 // zero the breakdown of C candidates (first flagged launch of a call or session)
 int cand_arm(apo_engine *e, uint32_t C) {
 	const uint64_t words = (uint64_t)C * (apo::CB_INT + 3);
-	CK(e->cand_acc.reserve(words));
+	CK(reserve(e, e->cand_acc, words));
 	CK(cudaMemsetAsync(e->cand_acc.p, 0, words * 8, e->stream));
 	e->cand_armed = true;
 	return APO_OK;
@@ -671,7 +728,7 @@ int cand_arm(apo_engine *e, uint32_t C) {
 int cand_upload_tbook(apo_engine *e, const uint32_t *codebook) {
 	uint32_t tab[8 * 16];
 	for (int j = 0; j < 8; j++) for (int k = 0; k < 16; k++) tab[16 * j + k] = codebook[256 * j + k];
-	CK(e->cand_book.reserve(8 * 16));
+	CK(reserve(e, e->cand_book, 8 * 16));
 	CK(cudaMemcpyAsync(e->cand_book.p, tab, sizeof tab, cudaMemcpyHostToDevice, e->stream));   // pageable source: consumed when this returns
 	return APO_OK;
 }
@@ -695,7 +752,7 @@ int launch_cand(apo_engine *e, const Evals &ev, uint32_t cand_offset) {
 
 // integers -> apo_candidate_report[C]; after the scoring call has completed (its partials are final)
 int cand_finish(apo_engine *e, uint32_t C) {
-	CK(e->cand_rep.reserve(C ? C : 1));
+	CK(reserve(e, e->cand_rep, C ? C : 1));
 	const long long *partials = e->partials_src ? e->partials_src : e->acc.p;
 	CK(apo::run_cand_report(e->cand_acc.p, (const unsigned long long *)(e->cand_acc.p + (uint64_t)apo::CB_INT * C), partials, C, e->cand_rep.p, e->stream));
 	e->timing.launches++;
@@ -720,7 +777,7 @@ int ccorp_check(apo_engine *e, bool records) {
 // zero the corpus blocks of C candidates (first flagged launch of a call or session)
 int ccorp_arm(apo_engine *e, uint32_t C) {
 	const uint64_t words = (uint64_t)C * apo::CC_WORDS;
-	CK(e->ccorp_acc.reserve(2 * words));                 // blocks | report scratch
+	CK(reserve(e, e->ccorp_acc, 2 * words));                 // blocks | report scratch
 	CK(cudaMemsetAsync(e->ccorp_acc.p, 0, words * 8, e->stream));
 	e->ccorp_armed = true;
 	return APO_OK;
@@ -740,7 +797,7 @@ int launch_ccorp(apo_engine *e, const Evals &ev, uint32_t cand_offset) {
 
 // blocks -> apo_corpus_report[C]
 int ccorp_finish(apo_engine *e, uint32_t C) {
-	CK(e->ccorp_rep.reserve(C ? C : 1));
+	CK(reserve(e, e->ccorp_rep, C ? C : 1));
 	CK(apo::run_cand_corpus_report(e->ccorp_acc.p, C, e->ccorp_rep.p, e->stream));
 	e->timing.launches++;
 	CK(cudaStreamSynchronize(e->stream));
@@ -872,7 +929,10 @@ int score_check(apo_engine *e, const apo_score_opts *o, uint32_t C, uint64_t T, 
 	if (wants_cand(o) && (rc = cand_check(e))) return rc;
 	if (wants_ccorp(o) && (rc = ccorp_check(e, records))) return rc;
 	CK(cudaSetDevice(e->device));
-	return T == kSession ? APO_OK : ensure_scratch(e, C, o->K);     // a session's scratch was sized by apo_score_begin
+	if (T == kSession) return APO_OK;                               // a session's scratch was sized by apo_score_begin
+	if ((rc = ensure_scratch(e, C, o->K))) return rc;
+	if (wants_cand(o)) CK(reserve(e, e->cand_acc, (uint64_t)C * (apo::CB_INT + 3)));   // cand_arm's, before route_twin
+	return APO_OK;
 }
 
 // The start of the launches: for a new call (begin) the timing choice over `bytes` streamed and the zeroed accumulators (whole:
@@ -1028,6 +1088,7 @@ extern "C" int apo_create(int device, apo_engine **out) {
 	e->env_force_fuse = getenv("APO_FORCE_FUSE") != nullptr;
 	e->env_no_staging = getenv("APO_NO_STAGING") != nullptr;
 	e->env_nccl_join = getenv("APO_JOIN_NCCL") != nullptr;
+	e->env_no_twin = getenv("APO_NO_TWIN") != nullptr;
 	if ((c = cudaStreamCreateWithFlags(&e->own_stream, cudaStreamNonBlocking)) != cudaSuccess) return bail("cudaStreamCreate", c);
 	if ((c = cudaStreamCreateWithFlags(&e->copy_stream, cudaStreamNonBlocking)) != cudaSuccess) return bail("cudaStreamCreate", c);
 	e->stream = e->own_stream;
@@ -1081,9 +1142,11 @@ extern "C" int apo_set_stream(apo_engine *e, uint64_t cuda_stream) {
 
 extern "C" int apo_set_tuning(apo_engine *e, uint32_t flags) {
 	if (!e) return APO_E_ARG;
-	if (flags & ~(APO_TUNE_NO_FUSE | APO_TUNE_FORCE_FUSE | APO_TUNE_NO_STAGING | APO_TUNE_NCCL_JOIN)) return fail(e, APO_E_ARG, "unknown tuning flag %#x", flags);
+	if (flags & ~(APO_TUNE_NO_FUSE | APO_TUNE_FORCE_FUSE | APO_TUNE_NO_STAGING | APO_TUNE_NCCL_JOIN | APO_TUNE_NO_TWIN))
+		return fail(e, APO_E_ARG, "unknown tuning flag %#x", flags);
 	e->env_no_fuse = (flags & APO_TUNE_NO_FUSE) != 0; e->env_force_fuse = (flags & APO_TUNE_FORCE_FUSE) != 0;
 	e->env_no_staging = (flags & APO_TUNE_NO_STAGING) != 0; e->env_nccl_join = (flags & APO_TUNE_NCCL_JOIN) != 0;
+	e->env_no_twin = (flags & APO_TUNE_NO_TWIN) != 0;
 	return APO_OK;
 }
 
@@ -1096,7 +1159,7 @@ extern "C" int apo_set_weights(apo_engine *e, const double w[APO_NDIM]) {
 	memcpy(e->W.w, w, sizeof e->W.w);
 	build_luts(e);
 	int rc = upload_luts(e);
-	if (rc == APO_OK && e->compact) rc = upload_ptab(e);
+	if (rc == APO_OK && (e->compact || e->twin)) rc = upload_ptab(e);
 	return rc;
 }
 
@@ -1130,9 +1193,9 @@ extern "C" int apo_reward_batch(apo_engine *e, const apo_record *recs, uint64_t 
 		if (finals) memcpy(finals, zfin, n * 8);
 		return APO_OK;
 	}
-	CK(e->batch_in.reserve(n));
-	CK(e->batch_out.reserve(n * (APO_NDIM + 1)));
-	CK(e->batch_mask.reserve(n));
+	CK(reserve(e, e->batch_in, n));
+	CK(reserve(e, e->batch_out, n * (APO_NDIM + 1)));
+	CK(reserve(e, e->batch_mask, n));
 	CK(cudaMemcpyAsync(e->batch_in.p, recs, n * sizeof(apo_record), cudaMemcpyHostToDevice, e->stream));
 	CK(apo::run_reward_batch(e->batch_in.p, n, e->W, e->d_lut.p, e->batch_out.p, e->batch_mask.p, e->batch_out.p + n * APO_NDIM, e->stream));
 	if (dims) CK(cudaMemcpyAsync(dims, e->batch_out.p, n * APO_NDIM * 8, cudaMemcpyDeviceToHost, e->stream));
@@ -1151,7 +1214,7 @@ extern "C" int apo_corpus_upload(apo_engine *e, const apo_record *recs, uint64_t
 	if (!e) return APO_E_ARG;
 	if (T && !recs) return fail(e, APO_E_ARG, "recs is NULL");
 	CK(cudaSetDevice(e->device));
-	CK(e->corpus.reserve(T ? T : 1));
+	CK(reserve(e, e->corpus, T ? T : 1));
 	if (T) { const int rc = h2d_rows(e, e->corpus.p, T * sizeof(apo_record), recs, T * sizeof(apo_record), T * sizeof(apo_record), 1, e->stream); if (rc) return rc; }
 	CK(apo::run_fill_durclass(e->corpus.p, 32, T, e->stream));        // resident records always carry the duration class
 	CK(cudaStreamSynchronize(e->stream));
@@ -1183,7 +1246,7 @@ extern "C" int apo_corpus_upload_json(apo_engine *e, const char *json, uint64_t 
 extern "C" int apo_corpus_generate(apo_engine *e, uint64_t seed, uint64_t t0, uint64_t T, uint32_t agent_permille) {
 	if (!e) return APO_E_ARG;
 	CK(cudaSetDevice(e->device));
-	CK(e->corpus.reserve(T ? T : 1));
+	CK(reserve(e, e->corpus, T ? T : 1));
 	CK(apo::run_gen_records(e->corpus.p, T, seed, 1u, 0, 1, t0, T, agent_permille, e->stream));
 	CK(cudaStreamSynchronize(e->stream));
 	e->corpus_T = T; e->corpus_base = t0;
@@ -1204,8 +1267,9 @@ extern "C" int apo_dims_upload(apo_engine *e, const float *dims, uint32_t C, uin
 	if (!e) return APO_E_ARG;
 	if (C && T && !dims) return fail(e, APO_E_ARG, "dims is NULL");
 	CK(cudaSetDevice(e->device));
+	drop_twin(e);
 	const uint64_t pitch = round_up(T ? T : 1, 32);
-	CK(e->dims.reserve((uint64_t)(C ? C : 1) * pitch * APO_NDIM));
+	CK(reserve(e, e->dims, (uint64_t)(C ? C : 1) * pitch * APO_NDIM));
 	if (C && T) {
 		// pad evaluations of every row are all-NaN = finalReward null
 		if (pitch != T) CK(cudaMemsetAsync(e->dims.p, 0xFF, (uint64_t)C * pitch * APO_NDIM * 4, e->stream));
@@ -1213,19 +1277,20 @@ extern "C" int apo_dims_upload(apo_engine *e, const float *dims, uint32_t C, uin
 	}
 	CK(cudaStreamSynchronize(e->stream));
 	e->dims_ptr = e->dims.p; e->dims_C = C; e->dims_T = T; e->dims_pitch = pitch; e->compact = false;
-	return APO_OK;
+	return build_twin(e);
 }
 
 extern "C" int apo_dims_generate(apo_engine *e, uint64_t seed, uint32_t c0, uint32_t C, uint64_t t0, uint64_t T, uint32_t agent_permille) {
 	if (!e) return APO_E_ARG;
 	CK(cudaSetDevice(e->device));
+	drop_twin(e);
 	const uint64_t pitch = round_up(T ? T : 1, 32);
-	CK(e->dims.reserve((uint64_t)(C ? C : 1) * pitch * APO_NDIM));
+	CK(reserve(e, e->dims, (uint64_t)(C ? C : 1) * pitch * APO_NDIM));
 	if (pitch != T && C) CK(cudaMemsetAsync(e->dims.p, 0xFF, (uint64_t)C * pitch * APO_NDIM * 4, e->stream));
 	CK(apo::run_gen_dims(e->dims.p, pitch, seed, c0, C, t0, T, agent_permille, e->stream));
 	CK(cudaStreamSynchronize(e->stream));
 	e->dims_ptr = e->dims.p; e->dims_C = C; e->dims_T = T; e->dims_pitch = pitch; e->compact = false;
-	return APO_OK;
+	return build_twin(e);
 }
 
 extern "C" int apo_dims_download(apo_engine *e, float *out, uint32_t c, uint64_t first, uint64_t n) {
@@ -1233,7 +1298,7 @@ extern "C" int apo_dims_download(apo_engine *e, float *out, uint32_t c, uint64_t
 	if ((!e->dims_ptr && !e->compact) || c >= e->dims_C || first + n > e->dims_T) return fail(e, APO_E_ARG, "range outside the evaluations");
 	CK(cudaSetDevice(e->device));
 	if (e->compact) {
-		CK(e->stage.reserve((n ? n : 1) * APO_NDIM));
+		CK(reserve(e, e->stage, (n ? n : 1) * APO_NDIM));
 		const uint64_t off = (uint64_t)c * e->dims_pitch + first;
 		CK(apo::run_decode(e->q8.p + off, e->qd2.p + off, e->qli.p + off, n, e->qbook.p, e->stage.p, e->stream));
 		CK(cudaMemcpyAsync(out, e->stage.p, n * APO_NDIM * 4, cudaMemcpyDeviceToHost, e->stream));
@@ -1249,6 +1314,7 @@ extern "C" int apo_dims_attach(apo_engine *e, uint64_t device_ptr, uint32_t C, u
 	if (!e) return APO_E_ARG;
 	if (!device_ptr || device_ptr % 16) return fail(e, APO_E_ARG, "device pointer must be non-NULL and 16-byte aligned");
 	if (pitch_evals % 4 || pitch_evals < round_up(T, 4)) return fail(e, APO_E_ARG, "pitch must be a multiple of 4 evaluations and >= T rounded up to 4");
+	drop_twin(e);                                       // never a copy of caller-owned memory: the caller may change it
 	e->dims_ptr = (const float *)(uintptr_t)device_ptr; e->dims_C = C; e->dims_T = T; e->dims_pitch = pitch_evals; e->compact = false;
 	return APO_OK;
 }
@@ -1264,6 +1330,11 @@ extern "C" int apo_dims_compact(apo_engine *e) {
 	if (e->compact) return APO_OK;
 	if (!e->dims_ptr || e->dims_C == 0) return fail(e, APO_E_STATE, "no dims loaded");
 	CK(cudaSetDevice(e->device));
+	if (e->twin) {                                      // the copy built at load already is this tensor in Form Q
+		e->twin = false; e->compact = true; e->dims_ptr = nullptr;
+		e->dims.release();
+		return APO_OK;
+	}
 	const uint32_t C = e->dims_C; const uint64_t T = e->dims_T, pitch_in = e->dims_pitch, pitch = round_up(T ? T : 1, 32);
 	int rc = compact_begin(e, C, pitch);
 	if (rc) return rc;
@@ -1279,11 +1350,12 @@ namespace {
 template <class Fill>
 int compact_stream(apo_engine *e, uint32_t C, uint64_t T, Fill fill) {
 	CK(cudaSetDevice(e->device));
+	drop_twin(e);
 	const uint64_t pitch = round_up(T ? T : 1, 32);
 	uint64_t Cc = (2ull << 30) / (pitch * 36);
 	if (Cc < 1) Cc = 1;
 	if (Cc > C) Cc = C ? C : 1;
-	CK(e->stage.reserve(Cc * pitch * APO_NDIM));
+	CK(reserve(e, e->stage, Cc * pitch * APO_NDIM));
 	int rc = compact_begin(e, C, pitch);
 	if (rc) return rc;
 	for (uint32_t c0 = 0; c0 < C; c0 += (uint32_t)Cc) {
@@ -1325,7 +1397,7 @@ int rollouts_upload_rows(apo_engine *e, const void *recs, uint32_t row, uint32_t
 	if (C && T && !recs) return fail(e, APO_E_ARG, "recs is NULL");
 	CK(cudaSetDevice(e->device));
 	const uint64_t pitch = round_up(T ? T : 1, 4);
-	CK(e->roll.reserve((uint64_t)(C ? C : 1) * pitch * row));
+	CK(reserve(e, e->roll, (uint64_t)(C ? C : 1) * pitch * row));
 	if (C && T) {
 		if (pitch != T) CK(cudaMemsetAsync(e->roll.p, 0, (uint64_t)C * pitch * row, e->stream));   // VALID clear
 		{ const int rc = h2d_rows(e, e->roll.p, pitch * row, recs, T * row, T * row, C, e->stream); if (rc) return rc; }
@@ -1339,7 +1411,7 @@ int rollouts_generate_rows(apo_engine *e, uint32_t row, uint64_t seed, uint32_t 
 	if (!e) return APO_E_ARG;
 	CK(cudaSetDevice(e->device));
 	const uint64_t pitch = round_up(T ? T : 1, 4);
-	CK(e->roll.reserve((uint64_t)(C ? C : 1) * pitch * row));
+	CK(reserve(e, e->roll, (uint64_t)(C ? C : 1) * pitch * row));
 	if (pitch != T && C) CK(cudaMemsetAsync(e->roll.p, 0, (uint64_t)C * pitch * row, e->stream));
 	if (row == 32) CK(apo::run_gen_records((apo_record *)e->roll.p, pitch, seed, 2u, c0, C, t0, T, agent_permille, e->stream));
 	else CK(apo::run_gen_records16((apo_record16 *)e->roll.p, pitch, seed, 2u, c0, C, t0, T, agent_permille, e->stream));
@@ -1406,6 +1478,8 @@ extern "C" int apo_score_accumulate(apo_engine *e, const apo_score_opts *o, uint
 	if (cand && (rc = cand_check(e))) return rc;
 	if (ccorp && (rc = ccorp_check(e, ev.records()))) return rc;
 	CK(cudaSetDevice(e->device));
+	if (cand && e->cand_every && !e->cand_armed && (rc = cand_arm(e, e->score_C))) return rc;   // allocates: before route_twin
+	route_twin(e, o, &ev);
 	if ((rc = resident_window(e, o, &ev)) || (rc = launch_score(e, o, ev, cand_offset))) return rc;
 	if (!ccorp) e->ccorp_every = false;
 	else if (e->ccorp_every) {                          // an earlier accumulate of the session did not set the flag: finish refuses
@@ -1414,7 +1488,6 @@ extern "C" int apo_score_accumulate(apo_engine *e, const apo_score_opts *o, uint
 	}
 	if (!cand) { e->cand_every = false; return APO_OK; }
 	if (!e->cand_every) return APO_OK;                  // an earlier accumulate of the session did not set the flag: finish refuses
-	if (!e->cand_armed && (rc = cand_arm(e, e->score_C))) return rc;
 	return launch_cand(e, ev, cand_offset);
 }
 
@@ -1441,7 +1514,9 @@ extern "C" int apo_score(apo_engine *e, const apo_score_opts *o, double *scores,
 	int rc = resident_evals(e, o, &ev);
 	if (rc) return rc;
 	const uint32_t C = ev.C;
-	if ((rc = score_check(e, o, C, ev.count, ev.records())) || (rc = resident_window(e, o, &ev))) return rc;
+	if ((rc = score_check(e, o, C, ev.count, ev.records()))) return rc;
+	route_twin(e, o, &ev);
+	if ((rc = resident_window(e, o, &ev))) return rc;
 	const bool tup = ev.form == apo::CAND_T;            // gather-and-add kernel: stand-alone corpus scan + tail
 	const double stream_bytes = (double)C * (double)ev.count * ev.bytes();
 	// One launch per call: the corpus scan (K2) rides on an extra warp of every scoring CTA and the last CTA finalises (K3,
@@ -1523,8 +1598,8 @@ int stream_host(apo_engine *e, const apo_score_opts *o, const HostTensor &h, dou
 	Evals ev;
 	ev.form = h.form; ev.C = C; ev.variant = (int)o->variant;
 	if ((rc = score_check(e, o, C, kStreamed, ev.records()))) return rc;
-	// Form Q / P: the lookup tables of K1q follow the codebook of THIS call; a resident Form Q tensor keeps its own and gets it
-	// back when the call returns, on every path (Restore)
+	// Form Q / P: the lookup tables of K1q follow the codebook of THIS call; a resident Form Q tensor (or the Form Q copy of a
+	// Form D one) keeps its own and gets it back when the call returns, on every path (Restore)
 	struct Restore {
 		apo_engine *e; uint32_t saved[8 * 256]; bool armed = false;
 		~Restore() { if (armed) { memcpy(e->qbook_host, saved, sizeof saved); upload_ptab(e); } }
@@ -1532,7 +1607,7 @@ int stream_host(apo_engine *e, const apo_score_opts *o, const HostTensor &h, dou
 	if (h.form == apo::CAND_Q) {
 		const bool same_book = memcmp(e->qbook_host, h.codebook, sizeof e->qbook_host) == 0 && e->d_ptab.p != nullptr;
 		if (!same_book) {
-			if (e->compact) { memcpy(restore.saved, e->qbook_host, sizeof restore.saved); restore.armed = true; }
+			if (e->compact || e->twin) { memcpy(restore.saved, e->qbook_host, sizeof restore.saved); restore.armed = true; }
 			memcpy(e->qbook_host, h.codebook, sizeof e->qbook_host);
 			if ((rc = upload_ptab(e))) return rc;
 		}
@@ -1547,7 +1622,7 @@ int stream_host(apo_engine *e, const apo_score_opts *o, const HostTensor &h, dou
 	Tc = Tc / tile * tile;
 	if (Tc < tile) Tc = tile;
 	if (Tc > round_up(T ? T : 1, tile)) Tc = round_up(T ? T : 1, tile);
-	for (int i = 0; i < 2; i++) CK(e->win[i].reserve((uint64_t)C * Tc * dev));
+	for (int i = 0; i < 2; i++) CK(reserve(e, e->win[i], (uint64_t)C * Tc * dev));
 	// pageable callers (malloc / ArrayBuffer / numpy) of the row formats: the driver would stage such copies through one small
 	// internal buffer on the calling thread; instead gather each chunk into pinned memory with a few host threads while the
 	// previous chunk is on the wire.  Pinned or registered callers (apo_host_alloc) are read in place.
@@ -1560,15 +1635,15 @@ int stream_host(apo_engine *e, const apo_score_opts *o, const HostTensor &h, dou
 				const uint32_t bits = h.codebook[256 * j + c];
 				if ((bits & 0x7FFFFFFFu) <= 0x7F800000u) code_ok[j >> 2] |= 1ull << (16 * (j & 3) + c);
 			}
-		CK(e->d_d2stream.reserve(4096));
-		CK(e->unpack_bad.reserve(1));
+		CK(reserve(e, e->d_d2stream, 4096));
+		CK(reserve(e, e->unpack_bad, 1));
 		CK(cudaMemcpyAsync(e->d_d2stream.p, h.d2book, 4096 * 4, cudaMemcpyHostToDevice, e->stream));   // bit patterns: empty slots are NaNs, flagged if named
 		CK(cudaMemsetAsync(e->unpack_bad.p, 0, 4, e->stream));
 	}
 	if (h.form == apo::CAND_T) {
-		CK(e->tups_pc.reserve(h.n_tuples ? h.n_tuples : 1));
-		CK(e->tups_pd.reserve(h.n_tuples ? h.n_tuples : 1));
-		CK(e->tups_d2.reserve(4096));
+		CK(reserve(e, e->tups_pc, h.n_tuples ? h.n_tuples : 1));
+		CK(reserve(e, e->tups_pd, h.n_tuples ? h.n_tuples : 1));
+		CK(reserve(e, e->tups_d2, 4096));
 	}
 	if ((rc = score_arm(e, o, C, true, (uint64_t)C * T * wire))) return rc;
 	if (h.form == apo::CAND_T) {                                   // the dictionary and its values, once for the whole call
@@ -1684,7 +1759,7 @@ int ensure_d2book(apo_engine *e) {
 		return x > y;
 	});
 	for (size_t c = 0; c < 4096; c++) e->d2book_host[c] = c < vals.size() ? vals[c] : 0xFFFFFFFFu;
-	CK(e->d_d2book.reserve(4096));
+	CK(reserve(e, e->d_d2book, 4096));
 	CK(cudaMemcpyAsync(e->d_d2book.p, e->d2book_host, 4096 * 4, cudaMemcpyHostToDevice, e->stream));
 	CK(cudaStreamSynchronize(e->stream));
 	e->d2book_n = (uint32_t)vals.size();
@@ -1710,7 +1785,7 @@ extern "C" int apo_dims_packed_download(apo_engine *e, uint32_t *pc, uint16_t *p
 	int rc = ensure_d2book(e);
 	if (rc) return rc;
 	if (n == 0) return APO_OK;
-	CK(e->stage.reserve((n * 6 + 3) / 4 + 16));
+	CK(reserve(e, e->stage, (n * 6 + 3) / 4 + 16));
 	uint32_t *dpc = (uint32_t *)e->stage.p;
 	unsigned short *dpd = (unsigned short *)(dpc + n);
 	uint32_t *bad = (uint32_t *)(e->stage.p + (n * 6 + 3) / 4 + 8);
@@ -1761,11 +1836,11 @@ extern "C" int apo_tuples_upload(apo_engine *e, const uint16_t *tl, const uint8_
 	CK(cudaSetDevice(e->device));
 	e->tup_C = 0; e->tup_T = 0; e->tup_n = 0;
 	const uint64_t pitch = round_up(T ? T : 1, 64);                // rows start 16-byte aligned in both planes
-	CK(e->tup_l.reserve((uint64_t)C * pitch));
-	CK(e->tup_h.reserve((uint64_t)C * pitch));
-	CK(e->tup_pc.reserve(n_tuples ? n_tuples : 1));
-	CK(e->tup_pd.reserve(n_tuples ? n_tuples : 1));
-	CK(e->tup_d2.reserve(4096));
+	CK(reserve(e, e->tup_l, (uint64_t)C * pitch));
+	CK(reserve(e, e->tup_h, (uint64_t)C * pitch));
+	CK(reserve(e, e->tup_pc, n_tuples ? n_tuples : 1));
+	CK(reserve(e, e->tup_pd, n_tuples ? n_tuples : 1));
+	CK(reserve(e, e->tup_d2, 4096));
 	if ((rc = h2d_rows(e, e->tup_l.p, pitch * 2, tl, T * 2, T * 2, C, e->stream))) { cudaStreamSynchronize(e->stream); return rc; }
 	if ((rc = h2d_rows(e, e->tup_h.p, pitch, th, T, T, C, e->stream))) { cudaStreamSynchronize(e->stream); return rc; }
 	if (n_tuples) {
@@ -1870,7 +1945,7 @@ extern "C" int apo_comm_init(apo_engine *e, int nranks, int rank, const uint8_t 
 	if (rc != 0) return fail(e, APO_E_NCCL, "ncclCommInitRank: %s", g_nccl.GetErrorString ? g_nccl.GetErrorString(rc) : "error");
 	e->comm = comm; e->nranks = nranks; e->rank = rank; e->acc_clean_words = 0; e->partials_src = nullptr;
 	// one tiny allreduce now so that the first scoring call does not pay NCCL's lazy connection setup (~1 s)
-	CK(e->misc.reserve(32));
+	CK(reserve(e, e->misc, 32));
 	CK(cudaMemsetAsync(e->misc.p + 24, 0, 8, e->stream));
 	const int wrc = g_nccl.AllReduce(e->misc.p + 24, e->misc.p + 24, 1, kNcclInt64, kNcclSum, e->comm, e->stream);
 	if (wrc != 0) return fail(e, APO_E_NCCL, "ncclAllReduce (warm-up): %s", g_nccl.GetErrorString ? g_nccl.GetErrorString(wrc) : "error");
