@@ -1,8 +1,10 @@
-"""What the Form Q copy of a resident Form D tensor buys: the configs[2] step (256 x 5 M Form D + the 5 M-record corpus, one
+"""What the compact copy of a resident Form D tensor buys: the configs[2] step (256 x 5 M Form D + the 5 M-record corpus, one
 apo_score call) on one engine, alternating blocks with TUNE_NO_TWIN set (K1 reads the 36 B/eval fp32 tensor) and clear (K1q
-reads the 14 B/eval copy built at load).  Reports per setting the ms/step median and spread, the scoring kernel's time and
-the bytes it moved per second (36 or 14 B per evaluation + 32 B per corpus record), whether the two settings gave identical
-integers, scores and top-K, and the wall time of apo_dims_generate with and without building the copy.
+reads the copy built at load: Form W words, 8 B/eval, when no coded dimension has more than 15 values, else the 14 B/eval
+Form Q planes).  Reports which copy is held (from the K1q instantiation a profiler record shows), per setting the ms/step
+median and spread, the scoring kernel's time and the bytes it moved per second (36, 14 or 8 B per evaluation + 32 B per corpus
+record), whether the two settings gave identical integers, scores and top-K, and the wall time of apo_dims_generate with and
+without building the copy.
 
     python examples/form_d_twin.py [--steps 20] [--rounds 3] [--out FILE.json]
 
@@ -11,6 +13,7 @@ import argparse
 import importlib
 import json
 import os
+import re
 import subprocess
 import sys
 import time
@@ -27,6 +30,24 @@ def card():
                               capture_output=True, text=True, timeout=30).stdout.strip()
     except Exception as ex:       # the numbers are still printed; without the card line they are not comparable
         return f"unknown ({ex})"
+
+
+def held_copy(fn):
+    """'W' or 'Q': the layout the K1q launch of fn() read (last template argument of k_reward9q), None if K1q did not run"""
+    import torch
+    from torch.profiler import ProfilerActivity, profile
+    torch.cuda.synchronize()
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        fn()
+        torch.cuda.synchronize()
+    for ev in prof.events():
+        m = re.search(r"k_reward9q<([^>]*)>", ev.name)
+        if m:
+            return "W" if m.group(1).split(",")[-1].strip() == "true" else "Q"
+        m = re.search(r"k_reward9qI(.*)EEvNS_8KqParams", ev.name)       # not demangled
+        if m:
+            return "W" if m.group(1).endswith("Lb1EE") else "Q"
+    return None
 
 
 def main():
@@ -57,6 +78,8 @@ def main():
                                   for name, v in load.items()}
         # the last load (flags 0) holds the copy; TUNE_NO_TWIN from here on only stops it being read
         eng.corpus_generate(seed, 0, T, 300)
+        copy = held_copy(lambda: eng.score(C, K, corpus=True))
+        out["copy"] = {"W": "Form W (8 B/eval)", "Q": "Form Q (14 B/eval)"}.get(copy, "none")
         stream = torch.cuda.current_stream()
         eng.set_stream(stream.cuda_stream)
         steps = {name: [] for name in settings}
@@ -78,7 +101,7 @@ def main():
                 last[name] = (r, eng.debug_partials(C))
         eng.set_tuning(0)
         eng.set_stream(0)
-        per_eval = {"k1_fp32": 36, "k1q_copy": 14}
+        per_eval = {"k1_fp32": 36, "k1q_copy": 8 if copy == "W" else 14}
         for name in settings:
             s, k = np.array(steps[name]), np.array(kernel[name])
             moved = per_eval[name] * C * T + 32 * T

@@ -143,7 +143,7 @@ int  apo_set_weights(apo_engine *e, const double w[APO_NDIM]);
 #define APO_TUNE_FORCE_FUSE  0x2u  /* corpus scan inside the scoring launch even when it cannot hide behind it   */
 #define APO_TUNE_NO_STAGING  0x4u  /* pageable host buffers straight to cudaMemcpy (no threaded pinned staging)  */
 #define APO_TUNE_NCCL_JOIN   0x8u  /* join shards with ncclAllReduce + k_finalize instead of the peer-memory join */
-#define APO_TUNE_NO_TWIN     0x10u /* no Form Q copy of a loaded Form D tensor is built or read: resident Form D runs K1 */
+#define APO_TUNE_NO_TWIN     0x10u /* no Form Q / W copy of a loaded Form D tensor is built or read: resident Form D runs K1 */
 int  apo_set_tuning(apo_engine *e, uint32_t flags);
 int  apo_get_weights(const apo_engine *e, double w[APO_NDIM]);
 
@@ -186,7 +186,10 @@ int apo_corpus_upload_json(apo_engine *e, const char *json, uint64_t len, uint64
  * Form R: one apo_record per (candidate, record); dims derived on device (TCS:668-763).
  * apo_dims_upload and apo_dims_generate also build a Form Q copy of the tensor (see below) when its evaluations are
  * categorical and at least 4 GiB of device memory stays free beside the copy; otherwise, quietly, they keep Form D alone.
- * Resident Form D calls with variant 0 and a window starting on a multiple of 8 then read the copy through K1q (14 B
+ * When no coded dimension (every one but d2) takes more than 15 values (true for dims produced by TCS:668-763) and 4 GiB
+ * also stay free beside the Form Q planes and one more 8-byte word per evaluation, the copy is kept as Form W instead: per
+ * evaluation eight 4-bit codes (15 = absent) and the fp32 tool_success_rate bits (one NaN pattern = absent), 8 B.
+ * Resident Form D calls with variant 0 and a window starting on a multiple of 8 then read the copy through K1q (8 B or 14 B
  * instead of 36 B per evaluation); other variants and windows read the fp32 tensor through K1.  The results are the same
  * either way.  The fp32 tensor stays loaded (apo_dims_layout 1, apo_dims_download); the copy goes with the next load or
  * attach, and whenever an engine allocation would otherwise fail for lack of device memory.  apo_dims_attach never
@@ -199,7 +202,7 @@ int apo_dims_download(apo_engine *e, float *out, uint32_t c, uint64_t first, uin
  * fp32 tool_success_rate + a 2-byte presence index per evaluation (14 B instead of 36 B), lossless.  Available when every
  * dimension except d2 takes <= 255 distinct values (true for dims produced by TCS:668-763).
  * apo_dims_compact transcodes the loaded Form D in place (the fp32 copy is released; when the Form Q copy
- * built at load is held, it becomes the tensor without a second transcode);
+ * built at load is held, it becomes the tensor without a second transcode; a Form W copy is released first);
  * the *_compact generate/upload variants never materialise the full fp32 tensor.  When the data
  * is not categorical they return APO_E_STATE: apo_dims_compact keeps the loaded Form D usable, the
  * streaming variants leave nothing loaded.  Scores, counts, top-K and the integer partial sums are

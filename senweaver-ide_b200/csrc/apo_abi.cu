@@ -100,6 +100,9 @@ struct apo_engine {
 	DevBuf<double> d_ptab, d_pair; DevBuf<float> stage, d_cbf, d_d2book, d_d2stream; uint32_t q_n0 = 0, q_n1 = 0; bool q_pair_ok = false;
 	DevBuf<uint32_t> unpack_bad;                              // k_unpack_p: an evaluation named an empty or NaN codebook slot
 	uint32_t qbook_host[8 * 256]; bool compact = false, twin = false;
+	// twin_w: the copy is held as Form W words (qw, 8 B per evaluation; the Form Q planes are released) because no coded
+	// dimension has more than 15 values
+	DevBuf<unsigned long long> qw; bool twin_w = false;
 	uint32_t d2book_host[4096]; uint32_t d2book_n = ~0u;       // Form P export of the resident tensor (~0 = not built yet)
 	DevBuf<uint8_t> roll; uint32_t roll_C = 0, roll_row = 32; uint64_t roll_T = 0, roll_pitch = 0;   // Form R (32 B) or R16 (16 B) rows
 	// Form T (csrc/apo_tuple.cu): resident index planes + dictionary; per call: product table of its codebook, table values
@@ -130,7 +133,7 @@ struct apo_engine {
 	void *peer_base[apo::PEER_MAX] = {nullptr}; bool peer_ipc[apo::PEER_MAX] = {false};
 	unsigned long long join_epoch = 0;
 	bool env_no_fuse = false, env_force_fuse = false, env_no_staging = false, env_nccl_join = false, env_no_twin = false;   // apo_set_tuning
-	double stream_bytes_per_ms = 7.4e9, stream_q_bytes_per_ms = 5.0e9, scan_ms_per_record = 3.35e-7;   // fuse heuristic, derived from the device at apo_create
+	double stream_bytes_per_ms = 7.4e9, stream_q_bytes_per_ms = 5.0e9, stream_w_bytes_per_ms = 6.0e9, scan_ms_per_record = 3.35e-7;   // fuse heuristic, derived from the device at apo_create
 	size_t mem_pitch_max = 0;
 	uint8_t *zc_host = nullptr; uint64_t zc_cap = 0;   // zero-copy block of the single-trace path
 	bool timing_on = true;
@@ -170,11 +173,11 @@ int fail(apo_engine *e, int code, const char *fmt, ...) {
 
 void drop_twin(apo_engine *e) {
 	if (!e->twin) return;
-	e->q8.release(); e->qd2.release(); e->qli.release();
-	e->twin = false;
+	e->q8.release(); e->qd2.release(); e->qli.release(); e->qw.release();
+	e->twin = e->twin_w = false;
 }
 
-// Every engine buffer grows through here.  The Form Q copy of the fp32 tensor is a cache: an allocation that fails for lack
+// Every engine buffer grows through here.  The Form Q / W copy of the fp32 tensor is a cache: an allocation that fails for lack
 // of device memory while it is held releases it and is tried once more, so holding it never fails a call that would succeed
 // without it.  Launches already queued may still read the copy: they finish first.  A resident call picks the evaluations
 // it reads (route_twin) only after its last allocation before its launches.
@@ -361,8 +364,8 @@ int compact_finish(apo_engine *e, uint32_t C, uint64_t T, uint64_t pitch, bool t
 	return APO_OK;
 }
 
-// After apo_dims_upload / apo_dims_generate: the Form Q copy of the engine's fp32 tensor, which resident Form D calls read
-// through K1q (route_twin) at 14 instead of 36 bytes per evaluation.  Built when the evaluations are categorical and at least
+// After apo_dims_upload / apo_dims_generate: the Form Q (or Form W, below) copy of the engine's fp32 tensor, which resident
+// Form D calls read through K1q (route_twin) at 14 (8) instead of 36 bytes per evaluation.  Built when the evaluations are categorical and at least
 // kTwinHeadroom of device memory stays free beside it; otherwise Form D is kept alone, without an error.
 constexpr uint64_t kTwinHeadroom = 4ull << 30;
 int build_twin(apo_engine *e) {
@@ -381,7 +384,20 @@ int build_twin(apo_engine *e) {
 	if (rc) return rc;
 	CK(apo::run_transcode(e->dims_ptr, pitch, C, T, e->q8.p, e->qd2.p, pitch, e->qbook.p, e->qbook.p + 8 * 256, e->stream));
 	rc = compact_finish(e, C, T, pitch, true);
-	return rc == APO_E_STATE ? APO_OK : rc;
+	if (rc != APO_OK) return rc == APO_E_STATE ? APO_OK : rc;
+	// A copy whose coded dimensions take at most 15 values each (dense codes 0-14, so 15 can mean absent; true for every tensor
+	// TCS:668-763 produces) is kept as Form W words instead: 8 instead of 14 bytes per evaluation.  They are packed from the
+	// planes, so the build peaks at the fp32 tensor + the planes + the words; without kTwinHeadroom beside that, Form Q stays.
+	for (int j = 0; j < 8; j++)
+		if (e->qbook_host[256 * j + 15] != 0xFFFFFFFFu) return APO_OK;
+	CK(cudaMemGetInfo(&free_bytes, &total_bytes));
+	if ((uint64_t)free_bytes < n * 8 + kTwinHeadroom) return APO_OK;
+	if (e->qw.reserve(n) != cudaSuccess) { cudaGetLastError(); return APO_OK; }
+	CK(apo::run_pack_w(e->q8.p, e->qd2.p, e->qli.p, n, e->qw.p, e->stream));
+	CK(cudaStreamSynchronize(e->stream));
+	e->q8.release(); e->qd2.release(); e->qli.release();
+	e->twin_w = true;
+	return APO_OK;
 }
 
 // true when the driver does not know the pointer: ordinary pageable host memory (malloc, JS ArrayBuffer, numpy)
@@ -608,13 +624,14 @@ struct Evals {
 	uint32_t n_tuples = 0;
 	const float *d2book = nullptr;
 	const uint32_t *codebook = nullptr;       // resident Form T: every launch rebuilds this codebook's tables (NULL: built once per call)
+	const unsigned long long *qw = nullptr;   // Form W words (the copy of a resident Form D tensor, route_twin)
 
 	bool records() const { return form == apo::CAND_REC32 || form == apo::CAND_REC16; }
 	uint32_t row() const { return form == apo::CAND_DIMS ? 36 : form == apo::CAND_REC32 ? 32 : 16; }
-	uint32_t bytes() const { return form == apo::CAND_T ? 3 : form == apo::CAND_Q ? 14 : row(); }   // read per evaluation
+	uint32_t bytes() const { return form == apo::CAND_T ? 3 : form == apo::CAND_Q ? 14 : form == apo::CAND_W ? 8 : row(); }   // read per evaluation
 	uint64_t tile() const {                   // evaluations per tile of the scoring kernel
 		return (uint64_t)(form == apo::CAND_T ? apo::kt_tile_evals() : form == apo::CAND_Q ? apo::kq_tile_evals(variant)
-		                                                                                   : apo::k1_tile_evals((int)row(), variant));
+		                  : form == apo::CAND_W ? apo::kw_tile_evals() : apo::k1_tile_evals((int)row(), variant));
 	}
 };
 
@@ -656,16 +673,22 @@ int resident_window(apo_engine *e, const apo_score_opts *o, Evals *ev) {
 	ev->idx_base = first;
 	if (ev->rows) ev->rows += first * ev->row();
 	if (ev->q8) { ev->q8 += first; ev->d2 += first; ev->li += first; }
+	if (ev->qw) ev->qw += first;
 	if (ev->tl) { ev->tl += first; ev->th += first; }
 	return APO_OK;
 }
 
-// A resident Form D call reads the Form Q copy through K1q instead when one is held, the variant is the default (1-4 name K1
-// tile shapes) and the window starts on K1q's 8-evaluation grid.  Before resident_window, after the call's last allocation
+// A resident Form D call reads the Form Q / W copy through K1q instead when one is held, the variant is the default (1-4 name
+// K1 tile shapes) and the window starts on K1q's 8-evaluation grid.  Before resident_window, after the call's last allocation
 // before its launches (reserve may release the copy).
 void route_twin(const apo_engine *e, const apo_score_opts *o, Evals *ev) {
 	if (ev->form != apo::CAND_DIMS || !e->twin || e->env_no_twin || o->variant != 0 || o->first % 8) return;
-	ev->form = apo::CAND_Q; ev->rows = nullptr;
+	ev->rows = nullptr;
+	if (e->twin_w) {                                         // <= 15 codes per dimension: the prefix table always fits
+		ev->form = apo::CAND_W; ev->qw = e->qw.p; ev->variant = 0;
+		return;
+	}
+	ev->form = apo::CAND_Q;
 	ev->q8 = e->q8.p; ev->d2 = e->qd2.p; ev->li = e->qli.p;
 	ev->variant = e->q_pair_ok ? 0 : 4;                      // as resident_evals for a compact tensor
 }
@@ -683,9 +706,9 @@ int launch_score(apo_engine *e, const apo_score_opts *o, const Evals &ev, uint32
 		P.tl = ev.tl; P.th = ev.th; P.pitch_evals = ev.pitch_evals; P.C = ev.C; P.T = ev.count;
 		P.acc = acc; P.tval = e->tup_val.p; P.n_tuples = ev.n_tuples; P.bad = e->tup_bad.p;
 		CK(apo::run_reward9t(P, e->sm_count, e->stream));
-	} else if (ev.form == apo::CAND_Q) {
+	} else if (ev.form == apo::CAND_Q || ev.form == apo::CAND_W) {
 		apo::KqParams Q{};
-		Q.q8 = ev.q8; Q.d2 = ev.d2; Q.li = ev.li; Q.pitch_evals = ev.pitch_evals; Q.C = ev.C; Q.T = ev.count;
+		Q.q8 = ev.q8; Q.d2 = ev.d2; Q.li = ev.li; Q.qw = ev.qw; Q.pitch_evals = ev.pitch_evals; Q.C = ev.C; Q.T = ev.count;
 		Q.acc = acc; Q.lut = e->d_lut.p; Q.ptab = e->d_ptab.p; Q.w2 = e->W.w[2];
 		Q.pair = e->d_pair.p; Q.cbf = e->d_cbf.p; Q.n0 = e->q_n0; Q.n1 = e->q_n1;
 		for (int j = 0; j < 8; j++) Q.wq[j] = e->W.w[kCodedDim[j]];
@@ -741,9 +764,9 @@ int launch_cand(apo_engine *e, const Evals &ev, uint32_t cand_offset) {
 	P.C = ev.C; P.T = ev.count; P.idx_base = ev.idx_base; P.pitch_evals = ev.pitch_evals; P.lut = e->d_lut.p;
 	P.ints = e->cand_acc.p + (uint64_t)apo::CB_INT * cand_offset;
 	P.ex = (unsigned long long *)(e->cand_acc.p + (uint64_t)apo::CB_INT * e->score_C) + 3ull * cand_offset;
-	P.rows = ev.rows; P.q8 = ev.q8; P.d2 = ev.d2; P.li = ev.li;
+	P.rows = ev.rows; P.q8 = ev.q8; P.d2 = ev.d2; P.li = ev.li; P.qw = ev.qw;
 	P.tl = ev.tl; P.th = ev.th; P.tb_pc = ev.tb_pc; P.tb_pd = ev.tb_pd; P.n_tuples = ev.n_tuples; P.d2book = ev.d2book;
-	if (ev.form == apo::CAND_Q) P.cbf = e->d_cbf.p;           // the tables of the codebook this call scores with (upload_ptab)
+	if (ev.form == apo::CAND_Q || ev.form == apo::CAND_W) P.cbf = e->d_cbf.p;   // the tables of the codebook this call scores with (upload_ptab)
 	if (ev.form == apo::CAND_T) P.tbook = e->cand_book.p;
 	CK(apo::run_cand_breakdown(P, ev.form, e->sm_count, e->stream));
 	e->timing.launches++;
@@ -1069,17 +1092,19 @@ extern "C" int apo_create(int device, apo_engine **out) {
 	e->mem_pitch_max = prop.memPitch;
 	{
 		// fuse heuristic (apo_score): the corpus scan rides on one warp per SM and must hide behind the evaluation stream.
-		// Stream rate = 0.9 x the pin bandwidth of this device for Form D / R (0.61 x for the SM-bound compact layout); scan
-		// rate = kScanRecordsPerSmCycle records per SM clock on that one warp.  Both only steer the fuse / no-fuse choice.
+		// Stream rate = 0.9 x the pin bandwidth of this device for Form D / R (0.61 x for the SM-bound compact layout, kWordFracOfPin
+		// x for Form W words); scan rate = kScanRecordsPerSmCycle records per SM clock on that one warp.  Both only steer the fuse /
+		// no-fuse choice.
 		int mem_khz = 0, bus_bits = 0, sm_khz = 0;
 		cudaDeviceGetAttribute(&mem_khz, cudaDevAttrMemoryClockRate, device);
 		cudaDeviceGetAttribute(&bus_bits, cudaDevAttrGlobalMemoryBusWidth, device);
 		cudaDeviceGetAttribute(&sm_khz, cudaDevAttrClockRate, device);
-		constexpr double kStreamFracOfPin = 0.90, kCompactFracOfPin = 0.61, kScanRecordsPerSmCycle = 1.0264e-2;
+		constexpr double kStreamFracOfPin = 0.90, kCompactFracOfPin = 0.61, kWordFracOfPin = 0.58 /* K1q on Form W: 2.0 TB/s of 3.35 on an H100 80GB HBM3 at 400 W */, kScanRecordsPerSmCycle = 1.0264e-2;
 		if (mem_khz > 0 && bus_bits > 0) {
 			const double pin_bytes_per_ms = 2.0 * (double)mem_khz * (double)bus_bits / 8.0;     // kHz x bytes = bytes per ms
 			e->stream_bytes_per_ms = kStreamFracOfPin * pin_bytes_per_ms;
 			e->stream_q_bytes_per_ms = kCompactFracOfPin * pin_bytes_per_ms;
+			e->stream_w_bytes_per_ms = kWordFracOfPin * pin_bytes_per_ms;
 		}
 		if (sm_khz > 0) e->scan_ms_per_record = 1.0 / (kScanRecordsPerSmCycle * (double)e->sm_count * (double)sm_khz);
 	}
@@ -1114,7 +1139,7 @@ extern "C" void apo_destroy(apo_engine *e) {
 	peer_teardown(e);
 	if (e->comm && g_nccl.CommDestroy) g_nccl.CommDestroy(e->comm);
 	if (e->zc_host) cudaFreeHost(e->zc_host);
-	e->q8.release(); e->qd2.release(); e->qli.release(); e->qbook.release(); e->d_ptab.release(); e->d_pair.release(); e->d_cbf.release(); e->d_d2book.release(); e->d_d2stream.release(); e->unpack_bad.release(); e->stage.release();
+	e->q8.release(); e->qd2.release(); e->qli.release(); e->qw.release(); e->qbook.release(); e->d_ptab.release(); e->d_pair.release(); e->d_cbf.release(); e->d_d2book.release(); e->d_d2stream.release(); e->unpack_bad.release(); e->stage.release();
 	e->d_lut.release(); e->corpus.release(); e->dims.release(); e->roll.release(); e->acc.release(); e->acc_joined.release(); e->acc_snapshot.release(); e->misc.release();
 	e->result.release(); e->keys.release(); e->sel_key.release(); e->sel_idx.release();
 	e->tups_pc.release(); e->tups_pd.release(); e->tups_d2.release();
@@ -1330,11 +1355,12 @@ extern "C" int apo_dims_compact(apo_engine *e) {
 	if (e->compact) return APO_OK;
 	if (!e->dims_ptr || e->dims_C == 0) return fail(e, APO_E_STATE, "no dims loaded");
 	CK(cudaSetDevice(e->device));
-	if (e->twin) {                                      // the copy built at load already is this tensor in Form Q
+	if (e->twin && !e->twin_w) {                        // the copy built at load already is this tensor in Form Q
 		e->twin = false; e->compact = true; e->dims_ptr = nullptr;
 		e->dims.release();
 		return APO_OK;
 	}
+	drop_twin(e);                                       // a Form W copy is not a compact tensor: transcode the fp32 one
 	const uint32_t C = e->dims_C; const uint64_t T = e->dims_T, pitch_in = e->dims_pitch, pitch = round_up(T ? T : 1, 32);
 	int rc = compact_begin(e, C, pitch);
 	if (rc) return rc;
@@ -1522,7 +1548,8 @@ extern "C" int apo_score(apo_engine *e, const apo_score_opts *o, double *scores,
 	// One launch per call: the corpus scan (K2) rides on an extra warp of every scoring CTA and the last CTA finalises (K3,
 	// after the peer-memory join when the record axis is sharded) ... when the scan can hide behind the evaluation stream.
 	// Both rates are derived from the device at apo_create.
-	const double k1_ms = stream_bytes / (ev.form == apo::CAND_Q ? e->stream_q_bytes_per_ms : e->stream_bytes_per_ms);
+	const double k1_ms = stream_bytes / (ev.form == apo::CAND_Q ? e->stream_q_bytes_per_ms
+	                                     : ev.form == apo::CAND_W ? e->stream_w_bytes_per_ms : e->stream_bytes_per_ms);
 	const double scan_ms = (double)e->corpus_T * e->scan_ms_per_record;
 	const bool one_launch = e->nranks == 1 || peer_join_active(e, C);
 	// ... or when it is tiny anyway (the IDE's real corpora, <= 1000 traces): at most 16 records per lane of the corpus warps,

@@ -102,6 +102,33 @@ struct LoadQ {
 	}
 };
 
+// Form W: one word per evaluation, nibble codes (15 = absent) through the [8][256] fp32 codebook, d2 NaN = absent
+struct LoadW {
+	static constexpr int U = 4;
+	struct Raw { unsigned long long q; };
+	__device__ static void fetch(const CandParams &P, uint32_t c, uint64_t t, Raw &R) {
+		R.q = __ldg(P.qw + (uint64_t)c * P.pitch_evals + t);
+	}
+	__device__ static void decode(const CandParams &, const CandSmem &S, const Raw &R, CandEval &E) {
+		const uint32_t w = (uint32_t)R.q;
+		uint32_t mask = 0;
+#pragma unroll
+		for (int j = 0; j < 8; j++) {
+			const int dim = j < 2 ? j : j + 1;
+			const uint32_t nib = (w >> (4 * j)) & 15u;
+			E.v[dim] = nib == 15u ? 0.0 : (double)S.tab[256 * j + nib];
+			mask |= (nib != 15u ? 1u : 0u) << dim;
+		}
+		const float d2 = __uint_as_float((uint32_t)(R.q >> 32));
+		const bool p2 = d2 == d2;
+		E.v[2] = p2 ? (double)d2 : 0.0;
+		mask |= (p2 ? 1u : 0u) << 2;
+		E.mask = mask;
+		E.valid = S.tw[mask] > 0.0 ? 1u : 0u;
+		E.fb = tally_of_d0(E.v[0], mask);
+	}
+};
+
 struct LoadT {
 	static constexpr int U = 4;
 	struct Raw { uint32_t idx; };
@@ -251,6 +278,7 @@ cudaError_t run_cand_breakdown(const CandParams &P, int source, int sm_count, cu
 	case CAND_REC16: return launch_cand<LoadRec<16>, 0>(P, sm_count, st);
 	case CAND_Q: return launch_cand<LoadQ, 1>(P, sm_count, st);
 	case CAND_T: return launch_cand<LoadT, 2>(P, sm_count, st);
+	case CAND_W: return launch_cand<LoadW, 1>(P, sm_count, st);
 	default: return cudaErrorInvalidValue;
 	}
 }

@@ -17,6 +17,10 @@
 // the host with the same IEEE multiplications as TCS:781), so a coded dimension costs one LDS.64
 // and one DADD; sums, division and the exact fixed-point accumulation are those of K1, hence the
 // integer partial sums are bit-identical to K1's and to the oracle's.
+//
+// Form W is the 8-byte variant of the copy the engine keeps of a resident Form D tensor (apo_abi.cu build_twin) when every
+// coded dimension takes at most 15 values: one word per evaluation, the eight dense codes as nibbles (15 = absent) and the
+// fp32 d2 bits (KW_D2_ABSENT = absent).  K1q reads it with one bulk copy per tile and derives the LUT entry from the nibbles.
 #include <cstdlib>
 #include "apo_device.cuh"
 #include "apo_kernels.h"
@@ -119,6 +123,28 @@ cudaError_t run_recode(unsigned long long *q8, float *d2, unsigned short *li, ui
 	uint64_t g = (n + 255) / 256;
 	if (g > 132ull * 32) g = 132ull * 32;
 	k_recode<<<(unsigned)g, 256, 0, st>>>(q8, d2, li, n, remap);
+	return cudaGetLastError();
+}
+
+// Form Q -> Form W (the 8-byte copy of a resident Form D tensor): the dense codes, every one < 15, as nibbles (255 -> 15)
+// and the fp32 tool_success_rate bits, KW_D2_ABSENT when dimension 2 is absent.
+__global__ void __launch_bounds__(256)
+k_pack_w(const unsigned long long *q8, const float *d2, const unsigned short *li, uint64_t n, unsigned long long *qw) {
+	for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x) {
+		const unsigned long long q = q8[i];
+		uint32_t w = 0;
+#pragma unroll
+		for (int j = 0; j < 8; j++) w |= ((uint32_t)(q >> (8 * j)) & 15u) << (4 * j);     // 255 -> 15
+		const uint32_t d = ((li[i] >> 6) & 1u) ? __float_as_uint(d2[i]) : KW_D2_ABSENT;     // rotated index: dim 2 lives in bit 6
+		qw[i] = (unsigned long long)w | ((unsigned long long)d << 32);
+	}
+}
+
+cudaError_t run_pack_w(const unsigned long long *q8, const float *d2, const unsigned short *li, uint64_t n, unsigned long long *qw, cudaStream_t st) {
+	if (n == 0) return cudaSuccess;
+	uint64_t g = (n + 255) / 256;
+	if (g > 132ull * 32) g = 132ull * 32;
+	k_pack_w<<<(unsigned)g, 256, 0, st>>>(q8, d2, li, n, qw);
 	return cudaGetLastError();
 }
 
@@ -275,18 +301,22 @@ cudaError_t run_decode(const unsigned long long *q8, const float *d2, const unsi
 // =================================================================== K1q
 struct QMeta { int32_t cand; int32_t n; };
 
-template <int CW, int EPT, int STAGES>
+// W: the stage holds Form W words (8 B per evaluation, one bulk copy) instead of the three Form Q planes (14 B, three copies),
+// and the code tables have 16 slots per coded dimension (slot 15 = absent = +0.0).
+template <int CW, int EPT, int STAGES, bool W = false>
 struct KqCfg {
 	static constexpr int NCONS = CW * 32;
 	static constexpr int TILE = NCONS * EPT;
-	static constexpr int Q8_BYTES = TILE * 8, D2_BYTES = TILE * 4, LI_BYTES = TILE * 2;
+	static constexpr int Q8_BYTES = TILE * 8, D2_BYTES = W ? 0 : TILE * 4, LI_BYTES = W ? 0 : TILE * 2;
 	static constexpr int STAGE_BYTES = Q8_BYTES + D2_BYTES + LI_BYTES;
+	static constexpr int NCODE = W ? 16 : 256;                    // table slots per coded dimension
 	static constexpr int LUT_OFF = STAGES * STAGE_BYTES;          // double2[512]
-	static constexpr int PTAB_OFF = LUT_OFF + 512 * 16;           // double[8][256]
-	static constexpr int CBF_OFF = PTAB_OFF + 8 * 256 * 8;        // float[8][256] code -> value (mixed-lookup variants)
-	static constexpr int PAIR_OFF = CBF_OFF + 8 * 256 * 4;        // double[KQ_PAIR_MAX] exact prefix fl(fl(0 + d0*w0) + d1*w1)
-	static constexpr int CAT_OFF = PAIR_OFF + KQ_PAIR_MAX * 8;    // categorical product table of the fused corpus scan
-	static constexpr int BAR_OFF = CAT_OFF + CAT_WORDS * 8;
+	static constexpr int PTAB_OFF = LUT_OFF + 512 * 16;           // double[8][NCODE]
+	static constexpr int CBF_OFF = PTAB_OFF + 8 * NCODE * 8;      // float[8][NCODE] code -> value (mixed-lookup variants)
+	static constexpr int PAIR_OFF = CBF_OFF + 8 * NCODE * 4;      // double[KQ_PAIR_MAX] exact prefix fl(fl(0 + d0*w0) + d1*w1); W: [16][16]
+	static constexpr int CAT_OFF = PAIR_OFF + (W ? 256 : KQ_PAIR_MAX) * 8;   // categorical product table of the fused corpus scan
+	static constexpr int WLUT_OFF = CAT_OFF + CAT_WORDS * 8;      // W: double2[512] indexed by w_lut_key (the corpus warp keeps LUT_OFF)
+	static constexpr int BAR_OFF = WLUT_OFF + (W ? 512 * 16 : 0);
 	static constexpr int META_OFF = BAR_OFF + 2 * STAGES * 8;
 	static constexpr int EX_OFF = META_OFF + STAGES * 8;
 	static constexpr int SMEM = EX_OFF + 18 * 8 + 16;
@@ -343,10 +373,50 @@ __device__ __forceinline__ void evalq_ws_mixed(unsigned long long q, float d2f, 
 	valid = t_out.x > 0.0 ? 1u : 0u;
 }
 
-template <int CW, int EPT, int STAGES, bool RECIP, int NF = -1>
+// Form W's LUT order: the presence bits as K1q derives them from a word, i.e. coded dimensions 4-7 (dims 5-8, the ones that
+// vary independently: lanes with different masks mostly hit different banks, as with lut_index) in bits 0-3, coded dimensions
+// 0-3 (dims 0, 1, 3, 4) in bits 4-7, dimension 2 in bit 8.  natural_mask: bit = dimension.
+__device__ __forceinline__ uint32_t w_lut_key(uint32_t m) {
+	return ((m >> 5) & 15u) | ((m & 3u) << 4) | (((m >> 3) & 3u) << 6) | (((m >> 2) & 1u) << 8);
+}
+
+// The same key from the nibble word of an evaluation (nibble 15 = absent) and the presence of its tool_success_rate.
+__device__ __forceinline__ uint32_t w_key_of(uint32_t w, bool p2) {
+	const uint32_t r = ~__funnelshift_l(w, w, 16);                   // coded dimensions 4-7 first; a nibble is zero iff absent
+	uint32_t z = (r | (r >> 1) | (r >> 2) | (r >> 3)) & 0x11111111u;  // bit 4k: nibble k present
+	z = (z | (z >> 3)) & 0x03030303u;                                 // gather the eight bits: 2 per byte, 4 per half, 8
+	z = (z | (z >> 6)) & 0x000F000Fu;
+	z = (z | (z >> 12)) & 0xFFu;
+	return z | (p2 ? 256u : 0u);
+}
+
+// Mixed-lookup evaluation of one Form W word: the operations and their order are those of evalq_ws_mixed.  The prefix
+// table is [16][16] indexed by the two low nibbles (absent rows / columns hold the absent entries), the others [8][16].
+template <int NF>
+__device__ __forceinline__ void evalw_ws_mixed(unsigned long long q, const double *ptab, const float *cbf, const double *pair,
+                                               const double (&wq)[8], double w2, const double2 *wlut, double &ws_out, double2 &t_out,
+                                               uint32_t &valid) {
+	const uint32_t w = (uint32_t)q;
+	const float d2 = __uint_as_float((uint32_t)(q >> 32));
+	const bool p2 = d2 == d2;                                         // absent = NaN
+	double ws = pair[w & 255u];
+	ws = __dadd_rn(ws, __dmul_rn((double)(p2 ? d2 : 0.0f), w2));    // +0.0 when absent, as Form Q stores it
+#pragma unroll
+	for (int j = 2; j < 8; j++) {
+		const uint32_t code = (w >> (4 * j)) & 15u;
+		if (j - 2 < NF) ws = __dadd_rn(ws, __dmul_rn((double)cbf[j * 16 + code], wq[j]));
+		else ws = __dadd_rn(ws, ptab[j * 16 + code]);
+	}
+	ws_out = ws;
+	t_out = wlut[w_key_of(w, p2)];
+	valid = t_out.x > 0.0 ? 1u : 0u;
+}
+
+template <int CW, int EPT, int STAGES, bool RECIP, int NF = -1, bool W = false>
 __global__ void __launch_bounds__((CW + 2) * 32, 1)
 k_reward9q(const KqParams P) {
-	using Cfg = KqCfg<CW, EPT, STAGES>;
+	using Cfg = KqCfg<CW, EPT, STAGES, W>;
+	static_assert(!W || NF >= 0, "Form W runs the mixed-lookup form only");
 	extern __shared__ __align__(128) uint8_t smem[];
 	double2 *s_lut = reinterpret_cast<double2 *>(smem + Cfg::LUT_OFF);
 	double *s_ptab = reinterpret_cast<double *>(smem + Cfg::PTAB_OFF);
@@ -359,12 +429,28 @@ k_reward9q(const KqParams P) {
 	unsigned long long *s_ex = reinterpret_cast<unsigned long long *>(smem + Cfg::EX_OFF);
 	bool *s_last = reinterpret_cast<bool *>(smem + Cfg::EX_OFF + 18 * 8);
 
+	double2 *s_wlut = reinterpret_cast<double2 *>(smem + Cfg::WLUT_OFF);
+
 	const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
 	for (int i = tid; i < 512; i += blockDim.x) s_lut[lut_index(i)] = make_double2(P.lut[i], P.lut[512 + i]);
+	if constexpr (W) {
+		// the host's [8][256] tables (dense codes < 15; slot 255 = absent = +0.0) cut to 16 slots, slot 15 = absent
+		for (int i = tid; i < 512; i += blockDim.x) s_wlut[w_lut_key(i)] = make_double2(P.lut[i], P.lut[512 + i]);
+		for (int i = tid; i < 8 * 16; i += blockDim.x) {
+			const int src = (i >> 4) * 256 + ((i & 15) < 15 ? (i & 15) : 255);
+			s_ptab[i] = P.ptab[src];
+			if (NF > 0) s_cbf[i] = P.cbf[src];
+		}
+		for (int i = tid; i < 256; i += blockDim.x) {                  // [c1][c0]: index = the two low nibbles of a word
+			const uint32_t c0 = min((uint32_t)i & 15u, P.n0), c1 = min((uint32_t)i >> 4, P.n1);
+			s_pair[i] = P.pair[c0 * (P.n1 + 1u) + c1];
+		}
+	} else {
 	for (int i = tid; i < 8 * 256; i += blockDim.x) s_ptab[i] = P.ptab[i];
 	if (NF >= 0) {
 		for (int i = tid; i < 8 * 256; i += blockDim.x) s_cbf[i] = P.cbf[i];
 		for (int i = tid; i < (int)((P.n0 + 1u) * (P.n1 + 1u)); i += blockDim.x) s_pair[i] = P.pair[i];
+	}
 	}
 	for (int i = tid; i < CAT_WORDS; i += blockDim.x) s_cat[i] = P.lut[1024 + i];
 	if (tid == 0) {
@@ -392,11 +478,16 @@ k_reward9q(const KqParams P) {
 				const uint32_t n = rem < (uint64_t)Cfg::TILE ? (uint32_t)rem : (uint32_t)Cfg::TILE;
 				const uint32_t n8 = (n + 7u) & ~7u;                         // 64 / 32 / 16 B multiples for the three bulk copies
 				meta[s].cand = (int32_t)c; meta[s].n = (int32_t)n;
-				mbar_expect_tx(&full[s], n8 * 14u);
 				uint8_t *st = smem + s * Cfg::STAGE_BYTES;
+				if constexpr (W) {
+					mbar_expect_tx(&full[s], n8 * 8u);
+					bulk_g2s(st, P.qw + (uint64_t)c * P.pitch_evals + e0, n8 * 8u, &full[s], pol);
+				} else {
+				mbar_expect_tx(&full[s], n8 * 14u);
 				bulk_g2s(st, P.q8 + (uint64_t)c * P.pitch_evals + e0, n8 * 8u, &full[s], pol);
 				bulk_g2s(st + Cfg::Q8_BYTES, P.d2 + (uint64_t)c * P.pitch_evals + e0, n8 * 4u, &full[s], pol);
 				bulk_g2s(st + Cfg::Q8_BYTES + Cfg::D2_BYTES, P.li + (uint64_t)c * P.pitch_evals + e0, n8 * 2u, &full[s], pol);
+				}
 			}
 		}
 	} else if (warp == CW + 1) {
@@ -418,6 +509,9 @@ k_reward9q(const KqParams P) {
 	auto evalq = [&](unsigned long long q, float d2f, uint32_t idx, double &ws, double2 &t, uint32_t &ok) {
 		if (NF >= 0) evalq_ws_mixed<(NF >= 0 ? NF : 0)>(q, d2f, idx, s_ptab, s_cbf, s_pair, n0, n1, wq, w2, s_lut, ws, t, ok);
 		else evalq_ws(q, d2f, idx, s_ptab, w2, s_lut, ws, t, ok);
+	};
+	auto evalw = [&](unsigned long long q, double &ws, double2 &t, uint32_t &ok) {
+		evalw_ws_mixed<(NF >= 0 ? NF : 0)>(q, s_ptab, s_cbf, s_pair, wq, w2, s_wlut, ws, t, ok);
 	};
 	auto flush = [&](int c) {
 		long long *dst = P.acc + (uint64_t)ACC_PER_CAND * c;
@@ -445,7 +539,8 @@ k_reward9q(const KqParams P) {
 				for (int k = 0; k < 4; k++) {
 					const int e = (4 * g + k) * Cfg::NCONS + tid;              // 8 B / 4 B lane stride: conflict-free
 					uint32_t ok;
-					evalq(sq[e], sd[e], sl[e], ws4[k], t4[k], ok);
+					if constexpr (W) evalw(sq[e], ws4[k], t4[k], ok);
+					else evalq(sq[e], sd[e], sl[e], ws4[k], t4[k], ok);
 					cnt += ok;
 				}
 				const bool generic = !RECIP && ((__double2hiint(t4[0].y) | __double2hiint(t4[1].y) |
@@ -465,7 +560,8 @@ k_reward9q(const KqParams P) {
 				const int e = k * Cfg::NCONS + tid;
 				if (e < n) {
 					double ws; double2 t; uint32_t ok;
-					evalq(sq[e], sd[e], sl[e], ws, t, ok);
+					if constexpr (W) evalw(sq[e], ws, t, ok);
+					else evalq(sq[e], sd[e], sl[e], ws, t, ok);
 					const long long x = to_fx(div_lut<RECIP>(ws, t));
 					fx_domain_acc(dom, x);
 					acc.add(x);
@@ -482,16 +578,16 @@ k_reward9q(const KqParams P) {
 	if (P.corpus_on) corpus_tail(P.corpus, s_ex, s_last, reinterpret_cast<unsigned long long *>(smem), 2048u);     // block-wide; stage 0 is free: scratch
 }
 
-template <int CW, int EPT, int STAGES, int NF = -1>
+template <int CW, int EPT, int STAGES, int NF = -1, bool W = false>
 static cudaError_t launch_kq(const KqParams &P, int grid, bool recip, cudaStream_t st) {
-	using Cfg = KqCfg<CW, EPT, STAGES>;
+	using Cfg = KqCfg<CW, EPT, STAGES, W>;
 	cudaError_t err;
 	if (recip) {
-		auto k = k_reward9q<CW, EPT, STAGES, true, NF>;
+		auto k = k_reward9q<CW, EPT, STAGES, true, NF, W>;
 		if ((err = allow_big_smem(k, Cfg::SMEM)) != cudaSuccess) return err;
 		k<<<grid, (CW + 2) * 32, Cfg::SMEM, st>>>(P);
 	} else {
-		auto k = k_reward9q<CW, EPT, STAGES, false, NF>;
+		auto k = k_reward9q<CW, EPT, STAGES, false, NF, W>;
 		if ((err = allow_big_smem(k, Cfg::SMEM)) != cudaSuccess) return err;
 		k<<<grid, (CW + 2) * 32, Cfg::SMEM, st>>>(P);
 	}
@@ -507,8 +603,12 @@ int kq_tile_evals(int variant) {
 	}
 }
 
+// Form W: 8 B per evaluation leave room for a deeper ring than Form Q's two 70 KB stages
+constexpr int KW_CW = 20, KW_EPT = 8, KW_STAGES = 4;
+int kw_tile_evals() { return KqCfg<KW_CW, KW_EPT, KW_STAGES, true>::TILE; }
+
 cudaError_t run_reward9q(KqParams P, int variant, bool recip, int sm_count, cudaStream_t st) {
-	const int tile = kq_tile_evals(variant);
+	const int tile = P.qw ? kw_tile_evals() : kq_tile_evals(variant);
 	P.tiles_per_cand = (uint32_t)((P.T + tile - 1) / tile);
 	P.total_tiles = (uint64_t)P.tiles_per_cand * P.C;
 	if (P.total_tiles == 0) return cudaSuccess;
@@ -520,6 +620,10 @@ cudaError_t run_reward9q(KqParams P, int variant, bool recip, int sm_count, cuda
 		const int more = (int)(want < (uint64_t)sm_count ? want : (uint64_t)sm_count);
 		if (more > grid) grid = more;
 	}
+	// Form W: prefix table + the six other coded dimensions from product tables (NF = 0).  With 16-slot tables and one 8-byte
+	// stage read, the fp32 reads of NF = 3 (Form Q's default) no longer pay for their F2F + DMUL: 5.62 against 5.33 ms per
+	// flagship step on an H100 80GB HBM3 at 400 W (NF = 1: 5.48 / 5.97 ms)
+	if (P.qw) return launch_kq<KW_CW, KW_EPT, KW_STAGES, 0, true>(P, grid, recip, st);
 	switch (variant) {
 	case 1: return launch_kq<16, 8, 3>(P, grid, recip, st);
 	case 2: return launch_kq<24, 4, 4>(P, grid, recip, st);

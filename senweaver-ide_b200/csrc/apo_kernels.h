@@ -115,6 +115,10 @@ struct KqParams {
 	int corpus_on;                  // as K1Params
 	K2Params corpus;
 	uint32_t *bad;                  // as K1Params
+	// Form W (the 8-byte copy of a resident Form D tensor): one word per evaluation, eight 4-bit dense codes (15 = absent) in
+	// bits 0-31 and the fp32 tool_success_rate bit pattern in bits 32-63 (0x7FC00000 = absent).  Non-NULL: K1q reads this
+	// instead of q8 / d2 / li, with the mixed-lookup tables above.
+	const unsigned long long *qw;
 };
 // ---- categorical product table layout (built by apo_abi.cu build_luts, read by the kernels)
 constexpr int CAT_D01 = 0;    // [fb + 3*err + 6*ended] -> fl(fl(0 + d0*w0) + d1*w1)      (12)
@@ -134,8 +138,12 @@ constexpr int DIR_D8 = 152;   // [2][11] min(turns, 10); 0 = absent             
 constexpr int CAT_WORDS = 176;
 
 constexpr int KQ_PAIR_MAX = 1024;   // entries of the prefix table that fit its shared-memory slot
+constexpr uint32_t KW_D2_ABSENT = 0x7FC00000u;   // Form W: the one NaN pattern of an absent tool_success_rate
 int kq_tile_evals(int variant);
+int kw_tile_evals();                // K1q on Form W
 cudaError_t run_reward9q(KqParams P, int variant, bool recip, int sm_count, cudaStream_t st);
+// Form Q planes with dense codes < 15 in every coded dimension -> Form W words
+cudaError_t run_pack_w(const unsigned long long *q8, const float *d2, const unsigned short *li, uint64_t n, unsigned long long *qw, cudaStream_t st);
 cudaError_t run_transcode(const float *dims, uint64_t pitch_in, uint32_t C, uint64_t T, unsigned long long *q8, float *d2,
                           uint64_t pitch_out, uint32_t *codebook, uint32_t *overflow, cudaStream_t st);
 cudaError_t run_recode(unsigned long long *q8, float *d2, unsigned short *li, uint64_t n, const uint8_t *remap, cudaStream_t st);
@@ -188,7 +196,7 @@ cudaError_t run_reward9t(KtParams P, int sm_count, cudaStream_t st);
 constexpr int CB_DIM = 0;        // 9 x (l0, l1, l2, count): exact sum of rint(v * 2^52) over non-null evaluations where dim i is present
 constexpr int CB_TALLY = 36;     // total, good, bad
 constexpr int CB_INT = 39;
-enum CandSource { CAND_DIMS = 0, CAND_REC32 = 1, CAND_REC16 = 2, CAND_Q = 3, CAND_T = 4 };
+enum CandSource { CAND_DIMS = 0, CAND_REC32 = 1, CAND_REC16 = 2, CAND_Q = 3, CAND_T = 4, CAND_W = 5 };
 struct CandParams {
 	uint32_t C;
 	uint64_t T;                     // evaluations per candidate in this launch
@@ -198,7 +206,7 @@ struct CandParams {
 	const unsigned long long *q8;   // Form Q planes
 	const float *d2;
 	const unsigned short *li;
-	const float *cbf;               // Form Q: [8][256] code -> fp32 value
+	const float *cbf;               // Form Q / W: [8][256] code -> fp32 value
 	const unsigned short *tl;       // Form T planes + dictionary
 	const unsigned char *th;
 	const uint32_t *tb_pc;
@@ -209,6 +217,7 @@ struct CandParams {
 	const double *lut;              // natural-mask LUT [512] total weight (<= 0: finalReward null)
 	long long *ints;                // [C][CB_INT] of candidate 0 of this launch
 	unsigned long long *ex;         // [C][3] of candidate 0 of this launch
+	const unsigned long long *qw;   // Form W words (KqParams::qw)
 };
 cudaError_t run_cand_breakdown(const CandParams &P, int source, int sm_count, cudaStream_t st);
 // ints / ex: the whole buffer; partials: the scoring call's candidate accumulators (4 words per candidate)
