@@ -1099,7 +1099,7 @@ extern "C" int apo_create(int device, apo_engine **out) {
 		cudaDeviceGetAttribute(&mem_khz, cudaDevAttrMemoryClockRate, device);
 		cudaDeviceGetAttribute(&bus_bits, cudaDevAttrGlobalMemoryBusWidth, device);
 		cudaDeviceGetAttribute(&sm_khz, cudaDevAttrClockRate, device);
-		constexpr double kStreamFracOfPin = 0.90, kCompactFracOfPin = 0.61, kWordFracOfPin = 0.58 /* K1q on Form W: 2.0 TB/s of 3.35 on an H100 80GB HBM3 at 400 W */, kScanRecordsPerSmCycle = 1.0264e-2;
+		constexpr double kStreamFracOfPin = 0.90, kCompactFracOfPin = 0.61, kWordFracOfPin = 0.65 /* K1q on Form W: 2.19 TB/s of 3.35 on an H100 80GB HBM3 at 400 W */, kScanRecordsPerSmCycle = 1.0264e-2;
 		if (mem_khz > 0 && bus_bits > 0) {
 			const double pin_bytes_per_ms = 2.0 * (double)mem_khz * (double)bus_bits / 8.0;     // kHz x bytes = bytes per ms
 			e->stream_bytes_per_ms = kStreamFracOfPin * pin_bytes_per_ms;

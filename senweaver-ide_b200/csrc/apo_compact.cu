@@ -302,21 +302,19 @@ cudaError_t run_decode(const unsigned long long *q8, const float *d2, const unsi
 struct QMeta { int32_t cand; int32_t n; };
 
 // W: the stage holds Form W words (8 B per evaluation, one bulk copy) instead of the three Form Q planes (14 B, three copies),
-// and the code tables have 16 slots per coded dimension (slot 15 = absent = +0.0).
+// and the code tables live in the static KwTables (kw_tab) instead of the dynamic layout.
 template <int CW, int EPT, int STAGES, bool W = false>
 struct KqCfg {
 	static constexpr int NCONS = CW * 32;
 	static constexpr int TILE = NCONS * EPT;
 	static constexpr int Q8_BYTES = TILE * 8, D2_BYTES = W ? 0 : TILE * 4, LI_BYTES = W ? 0 : TILE * 2;
 	static constexpr int STAGE_BYTES = Q8_BYTES + D2_BYTES + LI_BYTES;
-	static constexpr int NCODE = W ? 16 : 256;                    // table slots per coded dimension
 	static constexpr int LUT_OFF = STAGES * STAGE_BYTES;          // double2[512]
-	static constexpr int PTAB_OFF = LUT_OFF + 512 * 16;           // double[8][NCODE]
-	static constexpr int CBF_OFF = PTAB_OFF + 8 * NCODE * 8;      // float[8][NCODE] code -> value (mixed-lookup variants)
-	static constexpr int PAIR_OFF = CBF_OFF + 8 * NCODE * 4;      // double[KQ_PAIR_MAX] exact prefix fl(fl(0 + d0*w0) + d1*w1); W: [16][16]
-	static constexpr int CAT_OFF = PAIR_OFF + (W ? 256 : KQ_PAIR_MAX) * 8;   // categorical product table of the fused corpus scan
-	static constexpr int WLUT_OFF = CAT_OFF + CAT_WORDS * 8;      // W: double2[512] indexed by w_lut_key (the corpus warp keeps LUT_OFF)
-	static constexpr int BAR_OFF = WLUT_OFF + (W ? 512 * 16 : 0);
+	static constexpr int PTAB_OFF = LUT_OFF + 512 * 16;           // double[8][256]
+	static constexpr int CBF_OFF = PTAB_OFF + (W ? 0 : 8 * 256 * 8);        // float[8][256] code -> value (mixed-lookup variants)
+	static constexpr int PAIR_OFF = CBF_OFF + (W ? 0 : 8 * 256 * 4);        // double[KQ_PAIR_MAX] exact prefix fl(fl(0 + d0*w0) + d1*w1)
+	static constexpr int CAT_OFF = PAIR_OFF + (W ? 0 : KQ_PAIR_MAX * 8);    // categorical product table of the fused corpus scan
+	static constexpr int BAR_OFF = CAT_OFF + CAT_WORDS * 8;
 	static constexpr int META_OFF = BAR_OFF + 2 * STAGES * 8;
 	static constexpr int EX_OFF = META_OFF + STAGES * 8;
 	static constexpr int SMEM = EX_OFF + 18 * 8 + 16;
@@ -373,42 +371,80 @@ __device__ __forceinline__ void evalq_ws_mixed(unsigned long long q, float d2f, 
 	valid = t_out.x > 0.0 ? 1u : 0u;
 }
 
-// Form W's LUT order: the presence bits as K1q derives them from a word, i.e. coded dimensions 4-7 (dims 5-8, the ones that
-// vary independently: lanes with different masks mostly hit different banks, as with lut_index) in bits 0-3, coded dimensions
-// 0-3 (dims 0, 1, 3, 4) in bits 4-7, dimension 2 in bit 8.  natural_mask: bit = dimension.
-__device__ __forceinline__ uint32_t w_lut_key(uint32_t m) {
-	return ((m >> 5) & 15u) | ((m & 3u) << 4) | (((m >> 3) & 3u) << 6) | (((m >> 2) & 1u) << 8);
+// Form W's code tables, in static shared memory.  ptab: value*weight by code for coded dimensions 2-7 (slot 15 = absent =
+// +0.0), pair: the exact prefix fl(fl(0 + d0*w0) + d1*w1) indexed by the two low nibbles of a word, lut: double2[512]
+// indexed by kw_key (the corpus warp keeps its own lut_index copy in the dynamic layout).  ptab comes first and the block is
+// 256-byte aligned, so a product-table address is the block's address with its low byte replaced by 8 * code (kw_addr).
+struct KwTables {
+	double ptab[6][16];
+	double pair[256];
+	double2 lut[512];
+};
+__shared__ __align__(256) KwTables kw_tab;
+
+// Form W's LUT order: the key the multiply-gather of evalw_ws yields.  Key bit r takes coded dimension 6 - 2r and bit r + 4
+// coded dimension 7 - 2r (r = 0..3), bit 8 dimension 2: bits 0-2 hold dims 7, 5 and 3 (tokens, duration, tool use: the
+// presences that vary in real data), so lanes with different masks mostly read different banks of an LDS.128 quarter-warp.
+// natural_mask: bit = dimension; coded dimension k is dimension k < 2 ? k : k + 1.
+__device__ __forceinline__ uint32_t kw_key(uint32_t natural_mask) {
+	uint32_t key = ((natural_mask >> 2) & 1u) << 8;
+#pragma unroll
+	for (int r = 0; r < 4; r++) {
+		const int lo = 6 - 2 * r, hi = 7 - 2 * r;                    // coded dimensions
+		key |= ((natural_mask >> (lo < 2 ? lo : lo + 1)) & 1u) << r;
+		key |= ((natural_mask >> (hi < 2 ? hi : hi + 1)) & 1u) << (r + 4);
+	}
+	return key;
 }
 
-// The same key from the nibble word of an evaluation (nibble 15 = absent) and the presence of its tool_success_rate.
-__device__ __forceinline__ uint32_t w_key_of(uint32_t w, bool p2) {
-	const uint32_t r = ~__funnelshift_l(w, w, 16);                   // coded dimensions 4-7 first; a nibble is zero iff absent
-	uint32_t z = (r | (r >> 1) | (r >> 2) | (r >> 3)) & 0x11111111u;  // bit 4k: nibble k present
-	z = (z | (z >> 3)) & 0x03030303u;                                 // gather the eight bits: 2 per byte, 4 per half, 8
-	z = (z | (z >> 6)) & 0x000F000Fu;
-	z = (z | (z >> 12)) & 0xFFu;
-	return z | (p2 ? 256u : 0u);
+// Slot of prefix entry i = c0 + 16 c1 (the low byte of a word): row c1, column c0 ^ 4 (c1 & 3).  Real data has <= 3 codes in
+// dimension 0 and <= 4 in dimension 1; unswizzled, lanes with one c0 and different c1 would share a bank.
+__device__ __forceinline__ uint32_t kw_pair_slot(uint32_t i) { return i ^ ((i >> 2) & 12u); }
+
+// byte J of `offs` under the three high bytes of the 256-byte aligned shared address `base`: one PRMT, no add
+template <int J>
+__device__ __forceinline__ uint32_t kw_addr(uint32_t offs, uint32_t base) {
+	uint32_t r;
+	asm("prmt.b32 %0, %1, %2, %3;" : "=r"(r) : "r"(offs), "r"(base), "n"(0x7650 | J));
+	return r;
 }
 
-// Mixed-lookup evaluation of one Form W word: the operations and their order are those of evalq_ws_mixed.  The prefix
-// table is [16][16] indexed by the two low nibbles (absent rows / columns hold the absent entries), the others [8][16].
-template <int NF>
-__device__ __forceinline__ void evalw_ws_mixed(unsigned long long q, const double *ptab, const float *cbf, const double *pair,
-                                               const double (&wq)[8], double w2, const double2 *wlut, double &ws_out, double2 &t_out,
-                                               uint32_t &valid) {
+// Loads from the shared state space at a 32-bit address (smem_u32), so that a constant offset becomes the LDS immediate.
+__device__ __forceinline__ double lds_f64(uint32_t a) {
+	double v;
+	asm("ld.shared.f64 %0, [%1];" : "=d"(v) : "r"(a));
+	return v;
+}
+__device__ __forceinline__ double2 lds_f64x2(uint32_t a) {
+	double2 v;
+	asm("ld.shared.v2.f64 {%0, %1}, [%2];" : "=d"(v.x), "=d"(v.y) : "r"(a));
+	return v;
+}
+
+// One Form W word: the operations and their order are those of evalq_ws_mixed with NF = 0 (prefix table, fl(d2*w2), the six
+// other coded dimensions from product tables).  Integer work: the six product-table addresses come from two masked copies of
+// the word, one PRMT each; the LUT entry from a carry test per nibble and one multiply-gather.  tab = smem_u32(&kw_tab).
+__device__ __forceinline__ void evalw_ws(unsigned long long q, double w2, uint32_t tab, double &ws_out, double2 &t_out, uint32_t &valid) {
+	constexpr uint32_t PAIR = offsetof(KwTables, pair), LUT = offsetof(KwTables, lut);
 	const uint32_t w = (uint32_t)q;
 	const float d2 = __uint_as_float((uint32_t)(q >> 32));
 	const bool p2 = d2 == d2;                                         // absent = NaN
-	double ws = pair[w & 255u];
+	const uint32_t ev = (w << 3) & 0x78787878u;                      // byte k: 8 * nibble 2k
+	const uint32_t od = (w >> 1) & 0x78787878u;                      // byte k: 8 * nibble 2k + 1
+	double ws = lds_f64(tab + PAIR + kw_pair_slot(w & 255u) * 8u);
 	ws = __dadd_rn(ws, __dmul_rn((double)(p2 ? d2 : 0.0f), w2));    // +0.0 when absent, as Form Q stores it
-#pragma unroll
-	for (int j = 2; j < 8; j++) {
-		const uint32_t code = (w >> (4 * j)) & 15u;
-		if (j - 2 < NF) ws = __dadd_rn(ws, __dmul_rn((double)cbf[j * 16 + code], wq[j]));
-		else ws = __dadd_rn(ws, ptab[j * 16 + code]);
-	}
+	ws = __dadd_rn(ws, lds_f64(kw_addr<1>(ev, tab) + 0 * 128));      // coded dimension 2 = nibble 2
+	ws = __dadd_rn(ws, lds_f64(kw_addr<1>(od, tab) + 1 * 128));
+	ws = __dadd_rn(ws, lds_f64(kw_addr<2>(ev, tab) + 2 * 128));
+	ws = __dadd_rn(ws, lds_f64(kw_addr<2>(od, tab) + 3 * 128));
+	ws = __dadd_rn(ws, lds_f64(kw_addr<3>(ev, tab) + 4 * 128));
+	ws = __dadd_rn(ws, lds_f64(kw_addr<3>(od, tab) + 5 * 128));
 	ws_out = ws;
-	t_out = wlut[w_key_of(w, p2)];
+	// nibble k is 15 (absent) iff its low three bits carry into bit 3 on + 1 and bit 3 is set; present flags land on bits 4k
+	const uint32_t pres = (~(((w & 0x77777777u) + 0x11111111u) & w) & 0x88888888u) >> 3;
+	// bits 4k times 2^0 + 2^9 + 2^18 + 2^27 land on 64 distinct positions (no carries); bits 24-31 are the kw_key byte
+	const uint32_t key8 = (pres * 0x08040201u) >> 24;
+	t_out = lds_f64x2(key8 * 16u + (tab + LUT + (p2 ? 256u * 16u : 0u)));
 	valid = t_out.x > 0.0 ? 1u : 0u;
 }
 
@@ -416,7 +452,7 @@ template <int CW, int EPT, int STAGES, bool RECIP, int NF = -1, bool W = false>
 __global__ void __launch_bounds__((CW + 2) * 32, 1)
 k_reward9q(const KqParams P) {
 	using Cfg = KqCfg<CW, EPT, STAGES, W>;
-	static_assert(!W || NF >= 0, "Form W runs the mixed-lookup form only");
+	static_assert(!W || NF == 0, "Form W runs the prefix-table form only");
 	extern __shared__ __align__(128) uint8_t smem[];
 	double2 *s_lut = reinterpret_cast<double2 *>(smem + Cfg::LUT_OFF);
 	double *s_ptab = reinterpret_cast<double *>(smem + Cfg::PTAB_OFF);
@@ -429,21 +465,15 @@ k_reward9q(const KqParams P) {
 	unsigned long long *s_ex = reinterpret_cast<unsigned long long *>(smem + Cfg::EX_OFF);
 	bool *s_last = reinterpret_cast<bool *>(smem + Cfg::EX_OFF + 18 * 8);
 
-	double2 *s_wlut = reinterpret_cast<double2 *>(smem + Cfg::WLUT_OFF);
-
 	const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
 	for (int i = tid; i < 512; i += blockDim.x) s_lut[lut_index(i)] = make_double2(P.lut[i], P.lut[512 + i]);
 	if constexpr (W) {
 		// the host's [8][256] tables (dense codes < 15; slot 255 = absent = +0.0) cut to 16 slots, slot 15 = absent
-		for (int i = tid; i < 512; i += blockDim.x) s_wlut[w_lut_key(i)] = make_double2(P.lut[i], P.lut[512 + i]);
-		for (int i = tid; i < 8 * 16; i += blockDim.x) {
-			const int src = (i >> 4) * 256 + ((i & 15) < 15 ? (i & 15) : 255);
-			s_ptab[i] = P.ptab[src];
-			if (NF > 0) s_cbf[i] = P.cbf[src];
-		}
+		for (int i = tid; i < 512; i += blockDim.x) kw_tab.lut[kw_key(i)] = make_double2(P.lut[i], P.lut[512 + i]);
+		for (int i = tid; i < 6 * 16; i += blockDim.x) kw_tab.ptab[i >> 4][i & 15] = P.ptab[((i >> 4) + 2) * 256 + ((i & 15) < 15 ? (i & 15) : 255)];
 		for (int i = tid; i < 256; i += blockDim.x) {                  // [c1][c0]: index = the two low nibbles of a word
 			const uint32_t c0 = min((uint32_t)i & 15u, P.n0), c1 = min((uint32_t)i >> 4, P.n1);
-			s_pair[i] = P.pair[c0 * (P.n1 + 1u) + c1];
+			kw_tab.pair[kw_pair_slot(i)] = P.pair[c0 * (P.n1 + 1u) + c1];
 		}
 	} else {
 	for (int i = tid; i < 8 * 256; i += blockDim.x) s_ptab[i] = P.ptab[i];
@@ -510,9 +540,8 @@ k_reward9q(const KqParams P) {
 		if (NF >= 0) evalq_ws_mixed<(NF >= 0 ? NF : 0)>(q, d2f, idx, s_ptab, s_cbf, s_pair, n0, n1, wq, w2, s_lut, ws, t, ok);
 		else evalq_ws(q, d2f, idx, s_ptab, w2, s_lut, ws, t, ok);
 	};
-	auto evalw = [&](unsigned long long q, double &ws, double2 &t, uint32_t &ok) {
-		evalw_ws_mixed<(NF >= 0 ? NF : 0)>(q, s_ptab, s_cbf, s_pair, wq, w2, s_wlut, ws, t, ok);
-	};
+	const uint32_t tab = smem_u32(&kw_tab);
+	auto evalw = [&](unsigned long long q, double &ws, double2 &t, uint32_t &ok) { evalw_ws(q, w2, tab, ws, t, ok); };
 	auto flush = [&](int c) {
 		long long *dst = P.acc + (uint64_t)ACC_PER_CAND * c;
 		flush_acc128(acc, dst, lane);
