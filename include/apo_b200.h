@@ -328,6 +328,27 @@ int apo_score_host_tuples(apo_engine *e, const apo_score_opts *o, const uint16_t
                           uint32_t C, uint64_t T, double *scores, uint64_t *counts, int32_t *topk, apo_corpus_report *report);
 int apo_tuples_upload(apo_engine *e, const uint16_t *tl, const uint8_t *th, const uint32_t *tbook_pc, const uint16_t *tbook_pd,
                       uint32_t n_tuples, const uint32_t *codebook, const uint32_t *d2book, uint32_t C, uint64_t T);
+/* Form T built on the device from the loaded evaluations, without a host round trip.  It leaves the engine exactly as
+ * apo_tuples_upload would with the planes, dictionary and n_tuples that apo_tuple_encode_host makes of this tensor's Form P
+ * planes, and with the codebook and d2book that go with them (the tensor's own: apo_dims_codebook / apo_dims_d2book of its
+ * Form Q layout).  Dictionary order: most frequent first, ties by key (code word | d2book index << 32) ascending; the bytes
+ * are the same for every grid.  It reads the Form W copy that apo_dims_upload / apo_dims_generate keep of categorical dims, or
+ * a Form Q layout or copy whose coded dimensions take <= 15 values each.  Afterwards source APO_SRC_TUPLES scores the result;
+ * the loaded dims, their copy and their scoring are untouched, and the tuples stay loaded, independent of later dims loads,
+ * until the next apo_tuples_upload or apo_dims_tuples.  The build is rank-local: each shard gets its own dictionary.
+ * cap is clamped to APO_TUPLES_MAX.  APO_E_STATE, with nothing built, when: no dims are loaded; Form D is loaded without a
+ * copy (APO_TUNE_NO_TWIN, apo_dims_attach, too little device memory at load: call apo_dims_compact first); a coded
+ * dimension takes 16 or more values; tool_success_rate takes more than 4095 values; the evaluations hold more than cap
+ * distinct ones (*n_tuples then receives a lower bound greater than cap, as from apo_tuple_encode_host).  APO_E_NOMEM when
+ * the build's own allocations released the copy it reads.  After any failure no Form T is loaded; the dims are untouched.
+ * Device scratch of the build (a hash table sized from min(cap, C*T), ~16 B per possible entry) is released on return. */
+int apo_dims_tuples(apo_engine *e, uint32_t cap, uint32_t *n_tuples);
+/* Rows of the resident Form T tensor (built or uploaded): tl / th of candidate c, records [first, first + n). */
+int apo_tuples_download(apo_engine *e, uint16_t *tl, uint8_t *th, uint32_t c, uint64_t first, uint64_t n);
+/* Its dictionary and codebooks.  *n_tuples always receives n; the entries are written only when cap >= n (APO_E_ARG
+ * otherwise). */
+int apo_tuples_book(apo_engine *e, uint32_t *tbook_pc, uint16_t *tbook_pd, uint32_t cap,
+                    uint32_t *codebook /* [8*256] */, uint32_t *d2book /* [4096] */, uint32_t *n_tuples);
 /* Host buffers for the streaming calls and the uploads.  Any host pointer is accepted: pageable memory (malloc, a JS
  * ArrayBuffer, numpy) is gathered chunk by chunk into pinned staging buffers by a few host threads while
  * the previous chunk is on the wire; memory from apo_host_alloc (page-locked) is read in place and

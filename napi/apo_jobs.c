@@ -99,6 +99,9 @@ int apo_job_validate(apo_job *j)
 	case APO_JOB_COMM_INIT:
 		if (j->nranks < 1 || j->rank < 0 || j->rank >= j->nranks) return bad(j, "bad rank / nranks");
 		break;
+	case APO_JOB_DIMS_TUPLES:
+		if (j->cap > APO_TUPLES_MAX) return bad(j, "cap exceeds 16777215 dictionary entries");
+		break;
 	case APO_JOB_TEST_HOOK:
 		break;
 	default:
@@ -210,6 +213,12 @@ static void execute(apo_serial *s, apo_job *j)
 	case APO_JOB_COMM_INIT:
 		j->rc = apo_comm_init(e, j->nranks, j->rank, j->comm_id);
 		break;
+	case APO_JOB_DIMS_TUPLES: {
+		uint32_t n = 0;
+		j->rc = apo_dims_tuples(e, j->cap, &n);
+		j->n_out = n;
+		break;
+	}
 	default:
 		j->rc = APO_E_ARG;
 	}

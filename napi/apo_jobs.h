@@ -49,7 +49,8 @@ typedef enum {
 	APO_JOB_SCORE_HOST_TUPLES,     /* scoreHostTuples(handle, {tl, th, tbookPc, tbookPd, codebook, d2book}, C, T, corpus|null, K, candidates?) */
 	APO_JOB_REWARD_BATCH,          /* rewardBatch(handle, recs apo_record[n])                    */
 	APO_JOB_COMM_INIT,             /* commInit(handle, nranks, rank, id[128])                    */
-	APO_JOB_TEST_HOOK              /* tests: calls hook(hook_arg) in its turn                    */
+	APO_JOB_TEST_HOOK,             /* tests: calls hook(hook_arg) in its turn                    */
+	APO_JOB_DIMS_TUPLES            /* dimsTuples(handle, cap?) -> nTuples: resident Form T built from the loaded dims */
 } apo_job_kind;
 
 typedef struct apo_job {
@@ -60,6 +61,7 @@ typedef struct apo_job {
 	const void *corpus; uint64_t corpus_bytes;    /* optional apo_record[Tc] uploaded before a host scoring call */
 	const void *aux[5]; uint64_t aux_bytes[5];    /* Form T: th plane, tbook_pc, tbook_pd, codebook (8 x 256 u32), d2book (4096 u32); buf = tl plane */
 	uint32_t n_tuples;
+	uint32_t cap;                                 /* dimsTuples: dictionary capacity, <= APO_TUPLES_MAX */
 	uint32_t C, K, row_bytes, source, flags;
 	uint64_t T, first, count, idx_base;
 	int compact;

@@ -25,6 +25,7 @@
  *   rolloutsUpload(h, recs:ArrayBuffer, rowBytes 32|16, C, T)               -> Promise<void>
  *   corpusUpload(h, recs:ArrayBuffer apo_record[T], idxBase)                -> Promise<void>
  *   corpusUploadJson(h, utf8:ArrayBuffer, idxBase)                          -> Promise<number>   (records)
+ *   dimsTuples(h, cap?)                                                     -> Promise<number>   (nTuples) resident Form T from the loaded dims
  *   scoreResident(h, {C, K, source, corpus, first, count, candidates, candidateCorpus}) -> Promise<blocks>   ... scored many times
  *   score(h, dims, C, T, corpus|null, K, candidates?)                       -> Promise<blocks>   host streaming, Form D
  *   scoreHostRecords(h, recs, rowBytes, C, T, corpus|null, K, candidates?, candidateCorpus?) -> Promise<blocks>   host streaming, trace records
@@ -164,7 +165,7 @@ static void call_complete(napi_env env, napi_status st, void *data)
 			if ((v = copy_out(env, j->masks_out, 4u * (size_t)j->n_out))) napi_set_named_property(env, out, "masks", v);
 			if ((v = copy_out(env, j->finals_out, 8u * (size_t)j->n_out))) napi_set_named_property(env, out, "finals", v);
 			break;
-		case APO_JOB_CORPUS_UPLOAD_JSON:
+		case APO_JOB_CORPUS_UPLOAD_JSON: case APO_JOB_DIMS_TUPLES:
 			napi_create_double(env, (double)j->n_out, &out);
 			break;
 		default:
@@ -291,6 +292,18 @@ static napi_value CorpusUploadJson(napi_env env, napi_callback_info info)
 	if (argc < 2 || !get_buffer(env, argv[1], &c->job.buf, &c->job.buf_bytes)) arg_error(c, "corpusUploadJson(handle, utf8:ArrayBuffer, idxBase?:uint53)");
 	if (argc >= 3 && argv[2] && !is_nullish(env, argv[2]) && !get_u64(env, argv[2], &c->job.idx_base)) arg_error(c, "corpusUploadJson: idxBase must be a non-negative integer");
 	return submit(env, c, argv[0], c->job.buf ? argv[1] : NULL, NULL, "apo_corpus_upload_json");
+}
+
+/* dimsTuples(h, cap?) -> Promise<number of dictionary entries>: apo_dims_tuples, cap defaults to APO_TUPLES_MAX */
+static napi_value DimsTuples(napi_env env, napi_callback_info info)
+{
+	ARGS(2)
+	call_t *c = argc >= 1 ? new_call(env, argv[0], APO_JOB_DIMS_TUPLES) : NULL;
+	if (!c) return reject_now(env, "dimsTuples: invalid handle");
+	c->job.cap = APO_TUPLES_MAX;
+	if (argc >= 2 && argv[1] && !is_nullish(env, argv[1]) && !get_u32(env, argv[1], &c->job.cap))
+		arg_error(c, "dimsTuples(handle, cap?:uint32 <= 16777215)");
+	return submit(env, c, argv[0], NULL, NULL, "apo_dims_tuples");
 }
 
 static int opt_u32(napi_env env, napi_value obj, const char *key, uint32_t *out)
@@ -549,6 +562,7 @@ NAPI_MODULE_INIT()
 	    {"rolloutsUpload", NULL, RolloutsUpload, NULL, NULL, NULL, napi_default, NULL},
 	    {"corpusUpload", NULL, CorpusUpload, NULL, NULL, NULL, napi_default, NULL},
 	    {"corpusUploadJson", NULL, CorpusUploadJson, NULL, NULL, NULL, napi_default, NULL},
+	    {"dimsTuples", NULL, DimsTuples, NULL, NULL, NULL, napi_default, NULL},
 	    {"scoreResident", NULL, ScoreResident, NULL, NULL, NULL, napi_default, NULL},
 	    {"score", NULL, Score, NULL, NULL, NULL, napi_default, NULL},
 	    {"scoreHostRecords", NULL, ScoreHostRecords, NULL, NULL, NULL, napi_default, NULL},

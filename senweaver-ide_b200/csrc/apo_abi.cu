@@ -110,6 +110,8 @@ struct apo_engine {
 	DevBuf<uint32_t> tup_pc, tup_bad; DevBuf<unsigned short> tup_pd; DevBuf<float> tup_d2; DevBuf<double> tup_ptab; DevBuf<long long> tup_val;
 	uint32_t tup_book[8 * 256]; bool tup_used = false;
 	DevBuf<uint32_t> tups_pc; DevBuf<unsigned short> tups_pd; DevBuf<float> tups_d2;   // dictionary of a host-streaming call
+	// apo_dims_tuples scratch (released when the build returns): hash table, (key, count) pairs / keys in rank order, counters
+	DevBuf<unsigned long long> tb_table, tb_keys, tb_cnt, tb_misc;
 
 	// acc: [acc_words(C, nranks)] partial vector | [18] example scratch (inverted indices) | [1] ticket — one allocation, so one
 	// memset arms a scoring call.  acc_joined: the joined vector (> 1 rank); acc keeps this rank's partials.
@@ -1764,6 +1766,13 @@ extern "C" int apo_dims_compact_download(apo_engine *e, uint64_t *q8, float *d2,
 }
 
 namespace {
+// order of a d2book: by value, -0.0 (sign bit set) before +0.0
+bool d2_before(uint32_t x, uint32_t y) {
+	float fx, fy; memcpy(&fx, &x, 4); memcpy(&fy, &y, 4);
+	if (fx != fy) return fx < fy;
+	return x > y;
+}
+
 // d2book of the resident Form Q tensor: distinct tool_success_rate values ordered by value (built once per loaded tensor)
 int ensure_d2book(apo_engine *e) {
 	if (e->d2book_n != ~0u) return APO_OK;
@@ -1780,11 +1789,7 @@ int ensure_d2book(apo_engine *e) {
 	if (host[16384] > 4095) return fail(e, APO_E_STATE, "tool_success_rate takes %u distinct values: more than the 4095 Form P can index", host[16384]);
 	std::vector<uint32_t> vals;
 	for (int i = 0; i < 16384; i++) if (host[i] != 0xFFFFFFFFu) vals.push_back(host[i]);
-	std::sort(vals.begin(), vals.end(), [](uint32_t x, uint32_t y) {
-		float fx, fy; memcpy(&fx, &x, 4); memcpy(&fy, &y, 4);
-		if (fx != fy) return fx < fy;
-		return x > y;
-	});
+	std::sort(vals.begin(), vals.end(), d2_before);
 	for (size_t c = 0; c < 4096; c++) e->d2book_host[c] = c < vals.size() ? vals[c] : 0xFFFFFFFFu;
 	CK(reserve(e, e->d_d2book, 4096));
 	CK(cudaMemcpyAsync(e->d_d2book.p, e->d2book_host, 4096 * 4, cudaMemcpyHostToDevice, e->stream));
@@ -1878,6 +1883,160 @@ extern "C" int apo_tuples_upload(apo_engine *e, const uint16_t *tl, const uint8_
 	CK(cudaStreamSynchronize(e->stream));
 	memcpy(e->tup_book, codebook, sizeof e->tup_book);
 	e->tup_C = C; e->tup_T = T; e->tup_pitch = pitch; e->tup_n = n_tuples;
+	return APO_OK;
+}
+
+namespace {
+template <class T>
+int tb_reserve(apo_engine *e, DevBuf<T> &b, uint64_t n, const char *what) {
+	const cudaError_t c = reserve(e, b, n);
+	if (c == cudaSuccess) return APO_OK;
+	cudaGetLastError();
+	return fail(e, c == cudaErrorMemoryAllocation ? APO_E_NOMEM : APO_E_CUDA, "%s (%llu elements): %s", what, (unsigned long long)n, cudaGetErrorString(c));
+}
+
+int dims_tuples(apo_engine *e, uint32_t cap, uint32_t *n_tuples) {
+	if ((!e->dims_ptr && !e->compact) || e->dims_C == 0) return fail(e, APO_E_STATE, "no dims loaded");
+	if (!e->compact && (!e->twin || e->env_no_twin))
+		return fail(e, APO_E_STATE, "the loaded Form D tensor has no Form W / Q copy to build Form T from (APO_TUNE_NO_TWIN, apo_dims_attach, "
+		                            "or too little device memory at load): call apo_dims_compact first");
+	if (e->compact || !e->twin_w)
+		for (int j = 0; j < 8; j++)
+			if (e->qbook_host[256 * j + 15] != 0xFFFFFFFFu)
+				return fail(e, APO_E_STATE, "coded dimension %d takes 16 or more distinct values: Form T (like Form P) needs <= 15", j < 2 ? j : j + 1);
+	if (cap > APO_TUPLES_MAX) cap = APO_TUPLES_MAX;
+	const uint32_t C = e->dims_C;
+	const uint64_t T = e->dims_T, pitch = e->dims_pitch, N = (uint64_t)C * T;
+	const uint64_t m = std::min<uint64_t>(cap, N);                // at most this many dictionary entries
+	uint64_t slots = 1024;
+	while (slots < 2 * (m + 1)) slots <<= 1;
+	const uint64_t tpitch = round_up(T ? T : 1, 64);               // as apo_tuples_upload
+	// everything is allocated before the source is chosen: reserve may release the copy this build reads
+	int rc;
+	if ((rc = tb_reserve(e, e->tup_l, (uint64_t)C * tpitch, "Form T low plane")) || (rc = tb_reserve(e, e->tup_h, (uint64_t)C * tpitch, "Form T high plane")) ||
+	    (rc = tb_reserve(e, e->tup_pc, m ? m : 1, "dictionary")) || (rc = tb_reserve(e, e->tup_pd, m ? m : 1, "dictionary")) ||
+	    (rc = tb_reserve(e, e->tup_d2, 4096, "d2book")) || (rc = tb_reserve(e, e->tb_table, 2 * slots, "hash table")) ||
+	    (rc = tb_reserve(e, e->tb_keys, m ? m : 1, "keys")) || (rc = tb_reserve(e, e->tb_cnt, m ? m : 1, "counts")) ||
+	    (rc = tb_reserve(e, e->tb_misc, 4, "counters")))
+		return rc;
+	if (!e->compact && !e->twin)
+		return fail(e, APO_E_NOMEM, "device memory ran short: the Form W / Q copy of the loaded tensor was released to make room for the build; "
+		                            "free device memory and load the tensor again, or call apo_dims_compact");
+	apo::TbSource S{};
+	if (e->twin_w && !e->compact) S.qw = e->qw.p;
+	else { S.q8 = e->q8.p; S.d2 = e->qd2.p; S.li = e->qli.p; }
+	S.pitch = pitch; S.C = C; S.T = T;
+	unsigned long long *misc = e->tb_misc.p;                       // [0] keys inserted, [1] over flag / index miss, [2] compacted
+	CK(cudaMemsetAsync(misc, 0, 4 * 8, e->stream));
+	uint32_t n = 0;
+	std::vector<unsigned long long> keys, counts;
+	if (N) {
+		CK(apo::run_tb_clear(e->tb_table.p, slots, e->stream));
+		CK(apo::run_tb_count(S, e->tb_table.p, slots, cap, misc, (uint32_t *)(misc + 1), e->sm_count, e->stream));
+		unsigned long long h[2];
+		CK(cudaMemcpyAsync(h, misc, sizeof h, cudaMemcpyDeviceToHost, e->stream));
+		CK(cudaStreamSynchronize(e->stream));
+		if (h[1]) {
+			*n_tuples = h[0] > 0xFFFFFFFFull ? 0xFFFFFFFFu : (uint32_t)h[0];
+			return fail(e, APO_E_STATE, "the evaluations hold more than cap=%u distinct ones (at least %llu): keep Form W / Q", cap, h[0]);
+		}
+		n = (uint32_t)h[0];
+		CK(apo::run_tb_compact(e->tb_table.p, slots, e->tb_keys.p, e->tb_cnt.p, misc + 2, e->stream));
+		keys.resize(n); counts.resize(n);
+		CK(cudaMemcpyAsync(keys.data(), e->tb_keys.p, (uint64_t)n * 8, cudaMemcpyDeviceToHost, e->stream));
+		CK(cudaMemcpyAsync(counts.data(), e->tb_cnt.p, (uint64_t)n * 8, cudaMemcpyDeviceToHost, e->stream));
+		CK(cudaStreamSynchronize(e->stream));
+	}
+	// d2book: the distinct tool_success_rate values in ensure_d2book's order; a key's high half becomes its index
+	std::vector<uint32_t> d2;
+	for (uint32_t i = 0; i < n; i++) if ((uint32_t)(keys[i] >> 32) != apo::KW_D2_ABSENT) d2.push_back((uint32_t)(keys[i] >> 32));
+	std::sort(d2.begin(), d2.end());
+	d2.erase(std::unique(d2.begin(), d2.end()), d2.end());
+	if (d2.size() > 4095) return fail(e, APO_E_STATE, "tool_success_rate takes %zu distinct values: more than the 4095 Form T can index", d2.size());
+	std::sort(d2.begin(), d2.end(), d2_before);
+	uint32_t d2book[4096];
+	for (size_t c = 0; c < 4096; c++) d2book[c] = c < d2.size() ? d2[c] : 0xFFFFFFFFu;
+	// dictionary order: count desc, then tuple_key (code word | d2book index << 32) asc, as apo_tuple_encode_host
+	std::vector<std::pair<unsigned long long, unsigned long long>> order(n);     // (count, tuple key)
+	for (uint32_t i = 0; i < n; i++) {
+		const uint32_t hi = (uint32_t)(keys[i] >> 32);
+		const uint64_t pd = hi == apo::KW_D2_ABSENT ? 4095u : (uint64_t)(std::lower_bound(d2.begin(), d2.end(), hi, d2_before) - d2.begin());
+		order[i] = {counts[i], (keys[i] & 0xFFFFFFFFull) | (pd << 32)};
+	}
+	std::sort(order.begin(), order.end(), [](const std::pair<unsigned long long, unsigned long long> &x, const std::pair<unsigned long long, unsigned long long> &y) {
+		if (x.first != y.first) return x.first > y.first;
+		return x.second < y.second;
+	});
+	std::vector<uint32_t> tb_pc(n);
+	std::vector<uint16_t> tb_pd(n);
+	for (uint32_t r = 0; r < n; r++) {
+		const uint32_t pd = (uint32_t)(order[r].second >> 32);
+		tb_pc[r] = (uint32_t)order[r].second; tb_pd[r] = (uint16_t)pd;
+		keys[r] = (unsigned long long)tb_pc[r] | ((unsigned long long)(pd == 4095u ? apo::KW_D2_ABSENT : d2book[pd]) << 32);   // back to the evaluation key
+	}
+	CK(cudaMemcpyAsync(e->tup_d2.p, d2book, sizeof d2book, cudaMemcpyHostToDevice, e->stream));
+	if (n) {
+		CK(cudaMemcpyAsync(e->tup_pc.p, tb_pc.data(), (uint64_t)n * 4, cudaMemcpyHostToDevice, e->stream));
+		CK(cudaMemcpyAsync(e->tup_pd.p, tb_pd.data(), (uint64_t)n * 2, cudaMemcpyHostToDevice, e->stream));
+		CK(cudaMemcpyAsync(e->tb_keys.p, keys.data(), (uint64_t)n * 8, cudaMemcpyHostToDevice, e->stream));
+		// the index table holds only the dictionary (slots >= 2 n, so that it stays small enough for L2)
+		uint64_t islots = 1024;
+		while (islots < 2ull * n) islots <<= 1;
+		CK(apo::run_tb_clear(e->tb_table.p, islots, e->stream));
+		CK(apo::run_tb_insert(e->tb_keys.p, n, e->tb_table.p, islots, e->stream));
+		CK(apo::run_tb_index(S, e->tb_keys.p, n, e->tb_table.p, islots, e->tup_l.p, e->tup_h.p, tpitch, (uint32_t *)(misc + 1), e->sm_count, e->stream));
+	}
+	unsigned long long miss = 0;
+	CK(cudaMemcpyAsync(&miss, misc + 1, 8, cudaMemcpyDeviceToHost, e->stream));
+	CK(cudaStreamSynchronize(e->stream));
+	if (miss) return fail(e, APO_E_CUDA, "internal error: an evaluation's key is missing from the dictionary");
+	memcpy(e->tup_book, e->qbook_host, sizeof e->tup_book);
+	e->tup_C = C; e->tup_T = T; e->tup_pitch = tpitch; e->tup_n = n;
+	*n_tuples = n;
+	return APO_OK;
+}
+}  // namespace
+
+extern "C" int apo_dims_tuples(apo_engine *e, uint32_t cap, uint32_t *n_tuples) {
+	if (!e) return APO_E_ARG;
+	if (!n_tuples) return fail(e, APO_E_ARG, "n_tuples is NULL");
+	*n_tuples = 0;
+	CK(cudaSetDevice(e->device));
+	e->tup_C = 0; e->tup_T = 0; e->tup_n = 0;                      // a failure leaves no Form T loaded, as a failed apo_tuples_upload
+	const int rc = dims_tuples(e, cap, n_tuples);
+	if (rc != APO_OK) cudaStreamSynchronize(e->stream);           // nothing queued may still use the scratch when it is released
+	e->tb_table.release(); e->tb_keys.release(); e->tb_cnt.release(); e->tb_misc.release();
+	return rc;
+}
+
+extern "C" int apo_tuples_download(apo_engine *e, uint16_t *tl, uint8_t *th, uint32_t c, uint64_t first, uint64_t n) {
+	if (!e || !tl || !th) return fail(e, APO_E_ARG, "NULL argument");
+	if (e->tup_l.p == nullptr || e->tup_C == 0) return fail(e, APO_E_STATE, "no tuples loaded");
+	if (c >= e->tup_C || first > e->tup_T || n > e->tup_T - first) return fail(e, APO_E_ARG, "range outside the tuples");
+	if (n == 0) return APO_OK;
+	CK(cudaSetDevice(e->device));
+	const uint64_t off = (uint64_t)c * e->tup_pitch + first;
+	CK(cudaMemcpyAsync(tl, e->tup_l.p + off, n * 2, cudaMemcpyDeviceToHost, e->stream));
+	CK(cudaMemcpyAsync(th, e->tup_h.p + off, n, cudaMemcpyDeviceToHost, e->stream));
+	CK(cudaStreamSynchronize(e->stream));
+	return APO_OK;
+}
+
+extern "C" int apo_tuples_book(apo_engine *e, uint32_t *tbook_pc, uint16_t *tbook_pd, uint32_t cap, uint32_t *codebook, uint32_t *d2book,
+                               uint32_t *n_tuples) {
+	if (!e || !n_tuples) return fail(e, APO_E_ARG, "NULL argument");
+	if (e->tup_l.p == nullptr || e->tup_C == 0) return fail(e, APO_E_STATE, "no tuples loaded");
+	*n_tuples = e->tup_n;
+	if (cap < e->tup_n) return fail(e, APO_E_ARG, "cap=%u is smaller than the %u dictionary entries", cap, e->tup_n);
+	if (!codebook || !d2book || (e->tup_n && (!tbook_pc || !tbook_pd))) return fail(e, APO_E_ARG, "NULL argument");
+	CK(cudaSetDevice(e->device));
+	if (e->tup_n) {
+		CK(cudaMemcpyAsync(tbook_pc, e->tup_pc.p, (uint64_t)e->tup_n * 4, cudaMemcpyDeviceToHost, e->stream));
+		CK(cudaMemcpyAsync(tbook_pd, e->tup_pd.p, (uint64_t)e->tup_n * 2, cudaMemcpyDeviceToHost, e->stream));
+	}
+	CK(cudaMemcpyAsync(d2book, e->tup_d2.p, 4096 * 4, cudaMemcpyDeviceToHost, e->stream));
+	CK(cudaStreamSynchronize(e->stream));
+	memcpy(codebook, e->tup_book, sizeof e->tup_book);
 	return APO_OK;
 }
 

@@ -190,6 +190,34 @@ int kt_tile_evals();
 cudaError_t run_tuple_values(const TupleValParams &P, bool recip, cudaStream_t st);
 cudaError_t run_reward9t(KtParams P, int sm_count, cudaStream_t st);
 
+// Form T built on the device from a resident tensor's Form W words or Form Q planes (apo_dims_tuples).  The key of an
+// evaluation is its Form W word: eight 4-bit codes in the low half, the fp32 tool_success_rate bits (KW_D2_ABSENT = absent)
+// in the high half; the host maps the high half to the d2book index afterwards.  Hash tables hold {key, value} pairs,
+// TB_EMPTY = free (never a key: the high half of a key is a non-NaN value or KW_D2_ABSENT).
+constexpr unsigned long long TB_EMPTY = ~0ull;
+struct TbSource {
+	const unsigned long long *qw;   // Form W words, or NULL: Form Q planes q8 / d2 / li
+	const unsigned long long *q8;
+	const float *d2;
+	const unsigned short *li;
+	uint64_t pitch;                 // row pitch in evaluations, a multiple of 8
+	uint32_t C;
+	uint64_t T;                     // evaluations t >= T of a row are pads and are neither counted nor looked up
+};
+cudaError_t run_tb_clear(unsigned long long *table, uint64_t slots, cudaStream_t st);
+// table[slots] {key, count}: exact counts of the distinct keys; *nkeys = keys inserted, *over |= 1 once that exceeds cap
+// (the pass then stops early)
+cudaError_t run_tb_count(const TbSource &S, unsigned long long *table, uint64_t slots, uint64_t cap, unsigned long long *nkeys,
+                         uint32_t *over, int sm_count, cudaStream_t st);
+// the occupied slots of table as (key, count) pairs in any order; *n receives their number
+cudaError_t run_tb_compact(const unsigned long long *table, uint64_t slots, unsigned long long *keys, unsigned long long *counts,
+                           unsigned long long *n, cudaStream_t st);
+// table[slots] {key, rank} of keys[0, n) (keys in rank order), into a cleared table
+cudaError_t run_tb_insert(const unsigned long long *keys, uint32_t n, unsigned long long *table, uint64_t slots, cudaStream_t st);
+// tl / th [C][tpitch] = rank of every evaluation's key; *bad = 1 when a key is not in the table
+cudaError_t run_tb_index(const TbSource &S, const unsigned long long *keys, uint32_t n, const unsigned long long *table, uint64_t slots,
+                         unsigned short *tl, unsigned char *th, uint64_t tpitch, uint32_t *bad, int sm_count, cudaStream_t st);
+
 // ---- per-candidate breakdown (csrc/apo_cand.cu): a second pass over the evaluations a scoring call reads.
 // Own integer buffer, never part of the scoring accumulator vector: [C][CB_INT] words (a later cross-rank join is one
 // integer sum of this part) followed by the first-three 'bad' slots [nranks][C][3] (inverted indices as ex_insert keeps them).

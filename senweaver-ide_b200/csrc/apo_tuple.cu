@@ -11,6 +11,7 @@
 // k_tuple_values with exactly the operations of K1q (product-table lookups in push order, the same division, the same
 // rint(x * 2^52)), so summing table entries gives the integers K1 / K1q / the oracle produce: bit-exact by construction.
 // K1t then is a gather-and-add: the hot head of the table in shared memory, the tail through L1/L2.
+#include <cstdlib>
 #include "apo_device.cuh"
 #include "apo_kernels.h"
 
@@ -194,6 +195,273 @@ cudaError_t run_reward9t(KtParams P, int sm_count, cudaStream_t st) {
 	int grid = sm_count;
 	if ((uint64_t)grid > P.total_tiles) grid = (int)P.total_tiles;
 	k_reward9t<<<grid, KT_THREADS, smem, st>>>(P);
+	return cudaGetLastError();
+}
+
+// =================================================================== Form T built on the device (apo_dims_tuples)
+// Two passes over the resident evaluations, 8 per thread and step (one row segment of 64 B of Form W):
+//   count: exact counts of the distinct keys.  A warp first merges equal keys (match.any), then each CTA adds them into its
+//          own shared-memory table; a key that finds no room there (the CTA met more distinct keys than the table holds: the
+//          cold tail of the distribution) goes straight to the global table.  Generated data is heavily skewed, so nearly
+//          every evaluation ends in a shared-memory atomic and the global table sees one add per CTA and hot key.
+//   index: the rank of every evaluation's key, the hot head of the dictionary from a shared-memory table, the tail from the
+//          global one (which holds only the dictionary's entries, so it stays in L2), written as Form T's tl / th.
+// The dictionary order (count desc, key asc) is decided on the host from the exact counts: every grid gives the same bytes.
+constexpr int TB_THREADS = 512;
+constexpr int TB_GROUP = 8;                       // evaluations per thread and step
+constexpr uint32_t TB_CSLOTS = 8192;              // count pass: per-CTA table, 96 KB (8-byte keys, 4-byte counts)
+constexpr int TB_CPROBES = 8;                     // probes before a key goes to the global table
+constexpr uint32_t TB_ISLOTS = 8192;              // index pass: per-CTA table of the hot head, 96 KB
+constexpr uint32_t TB_IHOT = TB_ISLOTS / 2;       // dictionary entries in it (load 0.5: a miss ends after ~2.5 probes)
+
+__device__ __forceinline__ uint32_t tb_hash(unsigned long long k) {
+	uint32_t h = (uint32_t)k * 0x9E3779B1u ^ (uint32_t)(k >> 32) * 0x85EBCA77u;
+	h ^= h >> 15; h *= 0x2C1B3C6Du; h ^= h >> 12;
+	return h;
+}
+__device__ __forceinline__ uint32_t tb_shash(uint32_t h) { return (h * 0x9E3779B1u) >> 19; }   // 13 bits, independent of the low ones
+
+// keys of the 8 evaluations [t0, t0 + 8) of row c; bit q of the result set when t0 + q < T
+__device__ __forceinline__ uint32_t tb_keys(const TbSource &S, uint32_t c, uint64_t t0, unsigned long long k[TB_GROUP]) {
+	const uint64_t off = (uint64_t)c * S.pitch + t0;
+	if (S.qw) {
+#pragma unroll
+		for (int i = 0; i < TB_GROUP / 2; i++) {
+			const uint4 v = ld_stream16(S.qw + off + 2 * i);
+			k[2 * i] = (unsigned long long)v.x | ((unsigned long long)v.y << 32);
+			k[2 * i + 1] = (unsigned long long)v.z | ((unsigned long long)v.w << 32);
+		}
+	} else {
+		// k_pack_p's arithmetic: codes < 15 (checked on the host) and 255 = absent -> nibble 15; dimension 2 is bit 6 of li
+		const uint4 lv = ld_stream16(S.li + off);
+		const uint32_t lw[4] = {lv.x, lv.y, lv.z, lv.w};
+#pragma unroll
+		for (int h = 0; h < 2; h++) {
+			const uint4 dv = ld_stream16(S.d2 + off + 4 * h);
+			const uint32_t dw[4] = {dv.x, dv.y, dv.z, dv.w};
+#pragma unroll
+			for (int i = 0; i < 2; i++) {
+				const uint4 qv = ld_stream16(S.q8 + off + 4 * h + 2 * i);
+				const uint32_t qw[4] = {qv.x, qv.y, qv.z, qv.w};
+#pragma unroll
+				for (int e = 0; e < 2; e++) {
+					const int q = 4 * h + 2 * i + e;
+					uint32_t a = qw[2 * e] & 0x0F0F0F0Fu, b = qw[2 * e + 1] & 0x0F0F0F0Fu;
+					a = (a | (a >> 4)) & 0x00FF00FFu; a = (a | (a >> 8)) & 0xFFFFu;
+					b = (b | (b >> 4)) & 0x00FF00FFu; b = (b | (b >> 8)) & 0xFFFFu;
+					const uint32_t li = (lw[q >> 1] >> (16 * (q & 1))) & 0xFFFFu;
+					const uint32_t d = ((li >> 6) & 1u) ? dw[2 * i + e] : KW_D2_ABSENT;
+					k[q] = (unsigned long long)(a | (b << 16)) | ((unsigned long long)d << 32);
+				}
+			}
+		}
+	}
+	const uint64_t left = S.T - t0;
+	return left >= (uint64_t)TB_GROUP ? 0xFFu : (1u << left) - 1u;
+}
+
+__device__ __forceinline__ void tb_global_add(unsigned long long *table, uint32_t mask, unsigned long long k, unsigned long long n,
+                                              uint64_t cap, unsigned long long *nkeys, uint32_t *over) {
+	uint32_t h = tb_hash(k) & mask;
+	for (uint32_t p = 0; p <= mask; p++) {
+		unsigned long long *slot = table + 2ull * h;
+		unsigned long long cur = *(volatile unsigned long long *)slot;
+		if (cur == TB_EMPTY) {
+			cur = atomicCAS(slot, TB_EMPTY, k);
+			if (cur == TB_EMPTY) {
+				if (atomicAdd(nkeys, 1ull) + 1 > cap) atomicOr(over, 1u);
+				cur = k;
+			}
+		}
+		if (cur == k) { atomicAdd(slot + 1, n); return; }
+		h = (h + 1) & mask;
+	}
+	atomicOr(over, 1u);                           // the table is full: it holds more than cap keys
+}
+
+__global__ void __launch_bounds__(256)
+k_tb_clear(unsigned long long *table, uint64_t slots) {
+	for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < slots; i += (uint64_t)gridDim.x * blockDim.x)
+		reinterpret_cast<ulonglong2 *>(table)[i] = make_ulonglong2(TB_EMPTY, 0ull);
+}
+
+__global__ void __launch_bounds__(TB_THREADS, 2)
+k_tb_count(const TbSource S, unsigned long long *table, uint32_t mask, uint64_t cap, unsigned long long *nkeys, uint32_t *over) {
+	extern __shared__ __align__(16) unsigned long long s_tb[];
+	// 32-bit counts (a native shared-memory add; the 64-bit one is a CAS loop): run_tb_count gives no CTA 2^32 evaluations
+	unsigned long long *s_key = s_tb;
+	uint32_t *s_cnt = reinterpret_cast<uint32_t *>(s_tb + TB_CSLOTS);
+	for (uint32_t i = threadIdx.x; i < TB_CSLOTS; i += TB_THREADS) { s_key[i] = TB_EMPTY; s_cnt[i] = 0; }
+	__syncthreads();
+	const uint32_t lane = threadIdx.x & 31;
+	const uint64_t gpr = (S.T + TB_GROUP - 1) / TB_GROUP, groups = (uint64_t)S.C * gpr;
+	// the loop bound is warp-uniform (match.any and the early stop need every lane)
+	for (uint64_t base = (uint64_t)blockIdx.x * TB_THREADS; base < groups; base += (uint64_t)gridDim.x * TB_THREADS) {
+		const uint32_t stop = lane == 0 ? *(volatile uint32_t *)over : 0u;
+		if (__any_sync(0xFFFFFFFFu, stop)) break;           // more than cap keys: the call fails, the counts are not needed
+		const uint64_t g = base + threadIdx.x;
+		unsigned long long k[TB_GROUP];
+		uint32_t valid = 0;
+		if (g < groups) {
+			const uint32_t c = (uint32_t)(g / gpr);
+			valid = tb_keys(S, c, (g - (uint64_t)c * gpr) * TB_GROUP, k);
+		}
+#pragma unroll
+		for (int q = 0; q < TB_GROUP; q++) {
+			const unsigned long long key = (valid >> q) & 1u ? k[q] : TB_EMPTY;
+			const uint32_t peers = __match_any_sync(0xFFFFFFFFu, key);
+			if (key == TB_EMPTY || (uint32_t)(__ffs(peers) - 1) != lane) continue;
+			const uint32_t n = (uint32_t)__popc(peers);
+			const uint32_t h0 = tb_hash(key);
+			uint32_t h = tb_shash(h0) & (TB_CSLOTS - 1);
+			bool done = false;
+			for (int p = 0; p < TB_CPROBES; p++) {
+				unsigned long long cur = *(volatile unsigned long long *)&s_key[h];
+				if (cur == TB_EMPTY) {
+					cur = atomicCAS(&s_key[h], TB_EMPTY, key);
+					if (cur == TB_EMPTY) cur = key;
+				}
+				if (cur == key) { atomicAdd(&s_cnt[h], n); done = true; break; }
+				h = (h + 1) & (TB_CSLOTS - 1);
+			}
+			if (!done) tb_global_add(table, mask, key, n, cap, nkeys, over);
+		}
+	}
+	__syncthreads();
+	for (uint32_t i = threadIdx.x; i < TB_CSLOTS; i += TB_THREADS)
+		if (s_key[i] != TB_EMPTY) tb_global_add(table, mask, s_key[i], s_cnt[i], cap, nkeys, over);
+}
+
+__global__ void __launch_bounds__(256)
+k_tb_compact(const unsigned long long *table, uint64_t slots, unsigned long long *keys, unsigned long long *counts, unsigned long long *n) {
+	for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < slots; i += (uint64_t)gridDim.x * blockDim.x) {
+		const ulonglong2 v = reinterpret_cast<const ulonglong2 *>(table)[i];
+		if (v.x == TB_EMPTY) continue;
+		const unsigned long long o = atomicAdd(n, 1ull);
+		keys[o] = v.x; counts[o] = v.y;
+	}
+}
+
+__global__ void __launch_bounds__(256)
+k_tb_insert(const unsigned long long *keys, uint32_t n, unsigned long long *table, uint32_t mask) {
+	const uint32_t r = blockIdx.x * blockDim.x + threadIdx.x;
+	if (r >= n) return;
+	const unsigned long long k = keys[r];
+	uint32_t h = tb_hash(k) & mask;
+	while (atomicCAS(table + 2ull * h, TB_EMPTY, k) != TB_EMPTY) h = (h + 1) & mask;   // keys are distinct, slots >= 2 n
+	table[2ull * h + 1] = r;
+}
+
+__global__ void __launch_bounds__(TB_THREADS, 2)
+k_tb_index(const TbSource S, const unsigned long long *keys, uint32_t n, const unsigned long long *table, uint32_t mask,
+           unsigned short *tl, unsigned char *th, uint64_t tpitch, uint32_t *bad) {
+	extern __shared__ __align__(16) unsigned long long s_tb[];
+	unsigned long long *s_key = s_tb;
+	uint32_t *s_rank = reinterpret_cast<uint32_t *>(s_tb + TB_ISLOTS);
+	for (uint32_t i = threadIdx.x; i < TB_ISLOTS; i += TB_THREADS) s_key[i] = TB_EMPTY;
+	__syncthreads();
+	const uint32_t hot = n < TB_IHOT ? n : TB_IHOT;
+	for (uint32_t r = threadIdx.x; r < hot; r += TB_THREADS) {
+		const unsigned long long k = keys[r];
+		uint32_t h = tb_shash(tb_hash(k)) & (TB_ISLOTS - 1);
+		while (atomicCAS(&s_key[h], TB_EMPTY, k) != TB_EMPTY) h = (h + 1) & (TB_ISLOTS - 1);
+		s_rank[h] = r;
+	}
+	__syncthreads();
+	bool missing = false;
+	const uint64_t gpr = (S.T + TB_GROUP - 1) / TB_GROUP, groups = (uint64_t)S.C * gpr;
+	for (uint64_t g = (uint64_t)blockIdx.x * TB_THREADS + threadIdx.x; g < groups; g += (uint64_t)gridDim.x * TB_THREADS) {
+		const uint32_t c = (uint32_t)(g / gpr);
+		const uint64_t t0 = (g - (uint64_t)c * gpr) * TB_GROUP;
+		unsigned long long k[TB_GROUP];
+		const uint32_t valid = tb_keys(S, c, t0, k);
+		uint32_t lo[TB_GROUP / 2] = {0, 0, 0, 0}, hi[TB_GROUP / 4] = {0, 0};
+#pragma unroll
+		for (int q = 0; q < TB_GROUP; q++) {
+			uint32_t r = 0;
+			if ((valid >> q) & 1u) {
+				const uint32_t h0 = tb_hash(k[q]);
+				uint32_t h = tb_shash(h0) & (TB_ISLOTS - 1);
+				bool found = false;
+				for (;;) {
+					const unsigned long long cur = s_key[h];
+					if (cur == k[q]) { r = s_rank[h]; found = true; break; }
+					if (cur == TB_EMPTY) break;
+					h = (h + 1) & (TB_ISLOTS - 1);
+				}
+				if (!found) {
+					h = h0 & mask;
+					for (uint32_t p = 0;; p++) {
+						const ulonglong2 v = __ldg(reinterpret_cast<const ulonglong2 *>(table) + h);
+						if (v.x == k[q]) { r = (uint32_t)v.y; break; }
+						if (v.x == TB_EMPTY || p == mask) { missing = true; break; }
+						h = (h + 1) & mask;
+					}
+				}
+			}
+			lo[q >> 1] |= (r & 0xFFFFu) << (16 * (q & 1));
+			hi[q >> 2] |= ((r >> 16) & 0xFFu) << (8 * (q & 3));
+		}
+		const uint64_t o = (uint64_t)c * tpitch + t0;
+		*reinterpret_cast<uint4 *>(tl + o) = make_uint4(lo[0], lo[1], lo[2], lo[3]);
+		*reinterpret_cast<uint2 *>(th + o) = make_uint2(hi[0], hi[1]);
+	}
+	if (missing) atomicOr(bad, 1u);
+}
+
+namespace {
+int tb_grid(int sm_count, uint64_t groups) {
+	uint64_t grid = 2ull * (uint64_t)sm_count;                  // two 512-thread CTAs per SM
+	{ static const int env_grid = [] { const char *g = getenv("APO_K1_GRID"); return g ? atoi(g) : 0; }(); if (env_grid > 0 && (uint64_t)env_grid < grid) grid = (uint64_t)env_grid; }
+	const uint64_t need = (groups + TB_THREADS - 1) / TB_THREADS;
+	if (grid > need) grid = need;
+	return (int)(grid ? grid : 1);
+}
+}  // namespace
+
+cudaError_t run_tb_clear(unsigned long long *table, uint64_t slots, cudaStream_t st) {
+	uint64_t g = (slots + 255) / 256;
+	if (g > 132ull * 32) g = 132ull * 32;
+	k_tb_clear<<<(unsigned)g, 256, 0, st>>>(table, slots);
+	return cudaGetLastError();
+}
+
+cudaError_t run_tb_count(const TbSource &S, unsigned long long *table, uint64_t slots, uint64_t cap, unsigned long long *nkeys,
+                         uint32_t *over, int sm_count, cudaStream_t st) {
+	const uint64_t groups = (uint64_t)S.C * ((S.T + TB_GROUP - 1) / TB_GROUP);
+	if (groups == 0) return cudaSuccess;
+	const int smem = (int)(TB_CSLOTS * 12);
+	cudaError_t err = allow_big_smem(k_tb_count, smem);
+	if (err != cudaSuccess) return err;
+	int grid = tb_grid(sm_count, groups);
+	const uint64_t min_grid = groups / (1ull << 28) + 1;           // < 2^31 evaluations per CTA: its 32-bit counts cannot wrap
+	if ((uint64_t)grid < min_grid) grid = (int)min_grid;
+	k_tb_count<<<grid, TB_THREADS, smem, st>>>(S, table, (uint32_t)(slots - 1), cap, nkeys, over);
+	return cudaGetLastError();
+}
+
+cudaError_t run_tb_compact(const unsigned long long *table, uint64_t slots, unsigned long long *keys, unsigned long long *counts,
+                           unsigned long long *n, cudaStream_t st) {
+	uint64_t g = (slots + 255) / 256;
+	if (g > 132ull * 32) g = 132ull * 32;
+	k_tb_compact<<<(unsigned)g, 256, 0, st>>>(table, slots, keys, counts, n);
+	return cudaGetLastError();
+}
+
+cudaError_t run_tb_insert(const unsigned long long *keys, uint32_t n, unsigned long long *table, uint64_t slots, cudaStream_t st) {
+	if (n == 0) return cudaSuccess;
+	k_tb_insert<<<(n + 255) / 256, 256, 0, st>>>(keys, n, table, (uint32_t)(slots - 1));
+	return cudaGetLastError();
+}
+
+cudaError_t run_tb_index(const TbSource &S, const unsigned long long *keys, uint32_t n, const unsigned long long *table, uint64_t slots,
+                         unsigned short *tl, unsigned char *th, uint64_t tpitch, uint32_t *bad, int sm_count, cudaStream_t st) {
+	const uint64_t groups = (uint64_t)S.C * ((S.T + TB_GROUP - 1) / TB_GROUP);
+	if (groups == 0) return cudaSuccess;
+	const int smem = (int)(TB_ISLOTS * 12);
+	cudaError_t err = allow_big_smem(k_tb_index, smem);
+	if (err != cudaSuccess) return err;
+	k_tb_index<<<tb_grid(sm_count, groups), TB_THREADS, smem, st>>>(S, keys, n, table, (uint32_t)(slots - 1), tl, th, tpitch, bad);
 	return cudaGetLastError();
 }
 

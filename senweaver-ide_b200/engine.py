@@ -100,7 +100,8 @@ ABI_SYMBOLS = (
     "apo_rollouts16_generate", "apo_rollouts16_download", "apo_record_pack16", "apo_record_unpack16", "apo_duration_class", "apo_score",
     "apo_score_begin", "apo_score_accumulate", "apo_score_finish", "apo_score_host", "apo_score_host_records", "apo_score_host_compact", "apo_compact_encode_host",
     "apo_dims_compact_download", "apo_dims_codebook", "apo_packed_encode_host", "apo_score_host_packed", "apo_dims_packed_download", "apo_dims_d2book",
-    "apo_tuple_encode_host", "apo_score_host_tuples", "apo_tuples_upload", "apo_host_alloc", "apo_host_free",
+    "apo_tuple_encode_host", "apo_score_host_tuples", "apo_tuples_upload", "apo_dims_tuples", "apo_tuples_download", "apo_tuples_book",
+    "apo_host_alloc", "apo_host_free",
     "apo_last_timing", "apo_debug_partials", "apo_candidate_reports", "apo_candidate_corpus_reports", "apo_comm_unique_id", "apo_comm_init", "apo_comm_destroy", "apo_comm_join_mode",
 )
 
@@ -179,6 +180,9 @@ def load_library() -> C.CDLL:
     L.apo_tuple_encode_host.argtypes = [vp, vp, u32, u64, vp, vp, vp, vp, u32, vp, i32]
     L.apo_score_host_tuples.argtypes = [vp, C.POINTER(ScoreOpts), vp, vp, vp, vp, u32, vp, vp, u32, u64, vp, vp, vp, vp]
     L.apo_tuples_upload.argtypes = [vp, vp, vp, vp, vp, u32, vp, vp, u32, u64]
+    L.apo_dims_tuples.argtypes = [vp, u32, vp]
+    L.apo_tuples_download.argtypes = [vp, vp, vp, u32, u64, u64]
+    L.apo_tuples_book.argtypes = [vp, vp, vp, u32, vp, vp, vp]
     L.apo_dims_compact_download.argtypes = [vp, vp, vp, vp, u32, u64, u64]
     L.apo_dims_codebook.argtypes = [vp, vp]
     L.apo_last_timing.argtypes = [vp, C.POINTER(Timing)]
@@ -573,6 +577,36 @@ class Engine:
         tb_pc, tb_pd, codebook, d2book = self._tuple_args(tl, th, tbook, codebook, d2book)
         Cn, T = tl.shape
         self._ck(self._L.apo_tuples_upload(self._h, _p(tl), _p(th), _p(tb_pc), _p(tb_pd), tb_pc.size, _p(codebook), _p(d2book), Cn, T))
+
+    def dims_tuples(self, cap: int = TUPLES_MAX) -> int:
+        """apo_dims_tuples: build resident Form T on the device from the loaded evaluations (their Form W copy or Form Q layout);
+        returns the number of dictionary entries.  score(C, K, source=SRC_TUPLES) then reads 3 B per evaluation.  Raises
+        ApoError(APO_E_STATE) when the evaluations hold more than `cap` distinct ones (``.n_tuples`` is then a lower bound)."""
+        n = C.c_uint32(0)
+        rc = self._L.apo_dims_tuples(self._h, cap, C.addressof(n))
+        if rc != 0:
+            err = ApoError(rc, (self._L.apo_last_error(self._h) or b"").decode())
+            err.n_tuples = n.value
+            raise err
+        return n.value
+
+    def tuples_download(self, c: int, first: int, n: int):
+        """(tl uint16[n], th uint8[n]) of candidate c of the resident Form T tensor (built or uploaded)."""
+        tl, th = np.empty(n, np.uint16), np.empty(n, np.uint8)
+        self._ck(self._L.apo_tuples_download(self._h, _p(tl), _p(th), c, first, n))
+        return tl, th
+
+    def tuples_book(self):
+        """((tbook_pc, tbook_pd), codebook, d2book) of the resident Form T tensor: the arguments tuples_upload and
+        score_host_tuples take besides the planes."""
+        n = C.c_uint32(0)
+        cb, d2 = np.empty(8 * 256, np.uint32), np.empty(4096, np.uint32)
+        rc = self._L.apo_tuples_book(self._h, None, None, 0, _p(cb), _p(d2), C.addressof(n))   # learns n (APO_E_ARG when n > 0)
+        if rc != 0 and not (rc == -1 and n.value > 0):
+            self._ck(rc)
+        pc, pd = np.empty(n.value, np.uint32), np.empty(n.value, np.uint16)
+        self._ck(self._L.apo_tuples_book(self._h, _p(pc), _p(pd), n.value, _p(cb), _p(d2), C.addressof(n)))
+        return (pc, pd), cb, d2
 
     def last_timing(self) -> Timing:
         t = Timing()

@@ -29,6 +29,7 @@ interface ApoAddon {
 	rolloutsUpload(handle: unknown, records: ArrayBuffer, rowBytes: number, C: number, T: number): Promise<void>;
 	corpusUpload(handle: unknown, records: ArrayBuffer, idxBase: number): Promise<void>;
 	corpusUploadJson(handle: unknown, utf8: ArrayBuffer, idxBase: number): Promise<number>;
+	dimsTuples(handle: unknown, cap?: number): Promise<number>;
 	scoreResident(handle: unknown, query: ApoResidentQuery): Promise<Blocks>;
 	score(handle: unknown, dims: ArrayBuffer, C: number, T: number, corpus: ArrayBuffer | null, K: number, candidates?: boolean): Promise<Blocks>;
 	scoreHostRecords(handle: unknown, records: ArrayBuffer, rowBytes: number, C: number, T: number, corpus: ArrayBuffer | null, K: number,
@@ -159,6 +160,10 @@ export class ApoScoringMainService implements IApoScoringService {
 
 	async corpusUploadJson(persisted: string, idxBase?: number): Promise<number> {
 		return (await this._need()).corpusUploadJson(this._handle, ab(VSBuffer.fromString(persisted)), idxBase ?? 0);
+	}
+
+	async dimsTuples(cap?: number): Promise<number> {
+		return (await this._need()).dimsTuples(this._handle, cap);
 	}
 
 	async scoreResident(query: ApoResidentQuery): Promise<ApoScoreBlocks> {

@@ -39,7 +39,7 @@ export interface ApoTupleBuffers {
 export interface ApoResidentQuery {
 	C: number;              // candidates uploaded with dimsUpload / rolloutsUpload
 	K: number;              // beam width (APOConfig.beamWidth, APO:288)
-	source?: 0 | 1;         // 0 = dims (Form D / Form Q), 1 = per-(candidate, trace) records
+	source?: 0 | 1 | 2;     // 0 = dims (Form D / Form Q), 1 = per-(candidate, trace) records, 2 = Form T built by dimsTuples
 	corpus?: 0 | 1;         // also build the corpus report from the uploaded corpus
 	candidates?: 0 | 1;     // also build the per-candidate breakdown (ApoScoreBlocks.candidates)
 	candidateCorpus?: 0 | 1;   // source 1 only: also build every candidate's corpus report (ApoScoreBlocks.candidateCorpus)
@@ -67,6 +67,10 @@ export interface IApoScoringService {
 	corpusUpload(records: VSBuffer, idxBase?: number): Promise<void>;
 	/** Same from the persisted JSON string; resolves to the number of traces. */
 	corpusUploadJson(persisted: string, idxBase?: number): Promise<number>;
+	/** Build resident Form T (3 bytes per evaluation, source 2) on the device from the uploaded dims (apo_dims_tuples); resolves
+	 *  to the number of dictionary entries.  Rejects, leaving no Form T, when the dims hold more than cap distinct evaluations
+	 *  (default and maximum 16777215) or are not categorical.  Pays when the same dims are scored more than once. */
+	dimsTuples(cap?: number): Promise<number>;
 	scoreResident(query: ApoResidentQuery): Promise<ApoScoreBlocks>;
 
 	// ---- one-shot path: host buffers streamed through the device, nothing stays resident
@@ -101,6 +105,7 @@ export class ApoScoringService implements IApoScoringService {
 	rolloutsUpload(records: VSBuffer, rowBytes: 32 | 16, C: number, T: number) { return this._proxy.rolloutsUpload(records, rowBytes, C, T); }
 	corpusUpload(records: VSBuffer, idxBase?: number) { return this._proxy.corpusUpload(records, idxBase); }
 	corpusUploadJson(persisted: string, idxBase?: number) { return this._proxy.corpusUploadJson(persisted, idxBase); }
+	dimsTuples(cap?: number) { return this._proxy.dimsTuples(cap); }
 	scoreResident(query: ApoResidentQuery) { return this._proxy.scoreResident(query); }
 	score(dims: VSBuffer, C: number, T: number, corpus: VSBuffer | undefined, K: number, candidates?: boolean) {
 		return this._proxy.score(dims, C, T, corpus, K, candidates);
