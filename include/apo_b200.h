@@ -138,12 +138,15 @@ int  apo_set_stream(apo_engine *e, uint64_t cuda_stream);
 /* Replace the TCS:766-776 weights (default = reference values). */
 int  apo_set_weights(apo_engine *e, const double w[APO_NDIM]);
 /* Experiment / test switches of one handle (initial value: the environment variables APO_NO_FUSE, APO_FORCE_FUSE,
- * APO_NO_STAGING, APO_JOIN_NCCL, APO_NO_TWIN read once at apo_create).  Results are identical for every setting. */
+ * APO_NO_STAGING, APO_JOIN_NCCL, APO_NO_TWIN, APO_NO_TWIN_T, APO_TWIN_T read once at apo_create).  Results are identical for
+ * every setting. */
 #define APO_TUNE_NO_FUSE     0x1u  /* corpus scan / finalisation as stand-alone launches                         */
 #define APO_TUNE_FORCE_FUSE  0x2u  /* corpus scan inside the scoring launch even when it cannot hide behind it   */
 #define APO_TUNE_NO_STAGING  0x4u  /* pageable host buffers straight to cudaMemcpy (no threaded pinned staging)  */
 #define APO_TUNE_NCCL_JOIN   0x8u  /* join shards with ncclAllReduce + k_finalize instead of the peer-memory join */
 #define APO_TUNE_NO_TWIN     0x10u /* no Form Q / W copy of a loaded Form D tensor is built or read: resident Form D runs K1 */
+#define APO_TUNE_NO_TWIN_T   0x20u /* no Form T copy of a loaded Form D tensor is built or read: the Form Q / W copy as without it */
+#define APO_TUNE_TWIN_T      0x40u /* loads build the Form T copy whatever the tensor's size (tests, A/B runs on small tensors) */
 int  apo_set_tuning(apo_engine *e, uint32_t flags);
 int  apo_get_weights(const apo_engine *e, double w[APO_NDIM]);
 
@@ -193,7 +196,13 @@ int apo_corpus_upload_json(apo_engine *e, const char *json, uint64_t len, uint64
  * instead of 36 B per evaluation); other variants and windows read the fp32 tensor through K1.  The results are the same
  * either way.  The fp32 tensor stays loaded (apo_dims_layout 1, apo_dims_download); the copy goes with the next load or
  * attach, and whenever an engine allocation would otherwise fail for lack of device memory.  apo_dims_attach never
- * builds one: the caller owns that memory and may change it. */
+ * builds one: the caller owns that memory and may change it.
+ * Beside a Form W copy (or a Form Q one with <= 15 values per coded dimension) a tensor of at least 2^26 evaluations also gets
+ * a Form T copy (3 B per evaluation: indices into a dictionary of its distinct evaluations, built as apo_dims_tuples builds
+ * resident Form T) when it holds at most 2^20 distinct evaluations, the 24576 most frequent cover at least 3/4 of them, and
+ * 4 GiB stay free beside it; the same calls then read that copy through K1t whenever the weights keep every entry inside
+ * (-2, 2), else the Form W / Q copy.  It is not resident Form T (APO_SRC_TUPLES never sees it) and goes with the Form W / Q
+ * copy.  APO_TUNE_NO_TWIN_T turns it off, APO_TUNE_TWIN_T builds it at any size. */
 int apo_dims_upload(apo_engine *e, const float *dims, uint32_t C, uint64_t T);
 int apo_dims_generate(apo_engine *e, uint64_t seed, uint32_t c0, uint32_t C, uint64_t t0, uint64_t T,
                       uint32_t agent_permille);

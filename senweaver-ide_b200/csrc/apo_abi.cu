@@ -112,6 +112,13 @@ struct apo_engine {
 	DevBuf<uint32_t> tups_pc; DevBuf<unsigned short> tups_pd; DevBuf<float> tups_d2;   // dictionary of a host-streaming call
 	// apo_dims_tuples scratch (released when the build returns): hash table, (key, count) pairs / keys in rank order, counters
 	DevBuf<unsigned long long> tb_table, tb_keys, tb_cnt, tb_misc;
+	// Form T copy of a large resident Form D tensor (build_twin_t), beside its Form W / Q copy and released with it; never
+	// the Form T of apo_tuples_upload / apo_dims_tuples.  tt_val[recip]: the table values for the current weights, computed
+	// at build / apo_set_weights (recip = 0) or by the first call that asks (recip = 1); tt_ok[recip]: 0 not computed yet,
+	// 1 valid, 2 an entry is outside Form T's (-2, 2) domain (those calls read the Form W / Q copy)
+	DevBuf<unsigned short> tt_l; DevBuf<unsigned char> tt_h; DevBuf<uint32_t> tt_pc, tt_bad; DevBuf<unsigned short> tt_pd; DevBuf<float> tt_d2;
+	DevBuf<double> tt_ptab; DevBuf<long long> tt_val[2];
+	uint32_t tt_book[8 * 256]; uint32_t tt_C = 0, tt_n = 0; uint64_t tt_T = 0, tt_pitch = 0; uint8_t tt_ok[2] = {0, 0};
 
 	// acc: [acc_words(C, nranks)] partial vector | [18] example scratch (inverted indices) | [1] ticket — one allocation, so one
 	// memset arms a scoring call.  acc_joined: the joined vector (> 1 rank); acc keeps this rank's partials.
@@ -135,6 +142,7 @@ struct apo_engine {
 	void *peer_base[apo::PEER_MAX] = {nullptr}; bool peer_ipc[apo::PEER_MAX] = {false};
 	unsigned long long join_epoch = 0;
 	bool env_no_fuse = false, env_force_fuse = false, env_no_staging = false, env_nccl_join = false, env_no_twin = false;   // apo_set_tuning
+	bool env_no_twin_t = false, env_twin_t = false;
 	double stream_bytes_per_ms = 7.4e9, stream_q_bytes_per_ms = 5.0e9, stream_w_bytes_per_ms = 6.0e9, scan_ms_per_record = 3.35e-7;   // fuse heuristic, derived from the device at apo_create
 	size_t mem_pitch_max = 0;
 	uint8_t *zc_host = nullptr; uint64_t zc_cap = 0;   // zero-copy block of the single-trace path
@@ -173,13 +181,20 @@ int fail(apo_engine *e, int code, const char *fmt, ...) {
 		if (_c != cudaSuccess) return fail(e, APO_E_CUDA, "%s: %s (%s:%d)", #call, cudaGetErrorString(_c), __FILE__, __LINE__); \
 	} while (0)
 
+void drop_twin_t(apo_engine *e) {
+	e->tt_l.release(); e->tt_h.release(); e->tt_pc.release(); e->tt_pd.release(); e->tt_d2.release(); e->tt_bad.release(); e->tt_ptab.release();
+	e->tt_val[0].release(); e->tt_val[1].release();
+	e->tt_C = 0; e->tt_T = 0; e->tt_n = 0; e->tt_ok[0] = e->tt_ok[1] = 0;
+}
+
 void drop_twin(apo_engine *e) {
+	drop_twin_t(e);
 	if (!e->twin) return;
 	e->q8.release(); e->qd2.release(); e->qli.release(); e->qw.release();
 	e->twin = e->twin_w = false;
 }
 
-// Every engine buffer grows through here.  The Form Q / W copy of the fp32 tensor is a cache: an allocation that fails for lack
+// Every engine buffer grows through here.  The Form Q / W / T copies of the fp32 tensor are a cache: an allocation that fails for lack
 // of device memory while it is held releases it and is tried once more, so holding it never fails a call that would succeed
 // without it.  Launches already queued may still read the copy: they finish first.  A resident call picks the evaluations
 // it reads (route_twin) only after its last allocation before its launches.
@@ -370,7 +385,7 @@ int compact_finish(apo_engine *e, uint32_t C, uint64_t T, uint64_t pitch, bool t
 // Form D calls read through K1q (route_twin) at 14 (8) instead of 36 bytes per evaluation.  Built when the evaluations are categorical and at least
 // kTwinHeadroom of device memory stays free beside it; otherwise Form D is kept alone, without an error.
 constexpr uint64_t kTwinHeadroom = 4ull << 30;
-int build_twin(apo_engine *e) {
+int build_twin_wq(apo_engine *e) {
 	const uint32_t C = e->dims_C;
 	const uint64_t T = e->dims_T, pitch = e->dims_pitch, n = (uint64_t)C * pitch;
 	if (e->env_no_twin || C == 0 || T == 0) return APO_OK;
@@ -400,6 +415,14 @@ int build_twin(apo_engine *e) {
 	e->q8.release(); e->qd2.release(); e->qli.release();
 	e->twin_w = true;
 	return APO_OK;
+}
+
+int build_twin_t(apo_engine *e);   // beside apo_dims_tuples, whose machinery it uses
+
+// the copies of the engine's freshly loaded fp32 tensor: Form W / Q, then (large tensors) Form T beside it
+int build_twin(apo_engine *e) {
+	const int rc = build_twin_wq(e);
+	return rc == APO_OK && e->twin ? build_twin_t(e) : rc;
 }
 
 // true when the driver does not know the pointer: ordinary pageable host memory (malloc, JS ArrayBuffer, numpy)
@@ -594,6 +617,30 @@ int tuples_values(apo_engine *e, const uint32_t *book_host, const uint32_t *d_pc
 	return APO_OK;
 }
 
+// The table values of the Form T copy for the current weights and `recip` into the buffers build_twin_t allocated, and
+// whether every entry lies in Form T's domain.  Synchronises; no allocation (a scoring call runs this before route_twin).
+int twin_t_values(apo_engine *e, bool recip) {
+	const std::vector<double> tab = make_ptab(e->tt_book, e->W, std::nan(""));
+	CK(cudaMemcpyAsync(e->tt_ptab.p, tab.data(), 8 * 256 * 8, cudaMemcpyHostToDevice, e->stream));
+	CK(cudaMemsetAsync(e->tt_bad.p, 0, 4, e->stream));
+	apo::TupleValParams V{};
+	V.tb_pc = e->tt_pc.p; V.tb_pd = e->tt_pd.p; V.n = e->tt_n; V.ptab = e->tt_ptab.p; V.lut = e->d_lut.p; V.d2book = e->tt_d2.p; V.w2 = e->W.w[2];
+	V.tval = e->tt_val[recip].p; V.bad = e->tt_bad.p;
+	CK(apo::run_tuple_values(V, recip, e->stream));
+	uint32_t bad = 0;
+	CK(cudaMemcpyAsync(&bad, e->tt_bad.p, 4, cudaMemcpyDeviceToHost, e->stream));
+	CK(cudaStreamSynchronize(e->stream));
+	e->tt_ok[recip] = bad ? 2 : 1;
+	return APO_OK;
+}
+
+// a resident Form D call: the copy's values for its `recip`, computed once per weight set by the first call that needs them
+int twin_t_ready(apo_engine *e, const apo_score_opts *o) {
+	const bool recip = (o->flags & APO_SCORE_RECIP) != 0;
+	if (o->source != APO_SRC_DIMS || e->tt_C == 0 || e->env_no_twin_t || e->tt_ok[recip]) return APO_OK;
+	return twin_t_values(e, recip);
+}
+
 // after the scoring call has been synchronised: did K1t meet an index outside the dictionary, or an entry it cannot hold?
 int tuples_check(apo_engine *e) {
 	e->tup_used = false;
@@ -625,7 +672,8 @@ struct Evals {
 	const unsigned short *tb_pd = nullptr;
 	uint32_t n_tuples = 0;
 	const float *d2book = nullptr;
-	const uint32_t *codebook = nullptr;       // resident Form T: every launch rebuilds this codebook's tables (NULL: built once per call)
+	const uint32_t *codebook = nullptr;       // resident Form T: every launch rebuilds this codebook's tables (NULL: built once per call) ...
+	const long long *tval = nullptr;          // ... unless they are held (the Form T copy of a resident Form D tensor, route_twin)
 	const unsigned long long *qw = nullptr;   // Form W words (the copy of a resident Form D tensor, route_twin)
 
 	bool records() const { return form == apo::CAND_REC32 || form == apo::CAND_REC16; }
@@ -681,11 +729,20 @@ int resident_window(apo_engine *e, const apo_score_opts *o, Evals *ev) {
 }
 
 // A resident Form D call reads the Form Q / W copy through K1q instead when one is held, the variant is the default (1-4 name
-// K1 tile shapes) and the window starts on K1q's 8-evaluation grid.  Before resident_window, after the call's last allocation
-// before its launches (reserve may release the copy).
+// K1 tile shapes) and the window starts on K1q's 8-evaluation grid; under the same conditions it reads the Form T copy through
+// K1t when that is held and its values for this call's weights and `recip` are valid (twin_t_ready).  Before resident_window,
+// after the call's last allocation before its launches (reserve may release the copies).
 void route_twin(const apo_engine *e, const apo_score_opts *o, Evals *ev) {
 	if (ev->form != apo::CAND_DIMS || !e->twin || e->env_no_twin || o->variant != 0 || o->first % 8) return;
 	ev->rows = nullptr;
+	const bool recip = (o->flags & APO_SCORE_RECIP) != 0;
+	if (e->tt_C && !e->env_no_twin_t && e->tt_ok[recip] == 1) {
+		ev->form = apo::CAND_T; ev->pitch_evals = e->tt_pitch; ev->variant = 0;
+		ev->tl = e->tt_l.p; ev->th = e->tt_h.p;
+		ev->tb_pc = e->tt_pc.p; ev->tb_pd = e->tt_pd.p; ev->n_tuples = e->tt_n; ev->d2book = e->tt_d2.p;
+		ev->codebook = e->tt_book; ev->tval = e->tt_val[recip].p;
+		return;
+	}
 	if (e->twin_w) {                                         // <= 15 codes per dimension: the prefix table always fits
 		ev->form = apo::CAND_W; ev->qw = e->qw.p; ev->variant = 0;
 		return;
@@ -701,12 +758,14 @@ int launch_score(apo_engine *e, const apo_score_opts *o, const Evals &ev, uint32
 	const bool recip = (o->flags & APO_SCORE_RECIP) != 0;
 	long long *acc = e->acc.p + (uint64_t)ACC_PER_CAND * cand_offset;
 	int rc;
-	if (ev.codebook && (rc = tuples_values(e, ev.codebook, ev.tb_pc, ev.tb_pd, ev.n_tuples, ev.d2book, recip))) return rc;
+	if (ev.codebook && !ev.tval && (rc = tuples_values(e, ev.codebook, ev.tb_pc, ev.tb_pd, ev.n_tuples, ev.d2book, recip))) return rc;
 	if ((rc = record_k1_event(e, 0))) return rc;
 	if (ev.form == apo::CAND_T) {
 		apo::KtParams P{};
 		P.tl = ev.tl; P.th = ev.th; P.pitch_evals = ev.pitch_evals; P.C = ev.C; P.T = ev.count;
-		P.acc = acc; P.tval = e->tup_val.p; P.n_tuples = ev.n_tuples; P.bad = e->tup_bad.p;
+		P.acc = acc; P.n_tuples = ev.n_tuples;
+		// the copy's indices come from its own dictionary: its index flag is never set, and never read
+		P.tval = ev.tval ? ev.tval : e->tup_val.p; P.bad = ev.tval ? e->tt_bad.p : e->tup_bad.p;
 		CK(apo::run_reward9t(P, e->sm_count, e->stream));
 	} else if (ev.form == apo::CAND_Q || ev.form == apo::CAND_W) {
 		apo::KqParams Q{};
@@ -737,6 +796,13 @@ bool wants_cand(const apo_score_opts *o) { return (o->flags & APO_SCORE_CANDIDAT
 int cand_check(apo_engine *e) {
 	if (e->nranks > 1)
 		return fail(e, APO_E_STATE, "APO_SCORE_CANDIDATES is single-rank only: the per-candidate breakdown is not joined across the %d ranks of this handle", e->nranks);
+	return APO_OK;
+}
+
+// the breakdown's buffers (cand_arm's, and cand_upload_tbook's for Form T), allocated before route_twin
+int cand_reserve(apo_engine *e, uint32_t C) {
+	CK(reserve(e, e->cand_acc, (uint64_t)C * (apo::CB_INT + 3)));
+	CK(reserve(e, e->cand_book, 8 * 16));
 	return APO_OK;
 }
 
@@ -956,7 +1022,7 @@ int score_check(apo_engine *e, const apo_score_opts *o, uint32_t C, uint64_t T, 
 	CK(cudaSetDevice(e->device));
 	if (T == kSession) return APO_OK;                               // a session's scratch was sized by apo_score_begin
 	if ((rc = ensure_scratch(e, C, o->K))) return rc;
-	if (wants_cand(o)) CK(reserve(e, e->cand_acc, (uint64_t)C * (apo::CB_INT + 3)));   // cand_arm's, before route_twin
+	if (wants_cand(o) && (rc = cand_reserve(e, C))) return rc;
 	return APO_OK;
 }
 
@@ -1116,7 +1182,9 @@ extern "C" int apo_create(int device, apo_engine **out) {
 	e->env_no_staging = getenv("APO_NO_STAGING") != nullptr;
 	e->env_nccl_join = getenv("APO_JOIN_NCCL") != nullptr;
 	e->env_no_twin = getenv("APO_NO_TWIN") != nullptr;
-	if ((c = cudaStreamCreateWithFlags(&e->own_stream, cudaStreamNonBlocking)) != cudaSuccess) return bail("cudaStreamCreate", c);
+	e->env_no_twin_t = getenv("APO_NO_TWIN_T") != nullptr;
+	e->env_twin_t = getenv("APO_TWIN_T") != nullptr;
+	if ((c =cudaStreamCreateWithFlags(&e->own_stream, cudaStreamNonBlocking)) != cudaSuccess) return bail("cudaStreamCreate", c);
 	if ((c = cudaStreamCreateWithFlags(&e->copy_stream, cudaStreamNonBlocking)) != cudaSuccess) return bail("cudaStreamCreate", c);
 	e->stream = e->own_stream;
 	for (auto &ev : e->ev) if ((c = cudaEventCreate(&ev)) != cudaSuccess) return bail("cudaEventCreate", c);
@@ -1147,6 +1215,7 @@ extern "C" void apo_destroy(apo_engine *e) {
 	e->tups_pc.release(); e->tups_pd.release(); e->tups_d2.release();
 	e->cand_acc.release(); e->cand_rep.release(); e->cand_book.release(); e->ccorp_acc.release(); e->ccorp_rep.release();
 	e->tup_l.release(); e->tup_h.release(); e->tup_pc.release(); e->tup_pd.release(); e->tup_bad.release(); e->tup_d2.release(); e->tup_ptab.release(); e->tup_val.release();
+	drop_twin_t(e);
 	e->win[0].release(); e->win[1].release(); e->batch_in.release(); e->batch_out.release(); e->batch_mask.release();
 	if (e->h_result) cudaFreeHost(e->h_result);
 	if (e->h_domain) cudaFreeHost((void *)e->h_domain);
@@ -1169,11 +1238,12 @@ extern "C" int apo_set_stream(apo_engine *e, uint64_t cuda_stream) {
 
 extern "C" int apo_set_tuning(apo_engine *e, uint32_t flags) {
 	if (!e) return APO_E_ARG;
-	if (flags & ~(APO_TUNE_NO_FUSE | APO_TUNE_FORCE_FUSE | APO_TUNE_NO_STAGING | APO_TUNE_NCCL_JOIN | APO_TUNE_NO_TWIN))
+	if (flags & ~(APO_TUNE_NO_FUSE | APO_TUNE_FORCE_FUSE | APO_TUNE_NO_STAGING | APO_TUNE_NCCL_JOIN | APO_TUNE_NO_TWIN | APO_TUNE_NO_TWIN_T | APO_TUNE_TWIN_T))
 		return fail(e, APO_E_ARG, "unknown tuning flag %#x", flags);
 	e->env_no_fuse = (flags & APO_TUNE_NO_FUSE) != 0; e->env_force_fuse = (flags & APO_TUNE_FORCE_FUSE) != 0;
 	e->env_no_staging = (flags & APO_TUNE_NO_STAGING) != 0; e->env_nccl_join = (flags & APO_TUNE_NCCL_JOIN) != 0;
 	e->env_no_twin = (flags & APO_TUNE_NO_TWIN) != 0;
+	e->env_no_twin_t = (flags & APO_TUNE_NO_TWIN_T) != 0; e->env_twin_t = (flags & APO_TUNE_TWIN_T) != 0;
 	return APO_OK;
 }
 
@@ -1187,6 +1257,8 @@ extern "C" int apo_set_weights(apo_engine *e, const double w[APO_NDIM]) {
 	build_luts(e);
 	int rc = upload_luts(e);
 	if (rc == APO_OK && (e->compact || e->twin)) rc = upload_ptab(e);
+	e->tt_ok[0] = e->tt_ok[1] = 0;                          // the Form T copy's values belonged to the old weights
+	if (rc == APO_OK && e->tt_C) rc = twin_t_values(e, false);
 	return rc;
 }
 
@@ -1358,6 +1430,7 @@ extern "C" int apo_dims_compact(apo_engine *e) {
 	if (!e->dims_ptr || e->dims_C == 0) return fail(e, APO_E_STATE, "no dims loaded");
 	CK(cudaSetDevice(e->device));
 	if (e->twin && !e->twin_w) {                        // the copy built at load already is this tensor in Form Q
+		drop_twin_t(e);                                 // a compact tensor keeps no Form T copy
 		e->twin = false; e->compact = true; e->dims_ptr = nullptr;
 		e->dims.release();
 		return APO_OK;
@@ -1506,7 +1579,9 @@ extern "C" int apo_score_accumulate(apo_engine *e, const apo_score_opts *o, uint
 	if (cand && (rc = cand_check(e))) return rc;
 	if (ccorp && (rc = ccorp_check(e, ev.records()))) return rc;
 	CK(cudaSetDevice(e->device));
-	if (cand && e->cand_every && !e->cand_armed && (rc = cand_arm(e, e->score_C))) return rc;   // allocates: before route_twin
+	if (cand && (rc = cand_reserve(e, e->score_C))) return rc;                                  // allocates: before route_twin
+	if (cand && e->cand_every && !e->cand_armed && (rc = cand_arm(e, e->score_C))) return rc;
+	if ((rc = twin_t_ready(e, o))) return rc;
 	route_twin(e, o, &ev);
 	if ((rc = resident_window(e, o, &ev)) || (rc = launch_score(e, o, ev, cand_offset))) return rc;
 	if (!ccorp) e->ccorp_every = false;
@@ -1542,7 +1617,7 @@ extern "C" int apo_score(apo_engine *e, const apo_score_opts *o, double *scores,
 	int rc = resident_evals(e, o, &ev);
 	if (rc) return rc;
 	const uint32_t C = ev.C;
-	if ((rc = score_check(e, o, C, ev.count, ev.records()))) return rc;
+	if ((rc = score_check(e, o, C, ev.count, ev.records())) || (rc = twin_t_ready(e, o))) return rc;
 	route_twin(e, o, &ev);
 	if ((rc = resident_window(e, o, &ev))) return rc;
 	const bool tup = ev.form == apo::CAND_T;            // gather-and-add kernel: stand-alone corpus scan + tail
@@ -1887,15 +1962,28 @@ extern "C" int apo_tuples_upload(apo_engine *e, const uint16_t *tl, const uint8_
 }
 
 namespace {
+constexpr uint32_t kTwinTHot = 24576;   // K1t's shared-memory head of the table (KT_HOT_MAX, csrc/apo_tuple.cu)
+
+// Where a Form T build from the loaded evaluations goes: the engine's resident Form T (apo_dims_tuples), or the Form T copy of
+// its Form D tensor (build_twin_t).  The copy's buffers do not go through reserve: releasing the copies to make room would
+// release the one being built.
+struct TupleDst {
+	DevBuf<unsigned short> &l; DevBuf<unsigned char> &h; DevBuf<uint32_t> &pc; DevBuf<unsigned short> &pd; DevBuf<float> &d2;
+	uint32_t *book; uint32_t &C, &n; uint64_t &T, &pitch;
+	bool copy;
+};
+TupleDst resident_tuples(apo_engine *e) { return {e->tup_l, e->tup_h, e->tup_pc, e->tup_pd, e->tup_d2, e->tup_book, e->tup_C, e->tup_n, e->tup_T, e->tup_pitch, false}; }
+TupleDst copy_tuples(apo_engine *e) { return {e->tt_l, e->tt_h, e->tt_pc, e->tt_pd, e->tt_d2, e->tt_book, e->tt_C, e->tt_n, e->tt_T, e->tt_pitch, true}; }
+
 template <class T>
-int tb_reserve(apo_engine *e, DevBuf<T> &b, uint64_t n, const char *what) {
-	const cudaError_t c = reserve(e, b, n);
+int tb_reserve(apo_engine *e, DevBuf<T> &b, uint64_t n, const char *what, bool copy = false) {
+	const cudaError_t c = copy ? b.reserve(n) : reserve(e, b, n);
 	if (c == cudaSuccess) return APO_OK;
 	cudaGetLastError();
 	return fail(e, c == cudaErrorMemoryAllocation ? APO_E_NOMEM : APO_E_CUDA, "%s (%llu elements): %s", what, (unsigned long long)n, cudaGetErrorString(c));
 }
 
-int dims_tuples(apo_engine *e, uint32_t cap, uint32_t *n_tuples) {
+int dims_tuples(apo_engine *e, uint32_t cap, uint32_t *n_tuples, const TupleDst &D) {
 	if ((!e->dims_ptr && !e->compact) || e->dims_C == 0) return fail(e, APO_E_STATE, "no dims loaded");
 	if (!e->compact && (!e->twin || e->env_no_twin))
 		return fail(e, APO_E_STATE, "the loaded Form D tensor has no Form W / Q copy to build Form T from (APO_TUNE_NO_TWIN, apo_dims_attach, "
@@ -1913,11 +2001,12 @@ int dims_tuples(apo_engine *e, uint32_t cap, uint32_t *n_tuples) {
 	const uint64_t tpitch = round_up(T ? T : 1, 64);               // as apo_tuples_upload
 	// everything is allocated before the source is chosen: reserve may release the copy this build reads
 	int rc;
-	if ((rc = tb_reserve(e, e->tup_l, (uint64_t)C * tpitch, "Form T low plane")) || (rc = tb_reserve(e, e->tup_h, (uint64_t)C * tpitch, "Form T high plane")) ||
-	    (rc = tb_reserve(e, e->tup_pc, m ? m : 1, "dictionary")) || (rc = tb_reserve(e, e->tup_pd, m ? m : 1, "dictionary")) ||
-	    (rc = tb_reserve(e, e->tup_d2, 4096, "d2book")) || (rc = tb_reserve(e, e->tb_table, 2 * slots, "hash table")) ||
-	    (rc = tb_reserve(e, e->tb_keys, m ? m : 1, "keys")) || (rc = tb_reserve(e, e->tb_cnt, m ? m : 1, "counts")) ||
-	    (rc = tb_reserve(e, e->tb_misc, 4, "counters")))
+	const bool cp = D.copy;
+	if ((rc = tb_reserve(e, D.l, (uint64_t)C * tpitch, "Form T low plane", cp)) || (rc = tb_reserve(e, D.h, (uint64_t)C * tpitch, "Form T high plane", cp)) ||
+	    (rc = tb_reserve(e, D.pc, m ? m : 1, "dictionary", cp)) || (rc = tb_reserve(e, D.pd, m ? m : 1, "dictionary", cp)) ||
+	    (rc = tb_reserve(e, D.d2, 4096, "d2book", cp)) || (rc = tb_reserve(e, e->tb_table, 2 * slots, "hash table", cp)) ||
+	    (rc = tb_reserve(e, e->tb_keys, m ? m : 1, "keys", cp)) || (rc = tb_reserve(e, e->tb_cnt, m ? m : 1, "counts", cp)) ||
+	    (rc = tb_reserve(e, e->tb_misc, 4, "counters", cp)))
 		return rc;
 	if (!e->compact && !e->twin)
 		return fail(e, APO_E_NOMEM, "device memory ran short: the Form W / Q copy of the loaded tensor was released to make room for the build; "
@@ -1967,6 +2056,11 @@ int dims_tuples(apo_engine *e, uint32_t cap, uint32_t *n_tuples) {
 		if (x.first != y.first) return x.first > y.first;
 		return x.second < y.second;
 	});
+	if (D.copy) {                                                 // see build_twin_t
+		uint64_t head = 0;
+		for (uint32_t r = 0; r < n && r < kTwinTHot; r++) head += order[r].first;
+		if (head * 4 < N * 3) return APO_E_STATE;
+	}
 	std::vector<uint32_t> tb_pc(n);
 	std::vector<uint16_t> tb_pd(n);
 	for (uint32_t r = 0; r < n; r++) {
@@ -1974,25 +2068,67 @@ int dims_tuples(apo_engine *e, uint32_t cap, uint32_t *n_tuples) {
 		tb_pc[r] = (uint32_t)order[r].second; tb_pd[r] = (uint16_t)pd;
 		keys[r] = (unsigned long long)tb_pc[r] | ((unsigned long long)(pd == 4095u ? apo::KW_D2_ABSENT : d2book[pd]) << 32);   // back to the evaluation key
 	}
-	CK(cudaMemcpyAsync(e->tup_d2.p, d2book, sizeof d2book, cudaMemcpyHostToDevice, e->stream));
+	CK(cudaMemcpyAsync(D.d2.p, d2book, sizeof d2book, cudaMemcpyHostToDevice, e->stream));
 	if (n) {
-		CK(cudaMemcpyAsync(e->tup_pc.p, tb_pc.data(), (uint64_t)n * 4, cudaMemcpyHostToDevice, e->stream));
-		CK(cudaMemcpyAsync(e->tup_pd.p, tb_pd.data(), (uint64_t)n * 2, cudaMemcpyHostToDevice, e->stream));
+		CK(cudaMemcpyAsync(D.pc.p, tb_pc.data(), (uint64_t)n * 4, cudaMemcpyHostToDevice, e->stream));
+		CK(cudaMemcpyAsync(D.pd.p, tb_pd.data(), (uint64_t)n * 2, cudaMemcpyHostToDevice, e->stream));
 		CK(cudaMemcpyAsync(e->tb_keys.p, keys.data(), (uint64_t)n * 8, cudaMemcpyHostToDevice, e->stream));
 		// the index table holds only the dictionary (slots >= 2 n, so that it stays small enough for L2)
 		uint64_t islots = 1024;
 		while (islots < 2ull * n) islots <<= 1;
 		CK(apo::run_tb_clear(e->tb_table.p, islots, e->stream));
 		CK(apo::run_tb_insert(e->tb_keys.p, n, e->tb_table.p, islots, e->stream));
-		CK(apo::run_tb_index(S, e->tb_keys.p, n, e->tb_table.p, islots, e->tup_l.p, e->tup_h.p, tpitch, (uint32_t *)(misc + 1), e->sm_count, e->stream));
+		CK(apo::run_tb_index(S, e->tb_keys.p, n, e->tb_table.p, islots, D.l.p, D.h.p, tpitch, (uint32_t *)(misc + 1), e->sm_count, e->stream));
 	}
 	unsigned long long miss = 0;
 	CK(cudaMemcpyAsync(&miss, misc + 1, 8, cudaMemcpyDeviceToHost, e->stream));
 	CK(cudaStreamSynchronize(e->stream));
 	if (miss) return fail(e, APO_E_CUDA, "internal error: an evaluation's key is missing from the dictionary");
-	memcpy(e->tup_book, e->qbook_host, sizeof e->tup_book);
-	e->tup_C = C; e->tup_T = T; e->tup_pitch = tpitch; e->tup_n = n;
+	memcpy(D.book, e->qbook_host, sizeof e->tup_book);
+	D.C = C; D.T = T; D.pitch = tpitch; D.n = n;
 	*n_tuples = n;
+	return APO_OK;
+}
+
+// The Form T copy of a freshly loaded Form D tensor that holds a Form W / Q copy with <= 15 values per coded dimension: its
+// resident Form D calls then read 3 B per evaluation through K1t (route_twin).  Built when the tensor holds at least
+// kTwinTMinEvals evaluations (APO_TUNE_TWIN_T: any size), at most kTwinTCap distinct ones (the build's scratch is sized
+// from it; the table stays well inside L2), the kTwinTHot most frequent of them cover at least 3/4 of the evaluations (K1t
+// serves those from shared memory and gathers the rest from L2: on an H100 it beats K1q on Form W with 75 % of its reads in
+// the head and loses by 2x with 9 %, DESIGN §8), and kTwinHeadroom of device memory stays free beside the copy and the
+// build's scratch; otherwise no copy is kept, without an error.  The build also computes the table values for the weights.
+constexpr uint64_t kTwinTMinEvals = 1ull << 26;
+constexpr uint32_t kTwinTCap = 1u << 20;
+int build_twin_t(apo_engine *e) {
+	const uint32_t C = e->dims_C;
+	const uint64_t T = e->dims_T, N = (uint64_t)C * T;
+	if (e->env_no_twin_t || !(N >= kTwinTMinEvals || e->env_twin_t)) return APO_OK;
+	if (!e->twin_w)
+		for (int j = 0; j < 8; j++)
+			if (e->qbook_host[256 * j + 15] != 0xFFFFFFFFu) return APO_OK;
+	const uint64_t m = std::min<uint64_t>(kTwinTCap, N);
+	uint64_t slots = 1024;
+	while (slots < 2 * (m + 1)) slots <<= 1;
+	// index planes, dictionary, value tables; the build's hash table, keys and counts
+	const uint64_t need = 3 * (uint64_t)C * round_up(T, 64) + m * 6 + 2 * (m + 1) * 8 + 16 * slots + 16 * m;
+	size_t free_bytes = 0, total_bytes = 0;
+	CK(cudaMemGetInfo(&free_bytes, &total_bytes));
+	if ((uint64_t)free_bytes < need + kTwinHeadroom) return APO_OK;
+	const std::string keep_err = e->err;
+	uint32_t n = 0;
+	int rc = dims_tuples(e, kTwinTCap, &n, copy_tuples(e));
+	if (rc == APO_OK && (e->tt_val[0].reserve(n + 1ull) != cudaSuccess || e->tt_val[1].reserve(n + 1ull) != cudaSuccess ||
+	                     e->tt_ptab.reserve(8 * 256) != cudaSuccess || e->tt_bad.reserve(1) != cudaSuccess)) {
+		cudaGetLastError();
+		rc = APO_E_NOMEM;
+	}
+	if (rc == APO_OK) rc = twin_t_values(e, false);
+	if (rc != APO_OK) cudaStreamSynchronize(e->stream);          // nothing queued may still use what is released
+	e->tb_table.release(); e->tb_keys.release(); e->tb_cnt.release(); e->tb_misc.release();
+	if (rc == APO_OK) return APO_OK;
+	drop_twin_t(e);
+	if (rc != APO_E_STATE && rc != APO_E_NOMEM) return rc;
+	e->err = keep_err;                                          // more than kTwinTCap distinct evaluations, or no room: no copy
 	return APO_OK;
 }
 }  // namespace
@@ -2003,7 +2139,7 @@ extern "C" int apo_dims_tuples(apo_engine *e, uint32_t cap, uint32_t *n_tuples) 
 	*n_tuples = 0;
 	CK(cudaSetDevice(e->device));
 	e->tup_C = 0; e->tup_T = 0; e->tup_n = 0;                      // a failure leaves no Form T loaded, as a failed apo_tuples_upload
-	const int rc = dims_tuples(e, cap, n_tuples);
+	const int rc = dims_tuples(e, cap, n_tuples, resident_tuples(e));
 	if (rc != APO_OK) cudaStreamSynchronize(e->stream);           // nothing queued may still use the scratch when it is released
 	e->tb_table.release(); e->tb_keys.release(); e->tb_cnt.release(); e->tb_misc.release();
 	return rc;

@@ -22,6 +22,7 @@ TUPLES_MAX = 0xFFFFFF
 SCORE_CORPUS, SCORE_RECIP, SCORE_TIMING, SCORE_CANDIDATES = 0x1, 0x2, 0x4, 0x8
 SCORE_CANDIDATE_CORPUS = 0x10
 TUNE_NO_FUSE, TUNE_FORCE_FUSE, TUNE_NO_STAGING, TUNE_NCCL_JOIN, TUNE_NO_TWIN = 0x1, 0x2, 0x4, 0x8, 0x10
+TUNE_NO_TWIN_T, TUNE_TWIN_T = 0x20, 0x40
 F_ERRORS, F_ENDED, F_VALID, F_FAILSPAN = 0x01, 0x02, 0x08, 0x10
 UNIQUE_ID_BYTES = 128
 
