@@ -138,7 +138,7 @@ int  apo_set_stream(apo_engine *e, uint64_t cuda_stream);
 /* Replace the TCS:766-776 weights (default = reference values). */
 int  apo_set_weights(apo_engine *e, const double w[APO_NDIM]);
 /* Experiment / test switches of one handle (initial value: the environment variables APO_NO_FUSE, APO_FORCE_FUSE,
- * APO_NO_STAGING, APO_JOIN_NCCL, APO_NO_TWIN, APO_NO_TWIN_T, APO_TWIN_T read once at apo_create).  Results are identical for
+ * APO_NO_STAGING, APO_JOIN_NCCL, APO_NO_TWIN, APO_NO_TWIN_T, APO_TWIN_T, APO_NO_TWIN_T2 read once at apo_create).  Results are identical for
  * every setting. */
 #define APO_TUNE_NO_FUSE     0x1u  /* corpus scan / finalisation as stand-alone launches                         */
 #define APO_TUNE_FORCE_FUSE  0x2u  /* corpus scan inside the scoring launch even when it cannot hide behind it   */
@@ -147,6 +147,7 @@ int  apo_set_weights(apo_engine *e, const double w[APO_NDIM]);
 #define APO_TUNE_NO_TWIN     0x10u /* no Form Q / W copy of a loaded Form D tensor is built or read: resident Form D runs K1 */
 #define APO_TUNE_NO_TWIN_T   0x20u /* no Form T copy of a loaded Form D tensor is built or read: the Form Q / W copy as without it */
 #define APO_TUNE_TWIN_T      0x40u /* loads build the Form T copy whatever the tensor's size (tests, A/B runs on small tensors) */
+#define APO_TUNE_NO_TWIN_T2  0x80u /* no exception list of the Form T copy is built or read: the copy is read at 3 B per evaluation */
 int  apo_set_tuning(apo_engine *e, uint32_t flags);
 int  apo_get_weights(const apo_engine *e, double w[APO_NDIM]);
 
@@ -202,7 +203,11 @@ int apo_corpus_upload_json(apo_engine *e, const char *json, uint64_t len, uint64
  * resident Form T) when it holds at most 2^20 distinct evaluations, the 24576 most frequent cover at least 3/4 of them, and
  * 4 GiB stay free beside it; the same calls then read that copy through K1t whenever the weights keep every entry inside
  * (-2, 2), else the Form W / Q copy.  It is not resident Form T (APO_SRC_TUPLES never sees it) and goes with the Form W / Q
- * copy.  APO_TUNE_NO_TWIN_T turns it off, APO_TUNE_TWIN_T builds it at any size. */
+ * copy.  APO_TUNE_NO_TWIN_T turns it off, APO_TUNE_TWIN_T builds it at any size.
+ * When at most 1/64 of the evaluations have a dictionary index of 2^16 or more, the copy also holds a list of those
+ * evaluations, and the calls read 2 B per evaluation (the low 16 bits of every index) and correct the listed ones; with at
+ * most 2^16 distinct evaluations the list is empty.  APO_TUNE_NO_TWIN_T2 at the load builds no list, set later it keeps the
+ * calls at 3 B per evaluation. */
 int apo_dims_upload(apo_engine *e, const float *dims, uint32_t C, uint64_t T);
 int apo_dims_generate(apo_engine *e, uint64_t seed, uint32_t c0, uint32_t C, uint64_t t0, uint64_t T,
                       uint32_t agent_permille);
@@ -371,6 +376,11 @@ int apo_last_timing(const apo_engine *e, apo_timing *out);
  * and the count; 4*C int64 words.  Order-independent, hence identical for any grid,
  * shard or rank count. */
 int apo_debug_partials(apo_engine *e, int64_t *out, uint32_t C);
+/* The exception list of the Form T copy (see apo_dims_upload), for tests and diagnostics: *n_exceptions pairs {position in
+ * the row, full index} of the evaluations whose index is >= 2^16, rows in order, sorted by position (xs, 2 words each), and
+ * its block index (xb, *n_words = C * (blocks per row + 1) words: the list offset of row c's first exception at or after
+ * position 8192 b is xb[c * (blocks per row + 1) + b]).  Both counts are 0 when no list is held.  xb / xs may be NULL. */
+int apo_debug_twin_t_list(apo_engine *e, uint64_t *n_words, uint64_t *n_exceptions, uint32_t *xb, uint32_t *xs);
 
 /* ---- per-candidate breakdown: why candidate c scored what it scored ------------------
  * The corpus report (APO:498-625) answered per candidate, over the evaluations of c that the

@@ -119,6 +119,9 @@ struct apo_engine {
 	DevBuf<unsigned short> tt_l; DevBuf<unsigned char> tt_h; DevBuf<uint32_t> tt_pc, tt_bad; DevBuf<unsigned short> tt_pd; DevBuf<float> tt_d2;
 	DevBuf<double> tt_ptab; DevBuf<long long> tt_val[2];
 	uint32_t tt_book[8 * 256]; uint32_t tt_C = 0, tt_n = 0; uint64_t tt_T = 0, tt_pitch = 0; uint8_t tt_ok[2] = {0, 0};
+	// the copy's exception list (build_twin_t2): tt_t2 = K1t2 may read the copy from tt_l alone; tt_xs / tt_xb hold the
+	// tt_xn evaluations whose index is >= 2^16 and their block index (none when the dictionary has <= 2^16 entries)
+	DevBuf<uint2> tt_xs; DevBuf<uint32_t> tt_xb; uint64_t tt_xn = 0; uint32_t tt_nblk = 0; bool tt_t2 = false;
 
 	// acc: [acc_words(C, nranks)] partial vector | [18] example scratch (inverted indices) | [1] ticket — one allocation, so one
 	// memset arms a scoring call.  acc_joined: the joined vector (> 1 rank); acc keeps this rank's partials.
@@ -142,7 +145,7 @@ struct apo_engine {
 	void *peer_base[apo::PEER_MAX] = {nullptr}; bool peer_ipc[apo::PEER_MAX] = {false};
 	unsigned long long join_epoch = 0;
 	bool env_no_fuse = false, env_force_fuse = false, env_no_staging = false, env_nccl_join = false, env_no_twin = false;   // apo_set_tuning
-	bool env_no_twin_t = false, env_twin_t = false;
+	bool env_no_twin_t = false, env_twin_t = false, env_no_twin_t2 = false;
 	double stream_bytes_per_ms = 7.4e9, stream_q_bytes_per_ms = 5.0e9, stream_w_bytes_per_ms = 6.0e9, scan_ms_per_record = 3.35e-7;   // fuse heuristic, derived from the device at apo_create
 	size_t mem_pitch_max = 0;
 	uint8_t *zc_host = nullptr; uint64_t zc_cap = 0;   // zero-copy block of the single-trace path
@@ -183,8 +186,9 @@ int fail(apo_engine *e, int code, const char *fmt, ...) {
 
 void drop_twin_t(apo_engine *e) {
 	e->tt_l.release(); e->tt_h.release(); e->tt_pc.release(); e->tt_pd.release(); e->tt_d2.release(); e->tt_bad.release(); e->tt_ptab.release();
-	e->tt_val[0].release(); e->tt_val[1].release();
+	e->tt_val[0].release(); e->tt_val[1].release(); e->tt_xs.release(); e->tt_xb.release();
 	e->tt_C = 0; e->tt_T = 0; e->tt_n = 0; e->tt_ok[0] = e->tt_ok[1] = 0;
+	e->tt_xn = 0; e->tt_nblk = 0; e->tt_t2 = false;
 }
 
 void drop_twin(apo_engine *e) {
@@ -675,12 +679,16 @@ struct Evals {
 	const uint32_t *codebook = nullptr;       // resident Form T: every launch rebuilds this codebook's tables (NULL: built once per call) ...
 	const long long *tval = nullptr;          // ... unless they are held (the Form T copy of a resident Form D tensor, route_twin)
 	const unsigned long long *qw = nullptr;   // Form W words (the copy of a resident Form D tensor, route_twin)
+	bool t2 = false;                          // the Form T copy through K1t2: tl and the exception list, not th (route_twin)
+	const uint2 *xs = nullptr;
+	const uint32_t *xb = nullptr;
+	uint32_t xb_pitch = 0;
 
 	bool records() const { return form == apo::CAND_REC32 || form == apo::CAND_REC16; }
 	uint32_t row() const { return form == apo::CAND_DIMS ? 36 : form == apo::CAND_REC32 ? 32 : 16; }
-	uint32_t bytes() const { return form == apo::CAND_T ? 3 : form == apo::CAND_Q ? 14 : form == apo::CAND_W ? 8 : row(); }   // read per evaluation
+	uint32_t bytes() const { return form == apo::CAND_T ? (t2 ? 2 : 3) : form == apo::CAND_Q ? 14 : form == apo::CAND_W ? 8 : row(); }   // read per evaluation
 	uint64_t tile() const {                   // evaluations per tile of the scoring kernel
-		return (uint64_t)(form == apo::CAND_T ? apo::kt_tile_evals() : form == apo::CAND_Q ? apo::kq_tile_evals(variant)
+		return (uint64_t)(form == apo::CAND_T ? (t2 ? apo::kt2_tile_evals() : apo::kt_tile_evals()) : form == apo::CAND_Q ? apo::kq_tile_evals(variant)
 		                  : form == apo::CAND_W ? apo::kw_tile_evals() : apo::k1_tile_evals((int)row(), variant));
 	}
 };
@@ -730,8 +738,9 @@ int resident_window(apo_engine *e, const apo_score_opts *o, Evals *ev) {
 
 // A resident Form D call reads the Form Q / W copy through K1q instead when one is held, the variant is the default (1-4 name
 // K1 tile shapes) and the window starts on K1q's 8-evaluation grid; under the same conditions it reads the Form T copy through
-// K1t when that is held and its values for this call's weights and `recip` are valid (twin_t_ready).  Before resident_window,
-// after the call's last allocation before its launches (reserve may release the copies).
+// K1t when that is held and its values for this call's weights and `recip` are valid (twin_t_ready): through K1t2 from the
+// 16-bit plane when the copy holds an exception list and APO_TUNE_NO_TWIN_T2 is clear.  Before resident_window, after the
+// call's last allocation before its launches (reserve may release the copies).
 void route_twin(const apo_engine *e, const apo_score_opts *o, Evals *ev) {
 	if (ev->form != apo::CAND_DIMS || !e->twin || e->env_no_twin || o->variant != 0 || o->first % 8) return;
 	ev->rows = nullptr;
@@ -741,6 +750,7 @@ void route_twin(const apo_engine *e, const apo_score_opts *o, Evals *ev) {
 		ev->tl = e->tt_l.p; ev->th = e->tt_h.p;
 		ev->tb_pc = e->tt_pc.p; ev->tb_pd = e->tt_pd.p; ev->n_tuples = e->tt_n; ev->d2book = e->tt_d2.p;
 		ev->codebook = e->tt_book; ev->tval = e->tt_val[recip].p;
+		if (e->tt_t2 && !e->env_no_twin_t2) { ev->t2 = true; ev->xs = e->tt_xs.p; ev->xb = e->tt_xb.p; ev->xb_pitch = e->tt_nblk + 1; }
 		return;
 	}
 	if (e->twin_w) {                                         // <= 15 codes per dimension: the prefix table always fits
@@ -760,7 +770,13 @@ int launch_score(apo_engine *e, const apo_score_opts *o, const Evals &ev, uint32
 	int rc;
 	if (ev.codebook && !ev.tval && (rc = tuples_values(e, ev.codebook, ev.tb_pc, ev.tb_pd, ev.n_tuples, ev.d2book, recip))) return rc;
 	if ((rc = record_k1_event(e, 0))) return rc;
-	if (ev.form == apo::CAND_T) {
+	if (ev.form == apo::CAND_T && ev.t2) {
+		apo::Kt2Params P{};
+		P.tl = ev.tl; P.pitch_evals = ev.pitch_evals; P.C = ev.C; P.T = ev.count; P.first = ev.idx_base;
+		P.acc = acc; P.tval = ev.tval; P.n_tuples = ev.n_tuples;
+		P.xs = ev.xs; P.xb = ev.xb; P.xb_pitch = ev.xb_pitch;
+		CK(apo::run_reward9t2(P, e->sm_count, e->stream));
+	} else if (ev.form == apo::CAND_T) {
 		apo::KtParams P{};
 		P.tl = ev.tl; P.th = ev.th; P.pitch_evals = ev.pitch_evals; P.C = ev.C; P.T = ev.count;
 		P.acc = acc; P.n_tuples = ev.n_tuples;
@@ -1184,6 +1200,7 @@ extern "C" int apo_create(int device, apo_engine **out) {
 	e->env_no_twin = getenv("APO_NO_TWIN") != nullptr;
 	e->env_no_twin_t = getenv("APO_NO_TWIN_T") != nullptr;
 	e->env_twin_t = getenv("APO_TWIN_T") != nullptr;
+	e->env_no_twin_t2 = getenv("APO_NO_TWIN_T2") != nullptr;
 	if ((c =cudaStreamCreateWithFlags(&e->own_stream, cudaStreamNonBlocking)) != cudaSuccess) return bail("cudaStreamCreate", c);
 	if ((c = cudaStreamCreateWithFlags(&e->copy_stream, cudaStreamNonBlocking)) != cudaSuccess) return bail("cudaStreamCreate", c);
 	e->stream = e->own_stream;
@@ -1238,12 +1255,14 @@ extern "C" int apo_set_stream(apo_engine *e, uint64_t cuda_stream) {
 
 extern "C" int apo_set_tuning(apo_engine *e, uint32_t flags) {
 	if (!e) return APO_E_ARG;
-	if (flags & ~(APO_TUNE_NO_FUSE | APO_TUNE_FORCE_FUSE | APO_TUNE_NO_STAGING | APO_TUNE_NCCL_JOIN | APO_TUNE_NO_TWIN | APO_TUNE_NO_TWIN_T | APO_TUNE_TWIN_T))
+	if (flags & ~(APO_TUNE_NO_FUSE | APO_TUNE_FORCE_FUSE | APO_TUNE_NO_STAGING | APO_TUNE_NCCL_JOIN | APO_TUNE_NO_TWIN | APO_TUNE_NO_TWIN_T | APO_TUNE_TWIN_T |
+	              APO_TUNE_NO_TWIN_T2))
 		return fail(e, APO_E_ARG, "unknown tuning flag %#x", flags);
 	e->env_no_fuse = (flags & APO_TUNE_NO_FUSE) != 0; e->env_force_fuse = (flags & APO_TUNE_FORCE_FUSE) != 0;
 	e->env_no_staging = (flags & APO_TUNE_NO_STAGING) != 0; e->env_nccl_join = (flags & APO_TUNE_NCCL_JOIN) != 0;
 	e->env_no_twin = (flags & APO_TUNE_NO_TWIN) != 0;
 	e->env_no_twin_t = (flags & APO_TUNE_NO_TWIN_T) != 0; e->env_twin_t = (flags & APO_TUNE_TWIN_T) != 0;
+	e->env_no_twin_t2 = (flags & APO_TUNE_NO_TWIN_T2) != 0;
 	return APO_OK;
 }
 
@@ -1983,7 +2002,8 @@ int tb_reserve(apo_engine *e, DevBuf<T> &b, uint64_t n, const char *what, bool c
 	return fail(e, c == cudaErrorMemoryAllocation ? APO_E_NOMEM : APO_E_CUDA, "%s (%llu elements): %s", what, (unsigned long long)n, cudaGetErrorString(c));
 }
 
-int dims_tuples(apo_engine *e, uint32_t cap, uint32_t *n_tuples, const TupleDst &D) {
+// *n_high (may be NULL): the evaluations whose index is >= 2^16
+int dims_tuples(apo_engine *e, uint32_t cap, uint32_t *n_tuples, const TupleDst &D, uint64_t *n_high = nullptr) {
 	if ((!e->dims_ptr && !e->compact) || e->dims_C == 0) return fail(e, APO_E_STATE, "no dims loaded");
 	if (!e->compact && (!e->twin || e->env_no_twin))
 		return fail(e, APO_E_STATE, "the loaded Form D tensor has no Form W / Q copy to build Form T from (APO_TUNE_NO_TWIN, apo_dims_attach, "
@@ -2061,6 +2081,10 @@ int dims_tuples(apo_engine *e, uint32_t cap, uint32_t *n_tuples, const TupleDst 
 		for (uint32_t r = 0; r < n && r < kTwinTHot; r++) head += order[r].first;
 		if (head * 4 < N * 3) return APO_E_STATE;
 	}
+	if (n_high) {
+		*n_high = 0;
+		for (uint32_t r = 65536; r < n; r++) *n_high += order[r].first;
+	}
 	std::vector<uint32_t> tb_pc(n);
 	std::vector<uint16_t> tb_pd(n);
 	for (uint32_t r = 0; r < n; r++) {
@@ -2099,6 +2123,32 @@ int dims_tuples(apo_engine *e, uint32_t cap, uint32_t *n_tuples, const TupleDst 
 // build's scratch; otherwise no copy is kept, without an error.  The build also computes the table values for the weights.
 constexpr uint64_t kTwinTMinEvals = 1ull << 26;
 constexpr uint32_t kTwinTCap = 1u << 20;
+
+// The exception list of the Form T copy: with it resident Form D calls read 2 B per evaluation through K1t2 instead of 3 B
+// through K1t (route_twin).  Built from n_high, the evaluations whose index is >= 2^16 (known from the dictionary's
+// counts), when at most 1/kTwinT2Share of the evaluations are such exceptions (DESIGN §8: K1t2 corrects each one with
+// three dependent loads after its stream) and a row's positions fit 32 bits; otherwise, or without room for it, the copy
+// is read through K1t as before, without an error.  APO_TUNE_NO_TWIN_T2 at the load builds none.
+constexpr uint64_t kTwinT2Share = 64;
+int build_twin_t2(apo_engine *e, uint64_t n_high) {
+	const uint32_t C = e->tt_C;
+	const uint64_t T = e->tt_T;
+	if (e->env_no_twin_t2 || n_high * kTwinT2Share > (uint64_t)C * T || T > 0xFFFFFFFFull || n_high > 0xFFFFFFFFull) return APO_OK;
+	if (n_high) {
+		const uint32_t nblk = (uint32_t)((T + apo::KT_XBLOCK - 1) / apo::KT_XBLOCK);
+		if (e->tt_xb.reserve((uint64_t)C * (nblk + 1)) != cudaSuccess || e->tt_xs.reserve(n_high) != cudaSuccess) {
+			cudaGetLastError();
+			e->tt_xb.release(); e->tt_xs.release();
+			return APO_OK;
+		}
+		CK(apo::run_tx_build(e->tt_l.p, e->tt_h.p, e->tt_pitch, C, T, e->tt_xb.p, e->tt_xs.p, e->sm_count, e->stream));
+		CK(cudaStreamSynchronize(e->stream));                     // the load returns with the list built, as with the copy
+		e->tt_xn = n_high; e->tt_nblk = nblk;
+	}
+	e->tt_t2 = true;
+	return APO_OK;
+}
+
 int build_twin_t(apo_engine *e) {
 	const uint32_t C = e->dims_C;
 	const uint64_t T = e->dims_T, N = (uint64_t)C * T;
@@ -2109,20 +2159,24 @@ int build_twin_t(apo_engine *e) {
 	const uint64_t m = std::min<uint64_t>(kTwinTCap, N);
 	uint64_t slots = 1024;
 	while (slots < 2 * (m + 1)) slots <<= 1;
-	// index planes, dictionary, value tables; the build's hash table, keys and counts
-	const uint64_t need = 3 * (uint64_t)C * round_up(T, 64) + m * 6 + 2 * (m + 1) * 8 + 16 * slots + 16 * m;
+	// index planes, dictionary, value tables, the largest exception list and its block index; the build's hash table, keys
+	// and counts
+	const uint64_t need = 3 * (uint64_t)C * round_up(T, 64) + m * 6 + 2 * (m + 1) * 8 + 8 * (N / kTwinT2Share) +
+	                      4 * (uint64_t)C * (T / apo::KT_XBLOCK + 2) + 16 * slots + 16 * m;
 	size_t free_bytes = 0, total_bytes = 0;
 	CK(cudaMemGetInfo(&free_bytes, &total_bytes));
 	if ((uint64_t)free_bytes < need + kTwinHeadroom) return APO_OK;
 	const std::string keep_err = e->err;
 	uint32_t n = 0;
-	int rc = dims_tuples(e, kTwinTCap, &n, copy_tuples(e));
+	uint64_t n_high = 0;
+	int rc = dims_tuples(e, kTwinTCap, &n, copy_tuples(e), &n_high);
 	if (rc == APO_OK && (e->tt_val[0].reserve(n + 1ull) != cudaSuccess || e->tt_val[1].reserve(n + 1ull) != cudaSuccess ||
 	                     e->tt_ptab.reserve(8 * 256) != cudaSuccess || e->tt_bad.reserve(1) != cudaSuccess)) {
 		cudaGetLastError();
 		rc = APO_E_NOMEM;
 	}
 	if (rc == APO_OK) rc = twin_t_values(e, false);
+	if (rc == APO_OK) rc = build_twin_t2(e, n_high);
 	if (rc != APO_OK) cudaStreamSynchronize(e->stream);          // nothing queued may still use what is released
 	e->tb_table.release(); e->tb_keys.release(); e->tb_cnt.release(); e->tb_misc.release();
 	if (rc == APO_OK) return APO_OK;
@@ -2211,6 +2265,18 @@ extern "C" int apo_debug_partials(apo_engine *e, int64_t *out, uint32_t C) {
 	if (C != e->last_C || !e->acc.p) return fail(e, APO_E_STATE, "no scoring call with C=%u to read back", C);
 	CK(cudaSetDevice(e->device));
 	CK(cudaMemcpyAsync(out, e->partials_src ? e->partials_src : e->acc.p, 8ull * ACC_PER_CAND * C, cudaMemcpyDeviceToHost, e->stream));
+	CK(cudaStreamSynchronize(e->stream));
+	return APO_OK;
+}
+
+extern "C" int apo_debug_twin_t_list(apo_engine *e, uint64_t *n_words, uint64_t *n_exceptions, uint32_t *xb, uint32_t *xs) {
+	if (!e || !n_words || !n_exceptions) return fail(e, APO_E_ARG, "NULL argument");
+	*n_words = e->tt_xn ? (uint64_t)e->tt_C * (e->tt_nblk + 1) : 0;
+	*n_exceptions = e->tt_xn;
+	if (!e->tt_xn) return APO_OK;
+	CK(cudaSetDevice(e->device));
+	if (xb) CK(cudaMemcpyAsync(xb, e->tt_xb.p, *n_words * 4, cudaMemcpyDeviceToHost, e->stream));
+	if (xs) CK(cudaMemcpyAsync(xs, e->tt_xs.p, e->tt_xn * 8, cudaMemcpyDeviceToHost, e->stream));
 	CK(cudaStreamSynchronize(e->stream));
 	return APO_OK;
 }

@@ -190,6 +190,35 @@ int kt_tile_evals();
 cudaError_t run_tuple_values(const TupleValParams &P, bool recip, cudaStream_t st);
 cudaError_t run_reward9t(KtParams P, int sm_count, cudaStream_t st);
 
+// K1t2 (k_reward9t2): the Form T copy of a resident Form D tensor read from its 16-bit plane alone, 2 B per evaluation.  The
+// dictionary is in frequency order, so an index >= 2^16 is rare; such evaluations (exceptions) are listed per row, sorted by
+// position, as {position in the row, full index}, and the kernel replaces table[index & 0xFFFF], which the stream added, by
+// table[index].  xb[c][b] is the list offset of the first exception of row c at or after position b * KT_XBLOCK (b <= nblk:
+// xb[c][nblk] = xb[c + 1][0] ends the row), so any window finds its exceptions without a search.
+constexpr uint32_t KT_XBLOCK = 8192;
+struct Kt2Params {
+	const unsigned short *tl;       // [C][pitch] low 16 bits of the index, from the window start (a multiple of 8)
+	uint64_t pitch_evals;           // multiple of 8; tl 16-byte aligned
+	uint32_t C;
+	uint32_t tiles_per_cand;
+	uint64_t T;                     // evaluations of the window
+	uint64_t first;                 // window start in the row: the list's positions are absolute
+	uint64_t total_tiles;
+	long long *acc;
+	const long long *tval;          // [n_tuples + 1]
+	uint32_t n_tuples;
+	uint32_t hot;                   // entries [0, hot) are served from shared memory
+	const uint2 *xs;                // exceptions, or NULL: every index is below 2^16
+	const uint32_t *xb;             // [C][xb_pitch] block index of xs
+	uint32_t xb_pitch;              // blocks per row + 1
+};
+int kt2_tile_evals();
+cudaError_t run_reward9t2(Kt2Params P, int sm_count, cudaStream_t st);
+// the exception list of tl / th [C][tpitch] (T evaluations per row, T < 2^32): xb [C][nblk + 1] (nblk = ceil(T / KT_XBLOCK)),
+// then xs [xb[C - 1][nblk]].  The same bytes for every grid.
+cudaError_t run_tx_build(const unsigned short *tl, const unsigned char *th, uint64_t tpitch, uint32_t C, uint64_t T, uint32_t *xb,
+                         uint2 *xs, int sm_count, cudaStream_t st);
+
 // Form T built on the device from a resident tensor's Form W words or Form Q planes (apo_dims_tuples).  The key of an
 // evaluation is its Form W word: eight 4-bit codes in the low half, the fp32 tool_success_rate bits (KW_D2_ABSENT = absent)
 // in the high half; the host maps the high half to the d2book index afterwards.  Hash tables hold {key, value} pairs,

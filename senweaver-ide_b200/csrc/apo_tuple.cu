@@ -198,6 +198,253 @@ cudaError_t run_reward9t(KtParams P, int sm_count, cudaStream_t st) {
 	return cudaGetLastError();
 }
 
+// =================================================================== K1t2: the Form T copy from its 16-bit plane
+// The same gather-and-add as K1t over tl alone: the registers th took carry a second 16-byte word, so each thread keeps
+// 16 evaluations (32 B) in flight instead of 8 (24 B).  The exceptions (index >= 2^16, csrc/apo_kernels.h) of a CTA's
+// (candidate, tile range) segments are corrected by the CTA itself once its stream is done, with four independent
+// exceptions in flight per thread.
+constexpr int KT2_STEPS = 2;
+constexpr int KT2_TILE = KT_STEP_EVALS * KT2_STEPS;    // 16384 evaluations
+constexpr int KT2_XUNROLL = 4;                         // exceptions in flight per thread in the correction
+
+static_assert(KT_GROUP * KT2_STEPS <= 16, "the count field of a table entry sits 5 bits above the largest 16-entry sum");
+static_assert(KT_HOT_MAX <= 65536, "an exception's full index is never in the shared-memory head");
+
+int kt2_tile_evals() { return KT2_TILE; }
+
+// table entry -> (value, count)
+__device__ __forceinline__ long long kt_split(long long v, int &k) {
+	const long long kk = (v + (1ll << (KT_VALID_SHIFT - 1))) >> KT_VALID_SHIFT;
+	k = (int)kk;
+	return v - (kk << KT_VALID_SHIFT);
+}
+
+__global__ void __launch_bounds__(KT_THREADS, 1)
+k_reward9t2(const Kt2Params P) {
+	extern __shared__ __align__(16) long long s_hot[];
+	const int tid = threadIdx.x, lane = tid & 31;
+	for (uint32_t i = tid; i < P.hot; i += KT_THREADS) s_hot[i] = P.tval[i];
+	__syncthreads();
+	const uint32_t s_base = smem_u32(s_hot);
+	const uint32_t hot = P.hot;
+	const long long *tval = P.tval;
+
+	const uint64_t lo_t = P.total_tiles * blockIdx.x / gridDim.x;
+	const uint64_t hi_t = P.total_tiles * (blockIdx.x + 1ull) / gridDim.x;
+	if (lo_t >= hi_t) return;
+
+	uint32_t c = (uint32_t)(lo_t / P.tiles_per_cand), j = (uint32_t)(lo_t - (uint64_t)c * P.tiles_per_cand);
+	uint32_t cn = c, jn = j;
+	auto tile_n = [&](uint32_t jj) -> uint32_t {
+		const uint64_t rem = P.T - (uint64_t)jj * KT2_TILE;
+		return rem < (uint64_t)KT2_TILE ? (uint32_t)rem : (uint32_t)KT2_TILE;
+	};
+	auto prefetch = [&](uint32_t cc, uint32_t jj, uint4 (&R)[KT2_STEPS]) {
+		if (tile_n(jj) != (uint32_t)KT2_TILE) return;              // ragged row end: read by the scalar loop instead
+		const uint64_t e0 = (uint64_t)cc * P.pitch_evals + (uint64_t)jj * KT2_TILE + (uint64_t)tid * KT_GROUP;
+#pragma unroll
+		for (int k = 0; k < KT2_STEPS; k++) R[k] = ld_stream16(P.tl + e0 + (uint64_t)k * KT_STEP_EVALS);
+	};
+
+	Acc128 acc; acc.zero();
+	int cnt = 0;                                               // signed: a correction may remove more counts than a warp added
+	// the exceptions of window tiles [ja, jb) of row cc
+	auto correct = [&](uint32_t cc, uint32_t ja, uint32_t jb) {
+		const uint64_t lo = P.first + (uint64_t)ja * KT2_TILE;
+		const uint64_t hi = P.first + min((uint64_t)jb * KT2_TILE, P.T);
+		const uint32_t *xr = P.xb + (uint64_t)cc * P.xb_pitch;
+		const uint32_t x0 = xr[lo / KT_XBLOCK], x1 = xr[(hi - 1) / KT_XBLOCK + 1];   // the blocks holding [lo, hi)
+		for (uint32_t x = x0 + tid; x < x1; x += KT2_XUNROLL * KT_THREADS) {
+			uint32_t full[KT2_XUNROLL];
+#pragma unroll
+			for (int u = 0; u < KT2_XUNROLL; u++) {
+				const uint32_t xi = x + u * KT_THREADS;
+				const uint2 ex = xi < x1 ? __ldg(P.xs + xi) : make_uint2(0u, 0u);
+				full[u] = xi < x1 && ex.x >= lo && ex.x < hi ? ex.y : 0u;   // index 0: both entries equal, no change
+			}
+#pragma unroll
+			for (int u = 0; u < KT2_XUNROLL; u++) {
+				int kf, kl;
+				const long long vf = kt_split(tuple_entry(full[u], hot, s_base, tval), kf);
+				const long long vl = kt_split(tuple_entry(full[u] & 0xFFFFu, hot, s_base, tval), kl);
+				acc.add(vf - vl);
+				cnt += kf - kl;
+			}
+		}
+	};
+	auto flush = [&](int cand) {
+		long long *dst = P.acc + (uint64_t)ACC_PER_CAND * cand;
+		flush_acc128(acc, dst, lane);
+		const int n = (int)warp_sum_u32((uint32_t)cnt);
+		if (lane == 0 && n) atomicAdd((unsigned long long *)dst + 3, (unsigned long long)(long long)n);   // two's complement: a signed add
+		acc.zero(); cnt = 0;
+	};
+
+	uint4 R[KT2_STEPS] = {}, N[KT2_STEPS] = {};
+	prefetch(c, j, R);
+	int cur = -1;
+	for (uint64_t tile = lo_t; tile < hi_t; ++tile) {
+		if (++jn == P.tiles_per_cand) { jn = 0; cn++; }
+		if (tile + 1 < hi_t) prefetch(cn, jn, N);
+		if ((int)c != cur) { if (cur >= 0) flush(cur); cur = (int)c; }
+		const uint32_t n = tile_n(j);
+		if (n == (uint32_t)KT2_TILE) {
+			long long s = 0;
+#pragma unroll
+			for (int k = 0; k < KT2_STEPS; k++) {
+				const uint32_t lw[4] = {R[k].x, R[k].y, R[k].z, R[k].w};
+#pragma unroll
+				for (int q = 0; q < KT_GROUP; q++) s += tuple_entry((lw[q >> 1] >> (16 * (q & 1))) & 0xFFFFu, hot, s_base, tval);
+			}
+			int k16;
+			acc.add(kt_split(s, k16));                         // 16 entries: values in (-2^57, 2^57) + count * 2^58
+			cnt += k16;
+		} else {
+			const uint64_t e0 = (uint64_t)c * P.pitch_evals + (uint64_t)j * KT2_TILE;
+			for (uint32_t e = tid; e < n; e += KT_THREADS) {
+				const uint32_t idx = P.tl[e0 + e];
+				int k1;
+				acc.add(kt_split(idx < hot ? s_hot[idx] : __ldg(tval + idx), k1));
+				cnt += k1;
+			}
+		}
+#pragma unroll
+		for (int k = 0; k < KT2_STEPS; k++) R[k] = N[k];
+		c = cn; j = jn;
+	}
+	flush(cur);
+	// the corrections after the stream, one flush per candidate segment: inside the loop they would spill the prefetch
+	if (!P.xs) return;
+	const uint32_t c_lo = (uint32_t)(lo_t / P.tiles_per_cand), c_hi = (uint32_t)((hi_t - 1) / P.tiles_per_cand);
+	for (uint32_t cc = c_lo; cc <= c_hi; cc++) {
+		const uint32_t ja = cc == c_lo ? (uint32_t)(lo_t - (uint64_t)cc * P.tiles_per_cand) : 0u;
+		const uint32_t jb = cc == c_hi ? (uint32_t)(hi_t - (uint64_t)cc * P.tiles_per_cand) : P.tiles_per_cand;
+		correct(cc, ja, jb);
+		flush((int)cc);
+	}
+}
+
+namespace {
+int k1_env_grid() { static const int g = [] { const char *s = getenv("APO_K1_GRID"); return s ? atoi(s) : 0; }(); return g; }
+}  // namespace
+
+cudaError_t run_reward9t2(Kt2Params P, int sm_count, cudaStream_t st) {
+	P.tiles_per_cand = (uint32_t)((P.T + KT2_TILE - 1) / KT2_TILE);
+	P.total_tiles = (uint64_t)P.tiles_per_cand * P.C;
+	if (P.total_tiles == 0) return cudaSuccess;
+	const uint64_t entries = (uint64_t)P.n_tuples + 1;
+	P.hot = (uint32_t)(entries < KT_HOT_MAX ? entries : KT_HOT_MAX);
+	const int smem = (int)(((uint64_t)P.hot * 8 + 15) & ~15ull);
+	cudaError_t err = allow_big_smem(k_reward9t2, (int)(KT_HOT_MAX * 8));
+	if (err != cudaSuccess) return err;
+	int grid = sm_count;
+	if (k1_env_grid() > 0 && k1_env_grid() < grid) grid = k1_env_grid();   // tests: every CTA cut of the rows and the list
+	if ((uint64_t)grid > P.total_tiles) grid = (int)P.total_tiles;
+	k_reward9t2<<<grid, KT_THREADS, smem, st>>>(P);
+	return cudaGetLastError();
+}
+
+// ---- the exception list, built on the device from the planes: a count pass per (row, block), one exclusive scan over
+// [C][nblk + 1], and an ordered write pass.  Each (row, block) is one CTA's item, 32 evaluations per thread.
+constexpr int TX_THREADS = 256;
+constexpr int TX_EVALS = KT_XBLOCK / TX_THREADS;       // 32
+static_assert(TX_EVALS == 32, "one bit per evaluation of a thread");
+
+// bit q: evaluation t0 + q (< T) of the row has a non-zero high byte
+__device__ __forceinline__ uint32_t tx_mask(const unsigned char *th_row, uint64_t t0, uint64_t T) {
+	if (t0 >= T) return 0u;
+	const uint4 a = ld_stream16(th_row + t0), b = ld_stream16(th_row + t0 + 16);   // inside the row's 64-padded pitch
+	const uint32_t w[8] = {a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w};
+	uint32_t m = 0;
+#pragma unroll
+	for (int q = 0; q < 32; q++) m |= (((w[q >> 2] >> (8 * (q & 3))) & 0xFFu) != 0u ? 1u : 0u) << q;
+	const uint64_t left = T - t0;
+	return left >= 32 ? m : m & ((1u << left) - 1u);
+}
+
+__global__ void __launch_bounds__(TX_THREADS)
+k_tx_count(const unsigned char *th, uint64_t tpitch, uint32_t C, uint64_t T, uint32_t nblk, uint32_t *xb) {
+	__shared__ uint32_t s_w[TX_THREADS / 32];
+	const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+	for (uint64_t it = blockIdx.x; it < (uint64_t)C * nblk; it += gridDim.x) {
+		const uint32_t c = (uint32_t)(it / nblk), b = (uint32_t)(it - (uint64_t)c * nblk);
+		const uint32_t n = warp_sum_u32((uint32_t)__popc(tx_mask(th + (uint64_t)c * tpitch, (uint64_t)b * KT_XBLOCK + threadIdx.x * TX_EVALS, T)));
+		if (lane == 0) s_w[warp] = n;
+		__syncthreads();
+		if (threadIdx.x == 0) {
+			uint32_t s = 0;
+			for (int w = 0; w < TX_THREADS / 32; w++) s += s_w[w];
+			xb[(uint64_t)c * (nblk + 1) + b] = s;
+			if (b == nblk - 1) xb[(uint64_t)c * (nblk + 1) + nblk] = 0;
+		}
+		__syncthreads();
+	}
+}
+
+// exclusive scan of xb[0, n) in place, one CTA: each thread a contiguous run
+__global__ void __launch_bounds__(1024)
+k_tx_scan(uint32_t *xb, uint64_t n) {
+	__shared__ uint32_t s_w[32];
+	const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+	const uint64_t per = (n + 1023) / 1024, lo = min(n, (uint64_t)threadIdx.x * per), hi = min(n, lo + per);
+	uint32_t s = 0;
+	for (uint64_t i = lo; i < hi; i++) s += xb[i];
+	uint32_t incl = s;
+#pragma unroll
+	for (int o = 1; o < 32; o <<= 1) { const uint32_t v = __shfl_up_sync(0xFFFFFFFFu, incl, o); if (lane >= (uint32_t)o) incl += v; }
+	if (lane == 31) s_w[warp] = incl;
+	__syncthreads();
+	if (warp == 0) {
+		uint32_t w = s_w[lane];
+#pragma unroll
+		for (int o = 1; o < 32; o <<= 1) { const uint32_t v = __shfl_up_sync(0xFFFFFFFFu, w, o); if (lane >= (uint32_t)o) w += v; }
+		s_w[lane] = w;
+	}
+	__syncthreads();
+	uint32_t run = (warp ? s_w[warp - 1] : 0u) + incl - s;
+	for (uint64_t i = lo; i < hi; i++) { const uint32_t v = xb[i]; xb[i] = run; run += v; }
+}
+
+__global__ void __launch_bounds__(TX_THREADS)
+k_tx_write(const unsigned short *tl, const unsigned char *th, uint64_t tpitch, uint32_t C, uint64_t T, uint32_t nblk, const uint32_t *xb, uint2 *xs) {
+	__shared__ uint32_t s_w[TX_THREADS / 32];
+	const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+	for (uint64_t it = blockIdx.x; it < (uint64_t)C * nblk; it += gridDim.x) {
+		const uint32_t c = (uint32_t)(it / nblk), b = (uint32_t)(it - (uint64_t)c * nblk);
+		const uint64_t t0 = (uint64_t)b * KT_XBLOCK + threadIdx.x * TX_EVALS;
+		uint32_t m = tx_mask(th + (uint64_t)c * tpitch, t0, T);
+		const uint32_t n = (uint32_t)__popc(m);
+		uint32_t incl = n;
+#pragma unroll
+		for (int o = 1; o < 32; o <<= 1) { const uint32_t v = __shfl_up_sync(0xFFFFFFFFu, incl, o); if (lane >= (uint32_t)o) incl += v; }
+		if (lane == 31) s_w[warp] = incl;
+		__syncthreads();
+		uint32_t o = xb[(uint64_t)c * (nblk + 1) + b] + incl - n;
+		for (uint32_t w = 0; w < warp; w++) o += s_w[w];
+		while (m) {
+			const uint32_t q = (uint32_t)(__ffs(m) - 1);
+			m &= m - 1;
+			const uint64_t t = t0 + q, off = (uint64_t)c * tpitch + t;
+			xs[o++] = make_uint2((uint32_t)t, (uint32_t)tl[off] | ((uint32_t)th[off] << 16));
+		}
+		__syncthreads();
+	}
+}
+
+cudaError_t run_tx_build(const unsigned short *tl, const unsigned char *th, uint64_t tpitch, uint32_t C, uint64_t T, uint32_t *xb,
+                         uint2 *xs, int sm_count, cudaStream_t st) {
+	const uint32_t nblk = (uint32_t)((T + KT_XBLOCK - 1) / KT_XBLOCK);
+	const uint64_t items = (uint64_t)C * nblk;
+	if (items == 0) return cudaSuccess;
+	uint64_t grid = 8ull * (uint64_t)sm_count;
+	if (k1_env_grid() > 0 && (uint64_t)k1_env_grid() < grid) grid = (uint64_t)k1_env_grid();
+	if (grid > items) grid = items;
+	k_tx_count<<<(unsigned)grid, TX_THREADS, 0, st>>>(th, tpitch, C, T, nblk, xb);
+	k_tx_scan<<<1, 1024, 0, st>>>(xb, (uint64_t)C * (nblk + 1));
+	k_tx_write<<<(unsigned)grid, TX_THREADS, 0, st>>>(tl, th, tpitch, C, T, nblk, xb, xs);
+	return cudaGetLastError();
+}
+
 // =================================================================== Form T built on the device (apo_dims_tuples)
 // Two passes over the resident evaluations, 8 per thread and step (one row segment of 64 B of Form W):
 //   count: exact counts of the distinct keys.  A warp first merges equal keys (match.any), then each CTA adds them into its
