@@ -82,6 +82,49 @@ struct DevBuf {
 
 inline uint64_t round_up(uint64_t x, uint64_t m) { return (x + m - 1) / m * m; }
 
+// K1q's lookup tables for one Form Q / P codebook under the weights of generation `gen` (load_qtables)
+struct QTables {
+	uint32_t book[8 * 256];
+	DevBuf<double> ptab, pair; DevBuf<float> cbf;
+	uint32_t n0 = 0, n1 = 0; bool pair_ok = false;
+	uint64_t gen = 0;                        // apo_engine::weights_gen the tables were built for; 0: not built
+	void release() { ptab.release(); pair.release(); cbf.release(); gen = 0; }
+};
+
+// Form T (csrc/apo_tuple.cu): a dictionary of distinct evaluations as Form P pairs, with its d2book and codebook
+struct TupleDict {
+	DevBuf<uint32_t> pc; DevBuf<unsigned short> pd; DevBuf<float> d2;
+	uint32_t book[8 * 256]; uint32_t n = 0;
+	void release() { pc.release(); pd.release(); d2.release(); }
+};
+
+// a resident Form T tensor: the dictionary and the [C][pitch] index planes
+struct TupleTensor : TupleDict {
+	DevBuf<unsigned short> l; DevBuf<unsigned char> h; uint32_t C = 0; uint64_t T = 0, pitch = 0;
+	void unload() { C = 0; T = 0; n = 0; }
+	void release() { TupleDict::release(); l.release(); h.release(); unload(); }
+};
+
+// A dictionary's table values rint(finalReward·2^52) (tuple_values).  Held (the Form T copy): val[recip] keeps the values of
+// the current weights and ok[recip] says whether they are computed (0 not yet, 1 valid, 2 an entry is outside Form T's
+// (-2, 2) domain).  Otherwise the values of one call in val[0], checked once it has synchronised (finish_score).
+struct TupleVals {
+	const bool held;
+	DevBuf<double> ptab; DevBuf<long long> val[2]; DevBuf<uint32_t> bad;
+	uint8_t ok[2] = {0, 0};
+	explicit TupleVals(bool held = false) : held(held) {}
+	long long *out(bool recip) const { return val[held && recip].p; }
+	void release() { ptab.release(); val[0].release(); val[1].release(); bad.release(); ok[0] = ok[1] = 0; }
+};
+
+// The Form T copy of a large resident Form D tensor (build_twin_t), its held values and its exception list (build_twin_t2):
+// t2 = K1t2 may read the copy from `l` alone; xs / xb hold the xn evaluations whose index is >= 2^16 and their block index.
+struct TupleCopy : TupleTensor {
+	TupleVals vals{true};
+	DevBuf<uint2> xs; DevBuf<uint32_t> xb; uint64_t xn = 0; uint32_t nblk = 0; bool t2 = false;
+	void release() { TupleTensor::release(); vals.release(); xs.release(); xb.release(); xn = 0; nblk = 0; t2 = false; }
+};
+
 }  // namespace
 
 struct apo_engine {
@@ -97,31 +140,24 @@ struct apo_engine {
 	// Form Q (compact) copy of the evaluations: replaces dims/dims_ptr when `compact` is set; when `twin` is set it sits beside
 	// the engine's own fp32 tensor (built at load, a cache that is released whenever device memory runs short: see reserve)
 	DevBuf<unsigned long long> q8; DevBuf<float> qd2; DevBuf<unsigned short> qli; DevBuf<uint32_t> qbook;   // qbook: [8][256] codebook + [8] overflow flags
-	DevBuf<double> d_ptab, d_pair; DevBuf<float> stage, d_cbf, d_d2book, d_d2stream; uint32_t q_n0 = 0, q_n1 = 0; bool q_pair_ok = false;
+	DevBuf<float> stage, d_d2book, d_d2stream;
 	DevBuf<uint32_t> unpack_bad;                              // k_unpack_p: an evaluation named an empty or NaN codebook slot
-	uint32_t qbook_host[8 * 256]; bool compact = false, twin = false;
+	bool compact = false, twin = false;
+	// K1q's tables: qt for the resident Form Q tensor or the Form Q / W copy (rebuilt by apo_set_weights), qt_stream for the
+	// host-streaming Form Q / P calls (rebuilt by the next such call when its codebook or the weights changed)
+	QTables qt, qt_stream; uint64_t weights_gen = 1;
 	// twin_w: the copy is held as Form W words (qw, 8 B per evaluation; the Form Q planes are released) because no coded
 	// dimension has more than 15 values
 	DevBuf<unsigned long long> qw; bool twin_w = false;
 	uint32_t d2book_host[4096]; uint32_t d2book_n = ~0u;       // Form P export of the resident tensor (~0 = not built yet)
 	DevBuf<uint8_t> roll; uint32_t roll_C = 0, roll_row = 32; uint64_t roll_T = 0, roll_pitch = 0;   // Form R (32 B) or R16 (16 B) rows
-	// Form T (csrc/apo_tuple.cu): resident index planes + dictionary; per call: product table of its codebook, table values
-	DevBuf<unsigned short> tup_l; DevBuf<unsigned char> tup_h; uint32_t tup_C = 0, tup_n = 0; uint64_t tup_T = 0, tup_pitch = 0;
-	DevBuf<uint32_t> tup_pc, tup_bad; DevBuf<unsigned short> tup_pd; DevBuf<float> tup_d2; DevBuf<double> tup_ptab; DevBuf<long long> tup_val;
-	uint32_t tup_book[8 * 256]; bool tup_used = false;
-	DevBuf<uint32_t> tups_pc; DevBuf<unsigned short> tups_pd; DevBuf<float> tups_d2;   // dictionary of a host-streaming call
+	TupleTensor tup;                      // resident Form T (apo_tuples_upload / apo_dims_tuples)
+	TupleDict tups;                       // the dictionary of a host-streaming Form T call
+	TupleVals tvals;                      // the values a resident Form T launch or a host-streaming Form T call computes
+	TupleVals *tvals_check = nullptr;     // the values the running call checks once it has synchronised
+	TupleCopy tcopy;                      // the Form T copy of the fp32 tensor, released with its Form W / Q copy
 	// apo_dims_tuples scratch (released when the build returns): hash table, (key, count) pairs / keys in rank order, counters
 	DevBuf<unsigned long long> tb_table, tb_keys, tb_cnt, tb_misc;
-	// Form T copy of a large resident Form D tensor (build_twin_t), beside its Form W / Q copy and released with it; never
-	// the Form T of apo_tuples_upload / apo_dims_tuples.  tt_val[recip]: the table values for the current weights, computed
-	// at build / apo_set_weights (recip = 0) or by the first call that asks (recip = 1); tt_ok[recip]: 0 not computed yet,
-	// 1 valid, 2 an entry is outside Form T's (-2, 2) domain (those calls read the Form W / Q copy)
-	DevBuf<unsigned short> tt_l; DevBuf<unsigned char> tt_h; DevBuf<uint32_t> tt_pc, tt_bad; DevBuf<unsigned short> tt_pd; DevBuf<float> tt_d2;
-	DevBuf<double> tt_ptab; DevBuf<long long> tt_val[2];
-	uint32_t tt_book[8 * 256]; uint32_t tt_C = 0, tt_n = 0; uint64_t tt_T = 0, tt_pitch = 0; uint8_t tt_ok[2] = {0, 0};
-	// the copy's exception list (build_twin_t2): tt_t2 = K1t2 may read the copy from tt_l alone; tt_xs / tt_xb hold the
-	// tt_xn evaluations whose index is >= 2^16 and their block index (none when the dictionary has <= 2^16 entries)
-	DevBuf<uint2> tt_xs; DevBuf<uint32_t> tt_xb; uint64_t tt_xn = 0; uint32_t tt_nblk = 0; bool tt_t2 = false;
 
 	// acc: [acc_words(C, nranks)] partial vector | [18] example scratch (inverted indices) | [1] ticket — one allocation, so one
 	// memset arms a scoring call.  acc_joined: the joined vector (> 1 rank); acc keeps this rank's partials.
@@ -184,15 +220,8 @@ int fail(apo_engine *e, int code, const char *fmt, ...) {
 		if (_c != cudaSuccess) return fail(e, APO_E_CUDA, "%s: %s (%s:%d)", #call, cudaGetErrorString(_c), __FILE__, __LINE__); \
 	} while (0)
 
-void drop_twin_t(apo_engine *e) {
-	e->tt_l.release(); e->tt_h.release(); e->tt_pc.release(); e->tt_pd.release(); e->tt_d2.release(); e->tt_bad.release(); e->tt_ptab.release();
-	e->tt_val[0].release(); e->tt_val[1].release(); e->tt_xs.release(); e->tt_xb.release();
-	e->tt_C = 0; e->tt_T = 0; e->tt_n = 0; e->tt_ok[0] = e->tt_ok[1] = 0;
-	e->tt_xn = 0; e->tt_nblk = 0; e->tt_t2 = false;
-}
-
 void drop_twin(apo_engine *e) {
-	drop_twin_t(e);
+	e->tcopy.release();
 	if (!e->twin) return;
 	e->q8.release(); e->qd2.release(); e->qli.release(); e->qw.release();
 	e->twin = e->twin_w = false;
@@ -298,35 +327,40 @@ std::vector<double> make_ptab(const uint32_t *book, const apo::Weights &W, doubl
 	return tab;
 }
 
-int upload_ptab(apo_engine *e) {
-	const std::vector<double> tab = make_ptab(e->qbook_host, e->W);
-	CK(reserve(e, e->d_ptab, 8 * 256));
-	CK(cudaMemcpyAsync(e->d_ptab.p, tab.data(), 8 * 256 * 8, cudaMemcpyHostToDevice, e->stream));
+// q's tables for `book` under the current weights, rebuilt unless q already holds exactly those
+int load_qtables(apo_engine *e, QTables &q, const uint32_t *book) {
+	if (q.gen == e->weights_gen && memcmp(q.book, book, sizeof q.book) == 0) return APO_OK;
+	q.gen = 0;                                                    // until the tables below are complete
+	memmove(q.book, book, sizeof q.book);                         // apo_set_weights rebuilds q from its own book
+	const std::vector<double> tab = make_ptab(q.book, e->W);
+	CK(reserve(e, q.ptab, 8 * 256));
+	CK(cudaMemcpyAsync(q.ptab.p, tab.data(), 8 * 256 * 8, cudaMemcpyHostToDevice, e->stream));
 	// tables of the mixed-lookup variants: fp32 values per code, and the exact two-term prefix of dimensions 0 and 1
 	std::vector<float> cbf(8 * 256, 0.0f);
 	uint32_t used[8] = {0};
 	for (int j = 0; j < 8; j++)
 		for (int c = 0; c < 255; c++) {
-			const uint32_t bits = e->qbook_host[256 * j + c];
+			const uint32_t bits = q.book[256 * j + c];
 			if (bits == 0xFFFFFFFFu) continue;
 			memcpy(&cbf[256 * j + c], &bits, 4);
 			used[j] = (uint32_t)c + 1;                                // dense codes: 0 .. used-1
 		}
-	e->q_n0 = used[0]; e->q_n1 = used[1];
-	e->q_pair_ok = (uint64_t)(used[0] + 1) * (used[1] + 1) <= (uint64_t)apo::KQ_PAIR_MAX;
+	q.n0 = used[0]; q.n1 = used[1];
+	q.pair_ok = (uint64_t)(used[0] + 1) * (used[1] + 1) <= (uint64_t)apo::KQ_PAIR_MAX;
 	std::vector<double> pair(apo::KQ_PAIR_MAX, 0.0);
-	if (e->q_pair_ok)
+	if (q.pair_ok)
 		for (uint32_t a = 0; a <= used[0]; a++)
 			for (uint32_t b = 0; b <= used[1]; b++) {
 				volatile double s = tab[a < used[0] ? a : 255];           // fl(0 + d0*w0), +0.0 when absent
 				s = s + tab[256 + (b < used[1] ? b : 255)];               // + d1*w1 (TCS:781, second push)
 				pair[a * (used[1] + 1) + b] = s;
 			}
-	CK(reserve(e, e->d_cbf, 8 * 256));
-	CK(reserve(e, e->d_pair, apo::KQ_PAIR_MAX));
-	CK(cudaMemcpyAsync(e->d_cbf.p, cbf.data(), 8 * 256 * 4, cudaMemcpyHostToDevice, e->stream));
-	CK(cudaMemcpyAsync(e->d_pair.p, pair.data(), apo::KQ_PAIR_MAX * 8, cudaMemcpyHostToDevice, e->stream));
+	CK(reserve(e, q.cbf, 8 * 256));
+	CK(reserve(e, q.pair, apo::KQ_PAIR_MAX));
+	CK(cudaMemcpyAsync(q.cbf.p, cbf.data(), 8 * 256 * 4, cudaMemcpyHostToDevice, e->stream));
+	CK(cudaMemcpyAsync(q.pair.p, pair.data(), apo::KQ_PAIR_MAX * 8, cudaMemcpyHostToDevice, e->stream));
 	CK(cudaStreamSynchronize(e->stream));
+	q.gen = e->weights_gen;
 	return APO_OK;
 }
 
@@ -376,8 +410,7 @@ int compact_finish(apo_engine *e, uint32_t C, uint64_t T, uint64_t pitch, bool t
 	CK(apo::run_recode(e->q8.p, e->qd2.p, e->qli.p, (uint64_t)C * pitch, (const uint8_t *)e->stage.p, e->stream));
 	CK(cudaMemcpyAsync(e->qbook.p, dense, sizeof dense, cudaMemcpyHostToDevice, e->stream));
 	CK(cudaStreamSynchronize(e->stream));
-	memcpy(e->qbook_host, dense, sizeof e->qbook_host);
-	int rc = upload_ptab(e);
+	int rc = load_qtables(e, e->qt, dense);
 	if (rc) return rc;
 	if (twin) e->twin = true;
 	else { e->compact = true; e->dims_C = C; e->dims_T = T; e->dims_pitch = pitch; e->dims_ptr = nullptr; }
@@ -410,7 +443,7 @@ int build_twin_wq(apo_engine *e) {
 	// TCS:668-763 produces) is kept as Form W words instead: 8 instead of 14 bytes per evaluation.  They are packed from the
 	// planes, so the build peaks at the fp32 tensor + the planes + the words; without kTwinHeadroom beside that, Form Q stays.
 	for (int j = 0; j < 8; j++)
-		if (e->qbook_host[256 * j + 15] != 0xFFFFFFFFu) return APO_OK;
+		if (e->qt.book[256 * j + 15] != 0xFFFFFFFFu) return APO_OK;
 	CK(cudaMemGetInfo(&free_bytes, &total_bytes));
 	if ((uint64_t)free_bytes < n * 8 + kTwinHeadroom) return APO_OK;
 	if (e->qw.reserve(n) != cudaSuccess) { cudaGetLastError(); return APO_OK; }
@@ -604,56 +637,36 @@ int record_k1_event(apo_engine *e, int which) {
 	return APO_OK;
 }
 
-// Form T: finalReward of every dictionary entry for the current weights (device work on e->stream, no synchronisation)
-int tuples_values(apo_engine *e, const uint32_t *book_host, const uint32_t *d_pc, const unsigned short *d_pd, uint32_t n, const float *d_d2, bool recip) {
-	const std::vector<double> tab = make_ptab(book_host, e->W, std::nan(""));
-	CK(reserve(e, e->tup_ptab, 8 * 256));
-	CK(reserve(e, e->tup_val, (uint64_t)n + 1));
-	CK(reserve(e, e->tup_bad, 1));
-	CK(cudaMemcpyAsync(e->tup_ptab.p, tab.data(), 8 * 256 * 8, cudaMemcpyHostToDevice, e->stream));   // pageable source: consumed when this returns
-	if (!e->tup_used) CK(cudaMemsetAsync(e->tup_bad.p, 0, 4, e->stream));       // a session keeps the flags of its earlier launches
+// Form T: the table values of every entry of d for the current weights and `recip` into v (k_tuple_values).  Held values
+// (the copy): into the buffers build_twin_t allocated, so a scoring call allocates nothing after route_twin; then waits and
+// records whether every entry lies in Form T's domain.  Otherwise device work on e->stream only, which the call checks once
+// it has synchronised (finish_score).
+int tuple_values(apo_engine *e, const TupleDict &d, TupleVals &v, bool recip) {
+	const std::vector<double> tab = make_ptab(d.book, e->W, std::nan(""));
+	if (!v.held) {
+		CK(reserve(e, v.ptab, 8 * 256));
+		CK(reserve(e, v.val[0], (uint64_t)d.n + 1));
+		CK(reserve(e, v.bad, 1));
+	}
+	CK(cudaMemcpyAsync(v.ptab.p, tab.data(), 8 * 256 * 8, cudaMemcpyHostToDevice, e->stream));   // pageable source: consumed when this returns
+	if (e->tvals_check != &v) CK(cudaMemsetAsync(v.bad.p, 0, 4, e->stream));   // a session keeps the flags of its earlier launches
 	apo::TupleValParams V{};
-	V.tb_pc = d_pc; V.tb_pd = d_pd; V.n = n; V.ptab = e->tup_ptab.p; V.lut = e->d_lut.p; V.d2book = d_d2; V.w2 = e->W.w[2];
-	V.tval = e->tup_val.p; V.bad = e->tup_bad.p;
+	V.tb_pc = d.pc.p; V.tb_pd = d.pd.p; V.n = d.n; V.ptab = v.ptab.p; V.lut = e->d_lut.p; V.d2book = d.d2.p; V.w2 = e->W.w[2];
+	V.tval = v.out(recip); V.bad = v.bad.p;
 	CK(apo::run_tuple_values(V, recip, e->stream));
-	e->timing.launches++;
-	e->tup_used = true;
-	return APO_OK;
-}
-
-// The table values of the Form T copy for the current weights and `recip` into the buffers build_twin_t allocated, and
-// whether every entry lies in Form T's domain.  Synchronises; no allocation (a scoring call runs this before route_twin).
-int twin_t_values(apo_engine *e, bool recip) {
-	const std::vector<double> tab = make_ptab(e->tt_book, e->W, std::nan(""));
-	CK(cudaMemcpyAsync(e->tt_ptab.p, tab.data(), 8 * 256 * 8, cudaMemcpyHostToDevice, e->stream));
-	CK(cudaMemsetAsync(e->tt_bad.p, 0, 4, e->stream));
-	apo::TupleValParams V{};
-	V.tb_pc = e->tt_pc.p; V.tb_pd = e->tt_pd.p; V.n = e->tt_n; V.ptab = e->tt_ptab.p; V.lut = e->d_lut.p; V.d2book = e->tt_d2.p; V.w2 = e->W.w[2];
-	V.tval = e->tt_val[recip].p; V.bad = e->tt_bad.p;
-	CK(apo::run_tuple_values(V, recip, e->stream));
+	if (!v.held) { e->timing.launches++; e->tvals_check = &v; return APO_OK; }
 	uint32_t bad = 0;
-	CK(cudaMemcpyAsync(&bad, e->tt_bad.p, 4, cudaMemcpyDeviceToHost, e->stream));
+	CK(cudaMemcpyAsync(&bad, v.bad.p, 4, cudaMemcpyDeviceToHost, e->stream));
 	CK(cudaStreamSynchronize(e->stream));
-	e->tt_ok[recip] = bad ? 2 : 1;
+	v.ok[recip] = bad ? 2 : 1;
 	return APO_OK;
 }
 
 // a resident Form D call: the copy's values for its `recip`, computed once per weight set by the first call that needs them
 int twin_t_ready(apo_engine *e, const apo_score_opts *o) {
 	const bool recip = (o->flags & APO_SCORE_RECIP) != 0;
-	if (o->source != APO_SRC_DIMS || e->tt_C == 0 || e->env_no_twin_t || e->tt_ok[recip]) return APO_OK;
-	return twin_t_values(e, recip);
-}
-
-// after the scoring call has been synchronised: did K1t meet an index outside the dictionary, or an entry it cannot hold?
-int tuples_check(apo_engine *e) {
-	e->tup_used = false;
-	uint32_t bad = 0;
-	CK(cudaMemcpyAsync(&bad, e->tup_bad.p, 4, cudaMemcpyDeviceToHost, e->stream));
-	CK(cudaStreamSynchronize(e->stream));
-	if (bad & 2u) return fail(e, APO_E_ARG, "a dictionary entry is not representable in Form T (finalReward outside (-2, 2), or a tool_success_rate index without a value)");
-	if (bad & 1u) return fail(e, APO_E_ARG, "a tuple index is outside the dictionary");
-	return APO_OK;
+	if (o->source != APO_SRC_DIMS || e->tcopy.C == 0 || e->env_no_twin_t || e->tcopy.vals.ok[recip]) return APO_OK;
+	return tuple_values(e, e->tcopy, e->tcopy.vals, recip);
 }
 
 // ---- the evaluations one launch reads: a resident tensor (or a window of it), or one window of a host-streaming call
@@ -670,19 +683,14 @@ struct Evals {
 	const unsigned long long *q8 = nullptr;   // Form Q planes
 	const float *d2 = nullptr;
 	const unsigned short *li = nullptr;
-	const unsigned short *tl = nullptr;       // Form T planes + dictionary
-	const unsigned char *th = nullptr;
-	const uint32_t *tb_pc = nullptr;
-	const unsigned short *tb_pd = nullptr;
-	uint32_t n_tuples = 0;
-	const float *d2book = nullptr;
-	const uint32_t *codebook = nullptr;       // resident Form T: every launch rebuilds this codebook's tables (NULL: built once per call) ...
-	const long long *tval = nullptr;          // ... unless they are held (the Form T copy of a resident Form D tensor, route_twin)
+	const QTables *qt = nullptr;              // Form Q / W: K1q's tables of the codebook
 	const unsigned long long *qw = nullptr;   // Form W words (the copy of a resident Form D tensor, route_twin)
+	const unsigned short *tl = nullptr;       // Form T planes
+	const unsigned char *th = nullptr;
+	const TupleDict *dict = nullptr;          // Form T dictionary and its values: held (the copy, route_twin), computed by every
+	TupleVals *tv = nullptr;                  // launch (resident Form T) or, t_once, once for the whole call together with the
+	bool t_once = false;                      // breakdown's codebook table (host streaming)
 	bool t2 = false;                          // the Form T copy through K1t2: tl and the exception list, not th (route_twin)
-	const uint2 *xs = nullptr;
-	const uint32_t *xb = nullptr;
-	uint32_t xb_pitch = 0;
 
 	bool records() const { return form == apo::CAND_REC32 || form == apo::CAND_REC16; }
 	uint32_t row() const { return form == apo::CAND_DIMS ? 36 : form == apo::CAND_REC32 ? 32 : 16; }
@@ -693,6 +701,12 @@ struct Evals {
 	}
 };
 
+// ev reads all of the resident Form T tensor t with the values v
+void resident_tuples(Evals *ev, const TupleTensor &t, TupleVals &v) {
+	ev->form = apo::CAND_T; ev->C = t.C; ev->count = t.T; ev->pitch_evals = t.pitch;
+	ev->tl = t.l.p; ev->th = t.h.p; ev->dict = &t; ev->tv = &v;
+}
+
 // the whole tensor loaded for o->source (count = all its evaluations)
 int resident_evals(apo_engine *e, const apo_score_opts *o, Evals *ev) {
 	if (!o) return fail(e, APO_E_ARG, "opts is NULL");
@@ -701,10 +715,8 @@ int resident_evals(apo_engine *e, const apo_score_opts *o, Evals *ev) {
 	v = Evals{};
 	v.variant = (int)o->variant;
 	if (o->source == APO_SRC_TUPLES) {
-		if (e->tup_l.p == nullptr || e->tup_C == 0) return fail(e, APO_E_STATE, "no tuples loaded");
-		v.form = apo::CAND_T; v.C = e->tup_C; v.count = e->tup_T; v.pitch_evals = e->tup_pitch;
-		v.tl = e->tup_l.p; v.th = e->tup_h.p;
-		v.tb_pc = e->tup_pc.p; v.tb_pd = e->tup_pd.p; v.n_tuples = e->tup_n; v.d2book = e->tup_d2.p; v.codebook = e->tup_book;
+		if (e->tup.l.p == nullptr || e->tup.C == 0) return fail(e, APO_E_STATE, "no tuples loaded");
+		resident_tuples(&v, e->tup, e->tvals);
 	} else if (o->source == APO_SRC_ROLLOUTS) {
 		if (e->roll.p == nullptr || e->roll_C == 0) return fail(e, APO_E_STATE, "no rollouts loaded");
 		v.form = e->roll_row == 32 ? apo::CAND_REC32 : apo::CAND_REC16; v.C = e->roll_C; v.count = e->roll_T; v.pitch_evals = e->roll_pitch;
@@ -713,8 +725,8 @@ int resident_evals(apo_engine *e, const apo_score_opts *o, Evals *ev) {
 		if ((e->dims_ptr == nullptr && !e->compact) || e->dims_C == 0) return fail(e, APO_E_STATE, "no dims loaded");
 		v.C = e->dims_C; v.count = e->dims_T; v.pitch_evals = e->dims_pitch;
 		if (e->compact) {
-			v.form = apo::CAND_Q; v.q8 = e->q8.p; v.d2 = e->qd2.p; v.li = e->qli.p;
-			if ((v.variant == 0 || v.variant >= 5) && !e->q_pair_ok) v.variant = 4;   // prefix table would not fit: product tables only
+			v.form = apo::CAND_Q; v.q8 = e->q8.p; v.d2 = e->qd2.p; v.li = e->qli.p; v.qt = &e->qt;
+			if ((v.variant == 0 || v.variant >= 5) && !e->qt.pair_ok) v.variant = 4;   // prefix table would not fit: product tables only
 		} else {
 			v.rows = (const uint8_t *)e->dims_ptr;
 		}
@@ -741,25 +753,23 @@ int resident_window(apo_engine *e, const apo_score_opts *o, Evals *ev) {
 // K1t when that is held and its values for this call's weights and `recip` are valid (twin_t_ready): through K1t2 from the
 // 16-bit plane when the copy holds an exception list and APO_TUNE_NO_TWIN_T2 is clear.  Before resident_window, after the
 // call's last allocation before its launches (reserve may release the copies).
-void route_twin(const apo_engine *e, const apo_score_opts *o, Evals *ev) {
+void route_twin(apo_engine *e, const apo_score_opts *o, Evals *ev) {
 	if (ev->form != apo::CAND_DIMS || !e->twin || e->env_no_twin || o->variant != 0 || o->first % 8) return;
 	ev->rows = nullptr;
-	const bool recip = (o->flags & APO_SCORE_RECIP) != 0;
-	if (e->tt_C && !e->env_no_twin_t && e->tt_ok[recip] == 1) {
-		ev->form = apo::CAND_T; ev->pitch_evals = e->tt_pitch; ev->variant = 0;
-		ev->tl = e->tt_l.p; ev->th = e->tt_h.p;
-		ev->tb_pc = e->tt_pc.p; ev->tb_pd = e->tt_pd.p; ev->n_tuples = e->tt_n; ev->d2book = e->tt_d2.p;
-		ev->codebook = e->tt_book; ev->tval = e->tt_val[recip].p;
-		if (e->tt_t2 && !e->env_no_twin_t2) { ev->t2 = true; ev->xs = e->tt_xs.p; ev->xb = e->tt_xb.p; ev->xb_pitch = e->tt_nblk + 1; }
+	if (e->tcopy.C && !e->env_no_twin_t && e->tcopy.vals.ok[(o->flags & APO_SCORE_RECIP) != 0] == 1) {
+		resident_tuples(ev, e->tcopy, e->tcopy.vals);
+		ev->variant = 0;
+		ev->t2 = e->tcopy.t2 && !e->env_no_twin_t2;
 		return;
 	}
+	ev->qt = &e->qt;
 	if (e->twin_w) {                                         // <= 15 codes per dimension: the prefix table always fits
 		ev->form = apo::CAND_W; ev->qw = e->qw.p; ev->variant = 0;
 		return;
 	}
 	ev->form = apo::CAND_Q;
 	ev->q8 = e->q8.p; ev->d2 = e->qd2.p; ev->li = e->qli.p;
-	ev->variant = e->q_pair_ok ? 0 : 4;                      // as resident_evals for a compact tensor
+	ev->variant = e->qt.pair_ok ? 0 : 4;                     // as resident_evals for a compact tensor
 }
 
 // one scoring launch (K1 / K1q / K1t) over ev into candidates [cand_offset, ...); fused: the corpus scan and the tail ride on it
@@ -768,26 +778,24 @@ int launch_score(apo_engine *e, const apo_score_opts *o, const Evals &ev, uint32
 	const bool recip = (o->flags & APO_SCORE_RECIP) != 0;
 	long long *acc = e->acc.p + (uint64_t)ACC_PER_CAND * cand_offset;
 	int rc;
-	if (ev.codebook && !ev.tval && (rc = tuples_values(e, ev.codebook, ev.tb_pc, ev.tb_pd, ev.n_tuples, ev.d2book, recip))) return rc;
+	if (ev.form == apo::CAND_T && !ev.t_once && !ev.tv->held && (rc = tuple_values(e, *ev.dict, *ev.tv, recip))) return rc;
 	if ((rc = record_k1_event(e, 0))) return rc;
 	if (ev.form == apo::CAND_T && ev.t2) {
 		apo::Kt2Params P{};
 		P.tl = ev.tl; P.pitch_evals = ev.pitch_evals; P.C = ev.C; P.T = ev.count; P.first = ev.idx_base;
-		P.acc = acc; P.tval = ev.tval; P.n_tuples = ev.n_tuples;
-		P.xs = ev.xs; P.xb = ev.xb; P.xb_pitch = ev.xb_pitch;
+		P.acc = acc; P.tval = ev.tv->out(recip); P.n_tuples = ev.dict->n;
+		P.xs = e->tcopy.xs.p; P.xb = e->tcopy.xb.p; P.xb_pitch = e->tcopy.nblk + 1;   // only the copy holds an exception list
 		CK(apo::run_reward9t2(P, e->sm_count, e->stream));
 	} else if (ev.form == apo::CAND_T) {
 		apo::KtParams P{};
 		P.tl = ev.tl; P.th = ev.th; P.pitch_evals = ev.pitch_evals; P.C = ev.C; P.T = ev.count;
-		P.acc = acc; P.n_tuples = ev.n_tuples;
-		// the copy's indices come from its own dictionary: its index flag is never set, and never read
-		P.tval = ev.tval ? ev.tval : e->tup_val.p; P.bad = ev.tval ? e->tt_bad.p : e->tup_bad.p;
+		P.acc = acc; P.n_tuples = ev.dict->n; P.tval = ev.tv->out(recip); P.bad = ev.tv->bad.p;
 		CK(apo::run_reward9t(P, e->sm_count, e->stream));
 	} else if (ev.form == apo::CAND_Q || ev.form == apo::CAND_W) {
 		apo::KqParams Q{};
 		Q.q8 = ev.q8; Q.d2 = ev.d2; Q.li = ev.li; Q.qw = ev.qw; Q.pitch_evals = ev.pitch_evals; Q.C = ev.C; Q.T = ev.count;
-		Q.acc = acc; Q.lut = e->d_lut.p; Q.ptab = e->d_ptab.p; Q.w2 = e->W.w[2];
-		Q.pair = e->d_pair.p; Q.cbf = e->d_cbf.p; Q.n0 = e->q_n0; Q.n1 = e->q_n1;
+		Q.acc = acc; Q.lut = e->d_lut.p; Q.ptab = ev.qt->ptab.p; Q.w2 = e->W.w[2];
+		Q.pair = ev.qt->pair.p; Q.cbf = ev.qt->cbf.p; Q.n0 = ev.qt->n0; Q.n1 = ev.qt->n1;
 		for (int j = 0; j < 8; j++) Q.wq[j] = e->W.w[kCodedDim[j]];
 		Q.bad = (uint32_t *)e->h_domain;
 		if (fused) { Q.corpus_on = 1; Q.corpus = *fused; }
@@ -843,15 +851,17 @@ int cand_upload_tbook(apo_engine *e, const uint32_t *codebook) {
 // the breakdown pass over ev into candidates [cand_offset, ...)
 int launch_cand(apo_engine *e, const Evals &ev, uint32_t cand_offset) {
 	if (!ev.count) return APO_OK;
-	if (ev.codebook) { const int rc = cand_upload_tbook(e, ev.codebook); if (rc) return rc; }
+	if (ev.form == apo::CAND_T && !ev.t_once) { const int rc = cand_upload_tbook(e, ev.dict->book); if (rc) return rc; }
 	apo::CandParams P{};
 	P.C = ev.C; P.T = ev.count; P.idx_base = ev.idx_base; P.pitch_evals = ev.pitch_evals; P.lut = e->d_lut.p;
 	P.ints = e->cand_acc.p + (uint64_t)apo::CB_INT * cand_offset;
 	P.ex = (unsigned long long *)(e->cand_acc.p + (uint64_t)apo::CB_INT * e->score_C) + 3ull * cand_offset;
 	P.rows = ev.rows; P.q8 = ev.q8; P.d2 = ev.d2; P.li = ev.li; P.qw = ev.qw;
-	P.tl = ev.tl; P.th = ev.th; P.tb_pc = ev.tb_pc; P.tb_pd = ev.tb_pd; P.n_tuples = ev.n_tuples; P.d2book = ev.d2book;
-	if (ev.form == apo::CAND_Q || ev.form == apo::CAND_W) P.cbf = e->d_cbf.p;   // the tables of the codebook this call scores with (upload_ptab)
-	if (ev.form == apo::CAND_T) P.tbook = e->cand_book.p;
+	P.tl = ev.tl; P.th = ev.th;
+	if (ev.qt) P.cbf = ev.qt->cbf.p;
+	if (ev.form == apo::CAND_T) {
+		P.tb_pc = ev.dict->pc.p; P.tb_pd = ev.dict->pd.p; P.n_tuples = ev.dict->n; P.d2book = ev.dict->d2.p; P.tbook = e->cand_book.p;
+	}
 	CK(apo::run_cand_breakdown(P, ev.form, e->sm_count, e->stream));
 	e->timing.launches++;
 	return APO_OK;
@@ -1000,7 +1010,14 @@ int finish_score(apo_engine *e, const apo_score_opts *o, uint32_t C, double *sco
 		cudaEventElapsedTime(&ms, e->ev[3], e->ev[4]); e->timing.finalize_ms = ms;
 		cudaEventElapsedTime(&ms, e->ev[0], e->ev[4]); e->timing.total_ms = ms;
 	}
-	if (e->tup_used && (rc = tuples_check(e))) return rc;
+	if (const TupleVals *v = e->tvals_check) {                     // did K1t meet an index outside the dictionary, or an entry it cannot hold?
+		e->tvals_check = nullptr;
+		uint32_t bad = 0;
+		CK(cudaMemcpyAsync(&bad, v->bad.p, 4, cudaMemcpyDeviceToHost, e->stream));
+		CK(cudaStreamSynchronize(e->stream));
+		if (bad & 2u) return fail(e, APO_E_ARG, "a dictionary entry is not representable in Form T (finalReward outside (-2, 2), or a tool_success_rate index without a value)");
+		if (bad & 1u) return fail(e, APO_E_ARG, "a tuple index is outside the dictionary");
+	}
 	if (unpacked) {                                                // the stream is synchronised
 		uint32_t bad = 0;
 		CK(cudaMemcpyAsync(&bad, e->unpack_bad.p, 4, cudaMemcpyDeviceToHost, e->stream));
@@ -1226,13 +1243,12 @@ extern "C" void apo_destroy(apo_engine *e) {
 	peer_teardown(e);
 	if (e->comm && g_nccl.CommDestroy) g_nccl.CommDestroy(e->comm);
 	if (e->zc_host) cudaFreeHost(e->zc_host);
-	e->q8.release(); e->qd2.release(); e->qli.release(); e->qw.release(); e->qbook.release(); e->d_ptab.release(); e->d_pair.release(); e->d_cbf.release(); e->d_d2book.release(); e->d_d2stream.release(); e->unpack_bad.release(); e->stage.release();
+	e->q8.release(); e->qd2.release(); e->qli.release(); e->qw.release(); e->qbook.release(); e->d_d2book.release(); e->d_d2stream.release(); e->unpack_bad.release(); e->stage.release();
+	e->qt.release(); e->qt_stream.release();
 	e->d_lut.release(); e->corpus.release(); e->dims.release(); e->roll.release(); e->acc.release(); e->acc_joined.release(); e->acc_snapshot.release(); e->misc.release();
 	e->result.release(); e->keys.release(); e->sel_key.release(); e->sel_idx.release();
-	e->tups_pc.release(); e->tups_pd.release(); e->tups_d2.release();
 	e->cand_acc.release(); e->cand_rep.release(); e->cand_book.release(); e->ccorp_acc.release(); e->ccorp_rep.release();
-	e->tup_l.release(); e->tup_h.release(); e->tup_pc.release(); e->tup_pd.release(); e->tup_bad.release(); e->tup_d2.release(); e->tup_ptab.release(); e->tup_val.release();
-	drop_twin_t(e);
+	e->tup.release(); e->tups.release(); e->tvals.release(); e->tcopy.release();
 	e->win[0].release(); e->win[1].release(); e->batch_in.release(); e->batch_out.release(); e->batch_mask.release();
 	if (e->h_result) cudaFreeHost(e->h_result);
 	if (e->h_domain) cudaFreeHost((void *)e->h_domain);
@@ -1273,11 +1289,12 @@ extern "C" int apo_set_weights(apo_engine *e, const double w[APO_NDIM]) {
 			return fail(e, APO_E_ARG, "weights must be 0 or within [1e-100, 1e100]");
 	CK(cudaSetDevice(e->device));
 	memcpy(e->W.w, w, sizeof e->W.w);
+	e->weights_gen++;
 	build_luts(e);
 	int rc = upload_luts(e);
-	if (rc == APO_OK && (e->compact || e->twin)) rc = upload_ptab(e);
-	e->tt_ok[0] = e->tt_ok[1] = 0;                          // the Form T copy's values belonged to the old weights
-	if (rc == APO_OK && e->tt_C) rc = twin_t_values(e, false);
+	if (rc == APO_OK && (e->compact || e->twin)) rc = load_qtables(e, e->qt, e->qt.book);
+	e->tcopy.vals.ok[0] = e->tcopy.vals.ok[1] = 0;          // the Form T copy's values belonged to the old weights
+	if (rc == APO_OK && e->tcopy.C) rc = tuple_values(e, e->tcopy, e->tcopy.vals, false);
 	return rc;
 }
 
@@ -1449,7 +1466,7 @@ extern "C" int apo_dims_compact(apo_engine *e) {
 	if (!e->dims_ptr || e->dims_C == 0) return fail(e, APO_E_STATE, "no dims loaded");
 	CK(cudaSetDevice(e->device));
 	if (e->twin && !e->twin_w) {                        // the copy built at load already is this tensor in Form Q
-		drop_twin_t(e);                                 // a compact tensor keeps no Form T copy
+		e->tcopy.release();                             // a compact tensor keeps no Form T copy
 		e->twin = false; e->compact = true; e->dims_ptr = nullptr;
 		e->dims.release();
 		return APO_OK;
@@ -1682,6 +1699,21 @@ int tuples_args(apo_engine *e, const uint16_t *tl, const uint8_t *th, const uint
 	return APO_OK;
 }
 
+// the caller's dictionary of n entries into d (pageable sources are consumed when this returns)
+int dict_upload(apo_engine *e, TupleDict &d, const uint32_t *pc, const uint16_t *pd, uint32_t n, const uint32_t *codebook, const uint32_t *d2book) {
+	CK(reserve(e, d.pc, n ? n : 1));
+	CK(reserve(e, d.pd, n ? n : 1));
+	CK(reserve(e, d.d2, 4096));
+	if (n) {
+		CK(cudaMemcpyAsync(d.pc.p, pc, (uint64_t)n * 4, cudaMemcpyHostToDevice, e->stream));
+		CK(cudaMemcpyAsync(d.pd.p, pd, (uint64_t)n * 2, cudaMemcpyHostToDevice, e->stream));
+	}
+	CK(cudaMemcpyAsync(d.d2.p, d2book, 4096 * 4, cudaMemcpyHostToDevice, e->stream));   // bit patterns: unused slots are NaNs, flagged if an entry names one
+	memcpy(d.book, codebook, sizeof d.book);
+	d.n = n;
+	return APO_OK;
+}
+
 // A tensor [C][T] in the caller's memory for the host-streaming calls: the planes of one layout, each [C][T] at `bytes` per
 // evaluation.  D / R / R16: the rows; Q: q8, d2, li; P: pc, pd; T: tl, th.
 struct HostTensor {
@@ -1721,20 +1753,10 @@ int stream_host(apo_engine *e, const apo_score_opts *o, const HostTensor &h, dou
 	Evals ev;
 	ev.form = h.form; ev.C = C; ev.variant = (int)o->variant;
 	if ((rc = score_check(e, o, C, kStreamed, ev.records()))) return rc;
-	// Form Q / P: the lookup tables of K1q follow the codebook of THIS call; a resident Form Q tensor (or the Form Q copy of a
-	// Form D one) keeps its own and gets it back when the call returns, on every path (Restore)
-	struct Restore {
-		apo_engine *e; uint32_t saved[8 * 256]; bool armed = false;
-		~Restore() { if (armed) { memcpy(e->qbook_host, saved, sizeof saved); upload_ptab(e); } }
-	} restore{e};
-	if (h.form == apo::CAND_Q) {
-		const bool same_book = memcmp(e->qbook_host, h.codebook, sizeof e->qbook_host) == 0 && e->d_ptab.p != nullptr;
-		if (!same_book) {
-			if (e->compact || e->twin) { memcpy(restore.saved, e->qbook_host, sizeof restore.saved); restore.armed = true; }
-			memcpy(e->qbook_host, h.codebook, sizeof e->qbook_host);
-			if ((rc = upload_ptab(e))) return rc;
-		}
-		ev.variant = e->q_pair_ok ? 0 : 4;
+	if (h.form == apo::CAND_Q) {                                   // Form Q / P: K1q's tables of this call's codebook
+		if ((rc = load_qtables(e, e->qt_stream, h.codebook))) return rc;
+		ev.qt = &e->qt_stream;
+		ev.variant = e->qt_stream.pair_ok ? 0 : 4;
 	}
 	uint64_t wire = 0;                                             // bytes per evaluation over PCIe
 	for (int k = 0; k < h.planes; k++) wire += h.plane[k].bytes;
@@ -1763,21 +1785,12 @@ int stream_host(apo_engine *e, const apo_score_opts *o, const HostTensor &h, dou
 		CK(cudaMemcpyAsync(e->d_d2stream.p, h.d2book, 4096 * 4, cudaMemcpyHostToDevice, e->stream));   // bit patterns: empty slots are NaNs, flagged if named
 		CK(cudaMemsetAsync(e->unpack_bad.p, 0, 4, e->stream));
 	}
-	if (h.form == apo::CAND_T) {
-		CK(reserve(e, e->tups_pc, h.n_tuples ? h.n_tuples : 1));
-		CK(reserve(e, e->tups_pd, h.n_tuples ? h.n_tuples : 1));
-		CK(reserve(e, e->tups_d2, 4096));
-	}
 	if ((rc = score_arm(e, o, C, true, (uint64_t)C * T * wire))) return rc;
 	if (h.form == apo::CAND_T) {                                   // the dictionary and its values, once for the whole call
 		if (wants_cand(o) && (rc = cand_upload_tbook(e, h.codebook))) return rc;
-		if (h.n_tuples) {
-			CK(cudaMemcpyAsync(e->tups_pc.p, h.tb_pc, (uint64_t)h.n_tuples * 4, cudaMemcpyHostToDevice, e->stream));
-			CK(cudaMemcpyAsync(e->tups_pd.p, h.tb_pd, (uint64_t)h.n_tuples * 2, cudaMemcpyHostToDevice, e->stream));
-		}
-		CK(cudaMemcpyAsync(e->tups_d2.p, h.d2book, 4096 * 4, cudaMemcpyHostToDevice, e->stream));   // bit patterns: unused slots are NaNs, flagged if an entry names one
-		ev.tb_pc = e->tups_pc.p; ev.tb_pd = e->tups_pd.p; ev.n_tuples = h.n_tuples; ev.d2book = e->tups_d2.p;
-		if ((rc = tuples_values(e, h.codebook, ev.tb_pc, ev.tb_pd, ev.n_tuples, ev.d2book, (o->flags & APO_SCORE_RECIP) != 0))) return rc;
+		if ((rc = dict_upload(e, e->tups, h.tb_pc, h.tb_pd, h.n_tuples, h.codebook, h.d2book))) return rc;
+		ev.dict = &e->tups; ev.tv = &e->tvals; ev.t_once = true;
+		if ((rc = tuple_values(e, e->tups, e->tvals, (o->flags & APO_SCORE_RECIP) != 0))) return rc;
 	}
 	const uint64_t CTc = (uint64_t)C * Tc;
 	ev.pitch_evals = Tc;
@@ -1832,7 +1845,7 @@ int score_host(apo_engine *e, const apo_score_opts *o, const HostTensor &h, doub
 		// a failure in the middle of the chunk loop: nothing may still be reading the caller's memory when we return
 		cudaStreamSynchronize(e->copy_stream);
 		cudaStreamSynchronize(e->stream);
-		if (h.form == apo::CAND_T) e->tup_used = false;
+		if (h.form == apo::CAND_T) e->tvals_check = nullptr;
 	}
 	return rc;
 }
@@ -1842,7 +1855,7 @@ int score_host(apo_engine *e, const apo_score_opts *o, const HostTensor &h, doub
 extern "C" int apo_dims_codebook(apo_engine *e, uint32_t *codebook) {
 	if (!e || !codebook) return fail(e, APO_E_ARG, "NULL argument");
 	if (!e->compact) return fail(e, APO_E_STATE, "no compact (Form Q) evaluations loaded");
-	memcpy(codebook, e->qbook_host, sizeof e->qbook_host);
+	memcpy(codebook, e->qt.book, sizeof e->qt.book);
 	return APO_OK;
 }
 
@@ -1960,39 +1973,20 @@ extern "C" int apo_tuples_upload(apo_engine *e, const uint16_t *tl, const uint8_
 	int rc;
 	if ((rc = tuples_args(e, tl, th, tbook_pc, tbook_pd, n_tuples, codebook, d2book, C, T))) return rc;
 	CK(cudaSetDevice(e->device));
-	e->tup_C = 0; e->tup_T = 0; e->tup_n = 0;
+	e->tup.unload();
 	const uint64_t pitch = round_up(T ? T : 1, 64);                // rows start 16-byte aligned in both planes
-	CK(reserve(e, e->tup_l, (uint64_t)C * pitch));
-	CK(reserve(e, e->tup_h, (uint64_t)C * pitch));
-	CK(reserve(e, e->tup_pc, n_tuples ? n_tuples : 1));
-	CK(reserve(e, e->tup_pd, n_tuples ? n_tuples : 1));
-	CK(reserve(e, e->tup_d2, 4096));
-	if ((rc = h2d_rows(e, e->tup_l.p, pitch * 2, tl, T * 2, T * 2, C, e->stream))) { cudaStreamSynchronize(e->stream); return rc; }
-	if ((rc = h2d_rows(e, e->tup_h.p, pitch, th, T, T, C, e->stream))) { cudaStreamSynchronize(e->stream); return rc; }
-	if (n_tuples) {
-		CK(cudaMemcpyAsync(e->tup_pc.p, tbook_pc, (uint64_t)n_tuples * 4, cudaMemcpyHostToDevice, e->stream));
-		CK(cudaMemcpyAsync(e->tup_pd.p, tbook_pd, (uint64_t)n_tuples * 2, cudaMemcpyHostToDevice, e->stream));
-	}
-	CK(cudaMemcpyAsync(e->tup_d2.p, d2book, 4096 * 4, cudaMemcpyHostToDevice, e->stream));
+	CK(reserve(e, e->tup.l, (uint64_t)C * pitch));
+	CK(reserve(e, e->tup.h, (uint64_t)C * pitch));
+	if ((rc = dict_upload(e, e->tup, tbook_pc, tbook_pd, n_tuples, codebook, d2book))) return rc;
+	if ((rc = h2d_rows(e, e->tup.l.p, pitch * 2, tl, T * 2, T * 2, C, e->stream))) { cudaStreamSynchronize(e->stream); return rc; }
+	if ((rc = h2d_rows(e, e->tup.h.p, pitch, th, T, T, C, e->stream))) { cudaStreamSynchronize(e->stream); return rc; }
 	CK(cudaStreamSynchronize(e->stream));
-	memcpy(e->tup_book, codebook, sizeof e->tup_book);
-	e->tup_C = C; e->tup_T = T; e->tup_pitch = pitch; e->tup_n = n_tuples;
+	e->tup.C = C; e->tup.T = T; e->tup.pitch = pitch;
 	return APO_OK;
 }
 
 namespace {
 constexpr uint32_t kTwinTHot = 24576;   // K1t's shared-memory head of the table (KT_HOT_MAX, csrc/apo_tuple.cu)
-
-// Where a Form T build from the loaded evaluations goes: the engine's resident Form T (apo_dims_tuples), or the Form T copy of
-// its Form D tensor (build_twin_t).  The copy's buffers do not go through reserve: releasing the copies to make room would
-// release the one being built.
-struct TupleDst {
-	DevBuf<unsigned short> &l; DevBuf<unsigned char> &h; DevBuf<uint32_t> &pc; DevBuf<unsigned short> &pd; DevBuf<float> &d2;
-	uint32_t *book; uint32_t &C, &n; uint64_t &T, &pitch;
-	bool copy;
-};
-TupleDst resident_tuples(apo_engine *e) { return {e->tup_l, e->tup_h, e->tup_pc, e->tup_pd, e->tup_d2, e->tup_book, e->tup_C, e->tup_n, e->tup_T, e->tup_pitch, false}; }
-TupleDst copy_tuples(apo_engine *e) { return {e->tt_l, e->tt_h, e->tt_pc, e->tt_pd, e->tt_d2, e->tt_book, e->tt_C, e->tt_n, e->tt_T, e->tt_pitch, true}; }
 
 template <class T>
 int tb_reserve(apo_engine *e, DevBuf<T> &b, uint64_t n, const char *what, bool copy = false) {
@@ -2002,15 +1996,22 @@ int tb_reserve(apo_engine *e, DevBuf<T> &b, uint64_t n, const char *what, bool c
 	return fail(e, c == cudaErrorMemoryAllocation ? APO_E_NOMEM : APO_E_CUDA, "%s (%llu elements): %s", what, (unsigned long long)n, cudaGetErrorString(c));
 }
 
-// *n_high (may be NULL): the evaluations whose index is >= 2^16
-int dims_tuples(apo_engine *e, uint32_t cap, uint32_t *n_tuples, const TupleDst &D, uint64_t *n_high = nullptr) {
+void tb_release(apo_engine *e, int rc) {
+	if (rc != APO_OK) cudaStreamSynchronize(e->stream);          // nothing a failed build queued may still use what is released
+	e->tb_table.release(); e->tb_keys.release(); e->tb_cnt.release(); e->tb_misc.release();
+}
+
+// Form T of the loaded evaluations into D: the engine's resident Form T (apo_dims_tuples), or the Form T copy of its Form D
+// tensor (copy, build_twin_t; *n_high: the evaluations whose index is >= 2^16).  The copy's buffers do not go through
+// reserve: releasing the copies to make room would release the one being built.
+int dims_tuples(apo_engine *e, uint32_t cap, uint32_t *n_tuples, TupleTensor &D, bool copy, uint64_t *n_high = nullptr) {
 	if ((!e->dims_ptr && !e->compact) || e->dims_C == 0) return fail(e, APO_E_STATE, "no dims loaded");
 	if (!e->compact && (!e->twin || e->env_no_twin))
 		return fail(e, APO_E_STATE, "the loaded Form D tensor has no Form W / Q copy to build Form T from (APO_TUNE_NO_TWIN, apo_dims_attach, "
 		                            "or too little device memory at load): call apo_dims_compact first");
 	if (e->compact || !e->twin_w)
 		for (int j = 0; j < 8; j++)
-			if (e->qbook_host[256 * j + 15] != 0xFFFFFFFFu)
+			if (e->qt.book[256 * j + 15] != 0xFFFFFFFFu)
 				return fail(e, APO_E_STATE, "coded dimension %d takes 16 or more distinct values: Form T (like Form P) needs <= 15", j < 2 ? j : j + 1);
 	if (cap > APO_TUPLES_MAX) cap = APO_TUPLES_MAX;
 	const uint32_t C = e->dims_C;
@@ -2021,12 +2022,11 @@ int dims_tuples(apo_engine *e, uint32_t cap, uint32_t *n_tuples, const TupleDst 
 	const uint64_t tpitch = round_up(T ? T : 1, 64);               // as apo_tuples_upload
 	// everything is allocated before the source is chosen: reserve may release the copy this build reads
 	int rc;
-	const bool cp = D.copy;
-	if ((rc = tb_reserve(e, D.l, (uint64_t)C * tpitch, "Form T low plane", cp)) || (rc = tb_reserve(e, D.h, (uint64_t)C * tpitch, "Form T high plane", cp)) ||
-	    (rc = tb_reserve(e, D.pc, m ? m : 1, "dictionary", cp)) || (rc = tb_reserve(e, D.pd, m ? m : 1, "dictionary", cp)) ||
-	    (rc = tb_reserve(e, D.d2, 4096, "d2book", cp)) || (rc = tb_reserve(e, e->tb_table, 2 * slots, "hash table", cp)) ||
-	    (rc = tb_reserve(e, e->tb_keys, m ? m : 1, "keys", cp)) || (rc = tb_reserve(e, e->tb_cnt, m ? m : 1, "counts", cp)) ||
-	    (rc = tb_reserve(e, e->tb_misc, 4, "counters", cp)))
+	if ((rc = tb_reserve(e, D.l, (uint64_t)C * tpitch, "Form T low plane", copy)) || (rc = tb_reserve(e, D.h, (uint64_t)C * tpitch, "Form T high plane", copy)) ||
+	    (rc = tb_reserve(e, D.pc, m ? m : 1, "dictionary", copy)) || (rc = tb_reserve(e, D.pd, m ? m : 1, "dictionary", copy)) ||
+	    (rc = tb_reserve(e, D.d2, 4096, "d2book", copy)) || (rc = tb_reserve(e, e->tb_table, 2 * slots, "hash table", copy)) ||
+	    (rc = tb_reserve(e, e->tb_keys, m ? m : 1, "keys", copy)) || (rc = tb_reserve(e, e->tb_cnt, m ? m : 1, "counts", copy)) ||
+	    (rc = tb_reserve(e, e->tb_misc, 4, "counters", copy)))
 		return rc;
 	if (!e->compact && !e->twin)
 		return fail(e, APO_E_NOMEM, "device memory ran short: the Form W / Q copy of the loaded tensor was released to make room for the build; "
@@ -2076,12 +2076,10 @@ int dims_tuples(apo_engine *e, uint32_t cap, uint32_t *n_tuples, const TupleDst 
 		if (x.first != y.first) return x.first > y.first;
 		return x.second < y.second;
 	});
-	if (D.copy) {                                                 // see build_twin_t
+	if (copy) {                                                   // see build_twin_t
 		uint64_t head = 0;
 		for (uint32_t r = 0; r < n && r < kTwinTHot; r++) head += order[r].first;
 		if (head * 4 < N * 3) return APO_E_STATE;
-	}
-	if (n_high) {
 		*n_high = 0;
 		for (uint32_t r = 65536; r < n; r++) *n_high += order[r].first;
 	}
@@ -2108,7 +2106,7 @@ int dims_tuples(apo_engine *e, uint32_t cap, uint32_t *n_tuples, const TupleDst 
 	CK(cudaMemcpyAsync(&miss, misc + 1, 8, cudaMemcpyDeviceToHost, e->stream));
 	CK(cudaStreamSynchronize(e->stream));
 	if (miss) return fail(e, APO_E_CUDA, "internal error: an evaluation's key is missing from the dictionary");
-	memcpy(D.book, e->qbook_host, sizeof e->tup_book);
+	memcpy(D.book, e->qt.book, sizeof D.book);
 	D.C = C; D.T = T; D.pitch = tpitch; D.n = n;
 	*n_tuples = n;
 	return APO_OK;
@@ -2131,21 +2129,22 @@ constexpr uint32_t kTwinTCap = 1u << 20;
 // is read through K1t as before, without an error.  APO_TUNE_NO_TWIN_T2 at the load builds none.
 constexpr uint64_t kTwinT2Share = 64;
 int build_twin_t2(apo_engine *e, uint64_t n_high) {
-	const uint32_t C = e->tt_C;
-	const uint64_t T = e->tt_T;
+	TupleCopy &t = e->tcopy;
+	const uint32_t C = t.C;
+	const uint64_t T = t.T;
 	if (e->env_no_twin_t2 || n_high * kTwinT2Share > (uint64_t)C * T || T > 0xFFFFFFFFull || n_high > 0xFFFFFFFFull) return APO_OK;
 	if (n_high) {
 		const uint32_t nblk = (uint32_t)((T + apo::KT_XBLOCK - 1) / apo::KT_XBLOCK);
-		if (e->tt_xb.reserve((uint64_t)C * (nblk + 1)) != cudaSuccess || e->tt_xs.reserve(n_high) != cudaSuccess) {
+		if (t.xb.reserve((uint64_t)C * (nblk + 1)) != cudaSuccess || t.xs.reserve(n_high) != cudaSuccess) {
 			cudaGetLastError();
-			e->tt_xb.release(); e->tt_xs.release();
+			t.xb.release(); t.xs.release();
 			return APO_OK;
 		}
-		CK(apo::run_tx_build(e->tt_l.p, e->tt_h.p, e->tt_pitch, C, T, e->tt_xb.p, e->tt_xs.p, e->sm_count, e->stream));
+		CK(apo::run_tx_build(t.l.p, t.h.p, t.pitch, C, T, t.xb.p, t.xs.p, e->sm_count, e->stream));
 		CK(cudaStreamSynchronize(e->stream));                     // the load returns with the list built, as with the copy
-		e->tt_xn = n_high; e->tt_nblk = nblk;
+		t.xn = n_high; t.nblk = nblk;
 	}
-	e->tt_t2 = true;
+	t.t2 = true;
 	return APO_OK;
 }
 
@@ -2155,7 +2154,7 @@ int build_twin_t(apo_engine *e) {
 	if (e->env_no_twin_t || !(N >= kTwinTMinEvals || e->env_twin_t)) return APO_OK;
 	if (!e->twin_w)
 		for (int j = 0; j < 8; j++)
-			if (e->qbook_host[256 * j + 15] != 0xFFFFFFFFu) return APO_OK;
+			if (e->qt.book[256 * j + 15] != 0xFFFFFFFFu) return APO_OK;
 	const uint64_t m = std::min<uint64_t>(kTwinTCap, N);
 	uint64_t slots = 1024;
 	while (slots < 2 * (m + 1)) slots <<= 1;
@@ -2169,18 +2168,18 @@ int build_twin_t(apo_engine *e) {
 	const std::string keep_err = e->err;
 	uint32_t n = 0;
 	uint64_t n_high = 0;
-	int rc = dims_tuples(e, kTwinTCap, &n, copy_tuples(e), &n_high);
-	if (rc == APO_OK && (e->tt_val[0].reserve(n + 1ull) != cudaSuccess || e->tt_val[1].reserve(n + 1ull) != cudaSuccess ||
-	                     e->tt_ptab.reserve(8 * 256) != cudaSuccess || e->tt_bad.reserve(1) != cudaSuccess)) {
+	TupleVals &v = e->tcopy.vals;
+	int rc = dims_tuples(e, kTwinTCap, &n, e->tcopy, true, &n_high);
+	if (rc == APO_OK && (v.val[0].reserve(n + 1ull) != cudaSuccess || v.val[1].reserve(n + 1ull) != cudaSuccess ||
+	                     v.ptab.reserve(8 * 256) != cudaSuccess || v.bad.reserve(1) != cudaSuccess)) {
 		cudaGetLastError();
 		rc = APO_E_NOMEM;
 	}
-	if (rc == APO_OK) rc = twin_t_values(e, false);
+	if (rc == APO_OK) rc = tuple_values(e, e->tcopy, v, false);
 	if (rc == APO_OK) rc = build_twin_t2(e, n_high);
-	if (rc != APO_OK) cudaStreamSynchronize(e->stream);          // nothing queued may still use what is released
-	e->tb_table.release(); e->tb_keys.release(); e->tb_cnt.release(); e->tb_misc.release();
+	tb_release(e, rc);
 	if (rc == APO_OK) return APO_OK;
-	drop_twin_t(e);
+	e->tcopy.release();
 	if (rc != APO_E_STATE && rc != APO_E_NOMEM) return rc;
 	e->err = keep_err;                                          // more than kTwinTCap distinct evaluations, or no room: no copy
 	return APO_OK;
@@ -2192,22 +2191,21 @@ extern "C" int apo_dims_tuples(apo_engine *e, uint32_t cap, uint32_t *n_tuples) 
 	if (!n_tuples) return fail(e, APO_E_ARG, "n_tuples is NULL");
 	*n_tuples = 0;
 	CK(cudaSetDevice(e->device));
-	e->tup_C = 0; e->tup_T = 0; e->tup_n = 0;                      // a failure leaves no Form T loaded, as a failed apo_tuples_upload
-	const int rc = dims_tuples(e, cap, n_tuples, resident_tuples(e));
-	if (rc != APO_OK) cudaStreamSynchronize(e->stream);           // nothing queued may still use the scratch when it is released
-	e->tb_table.release(); e->tb_keys.release(); e->tb_cnt.release(); e->tb_misc.release();
+	e->tup.unload();                                               // a failure leaves no Form T loaded, as a failed apo_tuples_upload
+	const int rc = dims_tuples(e, cap, n_tuples, e->tup, false);
+	tb_release(e, rc);
 	return rc;
 }
 
 extern "C" int apo_tuples_download(apo_engine *e, uint16_t *tl, uint8_t *th, uint32_t c, uint64_t first, uint64_t n) {
 	if (!e || !tl || !th) return fail(e, APO_E_ARG, "NULL argument");
-	if (e->tup_l.p == nullptr || e->tup_C == 0) return fail(e, APO_E_STATE, "no tuples loaded");
-	if (c >= e->tup_C || first > e->tup_T || n > e->tup_T - first) return fail(e, APO_E_ARG, "range outside the tuples");
+	if (e->tup.l.p == nullptr || e->tup.C == 0) return fail(e, APO_E_STATE, "no tuples loaded");
+	if (c >= e->tup.C || first > e->tup.T || n > e->tup.T - first) return fail(e, APO_E_ARG, "range outside the tuples");
 	if (n == 0) return APO_OK;
 	CK(cudaSetDevice(e->device));
-	const uint64_t off = (uint64_t)c * e->tup_pitch + first;
-	CK(cudaMemcpyAsync(tl, e->tup_l.p + off, n * 2, cudaMemcpyDeviceToHost, e->stream));
-	CK(cudaMemcpyAsync(th, e->tup_h.p + off, n, cudaMemcpyDeviceToHost, e->stream));
+	const uint64_t off = (uint64_t)c * e->tup.pitch + first;
+	CK(cudaMemcpyAsync(tl, e->tup.l.p + off, n * 2, cudaMemcpyDeviceToHost, e->stream));
+	CK(cudaMemcpyAsync(th, e->tup.h.p + off, n, cudaMemcpyDeviceToHost, e->stream));
 	CK(cudaStreamSynchronize(e->stream));
 	return APO_OK;
 }
@@ -2215,18 +2213,19 @@ extern "C" int apo_tuples_download(apo_engine *e, uint16_t *tl, uint8_t *th, uin
 extern "C" int apo_tuples_book(apo_engine *e, uint32_t *tbook_pc, uint16_t *tbook_pd, uint32_t cap, uint32_t *codebook, uint32_t *d2book,
                                uint32_t *n_tuples) {
 	if (!e || !n_tuples) return fail(e, APO_E_ARG, "NULL argument");
-	if (e->tup_l.p == nullptr || e->tup_C == 0) return fail(e, APO_E_STATE, "no tuples loaded");
-	*n_tuples = e->tup_n;
-	if (cap < e->tup_n) return fail(e, APO_E_ARG, "cap=%u is smaller than the %u dictionary entries", cap, e->tup_n);
-	if (!codebook || !d2book || (e->tup_n && (!tbook_pc || !tbook_pd))) return fail(e, APO_E_ARG, "NULL argument");
+	if (e->tup.l.p == nullptr || e->tup.C == 0) return fail(e, APO_E_STATE, "no tuples loaded");
+	const uint32_t n = e->tup.n;
+	*n_tuples = n;
+	if (cap < n) return fail(e, APO_E_ARG, "cap=%u is smaller than the %u dictionary entries", cap, n);
+	if (!codebook || !d2book || (n && (!tbook_pc || !tbook_pd))) return fail(e, APO_E_ARG, "NULL argument");
 	CK(cudaSetDevice(e->device));
-	if (e->tup_n) {
-		CK(cudaMemcpyAsync(tbook_pc, e->tup_pc.p, (uint64_t)e->tup_n * 4, cudaMemcpyDeviceToHost, e->stream));
-		CK(cudaMemcpyAsync(tbook_pd, e->tup_pd.p, (uint64_t)e->tup_n * 2, cudaMemcpyDeviceToHost, e->stream));
+	if (n) {
+		CK(cudaMemcpyAsync(tbook_pc, e->tup.pc.p, (uint64_t)n * 4, cudaMemcpyDeviceToHost, e->stream));
+		CK(cudaMemcpyAsync(tbook_pd, e->tup.pd.p, (uint64_t)n * 2, cudaMemcpyDeviceToHost, e->stream));
 	}
-	CK(cudaMemcpyAsync(d2book, e->tup_d2.p, 4096 * 4, cudaMemcpyDeviceToHost, e->stream));
+	CK(cudaMemcpyAsync(d2book, e->tup.d2.p, 4096 * 4, cudaMemcpyDeviceToHost, e->stream));
 	CK(cudaStreamSynchronize(e->stream));
-	memcpy(codebook, e->tup_book, sizeof e->tup_book);
+	memcpy(codebook, e->tup.book, sizeof e->tup.book);
 	return APO_OK;
 }
 
@@ -2271,12 +2270,12 @@ extern "C" int apo_debug_partials(apo_engine *e, int64_t *out, uint32_t C) {
 
 extern "C" int apo_debug_twin_t_list(apo_engine *e, uint64_t *n_words, uint64_t *n_exceptions, uint32_t *xb, uint32_t *xs) {
 	if (!e || !n_words || !n_exceptions) return fail(e, APO_E_ARG, "NULL argument");
-	*n_words = e->tt_xn ? (uint64_t)e->tt_C * (e->tt_nblk + 1) : 0;
-	*n_exceptions = e->tt_xn;
-	if (!e->tt_xn) return APO_OK;
+	*n_words = e->tcopy.xn ? (uint64_t)e->tcopy.C * (e->tcopy.nblk + 1) : 0;
+	*n_exceptions = e->tcopy.xn;
+	if (!e->tcopy.xn) return APO_OK;
 	CK(cudaSetDevice(e->device));
-	if (xb) CK(cudaMemcpyAsync(xb, e->tt_xb.p, *n_words * 4, cudaMemcpyDeviceToHost, e->stream));
-	if (xs) CK(cudaMemcpyAsync(xs, e->tt_xs.p, e->tt_xn * 8, cudaMemcpyDeviceToHost, e->stream));
+	if (xb) CK(cudaMemcpyAsync(xb, e->tcopy.xb.p, *n_words * 4, cudaMemcpyDeviceToHost, e->stream));
+	if (xs) CK(cudaMemcpyAsync(xs, e->tcopy.xs.p, e->tcopy.xn * 8, cudaMemcpyDeviceToHost, e->stream));
 	CK(cudaStreamSynchronize(e->stream));
 	return APO_OK;
 }
