@@ -394,7 +394,11 @@ int apo_debug_twin_t_list(apo_engine *e, uint64_t *n_words, uint64_t *n_exceptio
  * once to binary64 (v = the fp32 value widened for Form D / Q / P / T, the TCS:668-763 binary64
  * value for Form R / R16), avg = sum / count and the flags of APO:575/591/802/819, by the code
  * that fills apo_corpus_report.dim.  A Form R candidate row therefore has the breakdown that the
- * corpus report of that row has on every shared field.  Single rank only: APO_E_STATE on a handle
+ * corpus report of that row has on every shared field.  Domain: rint(v * 2^52) is an int64 only
+ * for |v| < 2048, so a flagged call fails with APO_E_ARG (and leaves no breakdown) when an
+ * evaluation with a non-null finalReward has a present dimension with |v| >= 2048, even where a
+ * weight of 0 or cancelling weighted terms keep its finalReward in range; absent values and null
+ * evaluations may hold any value.  Single rank only: APO_E_STATE on a handle
  * after apo_comm_init with more than one rank (apo_comm_init with nranks == 1 leaves the handle
  * single-rank, with no communicator, so the breakdown stays available). */
 typedef struct apo_candidate_report {

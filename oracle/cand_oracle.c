@@ -7,7 +7,9 @@
  *   - over evaluations with a non-null finalReward (TCS:784 / APO:550): the exact integer sum of rint(fr * 2^52) and, per
  *     present dimension, of rint(v * 2^52) with v the fp32 value widened (Form D) or the binary64 TCS:668-763 value
  *     (Form R), as __int128, and the counts;
- *   - the first three record positions (idx_base + t, ascending) whose tally is 'bad'.
+ *   - the first three record positions (idx_base + t, ascending) whose tally is 'bad';
+ *   - refused = 1 when such an evaluation has a present dimension with |v| >= 2048 (+-inf included): rint(v * 2^52) does not fit in
+ *     int64 there (llrint's result is unspecified), so the term is left out and the engine fails the call with APO_E_ARG.
  * Rounding to binary64 and the report rules are applied by oracle/candidates.py.
  */
 #include <math.h>
@@ -18,12 +20,14 @@
 #include "cand_oracle.h"
 
 static const double kFx = 4503599627370496.0;   /* 2^52 */
+static const double kFxBound = 2048.0;           /* |v| < 2^11 <=> |rint(v * 2^52)| < 2^63 */
 
 typedef struct {
 	uint64_t total, good, bad, withReward;
 	__int128 rew, dim[ORC_NDIM];
 	uint64_t dimCount[ORC_NDIM];
 	int64_t ex[3]; int nex;
+	int refused;
 } acc_t;
 
 static void acc_zero(acc_t *a) { memset(a, 0, sizeof *a); for (int k = 0; k < 3; k++) a->ex[k] = -1; }
@@ -36,8 +40,11 @@ static void acc_eval(acc_t *a, const double d[ORC_NDIM], int valid, double fr, i
 	if (!valid) return;
 	a->withReward++;
 	a->rew += (__int128)llrint(fr * kFx);
-	for (int i = 0; i < ORC_NDIM; i++)
-		if (d[i] == d[i]) { a->dim[i] += (__int128)llrint(d[i] * kFx); a->dimCount[i]++; }
+	for (int i = 0; i < ORC_NDIM; i++) {
+		if (d[i] != d[i]) continue;                                         /* absent */
+		if (!(fabs(d[i]) < kFxBound)) { a->refused = 1; continue; }
+		a->dim[i] += (__int128)llrint(d[i] * kFx); a->dimCount[i]++;
+	}
 }
 
 /* b follows a on the record axis */
@@ -45,6 +52,7 @@ static void acc_merge(acc_t *a, const acc_t *b) {
 	a->total += b->total; a->good += b->good; a->bad += b->bad; a->withReward += b->withReward; a->rew += b->rew;
 	for (int i = 0; i < ORC_NDIM; i++) { a->dim[i] += b->dim[i]; a->dimCount[i] += b->dimCount[i]; }
 	for (int k = 0; k < b->nex && a->nex < 3; k++) a->ex[a->nex++] = b->ex[k];
+	a->refused |= b->refused;
 }
 
 static void acc_out(const acc_t *a, orc_cand_fx *o) {
@@ -54,6 +62,7 @@ static void acc_out(const acc_t *a, orc_cand_fx *o) {
 		o->dim_lo[i] = (uint64_t)a->dim[i]; o->dim_hi[i] = (int64_t)(a->dim[i] >> 64); o->dim_count[i] = a->dimCount[i];
 	}
 	for (int k = 0; k < 3; k++) o->badExamples[k] = a->ex[k];
+	o->refused = (uint32_t)a->refused; o->pad = 0;
 }
 
 static void eval_row(acc_t *a, const float row[ORC_NDIM], const double w[ORC_NDIM], int64_t pos) {

@@ -17,6 +17,8 @@ typedef struct {
 	uint64_t dim_lo[ORC_NDIM]; int64_t dim_hi[ORC_NDIM];   /* sum of rint(v * 2^52) over non-null evaluations with dim i present */
 	uint64_t dim_count[ORC_NDIM];
 	int64_t  badExamples[3];                               /* -1 = none */
+	uint32_t refused;                                      /* 1: a counted present dimension with |v| >= 2048 (term left out) */
+	uint32_t pad;
 } orc_cand_fx;
 
 /* Form D [C][pitch][9] fp32 (NaN = absent); positions idx_base + t */

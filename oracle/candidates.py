@@ -3,6 +3,10 @@
 TEST INFRASTRUCTURE ONLY, like the rest of oracle/.  The C side returns exact integers; this module rounds each sum once
 to binary64 (Python's int -> float conversion is correctly rounded, and the scaling by 2^-52 is exact) and applies the
 report rules of APO:546-547, 556-568, 575, 591, 802, 819, the same rules the engine's corpus report applies.
+
+Domain: rint(v * 2^52) fits in int64 only for |v| < 2048.  When an evaluation with a non-null finalReward has a present
+dimension outside that range, the engine fails an APO_SCORE_CANDIDATES call with APO_E_ARG; the functions here raise
+CandDomainError, which still carries the breakdowns (without the refused terms) for the checks that need the other integers.
 """
 from __future__ import annotations
 
@@ -22,7 +26,19 @@ class CandFx(C.Structure):
     _fields_ = [("total", C.c_uint64), ("good", C.c_uint64), ("bad", C.c_uint64), ("none", C.c_uint64), ("withReward", C.c_uint64),
                 ("rew_lo", C.c_uint64), ("rew_hi", C.c_int64),
                 ("dim_lo", C.c_uint64 * NDIM), ("dim_hi", C.c_int64 * NDIM), ("dim_count", C.c_uint64 * NDIM),
-                ("badExamples", C.c_int64 * 3)]
+                ("badExamples", C.c_int64 * 3), ("refused", C.c_uint32), ("pad", C.c_uint32)]
+
+
+FX_BOUND = 2048.0      # |v| < 2^11: the dimension values whose rint(v * 2^52) is an int64
+
+
+class CandDomainError(ValueError):
+    """A counted evaluation has a present dimension with |v| >= 2048: no exact fixed-point sum, the call is refused.
+    reports: the breakdowns with those terms left out; refused: the candidates that hold such a value."""
+
+    def __init__(self, reports: list[dict], refused: list[int]):
+        super().__init__(f"candidates {refused} hold a counted dimension value with |v| >= {FX_BOUND:g}")
+        self.reports, self.refused = reports, refused
 
 
 def build(force: bool = False) -> str:
@@ -72,6 +88,14 @@ def dimstat(fx: int, count: int) -> dict:
             "sugg_flag": int(count >= 3 and avg < 0.0), "sugg_priority": 2 if avg < -0.5 else 1}      # APO:802, 819
 
 
+def _reports(out) -> list[dict]:
+    reps = [_report(r) for r in out]
+    refused = [c for c, r in enumerate(out) if r.refused]
+    if refused:
+        raise CandDomainError(reps, refused)
+    return reps
+
+
 def _report(r: CandFx) -> dict:
     good, bad, n = int(r.good), int(r.bad), int(r.withReward)
     rfx = _i128(r.rew_lo, r.rew_hi)
@@ -92,7 +116,7 @@ def cand_dims(dims: np.ndarray, T: int | None = None, idx_base: int = 0, w=None)
     w = weights() if w is None else np.ascontiguousarray(w, np.float64)
     out = (CandFx * Cn)()
     lib().orc_cand_dims(_p(dims), Cn, T, pitch, idx_base, _p(w), out)
-    return [_report(r) for r in out]
+    return _reports(out)
 
 
 def cand_records(recs: np.ndarray, T: int | None = None, idx_base: int = 0, w=None) -> list[dict]:
@@ -103,7 +127,7 @@ def cand_records(recs: np.ndarray, T: int | None = None, idx_base: int = 0, w=No
     w = weights() if w is None else np.ascontiguousarray(w, np.float64)
     out = (CandFx * Cn)()
     lib().orc_cand_records(_p(recs), Cn, T, pitch, idx_base, _p(w), out)
-    return [_report(r) for r in out]
+    return _reports(out)
 
 
 def cand_generated(seed: int, cands, t0: int, T: int, agent_permille: int = 300, w=None, nthreads: int = 8,
@@ -115,4 +139,4 @@ def cand_generated(seed: int, cands, t0: int, T: int, agent_permille: int = 300,
     out = (CandFx * len(cands))()
     f = lib().orc_cand_generated_records if records else lib().orc_cand_generated
     f(seed, _p(cands), len(cands), t0, T, agent_permille, _p(w), out, nthreads)
-    return [_report(r) for r in out]
+    return _reports(out)

@@ -192,7 +192,7 @@ struct apo_engine {
 	uint32_t score_C = 0; bool scoring = false;
 	apo_timing timing{};
 	// per-candidate breakdown (APO_SCORE_CANDIDATES, csrc/apo_cand.cu): its own integers, never part of the accumulator vector
-	DevBuf<long long> cand_acc;              // [C][CB_INT] integers | [C][3] first-three 'bad' slots
+	DevBuf<long long> cand_acc;              // [C][CB_INT] integers | [C][3] first-three 'bad' slots | domain word
 	DevBuf<apo_candidate_report> cand_rep;   // reports of the last flagged call
 	DevBuf<float> cand_book;                 // Form T: [8][16] code -> fp32 value of the dictionary's codebook
 	uint32_t cand_C = 0;
@@ -824,15 +824,17 @@ int cand_check(apo_engine *e) {
 }
 
 // the breakdown's buffers (cand_arm's, and cand_upload_tbook's for Form T), allocated before route_twin
+uint64_t cand_words(uint32_t C) { return (uint64_t)C * (apo::CB_INT + 3) + 1; }
+
 int cand_reserve(apo_engine *e, uint32_t C) {
-	CK(reserve(e, e->cand_acc, (uint64_t)C * (apo::CB_INT + 3)));
+	CK(reserve(e, e->cand_acc, cand_words(C)));
 	CK(reserve(e, e->cand_book, 8 * 16));
 	return APO_OK;
 }
 
 // zero the breakdown of C candidates (first flagged launch of a call or session)
 int cand_arm(apo_engine *e, uint32_t C) {
-	const uint64_t words = (uint64_t)C * (apo::CB_INT + 3);
+	const uint64_t words = cand_words(C);
 	CK(reserve(e, e->cand_acc, words));
 	CK(cudaMemsetAsync(e->cand_acc.p, 0, words * 8, e->stream));
 	e->cand_armed = true;
@@ -856,6 +858,7 @@ int launch_cand(apo_engine *e, const Evals &ev, uint32_t cand_offset) {
 	P.C = ev.C; P.T = ev.count; P.idx_base = ev.idx_base; P.pitch_evals = ev.pitch_evals; P.lut = e->d_lut.p;
 	P.ints = e->cand_acc.p + (uint64_t)apo::CB_INT * cand_offset;
 	P.ex = (unsigned long long *)(e->cand_acc.p + (uint64_t)apo::CB_INT * e->score_C) + 3ull * cand_offset;
+	P.dom = (unsigned int *)(e->cand_acc.p + cand_words(e->score_C) - 1);
 	P.rows = ev.rows; P.q8 = ev.q8; P.d2 = ev.d2; P.li = ev.li; P.qw = ev.qw;
 	P.tl = ev.tl; P.th = ev.th;
 	if (ev.qt) P.cbf = ev.qt->cbf.p;
@@ -873,7 +876,12 @@ int cand_finish(apo_engine *e, uint32_t C) {
 	const long long *partials = e->partials_src ? e->partials_src : e->acc.p;
 	CK(apo::run_cand_report(e->cand_acc.p, (const unsigned long long *)(e->cand_acc.p + (uint64_t)apo::CB_INT * C), partials, C, e->cand_rep.p, e->stream));
 	e->timing.launches++;
+	uint32_t dom = 0;                                              // k_cand_breakdown's domain word (pageable: the copy waits for the stream)
+	CK(cudaMemcpyAsync(&dom, e->cand_acc.p + cand_words(C) - 1, 4, cudaMemcpyDeviceToHost, e->stream));
 	CK(cudaStreamSynchronize(e->stream));
+	if (dom)
+		return fail(e, APO_E_ARG, "APO_SCORE_CANDIDATES: an evaluation with a finalReward has a dimension with |v| >= 2048 (or NaN), "
+		                          "whose rint(v * 2^52) has no exact fixed-point sum");
 	e->cand_C = C; e->cand_ready = true;
 	return APO_OK;
 }

@@ -3,7 +3,10 @@
 //
 //   k_cand_breakdown<Loader>  one pass over the evaluations a scoring call reads (the same window, candidate offset and
 //                             record positions): per candidate the feedback tallies, the exact fixed-point sum and count of
-//                             every present dimension over the non-null evaluations, and the first three 'bad' positions
+//                             every present dimension over the non-null evaluations, and the first three 'bad' positions.
+//                             Domain: a present dimension of a non-null evaluation must satisfy |v| < 2048, where rint(v * 2^52)
+//                             still fits in int64; any other value raises P.dom and the call fails with APO_E_ARG (the scoring
+//                             kernels bound only finalReward, so d4 = 3000 with w4 = 0 scores normally but has no exact sum)
 //   k_cand_report             integers -> apo_candidate_report[C] with the rules of the corpus report (apo_corpus.cuh
 //                             report_*), rewardSum / withReward taken from the scoring call's own accumulators
 //
@@ -14,6 +17,7 @@
 //
 // For record sources a second feature (APO_SCORE_CANDIDATE_CORPUS, k_cand_corpus below) goes further: the whole corpus
 // report of every candidate's records — patterns, per-mode tallies and tool totals included — by the corpus scan's own code.
+#include <cstdlib>
 #include "apo_device.cuh"
 #include "apo_format.h"
 #include "apo_kernels.h"
@@ -25,8 +29,14 @@ constexpr int CB_THREADS = 256;
 constexpr int CB_GROUPS = 32;                       // groups of 32 consecutive evaluations per warp tile
 constexpr int CB_TILE = 32 * CB_GROUPS;             // evaluations per warp tile (one candidate)
 constexpr uint32_t CB_RUN_TILES = 1u << 16;         // flush at least every 64 M evaluations: per-lane counters stay < 2^21
+// |v| < 2^11 <=> |rint(v * 2^52)| < 2^63: the dimension values with an exact term.  Every value a loader decodes is an fp32
+// widened, and |v| >= 2048, +-inf and NaN are exactly the fp32 magnitudes whose bits are >= 0x45000000 (2048.0f).
+constexpr uint32_t CB_FX_BOUND_F32 = 0x45000000u;
 
-struct CandEval { double v[APO_NDIM]; uint32_t mask; uint32_t valid; uint32_t fb; };   // fb: 0 none, 1 good, 2 bad
+// fb: 0 none, 1 good, 2 bad; mag: the largest fp32 magnitude (as bits) of a present dimension, when the loader CHECKs
+struct CandEval { double v[APO_NDIM]; uint32_t mask; uint32_t valid; uint32_t fb; uint32_t mag; };
+
+__device__ __forceinline__ uint32_t mag_bits(float f) { return __float_as_uint(f) & 0x7FFFFFFFu; }
 
 // shared tables: the total-weight LUT and the code -> value table of the source (Form Q 8 x 256, Form T 8 x 16)
 struct CandSmem { double tw[512]; float tab[8 * 256]; };
@@ -36,8 +46,13 @@ __device__ __forceinline__ uint32_t tally_of_d0(double d0, uint32_t mask) {
 	return (mask & 1u) ? (d0 == 1.0 ? 1u : (d0 == -1.0 ? 2u : 0u)) : 0u;
 }
 
+// Each loader says whether its values can leave the fixed-point domain (CHECK): record sources cannot (reward_dims yields
+// values in [-1, 1] and the duration classes), the fp32 rows and the codebooks can.  MIN_CTAS is the kernel's launch bound
+// in CTAs per SM: 2 keeps Form D / Q / W at <= 128 registers (two CTAs per SM) with the check.
 struct LoadDims {
 	static constexpr int U = 4;                      // groups of 32 evaluations in flight per lane
+	static constexpr int MIN_CTAS = 2;
+	static constexpr bool CHECK = true;
 	struct Raw { float f[APO_NDIM]; };
 	__device__ static void fetch(const CandParams &P, uint32_t c, uint64_t t, Raw &R) {
 		const float *p = reinterpret_cast<const float *>(P.rows) + ((uint64_t)c * P.pitch_evals + t) * APO_NDIM;
@@ -45,14 +60,16 @@ struct LoadDims {
 		for (int i = 0; i < APO_NDIM; i++) R.f[i] = __ldg(p + i);
 	}
 	__device__ static void decode(const CandParams &, const CandSmem &S, const Raw &R, CandEval &E) {
-		uint32_t mask = 0;
+		uint32_t mask = 0, mag = 0;
 #pragma unroll
 		for (int i = 0; i < APO_NDIM; i++) {
 			const bool p = R.f[i] == R.f[i];
 			E.v[i] = p ? (double)R.f[i] : 0.0;
 			mask |= (p ? 1u : 0u) << i;
+			mag = max(mag, p ? mag_bits(R.f[i]) : 0u);
 		}
 		E.mask = mask;
+		E.mag = mag;
 		E.valid = S.tw[mask] > 0.0 ? 1u : 0u;
 		E.fb = tally_of_d0(E.v[0], mask);
 	}
@@ -61,6 +78,8 @@ struct LoadDims {
 template <int ROW>
 struct LoadRec {
 	static constexpr int U = ROW == 32 ? 2 : 4;       // the record decode is a long dependent chain: 4 x 32 B spills
+	static constexpr int MIN_CTAS = 1;
+	static constexpr bool CHECK = false;
 	struct Raw { uint4 q[ROW / 16]; };
 	__device__ static void fetch(const CandParams &P, uint32_t c, uint64_t t, Raw &R) {
 		const uint4 *p = reinterpret_cast<const uint4 *>(P.rows + ((uint64_t)c * P.pitch_evals + t) * ROW);
@@ -79,24 +98,29 @@ struct LoadRec {
 
 struct LoadQ {
 	static constexpr int U = 4;
+	static constexpr int MIN_CTAS = 2;
+	static constexpr bool CHECK = true;
 	struct Raw { unsigned long long q; float d2; uint32_t li; };
 	__device__ static void fetch(const CandParams &P, uint32_t c, uint64_t t, Raw &R) {
 		const uint64_t o = (uint64_t)c * P.pitch_evals + t;
 		R.q = __ldg(P.q8 + o); R.d2 = __ldg(P.d2 + o); R.li = __ldg(P.li + o);
 	}
 	__device__ static void decode(const CandParams &, const CandSmem &S, const Raw &R, CandEval &E) {
-		uint32_t mask = 0;
+		uint32_t mask = 0, mag = 0;
 #pragma unroll
 		for (int j = 0; j < 8; j++) {
 			const int dim = j < 2 ? j : j + 1;
 			const uint32_t code = (uint32_t)(R.q >> (8 * j)) & 255u;
-			E.v[dim] = code == 255u ? 0.0 : (double)S.tab[256 * j + code];
+			const float f = S.tab[256 * j + code];
+			E.v[dim] = code == 255u ? 0.0 : (double)f;
 			mask |= (code != 255u ? 1u : 0u) << dim;
+			mag = max(mag, code == 255u ? 0u : mag_bits(f));
 		}
 		const bool p2 = ((R.li >> 6) & 1u) != 0;                              // rotated index: dimension 2 lives in bit 6
 		E.v[2] = p2 ? (double)R.d2 : 0.0;
 		mask |= (p2 ? 1u : 0u) << 2;
 		E.mask = mask;
+		E.mag = max(mag, p2 ? mag_bits(R.d2) : 0u);
 		E.valid = S.tw[mask] > 0.0 ? 1u : 0u;
 		E.fb = tally_of_d0(E.v[0], mask);
 	}
@@ -105,25 +129,30 @@ struct LoadQ {
 // Form W: one word per evaluation, nibble codes (15 = absent) through the [8][256] fp32 codebook, d2 NaN = absent
 struct LoadW {
 	static constexpr int U = 4;
+	static constexpr int MIN_CTAS = 2;
+	static constexpr bool CHECK = true;
 	struct Raw { unsigned long long q; };
 	__device__ static void fetch(const CandParams &P, uint32_t c, uint64_t t, Raw &R) {
 		R.q = __ldg(P.qw + (uint64_t)c * P.pitch_evals + t);
 	}
 	__device__ static void decode(const CandParams &, const CandSmem &S, const Raw &R, CandEval &E) {
 		const uint32_t w = (uint32_t)R.q;
-		uint32_t mask = 0;
+		uint32_t mask = 0, mag = 0;
 #pragma unroll
 		for (int j = 0; j < 8; j++) {
 			const int dim = j < 2 ? j : j + 1;
 			const uint32_t nib = (w >> (4 * j)) & 15u;
-			E.v[dim] = nib == 15u ? 0.0 : (double)S.tab[256 * j + nib];
+			const float f = S.tab[256 * j + nib];
+			E.v[dim] = nib == 15u ? 0.0 : (double)f;
 			mask |= (nib != 15u ? 1u : 0u) << dim;
+			mag = max(mag, nib == 15u ? 0u : mag_bits(f));
 		}
 		const float d2 = __uint_as_float((uint32_t)(R.q >> 32));
 		const bool p2 = d2 == d2;
 		E.v[2] = p2 ? (double)d2 : 0.0;
 		mask |= (p2 ? 1u : 0u) << 2;
 		E.mask = mask;
+		E.mag = max(mag, p2 ? mag_bits(d2) : 0u);
 		E.valid = S.tw[mask] > 0.0 ? 1u : 0u;
 		E.fb = tally_of_d0(E.v[0], mask);
 	}
@@ -131,6 +160,8 @@ struct LoadW {
 
 struct LoadT {
 	static constexpr int U = 4;
+	static constexpr int MIN_CTAS = 1;
+	static constexpr bool CHECK = true;
 	struct Raw { uint32_t idx; };
 	__device__ static void fetch(const CandParams &P, uint32_t c, uint64_t t, Raw &R) {
 		const uint64_t o = (uint64_t)c * P.pitch_evals + t;
@@ -153,6 +184,10 @@ struct LoadT {
 		E.v[2] = p2 ? (double)__ldg(P.d2book + k2) : 0.0;
 		mask |= (p2 ? 1u : 0u) << 2;
 		E.mask = mask;
+		uint32_t mag = 0;                                                      // every value is an fp32 widened: exact
+#pragma unroll
+		for (int i = 0; i < APO_NDIM; i++) mag = max(mag, mag_bits((float)E.v[i]));   // absent: 0.0
+		E.mag = mag;
 		E.valid = S.tw[mask] > 0.0 ? 1u : 0u;
 		E.fb = tally_of_d0(E.v[0], mask);
 	}
@@ -163,7 +198,7 @@ struct LoadT {
 // three 'bad' positions of a run are found with ballots over groups of 32 consecutive evaluations (ascending order
 // inside the run), then merged into the candidate's slots with ex_insert, gated on the third slot.
 template <class L, int TABLE>
-__global__ void __launch_bounds__(CB_THREADS)
+__global__ void __launch_bounds__(CB_THREADS, L::MIN_CTAS)
 k_cand_breakdown(const CandParams P, uint32_t tiles_per_cand, uint64_t total_tiles) {
 	__shared__ CandSmem S;
 	for (int i = threadIdx.x; i < 512; i += CB_THREADS) S.tw[i] = P.lut[i];
@@ -178,6 +213,7 @@ k_cand_breakdown(const CandParams P, uint32_t tiles_per_cand, uint64_t total_til
 
 	Acc128 acc[APO_NDIM];
 	uint32_t cnt[APO_NDIM], n = 0, good = 0, bad = 0, nfound = 0, run = 0;
+	uint32_t dom = 0;                                                    // largest CandEval::mag of a counted evaluation
 	unsigned long long f0 = 0ull, f1 = 0ull, f2 = 0ull;                 // first 'bad' positions of the run (nfound of them)
 #pragma unroll
 	for (int i = 0; i < APO_NDIM; i++) { acc[i].zero(); cnt[i] = 0; }
@@ -232,6 +268,7 @@ k_cand_breakdown(const CandParams P, uint32_t tiles_per_cand, uint64_t total_til
 					isbad = E.fb == 2u;
 					bad += isbad ? 1u : 0u;
 					if (E.valid) {
+						if (L::CHECK) dom = max(dom, E.mag);
 #pragma unroll
 						for (int i = 0; i < APO_NDIM; i++) {
 							const bool p = (E.mask >> i) & 1u;
@@ -254,7 +291,11 @@ k_cand_breakdown(const CandParams P, uint32_t tiles_per_cand, uint64_t total_til
 		}
 	}
 	flush(cur);
+	if (dom >= CB_FX_BOUND_F32) atomicOr(P.dom, 1u);
 }
+
+// APO_K1_GRID caps the grids of both per-candidate passes as it caps the scoring kernels' (tuning and tests only, read once)
+static uint64_t cand_env_grid() { static const int g = [] { const char *s = getenv("APO_K1_GRID"); return s ? atoi(s) : 0; }(); return g > 0 ? (uint64_t)g : 0; }
 
 template <class L, int TABLE>
 static cudaError_t launch_cand(const CandParams &P, int sm_count, cudaStream_t st) {
@@ -267,6 +308,7 @@ static cudaError_t launch_cand(const CandParams &P, int sm_count, cudaStream_t s
 	uint64_t grid = (uint64_t)sm_count * (uint64_t)(per_sm > 0 ? per_sm : 1);
 	const uint64_t need = (total_tiles + (CB_THREADS / 32) - 1) / (CB_THREADS / 32);
 	if (grid > need) grid = need;
+	if (cand_env_grid() && cand_env_grid() < grid) grid = cand_env_grid();
 	k_cand_breakdown<L, TABLE><<<(unsigned)grid, CB_THREADS, 0, st>>>(P, tiles_per_cand, total_tiles);
 	return cudaGetLastError();
 }
@@ -419,6 +461,7 @@ static cudaError_t launch_cand_corpus(const CandCorpusParams &P, int sm_count, c
 	uint64_t grid = (uint64_t)sm_count * (uint64_t)(per_sm > 0 ? per_sm : 1);
 	const uint64_t need = (total_tiles + CC_WARPS - 1) / CC_WARPS;
 	if (grid > need) grid = need;
+	if (cand_env_grid() && cand_env_grid() < grid) grid = cand_env_grid();
 	k_cand_corpus<ROW><<<(unsigned)grid, CC_THREADS, 0, st>>>(P, tiles_per_cand, total_tiles);
 	return cudaGetLastError();
 }

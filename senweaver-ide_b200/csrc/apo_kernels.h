@@ -249,7 +249,8 @@ cudaError_t run_tb_index(const TbSource &S, const unsigned long long *keys, uint
 
 // ---- per-candidate breakdown (csrc/apo_cand.cu): a second pass over the evaluations a scoring call reads.
 // Own integer buffer, never part of the scoring accumulator vector: [C][CB_INT] words (a later cross-rank join is one
-// integer sum of this part) followed by the first-three 'bad' slots [nranks][C][3] (inverted indices as ex_insert keeps them).
+// integer sum of this part) followed by the first-three 'bad' slots [nranks][C][3] (inverted indices as ex_insert keeps them)
+// and one domain word (CandParams::dom).
 constexpr int CB_DIM = 0;        // 9 x (l0, l1, l2, count): exact sum of rint(v * 2^52) over non-null evaluations where dim i is present
 constexpr int CB_TALLY = 36;     // total, good, bad
 constexpr int CB_INT = 39;
@@ -275,6 +276,7 @@ struct CandParams {
 	long long *ints;                // [C][CB_INT] of candidate 0 of this launch
 	unsigned long long *ex;         // [C][3] of candidate 0 of this launch
 	const unsigned long long *qw;   // Form W words (KqParams::qw)
+	unsigned int *dom;              // set to 1 when a counted evaluation has a present dimension with |v| >= 2048 (or NaN)
 };
 cudaError_t run_cand_breakdown(const CandParams &P, int source, int sm_count, cudaStream_t st);
 // ints / ex: the whole buffer; partials: the scoring call's candidate accumulators (4 words per candidate)
