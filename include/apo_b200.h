@@ -205,8 +205,8 @@ int apo_corpus_upload_json(apo_engine *e, const char *json, uint64_t len, uint64
  * (-2, 2), else the Form W / Q copy.  It is not resident Form T (APO_SRC_TUPLES never sees it) and goes with the Form W / Q
  * copy.  APO_TUNE_NO_TWIN_T turns it off, APO_TUNE_TWIN_T builds it at any size.
  * When at most 1/64 of the evaluations have a dictionary index of 2^16 or more, the copy also holds a list of those
- * evaluations, and the calls read 2 B per evaluation (the low 16 bits of every index) and correct the listed ones; with at
- * most 2^16 distinct evaluations the list is empty.  APO_TUNE_NO_TWIN_T2 at the load builds no list, set later it keeps the
+ * evaluations, and the calls read 2 B per evaluation (a 16-bit slot plane built beside the copy: 2 B more of device memory
+ * per evaluation) and correct the listed ones; with at most 2^16 distinct evaluations the list is empty.  APO_TUNE_NO_TWIN_T2 at the load builds no list, set later it keeps the
  * calls at 3 B per evaluation. */
 int apo_dims_upload(apo_engine *e, const float *dims, uint32_t C, uint64_t T);
 int apo_dims_generate(apo_engine *e, uint64_t seed, uint32_t c0, uint32_t C, uint64_t t0, uint64_t T,

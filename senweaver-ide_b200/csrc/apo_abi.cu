@@ -108,21 +108,33 @@ struct TupleTensor : TupleDict {
 // A dictionary's table values rint(finalReward·2^52) (tuple_values).  Held (the Form T copy): val[recip] keeps the values of
 // the current weights and ok[recip] says whether they are computed (0 not yet, 1 valid, 2 an entry is outside Form T's
 // (-2, 2) domain).  Otherwise the values of one call in val[0], checked once it has synchronised (finish_score).
+// Held values of a copy with a slot plane (build_twin_t2) also keep sval[recip], the table in K1t2's slot order (slot_h
+// replicated entries, single slots up to slot_end: apo_kernels.h), re-derived with every val[recip].
 struct TupleVals {
 	const bool held;
 	DevBuf<double> ptab; DevBuf<long long> val[2]; DevBuf<uint32_t> bad;
 	uint8_t ok[2] = {0, 0};
+	DevBuf<long long> sval[2]; uint32_t slot_h = 0, slot_end = 0; bool slots = false;
 	explicit TupleVals(bool held = false) : held(held) {}
 	long long *out(bool recip) const { return val[held && recip].p; }
-	void release() { ptab.release(); val[0].release(); val[1].release(); bad.release(); ok[0] = ok[1] = 0; }
+	uint32_t n_slots() const { return slot_end + (apo::KT_SLOT_REP - 1) * slot_h + 1; }
+	void release() {
+		ptab.release(); val[0].release(); val[1].release(); bad.release(); ok[0] = ok[1] = 0;
+		sval[0].release(); sval[1].release(); slot_h = slot_end = 0; slots = false;
+	}
 };
 
 // The Form T copy of a large resident Form D tensor (build_twin_t), its held values and its exception list (build_twin_t2):
-// t2 = K1t2 may read the copy from `l` alone; xs / xb hold the xn evaluations whose index is >= 2^16 and their block index.
+// t2 = K1t2 may read the copy from its slot plane `s` alone; xs / xb hold the xn evaluations whose index is >= 2^16 and their
+// block index, ys / yb the yn whose entry has no slot.
 struct TupleCopy : TupleTensor {
 	TupleVals vals{true};
 	DevBuf<uint2> xs; DevBuf<uint32_t> xb; uint64_t xn = 0; uint32_t nblk = 0; bool t2 = false;
-	void release() { TupleTensor::release(); vals.release(); xs.release(); xb.release(); xn = 0; nblk = 0; t2 = false; }
+	DevBuf<unsigned short> s; DevBuf<uint2> ys; DevBuf<uint32_t> yb; uint64_t yn = 0;
+	void release() {
+		TupleTensor::release(); vals.release(); xs.release(); xb.release(); xn = 0; nblk = 0; t2 = false;
+		s.release(); ys.release(); yb.release(); yn = 0;
+	}
 };
 
 }  // namespace
@@ -655,6 +667,7 @@ int tuple_values(apo_engine *e, const TupleDict &d, TupleVals &v, bool recip) {
 	V.tval = v.out(recip); V.bad = v.bad.p;
 	CK(apo::run_tuple_values(V, recip, e->stream));
 	if (!v.held) { e->timing.launches++; e->tvals_check = &v; return APO_OK; }
+	if (v.slots) CK(apo::run_tuple_slots(v.out(recip), v.slot_h, v.slot_end, v.sval[recip].p, e->stream));
 	uint32_t bad = 0;
 	CK(cudaMemcpyAsync(&bad, v.bad.p, 4, cudaMemcpyDeviceToHost, e->stream));
 	CK(cudaStreamSynchronize(e->stream));
@@ -690,7 +703,8 @@ struct Evals {
 	const TupleDict *dict = nullptr;          // Form T dictionary and its values: held (the copy, route_twin), computed by every
 	TupleVals *tv = nullptr;                  // launch (resident Form T) or, t_once, once for the whole call together with the
 	bool t_once = false;                      // breakdown's codebook table (host streaming)
-	bool t2 = false;                          // the Form T copy through K1t2: tl and the exception list, not th (route_twin)
+	bool t2 = false;                          // the Form T copy through K1t2: the slot plane ts and the lists (route_twin)
+	const unsigned short *ts = nullptr;
 
 	bool records() const { return form == apo::CAND_REC32 || form == apo::CAND_REC16; }
 	uint32_t row() const { return form == apo::CAND_DIMS ? 36 : form == apo::CAND_REC32 ? 32 : 16; }
@@ -745,6 +759,7 @@ int resident_window(apo_engine *e, const apo_score_opts *o, Evals *ev) {
 	if (ev->q8) { ev->q8 += first; ev->d2 += first; ev->li += first; }
 	if (ev->qw) ev->qw += first;
 	if (ev->tl) { ev->tl += first; ev->th += first; }
+	if (ev->ts) ev->ts += first;
 	return APO_OK;
 }
 
@@ -760,6 +775,7 @@ void route_twin(apo_engine *e, const apo_score_opts *o, Evals *ev) {
 		resident_tuples(ev, e->tcopy, e->tcopy.vals);
 		ev->variant = 0;
 		ev->t2 = e->tcopy.t2 && !e->env_no_twin_t2;
+		if (ev->t2) ev->ts = e->tcopy.s.p;
 		return;
 	}
 	ev->qt = &e->qt;
@@ -781,10 +797,12 @@ int launch_score(apo_engine *e, const apo_score_opts *o, const Evals &ev, uint32
 	if (ev.form == apo::CAND_T && !ev.t_once && !ev.tv->held && (rc = tuple_values(e, *ev.dict, *ev.tv, recip))) return rc;
 	if ((rc = record_k1_event(e, 0))) return rc;
 	if (ev.form == apo::CAND_T && ev.t2) {
-		apo::Kt2Params P{};
-		P.tl = ev.tl; P.pitch_evals = ev.pitch_evals; P.C = ev.C; P.T = ev.count; P.first = ev.idx_base;
-		P.acc = acc; P.tval = ev.tv->out(recip); P.n_tuples = ev.dict->n;
-		P.xs = e->tcopy.xs.p; P.xb = e->tcopy.xb.p; P.xb_pitch = e->tcopy.nblk + 1;   // only the copy holds an exception list
+		apo::Kt2Params P{};                                  // only the copy holds a slot plane and lists
+		P.ts = ev.ts; P.pitch_evals = ev.pitch_evals; P.C = ev.C; P.T = ev.count; P.first = ev.idx_base;
+		P.acc = acc; P.sval = ev.tv->sval[recip].p; P.n_slots = ev.tv->n_slots(); P.tval = ev.tv->out(recip); P.n_tuples = ev.dict->n;
+		P.xb_pitch = e->tcopy.nblk + 1;
+		if (e->tcopy.xn) { P.xs = e->tcopy.xs.p; P.xb = e->tcopy.xb.p; }
+		if (e->tcopy.yn) { P.ys = e->tcopy.ys.p; P.yb = e->tcopy.yb.p; }
 		CK(apo::run_reward9t2(P, e->sm_count, e->stream));
 	} else if (ev.form == apo::CAND_T) {
 		apo::KtParams P{};
@@ -2010,9 +2028,10 @@ void tb_release(apo_engine *e, int rc) {
 }
 
 // Form T of the loaded evaluations into D: the engine's resident Form T (apo_dims_tuples), or the Form T copy of its Form D
-// tensor (copy, build_twin_t; *n_high: the evaluations whose index is >= 2^16).  The copy's buffers do not go through
-// reserve: releasing the copies to make room would release the one being built.
-int dims_tuples(apo_engine *e, uint32_t cap, uint32_t *n_tuples, TupleTensor &D, bool copy, uint64_t *n_high = nullptr) {
+// tensor (copy, build_twin_t; *n_high: the evaluations whose index is >= 2^16, *counts: those of the entries below 2^16).  The
+// copy's buffers do not go through reserve: releasing the copies to make room would release the one being built.
+int dims_tuples(apo_engine *e, uint32_t cap, uint32_t *n_tuples, TupleTensor &D, bool copy, uint64_t *n_high = nullptr,
+                std::vector<uint64_t> *counts16 = nullptr) {
 	if ((!e->dims_ptr && !e->compact) || e->dims_C == 0) return fail(e, APO_E_STATE, "no dims loaded");
 	if (!e->compact && (!e->twin || e->env_no_twin))
 		return fail(e, APO_E_STATE, "the loaded Form D tensor has no Form W / Q copy to build Form T from (APO_TUNE_NO_TWIN, apo_dims_attach, "
@@ -2090,6 +2109,8 @@ int dims_tuples(apo_engine *e, uint32_t cap, uint32_t *n_tuples, TupleTensor &D,
 		if (head * 4 < N * 3) return APO_E_STATE;
 		*n_high = 0;
 		for (uint32_t r = 65536; r < n; r++) *n_high += order[r].first;
+		counts16->resize(std::min<uint32_t>(n, 65536));
+		for (size_t r = 0; r < counts16->size(); r++) (*counts16)[r] = order[r].first;
 	}
 	std::vector<uint32_t> tb_pc(n);
 	std::vector<uint16_t> tb_pd(n);
@@ -2132,26 +2153,53 @@ constexpr uint32_t kTwinTCap = 1u << 20;
 
 // The exception list of the Form T copy: with it resident Form D calls read 2 B per evaluation through K1t2 instead of 3 B
 // through K1t (route_twin).  Built from n_high, the evaluations whose index is >= 2^16 (known from the dictionary's
-// counts), when at most 1/kTwinT2Share of the evaluations are such exceptions (DESIGN §8: K1t2 corrects each one with
-// three dependent loads after its stream) and a row's positions fit 32 bits; otherwise, or without room for it, the copy
-// is read through K1t as before, without an error.  APO_TUNE_NO_TWIN_T2 at the load builds none.
+// counts), when at most 1/kTwinT2Share of the evaluations are such exceptions (DESIGN §8: K1t2 corrects each one after its
+// stream) and a row's positions fit 32 bits; otherwise, or without room for it, the copy is read through K1t as before,
+// without an error.  APO_TUNE_NO_TWIN_T2 at the load builds none.
+// K1t2 reads the slot plane `s` (apo_kernels.h): the KT_SLOT_H most frequent entries get one copy per shared-memory bank pair,
+// fewer (down to none) when the evaluations of the entries left without a slot would exceed 1/kTwinT2Share of them; those
+// evaluations make the second list.  Slot plane, slot-order tables and that list need room too, or K1t serves the copy.
 constexpr uint64_t kTwinT2Share = 64;
-int build_twin_t2(apo_engine *e, uint64_t n_high) {
+int build_twin_t2(apo_engine *e, uint64_t n_high, const std::vector<uint64_t> &counts16) {
 	TupleCopy &t = e->tcopy;
 	const uint32_t C = t.C;
-	const uint64_t T = t.T;
-	if (e->env_no_twin_t2 || n_high * kTwinT2Share > (uint64_t)C * T || T > 0xFFFFFFFFull || n_high > 0xFFFFFFFFull) return APO_OK;
+	const uint64_t T = t.T, N = (uint64_t)C * T;
+	if (e->env_no_twin_t2 || n_high * kTwinT2Share > N || T > 0xFFFFFFFFull || n_high > 0xFFFFFFFFull) return APO_OK;
+	const uint32_t nblk = (uint32_t)((T + apo::KT_XBLOCK - 1) / apo::KT_XBLOCK);
+	t.nblk = nblk;
 	if (n_high) {
-		const uint32_t nblk = (uint32_t)((T + apo::KT_XBLOCK - 1) / apo::KT_XBLOCK);
 		if (t.xb.reserve((uint64_t)C * (nblk + 1)) != cudaSuccess || t.xs.reserve(n_high) != cudaSuccess) {
 			cudaGetLastError();
 			t.xb.release(); t.xs.release();
 			return APO_OK;
 		}
-		CK(apo::run_tx_build(t.l.p, t.h.p, t.pitch, C, T, t.xb.p, t.xs.p, e->sm_count, e->stream));
-		CK(cudaStreamSynchronize(e->stream));                     // the load returns with the list built, as with the copy
-		t.xn = n_high; t.nblk = nblk;
+		CK(apo::run_tx_build(t.l.p, t.h.p, t.pitch, C, T, 65536u, t.xb.p, t.xs.p, e->sm_count, e->stream));
+		t.xn = n_high;
 	}
+	uint32_t h = std::min<uint32_t>(apo::KT_SLOT_H, t.n), end = 0;
+	uint64_t ny = 0;
+	for (;; h /= 2) {
+		end = apo::kt_slot_end(t.n, h);
+		ny = 0;
+		for (size_t r = end; r < counts16.size(); r++) ny += counts16[r];
+		if (ny * kTwinT2Share <= N || h == 0) break;
+	}
+	TupleVals &v = t.vals;
+	const uint32_t n_slots = end + (apo::KT_SLOT_REP - 1) * h + 1;
+	if (t.s.reserve((uint64_t)C * t.pitch) != cudaSuccess || v.sval[0].reserve(n_slots) != cudaSuccess || v.sval[1].reserve(n_slots) != cudaSuccess ||
+	    (ny && (t.yb.reserve((uint64_t)C * (nblk + 1)) != cudaSuccess || t.ys.reserve(ny) != cudaSuccess))) {
+		cudaGetLastError();
+		t.s.release(); v.sval[0].release(); v.sval[1].release(); t.ys.release(); t.yb.release();
+		CK(cudaStreamSynchronize(e->stream));
+		return APO_OK;                                            // the exception list alone: K1t reads the copy
+	}
+	CK(apo::run_slot_plane(t.l.p, t.h.p, t.pitch, C, T, h, end, t.s.p, e->stream));
+	if (ny) CK(apo::run_tx_build(t.l.p, t.h.p, t.pitch, C, T, end, t.yb.p, t.ys.p, e->sm_count, e->stream));
+	v.slot_h = h; v.slot_end = end; v.slots = true;
+	for (int r = 0; r < 2; r++)                                     // the values computed so far (build_twin_t: recip = 0)
+		if (v.ok[r]) CK(apo::run_tuple_slots(v.out(r), h, end, v.sval[r].p, e->stream));
+	CK(cudaStreamSynchronize(e->stream));                         // the load returns with the lists built, as with the copy
+	t.yn = ny;
 	t.t2 = true;
 	return APO_OK;
 }
@@ -2166,25 +2214,27 @@ int build_twin_t(apo_engine *e) {
 	const uint64_t m = std::min<uint64_t>(kTwinTCap, N);
 	uint64_t slots = 1024;
 	while (slots < 2 * (m + 1)) slots <<= 1;
-	// index planes, dictionary, value tables, the largest exception list and its block index; the build's hash table, keys
-	// and counts
+	// index planes, dictionary, value tables, the largest exception list and its block index; the slot plane, the slot-order
+	// tables and the second list; the build's hash table, keys and counts
 	const uint64_t need = 3 * (uint64_t)C * round_up(T, 64) + m * 6 + 2 * (m + 1) * 8 + 8 * (N / kTwinT2Share) +
-	                      4 * (uint64_t)C * (T / apo::KT_XBLOCK + 2) + 16 * slots + 16 * m;
+	                      4 * (uint64_t)C * (T / apo::KT_XBLOCK + 2) + 2 * (uint64_t)C * round_up(T, 64) + 2 * 65536 * 8 +
+	                      8 * (N / kTwinT2Share) + 4 * (uint64_t)C * (T / apo::KT_XBLOCK + 2) + 16 * slots + 16 * m;
 	size_t free_bytes = 0, total_bytes = 0;
 	CK(cudaMemGetInfo(&free_bytes, &total_bytes));
 	if ((uint64_t)free_bytes < need + kTwinHeadroom) return APO_OK;
 	const std::string keep_err = e->err;
 	uint32_t n = 0;
 	uint64_t n_high = 0;
+	std::vector<uint64_t> counts16;
 	TupleVals &v = e->tcopy.vals;
-	int rc = dims_tuples(e, kTwinTCap, &n, e->tcopy, true, &n_high);
+	int rc = dims_tuples(e, kTwinTCap, &n, e->tcopy, true, &n_high, &counts16);
 	if (rc == APO_OK && (v.val[0].reserve(n + 1ull) != cudaSuccess || v.val[1].reserve(n + 1ull) != cudaSuccess ||
 	                     v.ptab.reserve(8 * 256) != cudaSuccess || v.bad.reserve(1) != cudaSuccess)) {
 		cudaGetLastError();
 		rc = APO_E_NOMEM;
 	}
 	if (rc == APO_OK) rc = tuple_values(e, e->tcopy, v, false);
-	if (rc == APO_OK) rc = build_twin_t2(e, n_high);
+	if (rc == APO_OK) rc = build_twin_t2(e, n_high, counts16);
 	tb_release(e, rc);
 	if (rc == APO_OK) return APO_OK;
 	e->tcopy.release();

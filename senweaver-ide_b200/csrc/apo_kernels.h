@@ -190,34 +190,60 @@ int kt_tile_evals();
 cudaError_t run_tuple_values(const TupleValParams &P, bool recip, cudaStream_t st);
 cudaError_t run_reward9t(KtParams P, int sm_count, cudaStream_t st);
 
-// K1t2 (k_reward9t2): the Form T copy of a resident Form D tensor read from its 16-bit plane alone, 2 B per evaluation.  The
-// dictionary is in frequency order, so an index >= 2^16 is rare; such evaluations (exceptions) are listed per row, sorted by
-// position, as {position in the row, full index}, and the kernel replaces table[index & 0xFFFF], which the stream added, by
-// table[index].  xb[c][b] is the list offset of the first exception of row c at or after position b * KT_XBLOCK (b <= nblk:
-// xb[c][nblk] = xb[c + 1][0] ends the row), so any window finds its exceptions without a search.
+// K1t2 (k_reward9t2): the Form T copy of a resident Form D tensor read from a 16-bit plane alone, 2 B per evaluation.  That
+// plane (ts) holds SLOTS of a slot-ordered copy of the table, chosen at load so that the shared-memory gather of one warp
+// instruction meets few bank conflicts:
+//   entry e <  h         16 slots 16 e + k, one per bank pair k (8-byte slots, 16 bank pairs); which copy an evaluation names
+//                        is chosen per half-warp instruction of K1t2 (k_slot_plane): apart from the bank pairs its single-slot
+//                        lanes need, when the window starts on the 128-evaluation grid
+//   zero slot 16 h       value 0, count 0
+//   entry e in [h, end)  one slot e + 15 h + 1 (end <= 2^16 - 1 - 15 h: every slot fits 16 bits)
+//   entry e >= end       the zero slot, and the evaluation is listed
+// Every copy holds the same value, so the choice of copy never changes a result.  Two lists of evaluations are added after
+// the stream from the entry-order table: the exceptions (index >= 2^16) and the evaluations of entries in [end, 2^16).  A list
+// holds per row, sorted by position, {position in the row, full index}; xb[c][b] is the list offset of the first listed
+// evaluation of row c at or after position b * KT_XBLOCK (b <= nblk: xb[c][nblk] = xb[c + 1][0] ends the row), so any window
+// finds its evaluations without a search.
 constexpr uint32_t KT_XBLOCK = 8192;
+constexpr uint32_t KT_SLOT_REP = 16;              // slots of a replicated entry
+constexpr uint32_t KT_SLOT_H = 512;               // replicated entries when the list of entries [end, 2^16) stays short
+// [end, 2^16): the entries without a slot when h of them are replicated
+inline uint32_t kt_slot_end(uint32_t n, uint32_t h) {
+	const uint32_t e = 65535u - (KT_SLOT_REP - 1) * h;
+	return n < e ? n : e;
+}
 struct Kt2Params {
-	const unsigned short *tl;       // [C][pitch] low 16 bits of the index, from the window start (a multiple of 8)
-	uint64_t pitch_evals;           // multiple of 8; tl 16-byte aligned
+	const unsigned short *ts;       // [C][pitch] slots, from the window start (a multiple of 8)
+	uint64_t pitch_evals;           // multiple of 8; ts 16-byte aligned
 	uint32_t C;
 	uint32_t tiles_per_cand;
 	uint64_t T;                     // evaluations of the window
-	uint64_t first;                 // window start in the row: the list's positions are absolute
+	uint64_t first;                 // window start in the row: the lists' positions are absolute
 	uint64_t total_tiles;
 	long long *acc;
-	const long long *tval;          // [n_tuples + 1]
+	const long long *sval;          // [n_slots] the table in slot order
+	uint32_t n_slots;
+	uint32_t hot;                   // slots [0, hot) are served from shared memory
+	const long long *tval;          // [n_tuples + 1] the table in entry order; tval[n_tuples] = 0
 	uint32_t n_tuples;
-	uint32_t hot;                   // entries [0, hot) are served from shared memory
+	uint32_t xb_pitch;              // blocks per row + 1
 	const uint2 *xs;                // exceptions, or NULL: every index is below 2^16
 	const uint32_t *xb;             // [C][xb_pitch] block index of xs
-	uint32_t xb_pitch;              // blocks per row + 1
+	const uint2 *ys;                // evaluations of entries [end, 2^16), or NULL: none
+	const uint32_t *yb;             // [C][xb_pitch] block index of ys
 };
 int kt2_tile_evals();
 cudaError_t run_reward9t2(Kt2Params P, int sm_count, cudaStream_t st);
-// the exception list of tl / th [C][tpitch] (T evaluations per row, T < 2^32): xb [C][nblk + 1] (nblk = ceil(T / KT_XBLOCK)),
-// then xs [xb[C - 1][nblk]].  The same bytes for every grid.
-cudaError_t run_tx_build(const unsigned short *tl, const unsigned char *th, uint64_t tpitch, uint32_t C, uint64_t T, uint32_t *xb,
-                         uint2 *xs, int sm_count, cudaStream_t st);
+// the list of tl / th [C][tpitch] (T evaluations per row, T < 2^32) of the evaluations whose index is >= 2^16 (lo >= 2^16:
+// the exceptions) or in [lo, 2^16): xb [C][nblk + 1] (nblk = ceil(T / KT_XBLOCK)), then xs [xb[C - 1][nblk]].  The same bytes
+// for every grid.
+cudaError_t run_tx_build(const unsigned short *tl, const unsigned char *th, uint64_t tpitch, uint32_t C, uint64_t T, uint32_t lo,
+                         uint32_t *xb, uint2 *xs, int sm_count, cudaStream_t st);
+// the slot-order table sval [end + 15 h + 1] of the entry-order one
+cudaError_t run_tuple_slots(const long long *tval, uint32_t h, uint32_t end, long long *sval, cudaStream_t st);
+// the slot plane ts [C][tpitch] of tl / th (positions t >= T are left alone)
+cudaError_t run_slot_plane(const unsigned short *tl, const unsigned char *th, uint64_t tpitch, uint32_t C, uint64_t T, uint32_t h,
+                           uint32_t end, unsigned short *ts, cudaStream_t st);
 
 // Form T built on the device from a resident tensor's Form W words or Form Q planes (apo_dims_tuples).  The key of an
 // evaluation is its Form W word: eight 4-bit codes in the low half, the fp32 tool_success_rate bits (KW_D2_ABSENT = absent)

@@ -198,17 +198,18 @@ cudaError_t run_reward9t(KtParams P, int sm_count, cudaStream_t st) {
 	return cudaGetLastError();
 }
 
-// =================================================================== K1t2: the Form T copy from its 16-bit plane
-// The same gather-and-add as K1t over tl alone: the registers th took carry a second 16-byte word, so each thread keeps
-// 16 evaluations (32 B) in flight instead of 8 (24 B).  The exceptions (index >= 2^16, csrc/apo_kernels.h) of a CTA's
-// (candidate, tile range) segments are corrected by the CTA itself once its stream is done, with four independent
-// exceptions in flight per thread.
+// =================================================================== K1t2: the Form T copy from its 16-bit slot plane
+// The same gather-and-add as K1t over one 16-bit plane: the registers th took carry a second 16-byte word, so each thread
+// keeps 16 evaluations (32 B) in flight instead of 8 (24 B).  The plane names slots of the slot-ordered table (apo_kernels.h):
+// the hot entries have one copy per shared-memory bank pair and k_slot_plane picked, per half-warp instruction, copies that
+// keep clear of each other and of the single-slot lanes.  The listed evaluations (exceptions and the entries without a slot)
+// read the zero slot; the CTA adds them from the entry-order table once its stream is done, four in flight per thread.
 constexpr int KT2_STEPS = 2;
 constexpr int KT2_TILE = KT_STEP_EVALS * KT2_STEPS;    // 16384 evaluations
-constexpr int KT2_XUNROLL = 4;                         // exceptions in flight per thread in the correction
+constexpr int KT2_XUNROLL = 4;                         // listed evaluations in flight per thread in the correction
+constexpr uint32_t KT2_HOT_MAX = 28672;                // 224 KB of shared memory: the slot-order head
 
 static_assert(KT_GROUP * KT2_STEPS <= 16, "the count field of a table entry sits 5 bits above the largest 16-entry sum");
-static_assert(KT_HOT_MAX <= 65536, "an exception's full index is never in the shared-memory head");
 
 int kt2_tile_evals() { return KT2_TILE; }
 
@@ -219,15 +220,18 @@ __device__ __forceinline__ long long kt_split(long long v, int &k) {
 	return v - (kk << KT_VALID_SHIFT);
 }
 
+// DIAG (examples/k1t2_gather.py, builds with APO_K1T2_DIAG only): 1 adds the raw slots (the stream alone), 2 clamps the
+// gather to the shared-memory head (no ld.global).  Their sums are not the table's.
+template <int DIAG>
 __global__ void __launch_bounds__(KT_THREADS, 1)
 k_reward9t2(const Kt2Params P) {
 	extern __shared__ __align__(16) long long s_hot[];
 	const int tid = threadIdx.x, lane = tid & 31;
-	for (uint32_t i = tid; i < P.hot; i += KT_THREADS) s_hot[i] = P.tval[i];
+	for (uint32_t i = tid; i < P.hot; i += KT_THREADS) s_hot[i] = P.sval[i];
 	__syncthreads();
 	const uint32_t s_base = smem_u32(s_hot);
 	const uint32_t hot = P.hot;
-	const long long *tval = P.tval;
+	const long long *sval = P.sval;
 
 	const uint64_t lo_t = P.total_tiles * blockIdx.x / gridDim.x;
 	const uint64_t hi_t = P.total_tiles * (blockIdx.x + 1ull) / gridDim.x;
@@ -243,40 +247,43 @@ k_reward9t2(const Kt2Params P) {
 		if (tile_n(jj) != (uint32_t)KT2_TILE) return;              // ragged row end: read by the scalar loop instead
 		const uint64_t e0 = (uint64_t)cc * P.pitch_evals + (uint64_t)jj * KT2_TILE + (uint64_t)tid * KT_GROUP;
 #pragma unroll
-		for (int k = 0; k < KT2_STEPS; k++) R[k] = ld_stream16(P.tl + e0 + (uint64_t)k * KT_STEP_EVALS);
+		for (int k = 0; k < KT2_STEPS; k++) R[k] = ld_stream16(P.ts + e0 + (uint64_t)k * KT_STEP_EVALS);
+	};
+	auto entry = [&](uint32_t slot) -> long long {
+		if (DIAG == 1) return (long long)slot;
+		if (DIAG == 2) return s_hot[min(slot, hot - 1)];
+		return tuple_entry(slot, hot, s_base, sval);
 	};
 
 	Acc128 acc; acc.zero();
-	int cnt = 0;                                               // signed: a correction may remove more counts than a warp added
-	// the exceptions of window tiles [ja, jb) of row cc
-	auto correct = [&](uint32_t cc, uint32_t ja, uint32_t jb) {
+	int cnt = 0;
+	// the listed evaluations (list ls, block index lb) of window tiles [ja, jb) of row cc, from the entry-order table
+	auto correct = [&](const uint2 *ls, const uint32_t *lb, uint32_t cc, uint32_t ja, uint32_t jb) {
 		const uint64_t lo = P.first + (uint64_t)ja * KT2_TILE;
 		const uint64_t hi = P.first + min((uint64_t)jb * KT2_TILE, P.T);
-		const uint32_t *xr = P.xb + (uint64_t)cc * P.xb_pitch;
+		const uint32_t *xr = lb + (uint64_t)cc * P.xb_pitch;
 		const uint32_t x0 = xr[lo / KT_XBLOCK], x1 = xr[(hi - 1) / KT_XBLOCK + 1];   // the blocks holding [lo, hi)
 		for (uint32_t x = x0 + tid; x < x1; x += KT2_XUNROLL * KT_THREADS) {
 			uint32_t full[KT2_XUNROLL];
 #pragma unroll
 			for (int u = 0; u < KT2_XUNROLL; u++) {
 				const uint32_t xi = x + u * KT_THREADS;
-				const uint2 ex = xi < x1 ? __ldg(P.xs + xi) : make_uint2(0u, 0u);
-				full[u] = xi < x1 && ex.x >= lo && ex.x < hi ? ex.y : 0u;   // index 0: both entries equal, no change
+				const uint2 ex = xi < x1 ? __ldg(ls + xi) : make_uint2(0u, 0u);
+				full[u] = xi < x1 && ex.x >= lo && ex.x < hi ? ex.y : P.n_tuples;   // the zero sentinel: no change
 			}
 #pragma unroll
 			for (int u = 0; u < KT2_XUNROLL; u++) {
-				int kf, kl;
-				const long long vf = kt_split(tuple_entry(full[u], hot, s_base, tval), kf);
-				const long long vl = kt_split(tuple_entry(full[u] & 0xFFFFu, hot, s_base, tval), kl);
-				acc.add(vf - vl);
-				cnt += kf - kl;
+				int k;
+				acc.add(kt_split(__ldg(P.tval + full[u]), k));
+				cnt += k;
 			}
 		}
 	};
 	auto flush = [&](int cand) {
 		long long *dst = P.acc + (uint64_t)ACC_PER_CAND * cand;
 		flush_acc128(acc, dst, lane);
-		const int n = (int)warp_sum_u32((uint32_t)cnt);
-		if (lane == 0 && n) atomicAdd((unsigned long long *)dst + 3, (unsigned long long)(long long)n);   // two's complement: a signed add
+		const uint32_t n = warp_sum_u32((uint32_t)cnt);
+		if (lane == 0 && n) atomicAdd((unsigned long long *)dst + 3, (unsigned long long)n);
 		acc.zero(); cnt = 0;
 	};
 
@@ -294,7 +301,7 @@ k_reward9t2(const Kt2Params P) {
 			for (int k = 0; k < KT2_STEPS; k++) {
 				const uint32_t lw[4] = {R[k].x, R[k].y, R[k].z, R[k].w};
 #pragma unroll
-				for (int q = 0; q < KT_GROUP; q++) s += tuple_entry((lw[q >> 1] >> (16 * (q & 1))) & 0xFFFFu, hot, s_base, tval);
+				for (int q = 0; q < KT_GROUP; q++) s += entry((lw[q >> 1] >> (16 * (q & 1))) & 0xFFFFu);
 			}
 			int k16;
 			acc.add(kt_split(s, k16));                         // 16 entries: values in (-2^57, 2^57) + count * 2^58
@@ -302,9 +309,9 @@ k_reward9t2(const Kt2Params P) {
 		} else {
 			const uint64_t e0 = (uint64_t)c * P.pitch_evals + (uint64_t)j * KT2_TILE;
 			for (uint32_t e = tid; e < n; e += KT_THREADS) {
-				const uint32_t idx = P.tl[e0 + e];
+				const uint32_t slot = P.ts[e0 + e];
 				int k1;
-				acc.add(kt_split(idx < hot ? s_hot[idx] : __ldg(tval + idx), k1));
+				acc.add(kt_split(DIAG ? entry(slot) : slot < hot ? s_hot[slot] : __ldg(sval + slot), k1));
 				cnt += k1;
 			}
 		}
@@ -314,12 +321,16 @@ k_reward9t2(const Kt2Params P) {
 	}
 	flush(cur);
 	// the corrections after the stream, one flush per candidate segment: inside the loop they would spill the prefetch
-	if (!P.xs) return;
+	if (!P.xs && !P.ys) return;
 	const uint32_t c_lo = (uint32_t)(lo_t / P.tiles_per_cand), c_hi = (uint32_t)((hi_t - 1) / P.tiles_per_cand);
 	for (uint32_t cc = c_lo; cc <= c_hi; cc++) {
 		const uint32_t ja = cc == c_lo ? (uint32_t)(lo_t - (uint64_t)cc * P.tiles_per_cand) : 0u;
 		const uint32_t jb = cc == c_hi ? (uint32_t)(hi_t - (uint64_t)cc * P.tiles_per_cand) : P.tiles_per_cand;
-		correct(cc, ja, jb);
+#pragma unroll 1
+		for (int y = 0; y < 2; y++) {
+			const uint2 *ls = y ? P.ys : P.xs;
+			if (ls) correct(ls, y ? P.yb : P.xb, cc, ja, jb);
+		}
 		flush((int)cc);
 	}
 }
@@ -328,47 +339,141 @@ namespace {
 int k1_env_grid() { static const int g = [] { const char *s = getenv("APO_K1_GRID"); return s ? atoi(s) : 0; }(); return g; }
 }  // namespace
 
+template <int DIAG>
+cudaError_t launch_reward9t2(const Kt2Params &P, int grid, int smem, cudaStream_t st) {
+	cudaError_t err = allow_big_smem(k_reward9t2<DIAG>, (int)(KT2_HOT_MAX * 8));   // set once per device: the largest head
+	if (err != cudaSuccess) return err;
+	k_reward9t2<DIAG><<<grid, KT_THREADS, smem, st>>>(P);
+	return cudaGetLastError();
+}
+
 cudaError_t run_reward9t2(Kt2Params P, int sm_count, cudaStream_t st) {
 	P.tiles_per_cand = (uint32_t)((P.T + KT2_TILE - 1) / KT2_TILE);
 	P.total_tiles = (uint64_t)P.tiles_per_cand * P.C;
 	if (P.total_tiles == 0) return cudaSuccess;
-	const uint64_t entries = (uint64_t)P.n_tuples + 1;
-	P.hot = (uint32_t)(entries < KT_HOT_MAX ? entries : KT_HOT_MAX);
+	P.hot = P.n_slots < KT2_HOT_MAX ? P.n_slots : KT2_HOT_MAX;
 	const int smem = (int)(((uint64_t)P.hot * 8 + 15) & ~15ull);
-	cudaError_t err = allow_big_smem(k_reward9t2, (int)(KT_HOT_MAX * 8));
-	if (err != cudaSuccess) return err;
 	int grid = sm_count;
-	if (k1_env_grid() > 0 && k1_env_grid() < grid) grid = k1_env_grid();   // tests: every CTA cut of the rows and the list
+	if (k1_env_grid() > 0 && k1_env_grid() < grid) grid = k1_env_grid();   // tests: every CTA cut of the rows and the lists
 	if ((uint64_t)grid > P.total_tiles) grid = (int)P.total_tiles;
-	k_reward9t2<<<grid, KT_THREADS, smem, st>>>(P);
+#ifdef APO_K1T2_DIAG
+	const char *d = getenv("APO_K1T2_DIAG");                    // read per launch: one process alternates the variants
+	if (d && atoi(d) == 1) return launch_reward9t2<1>(P, grid, smem, st);
+	if (d && atoi(d) == 2) return launch_reward9t2<2>(P, grid, smem, st);
+#endif
+	return launch_reward9t2<0>(P, grid, smem, st);
+}
+
+// ---- the slot-order table and the slot plane (apo_kernels.h)
+__global__ void __launch_bounds__(256)
+k_tuple_slots(const long long *tval, uint32_t h, uint32_t end, long long *sval) {
+	const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x, z = KT_SLOT_REP * h;
+	if (i > end + (KT_SLOT_REP - 1) * h) return;
+	sval[i] = i < z ? tval[i / KT_SLOT_REP] : i == z ? 0ll : tval[i - (KT_SLOT_REP - 1) * h - 1];
+}
+
+cudaError_t run_tuple_slots(const long long *tval, uint32_t h, uint32_t end, long long *sval, cudaStream_t st) {
+	const uint32_t n = end + (KT_SLOT_REP - 1) * h + 1;
+	k_tuple_slots<<<(n + 255) / 256, 256, 0, st>>>(tval, h, end, sval);
 	return cudaGetLastError();
 }
 
-// ---- the exception list, built on the device from the planes: a count pass per (row, block), one exclusive scan over
-// [C][nblk + 1], and an ordered write pass.  Each (row, block) is one CTA's item, 32 evaluations per thread.
+// One thread per half-warp instruction of K1t2 on a window that starts on the 128-evaluation grid: evaluations
+// b * 128 + 8 l + q, l < 16, of a row.  The single-slot lanes (and the zero slot) claim their bank pairs first; each distinct
+// hot entry then takes the copy in its own lane's bank pair if that is free, else the lowest free one (equal entries share a
+// copy: a broadcast).  When more distinct addresses meet than there are bank pairs the conflict cannot be avoided anyway.
+__global__ void __launch_bounds__(256)
+k_slot_plane(const unsigned short *tl, const unsigned char *th, uint64_t tpitch, uint32_t C, uint64_t T, uint32_t h, uint32_t end,
+             unsigned short *ts) {
+	const uint64_t nb = (T + 127) / 128, items = (uint64_t)C * nb * 8;
+	for (uint64_t it = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; it < items; it += (uint64_t)gridDim.x * blockDim.x) {
+		const uint32_t q = (uint32_t)(it & 7u);
+		const uint64_t r = it >> 3, c = r / nb, b = r - c * nb;
+		const uint64_t row = c * tpitch, t0 = b * 128 + q;
+		uint32_t e[16], used = 0, hot = 0;
+#pragma unroll
+		for (int l = 0; l < 16; l++) {
+			const uint64_t t = t0 + 8 * l;
+			e[l] = t < T ? (uint32_t)tl[row + t] | ((uint32_t)th[row + t] << 16) : 0xFFFFFFFFu;
+			if (e[l] < h) hot |= 1u << l;
+			else if (t < T) used |= 1u << ((e[l] < end ? e[l] + (KT_SLOT_REP - 1) * h + 1 : KT_SLOT_REP * h) & 15u);
+		}
+		uint32_t bp[16];
+#pragma unroll
+		for (int l = 0; l < 16; l++) {
+			bp[l] = 16;
+			if (!((hot >> l) & 1u)) continue;
+#pragma unroll
+			for (int m = 0; m < l; m++)
+				if (bp[l] == 16 && ((hot >> m) & 1u) && e[m] == e[l]) bp[l] = bp[m];
+			if (bp[l] == 16) {
+				const uint32_t free = ~used & 0xFFFFu;
+				bp[l] = ((free >> l) & 1u) || !free ? (uint32_t)l : (uint32_t)(__ffs(free) - 1);
+				used |= 1u << bp[l];
+			}
+		}
+#pragma unroll
+		for (int l = 0; l < 16; l++) {
+			const uint64_t t = t0 + 8 * l;
+			if (t >= T) continue;
+			const uint32_t s = (hot >> l) & 1u ? KT_SLOT_REP * e[l] + bp[l] : e[l] < end ? e[l] + (KT_SLOT_REP - 1) * h + 1 : KT_SLOT_REP * h;
+			ts[row + t] = (unsigned short)s;
+		}
+	}
+}
+
+cudaError_t run_slot_plane(const unsigned short *tl, const unsigned char *th, uint64_t tpitch, uint32_t C, uint64_t T, uint32_t h,
+                           uint32_t end, unsigned short *ts, cudaStream_t st) {
+	const uint64_t items = (uint64_t)C * ((T + 127) / 128) * 8;
+	if (items == 0) return cudaSuccess;
+	uint64_t g = (items + 255) / 256;
+	if (g > 132ull * 64) g = 132ull * 64;
+	k_slot_plane<<<(unsigned)g, 256, 0, st>>>(tl, th, tpitch, C, T, h, end, ts);
+	return cudaGetLastError();
+}
+
+// ---- the lists, built on the device from the planes: a count pass per (row, block), one exclusive scan over [C][nblk + 1],
+// and an ordered write pass.  Each (row, block) is one CTA's item, 32 evaluations per thread.  LOW: the evaluations whose
+// index is in [lo, 2^16) instead of the exceptions.
 constexpr int TX_THREADS = 256;
 constexpr int TX_EVALS = KT_XBLOCK / TX_THREADS;       // 32
 static_assert(TX_EVALS == 32, "one bit per evaluation of a thread");
 
-// bit q: evaluation t0 + q (< T) of the row has a non-zero high byte
-__device__ __forceinline__ uint32_t tx_mask(const unsigned char *th_row, uint64_t t0, uint64_t T) {
+// bit q: evaluation t0 + q (< T) of the row has a non-zero high byte (LOW: a zero high byte and a low half >= lo)
+template <bool LOW>
+__device__ __forceinline__ uint32_t tx_mask(const unsigned short *tl_row, const unsigned char *th_row, uint64_t t0, uint64_t T, uint32_t lo) {
 	if (t0 >= T) return 0u;
 	const uint4 a = ld_stream16(th_row + t0), b = ld_stream16(th_row + t0 + 16);   // inside the row's 64-padded pitch
 	const uint32_t w[8] = {a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w};
 	uint32_t m = 0;
+	if (LOW) {
 #pragma unroll
-	for (int q = 0; q < 32; q++) m |= (((w[q >> 2] >> (8 * (q & 3))) & 0xFFu) != 0u ? 1u : 0u) << q;
+		for (int i = 0; i < 4; i++) {
+			const uint4 v = ld_stream16(tl_row + t0 + 8 * i);
+			const uint32_t lw[4] = {v.x, v.y, v.z, v.w};
+#pragma unroll
+			for (int u = 0; u < 8; u++) {
+				const int q = 8 * i + u;
+				const bool in = ((w[q >> 2] >> (8 * (q & 3))) & 0xFFu) == 0u && ((lw[u >> 1] >> (16 * (u & 1))) & 0xFFFFu) >= lo;
+				m |= (in ? 1u : 0u) << q;
+			}
+		}
+	} else {
+#pragma unroll
+		for (int q = 0; q < 32; q++) m |= (((w[q >> 2] >> (8 * (q & 3))) & 0xFFu) != 0u ? 1u : 0u) << q;
+	}
 	const uint64_t left = T - t0;
 	return left >= 32 ? m : m & ((1u << left) - 1u);
 }
 
+template <bool LOW>
 __global__ void __launch_bounds__(TX_THREADS)
-k_tx_count(const unsigned char *th, uint64_t tpitch, uint32_t C, uint64_t T, uint32_t nblk, uint32_t *xb) {
+k_tx_count(const unsigned short *tl, const unsigned char *th, uint64_t tpitch, uint32_t C, uint64_t T, uint32_t lo, uint32_t nblk, uint32_t *xb) {
 	__shared__ uint32_t s_w[TX_THREADS / 32];
 	const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
 	for (uint64_t it = blockIdx.x; it < (uint64_t)C * nblk; it += gridDim.x) {
 		const uint32_t c = (uint32_t)(it / nblk), b = (uint32_t)(it - (uint64_t)c * nblk);
-		const uint32_t n = warp_sum_u32((uint32_t)__popc(tx_mask(th + (uint64_t)c * tpitch, (uint64_t)b * KT_XBLOCK + threadIdx.x * TX_EVALS, T)));
+		const uint32_t n = warp_sum_u32((uint32_t)__popc(tx_mask<LOW>(tl + (uint64_t)c * tpitch, th + (uint64_t)c * tpitch, (uint64_t)b * KT_XBLOCK + threadIdx.x * TX_EVALS, T, lo)));
 		if (lane == 0) s_w[warp] = n;
 		__syncthreads();
 		if (threadIdx.x == 0) {
@@ -405,14 +510,16 @@ k_tx_scan(uint32_t *xb, uint64_t n) {
 	for (uint64_t i = lo; i < hi; i++) { const uint32_t v = xb[i]; xb[i] = run; run += v; }
 }
 
+template <bool LOW>
 __global__ void __launch_bounds__(TX_THREADS)
-k_tx_write(const unsigned short *tl, const unsigned char *th, uint64_t tpitch, uint32_t C, uint64_t T, uint32_t nblk, const uint32_t *xb, uint2 *xs) {
+k_tx_write(const unsigned short *tl, const unsigned char *th, uint64_t tpitch, uint32_t C, uint64_t T, uint32_t lo, uint32_t nblk, const uint32_t *xb,
+           uint2 *xs) {
 	__shared__ uint32_t s_w[TX_THREADS / 32];
 	const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
 	for (uint64_t it = blockIdx.x; it < (uint64_t)C * nblk; it += gridDim.x) {
 		const uint32_t c = (uint32_t)(it / nblk), b = (uint32_t)(it - (uint64_t)c * nblk);
 		const uint64_t t0 = (uint64_t)b * KT_XBLOCK + threadIdx.x * TX_EVALS;
-		uint32_t m = tx_mask(th + (uint64_t)c * tpitch, t0, T);
+		uint32_t m = tx_mask<LOW>(tl + (uint64_t)c * tpitch, th + (uint64_t)c * tpitch, t0, T, lo);
 		const uint32_t n = (uint32_t)__popc(m);
 		uint32_t incl = n;
 #pragma unroll
@@ -431,17 +538,20 @@ k_tx_write(const unsigned short *tl, const unsigned char *th, uint64_t tpitch, u
 	}
 }
 
-cudaError_t run_tx_build(const unsigned short *tl, const unsigned char *th, uint64_t tpitch, uint32_t C, uint64_t T, uint32_t *xb,
-                         uint2 *xs, int sm_count, cudaStream_t st) {
+cudaError_t run_tx_build(const unsigned short *tl, const unsigned char *th, uint64_t tpitch, uint32_t C, uint64_t T, uint32_t lo,
+                         uint32_t *xb, uint2 *xs, int sm_count, cudaStream_t st) {
 	const uint32_t nblk = (uint32_t)((T + KT_XBLOCK - 1) / KT_XBLOCK);
 	const uint64_t items = (uint64_t)C * nblk;
 	if (items == 0) return cudaSuccess;
 	uint64_t grid = 8ull * (uint64_t)sm_count;
 	if (k1_env_grid() > 0 && (uint64_t)k1_env_grid() < grid) grid = (uint64_t)k1_env_grid();
 	if (grid > items) grid = items;
-	k_tx_count<<<(unsigned)grid, TX_THREADS, 0, st>>>(th, tpitch, C, T, nblk, xb);
+	const bool low = lo < 65536u;
+	if (low) k_tx_count<true><<<(unsigned)grid, TX_THREADS, 0, st>>>(tl, th, tpitch, C, T, lo, nblk, xb);
+	else k_tx_count<false><<<(unsigned)grid, TX_THREADS, 0, st>>>(tl, th, tpitch, C, T, lo, nblk, xb);
 	k_tx_scan<<<1, 1024, 0, st>>>(xb, (uint64_t)C * (nblk + 1));
-	k_tx_write<<<(unsigned)grid, TX_THREADS, 0, st>>>(tl, th, tpitch, C, T, nblk, xb, xs);
+	if (low) k_tx_write<true><<<(unsigned)grid, TX_THREADS, 0, st>>>(tl, th, tpitch, C, T, lo, nblk, xb, xs);
+	else k_tx_write<false><<<(unsigned)grid, TX_THREADS, 0, st>>>(tl, th, tpitch, C, T, lo, nblk, xb, xs);
 	return cudaGetLastError();
 }
 
