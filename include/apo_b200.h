@@ -138,7 +138,7 @@ int  apo_set_stream(apo_engine *e, uint64_t cuda_stream);
 /* Replace the TCS:766-776 weights (default = reference values). */
 int  apo_set_weights(apo_engine *e, const double w[APO_NDIM]);
 /* Experiment / test switches of one handle (initial value: the environment variables APO_NO_FUSE, APO_FORCE_FUSE,
- * APO_NO_STAGING, APO_JOIN_NCCL, APO_NO_TWIN, APO_NO_TWIN_T, APO_TWIN_T, APO_NO_TWIN_T2 read once at apo_create).  Results are identical for
+ * APO_NO_STAGING, APO_JOIN_NCCL, APO_NO_TWIN, APO_NO_TWIN_T, APO_TWIN_T, APO_NO_TWIN_T2, APO_NO_TWIN_H read once at apo_create).  Results are identical for
  * every setting. */
 #define APO_TUNE_NO_FUSE     0x1u  /* corpus scan / finalisation as stand-alone launches                         */
 #define APO_TUNE_FORCE_FUSE  0x2u  /* corpus scan inside the scoring launch even when it cannot hide behind it   */
@@ -148,6 +148,7 @@ int  apo_set_weights(apo_engine *e, const double w[APO_NDIM]);
 #define APO_TUNE_NO_TWIN_T   0x20u /* no Form T copy of a loaded Form D tensor is built or read: the Form Q / W copy as without it */
 #define APO_TUNE_TWIN_T      0x40u /* loads build the Form T copy whatever the tensor's size (tests, A/B runs on small tensors) */
 #define APO_TUNE_NO_TWIN_T2  0x80u /* no exception list of the Form T copy is built or read: the copy is read at 3 B per evaluation */
+#define APO_TUNE_NO_TWIN_H   0x100u /* no per-row counts of the Form T copy are built or read: whole rows read the copy as other windows */
 int  apo_set_tuning(apo_engine *e, uint32_t flags);
 int  apo_get_weights(const apo_engine *e, double w[APO_NDIM]);
 
@@ -207,7 +208,10 @@ int apo_corpus_upload_json(apo_engine *e, const char *json, uint64_t len, uint64
  * When at most 1/64 of the evaluations have a dictionary index of 2^16 or more, the copy also holds a list of those
  * evaluations, and the calls read 2 B per evaluation (a 16-bit slot plane built beside the copy: 2 B more of device memory
  * per evaluation) and correct the listed ones; with at most 2^16 distinct evaluations the list is empty.  APO_TUNE_NO_TWIN_T2 at the load builds no list, set later it keeps the
- * calls at 3 B per evaluation. */
+ * calls at 3 B per evaluation.
+ * The copy also holds, per row, how often each dictionary entry occurs in it (8 B per distinct (row, entry) pair) when those
+ * pairs take at most 1/2 B per evaluation and 4 GiB stay free beside them; calls whose window is the whole row (first 0,
+ * count 0 or T) then read those instead.  APO_TUNE_NO_TWIN_H at the load builds none, set later it reads the copy as above. */
 int apo_dims_upload(apo_engine *e, const float *dims, uint32_t C, uint64_t T);
 int apo_dims_generate(apo_engine *e, uint64_t seed, uint32_t c0, uint32_t C, uint64_t t0, uint64_t T,
                       uint32_t agent_permille);
@@ -381,6 +385,10 @@ int apo_debug_partials(apo_engine *e, int64_t *out, uint32_t C);
  * its block index (xb, *n_words = C * (blocks per row + 1) words: the list offset of row c's first exception at or after
  * position 8192 b is xb[c * (blocks per row + 1) + b]).  Both counts are 0 when no list is held.  xb / xs may be NULL. */
 int apo_debug_twin_t_list(apo_engine *e, uint64_t *n_words, uint64_t *n_exceptions, uint32_t *xb, uint32_t *xs);
+/* The per-row dictionary counts of the Form T copy (see apo_dims_upload), for tests and diagnostics: *n_pairs words, per row
+ * c < *rows the words [off[c], off[c + 1]) (off: *rows + 1 words) of the dictionary entries its evaluations name, ascending,
+ * each entry | count << 20.  Both counts are 0 when no counts are held.  off / pairs may be NULL. */
+int apo_debug_twin_h(apo_engine *e, uint32_t *rows, uint64_t *n_pairs, uint64_t *off, uint64_t *pairs);
 
 /* ---- per-candidate breakdown: why candidate c scored what it scored ------------------
  * The corpus report (APO:498-625) answered per candidate, over the evaluations of c that the

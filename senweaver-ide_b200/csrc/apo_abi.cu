@@ -126,14 +126,17 @@ struct TupleVals {
 
 // The Form T copy of a large resident Form D tensor (build_twin_t), its held values and its exception list (build_twin_t2):
 // t2 = K1t2 may read the copy from its slot plane `s` alone; xs / xb hold the xn evaluations whose index is >= 2^16 and their
-// block index, ys / yb the yn whose entry has no slot.
+// block index, ys / yb the yn whose entry has no slot.  hp / ho: the per-row dictionary counts K1h reads (build_twin_h), hn
+// pairs; hn = 0: none held.
 struct TupleCopy : TupleTensor {
 	TupleVals vals{true};
 	DevBuf<uint2> xs; DevBuf<uint32_t> xb; uint64_t xn = 0; uint32_t nblk = 0; bool t2 = false;
 	DevBuf<unsigned short> s; DevBuf<uint2> ys; DevBuf<uint32_t> yb; uint64_t yn = 0;
+	DevBuf<unsigned long long> hp; DevBuf<uint64_t> ho; uint64_t hn = 0;
 	void release() {
 		TupleTensor::release(); vals.release(); xs.release(); xb.release(); xn = 0; nblk = 0; t2 = false;
 		s.release(); ys.release(); yb.release(); yn = 0;
+		hp.release(); ho.release(); hn = 0;
 	}
 };
 
@@ -193,7 +196,7 @@ struct apo_engine {
 	void *peer_base[apo::PEER_MAX] = {nullptr}; bool peer_ipc[apo::PEER_MAX] = {false};
 	unsigned long long join_epoch = 0;
 	bool env_no_fuse = false, env_force_fuse = false, env_no_staging = false, env_nccl_join = false, env_no_twin = false;   // apo_set_tuning
-	bool env_no_twin_t = false, env_twin_t = false, env_no_twin_t2 = false;
+	bool env_no_twin_t = false, env_twin_t = false, env_no_twin_t2 = false, env_no_twin_h = false;
 	double stream_bytes_per_ms = 7.4e9, stream_q_bytes_per_ms = 5.0e9, stream_w_bytes_per_ms = 6.0e9, scan_ms_per_record = 3.35e-7;   // fuse heuristic, derived from the device at apo_create
 	size_t mem_pitch_max = 0;
 	uint8_t *zc_host = nullptr; uint64_t zc_cap = 0;   // zero-copy block of the single-trace path
@@ -705,10 +708,14 @@ struct Evals {
 	bool t_once = false;                      // breakdown's codebook table (host streaming)
 	bool t2 = false;                          // the Form T copy through K1t2: the slot plane ts and the lists (route_twin)
 	const unsigned short *ts = nullptr;
+	uint64_t hist = 0;                        // > 0: whole rows of the Form T copy through K1h, from its `hist` count pairs (route_twin)
 
 	bool records() const { return form == apo::CAND_REC32 || form == apo::CAND_REC16; }
 	uint32_t row() const { return form == apo::CAND_DIMS ? 36 : form == apo::CAND_REC32 ? 32 : 16; }
-	uint32_t bytes() const { return form == apo::CAND_T ? (t2 ? 2 : 3) : form == apo::CAND_Q ? 14 : form == apo::CAND_W ? 8 : row(); }   // read per evaluation
+	double bytes() const {                    // read per evaluation
+		if (hist) return 8.0 * (double)hist / ((double)C * (double)count);
+		return form == apo::CAND_T ? (t2 ? 2 : 3) : form == apo::CAND_Q ? 14 : form == apo::CAND_W ? 8 : row();
+	}
 	uint64_t tile() const {                   // evaluations per tile of the scoring kernel
 		return (uint64_t)(form == apo::CAND_T ? (t2 ? apo::kt2_tile_evals() : apo::kt_tile_evals()) : form == apo::CAND_Q ? apo::kq_tile_evals(variant)
 		                  : form == apo::CAND_W ? apo::kw_tile_evals() : apo::k1_tile_evals((int)row(), variant));
@@ -766,8 +773,9 @@ int resident_window(apo_engine *e, const apo_score_opts *o, Evals *ev) {
 // A resident Form D call reads the Form Q / W copy through K1q instead when one is held, the variant is the default (1-4 name
 // K1 tile shapes) and the window starts on K1q's 8-evaluation grid; under the same conditions it reads the Form T copy through
 // K1t when that is held and its values for this call's weights and `recip` are valid (twin_t_ready): through K1t2 from the
-// 16-bit plane when the copy holds an exception list and APO_TUNE_NO_TWIN_T2 is clear.  Before resident_window, after the
-// call's last allocation before its launches (reserve may release the copies).
+// 16-bit plane when the copy holds an exception list and APO_TUNE_NO_TWIN_T2 is clear; and through K1h from its counts when
+// the window is the whole row, the copy holds them and APO_TUNE_NO_TWIN_H is clear.  Before resident_window, after the call's
+// last allocation before its launches (reserve may release the copies).
 void route_twin(apo_engine *e, const apo_score_opts *o, Evals *ev) {
 	if (ev->form != apo::CAND_DIMS || !e->twin || e->env_no_twin || o->variant != 0 || o->first % 8) return;
 	ev->rows = nullptr;
@@ -776,6 +784,7 @@ void route_twin(apo_engine *e, const apo_score_opts *o, Evals *ev) {
 		ev->variant = 0;
 		ev->t2 = e->tcopy.t2 && !e->env_no_twin_t2;
 		if (ev->t2) ev->ts = e->tcopy.s.p;
+		if (!e->env_no_twin_h && o->first == 0 && (o->count == 0 || o->count == e->tcopy.T)) ev->hist = e->tcopy.hn;
 		return;
 	}
 	ev->qt = &e->qt;
@@ -796,7 +805,11 @@ int launch_score(apo_engine *e, const apo_score_opts *o, const Evals &ev, uint32
 	int rc;
 	if (ev.form == apo::CAND_T && !ev.t_once && !ev.tv->held && (rc = tuple_values(e, *ev.dict, *ev.tv, recip))) return rc;
 	if ((rc = record_k1_event(e, 0))) return rc;
-	if (ev.form == apo::CAND_T && ev.t2) {
+	if (ev.hist) {
+		apo::KhParams P{};                                   // only the copy holds counts
+		P.pairs = e->tcopy.hp.p; P.off = e->tcopy.ho.p; P.C = ev.C; P.nnz = ev.hist; P.acc = acc; P.tval = ev.tv->out(recip);
+		CK(apo::run_reward9th(P, e->sm_count, e->stream));
+	} else if (ev.form == apo::CAND_T && ev.t2) {
 		apo::Kt2Params P{};                                  // only the copy holds a slot plane and lists
 		P.ts = ev.ts; P.pitch_evals = ev.pitch_evals; P.C = ev.C; P.T = ev.count; P.first = ev.idx_base;
 		P.acc = acc; P.sval = ev.tv->sval[recip].p; P.n_slots = ev.tv->n_slots(); P.tval = ev.tv->out(recip); P.n_tuples = ev.dict->n;
@@ -1244,6 +1257,7 @@ extern "C" int apo_create(int device, apo_engine **out) {
 	e->env_no_twin_t = getenv("APO_NO_TWIN_T") != nullptr;
 	e->env_twin_t = getenv("APO_TWIN_T") != nullptr;
 	e->env_no_twin_t2 = getenv("APO_NO_TWIN_T2") != nullptr;
+	e->env_no_twin_h = getenv("APO_NO_TWIN_H") != nullptr;
 	if ((c =cudaStreamCreateWithFlags(&e->own_stream, cudaStreamNonBlocking)) != cudaSuccess) return bail("cudaStreamCreate", c);
 	if ((c = cudaStreamCreateWithFlags(&e->copy_stream, cudaStreamNonBlocking)) != cudaSuccess) return bail("cudaStreamCreate", c);
 	e->stream = e->own_stream;
@@ -1298,13 +1312,14 @@ extern "C" int apo_set_stream(apo_engine *e, uint64_t cuda_stream) {
 extern "C" int apo_set_tuning(apo_engine *e, uint32_t flags) {
 	if (!e) return APO_E_ARG;
 	if (flags & ~(APO_TUNE_NO_FUSE | APO_TUNE_FORCE_FUSE | APO_TUNE_NO_STAGING | APO_TUNE_NCCL_JOIN | APO_TUNE_NO_TWIN | APO_TUNE_NO_TWIN_T | APO_TUNE_TWIN_T |
-	              APO_TUNE_NO_TWIN_T2))
+	              APO_TUNE_NO_TWIN_T2 | APO_TUNE_NO_TWIN_H))
 		return fail(e, APO_E_ARG, "unknown tuning flag %#x", flags);
 	e->env_no_fuse = (flags & APO_TUNE_NO_FUSE) != 0; e->env_force_fuse = (flags & APO_TUNE_FORCE_FUSE) != 0;
 	e->env_no_staging = (flags & APO_TUNE_NO_STAGING) != 0; e->env_nccl_join = (flags & APO_TUNE_NCCL_JOIN) != 0;
 	e->env_no_twin = (flags & APO_TUNE_NO_TWIN) != 0;
 	e->env_no_twin_t = (flags & APO_TUNE_NO_TWIN_T) != 0; e->env_twin_t = (flags & APO_TUNE_TWIN_T) != 0;
 	e->env_no_twin_t2 = (flags & APO_TUNE_NO_TWIN_T2) != 0;
+	e->env_no_twin_h = (flags & APO_TUNE_NO_TWIN_H) != 0;
 	return APO_OK;
 }
 
@@ -2204,6 +2219,56 @@ int build_twin_t2(apo_engine *e, uint64_t n_high, const std::vector<uint64_t> &c
 	return APO_OK;
 }
 
+// The per-row dictionary counts of the Form T copy (apo_kernels.h KhParams): with them a call over whole rows reads 8 B per
+// distinct (row, entry) pair through K1h instead of 2 B per evaluation through K1t2 (route_twin).  The rows are counted in
+// batches whose dense [rows][entries] scratch stays within kTwinHScratch: a first sweep gives the exact number of pairs, and the
+// counts are kept when they take at most a quarter of K1t2's slot plane (8 nnz <= C T / 2) and kTwinHeadroom stays free beside
+// them; a second sweep writes them (a single batch keeps its counts from the first).  Otherwise, or without room, none are
+// held, without an error.  The scratch is freed before this returns.  APO_TUNE_NO_TWIN_H at the load builds none.
+constexpr uint64_t kTwinHScratch = 256ull << 20;
+int build_twin_h(apo_engine *e) {
+	TupleCopy &t = e->tcopy;
+	const uint32_t C = t.C;
+	const uint64_t T = t.T;
+	if (e->env_no_twin_h || C == 0 || T == 0 || T > 0xFFFFFFFFull || t.n == 0 || t.n > (1u << apo::KH_COUNT_SHIFT)) return APO_OK;
+	const uint32_t npitch = (uint32_t)round_up(t.n, 32), nchunk = (npitch + 8191) / 8192;
+	const uint32_t R = (uint32_t)std::min<uint64_t>(C, std::max<uint64_t>(1, kTwinHScratch / (4ull * npitch)));
+	const uint32_t nb = (C + R - 1) / R;
+	struct Scoped : DevBuf<uint32_t> { ~Scoped() { release(); } } cnt, nz;   // freed on every return path
+	if (cnt.reserve((uint64_t)R * npitch) != cudaSuccess || nz.reserve((uint64_t)R * nchunk + 1) != cudaSuccess) { cudaGetLastError(); return APO_OK; }
+	auto count = [&](uint32_t b) -> cudaError_t {
+		const uint32_t c0 = b * R, r = std::min(R, C - c0);
+		cudaError_t c = cudaMemsetAsync(cnt.p, 0, (uint64_t)r * npitch * 4, e->stream);
+		return c != cudaSuccess ? c : apo::run_th_count(t.l.p + (uint64_t)c0 * t.pitch, t.h.p + (uint64_t)c0 * t.pitch, t.pitch, r, T, npitch, cnt.p, nz.p, e->sm_count, e->stream);
+	};
+	std::vector<uint64_t> total(nb);
+	uint64_t nnz = 0;
+	for (uint32_t b = 0; b < nb; b++) {
+		CK(count(b));
+		uint32_t n = 0;
+		CK(cudaMemcpyAsync(&n, nz.p + (uint64_t)std::min(R, C - b * R) * nchunk, 4, cudaMemcpyDeviceToHost, e->stream));
+		CK(cudaStreamSynchronize(e->stream));
+		total[b] = n; nnz += n;
+	}
+	size_t free_bytes = 0, total_bytes = 0;
+	CK(cudaMemGetInfo(&free_bytes, &total_bytes));
+	if (nnz * 8 > (uint64_t)C * T / 2 || (uint64_t)free_bytes < nnz * 8 + 8ull * (C + 1) + kTwinHeadroom) return APO_OK;
+	if (t.hp.reserve(nnz) != cudaSuccess || t.ho.reserve(C + 1ull) != cudaSuccess) {
+		cudaGetLastError();
+		t.hp.release(); t.ho.release();
+		return APO_OK;
+	}
+	uint64_t base = 0;
+	for (uint32_t b = 0; b < nb; b++) {
+		if (nb > 1) CK(count(b));
+		CK(apo::run_th_write(cnt.p, std::min(R, C - b * R), npitch, nz.p, base, t.hp.p, t.ho.p + (uint64_t)b * R, e->sm_count, e->stream));
+		base += total[b];
+	}
+	CK(cudaStreamSynchronize(e->stream));                         // the load returns with the counts built, as with the copy
+	t.hn = nnz;
+	return APO_OK;
+}
+
 int build_twin_t(apo_engine *e) {
 	const uint32_t C = e->dims_C;
 	const uint64_t T = e->dims_T, N = (uint64_t)C * T;
@@ -2235,6 +2300,7 @@ int build_twin_t(apo_engine *e) {
 	}
 	if (rc == APO_OK) rc = tuple_values(e, e->tcopy, v, false);
 	if (rc == APO_OK) rc = build_twin_t2(e, n_high, counts16);
+	if (rc == APO_OK) rc = build_twin_h(e);
 	tb_release(e, rc);
 	if (rc == APO_OK) return APO_OK;
 	e->tcopy.release();
@@ -2334,6 +2400,18 @@ extern "C" int apo_debug_twin_t_list(apo_engine *e, uint64_t *n_words, uint64_t 
 	CK(cudaSetDevice(e->device));
 	if (xb) CK(cudaMemcpyAsync(xb, e->tcopy.xb.p, *n_words * 4, cudaMemcpyDeviceToHost, e->stream));
 	if (xs) CK(cudaMemcpyAsync(xs, e->tcopy.xs.p, e->tcopy.xn * 8, cudaMemcpyDeviceToHost, e->stream));
+	CK(cudaStreamSynchronize(e->stream));
+	return APO_OK;
+}
+
+extern "C" int apo_debug_twin_h(apo_engine *e, uint32_t *rows, uint64_t *n_pairs, uint64_t *off, uint64_t *pairs) {
+	if (!e || !rows || !n_pairs) return fail(e, APO_E_ARG, "NULL argument");
+	*n_pairs = e->tcopy.hn;
+	*rows = e->tcopy.hn ? e->tcopy.C : 0;
+	if (!e->tcopy.hn) return APO_OK;
+	CK(cudaSetDevice(e->device));
+	if (off) CK(cudaMemcpyAsync(off, e->tcopy.ho.p, (e->tcopy.C + 1ull) * 8, cudaMemcpyDeviceToHost, e->stream));
+	if (pairs) CK(cudaMemcpyAsync(pairs, e->tcopy.hp.p, e->tcopy.hn * 8, cudaMemcpyDeviceToHost, e->stream));
 	CK(cudaStreamSynchronize(e->stream));
 	return APO_OK;
 }

@@ -245,6 +245,29 @@ cudaError_t run_tuple_slots(const long long *tval, uint32_t h, uint32_t end, lon
 cudaError_t run_slot_plane(const unsigned short *tl, const unsigned char *th, uint64_t tpitch, uint32_t C, uint64_t T, uint32_t h,
                            uint32_t end, unsigned short *ts, cudaStream_t st);
 
+// K1h (k_reward9th): whole rows of the Form T copy from per-row dictionary counts.  A row's score needs only how often each
+// entry occurs in it: sum_t table[idx(c, t)] = sum_e count[c][e] * table[e], the same integer.  Per row c, pairs
+// [off[c], off[c + 1]) hold its entries that occur (t < T only), ascending, as entry | count << KH_COUNT_SHIFT.  The bytes
+// depend on tl / th and T alone.
+constexpr int KH_COUNT_SHIFT = 20;                // entries below 2^20 (the copy's dictionary cap), counts below 2^44
+struct KhParams {
+	const unsigned long long *pairs;  // [nnz]
+	const uint64_t *off;              // [C + 1]; off[0] = 0, off[C] = nnz
+	uint32_t C;
+	uint64_t nnz;
+	long long *acc;
+	const long long *tval;            // [n_tuples + 1] the table in entry order
+};
+cudaError_t run_reward9th(const KhParams &P, int sm_count, cudaStream_t st);
+// The counts of rows [0, R) of tl / th [R][tpitch] (evaluations t < T) into cnt [R][npitch] (npitch a multiple of 32, zeroed
+// by the caller), then nz [R * nchunk + 1] (nchunk = ceil(npitch / 8192)): the exclusive scan of the non-zero counts of every
+// (row, 8192-entry chunk); nz[R * nchunk] is their total.
+cudaError_t run_th_count(const unsigned short *tl, const unsigned char *th, uint64_t tpitch, uint32_t R, uint64_t T, uint32_t npitch,
+                         uint32_t *cnt, uint32_t *nz, int sm_count, cudaStream_t st);
+// the pairs of those rows from cnt and nz, from pairs[base] on, and their offsets off[0, R] (base included)
+cudaError_t run_th_write(const uint32_t *cnt, uint32_t R, uint32_t npitch, const uint32_t *nz, uint64_t base, unsigned long long *pairs,
+                         uint64_t *off, int sm_count, cudaStream_t st);
+
 // Form T built on the device from a resident tensor's Form W words or Form Q planes (apo_dims_tuples).  The key of an
 // evaluation is its Form W word: eight 4-bit codes in the low half, the fp32 tool_success_rate bits (KW_D2_ABSENT = absent)
 // in the high half; the host maps the high half to the d2book index afterwards.  Hash tables hold {key, value} pairs,

@@ -364,6 +364,183 @@ cudaError_t run_reward9t2(Kt2Params P, int sm_count, cudaStream_t st) {
 	return launch_reward9t2<0>(P, grid, smem, st);
 }
 
+// =================================================================== K1h: whole rows of the Form T copy from its counts
+// Each CTA takes a contiguous range of the pair array (the rows' pairs back to back), finds its first row by a binary search
+// of the offsets and walks the rows the range covers; every warp flushes once per row.  Per pair: one 8-byte load, the
+// entry's table value through the read-only path (a row's entries ascend, so a warp's gathers land in neighbouring sectors)
+// and the exact 128-bit count * value.
+constexpr int KH_THREADS = 1024;
+constexpr int KH_UNROLL = 8;                      // pairs in flight per thread
+
+// acc += n * v, exactly: n < 2^44, |v| < 2^53
+__device__ __forceinline__ void acc_add_mul(Acc128 &a, unsigned long long n, long long v) {
+	unsigned long long lo;
+	long long hi;
+	asm("mul.lo.u64 %0, %2, %3;\n\tmul.hi.s64 %1, %2, %3;" : "=l"(lo), "=l"(hi) : "l"(v), "l"((long long)n));
+	asm("add.cc.u64 %0, %0, %2;\n\taddc.s64 %1, %1, %3;" : "+l"(a.lo), "+l"(a.hi) : "l"(lo), "l"(hi));
+}
+
+__global__ void __launch_bounds__(KH_THREADS, 1)
+k_reward9th(const KhParams P) {
+	const int tid = threadIdx.x, lane = tid & 31;
+	const uint64_t lo = P.nnz * blockIdx.x / gridDim.x, hi = P.nnz * (blockIdx.x + 1ull) / gridDim.x;
+	if (lo >= hi) return;
+	uint32_t a = 0, b = P.C;                                       // off[a] <= lo < off[b]
+	while (b - a > 1) {
+		const uint32_t m = (a + b) / 2;
+		if (P.off[m] <= lo) a = m; else b = m;
+	}
+	for (uint32_t c = a; c < P.C; c++) {
+		const uint64_t r0 = P.off[c], r1 = P.off[c + 1];
+		if (r0 >= hi) break;
+		const uint64_t s = max(lo, r0), t = min(hi, r1);
+		Acc128 acc; acc.zero();
+		unsigned long long cnt = 0;
+		for (uint64_t p = s + tid; p < t; p += (uint64_t)KH_THREADS * KH_UNROLL) {
+			unsigned long long w[KH_UNROLL];
+#pragma unroll
+			for (int u = 0; u < KH_UNROLL; u++) {
+				const uint64_t q = p + (uint64_t)u * KH_THREADS;
+				if (q < t) { const uint2 v = ld_stream8(P.pairs + q); w[u] = (unsigned long long)v.x | ((unsigned long long)v.y << 32); }
+				else w[u] = 0;                                        // entry 0, count 0: adds nothing
+			}
+#pragma unroll
+			for (int u = 0; u < KH_UNROLL; u++) {
+				const unsigned long long n = w[u] >> KH_COUNT_SHIFT;
+				int k;
+				const long long v = kt_split(__ldg(P.tval + (uint32_t)(w[u] & ((1u << KH_COUNT_SHIFT) - 1u))), k);
+				acc_add_mul(acc, n, v);
+				cnt += k ? n : 0ull;
+			}
+		}
+		if (s >= t) continue;
+		long long *dst = P.acc + (uint64_t)ACC_PER_CAND * c;
+		flush_acc128(acc, dst, lane);
+		const unsigned long long nc = warp_sum_u64(cnt);
+		if (lane == 0 && nc) atomicAdd((unsigned long long *)dst + 3, nc);
+	}
+}
+
+cudaError_t run_reward9th(const KhParams &P, int sm_count, cudaStream_t st) {
+	if (P.nnz == 0) return cudaSuccess;
+	int grid = sm_count;
+	if (k1_env_grid() > 0 && k1_env_grid() < grid) grid = k1_env_grid();   // tests: every CTA cut of the rows
+	const uint64_t need = (P.nnz + KH_THREADS - 1) / KH_THREADS;
+	if ((uint64_t)grid > need) grid = (int)need;
+	k_reward9th<<<grid, KH_THREADS, 0, st>>>(P);
+	return cudaGetLastError();
+}
+
+// ---- the counts, built at load: a count pass into a dense [rows][npitch] scratch, then per (row, chunk of TH_CHUNK entries)
+// a count of the non-zero entries, one exclusive scan, and an ordered write
+constexpr int TH_THREADS = 256;
+constexpr uint32_t TH_CHUNK = TH_THREADS * 32;    // 32 entries per thread
+
+__global__ void __launch_bounds__(1024) k_tx_scan(uint32_t *xb, uint64_t n);   // the lists' scan, below
+
+__global__ void __launch_bounds__(256)
+k_th_count(const unsigned short *tl, const unsigned char *th, uint64_t tpitch, uint32_t R, uint64_t T, uint32_t npitch, uint32_t *cnt) {
+	const uint32_t lane = threadIdx.x & 31;
+	const uint64_t gpr = (T + 7) / 8, groups = (uint64_t)R * gpr;
+	// the loop bound is block-uniform: match.any needs every lane
+	for (uint64_t base = (uint64_t)blockIdx.x * blockDim.x; base < groups; base += (uint64_t)gridDim.x * blockDim.x) {
+		const uint64_t g = base + threadIdx.x;
+		uint64_t r = 0, t0 = T;
+		uint4 l = make_uint4(0u, 0u, 0u, 0u);
+		uint2 h = make_uint2(0u, 0u);
+		if (g < groups) {
+			r = g / gpr; t0 = (g - r * gpr) * 8;
+			l = ld_stream16(tl + r * tpitch + t0);
+			h = ld_stream8(th + r * tpitch + t0);
+		}
+		const uint32_t lw[4] = {l.x, l.y, l.z, l.w}, hw[2] = {h.x, h.y};
+#pragma unroll
+		for (int q = 0; q < 8; q++) {
+			const uint32_t sel = (q & 1 ? 0x0032u : 0x0010u) | ((4u + (q & 3)) << 8) | 0x4000u;   // as K1t
+			const uint32_t idx = __byte_perm(lw[q >> 1], hw[q >> 2], sel) & 0x00FFFFFFu;
+			const bool valid = t0 + q < T;                            // pads are not counted
+			const unsigned long long key = valid ? r * npitch + idx : ~0ull;
+			const uint32_t peers = __match_any_sync(0xFFFFFFFFu, key);
+			if (valid && (uint32_t)(__ffs(peers) - 1) == lane) atomicAdd(cnt + key, (uint32_t)__popc(peers));
+		}
+	}
+}
+
+// WRITE = false: nz[it] = the non-zero entries of item it = (row, chunk), and nz[R * nchunk] = 0 (the scan makes it the total).
+// WRITE: their pairs, from base + nz[it] on (nz scanned), and the row offsets.
+template <bool WRITE>
+__global__ void __launch_bounds__(TH_THREADS)
+k_th_rows(const uint32_t *cnt, uint32_t R, uint32_t npitch, uint32_t nchunk, uint32_t *nz, uint64_t base, unsigned long long *pairs,
+          uint64_t *off) {
+	__shared__ uint32_t s_w[TH_THREADS / 32];
+	const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+	const uint64_t items = (uint64_t)R * nchunk;
+	for (uint64_t it = blockIdx.x; it < items; it += gridDim.x) {
+		const uint32_t r = (uint32_t)(it / nchunk), b = (uint32_t)(it - (uint64_t)r * nchunk);
+		const uint32_t e0 = b * TH_CHUNK + threadIdx.x * 32;
+		uint32_t v[32], m = 0;
+#pragma unroll
+		for (int i = 0; i < 8; i++) {
+			const uint4 x = e0 < npitch ? *reinterpret_cast<const uint4 *>(cnt + (uint64_t)r * npitch + e0 + 4 * i) : make_uint4(0u, 0u, 0u, 0u);
+			v[4 * i] = x.x; v[4 * i + 1] = x.y; v[4 * i + 2] = x.z; v[4 * i + 3] = x.w;
+		}
+#pragma unroll
+		for (int q = 0; q < 32; q++) m |= (v[q] ? 1u : 0u) << q;
+		const uint32_t k = (uint32_t)__popc(m);
+		if (!WRITE) {
+			const uint32_t s = warp_sum_u32(k);
+			if (lane == 0) s_w[warp] = s;
+			__syncthreads();
+			if (threadIdx.x == 0) {
+				uint32_t t = 0;
+				for (int w = 0; w < TH_THREADS / 32; w++) t += s_w[w];
+				nz[it] = t;
+				if (it == items - 1) nz[items] = 0;
+			}
+			__syncthreads();
+			continue;
+		}
+		uint32_t incl = k;
+#pragma unroll
+		for (int o = 1; o < 32; o <<= 1) { const uint32_t x = __shfl_up_sync(0xFFFFFFFFu, incl, o); if (lane >= (uint32_t)o) incl += x; }
+		if (lane == 31) s_w[warp] = incl;
+		__syncthreads();
+		uint64_t o = base + nz[it] + incl - k;
+		for (uint32_t w = 0; w < warp; w++) o += s_w[w];
+		if (threadIdx.x == 0 && b == 0) off[r] = base + nz[it];
+		if (threadIdx.x == 0 && it == items - 1) off[R] = base + nz[items];
+#pragma unroll
+		for (int q = 0; q < 32; q++)
+			if ((m >> q) & 1u) pairs[o++] = (unsigned long long)(e0 + q) | ((unsigned long long)v[q] << KH_COUNT_SHIFT);
+		__syncthreads();
+	}
+}
+
+namespace {
+unsigned th_grid(uint64_t items, int sm_count) { return (unsigned)(items < 8ull * sm_count ? items : 8ull * sm_count); }
+}  // namespace
+
+cudaError_t run_th_count(const unsigned short *tl, const unsigned char *th, uint64_t tpitch, uint32_t R, uint64_t T, uint32_t npitch,
+                         uint32_t *cnt, uint32_t *nz, int sm_count, cudaStream_t st) {
+	const uint64_t groups = (uint64_t)R * ((T + 7) / 8);
+	const uint32_t nchunk = (npitch + TH_CHUNK - 1) / TH_CHUNK;
+	if (groups == 0 || nchunk == 0) return cudaSuccess;
+	k_th_count<<<th_grid((groups + 255) / 256, sm_count), 256, 0, st>>>(tl, th, tpitch, R, T, npitch, cnt);
+	const uint64_t items = (uint64_t)R * nchunk;
+	k_th_rows<false><<<th_grid(items, sm_count), TH_THREADS, 0, st>>>(cnt, R, npitch, nchunk, nz, 0, nullptr, nullptr);
+	k_tx_scan<<<1, 1024, 0, st>>>(nz, items + 1);
+	return cudaGetLastError();
+}
+
+cudaError_t run_th_write(const uint32_t *cnt, uint32_t R, uint32_t npitch, const uint32_t *nz, uint64_t base, unsigned long long *pairs,
+                         uint64_t *off, int sm_count, cudaStream_t st) {
+	const uint32_t nchunk = (npitch + TH_CHUNK - 1) / TH_CHUNK;
+	const uint64_t items = (uint64_t)R * nchunk;
+	if (items == 0) return cudaSuccess;
+	k_th_rows<true><<<th_grid(items, sm_count), TH_THREADS, 0, st>>>(cnt, R, npitch, nchunk, const_cast<uint32_t *>(nz), base, pairs, off);
+	return cudaGetLastError();
+}
+
 // ---- the slot-order table and the slot plane (apo_kernels.h)
 __global__ void __launch_bounds__(256)
 k_tuple_slots(const long long *tval, uint32_t h, uint32_t end, long long *sval) {

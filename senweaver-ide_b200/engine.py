@@ -22,7 +22,7 @@ TUPLES_MAX = 0xFFFFFF
 SCORE_CORPUS, SCORE_RECIP, SCORE_TIMING, SCORE_CANDIDATES = 0x1, 0x2, 0x4, 0x8
 SCORE_CANDIDATE_CORPUS = 0x10
 TUNE_NO_FUSE, TUNE_FORCE_FUSE, TUNE_NO_STAGING, TUNE_NCCL_JOIN, TUNE_NO_TWIN = 0x1, 0x2, 0x4, 0x8, 0x10
-TUNE_NO_TWIN_T, TUNE_TWIN_T, TUNE_NO_TWIN_T2 = 0x20, 0x40, 0x80
+TUNE_NO_TWIN_T, TUNE_TWIN_T, TUNE_NO_TWIN_T2, TUNE_NO_TWIN_H = 0x20, 0x40, 0x80, 0x100
 F_ERRORS, F_ENDED, F_VALID, F_FAILSPAN = 0x01, 0x02, 0x08, 0x10
 UNIQUE_ID_BYTES = 128
 
@@ -103,7 +103,7 @@ ABI_SYMBOLS = (
     "apo_dims_compact_download", "apo_dims_codebook", "apo_packed_encode_host", "apo_score_host_packed", "apo_dims_packed_download", "apo_dims_d2book",
     "apo_tuple_encode_host", "apo_score_host_tuples", "apo_tuples_upload", "apo_dims_tuples", "apo_tuples_download", "apo_tuples_book",
     "apo_host_alloc", "apo_host_free",
-    "apo_last_timing", "apo_debug_partials", "apo_debug_twin_t_list", "apo_candidate_reports", "apo_candidate_corpus_reports", "apo_comm_unique_id", "apo_comm_init", "apo_comm_destroy", "apo_comm_join_mode",
+    "apo_last_timing", "apo_debug_partials", "apo_debug_twin_t_list", "apo_debug_twin_h", "apo_candidate_reports", "apo_candidate_corpus_reports", "apo_comm_unique_id", "apo_comm_init", "apo_comm_destroy", "apo_comm_join_mode",
 )
 
 
@@ -189,6 +189,7 @@ def load_library() -> C.CDLL:
     L.apo_last_timing.argtypes = [vp, C.POINTER(Timing)]
     L.apo_debug_partials.argtypes = [vp, vp, u32]
     L.apo_debug_twin_t_list.argtypes = [vp, vp, vp, vp, vp]
+    L.apo_debug_twin_h.argtypes = [vp, vp, vp, vp, vp]
     L.apo_candidate_reports.argtypes = [vp, u32, u32, vp]
     L.apo_candidate_corpus_reports.argtypes = [vp, u32, u32, vp]
     L.apo_comm_unique_id.argtypes = [vp]
@@ -633,6 +634,18 @@ class Engine:
         xs = np.empty((nx.value, 2), np.uint32)
         self._ck(self._L.apo_debug_twin_t_list(self._h, C.byref(nw), C.byref(nx), _p(xb), _p(xs)))
         return xb, xs
+
+    def debug_twin_h(self):
+        """The Form T copy's per-row dictionary counts: (off [C + 1] uint64, pairs [n] uint64 entry | count << 20), or None
+        when none are held."""
+        rows, nh = C.c_uint32(0), C.c_uint64(0)
+        self._ck(self._L.apo_debug_twin_h(self._h, C.byref(rows), C.byref(nh), None, None))
+        if nh.value == 0:
+            return None
+        off = np.empty(rows.value + 1, np.uint64)
+        pairs = np.empty(nh.value, np.uint64)
+        self._ck(self._L.apo_debug_twin_h(self._h, C.byref(rows), C.byref(nh), _p(off), _p(pairs)))
+        return off, pairs
 
     # -- multi-GPU
     @staticmethod
