@@ -105,23 +105,17 @@ struct TupleTensor : TupleDict {
 	void release() { TupleDict::release(); l.release(); h.release(); unload(); }
 };
 
-// A dictionary's table values rint(finalReward·2^52) (tuple_values).  Held (the Form T copy): val[recip] keeps the values of
-// the current weights and ok[recip] says whether they are computed (0 not yet, 1 valid, 2 an entry is outside Form T's
-// (-2, 2) domain).  Otherwise the values of one call in val[0], checked once it has synchronised (finish_score).
-// Held values of a copy with a slot plane (build_twin_t2) also keep sval[recip], the table in K1t2's slot order (slot_h
-// replicated entries, single slots up to slot_end: apo_kernels.h), re-derived with every val[recip].
+// the table values rint(finalReward·2^52) of a dictionary's entries that one call computes (tuple_values)
 struct TupleVals {
-	const bool held;
-	DevBuf<double> ptab; DevBuf<long long> val[2]; DevBuf<uint32_t> bad;
-	uint8_t ok[2] = {0, 0};
-	DevBuf<long long> sval[2]; uint32_t slot_h = 0, slot_end = 0; bool slots = false;
-	explicit TupleVals(bool held = false) : held(held) {}
-	long long *out(bool recip) const { return val[held && recip].p; }
+	DevBuf<double> ptab; DevBuf<long long> val; DevBuf<uint32_t> bad;
+	void release() { ptab.release(); val.release(); bad.release(); }
+};
+
+// the Form T copy's values under the current weights (held_values): ok[recip] 0 not yet, 1 val[recip] valid, 2 outside (-2, 2)
+struct HeldVals {
+	DevBuf<double> ptab; DevBuf<long long> val[2], sval[2]; DevBuf<uint32_t> bad;   // sval: val in K1t2's slot order (apo_kernels.h)
+	uint8_t ok[2] = {0, 0}; uint32_t slot_h = 0, slot_end = 0;
 	uint32_t n_slots() const { return slot_end + (apo::KT_SLOT_REP - 1) * slot_h + 1; }
-	void release() {
-		ptab.release(); val[0].release(); val[1].release(); bad.release(); ok[0] = ok[1] = 0;
-		sval[0].release(); sval[1].release(); slot_h = slot_end = 0; slots = false;
-	}
 };
 
 // The Form T copy of a large resident Form D tensor (build_twin_t), its held values and its exception list (build_twin_t2):
@@ -129,16 +123,25 @@ struct TupleVals {
 // block index, ys / yb the yn whose entry has no slot.  hp / ho: the per-row dictionary counts K1h reads (build_twin_h), hn
 // pairs; hn = 0: none held.
 struct TupleCopy : TupleTensor {
-	TupleVals vals{true};
+	HeldVals vals;
 	DevBuf<uint2> xs; DevBuf<uint32_t> xb; uint64_t xn = 0; uint32_t nblk = 0; bool t2 = false;
 	DevBuf<unsigned short> s; DevBuf<uint2> ys; DevBuf<uint32_t> yb; uint64_t yn = 0;
 	DevBuf<unsigned long long> hp; DevBuf<uint64_t> ho; uint64_t hn = 0;
-	void release() {
-		TupleTensor::release(); vals.release(); xs.release(); xb.release(); xn = 0; nblk = 0; t2 = false;
-		s.release(); ys.release(); yb.release(); yn = 0;
-		hp.release(); ho.release(); hn = 0;
-	}
 };
+
+// What is derived from the engine's own fp32 Form D tensor at load (build_twin): kind, the Form Q copy in the engine's Form Q
+// planes (which otherwise hold a compact tensor) or the Form W words qw; t, the Form T copy beside it (t.C == 0: none).
+struct DimsCopy {
+	enum Kind { NONE, Q, W } kind = NONE;
+	DevBuf<unsigned long long> qw;
+	TupleCopy t;
+};
+
+// the tuning switches (apo_set_tuning) and the environment variables that set them when a handle is created
+const struct { const char *env; uint32_t bit; } kTuning[] = {
+	{"APO_NO_FUSE", APO_TUNE_NO_FUSE}, {"APO_FORCE_FUSE", APO_TUNE_FORCE_FUSE}, {"APO_NO_STAGING", APO_TUNE_NO_STAGING},
+	{"APO_JOIN_NCCL", APO_TUNE_NCCL_JOIN}, {"APO_NO_TWIN", APO_TUNE_NO_TWIN}, {"APO_NO_TWIN_T", APO_TUNE_NO_TWIN_T},
+	{"APO_TWIN_T", APO_TUNE_TWIN_T}, {"APO_NO_TWIN_T2", APO_TUNE_NO_TWIN_T2}, {"APO_NO_TWIN_H", APO_TUNE_NO_TWIN_H}};
 
 }  // namespace
 
@@ -152,25 +155,21 @@ struct apo_engine {
 
 	DevBuf<apo_record> corpus; uint64_t corpus_T = 0, corpus_base = 0;
 	DevBuf<float> dims; const float *dims_ptr = nullptr; uint32_t dims_C = 0; uint64_t dims_T = 0, dims_pitch = 0;
-	// Form Q (compact) copy of the evaluations: replaces dims/dims_ptr when `compact` is set; when `twin` is set it sits beside
-	// the engine's own fp32 tensor (built at load, a cache that is released whenever device memory runs short: see reserve)
+	// Form Q planes of the evaluations: the compact tensor (replacing dims/dims_ptr when `compact` is set) or the copy of kind Q
 	DevBuf<unsigned long long> q8; DevBuf<float> qd2; DevBuf<unsigned short> qli; DevBuf<uint32_t> qbook;   // qbook: [8][256] codebook + [8] overflow flags
 	DevBuf<float> stage, d_d2book, d_d2stream;
 	DevBuf<uint32_t> unpack_bad;                              // k_unpack_p: an evaluation named an empty or NaN codebook slot
-	bool compact = false, twin = false;
+	bool compact = false;
+	DimsCopy copy;                        // the copies of the fp32 tensor (a cache released whenever device memory runs short: see reserve)
 	// K1q's tables: qt for the resident Form Q tensor or the Form Q / W copy (rebuilt by apo_set_weights), qt_stream for the
 	// host-streaming Form Q / P calls (rebuilt by the next such call when its codebook or the weights changed)
 	QTables qt, qt_stream; uint64_t weights_gen = 1;
-	// twin_w: the copy is held as Form W words (qw, 8 B per evaluation; the Form Q planes are released) because no coded
-	// dimension has more than 15 values
-	DevBuf<unsigned long long> qw; bool twin_w = false;
 	uint32_t d2book_host[4096]; uint32_t d2book_n = ~0u;       // Form P export of the resident tensor (~0 = not built yet)
 	DevBuf<uint8_t> roll; uint32_t roll_C = 0, roll_row = 32; uint64_t roll_T = 0, roll_pitch = 0;   // Form R (32 B) or R16 (16 B) rows
 	TupleTensor tup;                      // resident Form T (apo_tuples_upload / apo_dims_tuples)
 	TupleDict tups;                       // the dictionary of a host-streaming Form T call
 	TupleVals tvals;                      // the values a resident Form T launch or a host-streaming Form T call computes
 	TupleVals *tvals_check = nullptr;     // the values the running call checks once it has synchronised
-	TupleCopy tcopy;                      // the Form T copy of the fp32 tensor, released with its Form W / Q copy
 	// apo_dims_tuples scratch (released when the build returns): hash table, (key, count) pairs / keys in rank order, counters
 	DevBuf<unsigned long long> tb_table, tb_keys, tb_cnt, tb_misc;
 
@@ -195,8 +194,7 @@ struct apo_engine {
 	uint8_t *peer_block = nullptr; uint64_t peer_slot_words = 0; bool peer_ok = false;
 	void *peer_base[apo::PEER_MAX] = {nullptr}; bool peer_ipc[apo::PEER_MAX] = {false};
 	unsigned long long join_epoch = 0;
-	bool env_no_fuse = false, env_force_fuse = false, env_no_staging = false, env_nccl_join = false, env_no_twin = false;   // apo_set_tuning
-	bool env_no_twin_t = false, env_twin_t = false, env_no_twin_t2 = false, env_no_twin_h = false;
+	uint32_t tune = 0;                   // APO_TUNE_* (apo_set_tuning)
 	double stream_bytes_per_ms = 7.4e9, stream_q_bytes_per_ms = 5.0e9, stream_w_bytes_per_ms = 6.0e9, scan_ms_per_record = 3.35e-7;   // fuse heuristic, derived from the device at apo_create
 	size_t mem_pitch_max = 0;
 	uint8_t *zc_host = nullptr; uint64_t zc_cap = 0;   // zero-copy block of the single-trace path
@@ -235,24 +233,19 @@ int fail(apo_engine *e, int code, const char *fmt, ...) {
 		if (_c != cudaSuccess) return fail(e, APO_E_CUDA, "%s: %s (%s:%d)", #call, cudaGetErrorString(_c), __FILE__, __LINE__); \
 	} while (0)
 
-void drop_twin(apo_engine *e) {
-	e->tcopy.release();
-	if (!e->twin) return;
-	e->q8.release(); e->qd2.release(); e->qli.release(); e->qw.release();
-	e->twin = e->twin_w = false;
-}
+void release_copies(apo_engine *e, bool keep_wq = false);   // with the copies' other code, behind the scoring helpers
 
 // Every engine buffer grows through here.  The Form Q / W / T copies of the fp32 tensor are a cache: an allocation that fails for lack
 // of device memory while it is held releases it and is tried once more, so holding it never fails a call that would succeed
 // without it.  Launches already queued may still read the copy: they finish first.  A resident call picks the evaluations
-// it reads (route_twin) only after its last allocation before its launches.
+// it reads (route_copy) only after its last allocation before its launches.
 template <class T>
 cudaError_t reserve(apo_engine *e, DevBuf<T> &b, uint64_t n) {
 	cudaError_t c = b.reserve(n);
-	if (c != cudaErrorMemoryAllocation || !e->twin) return c;
+	if (c != cudaErrorMemoryAllocation || e->copy.kind == DimsCopy::NONE) return c;
 	cudaGetLastError();
 	if ((c = cudaStreamSynchronize(e->stream)) != cudaSuccess) return c;
-	drop_twin(e);
+	release_copies(e);
 	return b.reserve(n);
 }
 
@@ -427,54 +420,10 @@ int compact_finish(apo_engine *e, uint32_t C, uint64_t T, uint64_t pitch, bool t
 	CK(cudaStreamSynchronize(e->stream));
 	int rc = load_qtables(e, e->qt, dense);
 	if (rc) return rc;
-	if (twin) e->twin = true;
+	if (twin) e->copy.kind = DimsCopy::Q;
 	else { e->compact = true; e->dims_C = C; e->dims_T = T; e->dims_pitch = pitch; e->dims_ptr = nullptr; }
 	e->d2book_n = ~0u;
 	return APO_OK;
-}
-
-// After apo_dims_upload / apo_dims_generate: the Form Q (or Form W, below) copy of the engine's fp32 tensor, which resident
-// Form D calls read through K1q (route_twin) at 14 (8) instead of 36 bytes per evaluation.  Built when the evaluations are categorical and at least
-// kTwinHeadroom of device memory stays free beside it; otherwise Form D is kept alone, without an error.
-constexpr uint64_t kTwinHeadroom = 4ull << 30;
-int build_twin_wq(apo_engine *e) {
-	const uint32_t C = e->dims_C;
-	const uint64_t T = e->dims_T, pitch = e->dims_pitch, n = (uint64_t)C * pitch;
-	if (e->env_no_twin || C == 0 || T == 0) return APO_OK;
-	size_t free_bytes = 0, total_bytes = 0;
-	CK(cudaMemGetInfo(&free_bytes, &total_bytes));
-	if ((uint64_t)free_bytes < n * 14 + kTwinHeadroom) return APO_OK;
-	if (e->q8.reserve(n) != cudaSuccess || e->qd2.reserve(n) != cudaSuccess || e->qli.reserve(n) != cudaSuccess) {
-		cudaGetLastError();                                 // another user of the device took the room since cudaMemGetInfo
-		e->q8.release(); e->qd2.release(); e->qli.release();
-		return APO_OK;
-	}
-	int rc = compact_begin(e, C, pitch);
-	if (rc) return rc;
-	CK(apo::run_transcode(e->dims_ptr, pitch, C, T, e->q8.p, e->qd2.p, pitch, e->qbook.p, e->qbook.p + 8 * 256, e->stream));
-	rc = compact_finish(e, C, T, pitch, true);
-	if (rc != APO_OK) return rc == APO_E_STATE ? APO_OK : rc;
-	// A copy whose coded dimensions take at most 15 values each (dense codes 0-14, so 15 can mean absent; true for every tensor
-	// TCS:668-763 produces) is kept as Form W words instead: 8 instead of 14 bytes per evaluation.  They are packed from the
-	// planes, so the build peaks at the fp32 tensor + the planes + the words; without kTwinHeadroom beside that, Form Q stays.
-	for (int j = 0; j < 8; j++)
-		if (e->qt.book[256 * j + 15] != 0xFFFFFFFFu) return APO_OK;
-	CK(cudaMemGetInfo(&free_bytes, &total_bytes));
-	if ((uint64_t)free_bytes < n * 8 + kTwinHeadroom) return APO_OK;
-	if (e->qw.reserve(n) != cudaSuccess) { cudaGetLastError(); return APO_OK; }
-	CK(apo::run_pack_w(e->q8.p, e->qd2.p, e->qli.p, n, e->qw.p, e->stream));
-	CK(cudaStreamSynchronize(e->stream));
-	e->q8.release(); e->qd2.release(); e->qli.release();
-	e->twin_w = true;
-	return APO_OK;
-}
-
-int build_twin_t(apo_engine *e);   // beside apo_dims_tuples, whose machinery it uses
-
-// the copies of the engine's freshly loaded fp32 tensor: Form W / Q, then (large tensors) Form T beside it
-int build_twin(apo_engine *e) {
-	const int rc = build_twin_wq(e);
-	return rc == APO_OK && e->twin ? build_twin_t(e) : rc;
 }
 
 // true when the driver does not know the pointer: ordinary pageable host memory (malloc, JS ArrayBuffer, numpy)
@@ -537,7 +486,7 @@ int copy_rows_h2d(apo_engine *e, void *dst, size_t dpitch, const void *src, size
 // when this returns).  Large pageable sources go through the staging buffers in column slices of all rows.
 int h2d_rows(apo_engine *e, void *dst, size_t dpitch, const void *src, size_t spitch, size_t width, uint32_t rows, cudaStream_t st) {
 	const uint64_t total = (uint64_t)width * rows;
-	if (total < (64ull << 20) || !is_pageable(src) || e->env_no_staging)
+	if (total < (64ull << 20) || !is_pageable(src) || (e->tune & APO_TUNE_NO_STAGING))
 		return copy_rows_h2d(e, dst, dpitch, src, spitch, width, rows, st);
 	const uint64_t cap = 256ull << 20;
 	int rc = ensure_stage(e, cap);
@@ -593,7 +542,7 @@ int ensure_scratch(apo_engine *e, uint32_t C, uint32_t K) {
 
 // the peer-memory join is used when the block exists on every rank and the partial vector fits its slots
 bool peer_join_active(const apo_engine *e, uint32_t C) {
-	return e->nranks > 1 && e->peer_ok && !e->env_nccl_join && acc_words(C, e->nranks) <= e->peer_slot_words;
+	return e->nranks > 1 && e->peer_ok && !(e->tune & APO_TUNE_NCCL_JOIN) && acc_words(C, e->nranks) <= e->peer_slot_words;
 }
 
 // layout of one rank's peer block: [PEER_MAX] arrival flags | [PEER_MAX] done-reading flags (128 B) | slot 0 | slot 1
@@ -652,37 +601,26 @@ int record_k1_event(apo_engine *e, int which) {
 	return APO_OK;
 }
 
-// Form T: the table values of every entry of d for the current weights and `recip` into v (k_tuple_values).  Held values
-// (the copy): into the buffers build_twin_t allocated, so a scoring call allocates nothing after route_twin; then waits and
-// records whether every entry lies in Form T's domain.  Otherwise device work on e->stream only, which the call checks once
-// it has synchronised (finish_score).
-int tuple_values(apo_engine *e, const TupleDict &d, TupleVals &v, bool recip) {
+// k_tuple_values: the table values of every entry of d for the current weights and `recip` into val, bad cleared first if clear_bad
+int launch_tuple_values(apo_engine *e, const TupleDict &d, double *ptab, long long *val, uint32_t *bad, bool recip, bool clear_bad) {
 	const std::vector<double> tab = make_ptab(d.book, e->W, std::nan(""));
-	if (!v.held) {
-		CK(reserve(e, v.ptab, 8 * 256));
-		CK(reserve(e, v.val[0], (uint64_t)d.n + 1));
-		CK(reserve(e, v.bad, 1));
-	}
-	CK(cudaMemcpyAsync(v.ptab.p, tab.data(), 8 * 256 * 8, cudaMemcpyHostToDevice, e->stream));   // pageable source: consumed when this returns
-	if (e->tvals_check != &v) CK(cudaMemsetAsync(v.bad.p, 0, 4, e->stream));   // a session keeps the flags of its earlier launches
+	CK(cudaMemcpyAsync(ptab, tab.data(), 8 * 256 * 8, cudaMemcpyHostToDevice, e->stream));   // pageable source: consumed when this returns
+	if (clear_bad) CK(cudaMemsetAsync(bad, 0, 4, e->stream));
 	apo::TupleValParams V{};
-	V.tb_pc = d.pc.p; V.tb_pd = d.pd.p; V.n = d.n; V.ptab = v.ptab.p; V.lut = e->d_lut.p; V.d2book = d.d2.p; V.w2 = e->W.w[2];
-	V.tval = v.out(recip); V.bad = v.bad.p;
+	V.tb_pc = d.pc.p; V.tb_pd = d.pd.p; V.n = d.n; V.ptab = ptab; V.lut = e->d_lut.p; V.d2book = d.d2.p; V.w2 = e->W.w[2];
+	V.tval = val; V.bad = bad;
 	CK(apo::run_tuple_values(V, recip, e->stream));
-	if (!v.held) { e->timing.launches++; e->tvals_check = &v; return APO_OK; }
-	if (v.slots) CK(apo::run_tuple_slots(v.out(recip), v.slot_h, v.slot_end, v.sval[recip].p, e->stream));
-	uint32_t bad = 0;
-	CK(cudaMemcpyAsync(&bad, v.bad.p, 4, cudaMemcpyDeviceToHost, e->stream));
-	CK(cudaStreamSynchronize(e->stream));
-	v.ok[recip] = bad ? 2 : 1;
 	return APO_OK;
 }
 
-// a resident Form D call: the copy's values for its `recip`, computed once per weight set by the first call that needs them
-int twin_t_ready(apo_engine *e, const apo_score_opts *o) {
-	const bool recip = (o->flags & APO_SCORE_RECIP) != 0;
-	if (o->source != APO_SRC_DIMS || e->tcopy.C == 0 || e->env_no_twin_t || e->tcopy.vals.ok[recip]) return APO_OK;
-	return tuple_values(e, e->tcopy, e->tcopy.vals, recip);
+// one call's values of its dictionary d into v: device work on e->stream only, checked once the call has synchronised (finish_score)
+int tuple_values(apo_engine *e, const TupleDict &d, TupleVals &v, bool recip) {
+	CK(reserve(e, v.ptab, 8 * 256));
+	CK(reserve(e, v.val, (uint64_t)d.n + 1));
+	CK(reserve(e, v.bad, 1));
+	if (const int rc = launch_tuple_values(e, d, v.ptab.p, v.val.p, v.bad.p, recip, e->tvals_check != &v)) return rc;   // a session keeps the flags of its earlier launches
+	e->timing.launches++; e->tvals_check = &v;
+	return APO_OK;
 }
 
 // ---- the evaluations one launch reads: a resident tensor (or a window of it), or one window of a host-streaming call
@@ -700,32 +638,30 @@ struct Evals {
 	const float *d2 = nullptr;
 	const unsigned short *li = nullptr;
 	const QTables *qt = nullptr;              // Form Q / W: K1q's tables of the codebook
-	const unsigned long long *qw = nullptr;   // Form W words (the copy of a resident Form D tensor, route_twin)
+	const unsigned long long *qw = nullptr;   // Form W words (the copy of a resident Form D tensor, route_copy)
 	const unsigned short *tl = nullptr;       // Form T planes
 	const unsigned char *th = nullptr;
-	const TupleDict *dict = nullptr;          // Form T dictionary and its values: held (the copy, route_twin), computed by every
-	TupleVals *tv = nullptr;                  // launch (resident Form T) or, t_once, once for the whole call together with the
-	bool t_once = false;                      // breakdown's codebook table (host streaming)
-	bool t2 = false;                          // the Form T copy through K1t2: the slot plane ts and the lists (route_twin)
-	const unsigned short *ts = nullptr;
-	uint64_t hist = 0;                        // > 0: whole rows of the Form T copy through K1h, from its `hist` count pairs (route_twin)
+	const TupleDict *dict = nullptr;          // Form T dictionary; its values (e->tvals) computed by every launch or, t_once, once
+	bool t_once = false;                      // for the whole call with the breakdown's codebook table (host streaming)
+	const TupleCopy *copy = nullptr;          // or the Form T copy of a resident Form D tensor, with its values, read by `read` (route_copy)
+	enum CopyRead { K1t, K1t2, K1h } read = K1t;
 
 	bool records() const { return form == apo::CAND_REC32 || form == apo::CAND_REC16; }
 	uint32_t row() const { return form == apo::CAND_DIMS ? 36 : form == apo::CAND_REC32 ? 32 : 16; }
 	double bytes() const {                    // read per evaluation
-		if (hist) return 8.0 * (double)hist / ((double)C * (double)count);
-		return form == apo::CAND_T ? (t2 ? 2 : 3) : form == apo::CAND_Q ? 14 : form == apo::CAND_W ? 8 : row();
+		if (read == K1h) return 8.0 * (double)copy->hn / ((double)C * (double)count);
+		return form == apo::CAND_T ? (read == K1t2 ? 2 : 3) : form == apo::CAND_Q ? 14 : form == apo::CAND_W ? 8 : row();
 	}
 	uint64_t tile() const {                   // evaluations per tile of the scoring kernel
-		return (uint64_t)(form == apo::CAND_T ? (t2 ? apo::kt2_tile_evals() : apo::kt_tile_evals()) : form == apo::CAND_Q ? apo::kq_tile_evals(variant)
+		return (uint64_t)(form == apo::CAND_T ? (read == K1t2 ? apo::kt2_tile_evals() : apo::kt_tile_evals()) : form == apo::CAND_Q ? apo::kq_tile_evals(variant)
 		                  : form == apo::CAND_W ? apo::kw_tile_evals() : apo::k1_tile_evals((int)row(), variant));
 	}
 };
 
-// ev reads all of the resident Form T tensor t with the values v
-void resident_tuples(Evals *ev, const TupleTensor &t, TupleVals &v) {
+// ev reads all of the resident Form T tensor t
+void resident_tuples(Evals *ev, const TupleTensor &t) {
 	ev->form = apo::CAND_T; ev->C = t.C; ev->count = t.T; ev->pitch_evals = t.pitch;
-	ev->tl = t.l.p; ev->th = t.h.p; ev->dict = &t; ev->tv = &v;
+	ev->tl = t.l.p; ev->th = t.h.p; ev->dict = &t;
 }
 
 // the whole tensor loaded for o->source (count = all its evaluations)
@@ -737,7 +673,7 @@ int resident_evals(apo_engine *e, const apo_score_opts *o, Evals *ev) {
 	v.variant = (int)o->variant;
 	if (o->source == APO_SRC_TUPLES) {
 		if (e->tup.l.p == nullptr || e->tup.C == 0) return fail(e, APO_E_STATE, "no tuples loaded");
-		resident_tuples(&v, e->tup, e->tvals);
+		resident_tuples(&v, e->tup);
 	} else if (o->source == APO_SRC_ROLLOUTS) {
 		if (e->roll.p == nullptr || e->roll_C == 0) return fail(e, APO_E_STATE, "no rollouts loaded");
 		v.form = e->roll_row == 32 ? apo::CAND_REC32 : apo::CAND_REC16; v.C = e->roll_C; v.count = e->roll_T; v.pitch_evals = e->roll_pitch;
@@ -766,61 +702,33 @@ int resident_window(apo_engine *e, const apo_score_opts *o, Evals *ev) {
 	if (ev->q8) { ev->q8 += first; ev->d2 += first; ev->li += first; }
 	if (ev->qw) ev->qw += first;
 	if (ev->tl) { ev->tl += first; ev->th += first; }
-	if (ev->ts) ev->ts += first;
 	return APO_OK;
 }
 
-// A resident Form D call reads the Form Q / W copy through K1q instead when one is held, the variant is the default (1-4 name
-// K1 tile shapes) and the window starts on K1q's 8-evaluation grid; under the same conditions it reads the Form T copy through
-// K1t when that is held and its values for this call's weights and `recip` are valid (twin_t_ready): through K1t2 from the
-// 16-bit plane when the copy holds an exception list and APO_TUNE_NO_TWIN_T2 is clear; and through K1h from its counts when
-// the window is the whole row, the copy holds them and APO_TUNE_NO_TWIN_H is clear.  Before resident_window, after the call's
-// last allocation before its launches (reserve may release the copies).
-void route_twin(apo_engine *e, const apo_score_opts *o, Evals *ev) {
-	if (ev->form != apo::CAND_DIMS || !e->twin || e->env_no_twin || o->variant != 0 || o->first % 8) return;
-	ev->rows = nullptr;
-	if (e->tcopy.C && !e->env_no_twin_t && e->tcopy.vals.ok[(o->flags & APO_SCORE_RECIP) != 0] == 1) {
-		resident_tuples(ev, e->tcopy, e->tcopy.vals);
-		ev->variant = 0;
-		ev->t2 = e->tcopy.t2 && !e->env_no_twin_t2;
-		if (ev->t2) ev->ts = e->tcopy.s.p;
-		if (!e->env_no_twin_h && o->first == 0 && (o->count == 0 || o->count == e->tcopy.T)) ev->hist = e->tcopy.hn;
-		return;
-	}
-	ev->qt = &e->qt;
-	if (e->twin_w) {                                         // <= 15 codes per dimension: the prefix table always fits
-		ev->form = apo::CAND_W; ev->qw = e->qw.p; ev->variant = 0;
-		return;
-	}
-	ev->form = apo::CAND_Q;
-	ev->q8 = e->q8.p; ev->d2 = e->qd2.p; ev->li = e->qli.p;
-	ev->variant = e->qt.pair_ok ? 0 : 4;                     // as resident_evals for a compact tensor
-}
-
-// one scoring launch (K1 / K1q / K1t) over ev into candidates [cand_offset, ...); fused: the corpus scan and the tail ride on it
+// one scoring launch (K1 / K1q / K1t / K1t2 / K1h) over ev into candidates [cand_offset, ...); fused: the corpus scan and tail ride on it
 int launch_score(apo_engine *e, const apo_score_opts *o, const Evals &ev, uint32_t cand_offset, const apo::K2Params *fused = nullptr) {
 	if (!ev.count) return APO_OK;
 	const bool recip = (o->flags & APO_SCORE_RECIP) != 0;
 	long long *acc = e->acc.p + (uint64_t)ACC_PER_CAND * cand_offset;
 	int rc;
-	if (ev.form == apo::CAND_T && !ev.t_once && !ev.tv->held && (rc = tuple_values(e, *ev.dict, *ev.tv, recip))) return rc;
+	if (ev.form == apo::CAND_T && !ev.copy && !ev.t_once && (rc = tuple_values(e, *ev.dict, e->tvals, recip))) return rc;
 	if ((rc = record_k1_event(e, 0))) return rc;
-	if (ev.hist) {
-		apo::KhParams P{};                                   // only the copy holds counts
-		P.pairs = e->tcopy.hp.p; P.off = e->tcopy.ho.p; P.C = ev.C; P.nnz = ev.hist; P.acc = acc; P.tval = ev.tv->out(recip);
+	if (const TupleCopy *t = ev.copy; ev.read == Evals::K1h) {   // the copy's values were computed before the route
+		apo::KhParams P{};
+		P.pairs = t->hp.p; P.off = t->ho.p; P.C = ev.C; P.nnz = t->hn; P.acc = acc; P.tval = t->vals.val[recip].p;
 		CK(apo::run_reward9th(P, e->sm_count, e->stream));
-	} else if (ev.form == apo::CAND_T && ev.t2) {
-		apo::Kt2Params P{};                                  // only the copy holds a slot plane and lists
-		P.ts = ev.ts; P.pitch_evals = ev.pitch_evals; P.C = ev.C; P.T = ev.count; P.first = ev.idx_base;
-		P.acc = acc; P.sval = ev.tv->sval[recip].p; P.n_slots = ev.tv->n_slots(); P.tval = ev.tv->out(recip); P.n_tuples = ev.dict->n;
-		P.xb_pitch = e->tcopy.nblk + 1;
-		if (e->tcopy.xn) { P.xs = e->tcopy.xs.p; P.xb = e->tcopy.xb.p; }
-		if (e->tcopy.yn) { P.ys = e->tcopy.ys.p; P.yb = e->tcopy.yb.p; }
+	} else if (ev.read == Evals::K1t2) {
+		apo::Kt2Params P{};
+		P.ts = t->s.p + ev.idx_base; P.pitch_evals = ev.pitch_evals; P.C = ev.C; P.T = ev.count; P.first = ev.idx_base;
+		P.acc = acc; P.sval = t->vals.sval[recip].p; P.n_slots = t->vals.n_slots(); P.tval = t->vals.val[recip].p; P.n_tuples = t->n;
+		P.xb_pitch = t->nblk + 1;
+		if (t->xn) { P.xs = t->xs.p; P.xb = t->xb.p; }
+		if (t->yn) { P.ys = t->ys.p; P.yb = t->yb.p; }
 		CK(apo::run_reward9t2(P, e->sm_count, e->stream));
 	} else if (ev.form == apo::CAND_T) {
 		apo::KtParams P{};
-		P.tl = ev.tl; P.th = ev.th; P.pitch_evals = ev.pitch_evals; P.C = ev.C; P.T = ev.count;
-		P.acc = acc; P.n_tuples = ev.dict->n; P.tval = ev.tv->out(recip); P.bad = ev.tv->bad.p;
+		P.tl = ev.tl; P.th = ev.th; P.pitch_evals = ev.pitch_evals; P.C = ev.C; P.T = ev.count; P.acc = acc; P.n_tuples = ev.dict->n;
+		P.tval = t ? t->vals.val[recip].p : e->tvals.val.p; P.bad = t ? t->vals.bad.p : e->tvals.bad.p;
 		CK(apo::run_reward9t(P, e->sm_count, e->stream));
 	} else if (ev.form == apo::CAND_Q || ev.form == apo::CAND_W) {
 		apo::KqParams Q{};
@@ -854,7 +762,7 @@ int cand_check(apo_engine *e) {
 	return APO_OK;
 }
 
-// the breakdown's buffers (cand_arm's, and cand_upload_tbook's for Form T), allocated before route_twin
+// the breakdown's buffers (cand_arm's, and cand_upload_tbook's for Form T), allocated before route_copy
 uint64_t cand_words(uint32_t C) { return (uint64_t)C * (apo::CB_INT + 3) + 1; }
 
 int cand_reserve(apo_engine *e, uint32_t C) {
@@ -1111,9 +1019,407 @@ int score_arm(apo_engine *e, const apo_score_opts *o, uint32_t C, bool begin, ui
 	return wants_ccorp(o) && !e->ccorp_armed ? ccorp_arm(e, C) : APO_OK;
 }
 
-}  // namespace
+// order of a d2book: by value, -0.0 (sign bit set) before +0.0
+bool d2_before(uint32_t x, uint32_t y) {
+	float fx, fy; memcpy(&fx, &x, 4); memcpy(&fy, &y, 4);
+	if (fx != fy) return fx < fy;
+	return x > y;
+}
 
-namespace {
+template <class T>
+int tb_reserve(apo_engine *e, DevBuf<T> &b, uint64_t n, const char *what, bool copy = false) {
+	const cudaError_t c = copy ? b.reserve(n) : reserve(e, b, n);
+	if (c == cudaSuccess) return APO_OK;
+	cudaGetLastError();
+	return fail(e, c == cudaErrorMemoryAllocation ? APO_E_NOMEM : APO_E_CUDA, "%s (%llu elements): %s", what, (unsigned long long)n, cudaGetErrorString(c));
+}
+
+void tb_release(apo_engine *e, int rc) {
+	if (rc != APO_OK) cudaStreamSynchronize(e->stream);          // nothing a failed build queued may still use what is released
+	e->tb_table.release(); e->tb_keys.release(); e->tb_cnt.release(); e->tb_misc.release();
+}
+
+struct TbRanked {
+	apo::TbSource S{};
+	uint64_t tpitch = 0;
+	uint32_t d2book[4096];
+	std::vector<std::pair<unsigned long long, unsigned long long>> order;     // (count, tuple key)
+};
+
+// Form T of the loaded evaluations into D: the engine's resident Form T (apo_dims_tuples), or the Form T copy of its Form D
+// tensor (copy, build_twin_t; its buffers do not go through reserve, which could release the copy being built).  First the
+// ranking into R: D's buffers and the scratch, the distinct evaluations (n_tuples: how many past cap), d2book, their order.
+int tuples_rank(apo_engine *e, uint32_t cap, uint32_t *n_tuples, TupleTensor &D, bool copy, TbRanked &R) {
+	if ((!e->dims_ptr && !e->compact) || e->dims_C == 0) return fail(e, APO_E_STATE, "no dims loaded");
+	if (!e->compact && (e->copy.kind == DimsCopy::NONE || (e->tune & APO_TUNE_NO_TWIN)))
+		return fail(e, APO_E_STATE, "the loaded Form D tensor has no Form W / Q copy to build Form T from (APO_TUNE_NO_TWIN, apo_dims_attach, "
+		                            "or too little device memory at load): call apo_dims_compact first");
+	if (e->copy.kind != DimsCopy::W)
+		for (int j = 0; j < 8; j++)
+			if (e->qt.book[256 * j + 15] != 0xFFFFFFFFu)
+				return fail(e, APO_E_STATE, "coded dimension %d takes 16 or more distinct values: Form T (like Form P) needs <= 15", j < 2 ? j : j + 1);
+	if (cap > APO_TUPLES_MAX) cap = APO_TUPLES_MAX;
+	const uint32_t C = e->dims_C;
+	const uint64_t T = e->dims_T, N = (uint64_t)C * T;
+	const uint64_t m = std::min<uint64_t>(cap, N);                // at most this many dictionary entries
+	uint64_t slots = 1024;
+	while (slots < 2 * (m + 1)) slots <<= 1;
+	const uint64_t tpitch = R.tpitch = round_up(T ? T : 1, 64);    // as apo_tuples_upload
+	// everything is allocated before the source is chosen: reserve may release the copy this build reads
+	int rc;
+	if ((rc = tb_reserve(e, D.l, (uint64_t)C * tpitch, "Form T low plane", copy)) || (rc = tb_reserve(e, D.h, (uint64_t)C * tpitch, "Form T high plane", copy)) ||
+	    (rc = tb_reserve(e, D.pc, m ? m : 1, "dictionary", copy)) || (rc = tb_reserve(e, D.pd, m ? m : 1, "dictionary", copy)) ||
+	    (rc = tb_reserve(e, D.d2, 4096, "d2book", copy)) || (rc = tb_reserve(e, e->tb_table, 2 * slots, "hash table", copy)) ||
+	    (rc = tb_reserve(e, e->tb_keys, m ? m : 1, "keys", copy)) || (rc = tb_reserve(e, e->tb_cnt, m ? m : 1, "counts", copy)) ||
+	    (rc = tb_reserve(e, e->tb_misc, 4, "counters", copy)))
+		return rc;
+	if (!e->compact && e->copy.kind == DimsCopy::NONE)
+		return fail(e, APO_E_NOMEM, "device memory ran short: the Form W / Q copy of the loaded tensor was released to make room for the build; "
+		                            "free device memory and load the tensor again, or call apo_dims_compact");
+	apo::TbSource &S = R.S;
+	if (e->copy.kind == DimsCopy::W) S.qw = e->copy.qw.p;
+	else { S.q8 = e->q8.p; S.d2 = e->qd2.p; S.li = e->qli.p; }
+	S.pitch = e->dims_pitch; S.C = C; S.T = T;
+	unsigned long long *misc = e->tb_misc.p;                       // [0] keys inserted, [1] over flag / index miss, [2] compacted
+	CK(cudaMemsetAsync(misc, 0, 4 * 8, e->stream));
+	uint32_t n = 0;
+	std::vector<unsigned long long> keys, counts;
+	if (N) {
+		CK(apo::run_tb_clear(e->tb_table.p, slots, e->stream));
+		CK(apo::run_tb_count(S, e->tb_table.p, slots, cap, misc, (uint32_t *)(misc + 1), e->sm_count, e->stream));
+		unsigned long long h[2];
+		CK(cudaMemcpyAsync(h, misc, sizeof h, cudaMemcpyDeviceToHost, e->stream));
+		CK(cudaStreamSynchronize(e->stream));
+		if (h[1]) {
+			if (n_tuples) *n_tuples = h[0] > 0xFFFFFFFFull ? 0xFFFFFFFFu : (uint32_t)h[0];
+			return fail(e, APO_E_STATE, "the evaluations hold more than cap=%u distinct ones (at least %llu): keep Form W / Q", cap, h[0]);
+		}
+		n = (uint32_t)h[0];
+		CK(apo::run_tb_compact(e->tb_table.p, slots, e->tb_keys.p, e->tb_cnt.p, misc + 2, e->stream));
+		keys.resize(n); counts.resize(n);
+		CK(cudaMemcpyAsync(keys.data(), e->tb_keys.p, (uint64_t)n * 8, cudaMemcpyDeviceToHost, e->stream));
+		CK(cudaMemcpyAsync(counts.data(), e->tb_cnt.p, (uint64_t)n * 8, cudaMemcpyDeviceToHost, e->stream));
+		CK(cudaStreamSynchronize(e->stream));
+	}
+	// d2book: the distinct tool_success_rate values in ensure_d2book's order; a key's high half becomes its index
+	std::vector<uint32_t> d2;
+	for (uint32_t i = 0; i < n; i++) if ((uint32_t)(keys[i] >> 32) != apo::KW_D2_ABSENT) d2.push_back((uint32_t)(keys[i] >> 32));
+	std::sort(d2.begin(), d2.end());
+	d2.erase(std::unique(d2.begin(), d2.end()), d2.end());
+	if (d2.size() > 4095) return fail(e, APO_E_STATE, "tool_success_rate takes %zu distinct values: more than the 4095 Form T can index", d2.size());
+	std::sort(d2.begin(), d2.end(), d2_before);
+	for (size_t c = 0; c < 4096; c++) R.d2book[c] = c < d2.size() ? d2[c] : 0xFFFFFFFFu;
+	// dictionary order: count desc, then tuple_key (code word | d2book index << 32) asc, as apo_tuple_encode_host
+	R.order.resize(n);
+	for (uint32_t i = 0; i < n; i++) {
+		const uint32_t hi = (uint32_t)(keys[i] >> 32);
+		const uint64_t pd = hi == apo::KW_D2_ABSENT ? 4095u : (uint64_t)(std::lower_bound(d2.begin(), d2.end(), hi, d2_before) - d2.begin());
+		R.order[i] = {counts[i], (keys[i] & 0xFFFFFFFFull) | (pd << 32)};
+	}
+	std::sort(R.order.begin(), R.order.end(), [](const std::pair<unsigned long long, unsigned long long> &x, const std::pair<unsigned long long, unsigned long long> &y) {
+		if (x.first != y.first) return x.first > y.first;
+		return x.second < y.second;
+	});
+	return APO_OK;
+}
+
+// Then the index pass: D's dictionary and d2book from the ranking, its index planes, its codebook
+int tuples_index(apo_engine *e, const TbRanked &R, TupleTensor &D) {
+	const uint32_t n = (uint32_t)R.order.size();
+	std::vector<uint32_t> tb_pc(n);
+	std::vector<uint16_t> tb_pd(n);
+	std::vector<unsigned long long> keys(n);
+	for (uint32_t r = 0; r < n; r++) {
+		const uint32_t pd = (uint32_t)(R.order[r].second >> 32);
+		tb_pc[r] = (uint32_t)R.order[r].second; tb_pd[r] = (uint16_t)pd;
+		keys[r] = (unsigned long long)tb_pc[r] | ((unsigned long long)(pd == 4095u ? apo::KW_D2_ABSENT : R.d2book[pd]) << 32);   // back to the evaluation key
+	}
+	CK(cudaMemcpyAsync(D.d2.p, R.d2book, sizeof R.d2book, cudaMemcpyHostToDevice, e->stream));
+	if (n) {
+		CK(cudaMemcpyAsync(D.pc.p, tb_pc.data(), (uint64_t)n * 4, cudaMemcpyHostToDevice, e->stream));
+		CK(cudaMemcpyAsync(D.pd.p, tb_pd.data(), (uint64_t)n * 2, cudaMemcpyHostToDevice, e->stream));
+		CK(cudaMemcpyAsync(e->tb_keys.p, keys.data(), (uint64_t)n * 8, cudaMemcpyHostToDevice, e->stream));
+		// the index table holds only the dictionary (slots >= 2 n, so that it stays small enough for L2)
+		uint64_t islots = 1024;
+		while (islots < 2ull * n) islots <<= 1;
+		CK(apo::run_tb_clear(e->tb_table.p, islots, e->stream));
+		CK(apo::run_tb_insert(e->tb_keys.p, n, e->tb_table.p, islots, e->stream));
+		CK(apo::run_tb_index(R.S, e->tb_keys.p, n, e->tb_table.p, islots, D.l.p, D.h.p, R.tpitch, (uint32_t *)(e->tb_misc.p + 1), e->sm_count, e->stream));
+	}
+	unsigned long long miss = 0;
+	CK(cudaMemcpyAsync(&miss, e->tb_misc.p + 1, 8, cudaMemcpyDeviceToHost, e->stream));
+	CK(cudaStreamSynchronize(e->stream));
+	if (miss) return fail(e, APO_E_CUDA, "internal error: an evaluation's key is missing from the dictionary");
+	memcpy(D.book, e->qt.book, sizeof D.book);
+	D.C = R.S.C; D.T = R.S.T; D.pitch = R.tpitch; D.n = n;
+	return APO_OK;
+}
+
+// ---- the copies of the engine's fp32 Form D tensor (DimsCopy): built at its load, read instead of it, released as one:
+// the Form T copy and, unless keep_wq, the Form W / Q copy
+void release_copies(apo_engine *e, bool keep_wq) {
+	TupleCopy &t = e->copy.t;
+	HeldVals &v = t.vals;
+	t.release();                                                   // index planes and dictionary
+	v.ptab.release(); v.val[0].release(); v.val[1].release(); v.sval[0].release(); v.sval[1].release(); v.bad.release();
+	v.ok[0] = v.ok[1] = 0; v.slot_h = v.slot_end = 0;
+	t.xs.release(); t.xb.release(); t.s.release(); t.ys.release(); t.yb.release(); t.hp.release(); t.ho.release();
+	t.xn = t.yn = t.hn = 0; t.nblk = 0; t.t2 = false;
+	if (keep_wq || e->copy.kind == DimsCopy::NONE) return;
+	e->q8.release(); e->qd2.release(); e->qli.release(); e->copy.qw.release();
+	e->copy.kind = DimsCopy::NONE;
+}
+
+// After apo_dims_upload / apo_dims_generate: the Form Q (or Form W, below) copy of the engine's fp32 tensor, which resident
+// Form D calls read through K1q (route_copy) at 14 (8) instead of 36 bytes per evaluation.  Built when the evaluations are categorical and at least
+// kTwinHeadroom of device memory stays free beside it; otherwise Form D is kept alone, without an error.
+constexpr uint64_t kTwinHeadroom = 4ull << 30;
+int build_twin_qw(apo_engine *e) {
+	const uint32_t C = e->dims_C;
+	const uint64_t T = e->dims_T, pitch = e->dims_pitch, n = (uint64_t)C * pitch;
+	if ((e->tune & APO_TUNE_NO_TWIN) || C == 0 || T == 0) return APO_OK;
+	size_t free_bytes = 0, total_bytes = 0;
+	CK(cudaMemGetInfo(&free_bytes, &total_bytes));
+	if ((uint64_t)free_bytes < n * 14 + kTwinHeadroom) return APO_OK;
+	if (e->q8.reserve(n) != cudaSuccess || e->qd2.reserve(n) != cudaSuccess || e->qli.reserve(n) != cudaSuccess) {
+		cudaGetLastError();                                 // another user of the device took the room since cudaMemGetInfo
+		e->q8.release(); e->qd2.release(); e->qli.release();
+		return APO_OK;
+	}
+	int rc = compact_begin(e, C, pitch);
+	if (rc) return rc;
+	CK(apo::run_transcode(e->dims_ptr, pitch, C, T, e->q8.p, e->qd2.p, pitch, e->qbook.p, e->qbook.p + 8 * 256, e->stream));
+	rc = compact_finish(e, C, T, pitch, true);
+	if (rc != APO_OK) return rc == APO_E_STATE ? APO_OK : rc;
+	// A copy whose coded dimensions take at most 15 values each (dense codes 0-14, so 15 can mean absent; true for every tensor
+	// TCS:668-763 produces) is kept as Form W words instead: 8 instead of 14 bytes per evaluation.  They are packed from the
+	// planes, so the build peaks at the fp32 tensor + the planes + the words; without kTwinHeadroom beside that, Form Q stays.
+	for (int j = 0; j < 8; j++)
+		if (e->qt.book[256 * j + 15] != 0xFFFFFFFFu) return APO_OK;
+	CK(cudaMemGetInfo(&free_bytes, &total_bytes));
+	if ((uint64_t)free_bytes < n * 8 + kTwinHeadroom) return APO_OK;
+	if (e->copy.qw.reserve(n) != cudaSuccess) { cudaGetLastError(); return APO_OK; }
+	CK(apo::run_pack_w(e->q8.p, e->qd2.p, e->qli.p, n, e->copy.qw.p, e->stream));
+	CK(cudaStreamSynchronize(e->stream));
+	e->q8.release(); e->qd2.release(); e->qli.release();
+	e->copy.kind = DimsCopy::W;
+	return APO_OK;
+}
+
+// the Form T copy's values for the weights and `recip` into buffers build_twin_t allocated; waits, and records ok[recip]
+int held_values(apo_engine *e, TupleCopy &t, bool recip) {
+	HeldVals &v = t.vals;
+	if (const int rc = launch_tuple_values(e, t, v.ptab.p, v.val[recip].p, v.bad.p, recip, true)) return rc;
+	if (t.t2) CK(apo::run_tuple_slots(v.val[recip].p, v.slot_h, v.slot_end, v.sval[recip].p, e->stream));
+	uint32_t bad = 0;
+	CK(cudaMemcpyAsync(&bad, v.bad.p, 4, cudaMemcpyDeviceToHost, e->stream));
+	CK(cudaStreamSynchronize(e->stream));
+	v.ok[recip] = bad ? 2 : 1;
+	return APO_OK;
+}
+
+// The Form T copy of a freshly loaded Form D tensor that holds a Form W / Q copy with <= 15 values per coded dimension: its
+// resident Form D calls then read 3 B per evaluation through K1t (route_copy).  Built when the tensor holds at least
+// kTwinTMinEvals evaluations (APO_TUNE_TWIN_T: any size), at most kTwinTCap distinct ones (the build's scratch is sized
+// from it; the table stays well inside L2), the KT_HOT_MAX most frequent of them cover at least 3/4 of the evaluations (K1t
+// serves those from shared memory and gathers the rest from L2: on an H100 it beats K1q on Form W with 75 % of its reads in
+// the head and loses by 2x with 9 %, DESIGN §8), and kTwinHeadroom of device memory stays free beside the copy and the
+// build's scratch; otherwise no copy is kept, without an error.  The build also computes the table values for the weights.
+constexpr uint64_t kTwinTMinEvals = 1ull << 26;
+constexpr uint32_t kTwinTCap = 1u << 20;
+
+// The exception list of the Form T copy: with it resident Form D calls read 2 B per evaluation through K1t2 instead of 3 B
+// through K1t (route_copy).  Built from n_high, the evaluations whose index is >= 2^16 (known from the dictionary's
+// counts), when at most 1/kTwinT2Share of the evaluations are such exceptions (DESIGN §8: K1t2 corrects each one after its
+// stream) and a row's positions fit 32 bits; otherwise, or without room for it, the copy is read through K1t as before,
+// without an error.  APO_TUNE_NO_TWIN_T2 at the load builds none.
+// K1t2 reads the slot plane `s` (apo_kernels.h): the KT_SLOT_H most frequent entries get one copy per shared-memory bank pair,
+// fewer (down to none) when the evaluations of the entries left without a slot would exceed 1/kTwinT2Share of them; those
+// evaluations make the second list.  Slot plane, slot-order tables and that list need room too, or K1t serves the copy.
+constexpr uint64_t kTwinT2Share = 64;
+int build_twin_t2(apo_engine *e, uint64_t n_high, const std::vector<uint64_t> &counts16) {
+	TupleCopy &t = e->copy.t;
+	const uint32_t C = t.C;
+	const uint64_t T = t.T, N = (uint64_t)C * T;
+	if ((e->tune & APO_TUNE_NO_TWIN_T2) || n_high * kTwinT2Share > N || T > 0xFFFFFFFFull || n_high > 0xFFFFFFFFull) return APO_OK;
+	const uint32_t nblk = (uint32_t)((T + apo::KT_XBLOCK - 1) / apo::KT_XBLOCK);
+	t.nblk = nblk;
+	if (n_high) {
+		if (t.xb.reserve((uint64_t)C * (nblk + 1)) != cudaSuccess || t.xs.reserve(n_high) != cudaSuccess) {
+			cudaGetLastError();
+			t.xb.release(); t.xs.release();
+			return APO_OK;
+		}
+		CK(apo::run_tx_build(t.l.p, t.h.p, t.pitch, C, T, 65536u, t.xb.p, t.xs.p, e->sm_count, e->stream));
+		t.xn = n_high;
+	}
+	uint32_t h = std::min<uint32_t>(apo::KT_SLOT_H, t.n), end = 0;
+	uint64_t ny = 0;
+	for (;; h /= 2) {
+		end = apo::kt_slot_end(t.n, h);
+		ny = 0;
+		for (size_t r = end; r < counts16.size(); r++) ny += counts16[r];
+		if (ny * kTwinT2Share <= N || h == 0) break;
+	}
+	HeldVals &v = t.vals;
+	v.slot_h = h; v.slot_end = end;                                 // read only once the slot plane is held (t2)
+	if (t.s.reserve((uint64_t)C * t.pitch) != cudaSuccess || v.sval[0].reserve(v.n_slots()) != cudaSuccess || v.sval[1].reserve(v.n_slots()) != cudaSuccess ||
+	    (ny && (t.yb.reserve((uint64_t)C * (nblk + 1)) != cudaSuccess || t.ys.reserve(ny) != cudaSuccess))) {
+		cudaGetLastError();
+		t.s.release(); v.sval[0].release(); v.sval[1].release(); t.ys.release(); t.yb.release();
+		CK(cudaStreamSynchronize(e->stream));
+		return APO_OK;                                            // the exception list alone: K1t reads the copy
+	}
+	CK(apo::run_slot_plane(t.l.p, t.h.p, t.pitch, C, T, h, end, t.s.p, e->stream));
+	if (ny) CK(apo::run_tx_build(t.l.p, t.h.p, t.pitch, C, T, end, t.yb.p, t.ys.p, e->sm_count, e->stream));
+	for (int r = 0; r < 2; r++)                                     // the values computed so far (build_twin_t: recip = 0)
+		if (v.ok[r]) CK(apo::run_tuple_slots(v.val[r].p, h, end, v.sval[r].p, e->stream));
+	CK(cudaStreamSynchronize(e->stream));                         // the load returns with the lists built, as with the copy
+	t.yn = ny;
+	t.t2 = true;
+	return APO_OK;
+}
+
+// The per-row dictionary counts of the Form T copy (apo_kernels.h KhParams): with them a call over whole rows reads 8 B per
+// distinct (row, entry) pair through K1h instead of 2 B per evaluation through K1t2 (route_copy).  The rows are counted in
+// batches whose dense [rows][entries] scratch stays within kTwinHScratch: a first sweep gives the exact number of pairs, and the
+// counts are kept when they take at most a quarter of K1t2's slot plane (8 nnz <= C T / 2) and kTwinHeadroom stays free beside
+// them; a second sweep writes them (a single batch keeps its counts from the first).  Otherwise, or without room, none are
+// held, without an error.  The scratch is freed before this returns.  APO_TUNE_NO_TWIN_H at the load builds none.
+constexpr uint64_t kTwinHScratch = 256ull << 20;
+int build_twin_h(apo_engine *e) {
+	TupleCopy &t = e->copy.t;
+	const uint32_t C = t.C;
+	const uint64_t T = t.T;
+	if ((e->tune & APO_TUNE_NO_TWIN_H) || C == 0 || T == 0 || T > 0xFFFFFFFFull || t.n == 0 || t.n > (1u << apo::KH_COUNT_SHIFT)) return APO_OK;
+	const uint32_t npitch = (uint32_t)round_up(t.n, 32), nchunk = (npitch + 8191) / 8192;
+	const uint32_t R = (uint32_t)std::min<uint64_t>(C, std::max<uint64_t>(1, kTwinHScratch / (4ull * npitch)));
+	const uint32_t nb = (C + R - 1) / R;
+	struct Scoped : DevBuf<uint32_t> { ~Scoped() { release(); } } cnt, nz;   // freed on every return path
+	if (cnt.reserve((uint64_t)R * npitch) != cudaSuccess || nz.reserve((uint64_t)R * nchunk + 1) != cudaSuccess) { cudaGetLastError(); return APO_OK; }
+	auto count = [&](uint32_t b) -> cudaError_t {
+		const uint32_t c0 = b * R, r = std::min(R, C - c0);
+		cudaError_t c = cudaMemsetAsync(cnt.p, 0, (uint64_t)r * npitch * 4, e->stream);
+		return c != cudaSuccess ? c : apo::run_th_count(t.l.p + (uint64_t)c0 * t.pitch, t.h.p + (uint64_t)c0 * t.pitch, t.pitch, r, T, npitch, cnt.p, nz.p, e->sm_count, e->stream);
+	};
+	std::vector<uint64_t> total(nb);
+	uint64_t nnz = 0;
+	for (uint32_t b = 0; b < nb; b++) {
+		CK(count(b));
+		uint32_t n = 0;
+		CK(cudaMemcpyAsync(&n, nz.p + (uint64_t)std::min(R, C - b * R) * nchunk, 4, cudaMemcpyDeviceToHost, e->stream));
+		CK(cudaStreamSynchronize(e->stream));
+		total[b] = n; nnz += n;
+	}
+	size_t free_bytes = 0, total_bytes = 0;
+	CK(cudaMemGetInfo(&free_bytes, &total_bytes));
+	if (nnz * 8 > (uint64_t)C * T / 2 || (uint64_t)free_bytes < nnz * 8 + 8ull * (C + 1) + kTwinHeadroom) return APO_OK;
+	if (t.hp.reserve(nnz) != cudaSuccess || t.ho.reserve(C + 1ull) != cudaSuccess) {
+		cudaGetLastError();
+		t.hp.release(); t.ho.release();
+		return APO_OK;
+	}
+	uint64_t base = 0;
+	for (uint32_t b = 0; b < nb; b++) {
+		if (nb > 1) CK(count(b));
+		CK(apo::run_th_write(cnt.p, std::min(R, C - b * R), npitch, nz.p, base, t.hp.p, t.ho.p + (uint64_t)b * R, e->sm_count, e->stream));
+		base += total[b];
+	}
+	CK(cudaStreamSynchronize(e->stream));                         // the load returns with the counts built, as with the copy
+	t.hn = nnz;
+	return APO_OK;
+}
+
+int build_twin_t(apo_engine *e) {
+	const uint32_t C = e->dims_C;
+	const uint64_t T = e->dims_T, N = (uint64_t)C * T;
+	if ((e->tune & APO_TUNE_NO_TWIN_T) || !(N >= kTwinTMinEvals || (e->tune & APO_TUNE_TWIN_T))) return APO_OK;
+	if (e->copy.kind != DimsCopy::W)
+		for (int j = 0; j < 8; j++)
+			if (e->qt.book[256 * j + 15] != 0xFFFFFFFFu) return APO_OK;
+	const uint64_t m = std::min<uint64_t>(kTwinTCap, N);
+	uint64_t slots = 1024;
+	while (slots < 2 * (m + 1)) slots <<= 1;
+	// index planes, dictionary, value tables, the largest exception list and its block index; the slot plane, the slot-order
+	// tables and the second list; the build's hash table, keys and counts
+	const uint64_t need = 3 * (uint64_t)C * round_up(T, 64) + m * 6 + 2 * (m + 1) * 8 + 8 * (N / kTwinT2Share) +
+	                      4 * (uint64_t)C * (T / apo::KT_XBLOCK + 2) + 2 * (uint64_t)C * round_up(T, 64) + 2 * 65536 * 8 +
+	                      8 * (N / kTwinT2Share) + 4 * (uint64_t)C * (T / apo::KT_XBLOCK + 2) + 16 * slots + 16 * m;
+	size_t free_bytes = 0, total_bytes = 0;
+	CK(cudaMemGetInfo(&free_bytes, &total_bytes));
+	if ((uint64_t)free_bytes < need + kTwinHeadroom) return APO_OK;
+	const std::string keep_err = e->err;
+	TupleCopy &t = e->copy.t;
+	TbRanked R;
+	int rc = tuples_rank(e, kTwinTCap, nullptr, t, true, R);
+	// the copy's rules on the ranked counts: head (of the KT_HOT_MAX most frequent), n_high (index >= 2^16), counts16 (each below)
+	uint64_t head = 0, n_high = 0;
+	std::vector<uint64_t> counts16;
+	for (size_t r = 0; rc == APO_OK && r < R.order.size(); r++) {
+		if (r < apo::KT_HOT_MAX) head += R.order[r].first;
+		if (r < 65536) counts16.push_back(R.order[r].first);
+		else n_high += R.order[r].first;
+	}
+	if (rc == APO_OK && head * 4 < N * 3) rc = APO_E_STATE;
+	if (rc == APO_OK) rc = tuples_index(e, R, t);
+	if (rc == APO_OK && (t.vals.val[0].reserve(t.n + 1ull) != cudaSuccess || t.vals.val[1].reserve(t.n + 1ull) != cudaSuccess ||
+	                     t.vals.ptab.reserve(8 * 256) != cudaSuccess || t.vals.bad.reserve(1) != cudaSuccess)) {
+		cudaGetLastError();
+		rc = APO_E_NOMEM;
+	}
+	if (rc == APO_OK) rc = held_values(e, t, false);
+	if (rc == APO_OK) rc = build_twin_t2(e, n_high, counts16);
+	if (rc == APO_OK) rc = build_twin_h(e);
+	tb_release(e, rc);
+	if (rc == APO_OK) return APO_OK;
+	release_copies(e, true);
+	if (rc != APO_E_STATE && rc != APO_E_NOMEM) return rc;
+	e->err = keep_err;                                          // more than kTwinTCap distinct evaluations, or no room: no copy
+	return APO_OK;
+}
+
+// the copies of the engine's freshly loaded fp32 tensor: Form W / Q, then (large tensors) Form T beside it
+int build_twin(apo_engine *e) {
+	const int rc = build_twin_qw(e);
+	return rc == APO_OK && e->copy.kind != DimsCopy::NONE ? build_twin_t(e) : rc;
+}
+
+// A resident Form D call reads a copy instead when one is held, the variant is the default (1-4 name K1 tile shapes) and the
+// window starts on K1q's 8-evaluation grid: the Form T copy when its values for the call's weights and `recip` (computed here by
+// the first call that needs them) are valid, else the Form Q / W copy.  After the call's last allocation before its launches.
+int route_copy(apo_engine *e, const apo_score_opts *o, Evals *ev) {
+	const bool recip = (o->flags & APO_SCORE_RECIP) != 0;
+	TupleCopy &t = e->copy.t;
+	const bool use_t = ev->form == apo::CAND_DIMS && t.C && !(e->tune & APO_TUNE_NO_TWIN_T);
+	int rc;
+	if (use_t && !t.vals.ok[recip] && (rc = held_values(e, t, recip))) return rc;
+	if (ev->form != apo::CAND_DIMS || e->copy.kind == DimsCopy::NONE || (e->tune & APO_TUNE_NO_TWIN) || o->variant != 0 || o->first % 8) return APO_OK;
+	ev->rows = nullptr;
+	if (use_t && t.vals.ok[recip] == 1) {
+		resident_tuples(ev, t);
+		ev->copy = &t; ev->variant = 0;
+		if (!(e->tune & APO_TUNE_NO_TWIN_H) && t.hn && o->first == 0 && (o->count == 0 || o->count == t.T)) ev->read = Evals::K1h;
+		else if (t.t2 && !(e->tune & APO_TUNE_NO_TWIN_T2)) ev->read = Evals::K1t2;
+		return APO_OK;
+	}
+	ev->qt = &e->qt;
+	if (e->copy.kind == DimsCopy::W) {                       // <= 15 codes per dimension: the prefix table always fits
+		ev->form = apo::CAND_W; ev->qw = e->copy.qw.p; ev->variant = 0;
+		return APO_OK;
+	}
+	ev->form = apo::CAND_Q;
+	ev->q8 = e->q8.p; ev->d2 = e->qd2.p; ev->li = e->qli.p;
+	ev->variant = e->qt.pair_ok ? 0 : 4;                     // as resident_evals for a compact tensor
+	return APO_OK;
+}
+
+// new weights (rc: the upload of their tables): K1q's tables of the compact tensor or the Form Q / W copy, the Form T copy's values
+int reweigh_copies(apo_engine *e, int rc) {
+	if (rc == APO_OK && (e->compact || e->copy.kind != DimsCopy::NONE)) rc = load_qtables(e, e->qt, e->qt.book);
+	e->copy.t.vals.ok[0] = e->copy.t.vals.ok[1] = 0;         // the Form T copy's values belonged to the old weights
+	return rc == APO_OK && e->copy.t.C ? held_values(e, e->copy.t, false) : rc;
+}
+
 struct PeerInfo {                        // exchanged with ncclAllGather at apo_comm_init, 128 bytes per rank
 	cudaIpcMemHandle_t handle;           // 64 B
 	uint64_t pid, ptr, host_hash;
@@ -1249,15 +1555,7 @@ extern "C" int apo_create(int device, apo_engine **out) {
 		if (sm_khz > 0) e->scan_ms_per_record = 1.0 / (kScanRecordsPerSmCycle * (double)e->sm_count * (double)sm_khz);
 	}
 	// experiment / test switches: the environment gives the initial value once per handle (never read per call), apo_set_tuning changes them
-	e->env_no_fuse = getenv("APO_NO_FUSE") != nullptr;
-	e->env_force_fuse = getenv("APO_FORCE_FUSE") != nullptr;
-	e->env_no_staging = getenv("APO_NO_STAGING") != nullptr;
-	e->env_nccl_join = getenv("APO_JOIN_NCCL") != nullptr;
-	e->env_no_twin = getenv("APO_NO_TWIN") != nullptr;
-	e->env_no_twin_t = getenv("APO_NO_TWIN_T") != nullptr;
-	e->env_twin_t = getenv("APO_TWIN_T") != nullptr;
-	e->env_no_twin_t2 = getenv("APO_NO_TWIN_T2") != nullptr;
-	e->env_no_twin_h = getenv("APO_NO_TWIN_H") != nullptr;
+	for (const auto &t : kTuning) if (getenv(t.env)) e->tune |= t.bit;
 	if ((c =cudaStreamCreateWithFlags(&e->own_stream, cudaStreamNonBlocking)) != cudaSuccess) return bail("cudaStreamCreate", c);
 	if ((c = cudaStreamCreateWithFlags(&e->copy_stream, cudaStreamNonBlocking)) != cudaSuccess) return bail("cudaStreamCreate", c);
 	e->stream = e->own_stream;
@@ -1283,12 +1581,13 @@ extern "C" void apo_destroy(apo_engine *e) {
 	peer_teardown(e);
 	if (e->comm && g_nccl.CommDestroy) g_nccl.CommDestroy(e->comm);
 	if (e->zc_host) cudaFreeHost(e->zc_host);
-	e->q8.release(); e->qd2.release(); e->qli.release(); e->qw.release(); e->qbook.release(); e->d_d2book.release(); e->d_d2stream.release(); e->unpack_bad.release(); e->stage.release();
+	release_copies(e);
+	e->q8.release(); e->qd2.release(); e->qli.release(); e->qbook.release(); e->d_d2book.release(); e->d_d2stream.release(); e->unpack_bad.release(); e->stage.release();
 	e->qt.release(); e->qt_stream.release();
 	e->d_lut.release(); e->corpus.release(); e->dims.release(); e->roll.release(); e->acc.release(); e->acc_joined.release(); e->acc_snapshot.release(); e->misc.release();
 	e->result.release(); e->keys.release(); e->sel_key.release(); e->sel_idx.release();
 	e->cand_acc.release(); e->cand_rep.release(); e->cand_book.release(); e->ccorp_acc.release(); e->ccorp_rep.release();
-	e->tup.release(); e->tups.release(); e->tvals.release(); e->tcopy.release();
+	e->tup.release(); e->tups.release(); e->tvals.release();
 	e->win[0].release(); e->win[1].release(); e->batch_in.release(); e->batch_out.release(); e->batch_mask.release();
 	if (e->h_result) cudaFreeHost(e->h_result);
 	if (e->h_domain) cudaFreeHost((void *)e->h_domain);
@@ -1311,15 +1610,10 @@ extern "C" int apo_set_stream(apo_engine *e, uint64_t cuda_stream) {
 
 extern "C" int apo_set_tuning(apo_engine *e, uint32_t flags) {
 	if (!e) return APO_E_ARG;
-	if (flags & ~(APO_TUNE_NO_FUSE | APO_TUNE_FORCE_FUSE | APO_TUNE_NO_STAGING | APO_TUNE_NCCL_JOIN | APO_TUNE_NO_TWIN | APO_TUNE_NO_TWIN_T | APO_TUNE_TWIN_T |
-	              APO_TUNE_NO_TWIN_T2 | APO_TUNE_NO_TWIN_H))
-		return fail(e, APO_E_ARG, "unknown tuning flag %#x", flags);
-	e->env_no_fuse = (flags & APO_TUNE_NO_FUSE) != 0; e->env_force_fuse = (flags & APO_TUNE_FORCE_FUSE) != 0;
-	e->env_no_staging = (flags & APO_TUNE_NO_STAGING) != 0; e->env_nccl_join = (flags & APO_TUNE_NCCL_JOIN) != 0;
-	e->env_no_twin = (flags & APO_TUNE_NO_TWIN) != 0;
-	e->env_no_twin_t = (flags & APO_TUNE_NO_TWIN_T) != 0; e->env_twin_t = (flags & APO_TUNE_TWIN_T) != 0;
-	e->env_no_twin_t2 = (flags & APO_TUNE_NO_TWIN_T2) != 0;
-	e->env_no_twin_h = (flags & APO_TUNE_NO_TWIN_H) != 0;
+	uint32_t known = 0;
+	for (const auto &t : kTuning) known |= t.bit;
+	if (flags & ~known) return fail(e, APO_E_ARG, "unknown tuning flag %#x", flags);
+	e->tune = flags;
 	return APO_OK;
 }
 
@@ -1332,11 +1626,7 @@ extern "C" int apo_set_weights(apo_engine *e, const double w[APO_NDIM]) {
 	memcpy(e->W.w, w, sizeof e->W.w);
 	e->weights_gen++;
 	build_luts(e);
-	int rc = upload_luts(e);
-	if (rc == APO_OK && (e->compact || e->twin)) rc = load_qtables(e, e->qt, e->qt.book);
-	e->tcopy.vals.ok[0] = e->tcopy.vals.ok[1] = 0;          // the Form T copy's values belonged to the old weights
-	if (rc == APO_OK && e->tcopy.C) rc = tuple_values(e, e->tcopy, e->tcopy.vals, false);
-	return rc;
+	return reweigh_copies(e, upload_luts(e));
 }
 
 extern "C" int apo_get_weights(const apo_engine *e, double w[APO_NDIM]) {
@@ -1443,7 +1733,7 @@ extern "C" int apo_dims_upload(apo_engine *e, const float *dims, uint32_t C, uin
 	if (!e) return APO_E_ARG;
 	if (C && T && !dims) return fail(e, APO_E_ARG, "dims is NULL");
 	CK(cudaSetDevice(e->device));
-	drop_twin(e);
+	release_copies(e);
 	const uint64_t pitch = round_up(T ? T : 1, 32);
 	CK(reserve(e, e->dims, (uint64_t)(C ? C : 1) * pitch * APO_NDIM));
 	if (C && T) {
@@ -1459,7 +1749,7 @@ extern "C" int apo_dims_upload(apo_engine *e, const float *dims, uint32_t C, uin
 extern "C" int apo_dims_generate(apo_engine *e, uint64_t seed, uint32_t c0, uint32_t C, uint64_t t0, uint64_t T, uint32_t agent_permille) {
 	if (!e) return APO_E_ARG;
 	CK(cudaSetDevice(e->device));
-	drop_twin(e);
+	release_copies(e);
 	const uint64_t pitch = round_up(T ? T : 1, 32);
 	CK(reserve(e, e->dims, (uint64_t)(C ? C : 1) * pitch * APO_NDIM));
 	if (pitch != T && C) CK(cudaMemsetAsync(e->dims.p, 0xFF, (uint64_t)C * pitch * APO_NDIM * 4, e->stream));
@@ -1490,7 +1780,7 @@ extern "C" int apo_dims_attach(apo_engine *e, uint64_t device_ptr, uint32_t C, u
 	if (!e) return APO_E_ARG;
 	if (!device_ptr || device_ptr % 16) return fail(e, APO_E_ARG, "device pointer must be non-NULL and 16-byte aligned");
 	if (pitch_evals % 4 || pitch_evals < round_up(T, 4)) return fail(e, APO_E_ARG, "pitch must be a multiple of 4 evaluations and >= T rounded up to 4");
-	drop_twin(e);                                       // never a copy of caller-owned memory: the caller may change it
+	release_copies(e);                                  // never a copy of caller-owned memory: the caller may change it
 	e->dims_ptr = (const float *)(uintptr_t)device_ptr; e->dims_C = C; e->dims_T = T; e->dims_pitch = pitch_evals; e->compact = false;
 	return APO_OK;
 }
@@ -1506,13 +1796,13 @@ extern "C" int apo_dims_compact(apo_engine *e) {
 	if (e->compact) return APO_OK;
 	if (!e->dims_ptr || e->dims_C == 0) return fail(e, APO_E_STATE, "no dims loaded");
 	CK(cudaSetDevice(e->device));
-	if (e->twin && !e->twin_w) {                        // the copy built at load already is this tensor in Form Q
-		e->tcopy.release();                             // a compact tensor keeps no Form T copy
-		e->twin = false; e->compact = true; e->dims_ptr = nullptr;
+	if (e->copy.kind == DimsCopy::Q) {                  // the copy built at load already is this tensor in Form Q
+		e->copy.kind = DimsCopy::NONE; e->compact = true; e->dims_ptr = nullptr;
+		release_copies(e);                              // the Form T copy: a compact tensor keeps none
 		e->dims.release();
 		return APO_OK;
 	}
-	drop_twin(e);                                       // a Form W copy is not a compact tensor: transcode the fp32 one
+	release_copies(e);                                  // a Form W copy is not a compact tensor: transcode the fp32 one
 	const uint32_t C = e->dims_C; const uint64_t T = e->dims_T, pitch_in = e->dims_pitch, pitch = round_up(T ? T : 1, 32);
 	int rc = compact_begin(e, C, pitch);
 	if (rc) return rc;
@@ -1528,7 +1818,7 @@ namespace {
 template <class Fill>
 int compact_stream(apo_engine *e, uint32_t C, uint64_t T, Fill fill) {
 	CK(cudaSetDevice(e->device));
-	drop_twin(e);
+	release_copies(e);
 	const uint64_t pitch = round_up(T ? T : 1, 32);
 	uint64_t Cc = (2ull << 30) / (pitch * 36);
 	if (Cc < 1) Cc = 1;
@@ -1656,10 +1946,9 @@ extern "C" int apo_score_accumulate(apo_engine *e, const apo_score_opts *o, uint
 	if (cand && (rc = cand_check(e))) return rc;
 	if (ccorp && (rc = ccorp_check(e, ev.records()))) return rc;
 	CK(cudaSetDevice(e->device));
-	if (cand && (rc = cand_reserve(e, e->score_C))) return rc;                                  // allocates: before route_twin
+	if (cand && (rc = cand_reserve(e, e->score_C))) return rc;                                  // allocates: before route_copy
 	if (cand && e->cand_every && !e->cand_armed && (rc = cand_arm(e, e->score_C))) return rc;
-	if ((rc = twin_t_ready(e, o))) return rc;
-	route_twin(e, o, &ev);
+	if ((rc = route_copy(e, o, &ev))) return rc;
 	if ((rc = resident_window(e, o, &ev)) || (rc = launch_score(e, o, ev, cand_offset))) return rc;
 	if (!ccorp) e->ccorp_every = false;
 	else if (e->ccorp_every) {                          // an earlier accumulate of the session did not set the flag: finish refuses
@@ -1694,8 +1983,7 @@ extern "C" int apo_score(apo_engine *e, const apo_score_opts *o, double *scores,
 	int rc = resident_evals(e, o, &ev);
 	if (rc) return rc;
 	const uint32_t C = ev.C;
-	if ((rc = score_check(e, o, C, ev.count, ev.records())) || (rc = twin_t_ready(e, o))) return rc;
-	route_twin(e, o, &ev);
+	if ((rc = score_check(e, o, C, ev.count, ev.records())) || (rc = route_copy(e, o, &ev))) return rc;
 	if ((rc = resident_window(e, o, &ev))) return rc;
 	const bool tup = ev.form == apo::CAND_T;            // gather-and-add kernel: stand-alone corpus scan + tail
 	const double stream_bytes = (double)C * (double)ev.count * ev.bytes();
@@ -1711,9 +1999,9 @@ extern "C" int apo_score(apo_engine *e, const apo_score_opts *o, double *scores,
 	const uint64_t tiles = (uint64_t)C * ((ev.count + ev.tile() - 1) / ev.tile());
 	const uint64_t ctas = tiles < (uint64_t)e->sm_count ? tiles : (uint64_t)e->sm_count;
 	const bool small_scan = e->corpus_T <= 16ull * 32ull * ctas;
-	const bool fuse = !tup && wants_corpus(e, o) && ev.count > 0 && !e->env_no_fuse && (k1_ms > 1.3 * scan_ms || small_scan || e->env_force_fuse);
+	const bool fuse = !tup && wants_corpus(e, o) && ev.count > 0 && !(e->tune & APO_TUNE_NO_FUSE) && (k1_ms > 1.3 * scan_ms || small_scan || (e->tune & APO_TUNE_FORCE_FUSE));
 	// without a corpus request the same tail still saves the K3 launch: an empty scan, then the last CTA finalises
-	const bool tail_only = !tup && !wants_corpus(e, o) && one_launch && ev.count > 0 && !e->env_no_fuse;
+	const bool tail_only = !tup && !wants_corpus(e, o) && one_launch && ev.count > 0 && !(e->tune & APO_TUNE_NO_FUSE);
 	const bool fused = fuse || tail_only;
 	if ((rc = score_arm(e, o, C, true, (uint64_t)stream_bytes, fused))) return rc;
 	apo::K2Params k2{};
@@ -1812,7 +2100,7 @@ int stream_host(apo_engine *e, const apo_score_opts *o, const HostTensor &h, dou
 	// pageable callers (malloc / ArrayBuffer / numpy) of the row formats: the driver would stage such copies through one small
 	// internal buffer on the calling thread; instead gather each chunk into pinned memory with a few host threads while the
 	// previous chunk is on the wire.  Pinned or registered callers (apo_host_alloc) are read in place.
-	const bool staged = rows && T > 0 && is_pageable(h.plane[0].p) && !e->env_no_staging;
+	const bool staged = rows && T > 0 && is_pageable(h.plane[0].p) && !(e->tune & APO_TUNE_NO_STAGING);
 	if (staged && (rc = ensure_stage(e, (uint64_t)C * Tc * wire))) return rc;
 	uint64_t code_ok[2] = {0, 0};      // Form P: bit 16 j + c set when code c of coded dimension j names a value (not empty, not NaN)
 	if (h.packed) {
@@ -1830,7 +2118,7 @@ int stream_host(apo_engine *e, const apo_score_opts *o, const HostTensor &h, dou
 	if (h.form == apo::CAND_T) {                                   // the dictionary and its values, once for the whole call
 		if (wants_cand(o) && (rc = cand_upload_tbook(e, h.codebook))) return rc;
 		if ((rc = dict_upload(e, e->tups, h.tb_pc, h.tb_pd, h.n_tuples, h.codebook, h.d2book))) return rc;
-		ev.dict = &e->tups; ev.tv = &e->tvals; ev.t_once = true;
+		ev.dict = &e->tups; ev.t_once = true;
 		if ((rc = tuple_values(e, e->tups, e->tvals, (o->flags & APO_SCORE_RECIP) != 0))) return rc;
 	}
 	const uint64_t CTc = (uint64_t)C * Tc;
@@ -1914,13 +2202,6 @@ extern "C" int apo_dims_compact_download(apo_engine *e, uint64_t *q8, float *d2,
 }
 
 namespace {
-// order of a d2book: by value, -0.0 (sign bit set) before +0.0
-bool d2_before(uint32_t x, uint32_t y) {
-	float fx, fy; memcpy(&fx, &x, 4); memcpy(&fy, &y, 4);
-	if (fx != fy) return fx < fy;
-	return x > y;
-}
-
 // d2book of the resident Form Q tensor: distinct tool_success_rate values ordered by value (built once per loaded tensor)
 int ensure_d2book(apo_engine *e) {
 	if (e->d2book_n != ~0u) return APO_OK;
@@ -2026,297 +2307,16 @@ extern "C" int apo_tuples_upload(apo_engine *e, const uint16_t *tl, const uint8_
 	return APO_OK;
 }
 
-namespace {
-constexpr uint32_t kTwinTHot = 24576;   // K1t's shared-memory head of the table (KT_HOT_MAX, csrc/apo_tuple.cu)
-
-template <class T>
-int tb_reserve(apo_engine *e, DevBuf<T> &b, uint64_t n, const char *what, bool copy = false) {
-	const cudaError_t c = copy ? b.reserve(n) : reserve(e, b, n);
-	if (c == cudaSuccess) return APO_OK;
-	cudaGetLastError();
-	return fail(e, c == cudaErrorMemoryAllocation ? APO_E_NOMEM : APO_E_CUDA, "%s (%llu elements): %s", what, (unsigned long long)n, cudaGetErrorString(c));
-}
-
-void tb_release(apo_engine *e, int rc) {
-	if (rc != APO_OK) cudaStreamSynchronize(e->stream);          // nothing a failed build queued may still use what is released
-	e->tb_table.release(); e->tb_keys.release(); e->tb_cnt.release(); e->tb_misc.release();
-}
-
-// Form T of the loaded evaluations into D: the engine's resident Form T (apo_dims_tuples), or the Form T copy of its Form D
-// tensor (copy, build_twin_t; *n_high: the evaluations whose index is >= 2^16, *counts: those of the entries below 2^16).  The
-// copy's buffers do not go through reserve: releasing the copies to make room would release the one being built.
-int dims_tuples(apo_engine *e, uint32_t cap, uint32_t *n_tuples, TupleTensor &D, bool copy, uint64_t *n_high = nullptr,
-                std::vector<uint64_t> *counts16 = nullptr) {
-	if ((!e->dims_ptr && !e->compact) || e->dims_C == 0) return fail(e, APO_E_STATE, "no dims loaded");
-	if (!e->compact && (!e->twin || e->env_no_twin))
-		return fail(e, APO_E_STATE, "the loaded Form D tensor has no Form W / Q copy to build Form T from (APO_TUNE_NO_TWIN, apo_dims_attach, "
-		                            "or too little device memory at load): call apo_dims_compact first");
-	if (e->compact || !e->twin_w)
-		for (int j = 0; j < 8; j++)
-			if (e->qt.book[256 * j + 15] != 0xFFFFFFFFu)
-				return fail(e, APO_E_STATE, "coded dimension %d takes 16 or more distinct values: Form T (like Form P) needs <= 15", j < 2 ? j : j + 1);
-	if (cap > APO_TUPLES_MAX) cap = APO_TUPLES_MAX;
-	const uint32_t C = e->dims_C;
-	const uint64_t T = e->dims_T, pitch = e->dims_pitch, N = (uint64_t)C * T;
-	const uint64_t m = std::min<uint64_t>(cap, N);                // at most this many dictionary entries
-	uint64_t slots = 1024;
-	while (slots < 2 * (m + 1)) slots <<= 1;
-	const uint64_t tpitch = round_up(T ? T : 1, 64);               // as apo_tuples_upload
-	// everything is allocated before the source is chosen: reserve may release the copy this build reads
-	int rc;
-	if ((rc = tb_reserve(e, D.l, (uint64_t)C * tpitch, "Form T low plane", copy)) || (rc = tb_reserve(e, D.h, (uint64_t)C * tpitch, "Form T high plane", copy)) ||
-	    (rc = tb_reserve(e, D.pc, m ? m : 1, "dictionary", copy)) || (rc = tb_reserve(e, D.pd, m ? m : 1, "dictionary", copy)) ||
-	    (rc = tb_reserve(e, D.d2, 4096, "d2book", copy)) || (rc = tb_reserve(e, e->tb_table, 2 * slots, "hash table", copy)) ||
-	    (rc = tb_reserve(e, e->tb_keys, m ? m : 1, "keys", copy)) || (rc = tb_reserve(e, e->tb_cnt, m ? m : 1, "counts", copy)) ||
-	    (rc = tb_reserve(e, e->tb_misc, 4, "counters", copy)))
-		return rc;
-	if (!e->compact && !e->twin)
-		return fail(e, APO_E_NOMEM, "device memory ran short: the Form W / Q copy of the loaded tensor was released to make room for the build; "
-		                            "free device memory and load the tensor again, or call apo_dims_compact");
-	apo::TbSource S{};
-	if (e->twin_w && !e->compact) S.qw = e->qw.p;
-	else { S.q8 = e->q8.p; S.d2 = e->qd2.p; S.li = e->qli.p; }
-	S.pitch = pitch; S.C = C; S.T = T;
-	unsigned long long *misc = e->tb_misc.p;                       // [0] keys inserted, [1] over flag / index miss, [2] compacted
-	CK(cudaMemsetAsync(misc, 0, 4 * 8, e->stream));
-	uint32_t n = 0;
-	std::vector<unsigned long long> keys, counts;
-	if (N) {
-		CK(apo::run_tb_clear(e->tb_table.p, slots, e->stream));
-		CK(apo::run_tb_count(S, e->tb_table.p, slots, cap, misc, (uint32_t *)(misc + 1), e->sm_count, e->stream));
-		unsigned long long h[2];
-		CK(cudaMemcpyAsync(h, misc, sizeof h, cudaMemcpyDeviceToHost, e->stream));
-		CK(cudaStreamSynchronize(e->stream));
-		if (h[1]) {
-			*n_tuples = h[0] > 0xFFFFFFFFull ? 0xFFFFFFFFu : (uint32_t)h[0];
-			return fail(e, APO_E_STATE, "the evaluations hold more than cap=%u distinct ones (at least %llu): keep Form W / Q", cap, h[0]);
-		}
-		n = (uint32_t)h[0];
-		CK(apo::run_tb_compact(e->tb_table.p, slots, e->tb_keys.p, e->tb_cnt.p, misc + 2, e->stream));
-		keys.resize(n); counts.resize(n);
-		CK(cudaMemcpyAsync(keys.data(), e->tb_keys.p, (uint64_t)n * 8, cudaMemcpyDeviceToHost, e->stream));
-		CK(cudaMemcpyAsync(counts.data(), e->tb_cnt.p, (uint64_t)n * 8, cudaMemcpyDeviceToHost, e->stream));
-		CK(cudaStreamSynchronize(e->stream));
-	}
-	// d2book: the distinct tool_success_rate values in ensure_d2book's order; a key's high half becomes its index
-	std::vector<uint32_t> d2;
-	for (uint32_t i = 0; i < n; i++) if ((uint32_t)(keys[i] >> 32) != apo::KW_D2_ABSENT) d2.push_back((uint32_t)(keys[i] >> 32));
-	std::sort(d2.begin(), d2.end());
-	d2.erase(std::unique(d2.begin(), d2.end()), d2.end());
-	if (d2.size() > 4095) return fail(e, APO_E_STATE, "tool_success_rate takes %zu distinct values: more than the 4095 Form T can index", d2.size());
-	std::sort(d2.begin(), d2.end(), d2_before);
-	uint32_t d2book[4096];
-	for (size_t c = 0; c < 4096; c++) d2book[c] = c < d2.size() ? d2[c] : 0xFFFFFFFFu;
-	// dictionary order: count desc, then tuple_key (code word | d2book index << 32) asc, as apo_tuple_encode_host
-	std::vector<std::pair<unsigned long long, unsigned long long>> order(n);     // (count, tuple key)
-	for (uint32_t i = 0; i < n; i++) {
-		const uint32_t hi = (uint32_t)(keys[i] >> 32);
-		const uint64_t pd = hi == apo::KW_D2_ABSENT ? 4095u : (uint64_t)(std::lower_bound(d2.begin(), d2.end(), hi, d2_before) - d2.begin());
-		order[i] = {counts[i], (keys[i] & 0xFFFFFFFFull) | (pd << 32)};
-	}
-	std::sort(order.begin(), order.end(), [](const std::pair<unsigned long long, unsigned long long> &x, const std::pair<unsigned long long, unsigned long long> &y) {
-		if (x.first != y.first) return x.first > y.first;
-		return x.second < y.second;
-	});
-	if (copy) {                                                   // see build_twin_t
-		uint64_t head = 0;
-		for (uint32_t r = 0; r < n && r < kTwinTHot; r++) head += order[r].first;
-		if (head * 4 < N * 3) return APO_E_STATE;
-		*n_high = 0;
-		for (uint32_t r = 65536; r < n; r++) *n_high += order[r].first;
-		counts16->resize(std::min<uint32_t>(n, 65536));
-		for (size_t r = 0; r < counts16->size(); r++) (*counts16)[r] = order[r].first;
-	}
-	std::vector<uint32_t> tb_pc(n);
-	std::vector<uint16_t> tb_pd(n);
-	for (uint32_t r = 0; r < n; r++) {
-		const uint32_t pd = (uint32_t)(order[r].second >> 32);
-		tb_pc[r] = (uint32_t)order[r].second; tb_pd[r] = (uint16_t)pd;
-		keys[r] = (unsigned long long)tb_pc[r] | ((unsigned long long)(pd == 4095u ? apo::KW_D2_ABSENT : d2book[pd]) << 32);   // back to the evaluation key
-	}
-	CK(cudaMemcpyAsync(D.d2.p, d2book, sizeof d2book, cudaMemcpyHostToDevice, e->stream));
-	if (n) {
-		CK(cudaMemcpyAsync(D.pc.p, tb_pc.data(), (uint64_t)n * 4, cudaMemcpyHostToDevice, e->stream));
-		CK(cudaMemcpyAsync(D.pd.p, tb_pd.data(), (uint64_t)n * 2, cudaMemcpyHostToDevice, e->stream));
-		CK(cudaMemcpyAsync(e->tb_keys.p, keys.data(), (uint64_t)n * 8, cudaMemcpyHostToDevice, e->stream));
-		// the index table holds only the dictionary (slots >= 2 n, so that it stays small enough for L2)
-		uint64_t islots = 1024;
-		while (islots < 2ull * n) islots <<= 1;
-		CK(apo::run_tb_clear(e->tb_table.p, islots, e->stream));
-		CK(apo::run_tb_insert(e->tb_keys.p, n, e->tb_table.p, islots, e->stream));
-		CK(apo::run_tb_index(S, e->tb_keys.p, n, e->tb_table.p, islots, D.l.p, D.h.p, tpitch, (uint32_t *)(misc + 1), e->sm_count, e->stream));
-	}
-	unsigned long long miss = 0;
-	CK(cudaMemcpyAsync(&miss, misc + 1, 8, cudaMemcpyDeviceToHost, e->stream));
-	CK(cudaStreamSynchronize(e->stream));
-	if (miss) return fail(e, APO_E_CUDA, "internal error: an evaluation's key is missing from the dictionary");
-	memcpy(D.book, e->qt.book, sizeof D.book);
-	D.C = C; D.T = T; D.pitch = tpitch; D.n = n;
-	*n_tuples = n;
-	return APO_OK;
-}
-
-// The Form T copy of a freshly loaded Form D tensor that holds a Form W / Q copy with <= 15 values per coded dimension: its
-// resident Form D calls then read 3 B per evaluation through K1t (route_twin).  Built when the tensor holds at least
-// kTwinTMinEvals evaluations (APO_TUNE_TWIN_T: any size), at most kTwinTCap distinct ones (the build's scratch is sized
-// from it; the table stays well inside L2), the kTwinTHot most frequent of them cover at least 3/4 of the evaluations (K1t
-// serves those from shared memory and gathers the rest from L2: on an H100 it beats K1q on Form W with 75 % of its reads in
-// the head and loses by 2x with 9 %, DESIGN §8), and kTwinHeadroom of device memory stays free beside the copy and the
-// build's scratch; otherwise no copy is kept, without an error.  The build also computes the table values for the weights.
-constexpr uint64_t kTwinTMinEvals = 1ull << 26;
-constexpr uint32_t kTwinTCap = 1u << 20;
-
-// The exception list of the Form T copy: with it resident Form D calls read 2 B per evaluation through K1t2 instead of 3 B
-// through K1t (route_twin).  Built from n_high, the evaluations whose index is >= 2^16 (known from the dictionary's
-// counts), when at most 1/kTwinT2Share of the evaluations are such exceptions (DESIGN §8: K1t2 corrects each one after its
-// stream) and a row's positions fit 32 bits; otherwise, or without room for it, the copy is read through K1t as before,
-// without an error.  APO_TUNE_NO_TWIN_T2 at the load builds none.
-// K1t2 reads the slot plane `s` (apo_kernels.h): the KT_SLOT_H most frequent entries get one copy per shared-memory bank pair,
-// fewer (down to none) when the evaluations of the entries left without a slot would exceed 1/kTwinT2Share of them; those
-// evaluations make the second list.  Slot plane, slot-order tables and that list need room too, or K1t serves the copy.
-constexpr uint64_t kTwinT2Share = 64;
-int build_twin_t2(apo_engine *e, uint64_t n_high, const std::vector<uint64_t> &counts16) {
-	TupleCopy &t = e->tcopy;
-	const uint32_t C = t.C;
-	const uint64_t T = t.T, N = (uint64_t)C * T;
-	if (e->env_no_twin_t2 || n_high * kTwinT2Share > N || T > 0xFFFFFFFFull || n_high > 0xFFFFFFFFull) return APO_OK;
-	const uint32_t nblk = (uint32_t)((T + apo::KT_XBLOCK - 1) / apo::KT_XBLOCK);
-	t.nblk = nblk;
-	if (n_high) {
-		if (t.xb.reserve((uint64_t)C * (nblk + 1)) != cudaSuccess || t.xs.reserve(n_high) != cudaSuccess) {
-			cudaGetLastError();
-			t.xb.release(); t.xs.release();
-			return APO_OK;
-		}
-		CK(apo::run_tx_build(t.l.p, t.h.p, t.pitch, C, T, 65536u, t.xb.p, t.xs.p, e->sm_count, e->stream));
-		t.xn = n_high;
-	}
-	uint32_t h = std::min<uint32_t>(apo::KT_SLOT_H, t.n), end = 0;
-	uint64_t ny = 0;
-	for (;; h /= 2) {
-		end = apo::kt_slot_end(t.n, h);
-		ny = 0;
-		for (size_t r = end; r < counts16.size(); r++) ny += counts16[r];
-		if (ny * kTwinT2Share <= N || h == 0) break;
-	}
-	TupleVals &v = t.vals;
-	const uint32_t n_slots = end + (apo::KT_SLOT_REP - 1) * h + 1;
-	if (t.s.reserve((uint64_t)C * t.pitch) != cudaSuccess || v.sval[0].reserve(n_slots) != cudaSuccess || v.sval[1].reserve(n_slots) != cudaSuccess ||
-	    (ny && (t.yb.reserve((uint64_t)C * (nblk + 1)) != cudaSuccess || t.ys.reserve(ny) != cudaSuccess))) {
-		cudaGetLastError();
-		t.s.release(); v.sval[0].release(); v.sval[1].release(); t.ys.release(); t.yb.release();
-		CK(cudaStreamSynchronize(e->stream));
-		return APO_OK;                                            // the exception list alone: K1t reads the copy
-	}
-	CK(apo::run_slot_plane(t.l.p, t.h.p, t.pitch, C, T, h, end, t.s.p, e->stream));
-	if (ny) CK(apo::run_tx_build(t.l.p, t.h.p, t.pitch, C, T, end, t.yb.p, t.ys.p, e->sm_count, e->stream));
-	v.slot_h = h; v.slot_end = end; v.slots = true;
-	for (int r = 0; r < 2; r++)                                     // the values computed so far (build_twin_t: recip = 0)
-		if (v.ok[r]) CK(apo::run_tuple_slots(v.out(r), h, end, v.sval[r].p, e->stream));
-	CK(cudaStreamSynchronize(e->stream));                         // the load returns with the lists built, as with the copy
-	t.yn = ny;
-	t.t2 = true;
-	return APO_OK;
-}
-
-// The per-row dictionary counts of the Form T copy (apo_kernels.h KhParams): with them a call over whole rows reads 8 B per
-// distinct (row, entry) pair through K1h instead of 2 B per evaluation through K1t2 (route_twin).  The rows are counted in
-// batches whose dense [rows][entries] scratch stays within kTwinHScratch: a first sweep gives the exact number of pairs, and the
-// counts are kept when they take at most a quarter of K1t2's slot plane (8 nnz <= C T / 2) and kTwinHeadroom stays free beside
-// them; a second sweep writes them (a single batch keeps its counts from the first).  Otherwise, or without room, none are
-// held, without an error.  The scratch is freed before this returns.  APO_TUNE_NO_TWIN_H at the load builds none.
-constexpr uint64_t kTwinHScratch = 256ull << 20;
-int build_twin_h(apo_engine *e) {
-	TupleCopy &t = e->tcopy;
-	const uint32_t C = t.C;
-	const uint64_t T = t.T;
-	if (e->env_no_twin_h || C == 0 || T == 0 || T > 0xFFFFFFFFull || t.n == 0 || t.n > (1u << apo::KH_COUNT_SHIFT)) return APO_OK;
-	const uint32_t npitch = (uint32_t)round_up(t.n, 32), nchunk = (npitch + 8191) / 8192;
-	const uint32_t R = (uint32_t)std::min<uint64_t>(C, std::max<uint64_t>(1, kTwinHScratch / (4ull * npitch)));
-	const uint32_t nb = (C + R - 1) / R;
-	struct Scoped : DevBuf<uint32_t> { ~Scoped() { release(); } } cnt, nz;   // freed on every return path
-	if (cnt.reserve((uint64_t)R * npitch) != cudaSuccess || nz.reserve((uint64_t)R * nchunk + 1) != cudaSuccess) { cudaGetLastError(); return APO_OK; }
-	auto count = [&](uint32_t b) -> cudaError_t {
-		const uint32_t c0 = b * R, r = std::min(R, C - c0);
-		cudaError_t c = cudaMemsetAsync(cnt.p, 0, (uint64_t)r * npitch * 4, e->stream);
-		return c != cudaSuccess ? c : apo::run_th_count(t.l.p + (uint64_t)c0 * t.pitch, t.h.p + (uint64_t)c0 * t.pitch, t.pitch, r, T, npitch, cnt.p, nz.p, e->sm_count, e->stream);
-	};
-	std::vector<uint64_t> total(nb);
-	uint64_t nnz = 0;
-	for (uint32_t b = 0; b < nb; b++) {
-		CK(count(b));
-		uint32_t n = 0;
-		CK(cudaMemcpyAsync(&n, nz.p + (uint64_t)std::min(R, C - b * R) * nchunk, 4, cudaMemcpyDeviceToHost, e->stream));
-		CK(cudaStreamSynchronize(e->stream));
-		total[b] = n; nnz += n;
-	}
-	size_t free_bytes = 0, total_bytes = 0;
-	CK(cudaMemGetInfo(&free_bytes, &total_bytes));
-	if (nnz * 8 > (uint64_t)C * T / 2 || (uint64_t)free_bytes < nnz * 8 + 8ull * (C + 1) + kTwinHeadroom) return APO_OK;
-	if (t.hp.reserve(nnz) != cudaSuccess || t.ho.reserve(C + 1ull) != cudaSuccess) {
-		cudaGetLastError();
-		t.hp.release(); t.ho.release();
-		return APO_OK;
-	}
-	uint64_t base = 0;
-	for (uint32_t b = 0; b < nb; b++) {
-		if (nb > 1) CK(count(b));
-		CK(apo::run_th_write(cnt.p, std::min(R, C - b * R), npitch, nz.p, base, t.hp.p, t.ho.p + (uint64_t)b * R, e->sm_count, e->stream));
-		base += total[b];
-	}
-	CK(cudaStreamSynchronize(e->stream));                         // the load returns with the counts built, as with the copy
-	t.hn = nnz;
-	return APO_OK;
-}
-
-int build_twin_t(apo_engine *e) {
-	const uint32_t C = e->dims_C;
-	const uint64_t T = e->dims_T, N = (uint64_t)C * T;
-	if (e->env_no_twin_t || !(N >= kTwinTMinEvals || e->env_twin_t)) return APO_OK;
-	if (!e->twin_w)
-		for (int j = 0; j < 8; j++)
-			if (e->qt.book[256 * j + 15] != 0xFFFFFFFFu) return APO_OK;
-	const uint64_t m = std::min<uint64_t>(kTwinTCap, N);
-	uint64_t slots = 1024;
-	while (slots < 2 * (m + 1)) slots <<= 1;
-	// index planes, dictionary, value tables, the largest exception list and its block index; the slot plane, the slot-order
-	// tables and the second list; the build's hash table, keys and counts
-	const uint64_t need = 3 * (uint64_t)C * round_up(T, 64) + m * 6 + 2 * (m + 1) * 8 + 8 * (N / kTwinT2Share) +
-	                      4 * (uint64_t)C * (T / apo::KT_XBLOCK + 2) + 2 * (uint64_t)C * round_up(T, 64) + 2 * 65536 * 8 +
-	                      8 * (N / kTwinT2Share) + 4 * (uint64_t)C * (T / apo::KT_XBLOCK + 2) + 16 * slots + 16 * m;
-	size_t free_bytes = 0, total_bytes = 0;
-	CK(cudaMemGetInfo(&free_bytes, &total_bytes));
-	if ((uint64_t)free_bytes < need + kTwinHeadroom) return APO_OK;
-	const std::string keep_err = e->err;
-	uint32_t n = 0;
-	uint64_t n_high = 0;
-	std::vector<uint64_t> counts16;
-	TupleVals &v = e->tcopy.vals;
-	int rc = dims_tuples(e, kTwinTCap, &n, e->tcopy, true, &n_high, &counts16);
-	if (rc == APO_OK && (v.val[0].reserve(n + 1ull) != cudaSuccess || v.val[1].reserve(n + 1ull) != cudaSuccess ||
-	                     v.ptab.reserve(8 * 256) != cudaSuccess || v.bad.reserve(1) != cudaSuccess)) {
-		cudaGetLastError();
-		rc = APO_E_NOMEM;
-	}
-	if (rc == APO_OK) rc = tuple_values(e, e->tcopy, v, false);
-	if (rc == APO_OK) rc = build_twin_t2(e, n_high, counts16);
-	if (rc == APO_OK) rc = build_twin_h(e);
-	tb_release(e, rc);
-	if (rc == APO_OK) return APO_OK;
-	e->tcopy.release();
-	if (rc != APO_E_STATE && rc != APO_E_NOMEM) return rc;
-	e->err = keep_err;                                          // more than kTwinTCap distinct evaluations, or no room: no copy
-	return APO_OK;
-}
-}  // namespace
-
 extern "C" int apo_dims_tuples(apo_engine *e, uint32_t cap, uint32_t *n_tuples) {
 	if (!e) return APO_E_ARG;
 	if (!n_tuples) return fail(e, APO_E_ARG, "n_tuples is NULL");
 	*n_tuples = 0;
 	CK(cudaSetDevice(e->device));
 	e->tup.unload();                                               // a failure leaves no Form T loaded, as a failed apo_tuples_upload
-	const int rc = dims_tuples(e, cap, n_tuples, e->tup, false);
+	TbRanked R;
+	int rc = tuples_rank(e, cap, n_tuples, e->tup, false, R);
+	if (rc == APO_OK) rc = tuples_index(e, R, e->tup);
+	if (rc == APO_OK) *n_tuples = e->tup.n;
 	tb_release(e, rc);
 	return rc;
 }
@@ -2394,24 +2394,24 @@ extern "C" int apo_debug_partials(apo_engine *e, int64_t *out, uint32_t C) {
 
 extern "C" int apo_debug_twin_t_list(apo_engine *e, uint64_t *n_words, uint64_t *n_exceptions, uint32_t *xb, uint32_t *xs) {
 	if (!e || !n_words || !n_exceptions) return fail(e, APO_E_ARG, "NULL argument");
-	*n_words = e->tcopy.xn ? (uint64_t)e->tcopy.C * (e->tcopy.nblk + 1) : 0;
-	*n_exceptions = e->tcopy.xn;
-	if (!e->tcopy.xn) return APO_OK;
+	*n_words = e->copy.t.xn ? (uint64_t)e->copy.t.C * (e->copy.t.nblk + 1) : 0;
+	*n_exceptions = e->copy.t.xn;
+	if (!e->copy.t.xn) return APO_OK;
 	CK(cudaSetDevice(e->device));
-	if (xb) CK(cudaMemcpyAsync(xb, e->tcopy.xb.p, *n_words * 4, cudaMemcpyDeviceToHost, e->stream));
-	if (xs) CK(cudaMemcpyAsync(xs, e->tcopy.xs.p, e->tcopy.xn * 8, cudaMemcpyDeviceToHost, e->stream));
+	if (xb) CK(cudaMemcpyAsync(xb, e->copy.t.xb.p, *n_words * 4, cudaMemcpyDeviceToHost, e->stream));
+	if (xs) CK(cudaMemcpyAsync(xs, e->copy.t.xs.p, e->copy.t.xn * 8, cudaMemcpyDeviceToHost, e->stream));
 	CK(cudaStreamSynchronize(e->stream));
 	return APO_OK;
 }
 
 extern "C" int apo_debug_twin_h(apo_engine *e, uint32_t *rows, uint64_t *n_pairs, uint64_t *off, uint64_t *pairs) {
 	if (!e || !rows || !n_pairs) return fail(e, APO_E_ARG, "NULL argument");
-	*n_pairs = e->tcopy.hn;
-	*rows = e->tcopy.hn ? e->tcopy.C : 0;
-	if (!e->tcopy.hn) return APO_OK;
+	*n_pairs = e->copy.t.hn;
+	*rows = e->copy.t.hn ? e->copy.t.C : 0;
+	if (!e->copy.t.hn) return APO_OK;
 	CK(cudaSetDevice(e->device));
-	if (off) CK(cudaMemcpyAsync(off, e->tcopy.ho.p, (e->tcopy.C + 1ull) * 8, cudaMemcpyDeviceToHost, e->stream));
-	if (pairs) CK(cudaMemcpyAsync(pairs, e->tcopy.hp.p, e->tcopy.hn * 8, cudaMemcpyDeviceToHost, e->stream));
+	if (off) CK(cudaMemcpyAsync(off, e->copy.t.ho.p, (e->copy.t.C + 1ull) * 8, cudaMemcpyDeviceToHost, e->stream));
+	if (pairs) CK(cudaMemcpyAsync(pairs, e->copy.t.hp.p, e->copy.t.hn * 8, cudaMemcpyDeviceToHost, e->stream));
 	CK(cudaStreamSynchronize(e->stream));
 	return APO_OK;
 }
@@ -2479,7 +2479,7 @@ extern "C" int apo_comm_init(apo_engine *e, int nranks, int rank, const uint8_t 
 
 extern "C" int apo_comm_join_mode(const apo_engine *e) {
 	if (!e || e->nranks <= 1) return 0;
-	return (e->peer_ok && !e->env_nccl_join) ? 2 : 1;
+	return (e->peer_ok && !(e->tune & APO_TUNE_NCCL_JOIN)) ? 2 : 1;
 }
 
 extern "C" int apo_comm_destroy(apo_engine *e) {

@@ -161,6 +161,7 @@ cudaError_t run_decode(const unsigned long long *q8, const float *d2, const unsi
 // evaluations; the reward of a dictionary entry is computed once (k_tuple_values), K1t sums table entries.
 constexpr uint32_t KT_TUPLES_MAX = 0xFFFFFFu;      // dictionary entries addressable by lo16 | hi8 << 16
 constexpr int KT_VALID_SHIFT = 58;                 // table entry = rint(finalReward * 2^52) + (counted << 58)
+constexpr uint32_t KT_HOT_MAX = 24576;             // K1t serves table entries [0, KT_HOT_MAX) from shared memory (192 KB)
 struct KtParams {
 	const unsigned short *tl;       // [C][pitch] low 16 bits of the tuple index
 	const unsigned char *th;        // [C][pitch] high 8 bits

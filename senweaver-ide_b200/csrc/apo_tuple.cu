@@ -65,7 +65,6 @@ constexpr int KT_STEPS = 1;                       // one 16-byte + one 8-byte lo
 constexpr int KT_GROUP = 8;                       // evaluations per thread and step
 constexpr int KT_STEP_EVALS = KT_THREADS * KT_GROUP;
 constexpr int KT_TILE = KT_STEP_EVALS * KT_STEPS; // 8192 evaluations
-constexpr uint32_t KT_HOT_MAX = 24576;            // 192 KB of shared memory
 
 static_assert(KT_GROUP * KT_STEPS <= 16, "the count field of a table entry sits 5 bits above the largest 16-entry sum");
 
