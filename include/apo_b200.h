@@ -149,6 +149,7 @@ int  apo_set_weights(apo_engine *e, const double w[APO_NDIM]);
 #define APO_TUNE_TWIN_T      0x40u /* loads build the Form T copy whatever the tensor's size (tests, A/B runs on small tensors) */
 #define APO_TUNE_NO_TWIN_T2  0x80u /* no exception list of the Form T copy is built or read: the copy is read at 3 B per evaluation */
 #define APO_TUNE_NO_TWIN_H   0x100u /* no per-row counts of the Form T copy are built or read: whole rows read the copy as other windows */
+#define APO_TUNE_NO_CORPUS_DIGEST 0x200u /* no corpus digest is built or read: scoring calls scan the resident corpus record by record */
 int  apo_set_tuning(apo_engine *e, uint32_t flags);
 int  apo_get_weights(const apo_engine *e, double w[APO_NDIM]);
 
@@ -161,7 +162,15 @@ int apo_reward_one(apo_engine *e, const apo_record *rec, double dims[APO_NDIM],
                    uint32_t *mask, double *final_reward);
 
 /* ---- corpus = the T trace records APOService._buildReport walks (APO:498-625) ------
- * idx_base = global index of recs[0] (shard offset); example indices are global. */
+ * idx_base = global index of recs[0] (shard offset); example indices are global.
+ * For a corpus of at least 2^20 records, the second scoring call with APO_SCORE_CORPUS after the load builds a corpus digest on
+ * the device (a corpus loaded to be reported once is scanned once and never pays for it), when the corpus holds at most 2^20
+ * and at most T/4 distinct reward keys (a VALID record's categorical dimension levels and its tool_success_rate value) and
+ * 4 GiB of device memory stay free beside it; otherwise, quietly, none.  The weights reach the corpus report only through
+ * these keys, so that call and the later ones derive the report from the counted keys and from the words no weight reaches
+ * (tallies, byMode, tool totals, pattern counts and examples) instead of scanning every record: the same report, bit for bit.
+ * The digest goes with the next corpus load; apo_set_weights keeps it.  With APO_TUNE_NO_CORPUS_DIGEST set, none is built
+ * and calls scan. */
 int apo_corpus_upload(apo_engine *e, const apo_record *recs, uint64_t T, uint64_t idx_base);
 int apo_corpus_generate(apo_engine *e, uint64_t seed, uint64_t t0, uint64_t T, uint32_t agent_permille);
 int apo_corpus_download(apo_engine *e, apo_record *out, uint64_t first, uint64_t n);
@@ -389,6 +398,12 @@ int apo_debug_twin_t_list(apo_engine *e, uint64_t *n_words, uint64_t *n_exceptio
  * c < *rows the words [off[c], off[c + 1]) (off: *rows + 1 words) of the dictionary entries its evaluations name, ascending,
  * each entry | count << 20.  Both counts are 0 when no counts are held.  off / pairs may be NULL. */
 int apo_debug_twin_h(apo_engine *e, uint32_t *rows, uint64_t *n_pairs, uint64_t *off, uint64_t *pairs);
+/* The corpus digest (see apo_corpus_upload), for tests and diagnostics: *n_entries entries of two words {binary64 bits of d2,
+ * slots | count << 22} (slots = i01 | i3 << 4 | i4 << 7 | i5 << 10 | i6 << 13 | i7 << 16 | i8 << 19, in any order) and 45
+ * fixed words: the corpus-block words of the tallies, byMode, pattern counts and tool totals (27), then the first three
+ * 'bad' records of each pattern as inverted indices (18, 0 = none).  *n_entries is 0 and nothing is written when no digest is
+ * held.  entries / fixed may be NULL. */
+int apo_debug_corpus_digest(apo_engine *e, uint64_t *n_entries, uint64_t *entries, int64_t *fixed);
 
 /* ---- per-candidate breakdown: why candidate c scored what it scored ------------------
  * The corpus report (APO:498-625) answered per candidate, over the evaluations of c that the

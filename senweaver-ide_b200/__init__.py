@@ -13,5 +13,5 @@ from .engine import (ApoError, CorpusReport, Engine, RECORD_DTYPE, ScoreResult, 
                      NDIM, NPAT, NMODE, SRC_DIMS, SRC_ROLLOUTS, SRC_TUPLES, TUPLES_MAX, build_library, load_library, LIB_PATH, ABI_SYMBOLS,
                      RECORD16_DTYPE, pack16, unpack16, records_from_json, host_empty, SCORE_TIMING, compact_encode_host, packed_encode_host, tuple_encode_host,
                      TUNE_NO_FUSE, TUNE_FORCE_FUSE, TUNE_NO_STAGING, TUNE_NCCL_JOIN, TUNE_NO_TWIN,
-                     TUNE_NO_TWIN_T, TUNE_TWIN_T, TUNE_NO_TWIN_T2, TUNE_NO_TWIN_H)
+                     TUNE_NO_TWIN_T, TUNE_TWIN_T, TUNE_NO_TWIN_T2, TUNE_NO_TWIN_H, TUNE_NO_CORPUS_DIGEST)
 from . import sharding  # noqa: F401

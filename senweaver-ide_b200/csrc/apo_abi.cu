@@ -23,7 +23,7 @@
 
 namespace {
 
-constexpr int ACC_PER_CAND = 4, CORP_FIXED = 68;
+constexpr int ACC_PER_CAND = 4, CORP_FIXED = 68, CORP_TALLY = 40;
 inline uint64_t acc_words(uint32_t C, int nranks) { return (uint64_t)ACC_PER_CAND * C + CORP_FIXED + 18ull * nranks; }
 
 std::string g_create_error;
@@ -137,11 +137,24 @@ struct DimsCopy {
 	TupleCopy t;
 };
 
+// What a scoring call's corpus report needs from a large resident corpus (build_digest, apo_kernels.h CorpusDigestParams): the
+// counted reward keys (ent, n of them; misc[2] holds n on the device) and the words that do not depend on the weights (fixed).
+// Built by the second scoring call with a corpus report after the corpus load (digest_prepare), so that a corpus loaded to be
+// reported once never pays for it.  uses: such calls since the load; tried: the build ran (held or not).
+struct CorpusDigest {
+	DevBuf<ulonglong2> ent; DevBuf<long long> fixed; DevBuf<unsigned long long> misc;
+	uint64_t n = 0; bool held = false;
+	uint32_t uses = 0; bool tried = false;
+	void release() { ent.release(); fixed.release(); misc.release(); n = 0; held = false; }
+	void reset() { release(); uses = 0; tried = false; }
+};
+
 // the tuning switches (apo_set_tuning) and the environment variables that set them when a handle is created
 const struct { const char *env; uint32_t bit; } kTuning[] = {
 	{"APO_NO_FUSE", APO_TUNE_NO_FUSE}, {"APO_FORCE_FUSE", APO_TUNE_FORCE_FUSE}, {"APO_NO_STAGING", APO_TUNE_NO_STAGING},
 	{"APO_JOIN_NCCL", APO_TUNE_NCCL_JOIN}, {"APO_NO_TWIN", APO_TUNE_NO_TWIN}, {"APO_NO_TWIN_T", APO_TUNE_NO_TWIN_T},
-	{"APO_TWIN_T", APO_TUNE_TWIN_T}, {"APO_NO_TWIN_T2", APO_TUNE_NO_TWIN_T2}, {"APO_NO_TWIN_H", APO_TUNE_NO_TWIN_H}};
+	{"APO_TWIN_T", APO_TUNE_TWIN_T}, {"APO_NO_TWIN_T2", APO_TUNE_NO_TWIN_T2}, {"APO_NO_TWIN_H", APO_TUNE_NO_TWIN_H},
+	{"APO_NO_CORPUS_DIGEST", APO_TUNE_NO_CORPUS_DIGEST}};
 
 }  // namespace
 
@@ -154,6 +167,7 @@ struct apo_engine {
 	DevBuf<double> d_lut;          // [0,512) total weight, [512,1024) reciprocal, [1024,1088) categorical products
 
 	DevBuf<apo_record> corpus; uint64_t corpus_T = 0, corpus_base = 0;
+	CorpusDigest digest;                  // of the resident corpus (build_digest), released by the next corpus load
 	DevBuf<float> dims; const float *dims_ptr = nullptr; uint32_t dims_C = 0; uint64_t dims_T = 0, dims_pitch = 0;
 	// Form Q planes of the evaluations: the compact tensor (replacing dims/dims_ptr when `compact` is set) or the copy of kind Q
 	DevBuf<unsigned long long> q8; DevBuf<float> qd2; DevBuf<unsigned short> qli; DevBuf<uint32_t> qbook;   // qbook: [8][256] codebook + [8] overflow flags
@@ -716,6 +730,10 @@ int launch_score(apo_engine *e, const apo_score_opts *o, const Evals &ev, uint32
 	if (const TupleCopy *t = ev.copy; ev.read == Evals::K1h) {   // the copy's values were computed before the route
 		apo::KhParams P{};
 		P.pairs = t->hp.p; P.off = t->ho.p; P.C = ev.C; P.nnz = t->hn; P.acc = acc; P.tval = t->vals.val[recip].p;
+		if (fused) {                                          // the digest pass (fused->T > 0: the corpus words) and the tail
+			P.corpus_on = 1; P.cd.k2 = *fused;
+			if (fused->T) { P.cd.ent = e->digest.ent.p; P.cd.n = e->digest.misc.p + 2; P.cd.fixed = e->digest.fixed.p; }
+		}
 		CK(apo::run_reward9th(P, e->sm_count, e->stream));
 	} else if (ev.read == Evals::K1t2) {
 		apo::Kt2Params P{};
@@ -871,6 +889,8 @@ int ccorp_finish(apo_engine *e, uint32_t C) {
 
 // K2 (+fused finalize) / allreduce / K3, then bring the result block home
 bool wants_corpus(const apo_engine *e, const apo_score_opts *o) { return (o->flags & APO_SCORE_CORPUS) && e->corpus_T > 0; }
+// the corpus words come from the digest instead of a scan of the records
+bool digest_on(const apo_engine *e) { return e->digest.held && !(e->tune & APO_TUNE_NO_CORPUS_DIGEST); }
 
 // the corpus block, the example scratch and the ticket belong to one corpus pass only, so that a scoring session can be
 // finished repeatedly while evaluations keep being accumulated (incremental scoring); they sit behind the candidate
@@ -906,7 +926,13 @@ int finish_score(apo_engine *e, const apo_score_opts *o, uint32_t C, double *sco
 	bool finalized = self_clean;
 	if (with_corpus && !fused_corpus) {
 		const apo::K2Params P = make_k2(e, C, F);
-		CK(apo::run_detect6(P, e->sm_count, e->stream));
+		if (digest_on(e)) {                                        // the counted keys of the corpus instead of its records
+			apo::CorpusDigestParams D{};
+			D.ent = e->digest.ent.p; D.n = e->digest.misc.p + 2; D.fixed = e->digest.fixed.p; D.k2 = P;
+			CK(apo::run_corpus_digest(D, e->digest.n, e->sm_count, e->stream));
+		} else {
+			CK(apo::run_detect6(P, e->sm_count, e->stream));
+		}
 		e->timing.launches++;
 		finalized = P.fuse_finalize != 0;
 	}
@@ -1584,7 +1610,7 @@ extern "C" void apo_destroy(apo_engine *e) {
 	release_copies(e);
 	e->q8.release(); e->qd2.release(); e->qli.release(); e->qbook.release(); e->d_d2book.release(); e->d_d2stream.release(); e->unpack_bad.release(); e->stage.release();
 	e->qt.release(); e->qt_stream.release();
-	e->d_lut.release(); e->corpus.release(); e->dims.release(); e->roll.release(); e->acc.release(); e->acc_joined.release(); e->acc_snapshot.release(); e->misc.release();
+	e->d_lut.release(); e->corpus.release(); e->digest.release(); e->dims.release(); e->roll.release(); e->acc.release(); e->acc_joined.release(); e->acc_snapshot.release(); e->misc.release();
 	e->result.release(); e->keys.release(); e->sel_key.release(); e->sel_idx.release();
 	e->cand_acc.release(); e->cand_rep.release(); e->cand_book.release(); e->ccorp_acc.release(); e->ccorp_rep.release();
 	e->tup.release(); e->tups.release(); e->tvals.release();
@@ -1676,10 +1702,77 @@ extern "C" int apo_reward_one(apo_engine *e, const apo_record *rec, double dims[
 }
 
 // =============================================================================== corpus
+namespace {
+// The corpus digest of the freshly loaded corpus (after its duration classes: the key reads them), or none, quietly: for corpora
+// of at least kDigestMinRecords records with at most kDigestCap and at most T / 4 distinct reward keys, when kDigestHeadroom
+// stays free beside the build.  The count pass stops early past the cap.  The fixed words come from one run of the stand-alone
+// scan into scratch, of which only the weight-independent words are kept.  Ends with the stream synchronised.
+constexpr uint64_t kDigestMinRecords = 1ull << 20, kDigestCap = 1ull << 20;
+constexpr uint64_t kDigestHeadroom = 4ull << 30;
+constexpr uint64_t kDigestSpill = 1ull << 20;      // keys the count pass may insert past the cap before every warp has stopped
+int build_digest_buffers(apo_engine *e) {
+	CorpusDigest &d = e->digest;
+	const uint64_t T = e->corpus_T;
+	if ((e->tune & APO_TUNE_NO_CORPUS_DIGEST) || T < kDigestMinRecords) return APO_OK;
+	const uint64_t cap = std::min<uint64_t>(kDigestCap, T / 4);
+	uint64_t slots = 1024;
+	while (slots < 2 * cap + kDigestSpill) slots <<= 1;
+	const uint64_t scratch_words = CORP_FIXED + 18 + ARM_WORDS;
+	size_t free_bytes = 0, total_bytes = 0;
+	CK(cudaMemGetInfo(&free_bytes, &total_bytes));
+	if ((uint64_t)free_bytes < slots * 24 + cap * 32 + scratch_words * 8 + kDigestHeadroom) return APO_OK;
+	struct ScopedT : DevBuf<ulonglong2> { ~ScopedT() { release(); } } table, big;
+	struct ScopedC : DevBuf<unsigned long long> { ~ScopedC() { release(); } } cnt;
+	struct ScopedS : DevBuf<long long> { ~ScopedS() { release(); } } scratch;
+	if (table.reserve(slots) != cudaSuccess || cnt.reserve(slots) != cudaSuccess || big.reserve(cap) != cudaSuccess ||
+	    scratch.reserve(scratch_words) != cudaSuccess || d.misc.reserve(3) != cudaSuccess || d.fixed.reserve(apo::CD_WORDS) != cudaSuccess) {
+		cudaGetLastError();
+		d.release();
+		return APO_OK;
+	}
+	CK(apo::run_cd_build(e->corpus.p, T, e->d_lut.p, table.p, cnt.p, slots, cap, d.misc.p, big.p, e->sm_count, e->stream));
+	CK(cudaMemsetAsync(scratch.p, 0, scratch_words * 8, e->stream));
+	apo::K2Params P{};
+	unsigned long long *arm = (unsigned long long *)(scratch.p + CORP_FIXED + 18);
+	P.recs = e->corpus.p; P.T = T; P.idx_base = e->corpus_base; P.C = 0; P.rank = 0;
+	P.acc = scratch.p; P.ex_scratch = arm; P.ticket = (unsigned int *)(arm + 18);
+	P.lut = e->d_lut.p; P.W = e->W; P.fuse_finalize = 0;
+	CK(apo::run_detect6(P, e->sm_count, e->stream));
+	CK(cudaMemcpyAsync(d.fixed.p, scratch.p + CORP_TALLY, apo::CD_FIXED * 8, cudaMemcpyDeviceToDevice, e->stream));
+	CK(cudaMemcpyAsync(d.fixed.p + apo::CD_FIXED, arm, 18 * 8, cudaMemcpyDeviceToDevice, e->stream));
+	unsigned long long m[3];
+	CK(cudaMemcpyAsync(m, d.misc.p, sizeof m, cudaMemcpyDeviceToHost, e->stream));
+	CK(cudaStreamSynchronize(e->stream));
+	if (m[1] || m[2] > cap) { d.release(); return APO_OK; }                    // more keys than the cap: the calls scan
+	if (d.ent.reserve(m[2] ? m[2] : 1) != cudaSuccess) { cudaGetLastError(); d.release(); return APO_OK; }
+	if (m[2]) CK(cudaMemcpyAsync(d.ent.p, big.p, m[2] * sizeof(ulonglong2), cudaMemcpyDeviceToDevice, e->stream));
+	CK(cudaStreamSynchronize(e->stream));
+	d.n = m[2]; d.held = true;
+	return APO_OK;
+}
+
+int build_digest(apo_engine *e) {
+	const int rc = build_digest_buffers(e);
+	if (!e->digest.held) e->digest.release();              // whatever stopped the build, nothing is kept
+	return rc;
+}
+
+// Before a scoring call's launches (and, for a resident call, before route_copy: the build allocates): the second call since
+// the corpus load that asks for the corpus report builds the digest, so that a corpus loaded to be reported once scans once.
+int digest_prepare(apo_engine *e, const apo_score_opts *o) {
+	CorpusDigest &d = e->digest;
+	if (!wants_corpus(e, o) || d.held || d.tried || (e->tune & APO_TUNE_NO_CORPUS_DIGEST)) return APO_OK;
+	if (d.uses++ == 0) return APO_OK;
+	d.tried = true;
+	return build_digest(e);
+}
+}  // namespace
+
 extern "C" int apo_corpus_upload(apo_engine *e, const apo_record *recs, uint64_t T, uint64_t idx_base) {
 	if (!e) return APO_E_ARG;
 	if (T && !recs) return fail(e, APO_E_ARG, "recs is NULL");
 	CK(cudaSetDevice(e->device));
+	e->digest.reset();
 	CK(reserve(e, e->corpus, T ? T : 1));
 	if (T) { const int rc = h2d_rows(e, e->corpus.p, T * sizeof(apo_record), recs, T * sizeof(apo_record), T * sizeof(apo_record), 1, e->stream); if (rc) return rc; }
 	CK(apo::run_fill_durclass(e->corpus.p, 32, T, e->stream));        // resident records always carry the duration class
@@ -1712,6 +1805,7 @@ extern "C" int apo_corpus_upload_json(apo_engine *e, const char *json, uint64_t 
 extern "C" int apo_corpus_generate(apo_engine *e, uint64_t seed, uint64_t t0, uint64_t T, uint32_t agent_permille) {
 	if (!e) return APO_E_ARG;
 	CK(cudaSetDevice(e->device));
+	e->digest.reset();
 	CK(reserve(e, e->corpus, T ? T : 1));
 	CK(apo::run_gen_records(e->corpus.p, T, seed, 1u, 0, 1, t0, T, agent_permille, e->stream));
 	CK(cudaStreamSynchronize(e->stream));
@@ -1972,7 +2066,7 @@ extern "C" int apo_score_finish(apo_engine *e, const apo_score_opts *o, double *
 		return fail(e, APO_E_STATE, "APO_SCORE_CANDIDATES: every apo_score_accumulate of the session must set the flag for a breakdown");
 	if (wants_ccorp(o) && !e->ccorp_every)
 		return fail(e, APO_E_STATE, "APO_SCORE_CANDIDATE_CORPUS: every apo_score_accumulate of the session must set the flag for the reports");
-	if ((rc = score_arm(e, o, e->score_C, false))) return rc;   // nothing accumulated yet: an empty breakdown
+	if ((rc = digest_prepare(e, o)) || (rc = score_arm(e, o, e->score_C, false))) return rc;   // nothing accumulated yet: an empty breakdown
 	return finish_score(e, o, e->score_C, scores, counts, topk, report);
 }
 
@@ -1983,7 +2077,7 @@ extern "C" int apo_score(apo_engine *e, const apo_score_opts *o, double *scores,
 	int rc = resident_evals(e, o, &ev);
 	if (rc) return rc;
 	const uint32_t C = ev.C;
-	if ((rc = score_check(e, o, C, ev.count, ev.records())) || (rc = route_copy(e, o, &ev))) return rc;
+	if ((rc = score_check(e, o, C, ev.count, ev.records())) || (rc = digest_prepare(e, o)) || (rc = route_copy(e, o, &ev))) return rc;
 	if ((rc = resident_window(e, o, &ev))) return rc;
 	const bool tup = ev.form == apo::CAND_T;            // gather-and-add kernel: stand-alone corpus scan + tail
 	const double stream_bytes = (double)C * (double)ev.count * ev.bytes();
@@ -2002,15 +2096,19 @@ extern "C" int apo_score(apo_engine *e, const apo_score_opts *o, double *scores,
 	const bool fuse = !tup && wants_corpus(e, o) && ev.count > 0 && !(e->tune & APO_TUNE_NO_FUSE) && (k1_ms > 1.3 * scan_ms || small_scan || (e->tune & APO_TUNE_FORCE_FUSE));
 	// without a corpus request the same tail still saves the K3 launch: an empty scan, then the last CTA finalises
 	const bool tail_only = !tup && !wants_corpus(e, o) && one_launch && ev.count > 0 && !(e->tune & APO_TUNE_NO_FUSE);
-	const bool fused = fuse || tail_only;
+	// K1h (whole rows of the Form T copy): every CTA runs the digest pass after its pairs, then the same tail; without a corpus
+	// request the tail alone
+	const bool kh = ev.read == Evals::K1h && one_launch && ev.count > 0 && !(e->tune & APO_TUNE_NO_FUSE) && (!wants_corpus(e, o) || digest_on(e));
+	const bool kh_corpus = kh && wants_corpus(e, o);
+	const bool fused = fuse || tail_only || kh;
 	if ((rc = score_arm(e, o, C, true, (uint64_t)stream_bytes, fused))) return rc;
 	apo::K2Params k2{};
 	if (fused) {
-		apo::FinalizeParams F = make_fin(e, C, o->K, fuse ? 1 : 0);
+		apo::FinalizeParams F = make_fin(e, C, o->K, fuse || kh_corpus ? 1 : 0);
 		// the finalising CTA is in this launch: it can leave the block zeroed (finish_score records that it did)
 		if (one_launch) { F.clean_ptr = e->acc.p; F.clean_words = (uint32_t)(acc_words(C, e->nranks) + ARM_WORDS); F.snapshot = e->acc_snapshot.p; }
 		k2 = make_k2(e, C, F);
-		if (tail_only) { k2.T = 0; k2.recs = nullptr; }
+		if (tail_only || (kh && !kh_corpus)) { k2.T = 0; k2.recs = nullptr; }
 	}
 	if ((rc = launch_score(e, o, ev, 0, fused ? &k2 : nullptr))) return rc;
 	if (wants_cand(o) && (rc = launch_cand(e, ev, 0))) return rc;
@@ -2081,7 +2179,7 @@ int stream_host(apo_engine *e, const apo_score_opts *o, const HostTensor &h, dou
 	}
 	Evals ev;
 	ev.form = h.form; ev.C = C; ev.variant = (int)o->variant;
-	if ((rc = score_check(e, o, C, kStreamed, ev.records()))) return rc;
+	if ((rc = score_check(e, o, C, kStreamed, ev.records())) || (rc = digest_prepare(e, o))) return rc;
 	if (h.form == apo::CAND_Q) {                                   // Form Q / P: K1q's tables of this call's codebook
 		if ((rc = load_qtables(e, e->qt_stream, h.codebook))) return rc;
 		ev.qt = &e->qt_stream;
@@ -2413,6 +2511,18 @@ extern "C" int apo_debug_twin_h(apo_engine *e, uint32_t *rows, uint64_t *n_pairs
 	if (off) CK(cudaMemcpyAsync(off, e->copy.t.ho.p, (e->copy.t.C + 1ull) * 8, cudaMemcpyDeviceToHost, e->stream));
 	if (pairs) CK(cudaMemcpyAsync(pairs, e->copy.t.hp.p, e->copy.t.hn * 8, cudaMemcpyDeviceToHost, e->stream));
 	CK(cudaStreamSynchronize(e->stream));
+	return APO_OK;
+}
+
+extern "C" int apo_debug_corpus_digest(apo_engine *e, uint64_t *n_entries, uint64_t *entries, int64_t *fixed) {
+	if (!e || !n_entries) return fail(e, APO_E_ARG, "NULL argument");
+	const CorpusDigest &d = e->digest;
+	*n_entries = d.held ? d.n : 0;
+	if (!d.held) return APO_OK;
+	CK(cudaSetDevice(e->device));
+	CK(cudaStreamSynchronize(e->stream));
+	if (entries && d.n) CK(cudaMemcpy(entries, d.ent.p, d.n * sizeof(ulonglong2), cudaMemcpyDeviceToHost));
+	if (fixed) CK(cudaMemcpy(fixed, d.fixed.p, apo::CD_WORDS * 8, cudaMemcpyDeviceToHost));
 	return APO_OK;
 }
 

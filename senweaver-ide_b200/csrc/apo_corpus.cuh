@@ -59,6 +59,34 @@ struct ScanAcc {
 	}
 };
 
+// The reward key of a VALID record: its categorical slots and d2 (CatIdx of record_ws_table_t).  Everything the weights touch
+// in the corpus report depends on a record through this key alone: the corpus scan (scan_record) takes the weighted sum and
+// mask record_ws_table_t computes on the way, the pass over the corpus digest (csrc/apo_kernels.cu k_corpus_digest) recomputes
+// them from a stored key (key_ws), and both then run key_reward.
+// TCS:777-783 for one key: the weighted sum in push order through the product table (record_ws_table_t's adds, from the
+// slots), and the presence mask (the last slot of a group = not pushed).
+__device__ __forceinline__ uint32_t key_ws(const CatIdx &ix, double w2, const double *cat, double &ws_out) {
+	double ws = cat[CAT_D01 + ix.i01];
+	ws = __dadd_rn(ws, __dmul_rn(ix.d2, w2));
+	ws = __dadd_rn(ws, cat[CAT_D3 + ix.i3]);
+	ws = __dadd_rn(ws, cat[CAT_D4 + ix.i4]);
+	ws = __dadd_rn(ws, cat[CAT_D5 + ix.i5]);
+	ws = __dadd_rn(ws, cat[CAT_D6 + ix.i6]);
+	ws = __dadd_rn(ws, cat[CAT_D7 + ix.i7]);
+	ws = __dadd_rn(ws, cat[CAT_D8 + ix.i8]);
+	ws_out = ws;
+	return 3u | (ix.i3 != 4u ? 0x1cu : 0u) | (ix.i5 != 4u ? 0x20u : 0u) | (ix.i6 != 6u ? 0x40u : 0u) | (ix.i7 != 4u ? 0x80u : 0u) |
+	       (ix.i8 != 4u ? 0x100u : 0u);
+}
+// TCS:784: true when the key's total weight is > 0, with fx = rint(finalReward * 2^52).  ROT: LUT stored at the bank-rotated index.
+template <bool ROT>
+__device__ __forceinline__ bool key_reward(double ws, uint32_t mask, const double2 *s_lut, long long &fx) {
+	const double2 tw = s_lut[ROT ? lut_index(mask) : mask];
+	if (!(tw.x > 0.0)) return false;
+	fx = to_fx(div_lut<false>(ws, tw));
+	return true;
+}
+
 // One record of the corpus: tallies, the weighted reward and the per-dimension census, the six 'bad'-gated predicates
 // (APO:509-538, 550-565, 644-755).  gi = global index of the record.  ROT: LUT stored at the bank-rotated index.
 template <bool ROT>
@@ -72,9 +100,9 @@ __device__ __forceinline__ void scan_record(ScanAcc &A, const apo_record &r, uns
 	if (r.flags & APO_F_VALID) {                                                 // APO:550, TCS:606
 		double ws; CatIdx ix;
 		const uint32_t mask = record_ws_table_t<true, true>(r, w2, s_cat, ws, ix);
-		const double2 tw = s_lut[ROT ? lut_index(mask) : mask];
-		if (tw.x > 0.0) {                                                        // TCS:784 totalWeight > 0
-			A.fxR += to_fx(div_lut<false>(ws, tw));
+		long long fx;
+		if (key_reward<ROT>(ws, mask, s_lut, fx)) {                              // TCS:784 totalWeight > 0
+			A.fxR += fx;
 			A.nValid++;
 			const unsigned long long one01 = 1ull << (10u * (ix.i01 % 6u));
 			if (ix.i01 >= 6u) A.c01b += one01; else A.c01a += one01;
@@ -101,6 +129,59 @@ __device__ __forceinline__ void scan_record(ScanAcc &A, const apo_record &r, uns
 				if (gk > *((volatile unsigned long long *)&s_ex[3 * p + 2])) ex_insert(&s_ex[3 * p], gk);
 			}
 		}
+	}
+}
+
+// The census of counted records -> exact per-dimension sums and counts (APO:556-565): sum = SUM_k count_k * rint(value_k * 2^52)
+// per dimension, as adding rint(value * 2^52) record by record.  cnt(g, k) is the count of slot k of group g: g = 0 the
+// (feedback, hasErrors, endTime) slot fb + 3 err + 6 ended (TCS:677-691), g = 3..8 the level of dimension g (k = 0..3, d6:
+// 0..5); absent slots are never asked for.  nv: the counted records (withReward, the d0 / d1 counts).  Every thread of the
+// caller's group calls cnt (it may be a warp collective); `writer` adds into the corpus block corp.  The d2 sum (CORP_DIM + 8)
+// and the reward limbs are the caller's.  Shared by the corpus scan (scan_flush) and the digest pass (k_corpus_digest).
+template <class Count, class N>
+__device__ __forceinline__ void census_flush(Count cnt, N nv, long long *corp, bool writer) {
+	// d0 / d1 from the (feedback, hasErrors, endTime) census: TCS:677-691
+	__int128 s0 = 0, s1 = 0;
+#pragma unroll
+	for (int ended = 0; ended < 2; ended++)
+#pragma unroll
+		for (int err = 0; err < 2; err++)
+#pragma unroll
+			for (int fb = 0; fb < 3; fb++) {
+				const N n = cnt(0, fb + 3 * err + 6 * ended);
+				const double d0 = fb == 1 ? 1.0 : (fb == 2 ? -1.0 : 0.0);
+				const double d1 = fb == 1 ? 1.0 : (err ? -0.5 : (ended ? 0.8 : 0.5));
+				s0 += (__int128)n * to_fx(d0);
+				s1 += (__int128)n * to_fx(d1);
+			}
+	const double lv_rel[4] = {1.0, -0.2, -0.5, -1.0}, lv_cnt[4] = {1.0, 0.3, -0.3, -0.8}, lv_dur[4] = {1.0, 0.5, 0.0, -0.5};
+	__int128 s3 = 0, s4 = 0, s5 = 0, s7 = 0, s8 = 0, s6 = 0;
+	N n3 = 0, n5 = 0, n6 = 0, n7 = 0, n8 = 0;
+#pragma unroll
+	for (int k = 0; k < 4; k++) {
+		const N a3 = cnt(3, k), a4 = cnt(4, k), a5 = cnt(5, k);
+		const N a7 = cnt(7, k), a8 = cnt(8, k);
+		s3 += (__int128)a3 * to_fx(lv_rel[k]); s4 += (__int128)a4 * to_fx(lv_cnt[k]); s5 += (__int128)a5 * to_fx(lv_dur[k]);
+		s7 += (__int128)a7 * to_fx(lv_dur[k]); s8 += (__int128)a8 * to_fx(lv_cnt[k]);
+		n3 += a3; n5 += a5; n7 += a7; n8 += a8;
+	}
+#pragma unroll
+	for (int k = 0; k < 6; k++) {                                                    // TCS:735: max(-1, 1 - k*0.4)
+		const N a6 = cnt(6, k);
+		double ef = __dadd_rn(1.0, -__dmul_rn((double)k, 0.4));
+		ef = ef < -1.0 ? -1.0 : ef;
+		s6 += (__int128)a6 * to_fx(ef);
+		n6 += a6;
+	}
+	if (writer) {
+		const __int128 sums[APO_NDIM] = {s0, s1, 0, s3, s4, s5, s6, s7, s8};
+		const N cnts[APO_NDIM] = {nv, nv, n3, n3, n3, n5, n6, n7, n8};                   // d2,d3,d4 are pushed together (TCS:695)
+#pragma unroll
+		for (int i = 0; i < APO_NDIM; i++) {
+			if (i != 2) add_i128(corp + CORP_DIM + 4 * i, sums[i]);
+			if (cnts[i]) atomicAdd((unsigned long long *)corp + CORP_DIM + 4 * i + 3, (unsigned long long)cnts[i]);
+		}
+		if (nv) atomicAdd((unsigned long long *)corp + CORP_REWARD + 3, (unsigned long long)nv);
 	}
 }
 
@@ -139,49 +220,19 @@ __device__ __forceinline__ void scan_flush(const ScanAcc &A, long long *corp, in
 		flush_acc128(b, corp + CORP_DIM + 4 * 2, lane);
 	}
 	const uint32_t nv = warp_sum_u32(A.nValid);
-	// d0 / d1 from the (feedback, hasErrors, endTime) census: TCS:677-691
-	__int128 s0 = 0, s1 = 0;
-#pragma unroll
-	for (int ended = 0; ended < 2; ended++)
-#pragma unroll
-		for (int err = 0; err < 2; err++)
-#pragma unroll
-			for (int fb = 0; fb < 3; fb++) {
-				const uint32_t n = field_sum<10>(ended ? A.c01b : A.c01a, fb + 3 * err);
-				const double d0 = fb == 1 ? 1.0 : (fb == 2 ? -1.0 : 0.0);
-				const double d1 = fb == 1 ? 1.0 : (err ? -0.5 : (ended ? 0.8 : 0.5));
-				s0 += (__int128)n * to_fx(d0);
-				s1 += (__int128)n * to_fx(d1);
-			}
-	const double lv_rel[4] = {1.0, -0.2, -0.5, -1.0}, lv_cnt[4] = {1.0, 0.3, -0.3, -0.8}, lv_dur[4] = {1.0, 0.5, 0.0, -0.5};
-	__int128 s3 = 0, s4 = 0, s5 = 0, s7 = 0, s8 = 0, s6 = 0;
-	uint32_t n3 = 0, n5 = 0, n6 = 0, n7 = 0, n8 = 0;
-#pragma unroll
-	for (int k = 0; k < 4; k++) {
-		const uint32_t a3 = field_sum<12>(A.c3, k), a4 = field_sum<12>(A.c4, k), a5 = field_sum<12>(A.c5, k);
-		const uint32_t a7 = field_sum<12>(A.c7, k), a8 = field_sum<12>(A.c8, k);
-		s3 += (__int128)a3 * to_fx(lv_rel[k]); s4 += (__int128)a4 * to_fx(lv_cnt[k]); s5 += (__int128)a5 * to_fx(lv_dur[k]);
-		s7 += (__int128)a7 * to_fx(lv_dur[k]); s8 += (__int128)a8 * to_fx(lv_cnt[k]);
-		n3 += a3; n5 += a5; n7 += a7; n8 += a8;
-	}
-#pragma unroll
-	for (int k = 0; k < 6; k++) {                                                    // TCS:735: max(-1, 1 - k*0.4)
-		const uint32_t a6 = field_sum<9>(A.c6, k);
-		double ef = __dadd_rn(1.0, -__dmul_rn((double)k, 0.4));
-		ef = ef < -1.0 ? -1.0 : ef;
-		s6 += (__int128)a6 * to_fx(ef);
-		n6 += a6;
-	}
-	if (lane == 0) {
-		const __int128 sums[APO_NDIM] = {s0, s1, 0, s3, s4, s5, s6, s7, s8};
-		const uint32_t cnts[APO_NDIM] = {nv, nv, n3, n3, n3, n5, n6, n7, n8};            // d2,d3,d4 are pushed together (TCS:695)
-#pragma unroll
-		for (int i = 0; i < APO_NDIM; i++) {
-			if (i != 2) add_i128(corp + CORP_DIM + 4 * i, sums[i]);
-			if (cnts[i]) atomicAdd((unsigned long long *)corp + CORP_DIM + 4 * i + 3, (unsigned long long)cnts[i]);
-		}
-		if (nv) atomicAdd((unsigned long long *)corp + CORP_REWARD + 3, (unsigned long long)nv);
-	}
+	census_flush(
+	    [&](int g, int k) -> uint32_t {
+		    switch (g) {
+		    case 0: return field_sum<10>(k >= 6 ? A.c01b : A.c01a, k % 6);
+		    case 3: return field_sum<12>(A.c3, k);
+		    case 4: return field_sum<12>(A.c4, k);
+		    case 5: return field_sum<12>(A.c5, k);
+		    case 6: return field_sum<9>(A.c6, k);
+		    case 7: return field_sum<12>(A.c7, k);
+		    default: return field_sum<12>(A.c8, k);
+		    }
+	    },
+	    nv, corp, lane == 0);
 }
 
 // One warp's share of the corpus: records t = first + lane, first + lane + stride, ...  All 32 lanes stay
@@ -251,6 +302,96 @@ __device__ __forceinline__ void corpus_tail(const K2Params &P, const unsigned lo
 	if (tid == 0) { corp[CORP_NREC] = (long long)P.T; *P.ticket = 0; }
 	__syncthreads();                                              // block-scope visibility is all the finalising CTA needs (it reads through L2)
 	if (P.fuse_finalize) finalize_and_publish(P.fin, s_scratch, scratch_keys);
+}
+
+// ---------------------------------------------------------------- the corpus digest pass (apo_kernels.h CorpusDigestParams)
+__device__ __forceinline__ CatIdx cd_key(const ulonglong2 &e) {
+	CatIdx ix;
+	const uint32_t s = (uint32_t)e.y;
+	ix.i01 = s & 15u; ix.i3 = (s >> 4) & 7u; ix.i4 = (s >> 7) & 7u; ix.i5 = (s >> 10) & 7u;
+	ix.i6 = (s >> 13) & 7u; ix.i7 = (s >> 16) & 7u; ix.i8 = (s >> 19) & 7u;
+	ix.d2 = __longlong_as_double((long long)e.x);
+	return ix;
+}
+
+// census counters of the digest pass: group g slot k (the slots census_flush asks for)
+__device__ __forceinline__ int cd_census(int g, int k) { return g == 0 ? k : g == 6 ? 24 + k : g < 6 ? 12 + 4 * (g - 3) + k : 30 + 4 * (g - 7) + k; }
+constexpr int CD_CENSUS = 38;
+// c into the 64-bit counter {lo, hi} of shared memory with native 32-bit adds (a 64-bit shared-memory add is a CAS loop, and
+// every entry of a CTA meets the same few counters): the low word's carry goes to the high word
+__device__ __forceinline__ void cd_add(uint32_t *lo, uint32_t *hi, unsigned long long c) {
+	const uint32_t l = (uint32_t)c, h = (uint32_t)(c >> 32);
+	const uint32_t carry = atomicAdd(lo, l) > 0xFFFFFFFFu - l ? 1u : 0u;
+	if (h + carry) atomicAdd(hi, h + carry);
+}
+
+// the block's census counters -> exact dimension sums (census_flush), by one thread; a call of its own keeps its 128-bit sums
+// out of the register budget of the kernels that run the pass (K1h: 64 registers)
+static __device__ __noinline__ void cd_census_flush(const uint32_t *s_lo, const uint32_t *s_hi, long long *corp) {
+	auto count = [&](int j) { return (unsigned long long)s_hi[j] << 32 | s_lo[j]; };
+	census_flush([&](int g, int k) { return count(cd_census(g, k)); }, count(CD_CENSUS), corp, true);
+}
+
+// One call's corpus words from the digest: each CTA takes a contiguous share of the entries and runs, per entry, what
+// scan_record runs per record (key_ws, key_reward), times the entry's count; CTA 0 adds the fixed words and seeds its example
+// slots; then the tail of the stand-alone scan (ticket, examples, the last CTA finalises when the call asks for it).  Run by
+// the stand-alone k_corpus_digest and, after its pairs, by every CTA of K1h (k_reward9th) on whole rows of the Form T copy.
+// Block-wide; every thread of every CTA of the launch must enter.  Works for any blockDim.x that is a multiple of 32 (<= 1024).
+// P.fixed == NULL: no corpus words (a call without a corpus report), only the tail.
+static __device__ __noinline__ void corpus_digest_block(const CorpusDigestParams &P) {
+	__shared__ unsigned long long s_ex[APO_NPAT * 3];
+	__shared__ double s_cat[CAT_WORDS];
+	__shared__ double2 s_lut[512];
+	__shared__ uint32_t s_lo[CD_CENSUS + 1], s_hi[CD_CENSUS + 1];   // + the counted records
+	__shared__ unsigned long long s_part[32][6];                   // per warp: the limb sums of the reward and of d2
+	__shared__ bool s_last;
+	const int tid = threadIdx.x, lane = tid & 31;
+	const K2Params &K = P.k2;
+	long long *corp = K.acc + (uint64_t)ACC_PER_CAND * K.C;
+	if (tid < APO_NPAT * 3) s_ex[tid] = blockIdx.x == 0 && P.fixed ? (unsigned long long)P.fixed[CD_FIXED + tid] : 0ull;
+	if (tid <= CD_CENSUS) { s_lo[tid] = 0u; s_hi[tid] = 0u; }
+	for (int i = tid; i < CAT_WORDS; i += blockDim.x) s_cat[i] = K.lut[1024 + i];
+	for (int i = tid; i < 512; i += blockDim.x) s_lut[i] = make_double2(K.lut[i], K.lut[512 + i]);
+	if (blockIdx.x == 0 && P.fixed && tid < CD_FIXED && P.fixed[tid]) atomicAdd((unsigned long long *)corp + CORP_TALLY + tid, (unsigned long long)P.fixed[tid]);
+	__syncthreads();
+	const double w2 = K.W.w[2];
+	const uint64_t n = P.fixed ? *P.n : 0, lo = n * blockIdx.x / gridDim.x, hi = n * (blockIdx.x + 1ull) / gridDim.x;
+	Acc128 R, D2; R.zero(); D2.zero();
+	for (uint64_t i = lo + tid; i < hi; i += blockDim.x) {
+		const ulonglong2 e = P.ent[i];
+		const CatIdx ix = cd_key(e);
+		const unsigned long long c = e.y >> CD_COUNT_SHIFT;
+		double ws;
+		const uint32_t mask = key_ws(ix, w2, s_cat, ws);
+		long long fx;
+		if (key_reward<false>(ws, mask, s_lut, fx)) {             // TCS:784 totalWeight > 0
+			acc_add_mul(R, c, fx);
+			acc_add_mul(D2, c, to_fx(ix.d2));                     // +0.0 when not pushed
+			auto add = [&](int j) { cd_add(&s_lo[j], &s_hi[j], c); };
+			add(CD_CENSUS);
+			add(cd_census(0, (int)ix.i01));
+			if (ix.i3 < 4u) { add(cd_census(3, (int)ix.i3)); add(cd_census(4, (int)ix.i4)); }
+			if (ix.i5 < 4u) add(cd_census(5, (int)ix.i5));
+			if (ix.i6 < 6u) add(cd_census(6, (int)ix.i6));
+			if (ix.i7 < 4u) add(cd_census(7, (int)ix.i7));
+			if (ix.i8 < 4u) add(cd_census(8, (int)ix.i8));
+		}
+	}
+	// the limbs are summed over the block first: one global atomic per limb and CTA (K1h runs this in 32 warps of every SM's
+	// CTA, and thousands of warps adding into the same six words serialise in L2)
+	const unsigned long long v[6] = {warp_sum_u64(R.lo & 0xffffffffull), warp_sum_u64(R.lo >> 32), warp_sum_u64((unsigned long long)R.hi),
+	                                 warp_sum_u64(D2.lo & 0xffffffffull), warp_sum_u64(D2.lo >> 32), warp_sum_u64((unsigned long long)D2.hi)};
+	if (lane == 0)
+		for (int k = 0; k < 6; k++) s_part[tid >> 5][k] = v[k];
+	__syncthreads();
+	if (tid >= 32 && tid < 38) {                                   // limb sums as flush_acc128 adds them (the high limb wraps as a signed sum)
+		const int k = tid - 32;
+		unsigned long long sum = 0;
+		for (int w = 0; w < (int)(blockDim.x >> 5); w++) sum += s_part[w][k];
+		if (sum) atomicAdd((unsigned long long *)corp + (k < 3 ? CORP_REWARD + k : CORP_DIM + 4 * 2 + k - 3), sum);
+	}
+	if (tid == 0) cd_census_flush(s_lo, s_hi, corp);
+	corpus_tail(K, s_ex, &s_last, reinterpret_cast<unsigned long long *>(s_lut), 1024u);   // the LUT (8 KB) is done with: scratch of the tail
 }
 
 __device__ __forceinline__ unsigned long long score_key(double s) {

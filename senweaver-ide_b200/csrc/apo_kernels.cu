@@ -513,6 +513,103 @@ cudaError_t run_finalize(const FinalizeParams &F, cudaStream_t st) {
 	return cudaGetLastError();
 }
 
+// =================================================================== corpus digest (apo_kernels.h)
+static_assert(CD_FIXED == CORP_NREC - CORP_TALLY, "the digest's fixed words are the corpus block's weight-independent ones");
+constexpr unsigned long long CD_EMPTY = ~0ull;   // never a key half: d2 is finite (never this NaN), the slots use 22 bits
+constexpr int CD_THREADS = 256;
+
+__device__ __forceinline__ uint32_t cd_slots(const CatIdx &ix) {
+	return ix.i01 | ix.i3 << 4 | ix.i4 << 7 | ix.i5 << 10 | ix.i6 << 13 | ix.i7 << 16 | ix.i8 << 19;
+}
+
+// {d2 bits, slots} -> its slot of the open-addressing table; claimed whole by one 128-bit CAS, so a key is never seen half written
+__device__ __forceinline__ void cd_insert(ulonglong2 *table, unsigned long long *cnt, uint32_t mask, ulonglong2 key, unsigned long long n,
+                                          uint64_t cap, unsigned long long *misc) {
+	uint32_t h = (uint32_t)mix64(key.x ^ mix64((unsigned long long)key.y + GOLD)) & mask;
+	for (uint32_t p = 0; p <= mask; p++) {
+		ulonglong2 cur;
+		asm volatile("ld.relaxed.gpu.global.v2.u64 {%0, %1}, [%2];" : "=l"(cur.x), "=l"(cur.y) : "l"(table + h));
+		if (cur.x == CD_EMPTY || cur.y == CD_EMPTY) {         // free, or being claimed: the CAS returns the slot as it is
+			cur = atomicCAS(table + h, make_ulonglong2(CD_EMPTY, CD_EMPTY), key);
+			if (cur.x == CD_EMPTY && cur.y == CD_EMPTY) {
+				if (atomicAdd(&misc[0], 1ull) + 1 > cap) atomicOr(&misc[1], 1ull);
+				cur = key;
+			}
+		}
+		if (cur.x == key.x && cur.y == key.y) { atomicAdd(cnt + h, n); return; }
+		h = (h + 1) & mask;
+	}
+	atomicOr(&misc[1], 1ull);                                   // the table is full: more than cap keys
+}
+
+__global__ void __launch_bounds__(CD_THREADS)
+k_cd_count(const apo_record *recs, uint64_t T, const double *cat, ulonglong2 *table, unsigned long long *cnt, uint32_t mask, uint64_t cap,
+           unsigned long long *misc) {
+	const uint32_t lane = threadIdx.x & 31;
+	const uint4 *src = reinterpret_cast<const uint4 *>(recs);
+	// the loop bound is warp-uniform (match.any and the early stop need every lane)
+	for (uint64_t t0 = (uint64_t)blockIdx.x * CD_THREADS + (threadIdx.x & ~31u); t0 < T; t0 += (uint64_t)gridDim.x * CD_THREADS) {
+		const unsigned long long stop = lane == 0 ? *(volatile unsigned long long *)&misc[1] : 0ull;
+		if (__any_sync(0xFFFFFFFFu, stop != 0ull)) break;   // more than cap keys: no digest
+		const uint64_t t = t0 + lane;
+		ulonglong2 key = make_ulonglong2(CD_EMPTY, CD_EMPTY);
+		if (t < T) {
+			union { uint4 q[2]; apo_record r; } u;
+			u.q[0] = __ldg(src + 2 * t); u.q[1] = __ldg(src + 2 * t + 1);
+			if (u.r.flags & APO_F_VALID) {
+				double ws; CatIdx ix;
+				record_ws_table_t<true, true>(u.r, 0.0, cat, ws, ix);     // the key alone: no weight enters it
+				key = make_ulonglong2((unsigned long long)__double_as_longlong(ix.d2), cd_slots(ix));
+			}
+		}
+		const uint32_t peers = __match_any_sync(0xFFFFFFFFu, key.x) & __match_any_sync(0xFFFFFFFFu, key.y);
+		if (key.x != CD_EMPTY && (uint32_t)(__ffs(peers) - 1) == lane) cd_insert(table, cnt, mask, key, (unsigned long long)__popc(peers), cap, misc);
+	}
+}
+
+__global__ void __launch_bounds__(CD_THREADS)
+k_cd_compact(const ulonglong2 *table, const unsigned long long *cnt, uint64_t slots, unsigned long long *misc, ulonglong2 *ent) {
+	if (*(volatile unsigned long long *)&misc[1]) return;
+	for (uint64_t i = (uint64_t)blockIdx.x * CD_THREADS + threadIdx.x; i < slots; i += (uint64_t)gridDim.x * CD_THREADS) {
+		const ulonglong2 k = table[i];
+		if (k.x == CD_EMPTY) continue;
+		const unsigned long long o = atomicAdd(&misc[2], 1ull);
+		ent[o] = make_ulonglong2(k.x, k.y | cnt[i] << CD_COUNT_SHIFT);
+	}
+}
+
+__global__ void __launch_bounds__(CD_THREADS)
+k_cd_clear(ulonglong2 *table, unsigned long long *cnt, uint64_t slots, unsigned long long *misc) {
+	for (uint64_t i = (uint64_t)blockIdx.x * CD_THREADS + threadIdx.x; i < slots; i += (uint64_t)gridDim.x * CD_THREADS) {
+		table[i] = make_ulonglong2(CD_EMPTY, CD_EMPTY);
+		cnt[i] = 0ull;
+	}
+	if (blockIdx.x == 0 && threadIdx.x < 3) misc[threadIdx.x] = 0ull;
+}
+
+cudaError_t run_cd_build(const apo_record *recs, uint64_t T, const double *lut, ulonglong2 *table, unsigned long long *cnt, uint64_t slots,
+                         uint64_t cap, unsigned long long *misc, ulonglong2 *ent, int sm_count, cudaStream_t st) {
+	const int grid = sm_count * 8;
+	k_cd_clear<<<grid, CD_THREADS, 0, st>>>(table, cnt, slots, misc);
+	k_cd_count<<<grid, CD_THREADS, 0, st>>>(recs, T, lut + 1024, table, cnt, (uint32_t)(slots - 1), cap, misc);
+	k_cd_compact<<<grid, CD_THREADS, 0, st>>>(table, cnt, slots, misc, ent);
+	return cudaGetLastError();
+}
+
+// One call's corpus words from the digest, then the tail (apo_corpus.cuh corpus_digest_block).
+__global__ void __launch_bounds__(CD_THREADS)
+k_corpus_digest(const __grid_constant__ CorpusDigestParams P) {      // grid constant: the pass reads P in place, no per-thread copy
+	corpus_digest_block(P);
+}
+
+cudaError_t run_corpus_digest(const CorpusDigestParams &P, uint64_t n_host, int sm_count, cudaStream_t st) {
+	uint64_t want = (n_host + 4 * CD_THREADS - 1) / (4 * CD_THREADS);    // about four entries per thread
+	int grid = sm_count;
+	if ((uint64_t)grid > want) grid = (int)(want ? want : 1);
+	k_corpus_digest<<<grid, CD_THREADS, 0, st>>>(P);
+	return cudaGetLastError();
+}
+
 // =================================================================== generators / single-trace path
 __global__ void __launch_bounds__(256)
 k_gen_dims(float *out, uint64_t pitch_evals, unsigned long long seed, uint32_t c0, uint32_t C, uint64_t t0, uint64_t T,

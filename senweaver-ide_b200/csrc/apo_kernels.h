@@ -246,6 +246,29 @@ cudaError_t run_tuple_slots(const long long *tval, uint32_t h, uint32_t end, lon
 cudaError_t run_slot_plane(const unsigned short *tl, const unsigned char *th, uint64_t tpitch, uint32_t C, uint64_t T, uint32_t h,
                            uint32_t end, unsigned short *ts, cudaStream_t st);
 
+// ---- corpus digest (apo_kernels.cu): what a scoring call's corpus report needs from a large resident corpus, built at load.
+// Only a VALID record's reward key (its categorical slots and d2: CatIdx) reaches the weight-dependent words of the report, so
+// those are sums over the distinct keys with their record counts; every other word does not depend on the weights at all.
+// Entry = {d2 bit pattern, slots | count << CD_COUNT_SHIFT}, slots = i01 | i3 << 4 | i4 << 7 | i5 << 10 | i6 << 13 | i7 << 16
+// | i8 << 19.  fixed: the corpus-block words [CORP_TALLY, CORP_NREC) (tallies, byMode, patterns, tool totals) followed by the
+// 18 first-three slots (inverted indices, as ex_insert keeps them) of the load-time scan.
+constexpr int CD_COUNT_SHIFT = 22;
+constexpr int CD_FIXED = 27;                 // CORP_NREC - CORP_TALLY
+constexpr int CD_WORDS = CD_FIXED + 18;
+struct CorpusDigestParams {
+	const ulonglong2 *ent;                   // [*n]
+	const unsigned long long *n;             // entry count
+	const long long *fixed;                  // [CD_WORDS]
+	K2Params k2;                             // block, example scratch, ticket, tables, weights and tail of the call (recs unused)
+};
+// the keys of recs[0, T) into table {key} / cnt [slots] (cleared first); misc[0] = keys inserted, misc[1] = 1 once that exceeds
+// cap (the pass then stops early), then the entries into ent [cap] and their number into misc[2] (none when misc[1] is set)
+cudaError_t run_cd_build(const apo_record *recs, uint64_t T, const double *lut, ulonglong2 *table, unsigned long long *cnt, uint64_t slots,
+                         uint64_t cap, unsigned long long *misc, ulonglong2 *ent, int sm_count, cudaStream_t st);
+// the corpus words of one scoring call from the digest, then the tail (corpus_tail) as the stand-alone scan runs it; n_host:
+// the entry count, sizes the grid
+cudaError_t run_corpus_digest(const CorpusDigestParams &P, uint64_t n_host, int sm_count, cudaStream_t st);
+
 // K1h (k_reward9th): whole rows of the Form T copy from per-row dictionary counts.  A row's score needs only how often each
 // entry occurs in it: sum_t table[idx(c, t)] = sum_e count[c][e] * table[e], the same integer.  Per row c, pairs
 // [off[c], off[c + 1]) hold its entries that occur (t < T only), ascending, as entry | count << KH_COUNT_SHIFT.  The bytes
@@ -258,6 +281,8 @@ struct KhParams {
 	uint64_t nnz;
 	long long *acc;
 	const long long *tval;            // [n_tuples + 1] the table in entry order
+	int corpus_on;                    // every CTA then runs the digest pass over its share of cd's entries and the tail
+	CorpusDigestParams cd;            // (cd.fixed NULL: the tail alone, for a call without a corpus report)
 };
 cudaError_t run_reward9th(const KhParams &P, int sm_count, cudaStream_t st);
 // The counts of rows [0, R) of tl / th [R][tpitch] (evaluations t < T) into cnt [R][npitch] (npitch a multiple of 32, zeroed

@@ -13,6 +13,7 @@
 // K1t then is a gather-and-add: the hot head of the table in shared memory, the tail through L1/L2.
 #include <cstdlib>
 #include "apo_device.cuh"
+#include "apo_corpus.cuh"
 #include "apo_kernels.h"
 
 namespace apo {
@@ -371,19 +372,8 @@ cudaError_t run_reward9t2(Kt2Params P, int sm_count, cudaStream_t st) {
 constexpr int KH_THREADS = 1024;
 constexpr int KH_UNROLL = 8;                      // pairs in flight per thread
 
-// acc += n * v, exactly: n < 2^44, |v| < 2^53
-__device__ __forceinline__ void acc_add_mul(Acc128 &a, unsigned long long n, long long v) {
-	unsigned long long lo;
-	long long hi;
-	asm("mul.lo.u64 %0, %2, %3;\n\tmul.hi.s64 %1, %2, %3;" : "=l"(lo), "=l"(hi) : "l"(v), "l"((long long)n));
-	asm("add.cc.u64 %0, %0, %2;\n\taddc.s64 %1, %1, %3;" : "+l"(a.lo), "+l"(a.hi) : "l"(lo), "l"(hi));
-}
-
-__global__ void __launch_bounds__(KH_THREADS, 1)
-k_reward9th(const KhParams P) {
-	const int tid = threadIdx.x, lane = tid & 31;
-	const uint64_t lo = P.nnz * blockIdx.x / gridDim.x, hi = P.nnz * (blockIdx.x + 1ull) / gridDim.x;
-	if (lo >= hi) return;
+// the rows of pairs [lo, hi) of one CTA
+__device__ __forceinline__ void kh_rows(const KhParams &P, uint64_t lo, uint64_t hi, int tid, int lane) {
 	uint32_t a = 0, b = P.C;                                       // off[a] <= lo < off[b]
 	while (b - a > 1) {
 		const uint32_t m = (a + b) / 2;
@@ -420,12 +410,21 @@ k_reward9th(const KhParams P) {
 	}
 }
 
+__global__ void __launch_bounds__(KH_THREADS, 1)
+k_reward9th(const __grid_constant__ KhParams P) {      // grid constant: the digest pass reads P.cd in place, no per-thread copy
+	const int tid = threadIdx.x, lane = tid & 31;
+	const uint64_t lo = P.nnz * blockIdx.x / gridDim.x, hi = P.nnz * (blockIdx.x + 1ull) / gridDim.x;
+	if (lo < hi) kh_rows(P, lo, hi, tid, lane);
+	if (P.corpus_on) corpus_digest_block(P.cd);                       // every CTA, with or without pairs: block-wide
+}
+
 cudaError_t run_reward9th(const KhParams &P, int sm_count, cudaStream_t st) {
-	if (P.nnz == 0) return cudaSuccess;
+	if (P.nnz == 0 && !P.corpus_on) return cudaSuccess;
 	int grid = sm_count;
 	if (k1_env_grid() > 0 && k1_env_grid() < grid) grid = k1_env_grid();   // tests: every CTA cut of the rows
 	const uint64_t need = (P.nnz + KH_THREADS - 1) / KH_THREADS;
 	if ((uint64_t)grid > need) grid = (int)need;
+	if (grid < 1) grid = 1;                                                  // no pairs: one CTA for the corpus words and the tail
 	k_reward9th<<<grid, KH_THREADS, 0, st>>>(P);
 	return cudaGetLastError();
 }

@@ -23,6 +23,7 @@ SCORE_CORPUS, SCORE_RECIP, SCORE_TIMING, SCORE_CANDIDATES = 0x1, 0x2, 0x4, 0x8
 SCORE_CANDIDATE_CORPUS = 0x10
 TUNE_NO_FUSE, TUNE_FORCE_FUSE, TUNE_NO_STAGING, TUNE_NCCL_JOIN, TUNE_NO_TWIN = 0x1, 0x2, 0x4, 0x8, 0x10
 TUNE_NO_TWIN_T, TUNE_TWIN_T, TUNE_NO_TWIN_T2, TUNE_NO_TWIN_H = 0x20, 0x40, 0x80, 0x100
+TUNE_NO_CORPUS_DIGEST = 0x200
 F_ERRORS, F_ENDED, F_VALID, F_FAILSPAN = 0x01, 0x02, 0x08, 0x10
 UNIQUE_ID_BYTES = 128
 
@@ -103,7 +104,7 @@ ABI_SYMBOLS = (
     "apo_dims_compact_download", "apo_dims_codebook", "apo_packed_encode_host", "apo_score_host_packed", "apo_dims_packed_download", "apo_dims_d2book",
     "apo_tuple_encode_host", "apo_score_host_tuples", "apo_tuples_upload", "apo_dims_tuples", "apo_tuples_download", "apo_tuples_book",
     "apo_host_alloc", "apo_host_free",
-    "apo_last_timing", "apo_debug_partials", "apo_debug_twin_t_list", "apo_debug_twin_h", "apo_candidate_reports", "apo_candidate_corpus_reports", "apo_comm_unique_id", "apo_comm_init", "apo_comm_destroy", "apo_comm_join_mode",
+    "apo_last_timing", "apo_debug_partials", "apo_debug_twin_t_list", "apo_debug_twin_h", "apo_debug_corpus_digest", "apo_candidate_reports", "apo_candidate_corpus_reports", "apo_comm_unique_id", "apo_comm_init", "apo_comm_destroy", "apo_comm_join_mode",
 )
 
 
@@ -190,6 +191,7 @@ def load_library() -> C.CDLL:
     L.apo_debug_partials.argtypes = [vp, vp, u32]
     L.apo_debug_twin_t_list.argtypes = [vp, vp, vp, vp, vp]
     L.apo_debug_twin_h.argtypes = [vp, vp, vp, vp, vp]
+    L.apo_debug_corpus_digest.argtypes = [vp, vp, vp, vp]
     L.apo_candidate_reports.argtypes = [vp, u32, u32, vp]
     L.apo_candidate_corpus_reports.argtypes = [vp, u32, u32, vp]
     L.apo_comm_unique_id.argtypes = [vp]
@@ -646,6 +648,19 @@ class Engine:
         pairs = np.empty(nh.value, np.uint64)
         self._ck(self._L.apo_debug_twin_h(self._h, C.byref(rows), C.byref(nh), _p(off), _p(pairs)))
         return off, pairs
+
+    def debug_corpus_digest(self):
+        """The corpus digest: (entries [n][2] uint64 {d2 bits, slots | count << 22}, fixed [45] int64: the tallies, byMode,
+        pattern and tool words of the corpus block, then the 18 first-three slots as inverted indices), or None when none
+        is held."""
+        n = C.c_uint64(0)
+        self._ck(self._L.apo_debug_corpus_digest(self._h, C.byref(n), None, None))
+        if n.value == 0:
+            return None
+        ent = np.empty((n.value, 2), np.uint64)
+        fixed = np.empty(45, np.int64)
+        self._ck(self._L.apo_debug_corpus_digest(self._h, C.byref(n), _p(ent), _p(fixed)))
+        return ent, fixed
 
     # -- multi-GPU
     @staticmethod
