@@ -8,7 +8,13 @@ reports (APO_SCORE_CANDIDATE_CORPUS), alternating plain / candidates / candidate
 corpus report of the same 8 candidates against the CPU oracle's report of their generated rows (integers, flags, examples
 and severities exactly; binary64 sums to 1e-12, the oracle merging per-thread slices).
 
-    python examples/candidates_cost.py [--steps 10] [--legs D,Q,T,R16,R] [--out FILE.json]
+Every leg also times the step with the per-candidate extremes (APO_SCORE_CANDIDATE_EXTREMES) in the same alternation.  On the
+fp32 legs its parity block is the lists of two of the 8 candidates against the model of tests/extremes_fixtures.py over the
+generated rows (positions and rewards bit for bit); on the rollout legs every list holds min(32, counts[c]) entries and R16
+and R give the same bytes.  Leg W is Form D through its Form W copy (the Form T copy held beside it is switched off), leg
+FALL is 64 x 1 M strictly falling rows through K1, where every group of 32 evaluations runs the extremes' merge network.
+
+    python examples/candidates_cost.py [--steps 10] [--legs D,W,Q,T,R16,R,FALL] [--out FILE.json]
 
 Prints one JSON object; the card name and power limit are read in the same run (nvidia-smi query)."""
 import argparse
@@ -23,6 +29,7 @@ import numpy as np
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
+sys.path.insert(0, os.path.join(ROOT, "tests"))
 
 
 def card():
@@ -50,20 +57,49 @@ def same(r, d):
     return list(r.badExamples) == d["badExamples"]
 
 
-def leg(eng, C, K, steps, score_kw, ref, picks):
-    plain, flagged = [], []
-    for _ in range(2):                                          # warm both shapes
-        eng.score(C, K, **score_kw)
-        eng.score(C, K, candidates=True, **score_kw)
-    for _ in range(steps):                                      # alternate: drift and other tenants hit both alike
-        t0 = time.perf_counter(); eng.score(C, K, **score_kw); plain.append(time.perf_counter() - t0)
-        t0 = time.perf_counter(); r = eng.score(C, K, candidates=True, **score_kw); flagged.append(time.perf_counter() - t0)
-    ok = [same(r.candidates[c], d) for c, d in zip(picks, ref)]
-    med_p, med_f = float(np.median(plain)) * 1e3, float(np.median(flagged)) * 1e3
-    return {"plain_ms_median": round(med_p, 3), "flagged_ms_median": round(med_f, 3), "ratio": round(med_f / med_p, 3),
-            "plain_ms_min": round(min(plain) * 1e3, 3), "flagged_ms_min": round(min(flagged) * 1e3, 3),
-            "parity": {"candidates": picks, "equal": all(ok), "per_candidate": ok,
-                       "bad_examples": [list(r.candidates[c].badExamples) for c in picks]}}
+def lists(x):
+    return (int(x.n), list(x.lowest), list(x.highest), np.array(x.lowestReward).tobytes(), np.array(x.highestReward).tobytes())
+
+
+def model_lists(m):
+    return (m["n"], m["lowest"], m["highest"], np.array(m["lowestReward"]).tobytes(), np.array(m["highestReward"]).tobytes())
+
+
+def extremes_parity(res, ref_ext):
+    """ref_ext: {candidate: model lists}; without models, every list holds min(32, counts[c]) entries"""
+    if ref_ext is None:
+        return {"equal": all(int(x.n) == min(32, int(n)) for x, n in zip(res.extremes, res.counts)), "check": "n == min(32, counts)"}
+    ok = {c: lists(res.extremes[c]) == model_lists(m) for c, m in ref_ext.items()}
+    return {"candidates": list(ok), "equal": all(ok.values())}
+
+
+def leg(eng, C, K, steps, score_kw, ref, picks, ref_ext=None):
+    """plain / candidates / extremes steps, alternating (ref None: the breakdown is not timed)"""
+    kinds = {"plain": {}, "extremes": {"extremes": True}}
+    if ref is not None:
+        kinds["candidates"] = {"candidates": True}
+    times = {k: [] for k in kinds}
+    for _ in range(2):                                          # warm every shape
+        for kw in kinds.values():
+            eng.score(C, K, **kw, **score_kw)
+    last = {}
+    for _ in range(steps):                                      # alternate: drift and other tenants hit all alike
+        for k, kw in kinds.items():
+            t0 = time.perf_counter(); last[k] = eng.score(C, K, **kw, **score_kw); times[k].append(time.perf_counter() - t0)
+    med = {k: float(np.median(v)) * 1e3 for k, v in times.items()}
+    out = {"plain_ms_median": round(med["plain"], 3), "extremes_ms_median": round(med["extremes"], 3),
+           "extremes_ratio": round(med["extremes"] / med["plain"], 3), "min_ms": {k: round(min(v) * 1e3, 3) for k, v in times.items()},
+           "launches": {k: int(r.timing.launches) for k, r in last.items()},
+           "same_scores": last["extremes"].scores.tobytes() == last["plain"].scores.tobytes()
+                          and last["extremes"].topk.tobytes() == last["plain"].topk.tobytes(),
+           "parity_extremes": extremes_parity(last["extremes"], ref_ext)}
+    if ref is not None:
+        r = last["candidates"]
+        ok = [same(r.candidates[c], d) for c, d in zip(picks, ref)]
+        out.update({"flagged_ms_median": round(med["candidates"], 3), "ratio": round(med["candidates"] / med["plain"], 3),
+                    "parity": {"candidates": picks, "equal": all(ok), "per_candidate": ok,
+                               "bad_examples": [list(r.candidates[c].badExamples) for c in picks]}})
+    return out
 
 
 def same_corpus(r, ref):
@@ -88,8 +124,8 @@ def same_corpus(r, ref):
 
 
 def corpus_leg(eng, C, K, steps, score_kw, ref, picks, ref_corpus):
-    """plain / candidates / candidate_corpus steps, alternating, with both parity blocks"""
-    kinds = {"plain": {}, "candidates": {"candidates": True}, "candidate_corpus": {"candidate_corpus": True}}
+    """plain / candidates / candidate_corpus / extremes steps, alternating, with the parity blocks"""
+    kinds = {"plain": {}, "candidates": {"candidates": True}, "candidate_corpus": {"candidate_corpus": True}, "extremes": {"extremes": True}}
     times = {k: [] for k in kinds}
     for _ in range(2):                                          # warm every shape
         for kw in kinds.values():
@@ -106,6 +142,8 @@ def corpus_leg(eng, C, K, steps, score_kw, ref, picks, ref_corpus):
             "candidate_corpus_ms_median": round(med["candidate_corpus"], 3),
             "candidates_ratio": round(med["candidates"] / med["plain"], 3),
             "candidate_corpus_ratio": round(med["candidate_corpus"] / med["plain"], 3),
+            "extremes_ms_median": round(med["extremes"], 3), "extremes_ratio": round(med["extremes"] / med["plain"], 3),
+            "parity_extremes": extremes_parity(last["extremes"], None), "extremes_bytes": bytes(last["extremes"].extremes),
             "min_ms": {k: round(min(v) * 1e3, 3) for k, v in times.items()},
             "parity": {"candidates": picks, "equal": all(ok), "per_candidate": ok},
             "parity_corpus": {"candidates": picks, "equal": all(ok_c), "per_candidate": ok_c,
@@ -122,6 +160,7 @@ def main():
     pkg = importlib.import_module("senweaver-ide_b200")
     import oracle
     from oracle import candidates as oc
+    import extremes_fixtures as xf
     legs = args.legs.split(",")
     out = {"card": card(), "steps": args.steps, "timing": "host clock around each synchronous apo_score call"}
     eng = pkg.Engine(0)
@@ -129,15 +168,21 @@ def main():
     picks = [int(x) for x in np.linspace(0, C - 1, 8).round()]
     nth = max(1, min(32, os.cpu_count() or 1))
     try:
-        if {"D", "Q", "T"} & set(legs):
+        if {"D", "W", "Q", "T"} & set(legs):
             ref = oc.cand_generated(seed, picks, 0, T, 300, nthreads=nth)
+            ref_ext = {c: xf.model(oracle.gen_dims(seed, c, 1, 0, T, 300, nth))[0] for c in (picks[0], picks[-1])}
             if "D" in legs:
                 eng.dims_generate(seed, 0, C, 0, T, 300)
-                out["form_d_256x5M"] = leg(eng, C, K, args.steps, {}, ref, picks)
+                out["form_d_256x5M"] = leg(eng, C, K, args.steps, {}, ref, picks, ref_ext)
+            if "W" in legs:
+                eng.dims_generate(seed, 0, C, 0, T, 300)
+                eng.set_tuning(pkg.TUNE_NO_TWIN_T)
+                out["form_w_copy_256x5M"] = leg(eng, C, K, args.steps, {}, ref, picks, ref_ext)
+                eng.set_tuning(0)
             if "Q" in legs or "T" in legs:
                 eng.dims_generate_compact(seed, 0, C, 0, T, 300)
             if "Q" in legs:
-                out["form_q_256x5M"] = leg(eng, C, K, args.steps, {}, ref, picks)
+                out["form_q_256x5M"] = leg(eng, C, K, args.steps, {}, ref, picks, ref_ext)
             if "T" in legs:
                 pc, pd = np.empty((C, T), np.uint32), np.empty((C, T), np.uint16)
                 for c in range(C):
@@ -147,7 +192,7 @@ def main():
                 del pc, pd
                 eng.tuples_upload(tl, th, tbook, book, d2book)
                 del tl, th
-                out["form_t_256x5M"] = leg(eng, C, K, args.steps, {"source": pkg.SRC_TUPLES}, ref, picks)
+                out["form_t_256x5M"] = leg(eng, C, K, args.steps, {"source": pkg.SRC_TUPLES}, ref, picks, ref_ext)
         if {"R16", "R"} & set(legs):
             Cr = 128
             picks_r = [int(x) for x in np.linspace(0, Cr - 1, 8).round()]
@@ -159,6 +204,18 @@ def main():
             if "R" in legs:
                 eng.rollouts_generate(seed, 0, Cr, 0, T, 300)
                 out["form_r_128x5M"] = corpus_leg(eng, Cr, K, args.steps, {"source": pkg.SRC_ROLLOUTS}, ref_r, picks_r, ref_rc)
+            if "R16" in legs and "R" in legs:                   # the same rollouts: the same lists
+                out["r16_r_extremes_equal"] = out["form_r16_128x5M"]["extremes_bytes"] == out["form_r_128x5M"]["extremes_bytes"]
+            for k in ("form_r16_128x5M", "form_r_128x5M"):
+                out.get(k, {}).pop("extremes_bytes", None)
+        if "FALL" in legs:
+            Cf, Tf = 64, 1_000_000
+            d = xf.falling(Tf, 1)
+            m = xf.model(d)[0]
+            eng.dims_upload(np.repeat(d, Cf, axis=0))
+            eng.set_tuning(pkg.TUNE_NO_TWIN)
+            out["falling_rows_k1_64x1M"] = leg(eng, Cf, K, args.steps, {}, None, None, {0: m, Cf - 1: m})
+            eng.set_tuning(0)
     finally:
         eng.close()
     out["card_after"] = card()

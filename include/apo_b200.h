@@ -271,6 +271,7 @@ int apo_record_unpack16(const apo_record16 *in, uint64_t n, apo_record *out);
 #define APO_SCORE_TIMING  0x4u   /* record the per-stage CUDA events of apo_timing also for a small call */
 #define APO_SCORE_CANDIDATES 0x8u /* also build the per-candidate breakdown (apo_candidate_reports) */
 #define APO_SCORE_CANDIDATE_CORPUS 0x10u /* also build the corpus report of every candidate's rollout records (apo_candidate_corpus_reports) */
+#define APO_SCORE_CANDIDATE_EXTREMES 0x20u /* also list the 32 lowest- and highest-reward evaluations of every candidate (apo_candidate_extremes) */
 typedef struct apo_score_opts {
 	uint32_t K;          /* beam width (top-K), 0..min(C, 16384) */
 	uint32_t source;     /* APO_SRC_* */
@@ -448,6 +449,33 @@ int apo_candidate_reports(apo_engine *e, uint32_t c0, uint32_t n, apo_candidate_
  * Reports of candidates [c0, c0 + n) of the last scoring call: APO_E_STATE when that call did not set the flag (or failed),
  * APO_E_ARG when the range exceeds its C. */
 int apo_candidate_corpus_reports(apo_engine *e, uint32_t c0, uint32_t n, apo_corpus_report *out);
+/* Per-candidate extremes: the evaluations candidate c did worst and best on, for the critique step of the beam loop.
+ * Built by a scoring call that sets APO_SCORE_CANDIDATE_EXTREMES (independent of APO_SCORE_CANDIDATES and
+ * APO_SCORE_CANDIDATE_CORPUS; any combination may be set): apo_score on every source (Form D and each of its copies, Form Q,
+ * resident Form T, Form R / R16), apo_score_finish (every apo_score_accumulate of the session must set it too, APO_E_STATE
+ * otherwise) and every apo_score_host*.  Over the evaluations of c that the call scored with a non-null finalReward:
+ *   lowest:  finalReward ascending, ties -> lower record position;
+ *   highest: finalReward descending, ties -> lower record position.
+ * Each reward is, bit for bit, the binary64 finalReward whose rint(fr * 2^52) the call summed into scores[c] (with
+ * APO_SCORE_RECIP ws * RN(1/tw), as the scoring kernels compute it), a zero reported as +0.0; order is by numeric value.  Null
+ * evaluations never appear (total weight 0, or for records a missing VALID flag).  Positions are absolute record positions, as
+ * badExamples: they include the window's first, a session covers the union of its windows in whatever order they arrive, a
+ * chunk of candidates accumulated at cand_offset lists candidate cand_offset + c, and the host-streaming calls give positions
+ * within the call's T.  A session that accumulates the same window twice lists its evaluations twice, as its sums count them
+ * twice.  Scores, counts, top-K and the reports are those of the same call without the flag.  Single rank only, as the
+ * breakdown (APO_E_STATE on a handle with more than one rank).
+ * Lists of candidates [c0, c0 + n) of the last scoring call: APO_E_STATE when that call did not set the flag (or failed),
+ * APO_E_ARG when the range exceeds its C. */
+#define APO_EXTREMES_N 32
+/* A struct tag without a typedef, as struct stat beside stat(): the getter carries the same name. */
+struct apo_candidate_extremes {
+	uint64_t n;                              /* filled slots of each list: min(32, counts[c]) */
+	int64_t  lowest[APO_EXTREMES_N];         /* record positions; -1 past n */
+	double   lowestReward[APO_EXTREMES_N];   /* NaN past n */
+	int64_t  highest[APO_EXTREMES_N];
+	double   highestReward[APO_EXTREMES_N];
+};                                          /* 1032 bytes */
+int apo_candidate_extremes(apo_engine *e, uint32_t c0, uint32_t n, struct apo_candidate_extremes *out);
 
 /* ---- multi-GPU: the record axis is sharded across ranks (one process per GPU, or one handle per GPU inside one
  * process); the packed int64 partial vectors of the shards are joined INSIDE the scoring launch: the finalising CTA

@@ -128,6 +128,14 @@ int apo_job_validate(apo_job *j)
 		if (!fits(j->C, sizeof(apo_corpus_report), 1, APO_JOB_CANDIDATE_CORPUS_MAX_BYTES))
 			return bad(j, "the per-candidate corpus reports of C candidates exceed 4 GiB");
 	}
+	if (j->flags & APO_SCORE_CANDIDATE_EXTREMES) {
+		if (j->kind != APO_JOB_SCORE_RESIDENT && j->kind != APO_JOB_SCORE_HOST && j->kind != APO_JOB_SCORE_HOST_RECORDS &&
+		    j->kind != APO_JOB_SCORE_HOST_TUPLES)
+			return bad(j, "the per-candidate extremes belong to a scoring call");
+		if (j->C == 0) return bad(j, "C must be > 0 for the per-candidate extremes");
+		if (!fits(j->C, sizeof(struct apo_candidate_extremes), 1, APO_JOB_CANDIDATE_EXTREMES_MAX_BYTES))
+			return bad(j, "the per-candidate extremes of C candidates exceed 4 GiB");
+	}
 	return APO_OK;
 }
 
@@ -140,8 +148,11 @@ int apo_job_prepare(apo_job *j)
 		j->scores = (double *)malloc(8u * (size_t)C); j->counts = (uint64_t *)malloc(8u * (size_t)C); j->topk = (int32_t *)malloc(4u * (size_t)K);
 		if (j->flags & APO_SCORE_CANDIDATES) j->candidates = (apo_candidate_report *)malloc(sizeof(apo_candidate_report) * (size_t)C);
 		if (j->flags & APO_SCORE_CANDIDATE_CORPUS) j->candidate_corpus = (apo_corpus_report *)malloc(sizeof(apo_corpus_report) * (size_t)C);
+		if (j->flags & APO_SCORE_CANDIDATE_EXTREMES)
+			j->candidate_extremes = (struct apo_candidate_extremes *)malloc(sizeof(struct apo_candidate_extremes) * (size_t)C);
 		if (!j->scores || !j->counts || !j->topk || ((j->flags & APO_SCORE_CANDIDATES) && !j->candidates) ||
-		    ((j->flags & APO_SCORE_CANDIDATE_CORPUS) && !j->candidate_corpus)) {
+		    ((j->flags & APO_SCORE_CANDIDATE_CORPUS) && !j->candidate_corpus) ||
+		    ((j->flags & APO_SCORE_CANDIDATE_EXTREMES) && !j->candidate_extremes)) {
 			apo_job_release(j); j->rc = APO_E_NOMEM; snprintf(j->err, sizeof j->err, "out of host memory"); return APO_E_NOMEM;
 		}
 	} else if (j->kind == APO_JOB_REWARD_BATCH) {
@@ -157,9 +168,9 @@ int apo_job_prepare(apo_job *j)
 void apo_job_release(apo_job *j)
 {
 	free(j->scores); free(j->counts); free(j->topk); free(j->dims_out); free(j->masks_out); free(j->finals_out); free(j->candidates);
-	free(j->candidate_corpus);
+	free(j->candidate_corpus); free(j->candidate_extremes);
 	j->scores = NULL; j->counts = NULL; j->topk = NULL; j->dims_out = NULL; j->masks_out = NULL; j->finals_out = NULL; j->candidates = NULL;
-	j->candidate_corpus = NULL;
+	j->candidate_corpus = NULL; j->candidate_extremes = NULL;
 }
 
 static void execute(apo_serial *s, apo_job *j)
@@ -224,6 +235,7 @@ static void execute(apo_serial *s, apo_job *j)
 	}
 	if (j->rc == APO_OK && j->candidates) j->rc = apo_candidate_reports(e, 0, j->C, j->candidates);
 	if (j->rc == APO_OK && j->candidate_corpus) j->rc = apo_candidate_corpus_reports(e, 0, j->C, j->candidate_corpus);
+	if (j->rc == APO_OK && j->candidate_extremes) j->rc = apo_candidate_extremes(e, 0, j->C, j->candidate_extremes);
 	if (j->rc != APO_OK) snprintf(j->err, sizeof j->err, "%s", apo_last_error(e));
 }
 

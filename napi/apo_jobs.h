@@ -43,10 +43,10 @@ typedef enum {
 	APO_JOB_ROLLOUTS_UPLOAD,       /* rolloutsUpload(handle, recs, rowBytes 32|16, C, T)         */
 	APO_JOB_CORPUS_UPLOAD,         /* corpusUpload(handle, recs apo_record[T], idxBase)          */
 	APO_JOB_CORPUS_UPLOAD_JSON,    /* corpusUploadJson(handle, utf8, idxBase)                    */
-	APO_JOB_SCORE_RESIDENT,        /* scoreResident(handle, {K, source, corpus, first, count, candidates, candidateCorpus}) */
-	APO_JOB_SCORE_HOST,            /* score(handle, dims, C, T, corpus|null, K, candidates?)                 */
-	APO_JOB_SCORE_HOST_RECORDS,    /* scoreHostRecords(handle, recs, rowBytes, C, T, corpus|null, K, candidates?, candidateCorpus?) */
-	APO_JOB_SCORE_HOST_TUPLES,     /* scoreHostTuples(handle, {tl, th, tbookPc, tbookPd, codebook, d2book}, C, T, corpus|null, K, candidates?) */
+	APO_JOB_SCORE_RESIDENT,        /* scoreResident(handle, {K, source, corpus, first, count, candidates, candidateCorpus, candidateExtremes}) */
+	APO_JOB_SCORE_HOST,            /* score(handle, dims, C, T, corpus|null, K, candidates?, candidateExtremes?) */
+	APO_JOB_SCORE_HOST_RECORDS,    /* scoreHostRecords(handle, recs, rowBytes, C, T, corpus|null, K, candidates?, candidateCorpus?, candidateExtremes?) */
+	APO_JOB_SCORE_HOST_TUPLES,     /* scoreHostTuples(handle, {tl, th, tbookPc, tbookPd, codebook, d2book}, C, T, corpus|null, K, candidates?, candidateExtremes?) */
 	APO_JOB_REWARD_BATCH,          /* rewardBatch(handle, recs apo_record[n])                    */
 	APO_JOB_COMM_INIT,             /* commInit(handle, nranks, rank, id[128])                    */
 	APO_JOB_TEST_HOOK,             /* tests: calls hook(hook_arg) in its turn                    */
@@ -71,6 +71,7 @@ typedef struct apo_job {
 	double *scores; uint64_t *counts; int32_t *topk; apo_corpus_report report;
 	apo_candidate_report *candidates;             /* [C], only when flags has APO_SCORE_CANDIDATES (apo_candidate_reports) */
 	apo_corpus_report *candidate_corpus;          /* [C], only when flags has APO_SCORE_CANDIDATE_CORPUS (apo_candidate_corpus_reports) */
+	struct apo_candidate_extremes *candidate_extremes;   /* [C], only when flags has APO_SCORE_CANDIDATE_EXTREMES (apo_candidate_extremes) */
 	double *dims_out; uint32_t *masks_out; double *finals_out; uint64_t n_out;
 	int rc; char err[256];
 } apo_job;
@@ -81,6 +82,9 @@ typedef struct apo_job {
 /* Same cap for the per-candidate corpus reports (C x sizeof(apo_corpus_report) = 784 B): about 5.5 M candidates.  They exist
  * for record jobs only (scoreResident with source APO_SRC_ROLLOUTS, scoreHostRecords); every other job is refused. */
 #define APO_JOB_CANDIDATE_CORPUS_MAX_BYTES (1ull << 32)
+/* Same cap for the per-candidate extremes (C x sizeof(struct apo_candidate_extremes) = 1032 B): about 4.16 M candidates.
+ * They belong to every scoring job. */
+#define APO_JOB_CANDIDATE_EXTREMES_MAX_BYTES (1ull << 32)
 
 /* Shape / size / overflow checks that need no engine; 0 = fine, else APO_E_ARG with the reason in j->err.
  * Everything that arrives from the renderer over IPC passes through here before a pointer is dereferenced. */

@@ -220,7 +220,10 @@ class APOService:
         When the result also carries the candidate's corpus report (rollout records scored with candidate_corpus=True,
         evaluateBeam(..., patterns=True)), the report adds byMode, the six problem patterns of APO:643-770 (examples = rollout
         indices) ahead of the dimension-low ones, and toolStats (TCS:603-624); its suggestions then follow the pattern and
-        mode rules of APO:830-859 as well.  Pure: it neither records the suggestions nor fires events nor touches storage."""
+        mode rules of APO:830-859 as well.  When the result carries the per-candidate extremes (extremes=True), the report
+        adds lowestRollouts / highestRollouts: the candidate's 32 lowest- and highest-reward rollouts as {"index", "finalReward"}
+        (reward ascending / descending, ties -> lower index), the sample runs the critique step reads; the caller looks the
+        rollouts up by index.  Pure: it neither records the suggestions nor fires events nor touches storage."""
         cc = res.candidate_corpus[c] if getattr(res, "candidate_corpus", None) is not None else None
         r = res.candidates[c] if res.candidates is not None else cc
         goodRate = float(r.goodRate)
@@ -239,6 +242,11 @@ class APOService:
             out["toolStats"] = {"totalToolCalls": int(cc.toolCalls), "totalToolSucceeded": int(cc.toolSucc),
                                 "totalToolFailed": int(cc.toolFail),
                                 "toolSuccessRate": None if cc.toolCalls == 0 else float(cc.toolSuccessRate)}
+        ex = res.extremes[c] if getattr(res, "extremes", None) is not None else None
+        if ex is not None:
+            n = int(ex.n)
+            out["lowestRollouts"] = [{"index": int(ex.lowest[i]), "finalReward": float(ex.lowestReward[i])} for i in range(n)]
+            out["highestRollouts"] = [{"index": int(ex.highest[i]), "finalReward": float(ex.highestReward[i])} for i in range(n)]
         return out
 
     @staticmethod
@@ -292,19 +300,22 @@ class APOService:
         return out
 
     # ---- beam evaluation: the step the reference delegates to its backend --------------------------------
-    def evaluateBeam(self, candidates, dims=None, rollouts=None, reports=False, patterns=False):
+    def evaluateBeam(self, candidates, dims=None, rollouts=None, reports=False, patterns=False, extremes=False):
         """Score a beam of VersionedPromptTemplate candidates on their rollout outcomes and keep the
         top `beamWidth` (score desc, ties -> lower index), then apply the APO:1138-1166 update with the
         strict `>` adoption rule (APO:1159).  dims: float32 [C][T][9] (NaN = absent) or rollouts:
         apo_record [C][T].  reports=True also builds the per-candidate breakdown (res.candidates, see
         candidateReport); with rollouts, reports=True and patterns=True also build every candidate's corpus
-        report (res.candidate_corpus: problem patterns, per-mode tallies, tool totals)."""
+        report (res.candidate_corpus: problem patterns, per-mode tallies, tool totals).  extremes=True also lists every
+        candidate's 32 lowest- and highest-reward rollouts (res.extremes)."""
         try:
             C = len(candidates)
             K = min(self._config["beamWidth"], C)
             extra = {"candidates": True} if reports else {}
             if reports and patterns and rollouts is not None:
                 extra["candidate_corpus"] = True
+            if extremes:
+                extra["extremes"] = True
             if dims is not None:
                 self._engine.dims_upload(np.ascontiguousarray(dims, np.float32))
                 res = self._engine.score(C, K, source=SRC_DIMS, **extra)
@@ -324,7 +335,8 @@ class APOService:
             print("[APO] Beam evaluation failed:", e)
             return None
 
-    def runBeamSearch(self, seedPrompt, proposeCandidates, rolloutDims=None, rounds=None, withReports=False, rolloutRecords=None):
+    def runBeamSearch(self, seedPrompt, proposeCandidates, rolloutDims=None, rounds=None, withReports=False, rolloutRecords=None,
+                      withExtremes=False):
         """Client-side round driver (SURVEY 8f rank 3) around the GPU top-K: each round expands every beam
         member into `branchFactor` children through the caller's `proposeCandidates(parent, n) -> [content]`
         hook (the LLM critique/edit step of APO:918-988 lives there), scores parents + children on
@@ -332,10 +344,13 @@ class APOService:
         one of the two), keeps the top `beamWidth` and applies the APO:1138-1166 update.  withReports=True calls
         `proposeCandidates(parent, n, report)` instead, with the candidateReport of the parent from the round that
         scored it (None for the unscored seed), so that the critique can name what the parent lost on; with
-        rolloutRecords that report also carries the parent's problem patterns, byMode and toolStats.  Returns the
-        final beam state."""
+        rolloutRecords that report also carries the parent's problem patterns, byMode and toolStats; withExtremes=True
+        (which needs withReports=True) adds the parent's lowestRollouts / highestRollouts, indices into the rollouts the
+        caller scored it on.  Returns the final beam state."""
         if (rolloutDims is None) == (rolloutRecords is None):
             raise ValueError("runBeamSearch needs exactly one of rolloutDims / rolloutRecords")
+        if withExtremes and not withReports:
+            raise ValueError("runBeamSearch: withExtremes needs withReports=True (the lists travel in the candidate reports)")
         rounds = rounds or self._config["beamRounds"]
         beam = [{"version": "v0", "content": seedPrompt, "score": None, "createdAt": time.time() * 1000.0}]
         counter = 0
@@ -350,9 +365,10 @@ class APOService:
                     cands.append({"version": f"v{counter}", "content": content, "score": None,
                                   "parentVersion": parent["version"], "createdAt": time.time() * 1000.0})
             if rolloutRecords is not None:
-                res = self.evaluateBeam(cands, rollouts=rolloutRecords(cands), reports=withReports, patterns=withReports)
+                res = self.evaluateBeam(cands, rollouts=rolloutRecords(cands), reports=withReports, patterns=withReports,
+                                        extremes=withExtremes)
             else:
-                res = self.evaluateBeam(cands, dims=rolloutDims(cands), reports=withReports)
+                res = self.evaluateBeam(cands, dims=rolloutDims(cands), reports=withReports, extremes=withExtremes)
             if res is None:
                 break
             if withReports:

@@ -8,6 +8,7 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <limits>
 #include <dlfcn.h>
 #include <unistd.h>
 #include <new>
@@ -231,6 +232,10 @@ struct apo_engine {
 	DevBuf<apo_corpus_report> ccorp_rep;     // reports of the last flagged call
 	uint32_t ccorp_C = 0;
 	bool ccorp_armed = false, ccorp_every = true, ccorp_ready = false;   // as cand_armed / cand_every / cand_ready
+	// per-candidate extremes (APO_SCORE_CANDIDATE_EXTREMES, csrc/apo_cand.cu k_cand_extremes): keys, converted by the getter
+	DevBuf<unsigned long long> ext_acc;      // [C][CX_WORDS] lists | [cand_ext_slots][CX_WORDS] segments of one launch
+	uint32_t ext_C = 0;
+	bool ext_armed = false, ext_every = true, ext_ready = false;         // as cand_armed / cand_every / cand_ready
 };
 
 namespace {
@@ -600,6 +605,7 @@ int begin_score(apo_engine *e, uint32_t C, bool whole = false) {
 	e->last_C = C; e->score_C = C; e->scoring = true; e->k1_used = 0;
 	e->cand_armed = false; e->cand_every = true; e->cand_ready = false;
 	e->ccorp_armed = false; e->ccorp_every = true; e->ccorp_ready = false;
+	e->ext_armed = false; e->ext_every = true; e->ext_ready = false;
 	e->timing = apo_timing{};
 	if (e->timing_on) CK(cudaEventRecord(e->ev[0], e->stream));
 	return APO_OK;
@@ -887,6 +893,58 @@ int ccorp_finish(apo_engine *e, uint32_t C) {
 	return APO_OK;
 }
 
+// ---- per-candidate extremes (APO_SCORE_CANDIDATE_EXTREMES)
+bool wants_ext(const apo_score_opts *o) { return (o->flags & APO_SCORE_CANDIDATE_EXTREMES) != 0; }
+
+int ext_check(apo_engine *e) {
+	if (e->nranks > 1)
+		return fail(e, APO_E_STATE, "APO_SCORE_CANDIDATE_EXTREMES is single-rank only: the per-candidate lists are not joined across the %d ranks of this handle", e->nranks);
+	return APO_OK;
+}
+
+// the lists of C candidates and the segment slots of one launch (and cand_upload_tbook's table for Form T), before route_copy
+int ext_reserve(apo_engine *e, uint32_t C) {
+	CK(reserve(e, e->ext_acc, ((uint64_t)C + apo::cand_ext_slots(e->sm_count, C)) * apo::CX_WORDS));
+	CK(reserve(e, e->cand_book, 8 * 16));
+	return APO_OK;
+}
+
+// empty lists (all-ones keys) for C candidates (first flagged launch of a call or session)
+int ext_arm(apo_engine *e, uint32_t C) {
+	if (int rc = ext_reserve(e, C)) return rc;
+	CK(cudaMemsetAsync(e->ext_acc.p, 0xFF, (uint64_t)C * apo::CX_WORDS * 8, e->stream));
+	e->ext_armed = true;
+	return APO_OK;
+}
+
+// the extremes pass and its merge over ev into candidates [cand_offset, ...)
+int launch_ext(apo_engine *e, const apo_score_opts *o, const Evals &ev, uint32_t cand_offset) {
+	if (!ev.count) return APO_OK;
+	if (ev.form == apo::CAND_T && !ev.t_once) { const int rc = cand_upload_tbook(e, ev.dict->book); if (rc) return rc; }
+	apo::CandExtParams X{};
+	apo::CandParams &P = X.src;
+	P.C = ev.C; P.T = ev.count; P.idx_base = ev.idx_base; P.pitch_evals = ev.pitch_evals; P.lut = e->d_lut.p;
+	P.rows = ev.rows; P.q8 = ev.q8; P.d2 = ev.d2; P.li = ev.li; P.qw = ev.qw;
+	P.tl = ev.tl; P.th = ev.th;
+	if (ev.qt) P.cbf = ev.qt->cbf.p;
+	if (ev.form == apo::CAND_T) {
+		P.tb_pc = ev.dict->pc.p; P.tb_pd = ev.dict->pd.p; P.n_tuples = ev.dict->n; P.d2book = ev.dict->d2.p; P.tbook = e->cand_book.p;
+	}
+	X.W = e->W;
+	X.lists = e->ext_acc.p + (uint64_t)apo::CX_WORDS * cand_offset;
+	X.seg = e->ext_acc.p + (uint64_t)apo::CX_WORDS * e->score_C;
+	CK(apo::run_cand_extremes(X, ev.form, (o->flags & APO_SCORE_RECIP) != 0, e->sm_count, e->stream));
+	e->timing.launches += 2;
+	return APO_OK;
+}
+
+// the lists are final once the call's launches have run: the getter converts the keys it is asked for
+int ext_finish(apo_engine *e, uint32_t C) {
+	CK(cudaStreamSynchronize(e->stream));
+	e->ext_C = C; e->ext_ready = true;
+	return APO_OK;
+}
+
 // K2 (+fused finalize) / allreduce / K3, then bring the result block home
 bool wants_corpus(const apo_engine *e, const apo_score_opts *o) { return (o->flags & APO_SCORE_CORPUS) && e->corpus_T > 0; }
 // the corpus words come from the digest instead of a scan of the records
@@ -998,7 +1056,8 @@ int finish_score(apo_engine *e, const apo_score_opts *o, uint32_t C, double *sco
 		if (bad) return fail(e, APO_E_ARG, "an evaluation names an empty or NaN slot of the codebook or of d2book");
 	}
 	if (wants_cand(o) && (rc = cand_finish(e, C))) return rc;
-	return wants_ccorp(o) ? ccorp_finish(e, C) : APO_OK;
+	if (wants_ccorp(o) && (rc = ccorp_finish(e, C))) return rc;
+	return wants_ext(o) ? ext_finish(e, C) : APO_OK;
 }
 
 // o's window against the T evaluations loaded
@@ -1025,10 +1084,12 @@ int score_check(apo_engine *e, const apo_score_opts *o, uint32_t C, uint64_t T, 
 	}
 	if (wants_cand(o) && (rc = cand_check(e))) return rc;
 	if (wants_ccorp(o) && (rc = ccorp_check(e, records))) return rc;
+	if (wants_ext(o) && (rc = ext_check(e))) return rc;
 	CK(cudaSetDevice(e->device));
 	if (T == kSession) return APO_OK;                               // a session's scratch was sized by apo_score_begin
 	if ((rc = ensure_scratch(e, C, o->K))) return rc;
 	if (wants_cand(o) && (rc = cand_reserve(e, C))) return rc;
+	if (wants_ext(o) && (rc = ext_reserve(e, C))) return rc;
 	return APO_OK;
 }
 
@@ -1042,6 +1103,7 @@ int score_arm(apo_engine *e, const apo_score_opts *o, uint32_t C, bool begin, ui
 	int rc;
 	if (begin && (rc = begin_score(e, C, whole))) return rc;
 	if (wants_cand(o) && !e->cand_armed && (rc = cand_arm(e, C))) return rc;
+	if (wants_ext(o) && !e->ext_armed && (rc = ext_arm(e, C))) return rc;
 	return wants_ccorp(o) && !e->ccorp_armed ? ccorp_arm(e, C) : APO_OK;
 }
 
@@ -1612,7 +1674,7 @@ extern "C" void apo_destroy(apo_engine *e) {
 	e->qt.release(); e->qt_stream.release();
 	e->d_lut.release(); e->corpus.release(); e->digest.release(); e->dims.release(); e->roll.release(); e->acc.release(); e->acc_joined.release(); e->acc_snapshot.release(); e->misc.release();
 	e->result.release(); e->keys.release(); e->sel_key.release(); e->sel_idx.release();
-	e->cand_acc.release(); e->cand_rep.release(); e->cand_book.release(); e->ccorp_acc.release(); e->ccorp_rep.release();
+	e->cand_acc.release(); e->cand_rep.release(); e->cand_book.release(); e->ccorp_acc.release(); e->ccorp_rep.release(); e->ext_acc.release();
 	e->tup.release(); e->tups.release(); e->tvals.release();
 	e->win[0].release(); e->win[1].release(); e->batch_in.release(); e->batch_out.release(); e->batch_mask.release();
 	if (e->h_result) cudaFreeHost(e->h_result);
@@ -2036,14 +2098,18 @@ extern "C" int apo_score_accumulate(apo_engine *e, const apo_score_opts *o, uint
 	if (rc) return rc;
 	if ((uint64_t)cand_offset + ev.C > e->score_C) return fail(e, APO_E_ARG, "candidates [%u,%u) exceed C_total=%u", cand_offset, cand_offset + ev.C, e->score_C);
 	if ((rc = check_window(e, o, ev.count))) return rc;
-	const bool cand = wants_cand(o), ccorp = wants_ccorp(o);
+	const bool cand = wants_cand(o), ccorp = wants_ccorp(o), ext = wants_ext(o);
 	if (cand && (rc = cand_check(e))) return rc;
 	if (ccorp && (rc = ccorp_check(e, ev.records()))) return rc;
+	if (ext && (rc = ext_check(e))) return rc;
 	CK(cudaSetDevice(e->device));
 	if (cand && (rc = cand_reserve(e, e->score_C))) return rc;                                  // allocates: before route_copy
 	if (cand && e->cand_every && !e->cand_armed && (rc = cand_arm(e, e->score_C))) return rc;
+	if (ext && e->ext_every && !e->ext_armed && (rc = ext_arm(e, e->score_C))) return rc;      // allocates too
 	if ((rc = route_copy(e, o, &ev))) return rc;
 	if ((rc = resident_window(e, o, &ev)) || (rc = launch_score(e, o, ev, cand_offset))) return rc;
+	if (!ext) e->ext_every = false;
+	else if (e->ext_every && (rc = launch_ext(e, o, ev, cand_offset))) return rc;   // else finish refuses
 	if (!ccorp) e->ccorp_every = false;
 	else if (e->ccorp_every) {                          // an earlier accumulate of the session did not set the flag: finish refuses
 		if (!e->ccorp_armed && (rc = ccorp_arm(e, e->score_C))) return rc;
@@ -2057,7 +2123,7 @@ extern "C" int apo_score_accumulate(apo_engine *e, const apo_score_opts *o, uint
 extern "C" int apo_score_finish(apo_engine *e, const apo_score_opts *o, double *scores, uint64_t *counts, int32_t *topk,
                                 apo_corpus_report *report) {
 	if (!e) return APO_E_ARG;
-	e->cand_ready = e->ccorp_ready = false;             // a failed finish leaves no breakdown behind either
+	e->cand_ready = e->ccorp_ready = e->ext_ready = false;   // a failed finish leaves no breakdown behind either
 	if (!o) return fail(e, APO_E_ARG, "opts is NULL");
 	if (!e->scoring) return fail(e, APO_E_STATE, "apo_score_begin has not been called");
 	int rc = score_check(e, o, e->score_C, kSession, true);      // the accumulate calls refused every other source
@@ -2066,13 +2132,15 @@ extern "C" int apo_score_finish(apo_engine *e, const apo_score_opts *o, double *
 		return fail(e, APO_E_STATE, "APO_SCORE_CANDIDATES: every apo_score_accumulate of the session must set the flag for a breakdown");
 	if (wants_ccorp(o) && !e->ccorp_every)
 		return fail(e, APO_E_STATE, "APO_SCORE_CANDIDATE_CORPUS: every apo_score_accumulate of the session must set the flag for the reports");
+	if (wants_ext(o) && !e->ext_every)
+		return fail(e, APO_E_STATE, "APO_SCORE_CANDIDATE_EXTREMES: every apo_score_accumulate of the session must set the flag for the lists");
 	if ((rc = digest_prepare(e, o)) || (rc = score_arm(e, o, e->score_C, false))) return rc;   // nothing accumulated yet: an empty breakdown
 	return finish_score(e, o, e->score_C, scores, counts, topk, report);
 }
 
 extern "C" int apo_score(apo_engine *e, const apo_score_opts *o, double *scores, uint64_t *counts, int32_t *topk, apo_corpus_report *report) {
 	if (!e) return APO_E_ARG;
-	e->cand_ready = e->ccorp_ready = false;             // a failed call leaves no breakdown behind either
+	e->cand_ready = e->ccorp_ready = e->ext_ready = false;   // a failed call leaves no breakdown behind either
 	Evals ev;
 	int rc = resident_evals(e, o, &ev);
 	if (rc) return rc;
@@ -2113,6 +2181,7 @@ extern "C" int apo_score(apo_engine *e, const apo_score_opts *o, double *scores,
 	if ((rc = launch_score(e, o, ev, 0, fused ? &k2 : nullptr))) return rc;
 	if (wants_cand(o) && (rc = launch_cand(e, ev, 0))) return rc;
 	if (wants_ccorp(o) && (rc = launch_ccorp(e, ev, 0))) return rc;
+	if (wants_ext(o) && (rc = launch_ext(e, o, ev, 0))) return rc;
 	return finish_score(e, o, C, scores, counts, topk, report, fused);
 }
 
@@ -2163,7 +2232,7 @@ int stream_host(apo_engine *e, const apo_score_opts *o, const HostTensor &h, dou
                 apo_corpus_report *report) {
 	const uint32_t C = h.C;
 	const uint64_t T = h.T;
-	e->cand_ready = e->ccorp_ready = false;
+	e->cand_ready = e->ccorp_ready = e->ext_ready = false;
 	if (!o) return fail(e, APO_E_ARG, "opts is NULL");
 	const bool rows = h.form != apo::CAND_Q && h.form != apo::CAND_T;
 	if (!rows && wants_ccorp(o)) return ccorp_check(e, false);   // the wire formats refuse it before they look at their inputs
@@ -2214,7 +2283,7 @@ int stream_host(apo_engine *e, const apo_score_opts *o, const HostTensor &h, dou
 	}
 	if ((rc = score_arm(e, o, C, true, (uint64_t)C * T * wire))) return rc;
 	if (h.form == apo::CAND_T) {                                   // the dictionary and its values, once for the whole call
-		if (wants_cand(o) && (rc = cand_upload_tbook(e, h.codebook))) return rc;
+		if ((wants_cand(o) || wants_ext(o)) && (rc = cand_upload_tbook(e, h.codebook))) return rc;
 		if ((rc = dict_upload(e, e->tups, h.tb_pc, h.tb_pd, h.n_tuples, h.codebook, h.d2book))) return rc;
 		ev.dict = &e->tups; ev.t_once = true;
 		if ((rc = tuple_values(e, e->tups, e->tvals, (o->flags & APO_SCORE_RECIP) != 0))) return rc;
@@ -2259,6 +2328,7 @@ int stream_host(apo_engine *e, const apo_score_opts *o, const HostTensor &h, dou
 		if ((rc = launch_score(e, o, ev, 0))) return rc;
 		if (wants_cand(o) && (rc = launch_cand(e, ev, 0))) return rc;
 		if (wants_ccorp(o) && (rc = launch_ccorp(e, ev, 0))) return rc;   // before the window is released
+		if (wants_ext(o) && (rc = launch_ext(e, o, ev, 0))) return rc;
 		CK(cudaEventRecord(e->win_free[b], e->stream));
 	}
 	return finish_score(e, o, C, scores, counts, topk, report, false, h.packed);
@@ -2547,6 +2617,37 @@ extern "C" int apo_candidate_corpus_reports(apo_engine *e, uint32_t c0, uint32_t
 	CK(cudaSetDevice(e->device));
 	CK(cudaMemcpyAsync(out, e->ccorp_rep.p + c0, (uint64_t)n * sizeof(apo_corpus_report), cudaMemcpyDeviceToHost, e->stream));
 	CK(cudaStreamSynchronize(e->stream));
+	return APO_OK;
+}
+
+extern "C" int apo_candidate_extremes(apo_engine *e, uint32_t c0, uint32_t n, struct apo_candidate_extremes *out) {
+	if (!e) return APO_E_ARG;
+	if (!e->ext_ready) return fail(e, APO_E_STATE, "the last scoring call did not set APO_SCORE_CANDIDATE_EXTREMES");
+	if ((uint64_t)c0 + n > e->ext_C) return fail(e, APO_E_ARG, "candidates [%u,%llu) exceed C=%u", c0, (unsigned long long)c0 + n, e->ext_C);
+	if (n == 0) return APO_OK;
+	if (!out) return fail(e, APO_E_ARG, "out is NULL");
+	CK(cudaSetDevice(e->device));
+	std::vector<unsigned long long> keys((uint64_t)n * apo::CX_WORDS);
+	CK(cudaMemcpyAsync(keys.data(), e->ext_acc.p + (uint64_t)c0 * apo::CX_WORDS, keys.size() * 8, cudaMemcpyDeviceToHost, e->stream));
+	CK(cudaStreamSynchronize(e->stream));
+	for (uint32_t c = 0; c < n; c++) {
+		const unsigned long long *k = keys.data() + (uint64_t)c * apo::CX_WORDS;   // [lowest, highest][32][value key, position]
+		struct apo_candidate_extremes &x = out[c];
+		x.n = 0;
+		for (int l = 0; l < 2; l++) {
+			int64_t *pos = l ? x.highest : x.lowest;
+			double *rew = l ? x.highestReward : x.lowestReward;
+			for (int i = 0; i < APO_EXTREMES_N; i++) {
+				const unsigned long long v = k[64 * l + 2 * i], p = k[64 * l + 2 * i + 1];
+				if (v == ~0ull && p == ~0ull) { pos[i] = -1; rew[i] = std::numeric_limits<double>::quiet_NaN(); continue; }
+				const unsigned long long ok = l ? ~v : v;                          // the highest list keys the complement
+				const unsigned long long bits = (ok >> 63) ? ok & ~(1ull << 63) : ~ok;
+				memcpy(&rew[i], &bits, 8);
+				pos[i] = (int64_t)p;
+				if (l == 0) x.n = (uint64_t)i + 1;
+			}
+		}
+	}
 	return APO_OK;
 }
 

@@ -497,4 +497,191 @@ cudaError_t run_cand_corpus_report(long long *blk, uint32_t C, apo_corpus_report
 	return cudaGetLastError();
 }
 
+// ================================================================ per-candidate extremes (APO_SCORE_CANDIDATE_EXTREMES)
+//   k_cand_extremes<Loader, TABLE, RECIP>  one pass over the evaluations a scoring call reads, with the breakdown's loaders
+//                                          and tile walk: every warp keeps the 32 smallest keys of each list of its current
+//                                          candidate in registers (lane i holds the i-th) and writes them to its segment
+//                                          slot when the candidate changes
+//   k_cand_extremes_merge                  one warp per candidate: the persistent lists merged with the segments of the
+//                                          warps whose tile range covers the candidate, in warp order
+// No locks and no atomics: a warp's candidates form a range [c_lo(w), c_hi(w)] with c_lo(w + 1) >= c_hi(w), so the slots
+// w + c of different warps never meet, and the merge finds the warps of a row by the pass's own range formula.
+struct XKey { unsigned long long v, p; };
+constexpr unsigned FULL = 0xffffffffu;
+__device__ __forceinline__ bool xlt(const XKey &a, const XKey &b) { return a.v < b.v || (a.v == b.v && a.p < b.p); }
+__device__ __forceinline__ XKey xshfl(const XKey &k, int src) { return {__shfl_sync(FULL, k.v, src), __shfl_sync(FULL, k.p, src)}; }
+__device__ __forceinline__ XKey xshfl_xor(const XKey &k, int m) { return {__shfl_xor_sync(FULL, k.v, m), __shfl_xor_sync(FULL, k.p, m)}; }
+__device__ __forceinline__ XKey xempty() { return {~0ull, ~0ull}; }
+
+// order-preserving u64 of a binary64 value (-0.0 taken as +0.0)
+__device__ __forceinline__ unsigned long long order_key(double x) {
+	const unsigned long long u = (unsigned long long)__double_as_longlong(x == 0.0 ? 0.0 : x);
+	return (u >> 63) ? ~u : (u | (1ull << 63));
+}
+
+// one key per lane -> ascending across the warp (bitonic sort, 15 compare-exchange steps)
+__device__ __forceinline__ XKey warp_sort(XKey k, int lane) {
+#pragma unroll
+	for (int s = 2; s <= 32; s <<= 1) {
+#pragma unroll
+		for (int j = s >> 1; j > 0; j >>= 1) {
+			const XKey o = xshfl_xor(k, j);
+			const bool want_min = ((lane & j) == 0) == ((lane & s) == 0);
+			if (want_min ? xlt(o, k) : xlt(k, o)) k = o;
+		}
+	}
+	return k;
+}
+
+// list <- the 32 smallest of list and s, both ascending across the warp: the lane-wise min against s reversed is bitonic,
+// five compare-exchange steps sort it
+__device__ __forceinline__ XKey warp_merge(XKey list, const XKey &s, int lane) {
+	const XKey r = xshfl(s, 31 - lane);
+	XKey m = xlt(r, list) ? r : list;
+#pragma unroll
+	for (int j = 16; j > 0; j >>= 1) {
+		const XKey o = xshfl_xor(m, j);
+		if ((lane & j) ? xlt(m, o) : xlt(o, m)) m = o;
+	}
+	return m;
+}
+
+// offer one new key per lane to an ascending list: sort and merge only when some key beats the list's last entry
+__device__ __forceinline__ void offer(XKey &list, const XKey &k, int lane) {
+	const XKey last = xshfl(list, 31);
+	if (__ballot_sync(FULL, xlt(k, last))) list = warp_merge(list, warp_sort(k, lane), lane);
+}
+
+__device__ __forceinline__ void store_lists(unsigned long long *slot, const XKey &lo, const XKey &hi, int lane) {
+	reinterpret_cast<ulonglong2 *>(slot)[lane] = make_ulonglong2(lo.v, lo.p);
+	reinterpret_cast<ulonglong2 *>(slot)[32 + lane] = make_ulonglong2(hi.v, hi.p);
+}
+__device__ __forceinline__ void load_lists(const unsigned long long *slot, XKey &lo, XKey &hi, int lane) {
+	const ulonglong2 a = reinterpret_cast<const ulonglong2 *>(slot)[lane], b = reinterpret_cast<const ulonglong2 *>(slot)[32 + lane];
+	lo = {a.x, a.y}; hi = {b.x, b.y};
+}
+
+template <class L, int TABLE, bool RECIP>
+__global__ void __launch_bounds__(CB_THREADS, L::MIN_CTAS)
+k_cand_extremes(const CandExtParams X, uint32_t tiles_per_cand, uint64_t total_tiles) {
+	const CandParams &P = X.src;
+	__shared__ CandSmem S;
+	__shared__ double s_rc[512];                                        // reciprocal of the total weight (div_lut)
+	for (int i = threadIdx.x; i < 512; i += CB_THREADS) { S.tw[i] = P.lut[i]; s_rc[i] = P.lut[512 + i]; }
+	if (TABLE == 1) for (int i = threadIdx.x; i < 8 * 256; i += CB_THREADS) S.tab[i] = P.cbf[i];
+	if (TABLE == 2) for (int i = threadIdx.x; i < 8 * 16; i += CB_THREADS) S.tab[i] = P.tbook[i];
+	__syncthreads();
+	const int lane = threadIdx.x & 31;
+	const uint64_t nwarps = (uint64_t)gridDim.x * (CB_THREADS / 32);
+	const uint64_t gw = (uint64_t)blockIdx.x * (CB_THREADS / 32) + (threadIdx.x >> 5);
+	const uint64_t lo = total_tiles * gw / nwarps, hi = total_tiles * (gw + 1) / nwarps;
+	if (lo >= hi) return;
+
+	XKey low = xempty(), high = xempty();
+	uint32_t cur = (uint32_t)(lo / tiles_per_cand);
+	for (uint64_t tile = lo; tile < hi; tile++) {
+		const uint32_t c = (uint32_t)(tile / tiles_per_cand), j = (uint32_t)(tile - (uint64_t)c * tiles_per_cand);
+		if (c != cur) {
+			store_lists(X.seg + (gw + cur) * CX_WORDS, low, high, lane);
+			low = high = xempty();
+			cur = c;
+		}
+		const uint64_t t0 = (uint64_t)j * CB_TILE;
+		for (int g0 = 0; g0 < CB_GROUPS; g0 += L::U) {
+			typename L::Raw R[L::U];
+			bool in[L::U];
+#pragma unroll
+			for (int u = 0; u < L::U; u++) {
+				const uint64_t t = t0 + (uint64_t)(g0 + u) * 32 + lane;
+				in[u] = t < P.T;
+				if (in[u]) L::fetch(P, c, t, R[u]);
+			}
+#pragma unroll
+			for (int u = 0; u < L::U; u++) {
+				const uint64_t t = t0 + (uint64_t)(g0 + u) * 32 + lane;
+				if (t - lane >= P.T) break;                                 // warp-uniform: the rest of the tile is past the row end
+				XKey kl = xempty(), kh = xempty();
+				if (in[u]) {
+					CandEval E;
+					L::decode(P, S, R[u], E);
+					if (E.valid) {
+						double ws = 0.0;                                    // TCS:777-784 in push order, absent values +0.0
+#pragma unroll
+						for (int i = 0; i < APO_NDIM; i++) ws = __dadd_rn(ws, __dmul_rn(E.v[i], X.W.w[i]));
+						const unsigned long long k = order_key(div_lut<RECIP>(ws, make_double2(S.tw[E.mask], s_rc[E.mask])));
+						kl = {k, P.idx_base + t};
+						kh = {~k, P.idx_base + t};
+					}
+				}
+				offer(low, kl, lane);
+				offer(high, kh, lane);
+			}
+		}
+	}
+	store_lists(X.seg + (gw + cur) * CX_WORDS, low, high, lane);
+}
+
+// the warp of the pass whose tile range holds `tile`: the largest w with total * w / nwarps <= tile
+__device__ __forceinline__ uint64_t tile_owner(uint64_t tile, uint64_t total_tiles, uint64_t nwarps) {
+	return ((tile + 1) * nwarps - 1) / total_tiles;
+}
+
+__global__ void __launch_bounds__(256)
+k_cand_extremes_merge(unsigned long long *lists, const unsigned long long *seg, uint32_t C, uint32_t tiles_per_cand,
+                      uint64_t total_tiles, uint64_t nwarps) {
+	const uint32_t c = blockIdx.x * (blockDim.x / 32) + (threadIdx.x >> 5);
+	if (c >= C) return;
+	const int lane = threadIdx.x & 31;
+	XKey low, high;
+	load_lists(lists + (uint64_t)c * CX_WORDS, low, high, lane);
+	const uint64_t w0 = tile_owner((uint64_t)c * tiles_per_cand, total_tiles, nwarps);
+	const uint64_t w1 = tile_owner((uint64_t)(c + 1) * tiles_per_cand - 1, total_tiles, nwarps);
+	for (uint64_t w = w0; w <= w1; w++) {
+		if (total_tiles * w / nwarps == total_tiles * (w + 1) / nwarps) continue;   // a warp without tiles wrote no segment
+		XKey sl, sh;
+		load_lists(seg + (w + c) * CX_WORDS, sl, sh, lane);
+		if (xlt(xshfl(sl, 0), xshfl(low, 31))) low = warp_merge(low, sl, lane);
+		if (xlt(xshfl(sh, 0), xshfl(high, 31))) high = warp_merge(high, sh, lane);
+	}
+	store_lists(lists + (uint64_t)c * CX_WORDS, low, high, lane);
+}
+
+template <class L, int TABLE, bool RECIP>
+static cudaError_t launch_ext(const CandExtParams &X, int sm_count, cudaStream_t st) {
+	const CandParams &P = X.src;
+	const uint32_t tiles_per_cand = (uint32_t)((P.T + CB_TILE - 1) / CB_TILE);
+	const uint64_t total_tiles = (uint64_t)tiles_per_cand * P.C;
+	if (total_tiles == 0) return cudaSuccess;
+	int per_sm = 0;
+	cudaError_t err = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_cand_extremes<L, TABLE, RECIP>, CB_THREADS, 0);
+	if (err != cudaSuccess) return err;
+	uint64_t grid = (uint64_t)sm_count * (uint64_t)(per_sm > 0 ? per_sm : 1);
+	const uint64_t need = (total_tiles + (CB_THREADS / 32) - 1) / (CB_THREADS / 32);
+	if (grid > need) grid = need;
+	if (cand_env_grid() && cand_env_grid() < grid) grid = cand_env_grid();
+	const uint64_t nwarps = grid * (CB_THREADS / 32);
+	if (nwarps > CX_MAX_WARPS_PER_SM * (uint64_t)sm_count) return cudaErrorInvalidConfiguration;   // more than the segment slots hold
+	k_cand_extremes<L, TABLE, RECIP><<<(unsigned)grid, CB_THREADS, 0, st>>>(X, tiles_per_cand, total_tiles);
+	if ((err = cudaGetLastError()) != cudaSuccess) return err;
+	k_cand_extremes_merge<<<(P.C + 7) / 8, 256, 0, st>>>(X.lists, X.seg, P.C, tiles_per_cand, total_tiles, nwarps);
+	return cudaGetLastError();
+}
+
+template <bool RECIP>
+static cudaError_t run_ext(const CandExtParams &X, int source, int sm_count, cudaStream_t st) {
+	switch (source) {
+	case CAND_DIMS: return launch_ext<LoadDims, 0, RECIP>(X, sm_count, st);
+	case CAND_REC32: return launch_ext<LoadRec<32>, 0, RECIP>(X, sm_count, st);
+	case CAND_REC16: return launch_ext<LoadRec<16>, 0, RECIP>(X, sm_count, st);
+	case CAND_Q: return launch_ext<LoadQ, 1, RECIP>(X, sm_count, st);
+	case CAND_T: return launch_ext<LoadT, 2, RECIP>(X, sm_count, st);
+	case CAND_W: return launch_ext<LoadW, 1, RECIP>(X, sm_count, st);
+	default: return cudaErrorInvalidValue;
+	}
+}
+
+cudaError_t run_cand_extremes(const CandExtParams &X, int source, bool recip, int sm_count, cudaStream_t st) {
+	return recip ? run_ext<true>(X, source, sm_count, st) : run_ext<false>(X, source, sm_count, st);
+}
+
 }  // namespace apo

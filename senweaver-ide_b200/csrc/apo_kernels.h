@@ -377,6 +377,22 @@ cudaError_t run_cand_corpus(const CandCorpusParams &P, int row, int sm_count, cu
 // blk: the whole buffer ([C][CC_WORDS] blocks, then the scratch)
 cudaError_t run_cand_corpus_report(long long *blk, uint32_t C, apo_corpus_report *out, cudaStream_t st);
 
+// ---- per-candidate extremes (csrc/apo_cand.cu): the 32 lowest and 32 highest finalRewards of every candidate.
+// A key is 128 bits {order-preserving u64 of the binary64 finalReward (complemented for the highest list), record position},
+// all ones = empty.  A list pair is CX_WORDS words: [2 lists: lowest, highest][32 keys ascending][value word, position word].
+// Own buffer: [C][CX_WORDS] lists that persist through a call or session | [cand_ext_slots(sm_count, C)][CX_WORDS] segments,
+// the runs of one launch's warps (warp w's run of candidate c in slot w + c).
+constexpr int CX_WORDS = 2 * 32 * 2;
+constexpr uint64_t CX_MAX_WARPS_PER_SM = 2048 / 32;   // the pass's grid never holds more warps than the SMs can host
+inline uint64_t cand_ext_slots(int sm_count, uint32_t C) { return CX_MAX_WARPS_PER_SM * (uint64_t)sm_count + C; }
+struct CandExtParams {
+	CandParams src;                 // the evaluations, as the breakdown reads them (ints / ex / dom unused)
+	Weights W;
+	unsigned long long *lists;      // [C][CX_WORDS] of candidate 0 of this launch
+	unsigned long long *seg;        // segment slots of this launch
+};
+cudaError_t run_cand_extremes(const CandExtParams &P, int source, bool recip, int sm_count, cudaStream_t st);
+
 int k1_tile_evals(int row, int variant);
 cudaError_t run_reward9(K1Params P, int row, int variant, bool recip, int sm_count, cudaStream_t st);
 cudaError_t run_detect6(const K2Params &P, int sm_count, cudaStream_t st);

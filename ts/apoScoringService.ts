@@ -26,6 +26,7 @@ export interface ApoScoreBlocks {
 	report: VSBuffer;   // struct apo_corpus_report (784 bytes)
 	candidates?: VSBuffer;   // apo_candidate_report[C] (376 bytes each, candidateReportCodec.ts); only when the call asked for it
 	candidateCorpus?: VSBuffer;   // apo_corpus_report[C] (784 bytes each, decodeCandidateCorpusReport); rollout records only, when asked for
+	candidateExtremes?: VSBuffer;   // struct apo_candidate_extremes[C] (1032 bytes each, decodeCandidateExtremes); only when asked for
 }
 
 /** Form T of a float32[C][T][9] tensor (include/apo_b200.h): tl uint16[C][T] | th uint8[C][T] = the 24-bit dictionary index of every
@@ -43,6 +44,7 @@ export interface ApoResidentQuery {
 	corpus?: 0 | 1;         // also build the corpus report from the uploaded corpus
 	candidates?: 0 | 1;     // also build the per-candidate breakdown (ApoScoreBlocks.candidates)
 	candidateCorpus?: 0 | 1;   // source 1 only: also build every candidate's corpus report (ApoScoreBlocks.candidateCorpus)
+	candidateExtremes?: 0 | 1;   // also list every candidate's 32 lowest- and highest-reward rollouts (ApoScoreBlocks.candidateExtremes)
 	first?: number;         // window [first, first + count) of the trace axis; count 0 = to the end
 	count?: number;
 }
@@ -75,16 +77,19 @@ export interface IApoScoringService {
 
 	// ---- one-shot path: host buffers streamed through the device, nothing stays resident
 	/** dims: float32[C][T][9] (pass C = 1, T = 4 of NaN for report-only calls).
-	 *  candidates: also return the per-candidate breakdown (ApoScoreBlocks.candidates), here and on the other one-shot calls. */
-	score(dims: VSBuffer, C: number, T: number, corpus: VSBuffer | undefined, K: number, candidates?: boolean): Promise<ApoScoreBlocks>;
+	 *  candidates: also return the per-candidate breakdown (ApoScoreBlocks.candidates), here and on the other one-shot calls;
+	 *  candidateExtremes: also return every candidate's 32 lowest- and highest-reward rollouts (ApoScoreBlocks.candidateExtremes). */
+	score(dims: VSBuffer, C: number, T: number, corpus: VSBuffer | undefined, K: number, candidates?: boolean,
+		candidateExtremes?: boolean): Promise<ApoScoreBlocks>;
 	/** [C][T] trace records (the IDE's own representation): 2.2x fewer PCIe bytes than fp32 dims with 16-byte rows.
 	 *  candidateCorpus: also return the corpus report of every candidate's records (ApoScoreBlocks.candidateCorpus). */
 	scoreHostRecords(records: VSBuffer, rowBytes: 32 | 16, C: number, T: number, corpus: VSBuffer | undefined, K: number, candidates?: boolean,
-		candidateCorpus?: boolean): Promise<ApoScoreBlocks>;
+		candidateCorpus?: boolean, candidateExtremes?: boolean): Promise<ApoScoreBlocks>;
 	/** fp32 evaluations -> Form T (include/apo_b200.h): a 24-bit dictionary index per evaluation (3 bytes instead of 36) + the
 	 *  dictionary of distinct evaluations.  For evaluations that are scored more than once, kept, or moved between processes. */
 	encodeTuples(dims: VSBuffer, C: number, T: number): Promise<ApoTupleBuffers | undefined>;
-	scoreTuples(tuples: ApoTupleBuffers, C: number, T: number, corpus: VSBuffer | undefined, K: number, candidates?: boolean): Promise<ApoScoreBlocks>;
+	scoreTuples(tuples: ApoTupleBuffers, C: number, T: number, corpus: VSBuffer | undefined, K: number, candidates?: boolean,
+		candidateExtremes?: boolean): Promise<ApoScoreBlocks>;
 }
 
 export const IApoScoringService = createDecorator<IApoScoringService>('senweaverApoScoringService');
@@ -107,16 +112,17 @@ export class ApoScoringService implements IApoScoringService {
 	corpusUploadJson(persisted: string, idxBase?: number) { return this._proxy.corpusUploadJson(persisted, idxBase); }
 	dimsTuples(cap?: number) { return this._proxy.dimsTuples(cap); }
 	scoreResident(query: ApoResidentQuery) { return this._proxy.scoreResident(query); }
-	score(dims: VSBuffer, C: number, T: number, corpus: VSBuffer | undefined, K: number, candidates?: boolean) {
-		return this._proxy.score(dims, C, T, corpus, K, candidates);
+	score(dims: VSBuffer, C: number, T: number, corpus: VSBuffer | undefined, K: number, candidates?: boolean, candidateExtremes?: boolean) {
+		return this._proxy.score(dims, C, T, corpus, K, candidates, candidateExtremes);
 	}
 	scoreHostRecords(records: VSBuffer, rowBytes: 32 | 16, C: number, T: number, corpus: VSBuffer | undefined, K: number, candidates?: boolean,
-		candidateCorpus?: boolean) {
-		return this._proxy.scoreHostRecords(records, rowBytes, C, T, corpus, K, candidates, candidateCorpus);
+		candidateCorpus?: boolean, candidateExtremes?: boolean) {
+		return this._proxy.scoreHostRecords(records, rowBytes, C, T, corpus, K, candidates, candidateCorpus, candidateExtremes);
 	}
 	encodeTuples(dims: VSBuffer, C: number, T: number) { return this._proxy.encodeTuples(dims, C, T); }
-	scoreTuples(tuples: ApoTupleBuffers, C: number, T: number, corpus: VSBuffer | undefined, K: number, candidates?: boolean) {
-		return this._proxy.scoreTuples(tuples, C, T, corpus, K, candidates);
+	scoreTuples(tuples: ApoTupleBuffers, C: number, T: number, corpus: VSBuffer | undefined, K: number, candidates?: boolean,
+		candidateExtremes?: boolean) {
+		return this._proxy.scoreTuples(tuples, C, T, corpus, K, candidates, candidateExtremes);
 	}
 }
 

@@ -12,7 +12,12 @@
  *  corpus report of each candidate's rollout records (problem patterns, byMode, tool totals included), decoded by
  *  traceRecordCodec's decodeCorpusReport.
  *
- *  The byte offsets below are pinned to the C structs by tests/test_napi_candidates.py and tests/test_candidate_corpus_cpu.py.
+ *  And the decoder of the per-candidate extremes (ApoScoreBlocks.candidateExtremes): struct apo_candidate_extremes[C], the
+ *  32 lowest- and 32 highest-reward rollouts of each candidate with their finalRewards — the sample runs the critique prompt
+ *  is built from (APO:918-962, 1003-1007).
+ *
+ *  The byte offsets below are pinned to the C structs by tests/test_napi_candidates.py, tests/test_candidate_corpus_cpu.py and
+ *  tests/test_napi_candidate_extremes.py.
  *--------------------------------------------------------------------------------------------*/
 import { VSBuffer } from '../../../../base/common/buffer.js';
 import { CorpusReportNumbers, DIM_NAMES, decodeCorpusReport } from './traceRecordCodec.js';
@@ -91,4 +96,36 @@ export function decodeCandidateCorpusReport(buf: VSBuffer, c: number): CorpusRep
 	const base = c * CORPUS_REPORT_BYTES;
 	if (c < 0 || base + CORPUS_REPORT_BYTES > buf.byteLength) { throw new RangeError(`candidate ${c} outside the block`); }
 	return decodeCorpusReport(buf.slice(base, base + CORPUS_REPORT_BYTES));
+}
+
+const EXTREMES_BYTES = 1032;             // sizeof(struct apo_candidate_extremes)
+const EXTREMES_N = 32;
+const OFF_EXT_N = 0;
+const OFF_LOWEST = 8;
+const OFF_LOWEST_REWARD = 264;
+const OFF_HIGHEST = 520;
+const OFF_HIGHEST_REWARD = 776;
+
+export interface CandidateExtremes {
+	candidate: number;
+	lowestRollouts: { index: number; finalReward: number }[];    // finalReward ascending, ties -> lower index
+	highestRollouts: { index: number; finalReward: number }[];   // finalReward descending, ties -> lower index
+}
+
+/** Number of entries in a candidateExtremes block. */
+export function candidateExtremesCount(buf: VSBuffer): number {
+	return Math.floor(buf.byteLength / EXTREMES_BYTES);
+}
+
+/** The lists of candidate c from a candidateExtremes block (ApoScoreBlocks.candidateExtremes); indices are rollout positions on
+ *  the candidate's record axis, rewards the finalRewards the scoring call summed. */
+export function decodeCandidateExtremes(buf: VSBuffer, c: number): CandidateExtremes {
+	const base = c * EXTREMES_BYTES;
+	if (c < 0 || base + EXTREMES_BYTES > buf.byteLength) { throw new RangeError(`candidate ${c} outside the block`); }
+	const v = new DataView(buf.buffer.buffer, buf.buffer.byteOffset + base, EXTREMES_BYTES);
+	const n = Math.min(u64(v, OFF_EXT_N), EXTREMES_N);
+	const list = (offIdx: number, offRew: number) => Array.from({ length: n }, (_, i) => ({
+		index: Number(v.getBigInt64(offIdx + 8 * i, true)), finalReward: v.getFloat64(offRew + 8 * i, true),
+	}));
+	return { candidate: c, lowestRollouts: list(OFF_LOWEST, OFF_LOWEST_REWARD), highestRollouts: list(OFF_HIGHEST, OFF_HIGHEST_REWARD) };
 }
