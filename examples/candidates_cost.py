@@ -14,6 +14,12 @@ generated rows (positions and rewards bit for bit); on the rollout legs every li
 and R give the same bytes.  Leg W is Form D through its Form W copy (the Form T copy held beside it is switched off), leg
 FALL is 64 x 1 M strictly falling rows through K1, where every group of 32 evaluations runs the extremes' merge network.
 
+Every leg also times the step with the per-candidate group scores (APO_SCORE_CANDIDATE_GROUPS) in the same alternation, under
+five label planes: G = 1, and G = 5 and 64 both as contiguous runs (t * G // T) and as a new label on every record (t % G).
+The labels are uploaded before each such step, outside its timing.  On the fp32 legs the parity block is the group scores
+of two of the 8 candidates against the model of tests/group_fixtures.py over the generated rows (every field bit for bit);
+on the rollout legs the non-null counts of every candidate's groups add up to counts[c], and R16 and R give the same bytes.
+
     python examples/candidates_cost.py [--steps 10] [--legs D,W,Q,T,R16,R,FALL] [--out FILE.json]
 
 Prints one JSON object; the card name and power limit are read in the same run (nvidia-smi query)."""
@@ -73,26 +79,83 @@ def extremes_parity(res, ref_ext):
     return {"candidates": list(ok), "equal": all(ok.values())}
 
 
-def leg(eng, C, K, steps, score_kw, ref, picks, ref_ext=None):
-    """plain / candidates / extremes steps, alternating (ref None: the breakdown is not timed)"""
-    kinds = {"plain": {}, "extremes": {"extremes": True}}
-    if ref is not None:
-        kinds["candidates"] = {"candidates": True}
+def label_sets(T):
+    """name -> (labels, G): G = 1, and G = 5 / 64 as contiguous runs and as a new label on every record"""
+    t = np.arange(T, dtype=np.int64)
+    out = {"groups_g1": (np.zeros(T, np.uint8), 1)}
+    for G in (5, 64):
+        out[f"groups_g{G}_runs"] = ((t * G) // T).astype(np.uint8), G
+        out[f"groups_g{G}_every"] = (t % G).astype(np.uint8), G
+    return out
+
+
+def group_rows(x):
+    return [[(s.total, s.good, s.bad, bits(s.goodRate), s.withReward, bits(s.rewardSum), bits(s.avgReward)) for s in row] for row in x]
+
+
+def model_rows(m):
+    return [[(s["total"], s["good"], s["bad"], bits(s["goodRate"]), s["withReward"], bits(s["rewardSum"]), bits(s["avgReward"]))
+             for s in row] for row in m]
+
+
+def groups_parity(last, sets, ref_grp):
+    """ref_grp: {candidate: {set name: model row}}; without models, every candidate's groups add up to counts[c]"""
+    out = {}
+    for k in sets:
+        r = last[k]
+        sums = all(sum(s.withReward for s in row) == int(n) for row, n in zip(r.groups, r.counts))
+        if ref_grp is None:
+            out[k] = {"equal": sums, "check": "sum of withReward == counts"}
+        else:
+            ok = {c: group_rows([r.groups[c]]) == model_rows([m[k]]) for c, m in ref_grp.items()}
+            out[k] = {"candidates": list(ok), "equal": all(ok.values()) and sums}
+    return out
+
+
+def timed(eng, C, K, steps, score_kw, kinds, sets):
+    """median / min of every kind of step, alternating; a group step first uploads its labels (outside the timing)"""
     times = {k: [] for k in kinds}
+
+    def one(k, kw):
+        if k in sets:
+            eng.record_groups_upload(*sets[k])
+        t0 = time.perf_counter(); r = eng.score(C, K, **kw, **score_kw); times[k].append(time.perf_counter() - t0)
+        return r
+
     for _ in range(2):                                          # warm every shape
-        for kw in kinds.values():
-            eng.score(C, K, **kw, **score_kw)
+        for k, kw in kinds.items():
+            one(k, kw)
+    for v in times.values():
+        v.clear()
     last = {}
     for _ in range(steps):                                      # alternate: drift and other tenants hit all alike
         for k, kw in kinds.items():
-            t0 = time.perf_counter(); last[k] = eng.score(C, K, **kw, **score_kw); times[k].append(time.perf_counter() - t0)
-    med = {k: float(np.median(v)) * 1e3 for k, v in times.items()}
+            last[k] = one(k, kw)
+    return last, times, {k: float(np.median(v)) * 1e3 for k, v in times.items()}
+
+
+def groups_block(last, med, sets, ref_grp):
+    return {"groups_ms_median": {k: round(med[k], 3) for k in sets}, "groups_ratio": {k: round(med[k] / med["plain"], 3) for k in sets},
+            "groups_same_scores": all(last[k].scores.tobytes() == last["plain"].scores.tobytes()
+                                      and last[k].topk.tobytes() == last["plain"].topk.tobytes() for k in sets),
+            "parity_groups": groups_parity(last, sets, ref_grp)}
+
+
+def leg(eng, C, K, steps, score_kw, ref, picks, ref_ext=None, sets=None, ref_grp=None):
+    """plain / candidates / extremes / groups steps, alternating (ref None: the breakdown is not timed)"""
+    sets = sets or {}
+    kinds = {"plain": {}, "extremes": {"extremes": True}}
+    if ref is not None:
+        kinds["candidates"] = {"candidates": True}
+    kinds.update({k: {"groups": True} for k in sets})
+    last, times, med = timed(eng, C, K, steps, score_kw, kinds, sets)
     out = {"plain_ms_median": round(med["plain"], 3), "extremes_ms_median": round(med["extremes"], 3),
            "extremes_ratio": round(med["extremes"] / med["plain"], 3), "min_ms": {k: round(min(v) * 1e3, 3) for k, v in times.items()},
            "launches": {k: int(r.timing.launches) for k, r in last.items()},
            "same_scores": last["extremes"].scores.tobytes() == last["plain"].scores.tobytes()
                           and last["extremes"].topk.tobytes() == last["plain"].topk.tobytes(),
            "parity_extremes": extremes_parity(last["extremes"], ref_ext)}
+    out.update(groups_block(last, med, sets, ref_grp))
     if ref is not None:
         r = last["candidates"]
         ok = [same(r.candidates[c], d) for c, d in zip(picks, ref)]
@@ -123,22 +186,16 @@ def same_corpus(r, ref):
     return (r.toolCalls, r.toolSucc, r.toolFail) == (ref.toolCalls, ref.toolSucc, ref.toolFail)
 
 
-def corpus_leg(eng, C, K, steps, score_kw, ref, picks, ref_corpus):
-    """plain / candidates / candidate_corpus / extremes steps, alternating, with the parity blocks"""
+def corpus_leg(eng, C, K, steps, score_kw, ref, picks, ref_corpus, sets):
+    """plain / candidates / candidate_corpus / extremes / groups steps, alternating, with the parity blocks"""
     kinds = {"plain": {}, "candidates": {"candidates": True}, "candidate_corpus": {"candidate_corpus": True}, "extremes": {"extremes": True}}
-    times = {k: [] for k in kinds}
-    for _ in range(2):                                          # warm every shape
-        for kw in kinds.values():
-            eng.score(C, K, **kw, **score_kw)
-    last = {}
-    for _ in range(steps):
-        for k, kw in kinds.items():
-            t0 = time.perf_counter(); last[k] = eng.score(C, K, **kw, **score_kw); times[k].append(time.perf_counter() - t0)
-    med = {k: float(np.median(v)) * 1e3 for k, v in times.items()}
+    kinds.update({k: {"groups": True} for k in sets})
+    last, times, med = timed(eng, C, K, steps, score_kw, kinds, sets)
     ok = [same(last["candidates"].candidates[c], d) for c, d in zip(picks, ref)]
     ok_c = [same_corpus(last["candidate_corpus"].candidate_corpus[c], d) for c, d in zip(picks, ref_corpus)]
     cc = last["candidate_corpus"].candidate_corpus
-    return {"plain_ms_median": round(med["plain"], 3), "candidates_ms_median": round(med["candidates"], 3),
+    return {**groups_block(last, med, sets, None), "groups_bytes": b"".join(bytes(last[k].groups) for k in sets),
+            "plain_ms_median": round(med["plain"], 3), "candidates_ms_median": round(med["candidates"], 3),
             "candidate_corpus_ms_median": round(med["candidate_corpus"], 3),
             "candidates_ratio": round(med["candidates"] / med["plain"], 3),
             "candidate_corpus_ratio": round(med["candidate_corpus"] / med["plain"], 3),
@@ -161,6 +218,7 @@ def main():
     import oracle
     from oracle import candidates as oc
     import extremes_fixtures as xf
+    import group_fixtures as gf
     legs = args.legs.split(",")
     out = {"card": card(), "steps": args.steps, "timing": "host clock around each synchronous apo_score call"}
     eng = pkg.Engine(0)
@@ -170,19 +228,25 @@ def main():
     try:
         if {"D", "W", "Q", "T"} & set(legs):
             ref = oc.cand_generated(seed, picks, 0, T, 300, nthreads=nth)
-            ref_ext = {c: xf.model(oracle.gen_dims(seed, c, 1, 0, T, 300, nth))[0] for c in (picks[0], picks[-1])}
+            sets = label_sets(T)
+            ref_ext, ref_grp = {}, {}
+            for c in (picks[0], picks[-1]):
+                d = oracle.gen_dims(seed, c, 1, 0, T, 300, nth)
+                ref_ext[c] = xf.model(d)[0]
+                ref_grp[c] = {k: gf.model(d, lab, G)[0] for k, (lab, G) in sets.items()}
+                del d
             if "D" in legs:
                 eng.dims_generate(seed, 0, C, 0, T, 300)
-                out["form_d_256x5M"] = leg(eng, C, K, args.steps, {}, ref, picks, ref_ext)
+                out["form_d_256x5M"] = leg(eng, C, K, args.steps, {}, ref, picks, ref_ext, sets, ref_grp)
             if "W" in legs:
                 eng.dims_generate(seed, 0, C, 0, T, 300)
                 eng.set_tuning(pkg.TUNE_NO_TWIN_T)
-                out["form_w_copy_256x5M"] = leg(eng, C, K, args.steps, {}, ref, picks, ref_ext)
+                out["form_w_copy_256x5M"] = leg(eng, C, K, args.steps, {}, ref, picks, ref_ext, sets, ref_grp)
                 eng.set_tuning(0)
             if "Q" in legs or "T" in legs:
                 eng.dims_generate_compact(seed, 0, C, 0, T, 300)
             if "Q" in legs:
-                out["form_q_256x5M"] = leg(eng, C, K, args.steps, {}, ref, picks, ref_ext)
+                out["form_q_256x5M"] = leg(eng, C, K, args.steps, {}, ref, picks, ref_ext, sets, ref_grp)
             if "T" in legs:
                 pc, pd = np.empty((C, T), np.uint32), np.empty((C, T), np.uint16)
                 for c in range(C):
@@ -192,7 +256,7 @@ def main():
                 del pc, pd
                 eng.tuples_upload(tl, th, tbook, book, d2book)
                 del tl, th
-                out["form_t_256x5M"] = leg(eng, C, K, args.steps, {"source": pkg.SRC_TUPLES}, ref, picks, ref_ext)
+                out["form_t_256x5M"] = leg(eng, C, K, args.steps, {"source": pkg.SRC_TUPLES}, ref, picks, ref_ext, sets, ref_grp)
         if {"R16", "R"} & set(legs):
             Cr = 128
             picks_r = [int(x) for x in np.linspace(0, Cr - 1, 8).round()]
@@ -200,21 +264,25 @@ def main():
             ref_rc = [oracle.report(oracle.gen_records(seed, oracle.STREAM_ROLLOUT, c, 1, 0, T, 300, nth), nthreads=nth) for c in picks_r]
             if "R16" in legs:
                 eng.rollouts16_generate(seed, 0, Cr, 0, T, 300)
-                out["form_r16_128x5M"] = corpus_leg(eng, Cr, K, args.steps, {"source": pkg.SRC_ROLLOUTS}, ref_r, picks_r, ref_rc)
+                out["form_r16_128x5M"] = corpus_leg(eng, Cr, K, args.steps, {"source": pkg.SRC_ROLLOUTS}, ref_r, picks_r, ref_rc, label_sets(T))
             if "R" in legs:
                 eng.rollouts_generate(seed, 0, Cr, 0, T, 300)
-                out["form_r_128x5M"] = corpus_leg(eng, Cr, K, args.steps, {"source": pkg.SRC_ROLLOUTS}, ref_r, picks_r, ref_rc)
+                out["form_r_128x5M"] = corpus_leg(eng, Cr, K, args.steps, {"source": pkg.SRC_ROLLOUTS}, ref_r, picks_r, ref_rc, label_sets(T))
             if "R16" in legs and "R" in legs:                   # the same rollouts: the same lists
                 out["r16_r_extremes_equal"] = out["form_r16_128x5M"]["extremes_bytes"] == out["form_r_128x5M"]["extremes_bytes"]
+                out["r16_r_groups_equal"] = out["form_r16_128x5M"]["groups_bytes"] == out["form_r_128x5M"]["groups_bytes"]
             for k in ("form_r16_128x5M", "form_r_128x5M"):
                 out.get(k, {}).pop("extremes_bytes", None)
+                out.get(k, {}).pop("groups_bytes", None)
         if "FALL" in legs:
             Cf, Tf = 64, 1_000_000
             d = xf.falling(Tf, 1)
             m = xf.model(d)[0]
+            sets_f = label_sets(Tf)
+            mg = {k: gf.model(d, lab, G)[0] for k, (lab, G) in sets_f.items()}
             eng.dims_upload(np.repeat(d, Cf, axis=0))
             eng.set_tuning(pkg.TUNE_NO_TWIN)
-            out["falling_rows_k1_64x1M"] = leg(eng, Cf, K, args.steps, {}, None, None, {0: m, Cf - 1: m})
+            out["falling_rows_k1_64x1M"] = leg(eng, Cf, K, args.steps, {}, None, None, {0: m, Cf - 1: m}, sets_f, {0: mg, Cf - 1: mg})
             eng.set_tuning(0)
     finally:
         eng.close()

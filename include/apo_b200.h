@@ -272,6 +272,7 @@ int apo_record_unpack16(const apo_record16 *in, uint64_t n, apo_record *out);
 #define APO_SCORE_CANDIDATES 0x8u /* also build the per-candidate breakdown (apo_candidate_reports) */
 #define APO_SCORE_CANDIDATE_CORPUS 0x10u /* also build the corpus report of every candidate's rollout records (apo_candidate_corpus_reports) */
 #define APO_SCORE_CANDIDATE_EXTREMES 0x20u /* also list the 32 lowest- and highest-reward evaluations of every candidate (apo_candidate_extremes) */
+#define APO_SCORE_CANDIDATE_GROUPS 0x40u /* also split every candidate's evaluations by record group (apo_candidate_groups) */
 typedef struct apo_score_opts {
 	uint32_t K;          /* beam width (top-K), 0..min(C, 16384) */
 	uint32_t source;     /* APO_SRC_* */
@@ -476,6 +477,36 @@ struct apo_candidate_extremes {
 	double   highestReward[APO_EXTREMES_N];
 };                                          /* 1032 bytes */
 int apo_candidate_extremes(apo_engine *e, uint32_t c0, uint32_t n, struct apo_candidate_extremes *out);
+/* Per-candidate group scores: where in the corpus candidate c wins or loses (one chat mode, one task category, a held-out
+ * split).  The caller labels every record position with a group; a scoring call that sets APO_SCORE_CANDIDATE_GROUPS then
+ * splits each candidate's evaluations by the group of their record.  It works wherever APO_SCORE_CANDIDATE_EXTREMES works
+ * (apo_score on every source and route, sessions, every apo_score_host*), combines with the other per-candidate flags in any
+ * mix, and leaves scores, counts, top-K and the other outputs as they are without it.
+ * Positions are those of the extremes: absolute record positions (the window's first included; a session covers every
+ * window it accumulated; the apo_score_host* calls use positions within the call's T); every candidate reads labels[t].
+ * Per (c, g), over the evaluations of c on records of group g that the call read:
+ *   total / good / bad:  tallies as apo_candidate_report (Form D / Q / P / T from d0, Form R / R16 from the feedback field);
+ *   withReward:          non-null evaluations; summed over g it is counts[c];
+ *   rewardSum:           the exact integer sum of rint(fr * 2^52) rounded once, fr bit for bit the finalReward the call summed
+ *                        into scores[c]; the integers of the G groups add up to the candidate's partial (apo_debug_partials);
+ *   avgReward:           rewardSum / withReward as the breakdown divides it (== scores[c] at G = 1), NaN when withReward == 0.
+ * Refusals, each before anything is launched and leaving no groups behind: APO_E_STATE with no labels uploaded, on a handle
+ * with more than one rank, for a session in which an accumulate did not set the flag, and for a session whose labels were
+ * uploaded again after it began to accumulate them; APO_E_ARG when a scored position is at or past the labels' T. */
+#define APO_GROUPS_MAX 64
+/* One label per record position: labels[t] < G, 1 <= G <= APO_GROUPS_MAX.  Held by the handle until the next call;
+ * T == 0 releases them.  Independent of dims / rollouts / corpus loads.  APO_E_ARG (the previous labels stay) when G is 0 or
+ * above APO_GROUPS_MAX or a label is >= G. */
+int apo_record_groups_upload(apo_engine *e, const uint8_t *labels, uint64_t T, uint32_t G);
+typedef struct apo_group_score {
+	uint64_t total, good, bad;     /* evaluations of c on records of group g that the call read; tallies as apo_candidate_report */
+	double   goodRate;             /* good / (good + bad), 0 when both are 0 */
+	uint64_t withReward;           /* non-null evaluations */
+	double   rewardSum, avgReward; /* exact sum of rint(fr * 2^52) rounded once; avgReward NaN when withReward == 0 */
+} apo_group_score;                 /* 56 bytes */
+/* out = [n][G] for candidates [c0, c0 + n) of the last scoring call; G must be the G that call scored with (APO_E_ARG
+ * otherwise).  APO_E_STATE when that call did not set the flag (or failed), APO_E_ARG when the range exceeds its C. */
+int apo_candidate_groups(apo_engine *e, uint32_t c0, uint32_t n, uint32_t G, apo_group_score *out);
 
 /* ---- multi-GPU: the record axis is sharded across ranks (one process per GPU, or one handle per GPU inside one
  * process); the packed int64 partial vectors of the shards are joined INSIDE the scoring launch: the finalising CTA

@@ -43,14 +43,15 @@ typedef enum {
 	APO_JOB_ROLLOUTS_UPLOAD,       /* rolloutsUpload(handle, recs, rowBytes 32|16, C, T)         */
 	APO_JOB_CORPUS_UPLOAD,         /* corpusUpload(handle, recs apo_record[T], idxBase)          */
 	APO_JOB_CORPUS_UPLOAD_JSON,    /* corpusUploadJson(handle, utf8, idxBase)                    */
-	APO_JOB_SCORE_RESIDENT,        /* scoreResident(handle, {K, source, corpus, first, count, candidates, candidateCorpus, candidateExtremes}) */
-	APO_JOB_SCORE_HOST,            /* score(handle, dims, C, T, corpus|null, K, candidates?, candidateExtremes?) */
-	APO_JOB_SCORE_HOST_RECORDS,    /* scoreHostRecords(handle, recs, rowBytes, C, T, corpus|null, K, candidates?, candidateCorpus?, candidateExtremes?) */
-	APO_JOB_SCORE_HOST_TUPLES,     /* scoreHostTuples(handle, {tl, th, tbookPc, tbookPd, codebook, d2book}, C, T, corpus|null, K, candidates?, candidateExtremes?) */
+	APO_JOB_SCORE_RESIDENT,        /* scoreResident(handle, {K, source, corpus, first, count, candidates, candidateCorpus, candidateExtremes, candidateGroups}) */
+	APO_JOB_SCORE_HOST,            /* score(handle, dims, C, T, corpus|null, K, candidates?, candidateExtremes?, candidateGroups?) */
+	APO_JOB_SCORE_HOST_RECORDS,    /* scoreHostRecords(handle, recs, rowBytes, C, T, corpus|null, K, candidates?, candidateCorpus?, candidateExtremes?, candidateGroups?) */
+	APO_JOB_SCORE_HOST_TUPLES,     /* scoreHostTuples(handle, {tl, th, tbookPc, tbookPd, codebook, d2book}, C, T, corpus|null, K, candidates?, candidateExtremes?, candidateGroups?) */
 	APO_JOB_REWARD_BATCH,          /* rewardBatch(handle, recs apo_record[n])                    */
 	APO_JOB_COMM_INIT,             /* commInit(handle, nranks, rank, id[128])                    */
 	APO_JOB_TEST_HOOK,             /* tests: calls hook(hook_arg) in its turn                    */
-	APO_JOB_DIMS_TUPLES            /* dimsTuples(handle, cap?) -> nTuples: resident Form T built from the loaded dims */
+	APO_JOB_DIMS_TUPLES,           /* dimsTuples(handle, cap?) -> nTuples: resident Form T built from the loaded dims */
+	APO_JOB_RECORD_GROUPS_UPLOAD   /* recordGroupsUpload(handle, labels u8[T], G): the record group of every position */
 } apo_job_kind;
 
 typedef struct apo_job {
@@ -63,6 +64,7 @@ typedef struct apo_job {
 	uint32_t n_tuples;
 	uint32_t cap;                                 /* dimsTuples: dictionary capacity, <= APO_TUPLES_MAX */
 	uint32_t C, K, row_bytes, source, flags;
+	uint32_t G;                                   /* recordGroupsUpload: groups of the labels; scoring jobs with APO_SCORE_CANDIDATE_GROUPS: the G they were uploaded with */
 	uint64_t T, first, count, idx_base;
 	int compact;
 	int nranks, rank; uint8_t comm_id[APO_UNIQUE_ID_BYTES];
@@ -72,6 +74,7 @@ typedef struct apo_job {
 	apo_candidate_report *candidates;             /* [C], only when flags has APO_SCORE_CANDIDATES (apo_candidate_reports) */
 	apo_corpus_report *candidate_corpus;          /* [C], only when flags has APO_SCORE_CANDIDATE_CORPUS (apo_candidate_corpus_reports) */
 	struct apo_candidate_extremes *candidate_extremes;   /* [C], only when flags has APO_SCORE_CANDIDATE_EXTREMES (apo_candidate_extremes) */
+	apo_group_score *candidate_groups;            /* [C][G], only when flags has APO_SCORE_CANDIDATE_GROUPS (apo_candidate_groups) */
 	double *dims_out; uint32_t *masks_out; double *finals_out; uint64_t n_out;
 	int rc; char err[256];
 } apo_job;
@@ -85,6 +88,8 @@ typedef struct apo_job {
 /* Same cap for the per-candidate extremes (C x sizeof(struct apo_candidate_extremes) = 1032 B): about 4.16 M candidates.
  * They belong to every scoring job. */
 #define APO_JOB_CANDIDATE_EXTREMES_MAX_BYTES (1ull << 32)
+/* Same cap for the per-candidate group scores (C x G x sizeof(apo_group_score) = 56 B each).  They belong to every scoring job. */
+#define APO_JOB_CANDIDATE_GROUPS_MAX_BYTES (1ull << 32)
 
 /* Shape / size / overflow checks that need no engine; 0 = fine, else APO_E_ARG with the reason in j->err.
  * Everything that arrives from the renderer over IPC passes through here before a pointer is dereferenced. */

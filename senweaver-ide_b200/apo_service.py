@@ -22,7 +22,7 @@ import uuid
 
 import numpy as np
 
-from .engine import DIM_NAMES, MODE_NAMES, SRC_DIMS, SRC_ROLLOUTS, Engine
+from .engine import DIM_NAMES, GROUPS_MAX, MODE_NAMES, SRC_DIMS, SRC_ROLLOUTS, Engine
 from .jsfmt import js_substring, js_to_fixed
 from .trace_collector import TraceCollectorService
 
@@ -84,6 +84,7 @@ class APOService:
         self._stateListeners, self._suggestionListeners = [], []
         self._dirty = False
         self._lastRolloutCount = 0
+        self._groupNames = None                                               # names of the record groups of the last evaluateBeam
         api = (getattr(productService, "senweaverApiConfig", None) or {}).get("apiBaseUrl") if productService else None
         self._apoApiUrl = f"{api or 'https://ide-api.senweaver.com'}/api/apo"          # APO:328-329
         self._loadFromStorage()
@@ -212,7 +213,7 @@ class APOService:
                             "relatedCategory": DIM_CATEGORY.get(name, "core_behavior"), "examples": []})
         return out
 
-    def candidateReport(self, res, c):
+    def candidateReport(self, res, c, groupNames=None):
         """The report of one beam candidate, shaped like _buildReport's, from a ScoreResult scored with the per-candidate
         breakdown (evaluateBeam(..., reports=True)): feedback tallies and goodRate of its rollouts, avgReward (== its score),
         rewardByDimension, the dimension-low patterns and the suggestions they raise (the rules of APO:574-596, 800-827, by
@@ -223,7 +224,10 @@ class APOService:
         mode rules of APO:830-859 as well.  When the result carries the per-candidate extremes (extremes=True), the report
         adds lowestRollouts / highestRollouts: the candidate's 32 lowest- and highest-reward rollouts as {"index", "finalReward"}
         (reward ascending / descending, ties -> lower index), the sample runs the critique step reads; the caller looks the
-        rollouts up by index.  Pure: it neither records the suggestions nor fires events nor touches storage."""
+        rollouts up by index.  When the result carries the per-candidate group scores (evaluateBeam(..., groups=(labels, names))),
+        the report adds byGroup: {name: {totalRollouts, goodFeedbackCount, badFeedbackCount, goodRate, avgReward}} over the
+        candidate's rollouts in each record group (avgReward None when none of them has a reward); names default to those of the
+        last evaluateBeam.  Pure: it neither records the suggestions nor fires events nor touches storage."""
         cc = res.candidate_corpus[c] if getattr(res, "candidate_corpus", None) is not None else None
         r = res.candidates[c] if res.candidates is not None else cc
         goodRate = float(r.goodRate)
@@ -247,7 +251,22 @@ class APOService:
             n = int(ex.n)
             out["lowestRollouts"] = [{"index": int(ex.lowest[i]), "finalReward": float(ex.lowestReward[i])} for i in range(n)]
             out["highestRollouts"] = [{"index": int(ex.highest[i]), "finalReward": float(ex.highestReward[i])} for i in range(n)]
+        gs = res.groups[c] if getattr(res, "groups", None) is not None else None
+        if gs is not None:
+            names = groupNames if groupNames is not None else (self._groupNames or [str(g) for g in range(len(gs))])
+            out["byGroup"] = {names[g]: {"totalRollouts": int(x.total), "goodFeedbackCount": int(x.good), "badFeedbackCount": int(x.bad),
+                                         "goodRate": float(x.goodRate), "avgReward": None if x.withReward == 0 else float(x.avgReward)}
+                              for g, x in enumerate(gs)}
         return out
+
+    @staticmethod
+    def _checkGroups(groups):
+        """(labels, names) of evaluateBeam / runBeamSearch: one uint8 label per rollout index, names unique, 1..GROUPS_MAX of them."""
+        labels, names = groups
+        names = list(names)
+        if not 1 <= len(names) <= GROUPS_MAX or len(set(names)) != len(names):
+            raise ValueError(f"record groups need 1..{GROUPS_MAX} unique names, got {names!r}")
+        return np.ascontiguousarray(labels, np.uint8).reshape(-1), names
 
     @staticmethod
     def _example_detail(p, t):
@@ -300,14 +319,15 @@ class APOService:
         return out
 
     # ---- beam evaluation: the step the reference delegates to its backend --------------------------------
-    def evaluateBeam(self, candidates, dims=None, rollouts=None, reports=False, patterns=False, extremes=False):
+    def evaluateBeam(self, candidates, dims=None, rollouts=None, reports=False, patterns=False, extremes=False, groups=None):
         """Score a beam of VersionedPromptTemplate candidates on their rollout outcomes and keep the
         top `beamWidth` (score desc, ties -> lower index), then apply the APO:1138-1166 update with the
         strict `>` adoption rule (APO:1159).  dims: float32 [C][T][9] (NaN = absent) or rollouts:
         apo_record [C][T].  reports=True also builds the per-candidate breakdown (res.candidates, see
         candidateReport); with rollouts, reports=True and patterns=True also build every candidate's corpus
         report (res.candidate_corpus: problem patterns, per-mode tallies, tool totals).  extremes=True also lists every
-        candidate's 32 lowest- and highest-reward rollouts (res.extremes)."""
+        candidate's 32 lowest- and highest-reward rollouts (res.extremes).  groups=(labels, names) also splits every candidate's
+        rollouts by record group (res.groups [C][G]): labels[t] < len(names) is the group of rollout index t."""
         try:
             C = len(candidates)
             K = min(self._config["beamWidth"], C)
@@ -316,6 +336,11 @@ class APOService:
                 extra["candidate_corpus"] = True
             if extremes:
                 extra["extremes"] = True
+            if groups is not None:
+                labels, names = self._checkGroups(groups)
+                self._engine.record_groups_upload(labels, len(names))
+                self._groupNames = names
+                extra["groups"] = True
             if dims is not None:
                 self._engine.dims_upload(np.ascontiguousarray(dims, np.float32))
                 res = self._engine.score(C, K, source=SRC_DIMS, **extra)
@@ -336,7 +361,7 @@ class APOService:
             return None
 
     def runBeamSearch(self, seedPrompt, proposeCandidates, rolloutDims=None, rounds=None, withReports=False, rolloutRecords=None,
-                      withExtremes=False):
+                      withExtremes=False, rolloutGroups=None):
         """Client-side round driver (SURVEY 8f rank 3) around the GPU top-K: each round expands every beam
         member into `branchFactor` children through the caller's `proposeCandidates(parent, n) -> [content]`
         hook (the LLM critique/edit step of APO:918-988 lives there), scores parents + children on
@@ -346,11 +371,17 @@ class APOService:
         scored it (None for the unscored seed), so that the critique can name what the parent lost on; with
         rolloutRecords that report also carries the parent's problem patterns, byMode and toolStats; withExtremes=True
         (which needs withReports=True) adds the parent's lowestRollouts / highestRollouts, indices into the rollouts the
-        caller scored it on.  Returns the final beam state."""
+        caller scored it on; rolloutGroups=(labels, names) (which needs withReports=True too) adds the parent's byGroup, so that
+        a label that marks a held-out part of the rollouts shows whether a child improved only where its critique looked.
+        Returns the final beam state."""
         if (rolloutDims is None) == (rolloutRecords is None):
             raise ValueError("runBeamSearch needs exactly one of rolloutDims / rolloutRecords")
         if withExtremes and not withReports:
             raise ValueError("runBeamSearch: withExtremes needs withReports=True (the lists travel in the candidate reports)")
+        if rolloutGroups is not None:
+            if not withReports:
+                raise ValueError("runBeamSearch: rolloutGroups needs withReports=True (the group scores travel in the candidate reports)")
+            rolloutGroups = self._checkGroups(rolloutGroups)
         rounds = rounds or self._config["beamRounds"]
         beam = [{"version": "v0", "content": seedPrompt, "score": None, "createdAt": time.time() * 1000.0}]
         counter = 0
@@ -366,9 +397,9 @@ class APOService:
                                   "parentVersion": parent["version"], "createdAt": time.time() * 1000.0})
             if rolloutRecords is not None:
                 res = self.evaluateBeam(cands, rollouts=rolloutRecords(cands), reports=withReports, patterns=withReports,
-                                        extremes=withExtremes)
+                                        extremes=withExtremes, groups=rolloutGroups)
             else:
-                res = self.evaluateBeam(cands, dims=rolloutDims(cands), reports=withReports, extremes=withExtremes)
+                res = self.evaluateBeam(cands, dims=rolloutDims(cands), reports=withReports, extremes=withExtremes, groups=rolloutGroups)
             if res is None:
                 break
             if withReports:

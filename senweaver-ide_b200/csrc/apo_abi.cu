@@ -236,6 +236,13 @@ struct apo_engine {
 	DevBuf<unsigned long long> ext_acc;      // [C][CX_WORDS] lists | [cand_ext_slots][CX_WORDS] segments of one launch
 	uint32_t ext_C = 0;
 	bool ext_armed = false, ext_every = true, ext_ready = false;         // as cand_armed / cand_every / cand_ready
+	// record groups (apo_record_groups_upload) and the per-candidate group scores (APO_SCORE_CANDIDATE_GROUPS, k_cand_groups)
+	DevBuf<uint8_t> grp_labels; uint64_t grp_T = 0; uint32_t grp_G = 0;
+	uint64_t grp_gen = 0;                    // counts uploads: a session's groups belong to the labels it armed with
+	DevBuf<long long> grp_acc;               // [C][G][GR_WORDS] words of the call or session
+	DevBuf<apo_group_score> grp_rep;         // [C][G] scores of the last flagged call
+	uint32_t grp_C = 0, grp_rep_G = 0, grp_arm_G = 0; uint64_t grp_arm_gen = 0;
+	bool grp_armed = false, grp_every = true, grp_ready = false;         // as cand_armed / cand_every / cand_ready
 };
 
 namespace {
@@ -606,6 +613,7 @@ int begin_score(apo_engine *e, uint32_t C, bool whole = false) {
 	e->cand_armed = false; e->cand_every = true; e->cand_ready = false;
 	e->ccorp_armed = false; e->ccorp_every = true; e->ccorp_ready = false;
 	e->ext_armed = false; e->ext_every = true; e->ext_ready = false;
+	e->grp_armed = false; e->grp_every = true; e->grp_ready = false;
 	e->timing = apo_timing{};
 	if (e->timing_on) CK(cudaEventRecord(e->ev[0], e->stream));
 	return APO_OK;
@@ -945,6 +953,67 @@ int ext_finish(apo_engine *e, uint32_t C) {
 	return APO_OK;
 }
 
+// ---- per-candidate group scores (APO_SCORE_CANDIDATE_GROUPS)
+bool wants_grp(const apo_score_opts *o) { return (o->flags & APO_SCORE_CANDIDATE_GROUPS) != 0; }
+
+// end: one past the last record position the call scores (0: not known here, a session's finish)
+int grp_check(apo_engine *e, uint64_t end) {
+	if (e->nranks > 1)
+		return fail(e, APO_E_STATE, "APO_SCORE_CANDIDATE_GROUPS is single-rank only: the per-candidate group scores are not joined across the %d ranks of this handle", e->nranks);
+	if (e->grp_T == 0) return fail(e, APO_E_STATE, "APO_SCORE_CANDIDATE_GROUPS: no record groups uploaded (apo_record_groups_upload)");
+	if (end > e->grp_T)
+		return fail(e, APO_E_ARG, "APO_SCORE_CANDIDATE_GROUPS: record position %llu is past the %llu labels uploaded", (unsigned long long)end - 1,
+		            (unsigned long long)e->grp_T);
+	return APO_OK;
+}
+
+// the words of C candidates under the labels' G (and cand_upload_tbook's table for Form T), before route_copy
+int grp_reserve(apo_engine *e, uint32_t C) {
+	CK(reserve(e, e->grp_acc, (uint64_t)(C ? C : 1) * e->grp_G * apo::GR_WORDS));
+	CK(reserve(e, e->cand_book, 8 * 16));
+	return APO_OK;
+}
+
+// zero the words of C candidates (first flagged launch of a call or session), which then belong to the labels held now
+int grp_arm(apo_engine *e, uint32_t C) {
+	if (int rc = grp_reserve(e, C)) return rc;
+	CK(cudaMemsetAsync(e->grp_acc.p, 0, (uint64_t)C * e->grp_G * apo::GR_WORDS * 8, e->stream));
+	e->grp_armed = true; e->grp_arm_G = e->grp_G; e->grp_arm_gen = e->grp_gen;
+	return APO_OK;
+}
+
+// the group pass over ev into candidates [cand_offset, ...)
+int launch_grp(apo_engine *e, const apo_score_opts *o, const Evals &ev, uint32_t cand_offset) {
+	if (!ev.count) return APO_OK;
+	if (ev.form == apo::CAND_T && !ev.t_once) { const int rc = cand_upload_tbook(e, ev.dict->book); if (rc) return rc; }
+	apo::CandGroupParams X{};
+	apo::CandParams &P = X.src;
+	P.C = ev.C; P.T = ev.count; P.idx_base = ev.idx_base; P.pitch_evals = ev.pitch_evals; P.lut = e->d_lut.p;
+	P.rows = ev.rows; P.q8 = ev.q8; P.d2 = ev.d2; P.li = ev.li; P.qw = ev.qw;
+	P.tl = ev.tl; P.th = ev.th;
+	if (ev.qt) P.cbf = ev.qt->cbf.p;
+	if (ev.form == apo::CAND_T) {
+		P.tb_pc = ev.dict->pc.p; P.tb_pd = ev.dict->pd.p; P.n_tuples = ev.dict->n; P.d2book = ev.dict->d2.p; P.tbook = e->cand_book.p;
+	}
+	X.W = e->W;
+	X.labels = e->grp_labels.p; X.G = e->grp_arm_G;
+	X.words = e->grp_acc.p + (uint64_t)cand_offset * X.G * apo::GR_WORDS;
+	CK(apo::run_cand_groups(X, ev.form, (o->flags & APO_SCORE_RECIP) != 0, e->sm_count, e->stream));
+	e->timing.launches++;
+	return APO_OK;
+}
+
+// words -> apo_group_score[C][G]
+int grp_finish(apo_engine *e, uint32_t C) {
+	const uint32_t G = e->grp_arm_G;
+	CK(reserve(e, e->grp_rep, (uint64_t)(C ? C : 1) * G));
+	CK(apo::run_cand_groups_report(e->grp_acc.p, C, G, e->grp_rep.p, e->stream));
+	e->timing.launches++;
+	CK(cudaStreamSynchronize(e->stream));
+	e->grp_C = C; e->grp_rep_G = G; e->grp_ready = true;
+	return APO_OK;
+}
+
 // K2 (+fused finalize) / allreduce / K3, then bring the result block home
 bool wants_corpus(const apo_engine *e, const apo_score_opts *o) { return (o->flags & APO_SCORE_CORPUS) && e->corpus_T > 0; }
 // the corpus words come from the digest instead of a scan of the records
@@ -1057,7 +1126,8 @@ int finish_score(apo_engine *e, const apo_score_opts *o, uint32_t C, double *sco
 	}
 	if (wants_cand(o) && (rc = cand_finish(e, C))) return rc;
 	if (wants_ccorp(o) && (rc = ccorp_finish(e, C))) return rc;
-	return wants_ext(o) ? ext_finish(e, C) : APO_OK;
+	if (wants_ext(o) && (rc = ext_finish(e, C))) return rc;
+	return wants_grp(o) ? grp_finish(e, C) : APO_OK;
 }
 
 // o's window against the T evaluations loaded
@@ -1085,11 +1155,14 @@ int score_check(apo_engine *e, const apo_score_opts *o, uint32_t C, uint64_t T, 
 	if (wants_cand(o) && (rc = cand_check(e))) return rc;
 	if (wants_ccorp(o) && (rc = ccorp_check(e, records))) return rc;
 	if (wants_ext(o) && (rc = ext_check(e))) return rc;
+	// the host-streaming calls check their T themselves (stream_host)
+	if (wants_grp(o) && T != kStreamed && (rc = grp_check(e, T == kSession ? 0 : (o->count ? o->first + o->count : T)))) return rc;
 	CK(cudaSetDevice(e->device));
 	if (T == kSession) return APO_OK;                               // a session's scratch was sized by apo_score_begin
 	if ((rc = ensure_scratch(e, C, o->K))) return rc;
 	if (wants_cand(o) && (rc = cand_reserve(e, C))) return rc;
 	if (wants_ext(o) && (rc = ext_reserve(e, C))) return rc;
+	if (wants_grp(o) && (rc = grp_reserve(e, C))) return rc;
 	return APO_OK;
 }
 
@@ -1104,6 +1177,7 @@ int score_arm(apo_engine *e, const apo_score_opts *o, uint32_t C, bool begin, ui
 	if (begin && (rc = begin_score(e, C, whole))) return rc;
 	if (wants_cand(o) && !e->cand_armed && (rc = cand_arm(e, C))) return rc;
 	if (wants_ext(o) && !e->ext_armed && (rc = ext_arm(e, C))) return rc;
+	if (wants_grp(o) && !e->grp_armed && (rc = grp_arm(e, C))) return rc;
 	return wants_ccorp(o) && !e->ccorp_armed ? ccorp_arm(e, C) : APO_OK;
 }
 
@@ -1675,6 +1749,7 @@ extern "C" void apo_destroy(apo_engine *e) {
 	e->d_lut.release(); e->corpus.release(); e->digest.release(); e->dims.release(); e->roll.release(); e->acc.release(); e->acc_joined.release(); e->acc_snapshot.release(); e->misc.release();
 	e->result.release(); e->keys.release(); e->sel_key.release(); e->sel_idx.release();
 	e->cand_acc.release(); e->cand_rep.release(); e->cand_book.release(); e->ccorp_acc.release(); e->ccorp_rep.release(); e->ext_acc.release();
+	e->grp_labels.release(); e->grp_acc.release(); e->grp_rep.release();
 	e->tup.release(); e->tups.release(); e->tvals.release();
 	e->win[0].release(); e->win[1].release(); e->batch_in.release(); e->batch_out.release(); e->batch_mask.release();
 	if (e->h_result) cudaFreeHost(e->h_result);
@@ -2098,18 +2173,22 @@ extern "C" int apo_score_accumulate(apo_engine *e, const apo_score_opts *o, uint
 	if (rc) return rc;
 	if ((uint64_t)cand_offset + ev.C > e->score_C) return fail(e, APO_E_ARG, "candidates [%u,%u) exceed C_total=%u", cand_offset, cand_offset + ev.C, e->score_C);
 	if ((rc = check_window(e, o, ev.count))) return rc;
-	const bool cand = wants_cand(o), ccorp = wants_ccorp(o), ext = wants_ext(o);
+	const bool cand = wants_cand(o), ccorp = wants_ccorp(o), ext = wants_ext(o), grp = wants_grp(o);
 	if (cand && (rc = cand_check(e))) return rc;
 	if (ccorp && (rc = ccorp_check(e, ev.records()))) return rc;
 	if (ext && (rc = ext_check(e))) return rc;
+	if (grp && (rc = grp_check(e, o->count ? o->first + o->count : ev.count))) return rc;
 	CK(cudaSetDevice(e->device));
 	if (cand && (rc = cand_reserve(e, e->score_C))) return rc;                                  // allocates: before route_copy
 	if (cand && e->cand_every && !e->cand_armed && (rc = cand_arm(e, e->score_C))) return rc;
 	if (ext && e->ext_every && !e->ext_armed && (rc = ext_arm(e, e->score_C))) return rc;      // allocates too
+	if (grp && e->grp_every && !e->grp_armed && (rc = grp_arm(e, e->score_C))) return rc;      // and so does this
 	if ((rc = route_copy(e, o, &ev))) return rc;
 	if ((rc = resident_window(e, o, &ev)) || (rc = launch_score(e, o, ev, cand_offset))) return rc;
 	if (!ext) e->ext_every = false;
 	else if (e->ext_every && (rc = launch_ext(e, o, ev, cand_offset))) return rc;   // else finish refuses
+	if (!grp) e->grp_every = false;
+	else if (e->grp_every && e->grp_arm_gen == e->grp_gen && (rc = launch_grp(e, o, ev, cand_offset))) return rc;   // else finish refuses
 	if (!ccorp) e->ccorp_every = false;
 	else if (e->ccorp_every) {                          // an earlier accumulate of the session did not set the flag: finish refuses
 		if (!e->ccorp_armed && (rc = ccorp_arm(e, e->score_C))) return rc;
@@ -2123,11 +2202,15 @@ extern "C" int apo_score_accumulate(apo_engine *e, const apo_score_opts *o, uint
 extern "C" int apo_score_finish(apo_engine *e, const apo_score_opts *o, double *scores, uint64_t *counts, int32_t *topk,
                                 apo_corpus_report *report) {
 	if (!e) return APO_E_ARG;
-	e->cand_ready = e->ccorp_ready = e->ext_ready = false;   // a failed finish leaves no breakdown behind either
+	e->cand_ready = e->ccorp_ready = e->ext_ready = e->grp_ready = false;   // a failed finish leaves no breakdown behind either
 	if (!o) return fail(e, APO_E_ARG, "opts is NULL");
 	if (!e->scoring) return fail(e, APO_E_STATE, "apo_score_begin has not been called");
 	int rc = score_check(e, o, e->score_C, kSession, true);      // the accumulate calls refused every other source
 	if (rc) return rc;
+	if (wants_grp(o) && !e->grp_every)
+		return fail(e, APO_E_STATE, "APO_SCORE_CANDIDATE_GROUPS: every apo_score_accumulate of the session must set the flag for the group scores");
+	if (wants_grp(o) && e->grp_armed && e->grp_arm_gen != e->grp_gen)
+		return fail(e, APO_E_STATE, "APO_SCORE_CANDIDATE_GROUPS: the record groups were uploaded again after the session began to accumulate them");
 	if (wants_cand(o) && !e->cand_every)
 		return fail(e, APO_E_STATE, "APO_SCORE_CANDIDATES: every apo_score_accumulate of the session must set the flag for a breakdown");
 	if (wants_ccorp(o) && !e->ccorp_every)
@@ -2140,7 +2223,7 @@ extern "C" int apo_score_finish(apo_engine *e, const apo_score_opts *o, double *
 
 extern "C" int apo_score(apo_engine *e, const apo_score_opts *o, double *scores, uint64_t *counts, int32_t *topk, apo_corpus_report *report) {
 	if (!e) return APO_E_ARG;
-	e->cand_ready = e->ccorp_ready = e->ext_ready = false;   // a failed call leaves no breakdown behind either
+	e->cand_ready = e->ccorp_ready = e->ext_ready = e->grp_ready = false;   // a failed call leaves no breakdown behind either
 	Evals ev;
 	int rc = resident_evals(e, o, &ev);
 	if (rc) return rc;
@@ -2182,6 +2265,7 @@ extern "C" int apo_score(apo_engine *e, const apo_score_opts *o, double *scores,
 	if (wants_cand(o) && (rc = launch_cand(e, ev, 0))) return rc;
 	if (wants_ccorp(o) && (rc = launch_ccorp(e, ev, 0))) return rc;
 	if (wants_ext(o) && (rc = launch_ext(e, o, ev, 0))) return rc;
+	if (wants_grp(o) && (rc = launch_grp(e, o, ev, 0))) return rc;
 	return finish_score(e, o, C, scores, counts, topk, report, fused);
 }
 
@@ -2232,7 +2316,7 @@ int stream_host(apo_engine *e, const apo_score_opts *o, const HostTensor &h, dou
                 apo_corpus_report *report) {
 	const uint32_t C = h.C;
 	const uint64_t T = h.T;
-	e->cand_ready = e->ccorp_ready = e->ext_ready = false;
+	e->cand_ready = e->ccorp_ready = e->ext_ready = e->grp_ready = false;
 	if (!o) return fail(e, APO_E_ARG, "opts is NULL");
 	const bool rows = h.form != apo::CAND_Q && h.form != apo::CAND_T;
 	if (!rows && wants_ccorp(o)) return ccorp_check(e, false);   // the wire formats refuse it before they look at their inputs
@@ -2248,7 +2332,7 @@ int stream_host(apo_engine *e, const apo_score_opts *o, const HostTensor &h, dou
 	}
 	Evals ev;
 	ev.form = h.form; ev.C = C; ev.variant = (int)o->variant;
-	if ((rc = score_check(e, o, C, kStreamed, ev.records())) || (rc = digest_prepare(e, o))) return rc;
+	if ((rc = score_check(e, o, C, kStreamed, ev.records())) || (wants_grp(o) && (rc = grp_check(e, T))) || (rc = digest_prepare(e, o))) return rc;
 	if (h.form == apo::CAND_Q) {                                   // Form Q / P: K1q's tables of this call's codebook
 		if ((rc = load_qtables(e, e->qt_stream, h.codebook))) return rc;
 		ev.qt = &e->qt_stream;
@@ -2283,7 +2367,7 @@ int stream_host(apo_engine *e, const apo_score_opts *o, const HostTensor &h, dou
 	}
 	if ((rc = score_arm(e, o, C, true, (uint64_t)C * T * wire))) return rc;
 	if (h.form == apo::CAND_T) {                                   // the dictionary and its values, once for the whole call
-		if ((wants_cand(o) || wants_ext(o)) && (rc = cand_upload_tbook(e, h.codebook))) return rc;
+		if ((wants_cand(o) || wants_ext(o) || wants_grp(o)) && (rc = cand_upload_tbook(e, h.codebook))) return rc;
 		if ((rc = dict_upload(e, e->tups, h.tb_pc, h.tb_pd, h.n_tuples, h.codebook, h.d2book))) return rc;
 		ev.dict = &e->tups; ev.t_once = true;
 		if ((rc = tuple_values(e, e->tups, e->tvals, (o->flags & APO_SCORE_RECIP) != 0))) return rc;
@@ -2329,6 +2413,7 @@ int stream_host(apo_engine *e, const apo_score_opts *o, const HostTensor &h, dou
 		if (wants_cand(o) && (rc = launch_cand(e, ev, 0))) return rc;
 		if (wants_ccorp(o) && (rc = launch_ccorp(e, ev, 0))) return rc;   // before the window is released
 		if (wants_ext(o) && (rc = launch_ext(e, o, ev, 0))) return rc;
+		if (wants_grp(o) && (rc = launch_grp(e, o, ev, 0))) return rc;
 		CK(cudaEventRecord(e->win_free[b], e->stream));
 	}
 	return finish_score(e, o, C, scores, counts, topk, report, false, h.packed);
@@ -2648,6 +2733,40 @@ extern "C" int apo_candidate_extremes(apo_engine *e, uint32_t c0, uint32_t n, st
 			}
 		}
 	}
+	return APO_OK;
+}
+
+extern "C" int apo_record_groups_upload(apo_engine *e, const uint8_t *labels, uint64_t T, uint32_t G) {
+	if (!e) return APO_E_ARG;
+	if (T == 0) {
+		CK(cudaSetDevice(e->device));
+		e->grp_labels.release();
+		e->grp_T = 0; e->grp_G = 0; e->grp_gen++;
+		return APO_OK;
+	}
+	if (G == 0 || G > APO_GROUPS_MAX) return fail(e, APO_E_ARG, "G=%u outside [1, %d]", G, APO_GROUPS_MAX);
+	if (!labels) return fail(e, APO_E_ARG, "labels is NULL");
+	for (uint64_t t = 0; t < T; t++)                                // from outside the program: the pass indexes its accumulators by them
+		if (labels[t] >= G) return fail(e, APO_E_ARG, "labels[%llu]=%u is not below G=%u", (unsigned long long)t, labels[t], G);
+	CK(cudaSetDevice(e->device));
+	e->grp_T = 0; e->grp_G = 0; e->grp_gen++;                      // the previous labels are gone once the buffer is reused
+	CK(reserve(e, e->grp_labels, T));
+	CK(cudaMemcpyAsync(e->grp_labels.p, labels, T, cudaMemcpyHostToDevice, e->stream));   // after every queued pass that reads them
+	CK(cudaStreamSynchronize(e->stream));
+	e->grp_T = T; e->grp_G = G;
+	return APO_OK;
+}
+
+extern "C" int apo_candidate_groups(apo_engine *e, uint32_t c0, uint32_t n, uint32_t G, apo_group_score *out) {
+	if (!e) return APO_E_ARG;
+	if (!e->grp_ready) return fail(e, APO_E_STATE, "the last scoring call did not set APO_SCORE_CANDIDATE_GROUPS");
+	if (G != e->grp_rep_G) return fail(e, APO_E_ARG, "G=%u is not the G=%u the last scoring call split by", G, e->grp_rep_G);
+	if ((uint64_t)c0 + n > e->grp_C) return fail(e, APO_E_ARG, "candidates [%u,%llu) exceed C=%u", c0, (unsigned long long)c0 + n, e->grp_C);
+	if (n == 0) return APO_OK;
+	if (!out) return fail(e, APO_E_ARG, "out is NULL");
+	CK(cudaSetDevice(e->device));
+	CK(cudaMemcpyAsync(out, e->grp_rep.p + (uint64_t)c0 * G, (uint64_t)n * G * sizeof(apo_group_score), cudaMemcpyDeviceToHost, e->stream));
+	CK(cudaStreamSynchronize(e->stream));
 	return APO_OK;
 }
 

@@ -38,6 +38,16 @@ struct CandEval { double v[APO_NDIM]; uint32_t mask; uint32_t valid; uint32_t fb
 
 __device__ __forceinline__ uint32_t mag_bits(float f) { return __float_as_uint(f) & 0x7FFFFFFFu; }
 
+// The finalReward of a non-null evaluation, bit for bit the one the scoring kernels sum: TCS:777-784 in push order with
+// absent values +0.0, divided through the total-weight LUT (tw) and its reciprocals (rc) as div_lut does
+template <bool RECIP>
+__device__ __forceinline__ double cand_final_reward(const CandEval &E, const Weights &W, const double *tw, const double *rc) {
+	double ws = 0.0;
+#pragma unroll
+	for (int i = 0; i < APO_NDIM; i++) ws = __dadd_rn(ws, __dmul_rn(E.v[i], W.w[i]));
+	return div_lut<RECIP>(ws, make_double2(tw[E.mask], rc[E.mask]));
+}
+
 // shared tables: the total-weight LUT and the code -> value table of the source (Form Q 8 x 256, Form T 8 x 16)
 struct CandSmem { double tw[512]; float tab[8 * 256]; };
 
@@ -605,10 +615,7 @@ k_cand_extremes(const CandExtParams X, uint32_t tiles_per_cand, uint64_t total_t
 					CandEval E;
 					L::decode(P, S, R[u], E);
 					if (E.valid) {
-						double ws = 0.0;                                    // TCS:777-784 in push order, absent values +0.0
-#pragma unroll
-						for (int i = 0; i < APO_NDIM; i++) ws = __dadd_rn(ws, __dmul_rn(E.v[i], X.W.w[i]));
-						const unsigned long long k = order_key(div_lut<RECIP>(ws, make_double2(S.tw[E.mask], s_rc[E.mask])));
+						const unsigned long long k = order_key(cand_final_reward<RECIP>(E, X.W, S.tw, s_rc));
 						kl = {k, P.idx_base + t};
 						kh = {~k, P.idx_base + t};
 					}
@@ -682,6 +689,189 @@ static cudaError_t run_ext(const CandExtParams &X, int source, int sm_count, cud
 
 cudaError_t run_cand_extremes(const CandExtParams &X, int source, bool recip, int sm_count, cudaStream_t st) {
 	return recip ? run_ext<true>(X, source, sm_count, st) : run_ext<false>(X, source, sm_count, st);
+}
+
+// ================================================================ per-candidate group scores (APO_SCORE_CANDIDATE_GROUPS)
+//   k_cand_groups<Loader, TABLE, RECIP>  one pass over the evaluations a scoring call reads, with the breakdown's loaders and
+//                                        tile walk: every group of 32 evaluations is split by the labels of its records
+//   k_cand_groups_report                 words -> apo_group_score[C][G] with the breakdown's report rules
+// A group of 32 evaluations is aggregated per label before it touches memory: the lanes that share a label (all 32 on the
+// fast path, __match_any_sync otherwise) reduce their terms with __reduce_add_sync, and the lowest of them adds the sums into
+// the warp's own shared accumulators of that label.  A term rint(fr * 2^52) enters as four 16-bit pieces of its two's
+// complement and a sign count, so 32 of them sum exactly in 32 bits whatever the labels are; the warp's accumulators hold a
+// run of CB_RUN_TILES tiles exactly (l0, l1 < 2^58, counts < 2^27) and are flushed into the (c, g) words when the candidate
+// changes and at the run limit, as k_cand_breakdown flushes.
+constexpr int GR_WARPS = CB_THREADS / 32;
+struct GroupSmem {
+	unsigned long long l0[GR_WARPS][APO_GROUPS_MAX], l1[GR_WARPS][APO_GROUPS_MAX];   // 2^0 and 2^32 limbs of the sum
+	uint32_t n[GR_WARPS][APO_GROUPS_MAX], good[GR_WARPS][APO_GROUPS_MAX], bad[GR_WARPS][APO_GROUPS_MAX];
+	uint32_t rew[GR_WARPS][APO_GROUPS_MAX], neg[GR_WARPS][APO_GROUPS_MAX];           // non-null terms, negative terms
+};
+// the fields of one evaluation (and, after __reduce_add_sync, of up to 32), 6 bits each
+constexpr int GP_N = 0, GP_GOOD = 6, GP_BAD = 12, GP_REW = 18, GP_NEG = 24;
+
+template <class L, int TABLE, bool RECIP>
+__global__ void __launch_bounds__(CB_THREADS, L::MIN_CTAS)
+k_cand_groups(const CandGroupParams X, uint32_t tiles_per_cand, uint64_t total_tiles) {
+	const CandParams &P = X.src;
+	__shared__ CandSmem S;
+	__shared__ double s_rc[512];                                        // reciprocal of the total weight (div_lut)
+	__shared__ GroupSmem A;
+	for (int i = threadIdx.x; i < 512; i += CB_THREADS) { S.tw[i] = P.lut[i]; s_rc[i] = P.lut[512 + i]; }
+	if (TABLE == 1) for (int i = threadIdx.x; i < 8 * 256; i += CB_THREADS) S.tab[i] = P.cbf[i];
+	if (TABLE == 2) for (int i = threadIdx.x; i < 8 * 16; i += CB_THREADS) S.tab[i] = P.tbook[i];
+	const int lane = threadIdx.x & 31, wp = threadIdx.x >> 5;
+	for (int g = lane; g < APO_GROUPS_MAX; g += 32) {
+		A.l0[wp][g] = A.l1[wp][g] = 0ull;
+		A.n[wp][g] = A.good[wp][g] = A.bad[wp][g] = A.rew[wp][g] = A.neg[wp][g] = 0u;
+	}
+	__syncthreads();
+	const uint64_t nwarps = (uint64_t)gridDim.x * GR_WARPS;
+	const uint64_t gw = (uint64_t)blockIdx.x * GR_WARPS + wp;
+	const uint64_t lo = total_tiles * gw / nwarps, hi = total_tiles * (gw + 1) / nwarps;
+	if (lo >= hi) return;
+	const uint8_t *labels = X.labels + P.idx_base;
+	const uint32_t G = X.G;
+	uint32_t run = 0;
+
+	auto flush = [&](uint32_t c) {
+		__syncwarp();
+		for (uint32_t g = lane; g < G; g += 32) {
+			unsigned long long *w = (unsigned long long *)X.words + ((uint64_t)c * G + g) * GR_WORDS;
+			const unsigned long long a0 = A.l0[wp][g], a1 = A.l1[wp][g];
+			const uint32_t neg = A.neg[wp][g], rew = A.rew[wp][g], n = A.n[wp][g], good = A.good[wp][g], bad = A.bad[wp][g];
+			if (a0) atomicAdd(w + 0, a0);
+			if (a1) atomicAdd(w + 1, a1);
+			if (neg) atomicAdd(w + 2, 0ull - (unsigned long long)neg);   // each negative term carries -2^64
+			if (rew) atomicAdd(w + 3, (unsigned long long)rew);
+			if (n) atomicAdd(w + GR_TALLY, (unsigned long long)n);
+			if (good) atomicAdd(w + GR_TALLY + 1, (unsigned long long)good);
+			if (bad) atomicAdd(w + GR_TALLY + 2, (unsigned long long)bad);
+			A.l0[wp][g] = A.l1[wp][g] = 0ull;
+			A.n[wp][g] = A.good[wp][g] = A.bad[wp][g] = A.rew[wp][g] = A.neg[wp][g] = 0u;
+		}
+		__syncwarp();
+		run = 0;
+	};
+
+	uint32_t cur = (uint32_t)(lo / tiles_per_cand);
+	for (uint64_t tile = lo; tile < hi; tile++) {
+		const uint32_t c = (uint32_t)(tile / tiles_per_cand), j = (uint32_t)(tile - (uint64_t)c * tiles_per_cand);
+		if (c != cur || run == CB_RUN_TILES) { flush(cur); cur = c; }
+		run++;
+		const uint64_t t0 = (uint64_t)j * CB_TILE;
+		for (int g0 = 0; g0 < CB_GROUPS; g0 += L::U) {
+			typename L::Raw R[L::U];
+			bool in[L::U];
+			uint32_t lab[L::U];
+#pragma unroll
+			for (int u = 0; u < L::U; u++) {
+				const uint64_t t = t0 + (uint64_t)(g0 + u) * 32 + lane;
+				in[u] = t < P.T;
+				lab[u] = in[u] ? (uint32_t)__ldg(labels + t) : 0u;            // past the row end: label 0, nothing added
+				if (in[u]) L::fetch(P, c, t, R[u]);
+			}
+#pragma unroll
+			for (int u = 0; u < L::U; u++) {
+				if (t0 + (uint64_t)(g0 + u) * 32 >= P.T) break;                 // warp-uniform: the rest of the tile is past the row end
+				uint32_t pk = 0;
+				unsigned long long x = 0ull;
+				if (in[u]) {
+					CandEval E;
+					L::decode(P, S, R[u], E);
+					pk = (1u << GP_N) | ((E.fb == 1u ? 1u : 0u) << GP_GOOD) | ((E.fb == 2u ? 1u : 0u) << GP_BAD);
+					if (E.valid) {
+						const long long fx = to_fx(cand_final_reward<RECIP>(E, X.W, S.tw, s_rc));
+						x = (unsigned long long)fx;
+						pk |= (1u << GP_REW) | ((fx < 0 ? 1u : 0u) << GP_NEG);
+					}
+				}
+				const uint32_t l = lab[u];
+				const uint32_t peers = __all_sync(FULL, l == __shfl_sync(FULL, l, 0)) ? FULL : __match_any_sync(FULL, l);
+				uint32_t s0 = (uint32_t)x & 0xFFFFu, s1 = (uint32_t)(x >> 16) & 0xFFFFu, s2 = (uint32_t)(x >> 32) & 0xFFFFu;
+				uint32_t s3 = (uint32_t)(x >> 48), sp = pk;
+				if (peers != (1u << lane)) {                                    // a label of its own needs no reduction: the
+					s0 = __reduce_add_sync(peers, s0);                          // reductions run once per distinct peer mask
+					s1 = __reduce_add_sync(peers, s1);
+					s2 = __reduce_add_sync(peers, s2);
+					s3 = __reduce_add_sync(peers, s3);
+					sp = __reduce_add_sync(peers, sp);
+				}
+				if (lane == __ffs((int)peers) - 1) {                          // the lowest lane of the label: one writer per label
+					A.l0[wp][l] += (unsigned long long)s0 + ((unsigned long long)s1 << 16);
+					A.l1[wp][l] += (unsigned long long)s2 + ((unsigned long long)s3 << 16);
+					A.n[wp][l] += (sp >> GP_N) & 63u;
+					A.good[wp][l] += (sp >> GP_GOOD) & 63u;
+					A.bad[wp][l] += (sp >> GP_BAD) & 63u;
+					A.rew[wp][l] += (sp >> GP_REW) & 63u;
+					A.neg[wp][l] += (sp >> GP_NEG) & 63u;
+				}
+				__syncwarp();                                                   // the next group's writer of a label may be another lane
+			}
+		}
+	}
+	flush(cur);
+}
+
+template <class L, int TABLE, bool RECIP>
+static cudaError_t launch_grp(const CandGroupParams &X, int sm_count, cudaStream_t st) {
+	const CandParams &P = X.src;
+	const uint32_t tiles_per_cand = (uint32_t)((P.T + CB_TILE - 1) / CB_TILE);
+	const uint64_t total_tiles = (uint64_t)tiles_per_cand * P.C;
+	if (total_tiles == 0) return cudaSuccess;
+	int per_sm = 0;
+	cudaError_t err = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_cand_groups<L, TABLE, RECIP>, CB_THREADS, 0);
+	if (err != cudaSuccess) return err;
+	uint64_t grid = (uint64_t)sm_count * (uint64_t)(per_sm > 0 ? per_sm : 1);
+	const uint64_t need = (total_tiles + GR_WARPS - 1) / GR_WARPS;
+	if (grid > need) grid = need;
+	if (cand_env_grid() && cand_env_grid() < grid) grid = cand_env_grid();
+	k_cand_groups<L, TABLE, RECIP><<<(unsigned)grid, CB_THREADS, 0, st>>>(X, tiles_per_cand, total_tiles);
+	return cudaGetLastError();
+}
+
+template <bool RECIP>
+static cudaError_t run_grp(const CandGroupParams &X, int source, int sm_count, cudaStream_t st) {
+	switch (source) {
+	case CAND_DIMS: return launch_grp<LoadDims, 0, RECIP>(X, sm_count, st);
+	case CAND_REC32: return launch_grp<LoadRec<32>, 0, RECIP>(X, sm_count, st);
+	case CAND_REC16: return launch_grp<LoadRec<16>, 0, RECIP>(X, sm_count, st);
+	case CAND_Q: return launch_grp<LoadQ, 1, RECIP>(X, sm_count, st);
+	case CAND_T: return launch_grp<LoadT, 2, RECIP>(X, sm_count, st);
+	case CAND_W: return launch_grp<LoadW, 1, RECIP>(X, sm_count, st);
+	default: return cudaErrorInvalidValue;
+	}
+}
+
+cudaError_t run_cand_groups(const CandGroupParams &X, int source, bool recip, int sm_count, cudaStream_t st) {
+	return recip ? run_grp<true>(X, source, sm_count, st) : run_grp<false>(X, source, sm_count, st);
+}
+
+// one thread per (c, g)
+__global__ void __launch_bounds__(256)
+k_cand_groups_report(const long long *words, uint64_t n, apo_group_score *out) {
+	const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+	if (i >= n) return;
+	const long long *w = words + i * GR_WORDS;
+	apo_group_score R;
+	R.total = (uint64_t)w[GR_TALLY];
+	R.good = (uint64_t)w[GR_TALLY + 1];
+	R.bad = (uint64_t)w[GR_TALLY + 2];
+	R.goodRate = report_good_rate(R.good, R.bad);
+	R.withReward = (uint64_t)w[3];
+	// l0 and l1 hold sums of unsigned 32-bit limbs: carry them into the signed limbs limbs_to_double reads
+	const __int128 v = ((__int128)w[2] << 64) + ((__int128)(unsigned long long)w[1] << 32) + (__int128)(unsigned long long)w[0];
+	const long long l[3] = {(long long)(v & 0xFFFFFFFF), (long long)((v >> 32) & 0xFFFFFFFF), (long long)(v >> 64)};
+	R.rewardSum = limbs_to_double(l);
+	R.avgReward = report_avg_reward(R.rewardSum, R.withReward);
+	out[i] = R;
+}
+
+cudaError_t run_cand_groups_report(const long long *words, uint32_t C, uint32_t G, apo_group_score *out, cudaStream_t st) {
+	const uint64_t n = (uint64_t)C * G;
+	if (n == 0) return cudaSuccess;
+	k_cand_groups_report<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(words, n, out);
+	return cudaGetLastError();
 }
 
 }  // namespace apo

@@ -393,6 +393,22 @@ struct CandExtParams {
 };
 cudaError_t run_cand_extremes(const CandExtParams &P, int source, bool recip, int sm_count, cudaStream_t st);
 
+// ---- per-candidate group scores (csrc/apo_cand.cu): every candidate's evaluations split by the label of their record.
+// Own buffer [C][G][GR_WORDS]: l0, l1, l2, withReward (the scoring partials' layout: the exact sum of rint(fr * 2^52) is
+// l2 * 2^64 + l1 * 2^32 + l0), then total, good, bad and one unused word.
+constexpr int GR_WORDS = 8;
+constexpr int GR_TALLY = 4;
+struct CandGroupParams {
+	CandParams src;                 // the evaluations, as the breakdown reads them (ints / ex / dom unused)
+	Weights W;
+	const uint8_t *labels;          // [labels T] group of every record position (src.idx_base + t)
+	uint32_t G;                     // 1..APO_GROUPS_MAX
+	long long *words;               // [C][G][GR_WORDS] of candidate 0 of this launch
+};
+cudaError_t run_cand_groups(const CandGroupParams &P, int source, bool recip, int sm_count, cudaStream_t st);
+// words: the whole buffer of C candidates
+cudaError_t run_cand_groups_report(const long long *words, uint32_t C, uint32_t G, apo_group_score *out, cudaStream_t st);
+
 int k1_tile_evals(int row, int variant);
 cudaError_t run_reward9(K1Params P, int row, int variant, bool recip, int sm_count, cudaStream_t st);
 cudaError_t run_detect6(const K2Params &P, int sm_count, cudaStream_t st);

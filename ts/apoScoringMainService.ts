@@ -21,7 +21,7 @@ import { VSBuffer } from '../../../../base/common/buffer.js';
 import { ApoResidentQuery, ApoScoreBlocks, ApoTupleBuffers, IApoScoringService } from '../common/apoScoringService.js';
 
 type Blocks = { scores: ArrayBuffer; counts: ArrayBuffer; topk: ArrayBuffer; report: ArrayBuffer; candidates?: ArrayBuffer; candidateCorpus?: ArrayBuffer;
-	candidateExtremes?: ArrayBuffer };
+	candidateExtremes?: ArrayBuffer; candidateGroups?: ArrayBuffer };
 
 interface ApoAddon {
 	create(device: number): unknown | null;             // null when no H100 / library: never throws
@@ -31,15 +31,16 @@ interface ApoAddon {
 	corpusUpload(handle: unknown, records: ArrayBuffer, idxBase: number): Promise<void>;
 	corpusUploadJson(handle: unknown, utf8: ArrayBuffer, idxBase: number): Promise<number>;
 	dimsTuples(handle: unknown, cap?: number): Promise<number>;
+	recordGroupsUpload(handle: unknown, labels: ArrayBuffer, G: number): Promise<void>;
 	scoreResident(handle: unknown, query: ApoResidentQuery): Promise<Blocks>;
 	score(handle: unknown, dims: ArrayBuffer, C: number, T: number, corpus: ArrayBuffer | null, K: number, candidates?: boolean,
-		candidateExtremes?: boolean): Promise<Blocks>;
+		candidateExtremes?: boolean, candidateGroups?: number): Promise<Blocks>;
 	scoreHostRecords(handle: unknown, records: ArrayBuffer, rowBytes: number, C: number, T: number, corpus: ArrayBuffer | null, K: number,
-		candidates?: boolean, candidateCorpus?: boolean, candidateExtremes?: boolean): Promise<Blocks>;
+		candidates?: boolean, candidateCorpus?: boolean, candidateExtremes?: boolean, candidateGroups?: number): Promise<Blocks>;
 	/** Form D -> Form T on worker threads of the addon (no GPU): 3 bytes per evaluation instead of 36; null = not categorical. */
 	encodeTuples(dims: ArrayBuffer, C: number, T: number, nthreads?: number): Promise<ApoTuples | null>;
 	scoreHostTuples(handle: unknown, tuples: ApoTuples, C: number, T: number, corpus: ArrayBuffer | null, K: number, candidates?: boolean,
-		candidateExtremes?: boolean): Promise<Blocks>;
+		candidateExtremes?: boolean, candidateGroups?: number): Promise<Blocks>;
 	rewardBatch(handle: unknown, records: ArrayBuffer): Promise<{ dims: ArrayBuffer; masks: ArrayBuffer; finals: ArrayBuffer }>;
 	recordsFromJson(utf8: ArrayBuffer): ArrayBuffer | null;
 }
@@ -62,6 +63,7 @@ function wrapBlocks(r: Blocks): ApoScoreBlocks {
 	if (r.candidates) { out.candidates = VSBuffer.wrap(new Uint8Array(r.candidates)); }     // apo_candidate_report[C]
 	if (r.candidateCorpus) { out.candidateCorpus = VSBuffer.wrap(new Uint8Array(r.candidateCorpus)); }     // apo_corpus_report[C]
 	if (r.candidateExtremes) { out.candidateExtremes = VSBuffer.wrap(new Uint8Array(r.candidateExtremes)); }     // struct apo_candidate_extremes[C]
+	if (r.candidateGroups) { out.candidateGroups = VSBuffer.wrap(new Uint8Array(r.candidateGroups)); }     // apo_group_score[C][G]
 	return out;
 }
 
@@ -170,15 +172,19 @@ export class ApoScoringMainService implements IApoScoringService {
 		return (await this._need()).dimsTuples(this._handle, cap);
 	}
 
+	async recordGroupsUpload(labels: VSBuffer, G: number): Promise<void> {
+		return (await this._need()).recordGroupsUpload(this._handle, ab(labels), G);
+	}
+
 	async scoreResident(query: ApoResidentQuery): Promise<ApoScoreBlocks> {
 		return wrapBlocks(await (await this._need()).scoreResident(this._handle, query));
 	}
 
 	// ---- one-shot path ------------------------------------------------------------------------
 	async score(dims: VSBuffer, C: number, T: number, corpus: VSBuffer | undefined, K: number, candidates?: boolean,
-		candidateExtremes?: boolean): Promise<ApoScoreBlocks> {
+		candidateExtremes?: boolean, candidateGroups?: number): Promise<ApoScoreBlocks> {
 		return wrapBlocks(await (await this._need()).score(this._handle, ab(dims), C, T, corpus ? ab(corpus) : null, K, !!candidates,
-			!!candidateExtremes));
+			!!candidateExtremes, candidateGroups ?? 0));
 	}
 
 	/** fp32 evaluations -> Form T (3 bytes per evaluation + the dictionary of distinct evaluations); undefined when the tensor is not
@@ -194,15 +200,15 @@ export class ApoScoringMainService implements IApoScoringService {
 
 	/** Same result as score() on the tensor the tuples were encoded from; 12x fewer bytes over IPC and PCIe. */
 	async scoreTuples(t: ApoTupleBuffers, C: number, T: number, corpus: VSBuffer | undefined, K: number, candidates?: boolean,
-		candidateExtremes?: boolean): Promise<ApoScoreBlocks> {
+		candidateExtremes?: boolean, candidateGroups?: number): Promise<ApoScoreBlocks> {
 		const raw: ApoTuples = { tl: ab(t.tl), th: ab(t.th), tbookPc: ab(t.tbookPc), tbookPd: ab(t.tbookPd), codebook: ab(t.codebook), d2book: ab(t.d2book), nTuples: t.nTuples };
 		return wrapBlocks(await (await this._need()).scoreHostTuples(this._handle, raw, C, T, corpus ? ab(corpus) : null, K, !!candidates,
-			!!candidateExtremes));
+			!!candidateExtremes, candidateGroups ?? 0));
 	}
 
 	async scoreHostRecords(records: VSBuffer, rowBytes: 32 | 16, C: number, T: number, corpus: VSBuffer | undefined, K: number,
-		candidates?: boolean, candidateCorpus?: boolean, candidateExtremes?: boolean): Promise<ApoScoreBlocks> {
+		candidates?: boolean, candidateCorpus?: boolean, candidateExtremes?: boolean, candidateGroups?: number): Promise<ApoScoreBlocks> {
 		return wrapBlocks(await (await this._need()).scoreHostRecords(this._handle, ab(records), rowBytes, C, T, corpus ? ab(corpus) : null, K, !!candidates,
-			!!candidateCorpus, !!candidateExtremes));
+			!!candidateCorpus, !!candidateExtremes, candidateGroups ?? 0));
 	}
 }

@@ -16,8 +16,11 @@
  *  32 lowest- and 32 highest-reward rollouts of each candidate with their finalRewards — the sample runs the critique prompt
  *  is built from (APO:918-962, 1003-1007).
  *
- *  The byte offsets below are pinned to the C structs by tests/test_napi_candidates.py, tests/test_candidate_corpus_cpu.py and
- *  tests/test_napi_candidate_extremes.py.
+ *  And the decoder of the per-candidate group scores (ApoScoreBlocks.candidateGroups): apo_group_score[C][G], each candidate's
+ *  tallies and exact mean reward on the rollouts of every record group (a chat mode, a task category, a held-out split).
+ *
+ *  The byte offsets below are pinned to the C structs by tests/test_napi_candidates.py, tests/test_candidate_corpus_cpu.py,
+ *  tests/test_napi_candidate_extremes.py and tests/test_candidate_groups_cpu.py.
  *--------------------------------------------------------------------------------------------*/
 import { VSBuffer } from '../../../../base/common/buffer.js';
 import { CorpusReportNumbers, DIM_NAMES, decodeCorpusReport } from './traceRecordCodec.js';
@@ -128,4 +131,38 @@ export function decodeCandidateExtremes(buf: VSBuffer, c: number): CandidateExtr
 		index: Number(v.getBigInt64(offIdx + 8 * i, true)), finalReward: v.getFloat64(offRew + 8 * i, true),
 	}));
 	return { candidate: c, lowestRollouts: list(OFF_LOWEST, OFF_LOWEST_REWARD), highestRollouts: list(OFF_HIGHEST, OFF_HIGHEST_REWARD) };
+}
+
+const GROUP_SCORE_BYTES = 56;            // sizeof(apo_group_score)
+const OFF_GRP_TOTAL = 0;
+const OFF_GRP_GOOD = 8;
+const OFF_GRP_BAD = 16;
+const OFF_GRP_GOOD_RATE = 24;
+const OFF_GRP_WITH_REWARD = 32;
+const OFF_GRP_REWARD_SUM = 40;
+const OFF_GRP_AVG_REWARD = 48;
+
+export interface GroupScore {
+	totalRollouts: number;
+	goodFeedbackCount: number;
+	badFeedbackCount: number;
+	goodRate: number;
+	withReward: number;
+	rewardSum: number;
+	avgReward: number | null;   // null when none of the group's rollouts has a reward
+}
+
+/** The group scores of a candidateGroups block (ApoScoreBlocks.candidateGroups) of C candidates and G groups: [C][G]. */
+export function decodeCandidateGroups(buf: VSBuffer, C: number, G: number): GroupScore[][] {
+	if (C < 0 || G < 1 || C * G * GROUP_SCORE_BYTES > buf.byteLength) { throw new RangeError(`${C} x ${G} group scores do not fit the block`); }
+	const v = new DataView(buf.buffer.buffer, buf.buffer.byteOffset, C * G * GROUP_SCORE_BYTES);
+	return Array.from({ length: C }, (_, c) => Array.from({ length: G }, (_, g) => {
+		const o = (c * G + g) * GROUP_SCORE_BYTES;
+		const withReward = u64(v, o + OFF_GRP_WITH_REWARD);
+		return {
+			totalRollouts: u64(v, o + OFF_GRP_TOTAL), goodFeedbackCount: u64(v, o + OFF_GRP_GOOD), badFeedbackCount: u64(v, o + OFF_GRP_BAD),
+			goodRate: v.getFloat64(o + OFF_GRP_GOOD_RATE, true), withReward, rewardSum: v.getFloat64(o + OFF_GRP_REWARD_SUM, true),
+			avgReward: withReward === 0 ? null : v.getFloat64(o + OFF_GRP_AVG_REWARD, true),
+		};
+	}));
 }
