@@ -5,8 +5,10 @@ record axis, against the CPU oracle's generator path (integers, first-three exam
 
 The rollout legs (R16, and R = the same rollouts as 32-byte records) also time the step with the per-candidate corpus
 reports (APO_SCORE_CANDIDATE_CORPUS), alternating plain / candidates / candidate_corpus, and add a second parity block: the
-corpus report of the same 8 candidates against the CPU oracle's report of their generated rows (integers, flags, examples
-and severities exactly; binary64 sums to 1e-12, the oracle merging per-thread slices).
+corpus report of the same 8 candidates against the exact report of their generated rows (tests/exact_report.py: every
+field bit for bit, each sum rounded once from its exact fixed-point integer).  Beside it, parity_corpus_seq keeps the older
+comparison with oracle.report (binary64 sums to 1e-12, the oracle summing per-thread slices in sequential binary64) and lists
+the fields that fail it.
 
 Every leg also times the step with the per-candidate extremes (APO_SCORE_CANDIDATE_EXTREMES) in the same alternation.  On the
 fp32 legs its parity block is the lists of two of the 8 candidates against the model of tests/extremes_fixtures.py over the
@@ -165,25 +167,42 @@ def leg(eng, C, K, steps, score_kw, ref, picks, ref_ext=None, sets=None, ref_grp
     return out
 
 
-def same_corpus(r, ref):
-    """apo_corpus_report against oracle.report (the comparison of tests/test_gpu_parity.py check_report)"""
+def seq_corpus_diff(r, ref):
+    """apo_corpus_report against oracle.report, the comparison of tests/test_gpu_parity.py check_report: integers, flags,
+    examples and severities exactly, binary64 sums and averages to 1e-12 (the oracle sums in sequential binary64, merging
+    per-thread slices).  Returns the fields that fail it, with both values."""
     close = lambda a, b: abs(a - b) <= 1e-12 * max(1.0, abs(b))
-    if (r.total, r.good, r.bad, r.none, r.withReward) != (ref.total, ref.good, ref.bad, ref.none, ref.withReward):
-        return False
-    if r.goodRate != ref.goodRate or any(list(r.byMode[m]) != list(ref.byMode[m]) or r.byModeGoodRate[m] != ref.byModeGoodRate[m]
-                                         for m in range(5)):
-        return False
-    if ref.withReward and not close(r.avgReward, ref.avgReward):
-        return False
+    out = []
+
+    def need(ok, name, a, b):
+        if not ok:
+            out.append([name, a, b] + ([abs(a - b)] if isinstance(a, float) else []))
+
+    for f in ("total", "good", "bad", "none", "withReward", "goodRate", "toolCalls", "toolSucc", "toolFail"):
+        need(getattr(r, f) == getattr(ref, f), f, getattr(r, f), getattr(ref, f))
+    for m in range(5):
+        need(list(r.byMode[m]) == list(ref.byMode[m]), f"byMode[{m}]", list(r.byMode[m]), list(ref.byMode[m]))
+        need(r.byModeGoodRate[m] == ref.byModeGoodRate[m], f"byModeGoodRate[{m}]", r.byModeGoodRate[m], ref.byModeGoodRate[m])
+    if ref.withReward:
+        need(close(r.avgReward, ref.avgReward), "avgReward", r.avgReward, ref.avgReward)
     for i in range(9):
         a, b = r.dim[i], ref.dim[i]
-        if a.count != b.count or not close(a.sum, b.sum) or not close(a.avg, b.avg) or (a.low_flag, a.sugg_flag) != (b.low_flag, b.sugg_flag):
-            return False
+        need(a.count == b.count, f"dim[{i}].count", a.count, b.count)
+        need(close(a.sum, b.sum), f"dim[{i}].sum", a.sum, b.sum)
+        need(close(a.avg, b.avg), f"dim[{i}].avg", a.avg, b.avg)
+        for f in ("low_flag", "sugg_flag"):
+            need(getattr(a, f) == getattr(b, f), f"dim[{i}].{f}", getattr(a, f), getattr(b, f))
     for p in range(6):
         a, b = r.pat[p], ref.pat[p]
-        if (a.count, a.flag, list(a.examples)) != (b.count, b.flag, list(b.examples)) or (b.flag and a.severity != b.severity):
-            return False
-    return (r.toolCalls, r.toolSucc, r.toolFail) == (ref.toolCalls, ref.toolSucc, ref.toolFail)
+        need((a.count, a.flag, list(a.examples)) == (b.count, b.flag, list(b.examples)), f"pat[{p}]",
+             [a.count, a.flag, list(a.examples)], [b.count, b.flag, list(b.examples)])
+        need(not b.flag or a.severity == b.severity, f"pat[{p}].severity", a.severity, b.severity)
+    return out
+
+
+def parity_block(picks, diffs):
+    return {"candidates": picks, "equal": not any(diffs), "per_candidate": [not d for d in diffs],
+            "differing": {str(c): d for c, d in zip(picks, diffs) if d}}
 
 
 def corpus_leg(eng, C, K, steps, score_kw, ref, picks, ref_corpus, sets):
@@ -192,8 +211,10 @@ def corpus_leg(eng, C, K, steps, score_kw, ref, picks, ref_corpus, sets):
     kinds.update({k: {"groups": True} for k in sets})
     last, times, med = timed(eng, C, K, steps, score_kw, kinds, sets)
     ok = [same(last["candidates"].candidates[c], d) for c, d in zip(picks, ref)]
-    ok_c = [same_corpus(last["candidate_corpus"].candidate_corpus[c], d) for c, d in zip(picks, ref_corpus)]
+    import exact_report as xr
     cc = last["candidate_corpus"].candidate_corpus
+    exact = [[list(x) for x in xr.diff_exact(cc[c], d)] for c, d in zip(picks, ref_corpus["exact"])]
+    seq = [seq_corpus_diff(cc[c], d) for c, d in zip(picks, ref_corpus["seq"])]
     return {**groups_block(last, med, sets, None), "groups_bytes": b"".join(bytes(last[k].groups) for k in sets),
             "plain_ms_median": round(med["plain"], 3), "candidates_ms_median": round(med["candidates"], 3),
             "candidate_corpus_ms_median": round(med["candidate_corpus"], 3),
@@ -203,8 +224,9 @@ def corpus_leg(eng, C, K, steps, score_kw, ref, picks, ref_corpus, sets):
             "parity_extremes": extremes_parity(last["extremes"], None), "extremes_bytes": bytes(last["extremes"].extremes),
             "min_ms": {k: round(min(v) * 1e3, 3) for k, v in times.items()},
             "parity": {"candidates": picks, "equal": all(ok), "per_candidate": ok},
-            "parity_corpus": {"candidates": picks, "equal": all(ok_c), "per_candidate": ok_c,
-                              "pattern_counts": [[int(cc[c].pat[p].count) for p in range(6)] for c in picks]}}
+            "parity_corpus": {**parity_block(picks, exact), "check": "exact report, every field bit for bit",
+                              "pattern_counts": [[int(cc[c].pat[p].count) for p in range(6)] for c in picks]},
+            "parity_corpus_seq": {**parity_block(picks, seq), "check": "oracle.report, binary64 sums to 1e-12"}}
 
 
 def main():
@@ -217,6 +239,7 @@ def main():
     pkg = importlib.import_module("senweaver-ide_b200")
     import oracle
     from oracle import candidates as oc
+    import exact_report as xr
     import extremes_fixtures as xf
     import group_fixtures as gf
     legs = args.legs.split(",")
@@ -261,7 +284,9 @@ def main():
             Cr = 128
             picks_r = [int(x) for x in np.linspace(0, Cr - 1, 8).round()]
             ref_r = oc.cand_generated(seed, picks_r, 0, T, 300, nthreads=nth, records=True)
-            ref_rc = [oracle.report(oracle.gen_records(seed, oracle.STREAM_ROLLOUT, c, 1, 0, T, 300, nth), nthreads=nth) for c in picks_r]
+            ref_rc = {"seq": [oracle.report(oracle.gen_records(seed, oracle.STREAM_ROLLOUT, c, 1, 0, T, 300, nth), nthreads=nth)
+                              for c in picks_r]}
+            ref_rc["exact"] = [xr.combine(q, d) for q, d in zip(ref_rc["seq"], ref_r)]
             if "R16" in legs:
                 eng.rollouts16_generate(seed, 0, Cr, 0, T, 300)
                 out["form_r16_128x5M"] = corpus_leg(eng, Cr, K, args.steps, {"source": pkg.SRC_ROLLOUTS}, ref_r, picks_r, ref_rc, label_sets(T))

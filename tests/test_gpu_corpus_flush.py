@@ -102,6 +102,15 @@ def check_oracle_ints(rep, ref):
 def test_36M_corpus_through_every_scan_host(engine, orc, apo, sm_count, kind, idx_base):
     recs, want = big_corpus(kind, sm_count, idx_base)
     ref = orc.report(recs, idx_base=idx_base, nthreads=16)
+    reps = every_scan_host(engine, orc, apo, recs, idx_base)
+    first = reps["K1"]
+    check_corpus(apo, orc, apo.engine.CorpusReport.from_buffer_copy(first), recs, kind, idx_base, want, ref)
+    assert all(v == first for v in reps.values()), [k for k, v in reps.items() if v != first]
+
+
+def every_scan_host(engine, orc, apo, recs, idx_base):
+    """{host: report bytes} of the corpus `recs`: the corpus warp of K1 / K1q / K1r / K1r16 in the scoring launch,
+    k_detect6_tiles, and a session"""
     engine.corpus_upload(recs, idx_base)
     dims, roll, roll16 = small_evals(orc, apo)
     reps = {}
@@ -125,9 +134,7 @@ def test_36M_corpus_through_every_scan_host(engine, orc, apo, sm_count, kind, id
     engine.score_begin(2)
     engine.score_accumulate(0)
     reps["session"] = bytes(engine.score_finish(2, 1, corpus=True).report)
-    first = reps["K1"]
-    check_corpus(apo, orc, apo.engine.CorpusReport.from_buffer_copy(first), recs, kind, idx_base, want, ref)
-    assert all(v == first for v in reps.values()), [k for k, v in reps.items() if v != first]
+    return reps
 
 
 GRIDSTRIDE_SCRIPT = r"""

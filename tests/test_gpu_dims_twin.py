@@ -7,15 +7,21 @@ import pytest
 
 pytestmark = pytest.mark.gpu
 
-def kernels(fn):
-    """the names of the CUDA kernels fn launched, from a torch.profiler record"""
+def kernels(fn, tries=3):
+    """the names of the CUDA kernels fn launched, from a torch.profiler record.  fn is a scoring call, so it launches a
+    k_reward9* kernel; now and then a record holds the call's cudaLaunchKernel and no kernel at all (see
+    test_gpu_dims_tuple_copy.kernels).  Such a record says nothing about the route, so fn() is profiled again."""
     import torch
     from torch.profiler import ProfilerActivity, profile
-    torch.cuda.synchronize()
-    with profile(activities=[ProfilerActivity.CUDA]) as prof:
-        fn()
+    for _ in range(tries):
         torch.cuda.synchronize()
-    return " ".join(ev.name for ev in prof.events())
+        with profile(activities=[ProfilerActivity.CUDA]) as prof:
+            fn()
+            torch.cuda.synchronize()
+        names = " ".join(ev.name for ev in prof.events())
+        if "k_reward9" in names:
+            break
+    return names
 
 
 def reads(engine, fn):
