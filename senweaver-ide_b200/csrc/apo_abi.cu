@@ -157,6 +157,23 @@ const struct { const char *env; uint32_t bit; } kTuning[] = {
 	{"APO_TWIN_T", APO_TUNE_TWIN_T}, {"APO_NO_TWIN_T2", APO_TUNE_NO_TWIN_T2}, {"APO_NO_TWIN_H", APO_TUNE_NO_TWIN_H},
 	{"APO_NO_CORPUS_DIGEST", APO_TUNE_NO_CORPUS_DIGEST}};
 
+// The per-candidate passes a scoring call can flag (csrc/apo_cand.cu), with the words of their messages.  tbook: the pass
+// reads every source, Form T through the 4-bit table (apo_engine::tbook).
+enum Pass { PASS_CAND, PASS_CCORP, PASS_EXT, PASS_GRP, NPASS };
+const struct { uint32_t flag; const char *name, *joined, *every; bool tbook; } kPass[NPASS] = {
+	{APO_SCORE_CANDIDATES, "APO_SCORE_CANDIDATES", "the per-candidate breakdown is", "a breakdown", true},
+	{APO_SCORE_CANDIDATE_CORPUS, "APO_SCORE_CANDIDATE_CORPUS", "the per-candidate corpus reports are", "the reports", false},
+	{APO_SCORE_CANDIDATE_EXTREMES, "APO_SCORE_CANDIDATE_EXTREMES", "the per-candidate lists are", "the lists", true},
+	{APO_SCORE_CANDIDATE_GROUPS, "APO_SCORE_CANDIDATE_GROUPS", "the per-candidate group scores are", "the group scores", true}};
+
+// one pass's state through a call or session
+struct PassState {
+	bool armed = false;                  // its words zeroed for this call / session
+	bool every = true;                   // every accumulate of the session so far set the flag
+	bool ready = false;                  // its reports are those of the last scoring call
+	uint32_t C = 0;                      // candidates of those reports
+};
+
 }  // namespace
 
 struct apo_engine {
@@ -219,30 +236,20 @@ struct apo_engine {
 	size_t k1_used = 0;
 	uint32_t score_C = 0; bool scoring = false;
 	apo_timing timing{};
-	// per-candidate breakdown (APO_SCORE_CANDIDATES, csrc/apo_cand.cu): its own integers, never part of the accumulator vector
-	DevBuf<long long> cand_acc;              // [C][CB_INT] integers | [C][3] first-three 'bad' slots | domain word
+	// the per-candidate passes (csrc/apo_cand.cu): their own words, never part of the accumulator vector
+	PassState pass[NPASS];
+	DevBuf<float> tbook;                     // Form T: [8][16] 4-bit code -> fp32 value of the dictionary's codebook
+	DevBuf<long long> cand_acc;              // breakdown: [C][CB_INT] integers | [C][3] first-three 'bad' slots | domain word
 	DevBuf<apo_candidate_report> cand_rep;   // reports of the last flagged call
-	DevBuf<float> cand_book;                 // Form T: [8][16] code -> fp32 value of the dictionary's codebook
-	uint32_t cand_C = 0;
-	bool cand_armed = false;                 // cand_acc zeroed for this call / session
-	bool cand_every = true;                  // every accumulate of the session so far set the flag
-	bool cand_ready = false;                 // cand_rep holds the breakdown of the last scoring call
-	// per-candidate corpus report (APO_SCORE_CANDIDATE_CORPUS, csrc/apo_cand.cu k_cand_corpus): its own blocks, as cand_acc
-	DevBuf<long long> ccorp_acc;             // [C][CC_WORDS] corpus blocks | [C][CC_WORDS] scratch of the report kernel
+	DevBuf<long long> ccorp_acc;             // corpus reports: [C][CC_WORDS] corpus blocks | [C][CC_WORDS] scratch of the report kernel
 	DevBuf<apo_corpus_report> ccorp_rep;     // reports of the last flagged call
-	uint32_t ccorp_C = 0;
-	bool ccorp_armed = false, ccorp_every = true, ccorp_ready = false;   // as cand_armed / cand_every / cand_ready
-	// per-candidate extremes (APO_SCORE_CANDIDATE_EXTREMES, csrc/apo_cand.cu k_cand_extremes): keys, converted by the getter
-	DevBuf<unsigned long long> ext_acc;      // [C][CX_WORDS] lists | [cand_ext_slots][CX_WORDS] segments of one launch
-	uint32_t ext_C = 0;
-	bool ext_armed = false, ext_every = true, ext_ready = false;         // as cand_armed / cand_every / cand_ready
-	// record groups (apo_record_groups_upload) and the per-candidate group scores (APO_SCORE_CANDIDATE_GROUPS, k_cand_groups)
+	DevBuf<unsigned long long> ext_acc;      // extremes: [C][CX_WORDS] lists | [cand_ext_slots][CX_WORDS] segments of one launch (keys, converted by the getter)
+	// record groups (apo_record_groups_upload) and the group scores
 	DevBuf<uint8_t> grp_labels; uint64_t grp_T = 0; uint32_t grp_G = 0;
 	uint64_t grp_gen = 0;                    // counts uploads: a session's groups belong to the labels it armed with
 	DevBuf<long long> grp_acc;               // [C][G][GR_WORDS] words of the call or session
 	DevBuf<apo_group_score> grp_rep;         // [C][G] scores of the last flagged call
-	uint32_t grp_C = 0, grp_rep_G = 0, grp_arm_G = 0; uint64_t grp_arm_gen = 0;
-	bool grp_armed = false, grp_every = true, grp_ready = false;         // as cand_armed / cand_every / cand_ready
+	uint32_t grp_rep_G = 0, grp_arm_G = 0; uint64_t grp_arm_gen = 0;
 };
 
 namespace {
@@ -610,10 +617,7 @@ int begin_score(apo_engine *e, uint32_t C, bool whole = false) {
 	*e->h_domain = 0u;                              // the previous call has been synchronised: no kernel writes it now
 	e->partials_src = e->nranks > 1 ? e->acc_joined.p : e->acc.p;
 	e->last_C = C; e->score_C = C; e->scoring = true; e->k1_used = 0;
-	e->cand_armed = false; e->cand_every = true; e->cand_ready = false;
-	e->ccorp_armed = false; e->ccorp_every = true; e->ccorp_ready = false;
-	e->ext_armed = false; e->ext_every = true; e->ext_ready = false;
-	e->grp_armed = false; e->grp_every = true; e->grp_ready = false;
+	for (PassState &s : e->pass) s = PassState{};
 	e->timing = apo_timing{};
 	if (e->timing_on) CK(cudaEventRecord(e->ev[0], e->stream));
 	return APO_OK;
@@ -785,181 +789,20 @@ int launch_score(apo_engine *e, const apo_score_opts *o, const Evals &ev, uint32
 	return APO_OK;
 }
 
-// ---- per-candidate breakdown (APO_SCORE_CANDIDATES)
-bool wants_cand(const apo_score_opts *o) { return (o->flags & APO_SCORE_CANDIDATES) != 0; }
+// ---- the per-candidate passes (APO_SCORE_CANDIDATES, _CANDIDATE_CORPUS, _CANDIDATE_EXTREMES, _CANDIDATE_GROUPS)
+bool wants(const apo_score_opts *o, int p) { return (o->flags & kPass[p].flag) != 0; }
 
-int cand_check(apo_engine *e) {
-	if (e->nranks > 1)
-		return fail(e, APO_E_STATE, "APO_SCORE_CANDIDATES is single-rank only: the per-candidate breakdown is not joined across the %d ranks of this handle", e->nranks);
-	return APO_OK;
-}
-
-// the breakdown's buffers (cand_arm's, and cand_upload_tbook's for Form T), allocated before route_copy
-uint64_t cand_words(uint32_t C) { return (uint64_t)C * (apo::CB_INT + 3) + 1; }
-
-int cand_reserve(apo_engine *e, uint32_t C) {
-	CK(reserve(e, e->cand_acc, cand_words(C)));
-	CK(reserve(e, e->cand_book, 8 * 16));
-	return APO_OK;
-}
-
-// zero the breakdown of C candidates (first flagged launch of a call or session)
-int cand_arm(apo_engine *e, uint32_t C) {
-	const uint64_t words = cand_words(C);
-	CK(reserve(e, e->cand_acc, words));
-	CK(cudaMemsetAsync(e->cand_acc.p, 0, words * 8, e->stream));
-	e->cand_armed = true;
-	return APO_OK;
-}
-
-// Form T dictionary codebook -> [8][16] fp32 values (4-bit codes, csrc/apo_tuple.cu)
-int cand_upload_tbook(apo_engine *e, const uint32_t *codebook) {
-	uint32_t tab[8 * 16];
-	for (int j = 0; j < 8; j++) for (int k = 0; k < 16; k++) tab[16 * j + k] = codebook[256 * j + k];
-	CK(reserve(e, e->cand_book, 8 * 16));
-	CK(cudaMemcpyAsync(e->cand_book.p, tab, sizeof tab, cudaMemcpyHostToDevice, e->stream));   // pageable source: consumed when this returns
-	return APO_OK;
-}
-
-// the breakdown pass over ev into candidates [cand_offset, ...)
-int launch_cand(apo_engine *e, const Evals &ev, uint32_t cand_offset) {
-	if (!ev.count) return APO_OK;
-	if (ev.form == apo::CAND_T && !ev.t_once) { const int rc = cand_upload_tbook(e, ev.dict->book); if (rc) return rc; }
-	apo::CandParams P{};
-	P.C = ev.C; P.T = ev.count; P.idx_base = ev.idx_base; P.pitch_evals = ev.pitch_evals; P.lut = e->d_lut.p;
-	P.ints = e->cand_acc.p + (uint64_t)apo::CB_INT * cand_offset;
-	P.ex = (unsigned long long *)(e->cand_acc.p + (uint64_t)apo::CB_INT * e->score_C) + 3ull * cand_offset;
-	P.dom = (unsigned int *)(e->cand_acc.p + cand_words(e->score_C) - 1);
-	P.rows = ev.rows; P.q8 = ev.q8; P.d2 = ev.d2; P.li = ev.li; P.qw = ev.qw;
-	P.tl = ev.tl; P.th = ev.th;
-	if (ev.qt) P.cbf = ev.qt->cbf.p;
-	if (ev.form == apo::CAND_T) {
-		P.tb_pc = ev.dict->pc.p; P.tb_pd = ev.dict->pd.p; P.n_tuples = ev.dict->n; P.d2book = ev.dict->d2.p; P.tbook = e->cand_book.p;
-	}
-	CK(apo::run_cand_breakdown(P, ev.form, e->sm_count, e->stream));
-	e->timing.launches++;
-	return APO_OK;
-}
-
-// integers -> apo_candidate_report[C]; after the scoring call has completed (its partials are final)
-int cand_finish(apo_engine *e, uint32_t C) {
-	CK(reserve(e, e->cand_rep, C ? C : 1));
-	const long long *partials = e->partials_src ? e->partials_src : e->acc.p;
-	CK(apo::run_cand_report(e->cand_acc.p, (const unsigned long long *)(e->cand_acc.p + (uint64_t)apo::CB_INT * C), partials, C, e->cand_rep.p, e->stream));
-	e->timing.launches++;
-	uint32_t dom = 0;                                              // k_cand_breakdown's domain word (pageable: the copy waits for the stream)
-	CK(cudaMemcpyAsync(&dom, e->cand_acc.p + cand_words(C) - 1, 4, cudaMemcpyDeviceToHost, e->stream));
-	CK(cudaStreamSynchronize(e->stream));
-	if (dom)
-		return fail(e, APO_E_ARG, "APO_SCORE_CANDIDATES: an evaluation with a finalReward has a dimension with |v| >= 2048 (or NaN), "
-		                          "whose rint(v * 2^52) has no exact fixed-point sum");
-	e->cand_C = C; e->cand_ready = true;
-	return APO_OK;
-}
-
-// ---- per-candidate corpus report (APO_SCORE_CANDIDATE_CORPUS)
-bool wants_ccorp(const apo_score_opts *o) { return (o->flags & APO_SCORE_CANDIDATE_CORPUS) != 0; }
+// a failed call or finish leaves no reports behind
+void unready_passes(apo_engine *e) { for (PassState &s : e->pass) s.ready = false; }
 
 // records: the call reads trace records (Form R / R16); the other forms carry only the nine reward values
-int ccorp_check(apo_engine *e, bool records) {
-	if (!records)
-		return fail(e, APO_E_ARG, "APO_SCORE_CANDIDATE_CORPUS needs rollout records (Form R / R16): this source holds reward values only, "
-		                          "without the fields the patterns, modes and tool totals read");
-	if (e->nranks > 1)
-		return fail(e, APO_E_STATE, "APO_SCORE_CANDIDATE_CORPUS is single-rank only: the per-candidate corpus reports are not joined across the %d ranks of this handle", e->nranks);
-	return APO_OK;
+int refuse_no_records(apo_engine *e) {
+	return fail(e, APO_E_ARG, "APO_SCORE_CANDIDATE_CORPUS needs rollout records (Form R / R16): this source holds reward values only, "
+	                          "without the fields the patterns, modes and tool totals read");
 }
 
-// zero the corpus blocks of C candidates (first flagged launch of a call or session)
-int ccorp_arm(apo_engine *e, uint32_t C) {
-	const uint64_t words = (uint64_t)C * apo::CC_WORDS;
-	CK(reserve(e, e->ccorp_acc, 2 * words));                 // blocks | report scratch
-	CK(cudaMemsetAsync(e->ccorp_acc.p, 0, words * 8, e->stream));
-	e->ccorp_armed = true;
-	return APO_OK;
-}
-
-// corpus scan of ev's trace records (Form R / R16) into candidates [cand_offset, ...)
-int launch_ccorp(apo_engine *e, const Evals &ev, uint32_t cand_offset) {
-	if (!ev.count) return APO_OK;
-	apo::CandCorpusParams P{};
-	P.C = ev.C; P.T = ev.count; P.idx_base = ev.idx_base; P.pitch_evals = ev.pitch_evals; P.rows = ev.rows;
-	P.lut = e->d_lut.p; P.w2 = e->W.w[2];
-	P.blk = e->ccorp_acc.p + (uint64_t)apo::CC_WORDS * cand_offset;
-	CK(apo::run_cand_corpus(P, (int)ev.row(), e->sm_count, e->stream));
-	e->timing.launches++;
-	return APO_OK;
-}
-
-// blocks -> apo_corpus_report[C]
-int ccorp_finish(apo_engine *e, uint32_t C) {
-	CK(reserve(e, e->ccorp_rep, C ? C : 1));
-	CK(apo::run_cand_corpus_report(e->ccorp_acc.p, C, e->ccorp_rep.p, e->stream));
-	e->timing.launches++;
-	CK(cudaStreamSynchronize(e->stream));
-	e->ccorp_C = C; e->ccorp_ready = true;
-	return APO_OK;
-}
-
-// ---- per-candidate extremes (APO_SCORE_CANDIDATE_EXTREMES)
-bool wants_ext(const apo_score_opts *o) { return (o->flags & APO_SCORE_CANDIDATE_EXTREMES) != 0; }
-
-int ext_check(apo_engine *e) {
-	if (e->nranks > 1)
-		return fail(e, APO_E_STATE, "APO_SCORE_CANDIDATE_EXTREMES is single-rank only: the per-candidate lists are not joined across the %d ranks of this handle", e->nranks);
-	return APO_OK;
-}
-
-// the lists of C candidates and the segment slots of one launch (and cand_upload_tbook's table for Form T), before route_copy
-int ext_reserve(apo_engine *e, uint32_t C) {
-	CK(reserve(e, e->ext_acc, ((uint64_t)C + apo::cand_ext_slots(e->sm_count, C)) * apo::CX_WORDS));
-	CK(reserve(e, e->cand_book, 8 * 16));
-	return APO_OK;
-}
-
-// empty lists (all-ones keys) for C candidates (first flagged launch of a call or session)
-int ext_arm(apo_engine *e, uint32_t C) {
-	if (int rc = ext_reserve(e, C)) return rc;
-	CK(cudaMemsetAsync(e->ext_acc.p, 0xFF, (uint64_t)C * apo::CX_WORDS * 8, e->stream));
-	e->ext_armed = true;
-	return APO_OK;
-}
-
-// the extremes pass and its merge over ev into candidates [cand_offset, ...)
-int launch_ext(apo_engine *e, const apo_score_opts *o, const Evals &ev, uint32_t cand_offset) {
-	if (!ev.count) return APO_OK;
-	if (ev.form == apo::CAND_T && !ev.t_once) { const int rc = cand_upload_tbook(e, ev.dict->book); if (rc) return rc; }
-	apo::CandExtParams X{};
-	apo::CandParams &P = X.src;
-	P.C = ev.C; P.T = ev.count; P.idx_base = ev.idx_base; P.pitch_evals = ev.pitch_evals; P.lut = e->d_lut.p;
-	P.rows = ev.rows; P.q8 = ev.q8; P.d2 = ev.d2; P.li = ev.li; P.qw = ev.qw;
-	P.tl = ev.tl; P.th = ev.th;
-	if (ev.qt) P.cbf = ev.qt->cbf.p;
-	if (ev.form == apo::CAND_T) {
-		P.tb_pc = ev.dict->pc.p; P.tb_pd = ev.dict->pd.p; P.n_tuples = ev.dict->n; P.d2book = ev.dict->d2.p; P.tbook = e->cand_book.p;
-	}
-	X.W = e->W;
-	X.lists = e->ext_acc.p + (uint64_t)apo::CX_WORDS * cand_offset;
-	X.seg = e->ext_acc.p + (uint64_t)apo::CX_WORDS * e->score_C;
-	CK(apo::run_cand_extremes(X, ev.form, (o->flags & APO_SCORE_RECIP) != 0, e->sm_count, e->stream));
-	e->timing.launches += 2;
-	return APO_OK;
-}
-
-// the lists are final once the call's launches have run: the getter converts the keys it is asked for
-int ext_finish(apo_engine *e, uint32_t C) {
-	CK(cudaStreamSynchronize(e->stream));
-	e->ext_C = C; e->ext_ready = true;
-	return APO_OK;
-}
-
-// ---- per-candidate group scores (APO_SCORE_CANDIDATE_GROUPS)
-bool wants_grp(const apo_score_opts *o) { return (o->flags & APO_SCORE_CANDIDATE_GROUPS) != 0; }
-
-// end: one past the last record position the call scores (0: not known here, a session's finish)
-int grp_check(apo_engine *e, uint64_t end) {
-	if (e->nranks > 1)
-		return fail(e, APO_E_STATE, "APO_SCORE_CANDIDATE_GROUPS is single-rank only: the per-candidate group scores are not joined across the %d ranks of this handle", e->nranks);
+// the labels cover the record positions below end (0: not known here, a session's finish)
+int labels_check(apo_engine *e, uint64_t end) {
 	if (e->grp_T == 0) return fail(e, APO_E_STATE, "APO_SCORE_CANDIDATE_GROUPS: no record groups uploaded (apo_record_groups_upload)");
 	if (end > e->grp_T)
 		return fail(e, APO_E_ARG, "APO_SCORE_CANDIDATE_GROUPS: record position %llu is past the %llu labels uploaded", (unsigned long long)end - 1,
@@ -967,50 +810,151 @@ int grp_check(apo_engine *e, uint64_t end) {
 	return APO_OK;
 }
 
-// the words of C candidates under the labels' G (and cand_upload_tbook's table for Form T), before route_copy
-int grp_reserve(apo_engine *e, uint32_t C) {
-	CK(reserve(e, e->grp_acc, (uint64_t)(C ? C : 1) * e->grp_G * apo::GR_WORDS));
-	CK(reserve(e, e->cand_book, 8 * 16));
-	return APO_OK;
-}
+// score_check's T for the host-streaming calls (they take no window) and for apo_score_finish (each accumulate checked its own)
+constexpr uint64_t kStreamed = ~0ull, kSession = ~0ull - 1;
 
-// zero the words of C candidates (first flagged launch of a call or session), which then belong to the labels held now
-int grp_arm(apo_engine *e, uint32_t C) {
-	if (int rc = grp_reserve(e, C)) return rc;
-	CK(cudaMemsetAsync(e->grp_acc.p, 0, (uint64_t)C * e->grp_G * apo::GR_WORDS * 8, e->stream));
-	e->grp_armed = true; e->grp_arm_G = e->grp_G; e->grp_arm_gen = e->grp_gen;
-	return APO_OK;
-}
-
-// the group pass over ev into candidates [cand_offset, ...)
-int launch_grp(apo_engine *e, const apo_score_opts *o, const Evals &ev, uint32_t cand_offset) {
-	if (!ev.count) return APO_OK;
-	if (ev.form == apo::CAND_T && !ev.t_once) { const int rc = cand_upload_tbook(e, ev.dict->book); if (rc) return rc; }
-	apo::CandGroupParams X{};
-	apo::CandParams &P = X.src;
-	P.C = ev.C; P.T = ev.count; P.idx_base = ev.idx_base; P.pitch_evals = ev.pitch_evals; P.lut = e->d_lut.p;
-	P.rows = ev.rows; P.q8 = ev.q8; P.d2 = ev.d2; P.li = ev.li; P.qw = ev.qw;
-	P.tl = ev.tl; P.th = ev.th;
-	if (ev.qt) P.cbf = ev.qt->cbf.p;
-	if (ev.form == apo::CAND_T) {
-		P.tb_pc = ev.dict->pc.p; P.tb_pd = ev.dict->pd.p; P.n_tuples = ev.dict->n; P.d2book = ev.dict->d2.p; P.tbook = e->cand_book.p;
+// The refusals of the flagged passes, in pass order.  records: the call reads trace records; end: one past the last record
+// position it scores (0: a session's finish; kStreamed: not known yet, the host-streaming calls check the labels themselves).
+int passes_check(apo_engine *e, const apo_score_opts *o, bool records, uint64_t end) {
+	for (int p = 0; p < NPASS; p++) {
+		if (!wants(o, p)) continue;
+		if (p == PASS_CCORP && !records) return refuse_no_records(e);
+		if (e->nranks > 1)
+			return fail(e, APO_E_STATE, "%s is single-rank only: %s not joined across the %d ranks of this handle", kPass[p].name, kPass[p].joined, e->nranks);
+		if (p == PASS_GRP && end != kStreamed) { const int rc = labels_check(e, end); if (rc) return rc; }
 	}
-	X.W = e->W;
-	X.labels = e->grp_labels.p; X.G = e->grp_arm_G;
-	X.words = e->grp_acc.p + (uint64_t)cand_offset * X.G * apo::GR_WORDS;
-	CK(apo::run_cand_groups(X, ev.form, (o->flags & APO_SCORE_RECIP) != 0, e->sm_count, e->stream));
-	e->timing.launches++;
 	return APO_OK;
 }
 
-// words -> apo_group_score[C][G]
-int grp_finish(apo_engine *e, uint32_t C) {
-	const uint32_t G = e->grp_arm_G;
-	CK(reserve(e, e->grp_rep, (uint64_t)(C ? C : 1) * G));
-	CK(apo::run_cand_groups_report(e->grp_acc.p, C, G, e->grp_rep.p, e->stream));
-	e->timing.launches++;
+uint64_t cand_words(uint32_t C) { return (uint64_t)C * (apo::CB_INT + 3) + 1; }
+
+// a pass's words for C candidates (and the Form T table), allocated before route_copy
+int pass_reserve(apo_engine *e, int p, uint32_t C) {
+	switch (p) {
+	case PASS_CAND: CK(reserve(e, e->cand_acc, cand_words(C))); break;
+	case PASS_CCORP: CK(reserve(e, e->ccorp_acc, 2ull * C * apo::CC_WORDS)); break;   // blocks | report scratch
+	case PASS_EXT: CK(reserve(e, e->ext_acc, ((uint64_t)C + apo::cand_ext_slots(e->sm_count, C)) * apo::CX_WORDS)); break;
+	case PASS_GRP: CK(reserve(e, e->grp_acc, (uint64_t)(C ? C : 1) * e->grp_G * apo::GR_WORDS)); break;
+	}
+	if (kPass[p].tbook) CK(reserve(e, e->tbook, 8 * 16));
+	return APO_OK;
+}
+
+// zero a pass's words for C candidates (first flagged launch of a call or session); the extremes' empty lists are all-ones keys
+int pass_arm(apo_engine *e, int p, uint32_t C) {
+	if (int rc = pass_reserve(e, p, C)) return rc;
+	switch (p) {
+	case PASS_CAND: CK(cudaMemsetAsync(e->cand_acc.p, 0, cand_words(C) * 8, e->stream)); break;
+	case PASS_CCORP: CK(cudaMemsetAsync(e->ccorp_acc.p, 0, (uint64_t)C * apo::CC_WORDS * 8, e->stream)); break;
+	case PASS_EXT: CK(cudaMemsetAsync(e->ext_acc.p, 0xFF, (uint64_t)C * apo::CX_WORDS * 8, e->stream)); break;
+	case PASS_GRP:                                                  // the words then belong to the labels held now
+		CK(cudaMemsetAsync(e->grp_acc.p, 0, (uint64_t)C * e->grp_G * apo::GR_WORDS * 8, e->stream));
+		e->grp_arm_G = e->grp_G; e->grp_arm_gen = e->grp_gen;
+		break;
+	}
+	e->pass[p].armed = true;
+	return APO_OK;
+}
+
+// Form T dictionary codebook -> [8][16] fp32 values (4-bit codes, csrc/apo_tuple.cu)
+int upload_tbook(apo_engine *e, const uint32_t *codebook) {
+	uint32_t tab[8 * 16];
+	for (int j = 0; j < 8; j++) for (int k = 0; k < 16; k++) tab[16 * j + k] = codebook[256 * j + k];
+	CK(reserve(e, e->tbook, 8 * 16));
+	CK(cudaMemcpyAsync(e->tbook.p, tab, sizeof tab, cudaMemcpyHostToDevice, e->stream));   // pageable source: consumed when this returns
+	return APO_OK;
+}
+
+// The flagged passes over ev into candidates [cand_offset, ...), behind its scoring launch.  A pass that an accumulate of the
+// session did not flag, or whose group words belong to labels uploaded since, is left out: apo_score_finish refuses it.
+int launch_passes(apo_engine *e, const apo_score_opts *o, const Evals &ev, uint32_t cand_offset) {
+	bool run[NPASS], any = false;
+	for (int p = 0; p < NPASS; p++) {
+		run[p] = wants(o, p) && e->pass[p].every && (p != PASS_GRP || e->grp_arm_gen == e->grp_gen);
+		any |= run[p];
+	}
+	if (!any || !ev.count) return APO_OK;
+	if (ev.form == apo::CAND_T && !ev.t_once) { const int rc = upload_tbook(e, ev.dict->book); if (rc) return rc; }
+	apo::CandEvals S{};
+	S.C = ev.C; S.T = ev.count; S.idx_base = ev.idx_base; S.pitch_evals = ev.pitch_evals; S.lut = e->d_lut.p;
+	S.rows = ev.rows; S.q8 = ev.q8; S.d2 = ev.d2; S.li = ev.li; S.qw = ev.qw;
+	S.tl = ev.tl; S.th = ev.th;
+	if (ev.qt) S.cbf = ev.qt->cbf.p;
+	if (ev.form == apo::CAND_T) {
+		S.tb_pc = ev.dict->pc.p; S.tb_pd = ev.dict->pd.p; S.n_tuples = ev.dict->n; S.d2book = ev.dict->d2.p; S.tbook = e->tbook.p;
+	}
+	const bool recip = (o->flags & APO_SCORE_RECIP) != 0;
+	if (run[PASS_CAND]) {
+		const apo::CandParams P{S, e->cand_acc.p + (uint64_t)apo::CB_INT * cand_offset,
+		                        (unsigned long long *)(e->cand_acc.p + (uint64_t)apo::CB_INT * e->score_C) + 3ull * cand_offset,
+		                        (unsigned int *)(e->cand_acc.p + cand_words(e->score_C) - 1)};
+		CK(apo::run_cand_breakdown(P, ev.form, e->sm_count, e->stream));
+		e->timing.launches++;
+	}
+	if (run[PASS_CCORP]) {
+		const apo::CandCorpusParams P{S, e->W.w[2], e->ccorp_acc.p + (uint64_t)apo::CC_WORDS * cand_offset};
+		CK(apo::run_cand_corpus(P, (int)ev.row(), e->sm_count, e->stream));
+		e->timing.launches++;
+	}
+	if (run[PASS_EXT]) {                                            // the pass and its merge
+		const apo::CandExtParams X{S, e->W, e->ext_acc.p + (uint64_t)apo::CX_WORDS * cand_offset, e->ext_acc.p + (uint64_t)apo::CX_WORDS * e->score_C};
+		CK(apo::run_cand_extremes(X, ev.form, recip, e->sm_count, e->stream));
+		e->timing.launches += 2;
+	}
+	if (run[PASS_GRP]) {
+		const uint32_t G = e->grp_arm_G;
+		const apo::CandGroupParams X{S, e->W, e->grp_labels.p, G, e->grp_acc.p + (uint64_t)cand_offset * G * apo::GR_WORDS};
+		CK(apo::run_cand_groups(X, ev.form, recip, e->sm_count, e->stream));
+		e->timing.launches++;
+	}
+	return APO_OK;
+}
+
+// The reports of the flagged passes, after the scoring call has completed (its partials are final): every report kernel, one
+// synchronise, then the breakdown's domain word.  Only a call that passes its check has its reports ready.
+int finish_passes(apo_engine *e, const apo_score_opts *o, uint32_t C) {
+	bool any = false;
+	for (int p = 0; p < NPASS; p++) any |= wants(o, p);
+	if (!any) return APO_OK;
+	if (wants(o, PASS_CAND)) {                                      // integers -> apo_candidate_report[C]
+		CK(reserve(e, e->cand_rep, C ? C : 1));
+		const long long *partials = e->partials_src ? e->partials_src : e->acc.p;
+		CK(apo::run_cand_report(e->cand_acc.p, (const unsigned long long *)(e->cand_acc.p + (uint64_t)apo::CB_INT * C), partials, C, e->cand_rep.p, e->stream));
+		e->timing.launches++;
+	}
+	if (wants(o, PASS_CCORP)) {                                     // blocks -> apo_corpus_report[C]
+		CK(reserve(e, e->ccorp_rep, C ? C : 1));
+		CK(apo::run_cand_corpus_report(e->ccorp_acc.p, C, e->ccorp_rep.p, e->stream));
+		e->timing.launches++;
+	}
+	if (wants(o, PASS_GRP)) {                                       // words -> apo_group_score[C][G]; the extremes' lists are final as they are
+		CK(reserve(e, e->grp_rep, (uint64_t)(C ? C : 1) * e->grp_arm_G));
+		CK(apo::run_cand_groups_report(e->grp_acc.p, C, e->grp_arm_G, e->grp_rep.p, e->stream));
+		e->timing.launches++;
+	}
+	uint32_t dom = 0;                                               // k_cand_breakdown's domain word (pageable: the copy waits for the stream)
+	if (wants(o, PASS_CAND)) CK(cudaMemcpyAsync(&dom, e->cand_acc.p + cand_words(C) - 1, 4, cudaMemcpyDeviceToHost, e->stream));
 	CK(cudaStreamSynchronize(e->stream));
-	e->grp_C = C; e->grp_rep_G = G; e->grp_ready = true;
+	if (dom)
+		return fail(e, APO_E_ARG, "APO_SCORE_CANDIDATES: an evaluation with a finalReward has a dimension with |v| >= 2048 (or NaN), "
+		                          "whose rint(v * 2^52) has no exact fixed-point sum");
+	for (int p = 0; p < NPASS; p++)
+		if (wants(o, p)) { e->pass[p].C = C; e->pass[p].ready = true; }
+	if (wants(o, PASS_GRP)) e->grp_rep_G = e->grp_arm_G;
+	return APO_OK;
+}
+
+// The refusals every report getter makes, in order: the last scoring call set the pass's flag (the groups: and split by G),
+// [c0, c0 + n) lies inside its candidates, and a range that is not empty has an out; then the device is current.
+int report_check(apo_engine *e, int p, uint32_t c0, uint32_t n, const void *out, uint32_t G = 0) {
+	if (!e) return APO_E_ARG;
+	if (!e->pass[p].ready) return fail(e, APO_E_STATE, "the last scoring call did not set %s", kPass[p].name);
+	if (p == PASS_GRP && G != e->grp_rep_G) return fail(e, APO_E_ARG, "G=%u is not the G=%u the last scoring call split by", G, e->grp_rep_G);
+	const uint32_t C = e->pass[p].C;
+	if ((uint64_t)c0 + n > C) return fail(e, APO_E_ARG, "candidates [%u,%llu) exceed C=%u", c0, (unsigned long long)c0 + n, C);
+	if (n == 0) return APO_OK;
+	if (!out) return fail(e, APO_E_ARG, "out is NULL");
+	CK(cudaSetDevice(e->device));
 	return APO_OK;
 }
 
@@ -1124,10 +1068,7 @@ int finish_score(apo_engine *e, const apo_score_opts *o, uint32_t C, double *sco
 		CK(cudaStreamSynchronize(e->stream));
 		if (bad) return fail(e, APO_E_ARG, "an evaluation names an empty or NaN slot of the codebook or of d2book");
 	}
-	if (wants_cand(o) && (rc = cand_finish(e, C))) return rc;
-	if (wants_ccorp(o) && (rc = ccorp_finish(e, C))) return rc;
-	if (wants_ext(o) && (rc = ext_finish(e, C))) return rc;
-	return wants_grp(o) ? grp_finish(e, C) : APO_OK;
+	return finish_passes(e, o, C);
 }
 
 // o's window against the T evaluations loaded
@@ -1136,9 +1077,6 @@ int check_window(apo_engine *e, const apo_score_opts *o, uint64_t T) {
 	if (o->first > T || (o->count && o->first + o->count > T)) return fail(e, APO_E_ARG, "window outside [0,%llu)", (unsigned long long)T);
 	return APO_OK;
 }
-
-// score_check's T for the host-streaming calls (they take no window) and for apo_score_finish (each accumulate checked its own)
-constexpr uint64_t kStreamed = ~0ull, kSession = ~0ull - 1;
 
 // The refusals apo_score, apo_score_finish and the host-streaming calls share, once each has checked its source, in this
 // order: beam width, window (inside the T evaluations loaded), per-candidate passes (records: the source holds trace
@@ -1152,17 +1090,13 @@ int score_check(apo_engine *e, const apo_score_opts *o, uint32_t C, uint64_t T, 
 	} else if (T != kSession && (rc = check_window(e, o, T))) {
 		return rc;
 	}
-	if (wants_cand(o) && (rc = cand_check(e))) return rc;
-	if (wants_ccorp(o) && (rc = ccorp_check(e, records))) return rc;
-	if (wants_ext(o) && (rc = ext_check(e))) return rc;
-	// the host-streaming calls check their T themselves (stream_host)
-	if (wants_grp(o) && T != kStreamed && (rc = grp_check(e, T == kSession ? 0 : (o->count ? o->first + o->count : T)))) return rc;
+	const uint64_t end = T == kStreamed ? kStreamed : T == kSession ? 0 : o->count ? o->first + o->count : T;
+	if ((rc = passes_check(e, o, records, end))) return rc;
 	CK(cudaSetDevice(e->device));
 	if (T == kSession) return APO_OK;                               // a session's scratch was sized by apo_score_begin
 	if ((rc = ensure_scratch(e, C, o->K))) return rc;
-	if (wants_cand(o) && (rc = cand_reserve(e, C))) return rc;
-	if (wants_ext(o) && (rc = ext_reserve(e, C))) return rc;
-	if (wants_grp(o) && (rc = grp_reserve(e, C))) return rc;
+	for (int p = 0; p < NPASS; p++)
+		if (wants(o, p) && (rc = pass_reserve(e, p, C))) return rc;
 	return APO_OK;
 }
 
@@ -1175,10 +1109,9 @@ int score_arm(apo_engine *e, const apo_score_opts *o, uint32_t C, bool begin, ui
 	if (peer_join_active(e, C)) e->join_epoch++;          // counts joined calls only: consecutive joins alternate between the two export slots
 	int rc;
 	if (begin && (rc = begin_score(e, C, whole))) return rc;
-	if (wants_cand(o) && !e->cand_armed && (rc = cand_arm(e, C))) return rc;
-	if (wants_ext(o) && !e->ext_armed && (rc = ext_arm(e, C))) return rc;
-	if (wants_grp(o) && !e->grp_armed && (rc = grp_arm(e, C))) return rc;
-	return wants_ccorp(o) && !e->ccorp_armed ? ccorp_arm(e, C) : APO_OK;
+	for (int p = 0; p < NPASS; p++)
+		if (wants(o, p) && !e->pass[p].armed && (rc = pass_arm(e, p, C))) return rc;
+	return APO_OK;
 }
 
 // order of a d2book: by value, -0.0 (sign bit set) before +0.0
@@ -1748,7 +1681,7 @@ extern "C" void apo_destroy(apo_engine *e) {
 	e->qt.release(); e->qt_stream.release();
 	e->d_lut.release(); e->corpus.release(); e->digest.release(); e->dims.release(); e->roll.release(); e->acc.release(); e->acc_joined.release(); e->acc_snapshot.release(); e->misc.release();
 	e->result.release(); e->keys.release(); e->sel_key.release(); e->sel_idx.release();
-	e->cand_acc.release(); e->cand_rep.release(); e->cand_book.release(); e->ccorp_acc.release(); e->ccorp_rep.release(); e->ext_acc.release();
+	e->cand_acc.release(); e->cand_rep.release(); e->tbook.release(); e->ccorp_acc.release(); e->ccorp_rep.release(); e->ext_acc.release();
 	e->grp_labels.release(); e->grp_acc.release(); e->grp_rep.release();
 	e->tup.release(); e->tups.release(); e->tvals.release();
 	e->win[0].release(); e->win[1].release(); e->batch_in.release(); e->batch_out.release(); e->batch_mask.release();
@@ -2173,57 +2106,39 @@ extern "C" int apo_score_accumulate(apo_engine *e, const apo_score_opts *o, uint
 	if (rc) return rc;
 	if ((uint64_t)cand_offset + ev.C > e->score_C) return fail(e, APO_E_ARG, "candidates [%u,%u) exceed C_total=%u", cand_offset, cand_offset + ev.C, e->score_C);
 	if ((rc = check_window(e, o, ev.count))) return rc;
-	const bool cand = wants_cand(o), ccorp = wants_ccorp(o), ext = wants_ext(o), grp = wants_grp(o);
-	if (cand && (rc = cand_check(e))) return rc;
-	if (ccorp && (rc = ccorp_check(e, ev.records()))) return rc;
-	if (ext && (rc = ext_check(e))) return rc;
-	if (grp && (rc = grp_check(e, o->count ? o->first + o->count : ev.count))) return rc;
+	if ((rc = passes_check(e, o, ev.records(), o->count ? o->first + o->count : ev.count))) return rc;
 	CK(cudaSetDevice(e->device));
-	if (cand && (rc = cand_reserve(e, e->score_C))) return rc;                                  // allocates: before route_copy
-	if (cand && e->cand_every && !e->cand_armed && (rc = cand_arm(e, e->score_C))) return rc;
-	if (ext && e->ext_every && !e->ext_armed && (rc = ext_arm(e, e->score_C))) return rc;      // allocates too
-	if (grp && e->grp_every && !e->grp_armed && (rc = grp_arm(e, e->score_C))) return rc;      // and so does this
+	for (int p = 0; p < NPASS; p++)                     // allocates: before route_copy
+		if (wants(o, p) && e->pass[p].every && !e->pass[p].armed && (rc = pass_arm(e, p, e->score_C))) return rc;
 	if ((rc = route_copy(e, o, &ev))) return rc;
 	if ((rc = resident_window(e, o, &ev)) || (rc = launch_score(e, o, ev, cand_offset))) return rc;
-	if (!ext) e->ext_every = false;
-	else if (e->ext_every && (rc = launch_ext(e, o, ev, cand_offset))) return rc;   // else finish refuses
-	if (!grp) e->grp_every = false;
-	else if (e->grp_every && e->grp_arm_gen == e->grp_gen && (rc = launch_grp(e, o, ev, cand_offset))) return rc;   // else finish refuses
-	if (!ccorp) e->ccorp_every = false;
-	else if (e->ccorp_every) {                          // an earlier accumulate of the session did not set the flag: finish refuses
-		if (!e->ccorp_armed && (rc = ccorp_arm(e, e->score_C))) return rc;
-		if ((rc = launch_ccorp(e, ev, cand_offset))) return rc;
-	}
-	if (!cand) { e->cand_every = false; return APO_OK; }
-	if (!e->cand_every) return APO_OK;                  // an earlier accumulate of the session did not set the flag: finish refuses
-	return launch_cand(e, ev, cand_offset);
+	for (int p = 0; p < NPASS; p++)                     // a pass this accumulate does not flag: finish refuses it
+		if (!wants(o, p)) e->pass[p].every = false;
+	return launch_passes(e, o, ev, cand_offset);
 }
 
 extern "C" int apo_score_finish(apo_engine *e, const apo_score_opts *o, double *scores, uint64_t *counts, int32_t *topk,
                                 apo_corpus_report *report) {
 	if (!e) return APO_E_ARG;
-	e->cand_ready = e->ccorp_ready = e->ext_ready = e->grp_ready = false;   // a failed finish leaves no breakdown behind either
+	unready_passes(e);
 	if (!o) return fail(e, APO_E_ARG, "opts is NULL");
 	if (!e->scoring) return fail(e, APO_E_STATE, "apo_score_begin has not been called");
 	int rc = score_check(e, o, e->score_C, kSession, true);      // the accumulate calls refused every other source
 	if (rc) return rc;
-	if (wants_grp(o) && !e->grp_every)
-		return fail(e, APO_E_STATE, "APO_SCORE_CANDIDATE_GROUPS: every apo_score_accumulate of the session must set the flag for the group scores");
-	if (wants_grp(o) && e->grp_armed && e->grp_arm_gen != e->grp_gen)
-		return fail(e, APO_E_STATE, "APO_SCORE_CANDIDATE_GROUPS: the record groups were uploaded again after the session began to accumulate them");
-	if (wants_cand(o) && !e->cand_every)
-		return fail(e, APO_E_STATE, "APO_SCORE_CANDIDATES: every apo_score_accumulate of the session must set the flag for a breakdown");
-	if (wants_ccorp(o) && !e->ccorp_every)
-		return fail(e, APO_E_STATE, "APO_SCORE_CANDIDATE_CORPUS: every apo_score_accumulate of the session must set the flag for the reports");
-	if (wants_ext(o) && !e->ext_every)
-		return fail(e, APO_E_STATE, "APO_SCORE_CANDIDATE_EXTREMES: every apo_score_accumulate of the session must set the flag for the lists");
+	for (const int p : {PASS_GRP, PASS_CAND, PASS_CCORP, PASS_EXT}) {
+		if (!wants(o, p)) continue;
+		if (!e->pass[p].every)
+			return fail(e, APO_E_STATE, "%s: every apo_score_accumulate of the session must set the flag for %s", kPass[p].name, kPass[p].every);
+		if (p == PASS_GRP && e->pass[p].armed && e->grp_arm_gen != e->grp_gen)
+			return fail(e, APO_E_STATE, "APO_SCORE_CANDIDATE_GROUPS: the record groups were uploaded again after the session began to accumulate them");
+	}
 	if ((rc = digest_prepare(e, o)) || (rc = score_arm(e, o, e->score_C, false))) return rc;   // nothing accumulated yet: an empty breakdown
 	return finish_score(e, o, e->score_C, scores, counts, topk, report);
 }
 
 extern "C" int apo_score(apo_engine *e, const apo_score_opts *o, double *scores, uint64_t *counts, int32_t *topk, apo_corpus_report *report) {
 	if (!e) return APO_E_ARG;
-	e->cand_ready = e->ccorp_ready = e->ext_ready = e->grp_ready = false;   // a failed call leaves no breakdown behind either
+	unready_passes(e);
 	Evals ev;
 	int rc = resident_evals(e, o, &ev);
 	if (rc) return rc;
@@ -2261,11 +2176,7 @@ extern "C" int apo_score(apo_engine *e, const apo_score_opts *o, double *scores,
 		k2 = make_k2(e, C, F);
 		if (tail_only || (kh && !kh_corpus)) { k2.T = 0; k2.recs = nullptr; }
 	}
-	if ((rc = launch_score(e, o, ev, 0, fused ? &k2 : nullptr))) return rc;
-	if (wants_cand(o) && (rc = launch_cand(e, ev, 0))) return rc;
-	if (wants_ccorp(o) && (rc = launch_ccorp(e, ev, 0))) return rc;
-	if (wants_ext(o) && (rc = launch_ext(e, o, ev, 0))) return rc;
-	if (wants_grp(o) && (rc = launch_grp(e, o, ev, 0))) return rc;
+	if ((rc = launch_score(e, o, ev, 0, fused ? &k2 : nullptr)) || (rc = launch_passes(e, o, ev, 0))) return rc;
 	return finish_score(e, o, C, scores, counts, topk, report, fused);
 }
 
@@ -2316,10 +2227,10 @@ int stream_host(apo_engine *e, const apo_score_opts *o, const HostTensor &h, dou
                 apo_corpus_report *report) {
 	const uint32_t C = h.C;
 	const uint64_t T = h.T;
-	e->cand_ready = e->ccorp_ready = e->ext_ready = e->grp_ready = false;
+	unready_passes(e);
 	if (!o) return fail(e, APO_E_ARG, "opts is NULL");
 	const bool rows = h.form != apo::CAND_Q && h.form != apo::CAND_T;
-	if (!rows && wants_ccorp(o)) return ccorp_check(e, false);   // the wire formats refuse it before they look at their inputs
+	if (!rows && wants(o, PASS_CCORP)) return refuse_no_records(e);   // the wire formats refuse it before they look at their inputs
 	int rc;
 	if (h.form == apo::CAND_T) {
 		if ((rc = tuples_args(e, (const uint16_t *)h.plane[0].p, (const uint8_t *)h.plane[1].p, h.tb_pc, h.tb_pd, h.n_tuples, h.codebook,
@@ -2332,7 +2243,7 @@ int stream_host(apo_engine *e, const apo_score_opts *o, const HostTensor &h, dou
 	}
 	Evals ev;
 	ev.form = h.form; ev.C = C; ev.variant = (int)o->variant;
-	if ((rc = score_check(e, o, C, kStreamed, ev.records())) || (wants_grp(o) && (rc = grp_check(e, T))) || (rc = digest_prepare(e, o))) return rc;
+	if ((rc = score_check(e, o, C, kStreamed, ev.records())) || (wants(o, PASS_GRP) && (rc = labels_check(e, T))) || (rc = digest_prepare(e, o))) return rc;
 	if (h.form == apo::CAND_Q) {                                   // Form Q / P: K1q's tables of this call's codebook
 		if ((rc = load_qtables(e, e->qt_stream, h.codebook))) return rc;
 		ev.qt = &e->qt_stream;
@@ -2367,7 +2278,7 @@ int stream_host(apo_engine *e, const apo_score_opts *o, const HostTensor &h, dou
 	}
 	if ((rc = score_arm(e, o, C, true, (uint64_t)C * T * wire))) return rc;
 	if (h.form == apo::CAND_T) {                                   // the dictionary and its values, once for the whole call
-		if ((wants_cand(o) || wants_ext(o) || wants_grp(o)) && (rc = cand_upload_tbook(e, h.codebook))) return rc;
+		if ((wants(o, PASS_CAND) || wants(o, PASS_EXT) || wants(o, PASS_GRP)) && (rc = upload_tbook(e, h.codebook))) return rc;
 		if ((rc = dict_upload(e, e->tups, h.tb_pc, h.tb_pd, h.n_tuples, h.codebook, h.d2book))) return rc;
 		ev.dict = &e->tups; ev.t_once = true;
 		if ((rc = tuple_values(e, e->tups, e->tvals, (o->flags & APO_SCORE_RECIP) != 0))) return rc;
@@ -2409,11 +2320,7 @@ int stream_host(apo_engine *e, const apo_score_opts *o, const HostTensor &h, dou
 			                     code_ok[1], e->unpack_bad.p, (unsigned long long *)w, (float *)(w + CTc * 8), (unsigned short *)(w + CTc * 12), Tc, e->stream));
 			e->timing.launches++;
 		}
-		if ((rc = launch_score(e, o, ev, 0))) return rc;
-		if (wants_cand(o) && (rc = launch_cand(e, ev, 0))) return rc;
-		if (wants_ccorp(o) && (rc = launch_ccorp(e, ev, 0))) return rc;   // before the window is released
-		if (wants_ext(o) && (rc = launch_ext(e, o, ev, 0))) return rc;
-		if (wants_grp(o) && (rc = launch_grp(e, o, ev, 0))) return rc;
+		if ((rc = launch_score(e, o, ev, 0)) || (rc = launch_passes(e, o, ev, 0))) return rc;   // before the window is released
 		CK(cudaEventRecord(e->win_free[b], e->stream));
 	}
 	return finish_score(e, o, C, scores, counts, topk, report, false, h.packed);
@@ -2682,36 +2589,21 @@ extern "C" int apo_debug_corpus_digest(apo_engine *e, uint64_t *n_entries, uint6
 }
 
 extern "C" int apo_candidate_reports(apo_engine *e, uint32_t c0, uint32_t n, apo_candidate_report *out) {
-	if (!e) return APO_E_ARG;
-	if (!e->cand_ready) return fail(e, APO_E_STATE, "the last scoring call did not set APO_SCORE_CANDIDATES");
-	if ((uint64_t)c0 + n > e->cand_C) return fail(e, APO_E_ARG, "candidates [%u,%llu) exceed C=%u", c0, (unsigned long long)c0 + n, e->cand_C);
-	if (n == 0) return APO_OK;
-	if (!out) return fail(e, APO_E_ARG, "out is NULL");
-	CK(cudaSetDevice(e->device));
+	if (const int rc = report_check(e, PASS_CAND, c0, n, out); rc || n == 0) return rc;
 	CK(cudaMemcpyAsync(out, e->cand_rep.p + c0, (uint64_t)n * sizeof(apo_candidate_report), cudaMemcpyDeviceToHost, e->stream));
 	CK(cudaStreamSynchronize(e->stream));
 	return APO_OK;
 }
 
 extern "C" int apo_candidate_corpus_reports(apo_engine *e, uint32_t c0, uint32_t n, apo_corpus_report *out) {
-	if (!e) return APO_E_ARG;
-	if (!e->ccorp_ready) return fail(e, APO_E_STATE, "the last scoring call did not set APO_SCORE_CANDIDATE_CORPUS");
-	if ((uint64_t)c0 + n > e->ccorp_C) return fail(e, APO_E_ARG, "candidates [%u,%llu) exceed C=%u", c0, (unsigned long long)c0 + n, e->ccorp_C);
-	if (n == 0) return APO_OK;
-	if (!out) return fail(e, APO_E_ARG, "out is NULL");
-	CK(cudaSetDevice(e->device));
+	if (const int rc = report_check(e, PASS_CCORP, c0, n, out); rc || n == 0) return rc;
 	CK(cudaMemcpyAsync(out, e->ccorp_rep.p + c0, (uint64_t)n * sizeof(apo_corpus_report), cudaMemcpyDeviceToHost, e->stream));
 	CK(cudaStreamSynchronize(e->stream));
 	return APO_OK;
 }
 
 extern "C" int apo_candidate_extremes(apo_engine *e, uint32_t c0, uint32_t n, struct apo_candidate_extremes *out) {
-	if (!e) return APO_E_ARG;
-	if (!e->ext_ready) return fail(e, APO_E_STATE, "the last scoring call did not set APO_SCORE_CANDIDATE_EXTREMES");
-	if ((uint64_t)c0 + n > e->ext_C) return fail(e, APO_E_ARG, "candidates [%u,%llu) exceed C=%u", c0, (unsigned long long)c0 + n, e->ext_C);
-	if (n == 0) return APO_OK;
-	if (!out) return fail(e, APO_E_ARG, "out is NULL");
-	CK(cudaSetDevice(e->device));
+	if (const int rc = report_check(e, PASS_EXT, c0, n, out); rc || n == 0) return rc;
 	std::vector<unsigned long long> keys((uint64_t)n * apo::CX_WORDS);
 	CK(cudaMemcpyAsync(keys.data(), e->ext_acc.p + (uint64_t)c0 * apo::CX_WORDS, keys.size() * 8, cudaMemcpyDeviceToHost, e->stream));
 	CK(cudaStreamSynchronize(e->stream));
@@ -2758,13 +2650,7 @@ extern "C" int apo_record_groups_upload(apo_engine *e, const uint8_t *labels, ui
 }
 
 extern "C" int apo_candidate_groups(apo_engine *e, uint32_t c0, uint32_t n, uint32_t G, apo_group_score *out) {
-	if (!e) return APO_E_ARG;
-	if (!e->grp_ready) return fail(e, APO_E_STATE, "the last scoring call did not set APO_SCORE_CANDIDATE_GROUPS");
-	if (G != e->grp_rep_G) return fail(e, APO_E_ARG, "G=%u is not the G=%u the last scoring call split by", G, e->grp_rep_G);
-	if ((uint64_t)c0 + n > e->grp_C) return fail(e, APO_E_ARG, "candidates [%u,%llu) exceed C=%u", c0, (unsigned long long)c0 + n, e->grp_C);
-	if (n == 0) return APO_OK;
-	if (!out) return fail(e, APO_E_ARG, "out is NULL");
-	CK(cudaSetDevice(e->device));
+	if (const int rc = report_check(e, PASS_GRP, c0, n, out, G); rc || n == 0) return rc;
 	CK(cudaMemcpyAsync(out, e->grp_rep.p + (uint64_t)c0 * G, (uint64_t)n * G * sizeof(apo_group_score), cudaMemcpyDeviceToHost, e->stream));
 	CK(cudaStreamSynchronize(e->stream));
 	return APO_OK;

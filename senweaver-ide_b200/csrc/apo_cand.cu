@@ -5,8 +5,8 @@
 //                             record positions): per candidate the feedback tallies, the exact fixed-point sum and count of
 //                             every present dimension over the non-null evaluations, and the first three 'bad' positions.
 //                             Domain: a present dimension of a non-null evaluation must satisfy |v| < 2048, where rint(v * 2^52)
-//                             still fits in int64; any other value raises P.dom and the call fails with APO_E_ARG (the scoring
-//                             kernels bound only finalReward, so d4 = 3000 with w4 = 0 scores normally but has no exact sum)
+//                             still fits in int64; any other value raises CandParams::dom and the call fails with APO_E_ARG (the
+//                             scoring kernels bound only finalReward, so d4 = 3000 with w4 = 0 scores normally but has no exact sum)
 //   k_cand_report             integers -> apo_candidate_report[C] with the rules of the corpus report (apo_corpus.cuh
 //                             report_*), rewardSum / withReward taken from the scoring call's own accumulators
 //
@@ -17,6 +17,8 @@
 //
 // For record sources a second feature (APO_SCORE_CANDIDATE_CORPUS, k_cand_corpus below) goes further: the whole corpus
 // report of every candidate's records — patterns, per-mode tallies and tool totals included — by the corpus scan's own code.
+// The extremes and the group scores follow.  Every pass is one walk (cand_walk) over the same warp tiles with its own
+// per-evaluation step and flush, and one launcher sizes every walk's grid (walk_grid).
 #include <cstdlib>
 #include "apo_device.cuh"
 #include "apo_format.h"
@@ -64,12 +66,12 @@ struct LoadDims {
 	static constexpr int MIN_CTAS = 2;
 	static constexpr bool CHECK = true;
 	struct Raw { float f[APO_NDIM]; };
-	__device__ static void fetch(const CandParams &P, uint32_t c, uint64_t t, Raw &R) {
+	__device__ static void fetch(const CandEvals &P, uint32_t c, uint64_t t, Raw &R) {
 		const float *p = reinterpret_cast<const float *>(P.rows) + ((uint64_t)c * P.pitch_evals + t) * APO_NDIM;
 #pragma unroll
 		for (int i = 0; i < APO_NDIM; i++) R.f[i] = __ldg(p + i);
 	}
-	__device__ static void decode(const CandParams &, const CandSmem &S, const Raw &R, CandEval &E) {
+	__device__ static void decode(const CandEvals &, const CandSmem &S, const Raw &R, CandEval &E) {
 		uint32_t mask = 0, mag = 0;
 #pragma unroll
 		for (int i = 0; i < APO_NDIM; i++) {
@@ -91,15 +93,19 @@ struct LoadRec {
 	static constexpr int MIN_CTAS = 1;
 	static constexpr bool CHECK = false;
 	struct Raw { uint4 q[ROW / 16]; };
-	__device__ static void fetch(const CandParams &P, uint32_t c, uint64_t t, Raw &R) {
+	__device__ static void fetch(const CandEvals &P, uint32_t c, uint64_t t, Raw &R) {
 		const uint4 *p = reinterpret_cast<const uint4 *>(P.rows + ((uint64_t)c * P.pitch_evals + t) * ROW);
 #pragma unroll
 		for (int k = 0; k < ROW / 16; k++) R.q[k] = __ldg(p + k);
 	}
-	__device__ static void decode(const CandParams &, const CandSmem &S, const Raw &R, CandEval &E) {
+	__device__ static apo_record record(const Raw &R) {
 		apo_record r;
-		if (ROW == 32) { memcpy(&r, &R, sizeof r); }
+		if constexpr (ROW == 32) { memcpy(&r, &R, sizeof r); }
 		else { apo_record16 p; memcpy(&p, &R, sizeof p); r = unpack16(p); }
+		return r;
+	}
+	__device__ static void decode(const CandEvals &, const CandSmem &S, const Raw &R, CandEval &E) {
+		const apo_record r = record(R);
 		E.mask = reward_dims(r, E.v);                                          // TCS:668-763 in binary64
 		E.valid = ((r.flags & APO_F_VALID) && S.tw[E.mask] > 0.0) ? 1u : 0u;  // TCS:606, 784
 		E.fb = r.feedback == 1 ? 1u : (r.feedback == 2 ? 2u : 0u);            // as the corpus scan counts (APO:509-516)
@@ -111,11 +117,11 @@ struct LoadQ {
 	static constexpr int MIN_CTAS = 2;
 	static constexpr bool CHECK = true;
 	struct Raw { unsigned long long q; float d2; uint32_t li; };
-	__device__ static void fetch(const CandParams &P, uint32_t c, uint64_t t, Raw &R) {
+	__device__ static void fetch(const CandEvals &P, uint32_t c, uint64_t t, Raw &R) {
 		const uint64_t o = (uint64_t)c * P.pitch_evals + t;
 		R.q = __ldg(P.q8 + o); R.d2 = __ldg(P.d2 + o); R.li = __ldg(P.li + o);
 	}
-	__device__ static void decode(const CandParams &, const CandSmem &S, const Raw &R, CandEval &E) {
+	__device__ static void decode(const CandEvals &, const CandSmem &S, const Raw &R, CandEval &E) {
 		uint32_t mask = 0, mag = 0;
 #pragma unroll
 		for (int j = 0; j < 8; j++) {
@@ -142,10 +148,10 @@ struct LoadW {
 	static constexpr int MIN_CTAS = 2;
 	static constexpr bool CHECK = true;
 	struct Raw { unsigned long long q; };
-	__device__ static void fetch(const CandParams &P, uint32_t c, uint64_t t, Raw &R) {
+	__device__ static void fetch(const CandEvals &P, uint32_t c, uint64_t t, Raw &R) {
 		R.q = __ldg(P.qw + (uint64_t)c * P.pitch_evals + t);
 	}
-	__device__ static void decode(const CandParams &, const CandSmem &S, const Raw &R, CandEval &E) {
+	__device__ static void decode(const CandEvals &, const CandSmem &S, const Raw &R, CandEval &E) {
 		const uint32_t w = (uint32_t)R.q;
 		uint32_t mask = 0, mag = 0;
 #pragma unroll
@@ -173,11 +179,11 @@ struct LoadT {
 	static constexpr int MIN_CTAS = 1;
 	static constexpr bool CHECK = true;
 	struct Raw { uint32_t idx; };
-	__device__ static void fetch(const CandParams &P, uint32_t c, uint64_t t, Raw &R) {
+	__device__ static void fetch(const CandEvals &P, uint32_t c, uint64_t t, Raw &R) {
 		const uint64_t o = (uint64_t)c * P.pitch_evals + t;
 		R.idx = (uint32_t)__ldg(P.tl + o) | ((uint32_t)__ldg(P.th + o) << 16);
 	}
-	__device__ static void decode(const CandParams &P, const CandSmem &S, const Raw &R, CandEval &E) {
+	__device__ static void decode(const CandEvals &P, const CandSmem &S, const Raw &R, CandEval &E) {
 		// an index outside the dictionary fails the scoring call (K1t); here it reads as an evaluation with nothing present
 		const bool in = R.idx < P.n_tuples;
 		const uint32_t w = in ? __ldg(P.tb_pc + R.idx) : 0xFFFFFFFFu;
@@ -203,33 +209,120 @@ struct LoadT {
 	}
 };
 
-// Every warp walks a contiguous range of warp tiles (candidate-major: tile = c * tiles_per_cand + j), keeps its lane
-// partials while the candidate stays the same and flushes them into the candidate's words when it changes.  The first
-// three 'bad' positions of a run are found with ballots over groups of 32 consecutive evaluations (ascending order
-// inside the run), then merged into the candidate's slots with ex_insert, gated on the third slot.
-template <class L, int TABLE>
-__global__ void __launch_bounds__(CB_THREADS, L::MIN_CTAS)
-k_cand_breakdown(const CandParams P, uint32_t tiles_per_cand, uint64_t total_tiles) {
-	__shared__ CandSmem S;
-	for (int i = threadIdx.x; i < 512; i += CB_THREADS) S.tw[i] = P.lut[i];
+// ================================================================ the walk every per-candidate pass shares
+constexpr int CB_WARPS = CB_THREADS / 32;
+
+// the total-weight LUT, its reciprocals into rc for the passes that divide as div_lut does (DIV), and the source's
+// code -> value table
+template <int TABLE, bool DIV = false>
+__device__ __forceinline__ void stage_tables(const CandEvals &P, CandSmem &S, double *rc = nullptr) {
+	for (int i = threadIdx.x; i < 512; i += CB_THREADS) {
+		S.tw[i] = P.lut[i];
+		if (DIV) rc[i] = P.lut[512 + i];
+	}
 	if (TABLE == 1) for (int i = threadIdx.x; i < 8 * 256; i += CB_THREADS) S.tab[i] = P.cbf[i];
 	if (TABLE == 2) for (int i = threadIdx.x; i < 8 * 16; i += CB_THREADS) S.tab[i] = P.tbook[i];
 	__syncthreads();
+}
+
+__device__ __forceinline__ uint64_t cand_warp() { return (uint64_t)blockIdx.x * CB_WARPS + (threadIdx.x >> 5); }
+
+struct NoSide { __device__ uint32_t operator()(uint64_t) const { return 0u; } };
+
+// Warp tiles of CB_TILE evaluations run candidate-major (tile = c * tiles_per_cand + j), and every warp walks a contiguous
+// range of them (the range k_cand_extremes_merge inverts).  A lane keeps L::U groups of 32 evaluations in flight, then
+// each(c, t, in, R, s) sees them in order: t is the lane's evaluation, in says whether it lies inside the row, and only then
+// do R (its fetch) and s (side(t), fetched with it) hold anything.  A group wholly past the row end ends the tile,
+// warp-uniformly.  flush(c) ends the warp's run of candidate c: when the candidate changes, after every RUN tiles (0: never)
+// and after the last tile.
+template <class L, uint32_t RUN, class Each, class Flush, class Side = NoSide>
+__device__ __forceinline__ void cand_walk(const CandEvals &P, uint32_t tiles_per_cand, uint64_t total_tiles, Each &&each, Flush &&flush,
+                                          Side side = {}) {
 	const int lane = threadIdx.x & 31;
-	const uint64_t nwarps = (uint64_t)gridDim.x * (CB_THREADS / 32);
-	const uint64_t gw = (uint64_t)blockIdx.x * (CB_THREADS / 32) + (threadIdx.x >> 5);
+	const uint64_t nwarps = (uint64_t)gridDim.x * CB_WARPS, gw = cand_warp();
 	const uint64_t lo = total_tiles * gw / nwarps, hi = total_tiles * (gw + 1) / nwarps;
 	if (lo >= hi) return;
+	uint32_t cur = (uint32_t)(lo / tiles_per_cand), run = 0;
+	for (uint64_t tile = lo; tile < hi; tile++) {
+		const uint32_t c = (uint32_t)(tile / tiles_per_cand), j = (uint32_t)(tile - (uint64_t)c * tiles_per_cand);
+		if (c != cur || (RUN && run == RUN)) { flush(cur); cur = c; run = 0; }
+		run++;
+		const uint64_t t0 = (uint64_t)j * CB_TILE;
+		for (int g0 = 0; g0 < CB_GROUPS; g0 += L::U) {
+			typename L::Raw R[L::U];
+			bool in[L::U];
+			uint32_t s[L::U];
+#pragma unroll
+			for (int u = 0; u < L::U; u++) {
+				const uint64_t t = t0 + (uint64_t)(g0 + u) * 32 + lane;
+				in[u] = t < P.T;
+				s[u] = in[u] ? side(t) : 0u;
+				if (in[u]) L::fetch(P, c, t, R[u]);
+			}
+#pragma unroll
+			for (int u = 0; u < L::U; u++) {
+				const uint64_t t = t0 + (uint64_t)(g0 + u) * 32 + lane;
+				if (t - lane >= P.T) break;                                 // warp-uniform: the rest of the tile is past the row end
+				each(c, t, in[u], R[u], s[u]);
+			}
+		}
+	}
+	flush(cur);
+}
 
+// APO_K1_GRID caps the grids of the per-candidate passes as it caps the scoring kernels' (tuning and tests only, read once)
+static uint64_t cand_env_grid() { static const int g = [] { const char *s = getenv("APO_K1_GRID"); return s ? atoi(s) : 0; }(); return g > 0 ? (uint64_t)g : 0; }
+
+// The tiles of a launch over P and the grid of a walk kernel for them: as many CTAs as the SMs hold at once, no more than the
+// tiles need, at most APO_K1_GRID.  grid = 0: nothing to walk.
+struct Walk { uint32_t tiles_per_cand; uint64_t total_tiles, grid; };
+
+template <class K>
+static cudaError_t walk_grid(K *kernel, const CandEvals &P, int sm_count, Walk &w) {
+	w.tiles_per_cand = (uint32_t)((P.T + CB_TILE - 1) / CB_TILE);
+	w.total_tiles = (uint64_t)w.tiles_per_cand * P.C;
+	w.grid = 0;
+	if (w.total_tiles == 0) return cudaSuccess;
+	int per_sm = 0;
+	const cudaError_t err = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, CB_THREADS, 0);
+	if (err != cudaSuccess) return err;
+	w.grid = (uint64_t)sm_count * (uint64_t)(per_sm > 0 ? per_sm : 1);
+	const uint64_t need = (w.total_tiles + CB_WARPS - 1) / CB_WARPS;
+	if (w.grid > need) w.grid = need;
+	if (cand_env_grid() && cand_env_grid() < w.grid) w.grid = cand_env_grid();
+	return cudaSuccess;
+}
+
+// a pass that is its walk kernel alone
+template <class X>
+static cudaError_t launch_walk(void (*kernel)(X, uint32_t, uint64_t), const X &x, int sm_count, cudaStream_t st) {
+	Walk w;
+	const cudaError_t err = walk_grid(kernel, x.src, sm_count, w);
+	if (err != cudaSuccess || w.grid == 0) return err;
+	kernel<<<(unsigned)w.grid, CB_THREADS, 0, st>>>(x, w.tiles_per_cand, w.total_tiles);
+	return cudaGetLastError();
+}
+
+// ================================================================ per-candidate breakdown (APO_SCORE_CANDIDATES)
+// Every warp keeps its lane partials while the candidate stays the same and flushes them into the candidate's words.  The
+// first three 'bad' positions of a run are found with ballots over groups of 32 consecutive evaluations (ascending order
+// inside the run), then merged into the candidate's slots with ex_insert, gated on the third slot.
+template <class L, int TABLE>
+__global__ void __launch_bounds__(CB_THREADS, L::MIN_CTAS)
+k_cand_breakdown(const CandParams X, uint32_t tiles_per_cand, uint64_t total_tiles) {
+	const CandEvals &P = X.src;
+	__shared__ CandSmem S;
+	stage_tables<TABLE>(P, S);
+	const int lane = threadIdx.x & 31;
 	Acc128 acc[APO_NDIM];
-	uint32_t cnt[APO_NDIM], n = 0, good = 0, bad = 0, nfound = 0, run = 0;
+	uint32_t cnt[APO_NDIM], n = 0, good = 0, bad = 0, nfound = 0;
 	uint32_t dom = 0;                                                    // largest CandEval::mag of a counted evaluation
 	unsigned long long f0 = 0ull, f1 = 0ull, f2 = 0ull;                 // first 'bad' positions of the run (nfound of them)
 #pragma unroll
 	for (int i = 0; i < APO_NDIM; i++) { acc[i].zero(); cnt[i] = 0; }
 
 	auto flush = [&](uint32_t c) {
-		long long *w = P.ints + (uint64_t)c * CB_INT;
+		long long *w = X.ints + (uint64_t)c * CB_INT;
 #pragma unroll
 		for (int i = 0; i < APO_NDIM; i++) {
 			flush_acc128(acc[i], w + CB_DIM + 4 * i, lane);
@@ -242,97 +335,46 @@ k_cand_breakdown(const CandParams P, uint32_t tiles_per_cand, uint64_t total_til
 			if (sn) atomicAdd((unsigned long long *)w + CB_TALLY, (unsigned long long)sn);
 			if (sg) atomicAdd((unsigned long long *)w + CB_TALLY + 1, (unsigned long long)sg);
 			if (sb) atomicAdd((unsigned long long *)w + CB_TALLY + 2, (unsigned long long)sb);
-			unsigned long long *slots = P.ex + 3ull * c;
+			unsigned long long *slots = X.ex + 3ull * c;
 			for (uint32_t k = 0; k < nfound; k++) {
 				const unsigned long long key = ~(k == 0 ? f0 : (k == 1 ? f1 : f2));   // inverted index (see ex_insert)
 				if (key > *((volatile unsigned long long *)&slots[2])) ex_insert(slots, key);
 			}
 		}
-		n = good = bad = 0; nfound = 0; run = 0;
+		n = good = bad = 0; nfound = 0;
 	};
-
-	uint32_t cur = (uint32_t)(lo / tiles_per_cand);
-	for (uint64_t tile = lo; tile < hi; tile++) {
-		const uint32_t c = (uint32_t)(tile / tiles_per_cand), j = (uint32_t)(tile - (uint64_t)c * tiles_per_cand);
-		if (c != cur || run == CB_RUN_TILES) { flush(cur); cur = c; }
-		run++;
-		const uint64_t t0 = (uint64_t)j * CB_TILE;
-		for (int g0 = 0; g0 < CB_GROUPS; g0 += L::U) {
-			typename L::Raw R[L::U];
-			bool in[L::U];
+	auto each = [&](uint32_t, uint64_t t, bool in, const typename L::Raw &R, uint32_t) {
+		bool isbad = false;
+		if (in) {
+			CandEval E;
+			L::decode(P, S, R, E);
+			n++;
+			good += E.fb == 1u ? 1u : 0u;
+			isbad = E.fb == 2u;
+			bad += isbad ? 1u : 0u;
+			if (E.valid) {
+				if (L::CHECK) dom = max(dom, E.mag);
 #pragma unroll
-			for (int u = 0; u < L::U; u++) {
-				const uint64_t t = t0 + (uint64_t)(g0 + u) * 32 + lane;
-				in[u] = t < P.T;
-				if (in[u]) L::fetch(P, c, t, R[u]);
-			}
-#pragma unroll
-			for (int u = 0; u < L::U; u++) {
-				if (t0 + (uint64_t)(g0 + u) * 32 >= P.T) break;                 // warp-uniform: the rest of the tile is past the row end
-				CandEval E;
-				bool isbad = false;
-				if (in[u]) {
-					L::decode(P, S, R[u], E);
-					n++;
-					good += E.fb == 1u ? 1u : 0u;
-					isbad = E.fb == 2u;
-					bad += isbad ? 1u : 0u;
-					if (E.valid) {
-						if (L::CHECK) dom = max(dom, E.mag);
-#pragma unroll
-						for (int i = 0; i < APO_NDIM; i++) {
-							const bool p = (E.mask >> i) & 1u;
-							acc[i].add(p ? to_fx(E.v[i]) : 0ll);
-							cnt[i] += p ? 1u : 0u;
-						}
-					}
-				}
-				if (nfound < 3) {                                                 // warp-uniform
-					unsigned int m = __ballot_sync(0xffffffffu, isbad);
-					while (m && nfound < 3) {
-						const uint32_t pos = (uint32_t)(__ffs((int)m) - 1);
-						const unsigned long long gi = P.idx_base + t0 + (uint64_t)(g0 + u) * 32 + pos;
-						if (nfound == 0) f0 = gi; else if (nfound == 1) f1 = gi; else f2 = gi;
-						nfound++;
-						m &= m - 1u;
-					}
+				for (int i = 0; i < APO_NDIM; i++) {
+					const bool p = (E.mask >> i) & 1u;
+					acc[i].add(p ? to_fx(E.v[i]) : 0ll);
+					cnt[i] += p ? 1u : 0u;
 				}
 			}
 		}
-	}
-	flush(cur);
-	if (dom >= CB_FX_BOUND_F32) atomicOr(P.dom, 1u);
-}
-
-// APO_K1_GRID caps the grids of both per-candidate passes as it caps the scoring kernels' (tuning and tests only, read once)
-static uint64_t cand_env_grid() { static const int g = [] { const char *s = getenv("APO_K1_GRID"); return s ? atoi(s) : 0; }(); return g > 0 ? (uint64_t)g : 0; }
-
-template <class L, int TABLE>
-static cudaError_t launch_cand(const CandParams &P, int sm_count, cudaStream_t st) {
-	const uint32_t tiles_per_cand = (uint32_t)((P.T + CB_TILE - 1) / CB_TILE);
-	const uint64_t total_tiles = (uint64_t)tiles_per_cand * P.C;
-	if (total_tiles == 0) return cudaSuccess;
-	int per_sm = 0;
-	cudaError_t err = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_cand_breakdown<L, TABLE>, CB_THREADS, 0);
-	if (err != cudaSuccess) return err;
-	uint64_t grid = (uint64_t)sm_count * (uint64_t)(per_sm > 0 ? per_sm : 1);
-	const uint64_t need = (total_tiles + (CB_THREADS / 32) - 1) / (CB_THREADS / 32);
-	if (grid > need) grid = need;
-	if (cand_env_grid() && cand_env_grid() < grid) grid = cand_env_grid();
-	k_cand_breakdown<L, TABLE><<<(unsigned)grid, CB_THREADS, 0, st>>>(P, tiles_per_cand, total_tiles);
-	return cudaGetLastError();
-}
-
-cudaError_t run_cand_breakdown(const CandParams &P, int source, int sm_count, cudaStream_t st) {
-	switch (source) {
-	case CAND_DIMS: return launch_cand<LoadDims, 0>(P, sm_count, st);
-	case CAND_REC32: return launch_cand<LoadRec<32>, 0>(P, sm_count, st);
-	case CAND_REC16: return launch_cand<LoadRec<16>, 0>(P, sm_count, st);
-	case CAND_Q: return launch_cand<LoadQ, 1>(P, sm_count, st);
-	case CAND_T: return launch_cand<LoadT, 2>(P, sm_count, st);
-	case CAND_W: return launch_cand<LoadW, 1>(P, sm_count, st);
-	default: return cudaErrorInvalidValue;
-	}
+		if (nfound < 3) {                                                     // warp-uniform
+			unsigned int m = __ballot_sync(0xffffffffu, isbad);
+			while (m && nfound < 3) {
+				const uint32_t pos = (uint32_t)(__ffs((int)m) - 1);
+				const unsigned long long gi = P.idx_base + (t - lane) + pos;
+				if (nfound == 0) f0 = gi; else if (nfound == 1) f1 = gi; else f2 = gi;
+				nfound++;
+				m &= m - 1u;
+			}
+		}
+	};
+	cand_walk<L, CB_RUN_TILES>(P, tiles_per_cand, total_tiles, each, flush);
+	if (dom >= CB_FX_BOUND_F32) atomicOr(X.dom, 1u);
 }
 
 // one thread per candidate
@@ -378,39 +420,31 @@ cudaError_t run_cand_report(const long long *ints, const unsigned long long *ex,
 //                           that a scoring call reads, into one corpus block per candidate
 //   k_cand_corpus_report    corpus block -> apo_corpus_report with build_report, the code of the corpus report itself
 static_assert(CC_WORDS == CORP_FIXED + APO_NPAT * 3, "one rank's corpus block with its example slots");
-constexpr int CC_THREADS = 256;
-constexpr int CC_WARPS = CC_THREADS / 32;
-constexpr int CC_GROUPS = 32;                               // records per lane in a warp tile (one candidate)
-constexpr int CC_TILE = 32 * CC_GROUPS;
-constexpr uint32_t CC_RUN_TILES = K2_CHUNK / CC_GROUPS;     // the packed ScanAcc fields hold K2_CHUNK records per lane
-static_assert(K2_CHUNK % CC_GROUPS == 0, "a chunk is a whole number of tiles");
+constexpr uint32_t CC_RUN_TILES = K2_CHUNK / CB_GROUPS;     // the packed ScanAcc fields hold K2_CHUNK records per lane
+static_assert(K2_CHUNK % CB_GROUPS == 0, "a chunk is a whole number of tiles");
 
-// Warps walk candidate-major tiles as k_cand_breakdown does.  A warp flushes its ScanAcc into the candidate's block when the
-// candidate changes and after every CC_RUN_TILES tiles; its pattern examples collect in the warp's own 18 shared slots and
-// are merged into the candidate's slots at every flush (ex_insert, gated on the third slot).
+// The walk of the breakdown over LoadRec's records.  A warp flushes its ScanAcc into the candidate's block when the candidate
+// changes and after every CC_RUN_TILES tiles; its pattern examples collect in the warp's own 18 shared slots and are merged
+// into the candidate's slots at every flush (ex_insert, gated on the third slot).
 template <int ROW>
-__global__ void __launch_bounds__(CC_THREADS)
-k_cand_corpus(const CandCorpusParams P, uint32_t tiles_per_cand, uint64_t total_tiles) {
+__global__ void __launch_bounds__(CB_THREADS)
+k_cand_corpus(const CandCorpusParams X, uint32_t tiles_per_cand, uint64_t total_tiles) {
+	const CandEvals &P = X.src;
 	__shared__ double s_cat[CAT_WORDS];
 	__shared__ double2 s_lut[512];                          // {total weight, reciprocal} per (natural) presence mask
-	__shared__ unsigned long long s_ex[CC_WARPS][APO_NPAT * 3];
+	__shared__ unsigned long long s_ex[CB_WARPS][APO_NPAT * 3];
 	const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
 	if (tid < CAT_WORDS) s_cat[tid] = P.lut[1024 + tid];
-	for (int i = tid; i < 512; i += CC_THREADS) s_lut[i] = make_double2(P.lut[i], P.lut[512 + i]);
+	for (int i = tid; i < 512; i += CB_THREADS) s_lut[i] = make_double2(P.lut[i], P.lut[512 + i]);
 	if (lane < APO_NPAT * 3) s_ex[warp][lane] = 0ull;
 	__syncthreads();
-	const uint64_t nwarps = (uint64_t)gridDim.x * CC_WARPS;
-	const uint64_t gw = (uint64_t)blockIdx.x * CC_WARPS + warp;
-	const uint64_t lo = total_tiles * gw / nwarps, hi = total_tiles * (gw + 1) / nwarps;
-	if (lo >= hi) return;
 	unsigned long long *ex = s_ex[warp];
-	constexpr int U = ROW == 32 ? 2 : 4;                   // records in flight per lane
 	ScanAcc A;
 	A.zero();
-	uint32_t nrec = 0, run = 0;
+	uint32_t nrec = 0;
 
 	auto flush = [&](uint32_t c) {
-		long long *corp = P.blk + (uint64_t)c * CC_WORDS;
+		long long *corp = X.blk + (uint64_t)c * CC_WORDS;
 		scan_flush(A, corp, lane);
 		const uint32_t n = warp_sum_u32(nrec);              // CORP_NREC: corpus_tail writes it for the corpus, the pass counts here
 		if (lane == 0 && n) atomicAdd((unsigned long long *)corp + CORP_NREC, (unsigned long long)n);
@@ -423,62 +457,19 @@ k_cand_corpus(const CandCorpusParams P, uint32_t tiles_per_cand, uint64_t total_
 		}
 		__syncwarp();
 		A.zero();
-		nrec = 0; run = 0;
+		nrec = 0;
 	};
-
-	uint32_t cur = (uint32_t)(lo / tiles_per_cand);
-	for (uint64_t tile = lo; tile < hi; tile++) {
-		const uint32_t c = (uint32_t)(tile / tiles_per_cand), j = (uint32_t)(tile - (uint64_t)c * tiles_per_cand);
-		if (c != cur || run == CC_RUN_TILES) { flush(cur); cur = c; }
-		run++;
-		const uint64_t t0 = (uint64_t)j * CC_TILE;
-		const uint4 *row = reinterpret_cast<const uint4 *>(P.rows + (uint64_t)c * P.pitch_evals * ROW);
-		for (int g0 = 0; g0 < CC_GROUPS; g0 += U) {
-			if (t0 + (uint64_t)g0 * 32 >= P.T) break;                           // warp-uniform: the rest of the tile is past the row end
-			uint4 q[U][ROW / 16];
-#pragma unroll
-			for (int u = 0; u < U; u++) {
-				const uint64_t t = t0 + (uint64_t)(g0 + u) * 32 + lane;
-				if (t < P.T) {
-#pragma unroll
-					for (int k = 0; k < ROW / 16; k++) q[u][k] = __ldg(row + t * (ROW / 16) + k);
-				}
-			}
-#pragma unroll
-			for (int u = 0; u < U; u++) {
-				const uint64_t t = t0 + (uint64_t)(g0 + u) * 32 + lane;
-				if (t < P.T) {
-					apo_record r;
-					if constexpr (ROW == 32) { memcpy(&r, q[u], sizeof r); }
-					else { apo_record16 p; memcpy(&p, q[u], sizeof p); r = unpack16(p); }
-					scan_record<false>(A, r, P.idx_base + t, ex, s_cat, s_lut, P.w2);
-					nrec++;
-				}
-			}
-		}
-	}
-	flush(cur);
-}
-
-template <int ROW>
-static cudaError_t launch_cand_corpus(const CandCorpusParams &P, int sm_count, cudaStream_t st) {
-	const uint32_t tiles_per_cand = (uint32_t)((P.T + CC_TILE - 1) / CC_TILE);
-	const uint64_t total_tiles = (uint64_t)tiles_per_cand * P.C;
-	if (total_tiles == 0) return cudaSuccess;
-	int per_sm = 0;
-	cudaError_t err = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_cand_corpus<ROW>, CC_THREADS, 0);
-	if (err != cudaSuccess) return err;
-	uint64_t grid = (uint64_t)sm_count * (uint64_t)(per_sm > 0 ? per_sm : 1);
-	const uint64_t need = (total_tiles + CC_WARPS - 1) / CC_WARPS;
-	if (grid > need) grid = need;
-	if (cand_env_grid() && cand_env_grid() < grid) grid = cand_env_grid();
-	k_cand_corpus<ROW><<<(unsigned)grid, CC_THREADS, 0, st>>>(P, tiles_per_cand, total_tiles);
-	return cudaGetLastError();
+	auto each = [&](uint32_t, uint64_t t, bool in, const typename LoadRec<ROW>::Raw &R, uint32_t) {
+		if (!in) return;
+		scan_record<false>(A, LoadRec<ROW>::record(R), P.idx_base + t, ex, s_cat, s_lut, X.w2);
+		nrec++;
+	};
+	cand_walk<LoadRec<ROW>, CC_RUN_TILES>(P, tiles_per_cand, total_tiles, each, flush);
 }
 
 cudaError_t run_cand_corpus(const CandCorpusParams &P, int row, int sm_count, cudaStream_t st) {
-	if (row == 32) return launch_cand_corpus<32>(P, sm_count, st);
-	if (row == 16) return launch_cand_corpus<16>(P, sm_count, st);
+	if (row == 32) return launch_walk(k_cand_corpus<32>, P, sm_count, st);
+	if (row == 16) return launch_walk(k_cand_corpus<16>, P, sm_count, st);
 	return cudaErrorInvalidValue;
 }
 
@@ -508,8 +499,8 @@ cudaError_t run_cand_corpus_report(long long *blk, uint32_t C, apo_corpus_report
 }
 
 // ================================================================ per-candidate extremes (APO_SCORE_CANDIDATE_EXTREMES)
-//   k_cand_extremes<Loader, TABLE, RECIP>  one pass over the evaluations a scoring call reads, with the breakdown's loaders
-//                                          and tile walk: every warp keeps the 32 smallest keys of each list of its current
+//   k_cand_extremes<Loader, TABLE, RECIP>  one pass over the evaluations a scoring call reads, on the shared loaders and
+//                                          walk: every warp keeps the 32 smallest keys of each list of its current
 //                                          candidate in registers (lane i holds the i-th) and writes them to its segment
 //                                          slot when the candidate changes
 //   k_cand_extremes_merge                  one warp per candidate: the persistent lists merged with the segments of the
@@ -574,58 +565,32 @@ __device__ __forceinline__ void load_lists(const unsigned long long *slot, XKey 
 template <class L, int TABLE, bool RECIP>
 __global__ void __launch_bounds__(CB_THREADS, L::MIN_CTAS)
 k_cand_extremes(const CandExtParams X, uint32_t tiles_per_cand, uint64_t total_tiles) {
-	const CandParams &P = X.src;
+	const CandEvals &P = X.src;
 	__shared__ CandSmem S;
 	__shared__ double s_rc[512];                                        // reciprocal of the total weight (div_lut)
-	for (int i = threadIdx.x; i < 512; i += CB_THREADS) { S.tw[i] = P.lut[i]; s_rc[i] = P.lut[512 + i]; }
-	if (TABLE == 1) for (int i = threadIdx.x; i < 8 * 256; i += CB_THREADS) S.tab[i] = P.cbf[i];
-	if (TABLE == 2) for (int i = threadIdx.x; i < 8 * 16; i += CB_THREADS) S.tab[i] = P.tbook[i];
-	__syncthreads();
+	stage_tables<TABLE, true>(P, S, s_rc);
 	const int lane = threadIdx.x & 31;
-	const uint64_t nwarps = (uint64_t)gridDim.x * (CB_THREADS / 32);
-	const uint64_t gw = (uint64_t)blockIdx.x * (CB_THREADS / 32) + (threadIdx.x >> 5);
-	const uint64_t lo = total_tiles * gw / nwarps, hi = total_tiles * (gw + 1) / nwarps;
-	if (lo >= hi) return;
-
 	XKey low = xempty(), high = xempty();
-	uint32_t cur = (uint32_t)(lo / tiles_per_cand);
-	for (uint64_t tile = lo; tile < hi; tile++) {
-		const uint32_t c = (uint32_t)(tile / tiles_per_cand), j = (uint32_t)(tile - (uint64_t)c * tiles_per_cand);
-		if (c != cur) {
-			store_lists(X.seg + (gw + cur) * CX_WORDS, low, high, lane);
-			low = high = xempty();
-			cur = c;
-		}
-		const uint64_t t0 = (uint64_t)j * CB_TILE;
-		for (int g0 = 0; g0 < CB_GROUPS; g0 += L::U) {
-			typename L::Raw R[L::U];
-			bool in[L::U];
-#pragma unroll
-			for (int u = 0; u < L::U; u++) {
-				const uint64_t t = t0 + (uint64_t)(g0 + u) * 32 + lane;
-				in[u] = t < P.T;
-				if (in[u]) L::fetch(P, c, t, R[u]);
-			}
-#pragma unroll
-			for (int u = 0; u < L::U; u++) {
-				const uint64_t t = t0 + (uint64_t)(g0 + u) * 32 + lane;
-				if (t - lane >= P.T) break;                                 // warp-uniform: the rest of the tile is past the row end
-				XKey kl = xempty(), kh = xempty();
-				if (in[u]) {
-					CandEval E;
-					L::decode(P, S, R[u], E);
-					if (E.valid) {
-						const unsigned long long k = order_key(cand_final_reward<RECIP>(E, X.W, S.tw, s_rc));
-						kl = {k, P.idx_base + t};
-						kh = {~k, P.idx_base + t};
-					}
-				}
-				offer(low, kl, lane);
-				offer(high, kh, lane);
+
+	auto flush = [&](uint32_t c) {
+		store_lists(X.seg + (cand_warp() + c) * CX_WORDS, low, high, lane);
+		low = high = xempty();
+	};
+	auto each = [&](uint32_t, uint64_t t, bool in, const typename L::Raw &R, uint32_t) {
+		XKey kl = xempty(), kh = xempty();
+		if (in) {
+			CandEval E;
+			L::decode(P, S, R, E);
+			if (E.valid) {
+				const unsigned long long k = order_key(cand_final_reward<RECIP>(E, X.W, S.tw, s_rc));
+				kl = {k, P.idx_base + t};
+				kh = {~k, P.idx_base + t};
 			}
 		}
-	}
-	store_lists(X.seg + (gw + cur) * CX_WORDS, low, high, lane);
+		offer(low, kl, lane);
+		offer(high, kh, lane);
+	};
+	cand_walk<L, 0>(P, tiles_per_cand, total_tiles, each, flush);
 }
 
 // the warp of the pass whose tile range holds `tile`: the largest w with total * w / nwarps <= tile
@@ -653,59 +618,34 @@ k_cand_extremes_merge(unsigned long long *lists, const unsigned long long *seg, 
 	store_lists(lists + (uint64_t)c * CX_WORDS, low, high, lane);
 }
 
+// the walk, then the merge of its segments into the persistent lists
 template <class L, int TABLE, bool RECIP>
-static cudaError_t launch_ext(const CandExtParams &X, int sm_count, cudaStream_t st) {
-	const CandParams &P = X.src;
-	const uint32_t tiles_per_cand = (uint32_t)((P.T + CB_TILE - 1) / CB_TILE);
-	const uint64_t total_tiles = (uint64_t)tiles_per_cand * P.C;
-	if (total_tiles == 0) return cudaSuccess;
-	int per_sm = 0;
-	cudaError_t err = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_cand_extremes<L, TABLE, RECIP>, CB_THREADS, 0);
-	if (err != cudaSuccess) return err;
-	uint64_t grid = (uint64_t)sm_count * (uint64_t)(per_sm > 0 ? per_sm : 1);
-	const uint64_t need = (total_tiles + (CB_THREADS / 32) - 1) / (CB_THREADS / 32);
-	if (grid > need) grid = need;
-	if (cand_env_grid() && cand_env_grid() < grid) grid = cand_env_grid();
-	const uint64_t nwarps = grid * (CB_THREADS / 32);
+static cudaError_t launch_pass(const CandExtParams &X, int sm_count, cudaStream_t st) {
+	Walk w;
+	cudaError_t err = walk_grid(k_cand_extremes<L, TABLE, RECIP>, X.src, sm_count, w);
+	if (err != cudaSuccess || w.grid == 0) return err;
+	const uint64_t nwarps = w.grid * CB_WARPS;
 	if (nwarps > CX_MAX_WARPS_PER_SM * (uint64_t)sm_count) return cudaErrorInvalidConfiguration;   // more than the segment slots hold
-	k_cand_extremes<L, TABLE, RECIP><<<(unsigned)grid, CB_THREADS, 0, st>>>(X, tiles_per_cand, total_tiles);
+	k_cand_extremes<L, TABLE, RECIP><<<(unsigned)w.grid, CB_THREADS, 0, st>>>(X, w.tiles_per_cand, w.total_tiles);
 	if ((err = cudaGetLastError()) != cudaSuccess) return err;
-	k_cand_extremes_merge<<<(P.C + 7) / 8, 256, 0, st>>>(X.lists, X.seg, P.C, tiles_per_cand, total_tiles, nwarps);
+	k_cand_extremes_merge<<<(X.src.C + 7) / 8, 256, 0, st>>>(X.lists, X.seg, X.src.C, w.tiles_per_cand, w.total_tiles, nwarps);
 	return cudaGetLastError();
 }
 
-template <bool RECIP>
-static cudaError_t run_ext(const CandExtParams &X, int source, int sm_count, cudaStream_t st) {
-	switch (source) {
-	case CAND_DIMS: return launch_ext<LoadDims, 0, RECIP>(X, sm_count, st);
-	case CAND_REC32: return launch_ext<LoadRec<32>, 0, RECIP>(X, sm_count, st);
-	case CAND_REC16: return launch_ext<LoadRec<16>, 0, RECIP>(X, sm_count, st);
-	case CAND_Q: return launch_ext<LoadQ, 1, RECIP>(X, sm_count, st);
-	case CAND_T: return launch_ext<LoadT, 2, RECIP>(X, sm_count, st);
-	case CAND_W: return launch_ext<LoadW, 1, RECIP>(X, sm_count, st);
-	default: return cudaErrorInvalidValue;
-	}
-}
-
-cudaError_t run_cand_extremes(const CandExtParams &X, int source, bool recip, int sm_count, cudaStream_t st) {
-	return recip ? run_ext<true>(X, source, sm_count, st) : run_ext<false>(X, source, sm_count, st);
-}
-
 // ================================================================ per-candidate group scores (APO_SCORE_CANDIDATE_GROUPS)
-//   k_cand_groups<Loader, TABLE, RECIP>  one pass over the evaluations a scoring call reads, with the breakdown's loaders and
-//                                        tile walk: every group of 32 evaluations is split by the labels of its records
+//   k_cand_groups<Loader, TABLE, RECIP>  one pass over the evaluations a scoring call reads, on the shared loaders and
+//                                        walk: every group of 32 evaluations is split by the labels of its records
 //   k_cand_groups_report                 words -> apo_group_score[C][G] with the breakdown's report rules
 // A group of 32 evaluations is aggregated per label before it touches memory: the lanes that share a label (all 32 on the
 // fast path, __match_any_sync otherwise) reduce their terms with __reduce_add_sync, and the lowest of them adds the sums into
 // the warp's own shared accumulators of that label.  A term rint(fr * 2^52) enters as four 16-bit pieces of its two's
 // complement and a sign count, so 32 of them sum exactly in 32 bits whatever the labels are; the warp's accumulators hold a
 // run of CB_RUN_TILES tiles exactly (l0, l1 < 2^58, counts < 2^27) and are flushed into the (c, g) words when the candidate
-// changes and at the run limit, as k_cand_breakdown flushes.
-constexpr int GR_WARPS = CB_THREADS / 32;
+// changes and at the breakdown's run limit.
 struct GroupSmem {
-	unsigned long long l0[GR_WARPS][APO_GROUPS_MAX], l1[GR_WARPS][APO_GROUPS_MAX];   // 2^0 and 2^32 limbs of the sum
-	uint32_t n[GR_WARPS][APO_GROUPS_MAX], good[GR_WARPS][APO_GROUPS_MAX], bad[GR_WARPS][APO_GROUPS_MAX];
-	uint32_t rew[GR_WARPS][APO_GROUPS_MAX], neg[GR_WARPS][APO_GROUPS_MAX];           // non-null terms, negative terms
+	unsigned long long l0[CB_WARPS][APO_GROUPS_MAX], l1[CB_WARPS][APO_GROUPS_MAX];   // 2^0 and 2^32 limbs of the sum
+	uint32_t n[CB_WARPS][APO_GROUPS_MAX], good[CB_WARPS][APO_GROUPS_MAX], bad[CB_WARPS][APO_GROUPS_MAX];
+	uint32_t rew[CB_WARPS][APO_GROUPS_MAX], neg[CB_WARPS][APO_GROUPS_MAX];           // non-null terms, negative terms
 };
 // the fields of one evaluation (and, after __reduce_add_sync, of up to 32), 6 bits each
 constexpr int GP_N = 0, GP_GOOD = 6, GP_BAD = 12, GP_REW = 18, GP_NEG = 24;
@@ -713,26 +653,18 @@ constexpr int GP_N = 0, GP_GOOD = 6, GP_BAD = 12, GP_REW = 18, GP_NEG = 24;
 template <class L, int TABLE, bool RECIP>
 __global__ void __launch_bounds__(CB_THREADS, L::MIN_CTAS)
 k_cand_groups(const CandGroupParams X, uint32_t tiles_per_cand, uint64_t total_tiles) {
-	const CandParams &P = X.src;
+	const CandEvals &P = X.src;
 	__shared__ CandSmem S;
 	__shared__ double s_rc[512];                                        // reciprocal of the total weight (div_lut)
 	__shared__ GroupSmem A;
-	for (int i = threadIdx.x; i < 512; i += CB_THREADS) { S.tw[i] = P.lut[i]; s_rc[i] = P.lut[512 + i]; }
-	if (TABLE == 1) for (int i = threadIdx.x; i < 8 * 256; i += CB_THREADS) S.tab[i] = P.cbf[i];
-	if (TABLE == 2) for (int i = threadIdx.x; i < 8 * 16; i += CB_THREADS) S.tab[i] = P.tbook[i];
 	const int lane = threadIdx.x & 31, wp = threadIdx.x >> 5;
 	for (int g = lane; g < APO_GROUPS_MAX; g += 32) {
 		A.l0[wp][g] = A.l1[wp][g] = 0ull;
 		A.n[wp][g] = A.good[wp][g] = A.bad[wp][g] = A.rew[wp][g] = A.neg[wp][g] = 0u;
 	}
-	__syncthreads();
-	const uint64_t nwarps = (uint64_t)gridDim.x * GR_WARPS;
-	const uint64_t gw = (uint64_t)blockIdx.x * GR_WARPS + wp;
-	const uint64_t lo = total_tiles * gw / nwarps, hi = total_tiles * (gw + 1) / nwarps;
-	if (lo >= hi) return;
+	stage_tables<TABLE, true>(P, S, s_rc);
 	const uint8_t *labels = X.labels + P.idx_base;
 	const uint32_t G = X.G;
-	uint32_t run = 0;
 
 	auto flush = [&](uint32_t c) {
 		__syncwarp();
@@ -751,100 +683,43 @@ k_cand_groups(const CandGroupParams X, uint32_t tiles_per_cand, uint64_t total_t
 			A.n[wp][g] = A.good[wp][g] = A.bad[wp][g] = A.rew[wp][g] = A.neg[wp][g] = 0u;
 		}
 		__syncwarp();
-		run = 0;
 	};
-
-	uint32_t cur = (uint32_t)(lo / tiles_per_cand);
-	for (uint64_t tile = lo; tile < hi; tile++) {
-		const uint32_t c = (uint32_t)(tile / tiles_per_cand), j = (uint32_t)(tile - (uint64_t)c * tiles_per_cand);
-		if (c != cur || run == CB_RUN_TILES) { flush(cur); cur = c; }
-		run++;
-		const uint64_t t0 = (uint64_t)j * CB_TILE;
-		for (int g0 = 0; g0 < CB_GROUPS; g0 += L::U) {
-			typename L::Raw R[L::U];
-			bool in[L::U];
-			uint32_t lab[L::U];
-#pragma unroll
-			for (int u = 0; u < L::U; u++) {
-				const uint64_t t = t0 + (uint64_t)(g0 + u) * 32 + lane;
-				in[u] = t < P.T;
-				lab[u] = in[u] ? (uint32_t)__ldg(labels + t) : 0u;            // past the row end: label 0, nothing added
-				if (in[u]) L::fetch(P, c, t, R[u]);
-			}
-#pragma unroll
-			for (int u = 0; u < L::U; u++) {
-				if (t0 + (uint64_t)(g0 + u) * 32 >= P.T) break;                 // warp-uniform: the rest of the tile is past the row end
-				uint32_t pk = 0;
-				unsigned long long x = 0ull;
-				if (in[u]) {
-					CandEval E;
-					L::decode(P, S, R[u], E);
-					pk = (1u << GP_N) | ((E.fb == 1u ? 1u : 0u) << GP_GOOD) | ((E.fb == 2u ? 1u : 0u) << GP_BAD);
-					if (E.valid) {
-						const long long fx = to_fx(cand_final_reward<RECIP>(E, X.W, S.tw, s_rc));
-						x = (unsigned long long)fx;
-						pk |= (1u << GP_REW) | ((fx < 0 ? 1u : 0u) << GP_NEG);
-					}
-				}
-				const uint32_t l = lab[u];
-				const uint32_t peers = __all_sync(FULL, l == __shfl_sync(FULL, l, 0)) ? FULL : __match_any_sync(FULL, l);
-				uint32_t s0 = (uint32_t)x & 0xFFFFu, s1 = (uint32_t)(x >> 16) & 0xFFFFu, s2 = (uint32_t)(x >> 32) & 0xFFFFu;
-				uint32_t s3 = (uint32_t)(x >> 48), sp = pk;
-				if (peers != (1u << lane)) {                                    // a label of its own needs no reduction: the
-					s0 = __reduce_add_sync(peers, s0);                          // reductions run once per distinct peer mask
-					s1 = __reduce_add_sync(peers, s1);
-					s2 = __reduce_add_sync(peers, s2);
-					s3 = __reduce_add_sync(peers, s3);
-					sp = __reduce_add_sync(peers, sp);
-				}
-				if (lane == __ffs((int)peers) - 1) {                          // the lowest lane of the label: one writer per label
-					A.l0[wp][l] += (unsigned long long)s0 + ((unsigned long long)s1 << 16);
-					A.l1[wp][l] += (unsigned long long)s2 + ((unsigned long long)s3 << 16);
-					A.n[wp][l] += (sp >> GP_N) & 63u;
-					A.good[wp][l] += (sp >> GP_GOOD) & 63u;
-					A.bad[wp][l] += (sp >> GP_BAD) & 63u;
-					A.rew[wp][l] += (sp >> GP_REW) & 63u;
-					A.neg[wp][l] += (sp >> GP_NEG) & 63u;
-				}
-				__syncwarp();                                                   // the next group's writer of a label may be another lane
+	// l: the label, fetched with the evaluation (past the row end: label 0, nothing added)
+	auto each = [&](uint32_t, uint64_t, bool in, const typename L::Raw &R, uint32_t l) {
+		uint32_t pk = 0;
+		unsigned long long x = 0ull;
+		if (in) {
+			CandEval E;
+			L::decode(P, S, R, E);
+			pk = (1u << GP_N) | ((E.fb == 1u ? 1u : 0u) << GP_GOOD) | ((E.fb == 2u ? 1u : 0u) << GP_BAD);
+			if (E.valid) {
+				const long long fx = to_fx(cand_final_reward<RECIP>(E, X.W, S.tw, s_rc));
+				x = (unsigned long long)fx;
+				pk |= (1u << GP_REW) | ((fx < 0 ? 1u : 0u) << GP_NEG);
 			}
 		}
-	}
-	flush(cur);
-}
-
-template <class L, int TABLE, bool RECIP>
-static cudaError_t launch_grp(const CandGroupParams &X, int sm_count, cudaStream_t st) {
-	const CandParams &P = X.src;
-	const uint32_t tiles_per_cand = (uint32_t)((P.T + CB_TILE - 1) / CB_TILE);
-	const uint64_t total_tiles = (uint64_t)tiles_per_cand * P.C;
-	if (total_tiles == 0) return cudaSuccess;
-	int per_sm = 0;
-	cudaError_t err = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_cand_groups<L, TABLE, RECIP>, CB_THREADS, 0);
-	if (err != cudaSuccess) return err;
-	uint64_t grid = (uint64_t)sm_count * (uint64_t)(per_sm > 0 ? per_sm : 1);
-	const uint64_t need = (total_tiles + GR_WARPS - 1) / GR_WARPS;
-	if (grid > need) grid = need;
-	if (cand_env_grid() && cand_env_grid() < grid) grid = cand_env_grid();
-	k_cand_groups<L, TABLE, RECIP><<<(unsigned)grid, CB_THREADS, 0, st>>>(X, tiles_per_cand, total_tiles);
-	return cudaGetLastError();
-}
-
-template <bool RECIP>
-static cudaError_t run_grp(const CandGroupParams &X, int source, int sm_count, cudaStream_t st) {
-	switch (source) {
-	case CAND_DIMS: return launch_grp<LoadDims, 0, RECIP>(X, sm_count, st);
-	case CAND_REC32: return launch_grp<LoadRec<32>, 0, RECIP>(X, sm_count, st);
-	case CAND_REC16: return launch_grp<LoadRec<16>, 0, RECIP>(X, sm_count, st);
-	case CAND_Q: return launch_grp<LoadQ, 1, RECIP>(X, sm_count, st);
-	case CAND_T: return launch_grp<LoadT, 2, RECIP>(X, sm_count, st);
-	case CAND_W: return launch_grp<LoadW, 1, RECIP>(X, sm_count, st);
-	default: return cudaErrorInvalidValue;
-	}
-}
-
-cudaError_t run_cand_groups(const CandGroupParams &X, int source, bool recip, int sm_count, cudaStream_t st) {
-	return recip ? run_grp<true>(X, source, sm_count, st) : run_grp<false>(X, source, sm_count, st);
+		const uint32_t peers = __all_sync(FULL, l == __shfl_sync(FULL, l, 0)) ? FULL : __match_any_sync(FULL, l);
+		uint32_t s0 = (uint32_t)x & 0xFFFFu, s1 = (uint32_t)(x >> 16) & 0xFFFFu, s2 = (uint32_t)(x >> 32) & 0xFFFFu;
+		uint32_t s3 = (uint32_t)(x >> 48), sp = pk;
+		if (peers != (1u << lane)) {                                    // a label of its own needs no reduction: the
+			s0 = __reduce_add_sync(peers, s0);                          // reductions run once per distinct peer mask
+			s1 = __reduce_add_sync(peers, s1);
+			s2 = __reduce_add_sync(peers, s2);
+			s3 = __reduce_add_sync(peers, s3);
+			sp = __reduce_add_sync(peers, sp);
+		}
+		if (lane == __ffs((int)peers) - 1) {                          // the lowest lane of the label: one writer per label
+			A.l0[wp][l] += (unsigned long long)s0 + ((unsigned long long)s1 << 16);
+			A.l1[wp][l] += (unsigned long long)s2 + ((unsigned long long)s3 << 16);
+			A.n[wp][l] += (sp >> GP_N) & 63u;
+			A.good[wp][l] += (sp >> GP_GOOD) & 63u;
+			A.bad[wp][l] += (sp >> GP_BAD) & 63u;
+			A.rew[wp][l] += (sp >> GP_REW) & 63u;
+			A.neg[wp][l] += (sp >> GP_NEG) & 63u;
+		}
+		__syncwarp();                                                   // the next group's writer of a label may be another lane
+	};
+	cand_walk<L, CB_RUN_TILES>(P, tiles_per_cand, total_tiles, each, flush, [&](uint64_t t) { return (uint32_t)__ldg(labels + t); });
 }
 
 // one thread per (c, g)
@@ -872,6 +747,40 @@ cudaError_t run_cand_groups_report(const long long *words, uint32_t C, uint32_t 
 	if (n == 0) return cudaSuccess;
 	k_cand_groups_report<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(words, n, out);
 	return cudaGetLastError();
+}
+
+// ================================================================ one dispatch for the passes that read every source
+template <class L, int TABLE, bool>
+static cudaError_t launch_pass(const CandParams &P, int sm_count, cudaStream_t st) {
+	return launch_walk(k_cand_breakdown<L, TABLE>, P, sm_count, st);
+}
+template <class L, int TABLE, bool RECIP>
+static cudaError_t launch_pass(const CandGroupParams &X, int sm_count, cudaStream_t st) {
+	return launch_walk(k_cand_groups<L, TABLE, RECIP>, X, sm_count, st);
+}
+
+// the loader of each source and the table it stages; RECIP: the division of the passes that divide (div_lut)
+template <bool RECIP, class X>
+static cudaError_t by_source(const X &x, int source, int sm_count, cudaStream_t st) {
+	switch (source) {
+	case CAND_DIMS: return launch_pass<LoadDims, 0, RECIP>(x, sm_count, st);
+	case CAND_REC32: return launch_pass<LoadRec<32>, 0, RECIP>(x, sm_count, st);
+	case CAND_REC16: return launch_pass<LoadRec<16>, 0, RECIP>(x, sm_count, st);
+	case CAND_Q: return launch_pass<LoadQ, 1, RECIP>(x, sm_count, st);
+	case CAND_T: return launch_pass<LoadT, 2, RECIP>(x, sm_count, st);
+	case CAND_W: return launch_pass<LoadW, 1, RECIP>(x, sm_count, st);
+	default: return cudaErrorInvalidValue;
+	}
+}
+
+cudaError_t run_cand_breakdown(const CandParams &P, int source, int sm_count, cudaStream_t st) {
+	return by_source<false>(P, source, sm_count, st);                  // the breakdown sums the dimensions: no division
+}
+cudaError_t run_cand_extremes(const CandExtParams &X, int source, bool recip, int sm_count, cudaStream_t st) {
+	return recip ? by_source<true>(X, source, sm_count, st) : by_source<false>(X, source, sm_count, st);
+}
+cudaError_t run_cand_groups(const CandGroupParams &X, int source, bool recip, int sm_count, cudaStream_t st) {
+	return recip ? by_source<true>(X, source, sm_count, st) : by_source<false>(X, source, sm_count, st);
 }
 
 }  // namespace apo

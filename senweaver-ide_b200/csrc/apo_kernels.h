@@ -330,7 +330,8 @@ constexpr int CB_DIM = 0;        // 9 x (l0, l1, l2, count): exact sum of rint(v
 constexpr int CB_TALLY = 36;     // total, good, bad
 constexpr int CB_INT = 39;
 enum CandSource { CAND_DIMS = 0, CAND_REC32 = 1, CAND_REC16 = 2, CAND_Q = 3, CAND_T = 4, CAND_W = 5 };
-struct CandParams {
+// The evaluations every per-candidate pass reads: those of one scoring launch (its window, candidate offset and record positions)
+struct CandEvals {
 	uint32_t C;
 	uint64_t T;                     // evaluations per candidate in this launch
 	uint64_t idx_base;              // record position of evaluation 0 of this launch (window start / streamed chunk start)
@@ -339,6 +340,7 @@ struct CandParams {
 	const unsigned long long *q8;   // Form Q planes
 	const float *d2;
 	const unsigned short *li;
+	const unsigned long long *qw;   // Form W words (KqParams::qw)
 	const float *cbf;               // Form Q / W: [8][256] code -> fp32 value
 	const unsigned short *tl;       // Form T planes + dictionary
 	const unsigned char *th;
@@ -347,10 +349,12 @@ struct CandParams {
 	uint32_t n_tuples;
 	const float *tbook;             // Form T: [8][16] 4-bit code -> fp32 value
 	const float *d2book;            // Form T: [4096] tool_success_rate values
-	const double *lut;              // natural-mask LUT [512] total weight (<= 0: finalReward null)
+	const double *lut;              // as K1Params::lut: [512] total weight (<= 0: finalReward null) | reciprocal | categorical products
+};
+struct CandParams {
+	CandEvals src;
 	long long *ints;                // [C][CB_INT] of candidate 0 of this launch
 	unsigned long long *ex;         // [C][3] of candidate 0 of this launch
-	const unsigned long long *qw;   // Form W words (KqParams::qw)
 	unsigned int *dom;              // set to 1 when a counted evaluation has a present dimension with |v| >= 2048 (or NaN)
 };
 cudaError_t run_cand_breakdown(const CandParams &P, int source, int sm_count, cudaStream_t st);
@@ -364,12 +368,7 @@ cudaError_t run_cand_report(const long long *ints, const unsigned long long *ex,
 // indices (ex_insert keys, 0 = empty), followed by [C][CC_WORDS] scratch where the report kernel converts them to index + 1.
 constexpr int CC_WORDS = 68 + 18;   // CORP_FIXED + one rank's 18 example slots
 struct CandCorpusParams {
-	uint32_t C;
-	uint64_t T;                     // records per candidate in this launch
-	uint64_t idx_base;              // record position of record 0 of this launch (window start / streamed chunk start)
-	uint64_t pitch_evals;           // candidate row pitch in records
-	const uint8_t *rows;            // Form R (32 B) / R16 (16 B): record 0 of candidate 0
-	const double *lut;              // as K1Params::lut (total weight | reciprocal | categorical product table)
+	CandEvals src;                  // Form R (32 B) / R16 (16 B) rows
 	double w2;
 	long long *blk;                 // [C][CC_WORDS] of candidate 0 of this launch
 };
@@ -386,7 +385,7 @@ constexpr int CX_WORDS = 2 * 32 * 2;
 constexpr uint64_t CX_MAX_WARPS_PER_SM = 2048 / 32;   // the pass's grid never holds more warps than the SMs can host
 inline uint64_t cand_ext_slots(int sm_count, uint32_t C) { return CX_MAX_WARPS_PER_SM * (uint64_t)sm_count + C; }
 struct CandExtParams {
-	CandParams src;                 // the evaluations, as the breakdown reads them (ints / ex / dom unused)
+	CandEvals src;
 	Weights W;
 	unsigned long long *lists;      // [C][CX_WORDS] of candidate 0 of this launch
 	unsigned long long *seg;        // segment slots of this launch
@@ -399,7 +398,7 @@ cudaError_t run_cand_extremes(const CandExtParams &P, int source, bool recip, in
 constexpr int GR_WORDS = 8;
 constexpr int GR_TALLY = 4;
 struct CandGroupParams {
-	CandParams src;                 // the evaluations, as the breakdown reads them (ints / ex / dom unused)
+	CandEvals src;
 	Weights W;
 	const uint8_t *labels;          // [labels T] group of every record position (src.idx_base + t)
 	uint32_t G;                     // 1..APO_GROUPS_MAX
