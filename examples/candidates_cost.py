@@ -22,6 +22,11 @@ The labels are uploaded before each such step, outside its timing.  On the fp32 
 of two of the 8 candidates against the model of tests/group_fixtures.py over the generated rows (every field bit for bit);
 on the rollout legs the non-null counts of every candidate's groups add up to counts[c], and R16 and R give the same bytes.
 
+Every leg also times the step with the per-candidate reward spread (APO_SCORE_CANDIDATE_SPREAD) in the same alternation.  Its
+parity block holds n and S1 of every candidate against apo_debug_partials (and mean against scores[c]); on the fp32 legs also
+the spreads of two of the 8 candidates against the exact model of tests/spread_fixtures.py over the generated rows (every
+field bit for bit), and on the rollout legs R16 and R give the same bytes.
+
     python examples/candidates_cost.py [--steps 10] [--legs D,W,Q,T,R16,R,FALL] [--out FILE.json]
 
 Prints one JSON object; the card name and power limit are read in the same run (nvidia-smi query)."""
@@ -114,6 +119,36 @@ def groups_parity(last, sets, ref_grp):
     return out
 
 
+def spread_row(s):
+    return (int(s.n), s.sum, s.sum_sq, bits(s.mean), bits(s.rewardSumSq), bits(s.variance), bits(s.stdDev), bits(s.stdErr))
+
+
+def model_spread(m):
+    return (m["n"], m["S1"], m["S2"], bits(m["mean"]), bits(m["rewardSumSq"]), bits(m["variance"]), bits(m["stdDev"]), bits(m["stdErr"]))
+
+
+def spread_parity(eng, res, ref_spr):
+    """n / S1 of every candidate against the scoring call's partials (every step of a leg sums the same integers), mean against
+    scores[c]; ref_spr: {candidate: model spread}"""
+    sums, counts = eng.debug_partials(len(res.spread))
+    every = all((s.sum, int(s.n)) == (sums[c], counts[c]) and (s.n == 0 or bits(s.mean) == bits(res.scores[c]))
+                for c, s in enumerate(res.spread))
+    out = {"n_s1_every_candidate": every}
+    if ref_spr:
+        ok = {c: spread_row(res.spread[c]) == model_spread(m) for c, m in ref_spr.items()}
+        out.update({"candidates": list(ok), "per_candidate": ok})
+        every = every and all(ok.values())
+    out["equal"] = every
+    return out
+
+
+def spread_block(eng, last, med, ref_spr):
+    return {"spread_ms_median": round(med["spread"], 3), "spread_ratio": round(med["spread"] / med["plain"], 3),
+            "spread_same_scores": last["spread"].scores.tobytes() == last["plain"].scores.tobytes()
+                                  and last["spread"].topk.tobytes() == last["plain"].topk.tobytes(),
+            "parity_spread": spread_parity(eng, last["spread"], ref_spr)}
+
+
 def timed(eng, C, K, steps, score_kw, kinds, sets):
     """median / min of every kind of step, alternating; a group step first uploads its labels (outside the timing)"""
     times = {k: [] for k in kinds}
@@ -143,10 +178,10 @@ def groups_block(last, med, sets, ref_grp):
             "parity_groups": groups_parity(last, sets, ref_grp)}
 
 
-def leg(eng, C, K, steps, score_kw, ref, picks, ref_ext=None, sets=None, ref_grp=None):
-    """plain / candidates / extremes / groups steps, alternating (ref None: the breakdown is not timed)"""
+def leg(eng, C, K, steps, score_kw, ref, picks, ref_ext=None, sets=None, ref_grp=None, ref_spr=None):
+    """plain / candidates / extremes / groups / spread steps, alternating (ref None: the breakdown is not timed)"""
     sets = sets or {}
-    kinds = {"plain": {}, "extremes": {"extremes": True}}
+    kinds = {"plain": {}, "extremes": {"extremes": True}, "spread": {"spread": True}}
     if ref is not None:
         kinds["candidates"] = {"candidates": True}
     kinds.update({k: {"groups": True} for k in sets})
@@ -158,6 +193,7 @@ def leg(eng, C, K, steps, score_kw, ref, picks, ref_ext=None, sets=None, ref_grp
                           and last["extremes"].topk.tobytes() == last["plain"].topk.tobytes(),
            "parity_extremes": extremes_parity(last["extremes"], ref_ext)}
     out.update(groups_block(last, med, sets, ref_grp))
+    out.update(spread_block(eng, last, med, ref_spr))
     if ref is not None:
         r = last["candidates"]
         ok = [same(r.candidates[c], d) for c, d in zip(picks, ref)]
@@ -206,8 +242,9 @@ def parity_block(picks, diffs):
 
 
 def corpus_leg(eng, C, K, steps, score_kw, ref, picks, ref_corpus, sets):
-    """plain / candidates / candidate_corpus / extremes / groups steps, alternating, with the parity blocks"""
-    kinds = {"plain": {}, "candidates": {"candidates": True}, "candidate_corpus": {"candidate_corpus": True}, "extremes": {"extremes": True}}
+    """plain / candidates / candidate_corpus / extremes / groups / spread steps, alternating, with the parity blocks"""
+    kinds = {"plain": {}, "candidates": {"candidates": True}, "candidate_corpus": {"candidate_corpus": True}, "extremes": {"extremes": True},
+             "spread": {"spread": True}}
     kinds.update({k: {"groups": True} for k in sets})
     last, times, med = timed(eng, C, K, steps, score_kw, kinds, sets)
     ok = [same(last["candidates"].candidates[c], d) for c, d in zip(picks, ref)]
@@ -216,6 +253,7 @@ def corpus_leg(eng, C, K, steps, score_kw, ref, picks, ref_corpus, sets):
     exact = [[list(x) for x in xr.diff_exact(cc[c], d)] for c, d in zip(picks, ref_corpus["exact"])]
     seq = [seq_corpus_diff(cc[c], d) for c, d in zip(picks, ref_corpus["seq"])]
     return {**groups_block(last, med, sets, None), "groups_bytes": b"".join(bytes(last[k].groups) for k in sets),
+            **spread_block(eng, last, med, None), "spread_bytes": bytes(last["spread"].spread),
             "plain_ms_median": round(med["plain"], 3), "candidates_ms_median": round(med["candidates"], 3),
             "candidate_corpus_ms_median": round(med["candidate_corpus"], 3),
             "candidates_ratio": round(med["candidates"] / med["plain"], 3),
@@ -242,6 +280,7 @@ def main():
     import exact_report as xr
     import extremes_fixtures as xf
     import group_fixtures as gf
+    import spread_fixtures as sf
     legs = args.legs.split(",")
     out = {"card": card(), "steps": args.steps, "timing": "host clock around each synchronous apo_score call"}
     eng = pkg.Engine(0)
@@ -252,24 +291,25 @@ def main():
         if {"D", "W", "Q", "T"} & set(legs):
             ref = oc.cand_generated(seed, picks, 0, T, 300, nthreads=nth)
             sets = label_sets(T)
-            ref_ext, ref_grp = {}, {}
+            ref_ext, ref_grp, ref_spr = {}, {}, {}
             for c in (picks[0], picks[-1]):
                 d = oracle.gen_dims(seed, c, 1, 0, T, 300, nth)
                 ref_ext[c] = xf.model(d)[0]
                 ref_grp[c] = {k: gf.model(d, lab, G)[0] for k, (lab, G) in sets.items()}
+                ref_spr[c] = sf.model(d)[0]
                 del d
             if "D" in legs:
                 eng.dims_generate(seed, 0, C, 0, T, 300)
-                out["form_d_256x5M"] = leg(eng, C, K, args.steps, {}, ref, picks, ref_ext, sets, ref_grp)
+                out["form_d_256x5M"] = leg(eng, C, K, args.steps, {}, ref, picks, ref_ext, sets, ref_grp, ref_spr)
             if "W" in legs:
                 eng.dims_generate(seed, 0, C, 0, T, 300)
                 eng.set_tuning(pkg.TUNE_NO_TWIN_T)
-                out["form_w_copy_256x5M"] = leg(eng, C, K, args.steps, {}, ref, picks, ref_ext, sets, ref_grp)
+                out["form_w_copy_256x5M"] = leg(eng, C, K, args.steps, {}, ref, picks, ref_ext, sets, ref_grp, ref_spr)
                 eng.set_tuning(0)
             if "Q" in legs or "T" in legs:
                 eng.dims_generate_compact(seed, 0, C, 0, T, 300)
             if "Q" in legs:
-                out["form_q_256x5M"] = leg(eng, C, K, args.steps, {}, ref, picks, ref_ext, sets, ref_grp)
+                out["form_q_256x5M"] = leg(eng, C, K, args.steps, {}, ref, picks, ref_ext, sets, ref_grp, ref_spr)
             if "T" in legs:
                 pc, pd = np.empty((C, T), np.uint32), np.empty((C, T), np.uint16)
                 for c in range(C):
@@ -279,7 +319,7 @@ def main():
                 del pc, pd
                 eng.tuples_upload(tl, th, tbook, book, d2book)
                 del tl, th
-                out["form_t_256x5M"] = leg(eng, C, K, args.steps, {"source": pkg.SRC_TUPLES}, ref, picks, ref_ext, sets, ref_grp)
+                out["form_t_256x5M"] = leg(eng, C, K, args.steps, {"source": pkg.SRC_TUPLES}, ref, picks, ref_ext, sets, ref_grp, ref_spr)
         if {"R16", "R"} & set(legs):
             Cr = 128
             picks_r = [int(x) for x in np.linspace(0, Cr - 1, 8).round()]
@@ -296,9 +336,11 @@ def main():
             if "R16" in legs and "R" in legs:                   # the same rollouts: the same lists
                 out["r16_r_extremes_equal"] = out["form_r16_128x5M"]["extremes_bytes"] == out["form_r_128x5M"]["extremes_bytes"]
                 out["r16_r_groups_equal"] = out["form_r16_128x5M"]["groups_bytes"] == out["form_r_128x5M"]["groups_bytes"]
+                out["r16_r_spread_equal"] = out["form_r16_128x5M"]["spread_bytes"] == out["form_r_128x5M"]["spread_bytes"]
             for k in ("form_r16_128x5M", "form_r_128x5M"):
                 out.get(k, {}).pop("extremes_bytes", None)
                 out.get(k, {}).pop("groups_bytes", None)
+                out.get(k, {}).pop("spread_bytes", None)
         if "FALL" in legs:
             Cf, Tf = 64, 1_000_000
             d = xf.falling(Tf, 1)
@@ -307,7 +349,8 @@ def main():
             mg = {k: gf.model(d, lab, G)[0] for k, (lab, G) in sets_f.items()}
             eng.dims_upload(np.repeat(d, Cf, axis=0))
             eng.set_tuning(pkg.TUNE_NO_TWIN)
-            out["falling_rows_k1_64x1M"] = leg(eng, Cf, K, args.steps, {}, None, None, {0: m, Cf - 1: m}, sets_f, {0: mg, Cf - 1: mg})
+            out["falling_rows_k1_64x1M"] = leg(eng, Cf, K, args.steps, {}, None, None, {0: m, Cf - 1: m}, sets_f, {0: mg, Cf - 1: mg},
+                                               {0: sf.model(d)[0], Cf - 1: sf.model(d)[0]})
             eng.set_tuning(0)
     finally:
         eng.close()

@@ -273,6 +273,7 @@ int apo_record_unpack16(const apo_record16 *in, uint64_t n, apo_record *out);
 #define APO_SCORE_CANDIDATE_CORPUS 0x10u /* also build the corpus report of every candidate's rollout records (apo_candidate_corpus_reports) */
 #define APO_SCORE_CANDIDATE_EXTREMES 0x20u /* also list the 32 lowest- and highest-reward evaluations of every candidate (apo_candidate_extremes) */
 #define APO_SCORE_CANDIDATE_GROUPS 0x40u /* also split every candidate's evaluations by record group (apo_candidate_groups) */
+#define APO_SCORE_CANDIDATE_SPREAD 0x80u /* also build every candidate's reward spread (apo_candidate_spread) */
 typedef struct apo_score_opts {
 	uint32_t K;          /* beam width (top-K), 0..min(C, 16384) */
 	uint32_t source;     /* APO_SRC_* */
@@ -507,6 +508,31 @@ typedef struct apo_group_score {
 /* out = [n][G] for candidates [c0, c0 + n) of the last scoring call; G must be the G that call scored with (APO_E_ARG
  * otherwise).  APO_E_STATE when that call did not set the flag (or failed), APO_E_ARG when the range exceeds its C. */
 int apo_candidate_groups(apo_engine *e, uint32_t c0, uint32_t n, uint32_t G, apo_group_score *out);
+/* Per-candidate reward spread: how far apart candidate c's rewards lie, so that a caller can tell whether the gap between two
+ * candidates' means is larger than the noise of the rollouts they were scored on.  Built by a scoring call that sets
+ * APO_SCORE_CANDIDATE_SPREAD; it works wherever APO_SCORE_CANDIDATE_EXTREMES works (apo_score on every source and route,
+ * apo_score_finish when every apo_score_accumulate of the session set it too, every apo_score_host*), combines with the other
+ * per-candidate flags in any mix, and leaves scores, counts, top-K and the other outputs as they are without it.
+ * Over the evaluations the call summed into scores[c], with x_t = rint(fr_t * 2^52) the int64 term it added (fr_t bit for bit
+ * the finalReward it summed, APO_SCORE_RECIP honoured):
+ *   n = counts[c],  S1 = sum x_t (the partial of apo_debug_partials),  S2 = sum x_t^2 (exact, < 2^192),
+ *   M = n * S2 - S1^2 (exact, 0 <= M < 2^256); RN = round to nearest even, (double)n = RN(n):
+ *   mean        = scores[c] bit for bit; NaN when n == 0
+ *   rewardSumSq = RN(S2) * 2^-104
+ *   variance    = RN(RN(RN(M) * 2^-104 / (double)n) / (double)(n - 1)) for n >= 2, NaN below; +0.0 when M == 0
+ *   stdDev      = sqrt_rn(variance)
+ *   stdErr      = sqrt_rn(RN(variance / (double)n))
+ * The exact integers let a caller pool calls or shards on the host without losing exactness.  Single rank only, as the
+ * breakdown (APO_E_STATE on a handle with more than one rank).  Spreads of candidates [c0, c0 + n) of the last scoring call:
+ * APO_E_STATE when that call did not set the flag (or failed), APO_E_ARG when the range exceeds its C. */
+struct apo_candidate_spread {
+	uint64_t n;           /* == counts[c] */
+	uint64_t sumLo;       /* S1 as a two's complement 128-bit integer: low word */
+	int64_t  sumHi;       /*                                           high word */
+	uint64_t sumSq[3];    /* S2, unsigned 192-bit, least significant word first */
+	double   mean, rewardSumSq, variance, stdDev, stdErr;
+};                        /* 88 bytes */
+int apo_candidate_spread(apo_engine *e, uint32_t c0, uint32_t n, struct apo_candidate_spread *out);
 
 /* ---- multi-GPU: the record axis is sharded across ranks (one process per GPU, or one handle per GPU inside one
  * process); the packed int64 partial vectors of the shards are joined INSIDE the scoring launch: the finalising CTA

@@ -227,7 +227,10 @@ class APOService:
         rollouts up by index.  When the result carries the per-candidate group scores (evaluateBeam(..., groups=(labels, names))),
         the report adds byGroup: {name: {totalRollouts, goodFeedbackCount, badFeedbackCount, goodRate, avgReward}} over the
         candidate's rollouts in each record group (avgReward None when none of them has a reward); names default to those of the
-        last evaluateBeam.  Pure: it neither records the suggestions nor fires events nor touches storage."""
+        last evaluateBeam.  When the result carries the per-candidate reward spread (evaluateBeam(..., spread=True)), the report
+        adds rewardStdDev (the sample standard deviation of its rollouts' rewards) and scoreStdErr (the standard error of
+        avgReward), both None with fewer than two rewarded rollouts: the scale against which a gap between two candidates'
+        scores can be read.  Pure: it neither records the suggestions nor fires events nor touches storage."""
         cc = res.candidate_corpus[c] if getattr(res, "candidate_corpus", None) is not None else None
         r = res.candidates[c] if res.candidates is not None else cc
         goodRate = float(r.goodRate)
@@ -257,6 +260,10 @@ class APOService:
             out["byGroup"] = {names[g]: {"totalRollouts": int(x.total), "goodFeedbackCount": int(x.good), "badFeedbackCount": int(x.bad),
                                          "goodRate": float(x.goodRate), "avgReward": None if x.withReward == 0 else float(x.avgReward)}
                               for g, x in enumerate(gs)}
+        sp = res.spread[c] if getattr(res, "spread", None) is not None else None
+        if sp is not None:
+            out["rewardStdDev"] = None if sp.n < 2 else float(sp.stdDev)
+            out["scoreStdErr"] = None if sp.n < 2 else float(sp.stdErr)
         return out
 
     @staticmethod
@@ -319,7 +326,8 @@ class APOService:
         return out
 
     # ---- beam evaluation: the step the reference delegates to its backend --------------------------------
-    def evaluateBeam(self, candidates, dims=None, rollouts=None, reports=False, patterns=False, extremes=False, groups=None):
+    def evaluateBeam(self, candidates, dims=None, rollouts=None, reports=False, patterns=False, extremes=False, groups=None,
+                     spread=False):
         """Score a beam of VersionedPromptTemplate candidates on their rollout outcomes and keep the
         top `beamWidth` (score desc, ties -> lower index), then apply the APO:1138-1166 update with the
         strict `>` adoption rule (APO:1159).  dims: float32 [C][T][9] (NaN = absent) or rollouts:
@@ -327,7 +335,9 @@ class APOService:
         candidateReport); with rollouts, reports=True and patterns=True also build every candidate's corpus
         report (res.candidate_corpus: problem patterns, per-mode tallies, tool totals).  extremes=True also lists every
         candidate's 32 lowest- and highest-reward rollouts (res.extremes).  groups=(labels, names) also splits every candidate's
-        rollouts by record group (res.groups [C][G]): labels[t] < len(names) is the group of rollout index t."""
+        rollouts by record group (res.groups [C][G]): labels[t] < len(names) is the group of rollout index t.  spread=True also
+        builds every candidate's reward spread (res.spread: exact sums, variance, standard deviation and standard error).  The
+        adoption rule stays the strict `>` on the means."""
         try:
             C = len(candidates)
             K = min(self._config["beamWidth"], C)
@@ -341,6 +351,8 @@ class APOService:
                 self._engine.record_groups_upload(labels, len(names))
                 self._groupNames = names
                 extra["groups"] = True
+            if spread:
+                extra["spread"] = True
             if dims is not None:
                 self._engine.dims_upload(np.ascontiguousarray(dims, np.float32))
                 res = self._engine.score(C, K, source=SRC_DIMS, **extra)
@@ -361,7 +373,7 @@ class APOService:
             return None
 
     def runBeamSearch(self, seedPrompt, proposeCandidates, rolloutDims=None, rounds=None, withReports=False, rolloutRecords=None,
-                      withExtremes=False, rolloutGroups=None):
+                      withExtremes=False, rolloutGroups=None, withSpread=False):
         """Client-side round driver (SURVEY 8f rank 3) around the GPU top-K: each round expands every beam
         member into `branchFactor` children through the caller's `proposeCandidates(parent, n) -> [content]`
         hook (the LLM critique/edit step of APO:918-988 lives there), scores parents + children on
@@ -372,12 +384,15 @@ class APOService:
         rolloutRecords that report also carries the parent's problem patterns, byMode and toolStats; withExtremes=True
         (which needs withReports=True) adds the parent's lowestRollouts / highestRollouts, indices into the rollouts the
         caller scored it on; rolloutGroups=(labels, names) (which needs withReports=True too) adds the parent's byGroup, so that
-        a label that marks a held-out part of the rollouts shows whether a child improved only where its critique looked.
-        Returns the final beam state."""
+        a label that marks a held-out part of the rollouts shows whether a child improved only where its critique looked;
+        withSpread=True (which needs withReports=True too) adds the parent's rewardStdDev / scoreStdErr, so that the critique
+        can tell a lead from the noise of the rollouts.  Returns the final beam state."""
         if (rolloutDims is None) == (rolloutRecords is None):
             raise ValueError("runBeamSearch needs exactly one of rolloutDims / rolloutRecords")
         if withExtremes and not withReports:
             raise ValueError("runBeamSearch: withExtremes needs withReports=True (the lists travel in the candidate reports)")
+        if withSpread and not withReports:
+            raise ValueError("runBeamSearch: withSpread needs withReports=True (the spreads travel in the candidate reports)")
         if rolloutGroups is not None:
             if not withReports:
                 raise ValueError("runBeamSearch: rolloutGroups needs withReports=True (the group scores travel in the candidate reports)")
@@ -397,9 +412,10 @@ class APOService:
                                   "parentVersion": parent["version"], "createdAt": time.time() * 1000.0})
             if rolloutRecords is not None:
                 res = self.evaluateBeam(cands, rollouts=rolloutRecords(cands), reports=withReports, patterns=withReports,
-                                        extremes=withExtremes, groups=rolloutGroups)
+                                        extremes=withExtremes, groups=rolloutGroups, spread=withSpread)
             else:
-                res = self.evaluateBeam(cands, dims=rolloutDims(cands), reports=withReports, extremes=withExtremes, groups=rolloutGroups)
+                res = self.evaluateBeam(cands, dims=rolloutDims(cands), reports=withReports, extremes=withExtremes, groups=rolloutGroups,
+                                        spread=withSpread)
             if res is None:
                 break
             if withReports:

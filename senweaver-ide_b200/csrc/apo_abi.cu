@@ -159,12 +159,13 @@ const struct { const char *env; uint32_t bit; } kTuning[] = {
 
 // The per-candidate passes a scoring call can flag (csrc/apo_cand.cu), with the words of their messages.  tbook: the pass
 // reads every source, Form T through the 4-bit table (apo_engine::tbook).
-enum Pass { PASS_CAND, PASS_CCORP, PASS_EXT, PASS_GRP, NPASS };
+enum Pass { PASS_CAND, PASS_CCORP, PASS_EXT, PASS_GRP, PASS_SPREAD, NPASS };
 const struct { uint32_t flag; const char *name, *joined, *every; bool tbook; } kPass[NPASS] = {
 	{APO_SCORE_CANDIDATES, "APO_SCORE_CANDIDATES", "the per-candidate breakdown is", "a breakdown", true},
 	{APO_SCORE_CANDIDATE_CORPUS, "APO_SCORE_CANDIDATE_CORPUS", "the per-candidate corpus reports are", "the reports", false},
 	{APO_SCORE_CANDIDATE_EXTREMES, "APO_SCORE_CANDIDATE_EXTREMES", "the per-candidate lists are", "the lists", true},
-	{APO_SCORE_CANDIDATE_GROUPS, "APO_SCORE_CANDIDATE_GROUPS", "the per-candidate group scores are", "the group scores", true}};
+	{APO_SCORE_CANDIDATE_GROUPS, "APO_SCORE_CANDIDATE_GROUPS", "the per-candidate group scores are", "the group scores", true},
+	{APO_SCORE_CANDIDATE_SPREAD, "APO_SCORE_CANDIDATE_SPREAD", "the per-candidate spreads are", "the spreads", true}};
 
 // one pass's state through a call or session
 struct PassState {
@@ -250,6 +251,8 @@ struct apo_engine {
 	DevBuf<long long> grp_acc;               // [C][G][GR_WORDS] words of the call or session
 	DevBuf<apo_group_score> grp_rep;         // [C][G] scores of the last flagged call
 	uint32_t grp_rep_G = 0, grp_arm_G = 0; uint64_t grp_arm_gen = 0;
+	DevBuf<unsigned long long> spread_acc;   // spread: [C][SP_WORDS] sums of squares of the call or session
+	DevBuf<struct apo_candidate_spread> spread_rep; // spreads of the last flagged call
 };
 
 namespace {
@@ -789,7 +792,7 @@ int launch_score(apo_engine *e, const apo_score_opts *o, const Evals &ev, uint32
 	return APO_OK;
 }
 
-// ---- the per-candidate passes (APO_SCORE_CANDIDATES, _CANDIDATE_CORPUS, _CANDIDATE_EXTREMES, _CANDIDATE_GROUPS)
+// ---- the per-candidate passes (APO_SCORE_CANDIDATES, _CANDIDATE_CORPUS, _CANDIDATE_EXTREMES, _CANDIDATE_GROUPS, _CANDIDATE_SPREAD)
 bool wants(const apo_score_opts *o, int p) { return (o->flags & kPass[p].flag) != 0; }
 
 // a failed call or finish leaves no reports behind
@@ -835,6 +838,7 @@ int pass_reserve(apo_engine *e, int p, uint32_t C) {
 	case PASS_CCORP: CK(reserve(e, e->ccorp_acc, 2ull * C * apo::CC_WORDS)); break;   // blocks | report scratch
 	case PASS_EXT: CK(reserve(e, e->ext_acc, ((uint64_t)C + apo::cand_ext_slots(e->sm_count, C)) * apo::CX_WORDS)); break;
 	case PASS_GRP: CK(reserve(e, e->grp_acc, (uint64_t)(C ? C : 1) * e->grp_G * apo::GR_WORDS)); break;
+	case PASS_SPREAD: CK(reserve(e, e->spread_acc, (uint64_t)(C ? C : 1) * apo::SP_WORDS)); break;
 	}
 	if (kPass[p].tbook) CK(reserve(e, e->tbook, 8 * 16));
 	return APO_OK;
@@ -851,6 +855,7 @@ int pass_arm(apo_engine *e, int p, uint32_t C) {
 		CK(cudaMemsetAsync(e->grp_acc.p, 0, (uint64_t)C * e->grp_G * apo::GR_WORDS * 8, e->stream));
 		e->grp_arm_G = e->grp_G; e->grp_arm_gen = e->grp_gen;
 		break;
+	case PASS_SPREAD: CK(cudaMemsetAsync(e->spread_acc.p, 0, (uint64_t)C * apo::SP_WORDS * 8, e->stream)); break;
 	}
 	e->pass[p].armed = true;
 	return APO_OK;
@@ -907,6 +912,11 @@ int launch_passes(apo_engine *e, const apo_score_opts *o, const Evals &ev, uint3
 		CK(apo::run_cand_groups(X, ev.form, recip, e->sm_count, e->stream));
 		e->timing.launches++;
 	}
+	if (run[PASS_SPREAD]) {
+		const apo::CandSpreadParams X{S, e->W, e->spread_acc.p + (uint64_t)apo::SP_WORDS * cand_offset};
+		CK(apo::run_cand_spread(X, ev.form, recip, e->sm_count, e->stream));
+		e->timing.launches++;
+	}
 	return APO_OK;
 }
 
@@ -930,6 +940,12 @@ int finish_passes(apo_engine *e, const apo_score_opts *o, uint32_t C) {
 	if (wants(o, PASS_GRP)) {                                       // words -> apo_group_score[C][G]; the extremes' lists are final as they are
 		CK(reserve(e, e->grp_rep, (uint64_t)(C ? C : 1) * e->grp_arm_G));
 		CK(apo::run_cand_groups_report(e->grp_acc.p, C, e->grp_arm_G, e->grp_rep.p, e->stream));
+		e->timing.launches++;
+	}
+	if (wants(o, PASS_SPREAD)) {                                    // sums of squares + the call's partials -> apo_candidate_spread[C]
+		CK(reserve(e, e->spread_rep, C ? C : 1));
+		const long long *partials = e->partials_src ? e->partials_src : e->acc.p;
+		CK(apo::run_cand_spread_report(e->spread_acc.p, partials, C, e->spread_rep.p, e->stream));
 		e->timing.launches++;
 	}
 	uint32_t dom = 0;                                               // k_cand_breakdown's domain word (pageable: the copy waits for the stream)
@@ -1683,6 +1699,7 @@ extern "C" void apo_destroy(apo_engine *e) {
 	e->result.release(); e->keys.release(); e->sel_key.release(); e->sel_idx.release();
 	e->cand_acc.release(); e->cand_rep.release(); e->tbook.release(); e->ccorp_acc.release(); e->ccorp_rep.release(); e->ext_acc.release();
 	e->grp_labels.release(); e->grp_acc.release(); e->grp_rep.release();
+	e->spread_acc.release(); e->spread_rep.release();
 	e->tup.release(); e->tups.release(); e->tvals.release();
 	e->win[0].release(); e->win[1].release(); e->batch_in.release(); e->batch_out.release(); e->batch_mask.release();
 	if (e->h_result) cudaFreeHost(e->h_result);
@@ -2125,7 +2142,7 @@ extern "C" int apo_score_finish(apo_engine *e, const apo_score_opts *o, double *
 	if (!e->scoring) return fail(e, APO_E_STATE, "apo_score_begin has not been called");
 	int rc = score_check(e, o, e->score_C, kSession, true);      // the accumulate calls refused every other source
 	if (rc) return rc;
-	for (const int p : {PASS_GRP, PASS_CAND, PASS_CCORP, PASS_EXT}) {
+	for (const int p : {PASS_GRP, PASS_CAND, PASS_CCORP, PASS_EXT, PASS_SPREAD}) {
 		if (!wants(o, p)) continue;
 		if (!e->pass[p].every)
 			return fail(e, APO_E_STATE, "%s: every apo_score_accumulate of the session must set the flag for %s", kPass[p].name, kPass[p].every);
@@ -2278,7 +2295,7 @@ int stream_host(apo_engine *e, const apo_score_opts *o, const HostTensor &h, dou
 	}
 	if ((rc = score_arm(e, o, C, true, (uint64_t)C * T * wire))) return rc;
 	if (h.form == apo::CAND_T) {                                   // the dictionary and its values, once for the whole call
-		if ((wants(o, PASS_CAND) || wants(o, PASS_EXT) || wants(o, PASS_GRP)) && (rc = upload_tbook(e, h.codebook))) return rc;
+		if ((wants(o, PASS_CAND) || wants(o, PASS_EXT) || wants(o, PASS_GRP) || wants(o, PASS_SPREAD)) && (rc = upload_tbook(e, h.codebook))) return rc;
 		if ((rc = dict_upload(e, e->tups, h.tb_pc, h.tb_pd, h.n_tuples, h.codebook, h.d2book))) return rc;
 		ev.dict = &e->tups; ev.t_once = true;
 		if ((rc = tuple_values(e, e->tups, e->tvals, (o->flags & APO_SCORE_RECIP) != 0))) return rc;
@@ -2652,6 +2669,13 @@ extern "C" int apo_record_groups_upload(apo_engine *e, const uint8_t *labels, ui
 extern "C" int apo_candidate_groups(apo_engine *e, uint32_t c0, uint32_t n, uint32_t G, apo_group_score *out) {
 	if (const int rc = report_check(e, PASS_GRP, c0, n, out, G); rc || n == 0) return rc;
 	CK(cudaMemcpyAsync(out, e->grp_rep.p + (uint64_t)c0 * G, (uint64_t)n * G * sizeof(apo_group_score), cudaMemcpyDeviceToHost, e->stream));
+	CK(cudaStreamSynchronize(e->stream));
+	return APO_OK;
+}
+
+extern "C" int apo_candidate_spread(apo_engine *e, uint32_t c0, uint32_t n, struct apo_candidate_spread *out) {
+	if (const int rc = report_check(e, PASS_SPREAD, c0, n, out); rc || n == 0) return rc;
+	CK(cudaMemcpyAsync(out, e->spread_rep.p + c0, (uint64_t)n * sizeof(struct apo_candidate_spread), cudaMemcpyDeviceToHost, e->stream));
 	CK(cudaStreamSynchronize(e->stream));
 	return APO_OK;
 }

@@ -17,7 +17,7 @@
 //
 // For record sources a second feature (APO_SCORE_CANDIDATE_CORPUS, k_cand_corpus below) goes further: the whole corpus
 // report of every candidate's records — patterns, per-mode tallies and tool totals included — by the corpus scan's own code.
-// The extremes and the group scores follow.  Every pass is one walk (cand_walk) over the same warp tiles with its own
+// The extremes, the group scores and the reward spread follow.  Every pass is one walk (cand_walk) over the same warp tiles with its own
 // per-evaluation step and flush, and one launcher sizes every walk's grid (walk_grid).
 #include <cstdlib>
 #include "apo_device.cuh"
@@ -749,6 +749,145 @@ cudaError_t run_cand_groups_report(const long long *words, uint32_t C, uint32_t 
 	return cudaGetLastError();
 }
 
+// ================================================================ per-candidate reward spread (APO_SCORE_CANDIDATE_SPREAD)
+//   k_cand_spread<Loader, TABLE, RECIP>  one pass over the evaluations a scoring call reads, on the shared loaders and walk:
+//                                        every lane sums x^2 exactly, x = rint(fr * 2^52) the term the call summed
+//   k_cand_spread_report                 n and S1 from the scoring call's partials, S2 from the words -> apo_candidate_spread
+// |x| <= 2^61 in the scoring domain (a term outside it fails the call), so x^2 < 2^127 is one exact unsigned 128-bit product
+// and a lane's 192-bit sum holds a run of CB_RUN_TILES tiles (2^21 terms) with room to spare.  A flush reduces the warp's sums
+// and adds the result into the candidate's three words with carried atomics: exact modulo 2^192 for any number of flushes,
+// and S2 < 2^192 for any n < 2^64.
+struct U192 { unsigned long long w0, w1, w2; };
+
+__device__ __forceinline__ void u192_add(U192 &a, unsigned long long w0, unsigned long long w1, unsigned long long w2) {
+	asm("add.cc.u64 %0, %0, %3;\n\taddc.cc.u64 %1, %1, %4;\n\taddc.u64 %2, %2, %5;" : "+l"(a.w0), "+l"(a.w1), "+l"(a.w2) : "l"(w0), "l"(w1), "l"(w2));
+}
+
+// a += x^2
+__device__ __forceinline__ void u192_add_sq(U192 &a, long long x) {
+	const unsigned long long u = x < 0 ? 0ull - (unsigned long long)x : (unsigned long long)x;
+	unsigned long long lo, hi;
+	asm("mul.lo.u64 %0, %2, %2;\n\tmul.hi.u64 %1, %2, %2;" : "=l"(lo), "=l"(hi) : "l"(u));
+	u192_add(a, lo, hi, 0ull);
+}
+
+// w[0..2] += v modulo 2^192: every atomic returns the word it added to, so its carry out is known exactly
+__device__ __forceinline__ void atomic_add_u192(unsigned long long *w, const U192 &v) {
+	unsigned long long c1 = 0ull, c2 = 0ull;
+	if (v.w0) { const unsigned long long o = atomicAdd(w, v.w0); c1 = o + v.w0 < o ? 1ull : 0ull; }
+	const unsigned long long m = v.w1 + c1;
+	c2 = m < c1 ? 1ull : 0ull;                                          // v.w1 all ones plus the carry
+	if (m) { const unsigned long long o = atomicAdd(w + 1, m); c2 += o + m < o ? 1ull : 0ull; }
+	const unsigned long long h = v.w2 + c2;
+	if (h) atomicAdd(w + 2, h);
+}
+
+template <class L, int TABLE, bool RECIP>
+__global__ void __launch_bounds__(CB_THREADS, L::MIN_CTAS)
+k_cand_spread(const CandSpreadParams X, uint32_t tiles_per_cand, uint64_t total_tiles) {
+	const CandEvals &P = X.src;
+	__shared__ CandSmem S;
+	__shared__ double s_rc[512];                                        // reciprocal of the total weight (div_lut)
+	stage_tables<TABLE, true>(P, S, s_rc);
+	const int lane = threadIdx.x & 31;
+	U192 a{0ull, 0ull, 0ull};
+
+	auto flush = [&](uint32_t c) {
+		U192 s = a;
+#pragma unroll
+		for (int o = 16; o > 0; o >>= 1)                                // 32 lanes of < 2^148 each: no carry leaves the sum
+			u192_add(s, __shfl_xor_sync(FULL, s.w0, o), __shfl_xor_sync(FULL, s.w1, o), __shfl_xor_sync(FULL, s.w2, o));
+		if (lane == 0 && (s.w0 | s.w1 | s.w2)) atomic_add_u192(X.words + (uint64_t)c * SP_WORDS, s);
+		a = U192{0ull, 0ull, 0ull};
+	};
+	auto each = [&](uint32_t, uint64_t, bool in, const typename L::Raw &R, uint32_t) {
+		if (!in) return;
+		CandEval E;
+		L::decode(P, S, R, E);
+		if (E.valid) u192_add_sq(a, to_fx(cand_final_reward<RECIP>(E, X.W, S.tw, s_rc)));
+	};
+	cand_walk<L, CB_RUN_TILES>(P, tiles_per_cand, total_tiles, each, flush);
+}
+
+// ---- exact 256-bit arithmetic of the report (little-endian words)
+// m += v * 2^(64 k)
+__device__ __forceinline__ void u256_add_at(unsigned long long m[4], unsigned __int128 v, int k) {
+	unsigned __int128 carry = v;
+	for (int i = k; i < 4 && carry; i++) {
+		const unsigned __int128 s = (unsigned __int128)m[i] + (unsigned long long)carry;
+		m[i] = (unsigned long long)s;
+		carry = (carry >> 64) + (s >> 64);
+	}
+}
+
+// RN(m) as binary64: the 64 bits below the leading one, the discarded bits ORed into the last of them (a sticky bit well below
+// the rounding position), then one correctly rounded conversion and an exact scaling
+__device__ __forceinline__ double u256_to_double(const unsigned long long m[4]) {
+	int k = 3;
+	while (k > 0 && m[k] == 0ull) k--;
+	if (k == 0) return __ull2double_rn(m[0]);
+	const int sh = 64 * k - __clzll((long long)m[k]);                 // bit index of the lowest of the 64 kept bits, >= 1
+	const int q = sh >> 6, b = sh & 63;
+	unsigned long long top = b ? (m[q] >> b) | (m[q + 1] << (64 - b)) : m[q];
+	bool sticky = b ? (m[q] << (64 - b)) != 0ull : false;
+	for (int i = 0; i < q; i++) sticky |= m[i] != 0ull;
+	return ldexp(__ull2double_rn(top | (sticky ? 1ull : 0ull)), sh);
+}
+
+// one thread per candidate
+__global__ void __launch_bounds__(256)
+k_cand_spread_report(const unsigned long long *words, const long long *partials, uint32_t C, struct apo_candidate_spread *out) {
+	const uint32_t c = blockIdx.x * blockDim.x + threadIdx.x;
+	if (c >= C) return;
+	long long l[4];
+#pragma unroll
+	for (int q = 0; q < 4; q++) l[q] = partials[(uint64_t)ACC_PER_CAND * c + q];
+	const uint64_t n = (uint64_t)l[3];
+	const __int128 s1 = ((__int128)l[2] << 64) + ((__int128)l[1] << 32) + (__int128)l[0];
+	const unsigned long long *w = words + (uint64_t)c * SP_WORDS;
+	const unsigned long long s2[4] = {w[0], w[1], w[2], 0ull};
+	struct apo_candidate_spread R;
+	R.n = n;
+	R.sumLo = (uint64_t)(unsigned __int128)s1;
+	R.sumHi = (int64_t)(s1 >> 64);
+	R.sumSq[0] = s2[0]; R.sumSq[1] = s2[1]; R.sumSq[2] = s2[2];
+	R.mean = report_avg_reward(limbs_to_double(l), n);                   // the division scores[c] is: same bits
+	R.rewardSumSq = __dmul_rn(u256_to_double(s2), 0x1p-104);
+	const double nan = __longlong_as_double(0x7ff8000000000000ll);
+	if (n < 2) {
+		R.variance = R.stdDev = R.stdErr = nan;
+	} else {
+		// M = n * S2 - S1^2, with n * S2 < 2^256 and |S1| < 2^128
+		unsigned long long a[4] = {0ull, 0ull, 0ull, 0ull}, b[4] = {0ull, 0ull, 0ull, 0ull};
+		for (int i = 0; i < 3; i++) u256_add_at(a, (unsigned __int128)n * s2[i], i);
+		const unsigned __int128 u = s1 < 0 ? (unsigned __int128)0 - (unsigned __int128)s1 : (unsigned __int128)s1;
+		const unsigned long long u0 = (unsigned long long)u, u1 = (unsigned long long)(u >> 64);
+		u256_add_at(b, (unsigned __int128)u0 * u0, 0);
+		u256_add_at(b, (unsigned __int128)u0 * u1, 1);
+		u256_add_at(b, (unsigned __int128)u0 * u1, 1);
+		u256_add_at(b, (unsigned __int128)u1 * u1, 2);
+		unsigned long long m[4], borrow = 0ull;
+		for (int i = 0; i < 4; i++) {
+			const unsigned long long d = a[i] - b[i];
+			const unsigned long long nb = (a[i] < b[i] ? 1ull : 0ull) | (d < borrow ? 1ull : 0ull);
+			m[i] = d - borrow;
+			borrow = nb;
+		}
+		const double dn = __ull2double_rn(n);
+		R.variance = __ddiv_rn(__ddiv_rn(__dmul_rn(u256_to_double(m), 0x1p-104), dn), __ull2double_rn(n - 1));
+		R.stdDev = __dsqrt_rn(R.variance);
+		R.stdErr = __dsqrt_rn(__ddiv_rn(R.variance, dn));
+	}
+	out[c] = R;
+}
+
+cudaError_t run_cand_spread_report(const unsigned long long *words, const long long *partials, uint32_t C, struct apo_candidate_spread *out,
+                                   cudaStream_t st) {
+	if (C == 0) return cudaSuccess;
+	k_cand_spread_report<<<(C + 255) / 256, 256, 0, st>>>(words, partials, C, out);
+	return cudaGetLastError();
+}
+
 // ================================================================ one dispatch for the passes that read every source
 template <class L, int TABLE, bool>
 static cudaError_t launch_pass(const CandParams &P, int sm_count, cudaStream_t st) {
@@ -757,6 +896,10 @@ static cudaError_t launch_pass(const CandParams &P, int sm_count, cudaStream_t s
 template <class L, int TABLE, bool RECIP>
 static cudaError_t launch_pass(const CandGroupParams &X, int sm_count, cudaStream_t st) {
 	return launch_walk(k_cand_groups<L, TABLE, RECIP>, X, sm_count, st);
+}
+template <class L, int TABLE, bool RECIP>
+static cudaError_t launch_pass(const CandSpreadParams &X, int sm_count, cudaStream_t st) {
+	return launch_walk(k_cand_spread<L, TABLE, RECIP>, X, sm_count, st);
 }
 
 // the loader of each source and the table it stages; RECIP: the division of the passes that divide (div_lut)
@@ -780,6 +923,9 @@ cudaError_t run_cand_extremes(const CandExtParams &X, int source, bool recip, in
 	return recip ? by_source<true>(X, source, sm_count, st) : by_source<false>(X, source, sm_count, st);
 }
 cudaError_t run_cand_groups(const CandGroupParams &X, int source, bool recip, int sm_count, cudaStream_t st) {
+	return recip ? by_source<true>(X, source, sm_count, st) : by_source<false>(X, source, sm_count, st);
+}
+cudaError_t run_cand_spread(const CandSpreadParams &X, int source, bool recip, int sm_count, cudaStream_t st) {
 	return recip ? by_source<true>(X, source, sm_count, st) : by_source<false>(X, source, sm_count, st);
 }
 

@@ -408,6 +408,20 @@ cudaError_t run_cand_groups(const CandGroupParams &P, int source, bool recip, in
 // words: the whole buffer of C candidates
 cudaError_t run_cand_groups_report(const long long *words, uint32_t C, uint32_t G, apo_group_score *out, cudaStream_t st);
 
+// ---- per-candidate reward spread (csrc/apo_cand.cu): the exact sum of squares of every candidate's terms rint(fr * 2^52).
+// Own buffer [C][SP_WORDS]: S2 as an unsigned 192-bit integer, least significant word first.  n and S1 are the scoring
+// call's own partials.
+constexpr int SP_WORDS = 3;
+struct CandSpreadParams {
+	CandEvals src;
+	Weights W;
+	unsigned long long *words;      // [C][SP_WORDS] of candidate 0 of this launch
+};
+cudaError_t run_cand_spread(const CandSpreadParams &P, int source, bool recip, int sm_count, cudaStream_t st);
+// words: the whole buffer; partials: the scoring call's candidate accumulators (4 words per candidate)
+cudaError_t run_cand_spread_report(const unsigned long long *words, const long long *partials, uint32_t C, struct apo_candidate_spread *out,
+                                   cudaStream_t st);
+
 int k1_tile_evals(int row, int variant);
 cudaError_t run_reward9(K1Params P, int row, int variant, bool recip, int sm_count, cudaStream_t st);
 cudaError_t run_detect6(const K2Params &P, int sm_count, cudaStream_t st);

@@ -25,6 +25,7 @@ SCORE_CANDIDATE_EXTREMES = 0x20
 EXTREMES_N = 32
 SCORE_CANDIDATE_GROUPS = 0x40
 GROUPS_MAX = 64
+SCORE_CANDIDATE_SPREAD = 0x80
 TUNE_NO_FUSE, TUNE_FORCE_FUSE, TUNE_NO_STAGING, TUNE_NCCL_JOIN, TUNE_NO_TWIN = 0x1, 0x2, 0x4, 0x8, 0x10
 TUNE_NO_TWIN_T, TUNE_TWIN_T, TUNE_NO_TWIN_T2, TUNE_NO_TWIN_H = 0x20, 0x40, 0x80, 0x100
 TUNE_NO_CORPUS_DIGEST = 0x200
@@ -93,6 +94,26 @@ class GroupScore(C.Structure):
                 ("withReward", C.c_uint64), ("rewardSum", C.c_double), ("avgReward", C.c_double)]
 
 
+class CandidateSpread(C.Structure):
+    """struct apo_candidate_spread: one candidate's reward spread.  n == counts[c]; the exact integers S1 = sum x (two's
+    complement 128-bit: sumLo, sumHi) and S2 = sum x^2 (unsigned 192-bit, sumSq least significant word first) of its terms
+    x = rint(fr * 2^52); mean == scores[c] (NaN when n == 0); rewardSumSq = RN(S2) * 2^-104; the unbiased variance, stdDev
+    and stdErr of the mean, each rounded as the header states (NaN when n < 2)."""
+    _fields_ = [("n", C.c_uint64), ("sumLo", C.c_uint64), ("sumHi", C.c_int64), ("sumSq", C.c_uint64 * 3),
+                ("mean", C.c_double), ("rewardSumSq", C.c_double), ("variance", C.c_double), ("stdDev", C.c_double),
+                ("stdErr", C.c_double)]
+
+    @property
+    def sum(self) -> int:
+        """S1 as a Python int"""
+        return (int(self.sumHi) << 64) | int(self.sumLo)
+
+    @property
+    def sum_sq(self) -> int:
+        """S2 as a Python int"""
+        return int(self.sumSq[0]) | (int(self.sumSq[1]) << 64) | (int(self.sumSq[2]) << 128)
+
+
 class Timing(C.Structure):
     _fields_ = [("reward_ms", C.c_float), ("corpus_ms", C.c_float), ("allreduce_ms", C.c_float),
                 ("finalize_ms", C.c_float), ("total_ms", C.c_float), ("launches", C.c_uint32), ("pad", C.c_uint32),
@@ -122,7 +143,7 @@ ABI_SYMBOLS = (
     "apo_dims_compact_download", "apo_dims_codebook", "apo_packed_encode_host", "apo_score_host_packed", "apo_dims_packed_download", "apo_dims_d2book",
     "apo_tuple_encode_host", "apo_score_host_tuples", "apo_tuples_upload", "apo_dims_tuples", "apo_tuples_download", "apo_tuples_book",
     "apo_host_alloc", "apo_host_free",
-    "apo_last_timing", "apo_debug_partials", "apo_debug_twin_t_list", "apo_debug_twin_h", "apo_debug_corpus_digest", "apo_candidate_reports", "apo_candidate_corpus_reports", "apo_candidate_extremes", "apo_record_groups_upload", "apo_candidate_groups", "apo_comm_unique_id", "apo_comm_init", "apo_comm_destroy", "apo_comm_join_mode",
+    "apo_last_timing", "apo_debug_partials", "apo_debug_twin_t_list", "apo_debug_twin_h", "apo_debug_corpus_digest", "apo_candidate_reports", "apo_candidate_corpus_reports", "apo_candidate_extremes", "apo_record_groups_upload", "apo_candidate_groups", "apo_candidate_spread", "apo_comm_unique_id", "apo_comm_init", "apo_comm_destroy", "apo_comm_join_mode",
 )
 
 
@@ -215,6 +236,7 @@ def load_library() -> C.CDLL:
     L.apo_candidate_extremes.argtypes = [vp, u32, u32, vp]
     L.apo_record_groups_upload.argtypes = [vp, vp, u64, u32]
     L.apo_candidate_groups.argtypes = [vp, u32, u32, u32, vp]
+    L.apo_candidate_spread.argtypes = [vp, u32, u32, vp]
     L.apo_comm_unique_id.argtypes = [vp]
     L.apo_comm_init.argtypes = [vp, i32, i32, vp]
     L.apo_comm_destroy.argtypes = [vp]
@@ -281,14 +303,16 @@ def records_from_json(text: str | bytes) -> np.ndarray:
 
 
 class ScoreResult:
-    __slots__ = ("scores", "counts", "topk", "report", "timing", "candidates", "candidate_corpus", "extremes", "groups")
+    __slots__ = ("scores", "counts", "topk", "report", "timing", "candidates", "candidate_corpus", "extremes", "groups", "spread")
 
-    def __init__(self, scores, counts, topk, report, timing, candidates=None, candidate_corpus=None, extremes=None, groups=None):
+    def __init__(self, scores, counts, topk, report, timing, candidates=None, candidate_corpus=None, extremes=None, groups=None,
+                 spread=None):
         self.scores, self.counts, self.topk, self.report, self.timing = scores, counts, topk, report, timing
         self.candidates = candidates        # CandidateReport array [C] when the call asked for the breakdown, else None
         self.candidate_corpus = candidate_corpus   # CorpusReport array [C] when the call asked for the per-candidate corpus reports
         self.extremes = extremes            # CandidateExtremes array [C] when the call asked for the per-candidate extremes
         self.groups = groups                # GroupScore array [C][G] when the call asked for the per-candidate group scores
+        self.spread = spread                # CandidateSpread array [C] when the call asked for the per-candidate reward spread
 
 
 class Engine:
@@ -430,12 +454,12 @@ class Engine:
 
     def score_host_records(self, recs: np.ndarray, K: int, corpus: bool = False, recip: bool = False, variant: int = 0,
                            candidates: bool = False, candidate_corpus: bool = False, extremes: bool = False,
-                           groups: bool = False) -> ScoreResult:
+                           groups: bool = False, spread: bool = False) -> ScoreResult:
         """recs: C-contiguous [C][T] of RECORD_DTYPE (32 B) or RECORD16_DTYPE (16 B) in host memory."""
         assert recs.flags.c_contiguous and recs.ndim == 2 and recs.dtype.itemsize in (32, 16)
         Cn, T = recs.shape
         o = self._opts(K, SRC_ROLLOUTS, corpus, recip, variant, 0, 0, candidates=candidates, candidate_corpus=candidate_corpus,
-                       extremes=extremes, groups=groups)
+                       extremes=extremes, groups=groups, spread=spread)
         scores = np.empty(Cn, np.float64)
         counts = np.empty(Cn, np.uint64)
         topk = np.empty(K, np.int32)
@@ -443,14 +467,15 @@ class Engine:
         self._ck(self._L.apo_score_host_records(self._h, C.byref(o), _p(recs), recs.dtype.itemsize, Cn, T, _p(scores), _p(counts),
                                                 _p(topk), C.byref(rep) if rep is not None else None))
         return ScoreResult(scores, counts, topk, rep, self.last_timing(), self._cands(Cn, candidates),
-                           self._ccorp(Cn, candidate_corpus), self._ext(Cn, extremes), self._grp(Cn, groups))
+                           self._ccorp(Cn, candidate_corpus), self._ext(Cn, extremes), self._grp(Cn, groups), self._spr(Cn, spread))
 
     # -- scoring
     def _opts(self, K, source, corpus, recip, variant, first, count, timing=False, candidates=False,
-              candidate_corpus=False, extremes=False, groups=False) -> ScoreOpts:
+              candidate_corpus=False, extremes=False, groups=False, spread=False) -> ScoreOpts:
         return ScoreOpts(K, source, (SCORE_CORPUS if corpus else 0) | (SCORE_RECIP if recip else 0) | (SCORE_TIMING if timing else 0)
                          | (SCORE_CANDIDATES if candidates else 0) | (SCORE_CANDIDATE_CORPUS if candidate_corpus else 0)
-                         | (SCORE_CANDIDATE_EXTREMES if extremes else 0) | (SCORE_CANDIDATE_GROUPS if groups else 0),
+                         | (SCORE_CANDIDATE_EXTREMES if extremes else 0) | (SCORE_CANDIDATE_GROUPS if groups else 0)
+                         | (SCORE_CANDIDATE_SPREAD if spread else 0),
                          variant, first, count)
 
     def _cands(self, Cn: int, wanted: bool):
@@ -465,6 +490,9 @@ class Engine:
     def _grp(self, Cn: int, wanted: bool):
         return self.candidate_groups(0, Cn) if wanted else None
 
+    def _spr(self, Cn: int, wanted: bool):
+        return self.candidate_spread(0, Cn) if wanted else None
+
     def record_groups_upload(self, labels, G: int = 0):
         """apo_record_groups_upload: labels uint8 [T], the group of every record position (< G <= GROUPS_MAX); an empty
         array releases them.  Scoring calls with groups=True then split every candidate's evaluations by these groups."""
@@ -478,6 +506,13 @@ class Engine:
         G = self._groups_G if G is None else G
         out = ((GroupScore * max(G, 1)) * n)()
         self._ck(self._L.apo_candidate_groups(self._h, c0, n, G, out if n else None))
+        return out
+
+    def candidate_spread(self, c0: int, n: int):
+        """apo_candidate_spread: CandidateSpread[n] of candidates [c0, c0+n) from the last scoring call, which must have set
+        spread=True (ApoError APO_E_STATE otherwise)."""
+        out = (CandidateSpread * n)()
+        self._ck(self._L.apo_candidate_spread(self._h, c0, n, out if n else None))
         return out
 
     def candidate_extremes(self, c0: int, n: int):
@@ -505,8 +540,8 @@ class Engine:
 
     def score(self, Cn: int, K: int, source: int = SRC_DIMS, corpus: bool = False, recip: bool = False,
               variant: int = 0, first: int = 0, count: int = 0, timing: bool = False, candidates: bool = False,
-              candidate_corpus: bool = False, extremes: bool = False, groups: bool = False) -> ScoreResult:
-        o = self._opts(K, source, corpus, recip, variant, first, count, timing, candidates, candidate_corpus, extremes, groups)
+              candidate_corpus: bool = False, extremes: bool = False, groups: bool = False, spread: bool = False) -> ScoreResult:
+        o = self._opts(K, source, corpus, recip, variant, first, count, timing, candidates, candidate_corpus, extremes, groups, spread)
         scores = np.empty(Cn, np.float64)
         counts = np.empty(Cn, np.uint64)
         topk = np.empty(K, np.int32)
@@ -518,7 +553,7 @@ class Engine:
             self._ck(rc)
         L.apo_last_timing(self._h, C.byref(t))
         return ScoreResult(scores, counts, topk, rep, t, self._cands(Cn, candidates), self._ccorp(Cn, candidate_corpus),
-                           self._ext(Cn, extremes), self._grp(Cn, groups))
+                           self._ext(Cn, extremes), self._grp(Cn, groups), self._spr(Cn, spread))
 
     # chunked form: begin / accumulate (per candidate chunk or record window) / finish
     def score_begin(self, C_total: int):
@@ -526,15 +561,15 @@ class Engine:
 
     def score_accumulate(self, cand_offset: int = 0, source: int = SRC_DIMS, recip: bool = False, variant: int = 0,
                          first: int = 0, count: int = 0, candidates: bool = False, candidate_corpus: bool = False,
-                         extremes: bool = False, groups: bool = False):
+                         extremes: bool = False, groups: bool = False, spread: bool = False):
         o = self._opts(0, source, False, recip, variant, first, count, candidates=candidates, candidate_corpus=candidate_corpus,
-                       extremes=extremes, groups=groups)
+                       extremes=extremes, groups=groups, spread=spread)
         self._ck(self._L.apo_score_accumulate(self._h, C.byref(o), cand_offset))
 
     def score_finish(self, C_total: int, K: int, corpus: bool = False, candidates: bool = False,
-                     candidate_corpus: bool = False, extremes: bool = False, groups: bool = False) -> ScoreResult:
+                     candidate_corpus: bool = False, extremes: bool = False, groups: bool = False, spread: bool = False) -> ScoreResult:
         o = self._opts(K, SRC_DIMS, corpus, False, 0, 0, 0, candidates=candidates, candidate_corpus=candidate_corpus, extremes=extremes,
-                       groups=groups)
+                       groups=groups, spread=spread)
         scores = np.empty(C_total, np.float64)
         counts = np.empty(C_total, np.uint64)
         topk = np.empty(K, np.int32)
@@ -542,14 +577,15 @@ class Engine:
         self._ck(self._L.apo_score_finish(self._h, C.byref(o), _p(scores), _p(counts), _p(topk),
                                           C.byref(rep) if rep is not None else None))
         return ScoreResult(scores, counts, topk, rep, self.last_timing(), self._cands(C_total, candidates),
-                           self._ccorp(C_total, candidate_corpus), self._ext(C_total, extremes), self._grp(C_total, groups))
+                           self._ccorp(C_total, candidate_corpus), self._ext(C_total, extremes), self._grp(C_total, groups),
+                           self._spr(C_total, spread))
 
     def score_host(self, dims: np.ndarray, K: int, corpus: bool = False, recip: bool = False, variant: int = 0,
-                   candidates: bool = False, extremes: bool = False, groups: bool = False) -> ScoreResult:
+                   candidates: bool = False, extremes: bool = False, groups: bool = False, spread: bool = False) -> ScoreResult:
         """dims: C-contiguous float32 [C][T][9] in (preferably pinned) host memory."""
         assert dims.dtype == np.float32 and dims.flags.c_contiguous and dims.ndim == 3 and dims.shape[2] == NDIM
         Cn, T, _ = dims.shape
-        o = self._opts(K, SRC_DIMS, corpus, recip, variant, 0, 0, candidates=candidates, extremes=extremes, groups=groups)
+        o = self._opts(K, SRC_DIMS, corpus, recip, variant, 0, 0, candidates=candidates, extremes=extremes, groups=groups, spread=spread)
         scores = np.empty(Cn, np.float64)
         counts = np.empty(Cn, np.uint64)
         topk = np.empty(K, np.int32)
@@ -557,7 +593,7 @@ class Engine:
         self._ck(self._L.apo_score_host(self._h, C.byref(o), _p(dims), Cn, T, _p(scores), _p(counts), _p(topk),
                                         C.byref(rep) if rep is not None else None))
         return ScoreResult(scores, counts, topk, rep, self.last_timing(), self._cands(Cn, candidates), extremes=self._ext(Cn, extremes),
-                           groups=self._grp(Cn, groups))
+                           groups=self._grp(Cn, groups), spread=self._spr(Cn, spread))
 
     # -- Form Q in host memory (compact wire format)
     def dims_codebook(self) -> np.ndarray:
@@ -573,13 +609,13 @@ class Engine:
 
     def score_host_compact(self, q8: np.ndarray, d2: np.ndarray, li: np.ndarray, codebook: np.ndarray, K: int, corpus: bool = False,
                            recip: bool = False, candidates: bool = False, extremes: bool = False,
-                          groups: bool = False) -> ScoreResult:
+                          groups: bool = False, spread: bool = False) -> ScoreResult:
         """q8 uint64 [C][T], d2 float32 [C][T], li uint16 [C][T] in (preferably pinned) host memory + the uint32[2048] codebook."""
         assert q8.dtype == np.uint64 and d2.dtype == np.float32 and li.dtype == np.uint16 and q8.shape == d2.shape == li.shape and q8.ndim == 2
         assert q8.flags.c_contiguous and d2.flags.c_contiguous and li.flags.c_contiguous
         codebook = np.ascontiguousarray(codebook, np.uint32)
         Cn, T = q8.shape
-        o = self._opts(K, SRC_DIMS, corpus, recip, 0, 0, 0, candidates=candidates, extremes=extremes, groups=groups)
+        o = self._opts(K, SRC_DIMS, corpus, recip, 0, 0, 0, candidates=candidates, extremes=extremes, groups=groups, spread=spread)
         scores = np.empty(Cn, np.float64)
         counts = np.empty(Cn, np.uint64)
         topk = np.empty(K, np.int32)
@@ -587,7 +623,7 @@ class Engine:
         self._ck(self._L.apo_score_host_compact(self._h, C.byref(o), _p(q8), _p(d2), _p(li), _p(codebook), Cn, T, _p(scores), _p(counts),
                                                 _p(topk), C.byref(rep) if rep is not None else None))
         return ScoreResult(scores, counts, topk, rep, self.last_timing(), self._cands(Cn, candidates), extremes=self._ext(Cn, extremes),
-                           groups=self._grp(Cn, groups))
+                           groups=self._grp(Cn, groups), spread=self._spr(Cn, spread))
 
     def dims_d2book(self) -> np.ndarray:
         out = np.empty(4096, np.uint32)
@@ -602,13 +638,13 @@ class Engine:
 
     def score_host_packed(self, pc: np.ndarray, pd: np.ndarray, codebook: np.ndarray, d2book: np.ndarray, K: int, corpus: bool = False,
                           recip: bool = False, candidates: bool = False, extremes: bool = False,
-                          groups: bool = False) -> ScoreResult:
+                          groups: bool = False, spread: bool = False) -> ScoreResult:
         """Form P: pc uint32 [C][T] (eight 4-bit codes), pd uint16 [C][T] (tool_success_rate index) + the two codebooks."""
         assert pc.dtype == np.uint32 and pd.dtype == np.uint16 and pc.shape == pd.shape and pc.ndim == 2 and pc.flags.c_contiguous and pd.flags.c_contiguous
         codebook, d2book = np.ascontiguousarray(codebook, np.uint32), np.ascontiguousarray(d2book, np.uint32)
         assert codebook.size == 2048 and d2book.size == 4096
         Cn, T = pc.shape
-        o = self._opts(K, SRC_DIMS, corpus, recip, 0, 0, 0, candidates=candidates, extremes=extremes, groups=groups)
+        o = self._opts(K, SRC_DIMS, corpus, recip, 0, 0, 0, candidates=candidates, extremes=extremes, groups=groups, spread=spread)
         scores = np.empty(Cn, np.float64)
         counts = np.empty(Cn, np.uint64)
         topk = np.empty(K, np.int32)
@@ -616,7 +652,7 @@ class Engine:
         self._ck(self._L.apo_score_host_packed(self._h, C.byref(o), _p(pc), _p(pd), _p(codebook), _p(d2book), Cn, T, _p(scores), _p(counts),
                                                _p(topk), C.byref(rep) if rep is not None else None))
         return ScoreResult(scores, counts, topk, rep, self.last_timing(), self._cands(Cn, candidates), extremes=self._ext(Cn, extremes),
-                           groups=self._grp(Cn, groups))
+                           groups=self._grp(Cn, groups), spread=self._spr(Cn, spread))
 
     @staticmethod
     def _tuple_args(tl, th, tbook, codebook, d2book):
@@ -629,12 +665,12 @@ class Engine:
 
     def score_host_tuples(self, tl: np.ndarray, th: np.ndarray, tbook, codebook: np.ndarray, d2book: np.ndarray, K: int, corpus: bool = False,
                           recip: bool = False, candidates: bool = False, extremes: bool = False,
-                          groups: bool = False) -> ScoreResult:
+                          groups: bool = False, spread: bool = False) -> ScoreResult:
         """Form T: tl uint16 [C][T] + th uint8 [C][T] (24-bit dictionary indices), tbook = (pc uint32 [n], pd uint16 [n]) the distinct
         evaluations as Form P pairs, + the two codebooks of Form P."""
         tb_pc, tb_pd, codebook, d2book = self._tuple_args(tl, th, tbook, codebook, d2book)
         Cn, T = tl.shape
-        o = self._opts(K, SRC_DIMS, corpus, recip, 0, 0, 0, candidates=candidates, extremes=extremes, groups=groups)
+        o = self._opts(K, SRC_DIMS, corpus, recip, 0, 0, 0, candidates=candidates, extremes=extremes, groups=groups, spread=spread)
         scores = np.empty(Cn, np.float64)
         counts = np.empty(Cn, np.uint64)
         topk = np.empty(K, np.int32)
@@ -642,7 +678,7 @@ class Engine:
         self._ck(self._L.apo_score_host_tuples(self._h, C.byref(o), _p(tl), _p(th), _p(tb_pc), _p(tb_pd), tb_pc.size, _p(codebook), _p(d2book), Cn, T,
                                                _p(scores), _p(counts), _p(topk), C.byref(rep) if rep is not None else None))
         return ScoreResult(scores, counts, topk, rep, self.last_timing(), self._cands(Cn, candidates), extremes=self._ext(Cn, extremes),
-                           groups=self._grp(Cn, groups))
+                           groups=self._grp(Cn, groups), spread=self._spr(Cn, spread))
 
     def tuples_upload(self, tl: np.ndarray, th: np.ndarray, tbook, codebook: np.ndarray, d2book: np.ndarray):
         """Make a Form T tensor resident: score(C, K, source=SRC_TUPLES) then reads 3 B per evaluation."""

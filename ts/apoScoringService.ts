@@ -28,6 +28,7 @@ export interface ApoScoreBlocks {
 	candidateCorpus?: VSBuffer;   // apo_corpus_report[C] (784 bytes each, decodeCandidateCorpusReport); rollout records only, when asked for
 	candidateExtremes?: VSBuffer;   // struct apo_candidate_extremes[C] (1032 bytes each, decodeCandidateExtremes); only when asked for
 	candidateGroups?: VSBuffer;   // apo_group_score[C][G] (56 bytes each, decodeCandidateGroups); only when asked for
+	candidateSpread?: VSBuffer;   // struct apo_candidate_spread[C] (88 bytes each, decodeCandidateSpread); only when asked for
 }
 
 /** Form T of a float32[C][T][9] tensor (include/apo_b200.h): tl uint16[C][T] | th uint8[C][T] = the 24-bit dictionary index of every
@@ -47,6 +48,7 @@ export interface ApoResidentQuery {
 	candidateCorpus?: 0 | 1;   // source 1 only: also build every candidate's corpus report (ApoScoreBlocks.candidateCorpus)
 	candidateExtremes?: 0 | 1;   // also list every candidate's 32 lowest- and highest-reward rollouts (ApoScoreBlocks.candidateExtremes)
 	candidateGroups?: number;   // G of the uploaded record groups: also split every candidate's rollouts by group (ApoScoreBlocks.candidateGroups)
+	candidateSpread?: 0 | 1;   // also build every candidate's reward spread (ApoScoreBlocks.candidateSpread)
 	first?: number;         // window [first, first + count) of the trace axis; count 0 = to the end
 	count?: number;
 }
@@ -84,18 +86,19 @@ export interface IApoScoringService {
 	/** dims: float32[C][T][9] (pass C = 1, T = 4 of NaN for report-only calls).
 	 *  candidates: also return the per-candidate breakdown (ApoScoreBlocks.candidates), here and on the other one-shot calls;
 	 *  candidateExtremes: also return every candidate's 32 lowest- and highest-reward rollouts (ApoScoreBlocks.candidateExtremes);
-	 *  candidateGroups: the G of recordGroupsUpload, also return every candidate's scores per record group (ApoScoreBlocks.candidateGroups). */
+	 *  candidateGroups: the G of recordGroupsUpload, also return every candidate's scores per record group (ApoScoreBlocks.candidateGroups);
+	 *  candidateSpread: also return every candidate's reward spread (ApoScoreBlocks.candidateSpread). */
 	score(dims: VSBuffer, C: number, T: number, corpus: VSBuffer | undefined, K: number, candidates?: boolean,
-		candidateExtremes?: boolean, candidateGroups?: number): Promise<ApoScoreBlocks>;
+		candidateExtremes?: boolean, candidateGroups?: number, candidateSpread?: boolean): Promise<ApoScoreBlocks>;
 	/** [C][T] trace records (the IDE's own representation): 2.2x fewer PCIe bytes than fp32 dims with 16-byte rows.
 	 *  candidateCorpus: also return the corpus report of every candidate's records (ApoScoreBlocks.candidateCorpus). */
 	scoreHostRecords(records: VSBuffer, rowBytes: 32 | 16, C: number, T: number, corpus: VSBuffer | undefined, K: number, candidates?: boolean,
-		candidateCorpus?: boolean, candidateExtremes?: boolean, candidateGroups?: number): Promise<ApoScoreBlocks>;
+		candidateCorpus?: boolean, candidateExtremes?: boolean, candidateGroups?: number, candidateSpread?: boolean): Promise<ApoScoreBlocks>;
 	/** fp32 evaluations -> Form T (include/apo_b200.h): a 24-bit dictionary index per evaluation (3 bytes instead of 36) + the
 	 *  dictionary of distinct evaluations.  For evaluations that are scored more than once, kept, or moved between processes. */
 	encodeTuples(dims: VSBuffer, C: number, T: number): Promise<ApoTupleBuffers | undefined>;
 	scoreTuples(tuples: ApoTupleBuffers, C: number, T: number, corpus: VSBuffer | undefined, K: number, candidates?: boolean,
-		candidateExtremes?: boolean, candidateGroups?: number): Promise<ApoScoreBlocks>;
+		candidateExtremes?: boolean, candidateGroups?: number, candidateSpread?: boolean): Promise<ApoScoreBlocks>;
 }
 
 export const IApoScoringService = createDecorator<IApoScoringService>('senweaverApoScoringService');
@@ -119,20 +122,25 @@ export class ApoScoringService implements IApoScoringService {
 	dimsTuples(cap?: number) { return this._proxy.dimsTuples(cap); }
 	recordGroupsUpload(labels: VSBuffer, G: number) { return this._proxy.recordGroupsUpload(labels, G); }
 	scoreResident(query: ApoResidentQuery) { return this._proxy.scoreResident(query); }
-	// A call without group scores sends the channel the same arguments as before the option existed.
+	// A call without group scores or spreads sends the channel the same arguments as before those options existed.
 	score(dims: VSBuffer, C: number, T: number, corpus: VSBuffer | undefined, K: number, candidates?: boolean, candidateExtremes?: boolean,
-		candidateGroups?: number) {
+		candidateGroups?: number, candidateSpread?: boolean) {
+		if (candidateSpread) { return this._proxy.score(dims, C, T, corpus, K, candidates, candidateExtremes, candidateGroups ?? 0, true); }
 		if (candidateGroups) { return this._proxy.score(dims, C, T, corpus, K, candidates, candidateExtremes, candidateGroups); }
 		return this._proxy.score(dims, C, T, corpus, K, candidates, candidateExtremes);
 	}
 	scoreHostRecords(records: VSBuffer, rowBytes: 32 | 16, C: number, T: number, corpus: VSBuffer | undefined, K: number, candidates?: boolean,
-		candidateCorpus?: boolean, candidateExtremes?: boolean, candidateGroups?: number) {
+		candidateCorpus?: boolean, candidateExtremes?: boolean, candidateGroups?: number, candidateSpread?: boolean) {
+		if (candidateSpread) {
+			return this._proxy.scoreHostRecords(records, rowBytes, C, T, corpus, K, candidates, candidateCorpus, candidateExtremes, candidateGroups ?? 0, true);
+		}
 		if (candidateGroups) { return this._proxy.scoreHostRecords(records, rowBytes, C, T, corpus, K, candidates, candidateCorpus, candidateExtremes, candidateGroups); }
 		return this._proxy.scoreHostRecords(records, rowBytes, C, T, corpus, K, candidates, candidateCorpus, candidateExtremes);
 	}
 	encodeTuples(dims: VSBuffer, C: number, T: number) { return this._proxy.encodeTuples(dims, C, T); }
 	scoreTuples(tuples: ApoTupleBuffers, C: number, T: number, corpus: VSBuffer | undefined, K: number, candidates?: boolean,
-		candidateExtremes?: boolean, candidateGroups?: number) {
+		candidateExtremes?: boolean, candidateGroups?: number, candidateSpread?: boolean) {
+		if (candidateSpread) { return this._proxy.scoreTuples(tuples, C, T, corpus, K, candidates, candidateExtremes, candidateGroups ?? 0, true); }
 		if (candidateGroups) { return this._proxy.scoreTuples(tuples, C, T, corpus, K, candidates, candidateExtremes, candidateGroups); }
 		return this._proxy.scoreTuples(tuples, C, T, corpus, K, candidates, candidateExtremes);
 	}

@@ -19,8 +19,12 @@
  *  And the decoder of the per-candidate group scores (ApoScoreBlocks.candidateGroups): apo_group_score[C][G], each candidate's
  *  tallies and exact mean reward on the rollouts of every record group (a chat mode, a task category, a held-out split).
  *
+ *  And the decoder of the per-candidate reward spreads (ApoScoreBlocks.candidateSpread): struct apo_candidate_spread[C], each
+ *  candidate's exact reward sums and the variance, standard deviation and standard error of its mean: the scale against which
+ *  the gap between two candidates' scores can be read.
+ *
  *  The byte offsets below are pinned to the C structs by tests/test_napi_candidates.py, tests/test_candidate_corpus_cpu.py,
- *  tests/test_napi_candidate_extremes.py and tests/test_candidate_groups_cpu.py.
+ *  tests/test_napi_candidate_extremes.py, tests/test_candidate_groups_cpu.py and tests/test_candidate_spread_cpu.py.
  *--------------------------------------------------------------------------------------------*/
 import { VSBuffer } from '../../../../base/common/buffer.js';
 import { CorpusReportNumbers, DIM_NAMES, decodeCorpusReport } from './traceRecordCodec.js';
@@ -165,4 +169,44 @@ export function decodeCandidateGroups(buf: VSBuffer, C: number, G: number): Grou
 			avgReward: withReward === 0 ? null : v.getFloat64(o + OFF_GRP_AVG_REWARD, true),
 		};
 	}));
+}
+
+const CANDIDATE_SPREAD_BYTES = 88;       // sizeof(struct apo_candidate_spread)
+const OFF_SPR_N = 0;
+const OFF_SPR_SUM_LO = 8;
+const OFF_SPR_SUM_HI = 16;
+const OFF_SPR_SUM_SQ = 24;
+const OFF_SPR_MEAN = 48;
+const OFF_SPR_REWARD_SUM_SQ = 56;
+const OFF_SPR_VARIANCE = 64;
+const OFF_SPR_STD_DEV = 72;
+const OFF_SPR_STD_ERR = 80;
+
+export interface CandidateSpread {
+	candidate: number;
+	n: number;                 // rewarded rollouts (== counts[c])
+	sum: bigint;               // exact sum of rint(finalReward * 2^52) over them
+	sumSq: bigint;             // exact sum of its squares
+	mean: number | null;       // == the candidate's score; null when n == 0
+	rewardSumSq: number;       // sumSq * 2^-104, rounded once
+	variance: number | null;   // sample variance of the rewards; null when n < 2
+	stdDev: number | null;
+	stdErr: number | null;     // standard error of mean
+}
+
+/** The reward spreads of a candidateSpread block (ApoScoreBlocks.candidateSpread) of C candidates. */
+export function decodeCandidateSpread(buf: VSBuffer, C: number): CandidateSpread[] {
+	if (C < 0 || C * CANDIDATE_SPREAD_BYTES > buf.byteLength) { throw new RangeError(`${C} candidate spreads do not fit the block`); }
+	return Array.from({ length: C }, (_, c) => {
+		const v = new DataView(buf.buffer.buffer, buf.buffer.byteOffset + c * CANDIDATE_SPREAD_BYTES, CANDIDATE_SPREAD_BYTES);
+		const n = u64(v, OFF_SPR_N);
+		const f = (o: number) => v.getFloat64(o, true);
+		const sumSq = v.getBigUint64(OFF_SPR_SUM_SQ, true) | (v.getBigUint64(OFF_SPR_SUM_SQ + 8, true) << 64n) |
+			(v.getBigUint64(OFF_SPR_SUM_SQ + 16, true) << 128n);
+		return {
+			candidate: c, n, sum: (v.getBigInt64(OFF_SPR_SUM_HI, true) << 64n) | v.getBigUint64(OFF_SPR_SUM_LO, true), sumSq,
+			mean: n === 0 ? null : f(OFF_SPR_MEAN), rewardSumSq: f(OFF_SPR_REWARD_SUM_SQ),
+			variance: n < 2 ? null : f(OFF_SPR_VARIANCE), stdDev: n < 2 ? null : f(OFF_SPR_STD_DEV), stdErr: n < 2 ? null : f(OFF_SPR_STD_ERR),
+		};
+	});
 }
