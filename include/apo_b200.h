@@ -294,7 +294,12 @@ int apo_score(apo_engine *e, const apo_score_opts *o, double *scores, uint64_t *
  * begin + one accumulate + finish.  finish may be called repeatedly within one session: the
  * candidate accumulators are exact integers that only ever grow by later accumulate calls, so
  * new records (a window that was not scored yet) can be added as they arrive and the ranking
- * refreshed without rescanning the old ones (incremental scoring). */
+ * refreshed without rescanning the old ones (incremental scoring).  Every exact sum stays exact
+ * for any number of accumulates (any number of host-streaming windows) while a candidate has
+ * fewer than 2^64 evaluations: the partials, the breakdown's dimension sums, the group scores'
+ * and the corpus reports' sums keep 32-bit limbs that accumulate never carries, so when a run of
+ * launches could take one past 2^63 a small carry kernel first rewrites every such sum to the same
+ * value with l0, l1 < 2^32 (a session of a few thousand accumulates launches none). */
 int apo_score_begin(apo_engine *e, uint32_t C_total);
 int apo_score_accumulate(apo_engine *e, const apo_score_opts *o, uint32_t cand_offset);
 int apo_score_finish(apo_engine *e, const apo_score_opts *o, double *scores, uint64_t *counts,
@@ -390,7 +395,8 @@ int apo_last_timing(const apo_engine *e, apo_timing *out);
 /* Exact partial sums of the last apo_score: per candidate the integer
  * sum_t rint(finalReward * 2^52) as three int64 limbs (value = l2*2^64 + l1*2^32 + l0)
  * and the count; 4*C int64 words.  Order-independent, hence identical for any grid,
- * shard or rank count. */
+ * shard or rank count.  The value is exact in sessions of any length; how it splits into limbs
+ * changes when a long session carries them (apo_score_begin). */
 int apo_debug_partials(apo_engine *e, int64_t *out, uint32_t C);
 /* The exception list of the Form T copy (see apo_dims_upload), for tests and diagnostics: *n_exceptions pairs {position in
  * the row, full index} of the evaluations whose index is >= 2^16, rows in order, sorted by position (xs, 2 words each), and

@@ -236,6 +236,7 @@ struct apo_engine {
 	std::vector<cudaEvent_t> k1_ev;      // start/stop pairs of the K1 launches of the current scoring call
 	size_t k1_used = 0;
 	uint32_t score_C = 0; bool scoring = false;
+	uint64_t limb_flushes = 0;           // bound on the flushes into any one limb triple since the call began or limb_guard carried
 	apo_timing timing{};
 	// the per-candidate passes (csrc/apo_cand.cu): their own words, never part of the accumulator vector
 	PassState pass[NPASS];
@@ -619,7 +620,7 @@ int begin_score(apo_engine *e, uint32_t C, bool whole = false) {
 	e->acc_clean_words = 0;                         // from here on the block is in use
 	*e->h_domain = 0u;                              // the previous call has been synchronised: no kernel writes it now
 	e->partials_src = e->nranks > 1 ? e->acc_joined.p : e->acc.p;
-	e->last_C = C; e->score_C = C; e->scoring = true; e->k1_used = 0;
+	e->last_C = C; e->score_C = C; e->scoring = true; e->k1_used = 0; e->limb_flushes = 0;
 	for (PassState &s : e->pass) s = PassState{};
 	e->timing = apo_timing{};
 	if (e->timing_on) CK(cudaEventRecord(e->ev[0], e->stream));
@@ -917,6 +918,27 @@ int launch_passes(apo_engine *e, const apo_score_opts *o, const Evals &ev, uint3
 		CK(apo::run_cand_spread(X, ev.form, recip, e->sm_count, e->stream));
 		e->timing.launches++;
 	}
+	return APO_OK;
+}
+
+// Before the launches over ev of an accumulate or a host-streaming window: when they could take a limb triple past
+// apo::LIMB_FLUSH_MAX flushes, carry every triple that accumulates across launches (the candidate partials and the armed passes'
+// sum words) first.  The scoring and pass kernels stay as they are; a session or call that stays under the bound launches nothing.
+int limb_guard(apo_engine *e, const Evals &ev) {
+	const uint64_t b = apo::limb_flush_bound(ev.count, e->sm_count);
+	if (e->limb_flushes + b > apo::LIMB_FLUSH_MAX) {
+		const uint32_t C = e->score_C;
+		CK(apo::run_carry_limbs(e->acc.p, C, ACC_PER_CAND, 0, 1, e->stream));
+		e->timing.launches++;
+		if (e->pass[PASS_CAND].armed) { CK(apo::run_carry_limbs(e->cand_acc.p, C, apo::CB_INT, apo::CB_DIM, APO_NDIM, e->stream)); e->timing.launches++; }
+		if (e->pass[PASS_CCORP].armed) {                                // CORP_REWARD (word 0) and the nine CORP_DIM triples behind it
+			CK(apo::run_carry_limbs(e->ccorp_acc.p, C, apo::CC_WORDS, 0, 1 + APO_NDIM, e->stream));
+			e->timing.launches++;
+		}
+		if (e->pass[PASS_GRP].armed) { CK(apo::run_carry_limbs(e->grp_acc.p, (uint64_t)C * e->grp_arm_G, apo::GR_WORDS, 0, 1, e->stream)); e->timing.launches++; }
+		e->limb_flushes = 0;
+	}
+	e->limb_flushes += b;
 	return APO_OK;
 }
 
@@ -2128,7 +2150,7 @@ extern "C" int apo_score_accumulate(apo_engine *e, const apo_score_opts *o, uint
 	for (int p = 0; p < NPASS; p++)                     // allocates: before route_copy
 		if (wants(o, p) && e->pass[p].every && !e->pass[p].armed && (rc = pass_arm(e, p, e->score_C))) return rc;
 	if ((rc = route_copy(e, o, &ev))) return rc;
-	if ((rc = resident_window(e, o, &ev)) || (rc = launch_score(e, o, ev, cand_offset))) return rc;
+	if ((rc = resident_window(e, o, &ev)) || (rc = limb_guard(e, ev)) || (rc = launch_score(e, o, ev, cand_offset))) return rc;
 	for (int p = 0; p < NPASS; p++)                     // a pass this accumulate does not flag: finish refuses it
 		if (!wants(o, p)) e->pass[p].every = false;
 	return launch_passes(e, o, ev, cand_offset);
@@ -2337,7 +2359,7 @@ int stream_host(apo_engine *e, const apo_score_opts *o, const HostTensor &h, dou
 			                     code_ok[1], e->unpack_bad.p, (unsigned long long *)w, (float *)(w + CTc * 8), (unsigned short *)(w + CTc * 12), Tc, e->stream));
 			e->timing.launches++;
 		}
-		if ((rc = launch_score(e, o, ev, 0)) || (rc = launch_passes(e, o, ev, 0))) return rc;   // before the window is released
+		if ((rc = limb_guard(e, ev)) || (rc = launch_score(e, o, ev, 0)) || (rc = launch_passes(e, o, ev, 0))) return rc;   // before the window is released
 		CK(cudaEventRecord(e->win_free[b], e->stream));
 	}
 	return finish_score(e, o, C, scores, counts, topk, report, false, h.packed);

@@ -641,7 +641,8 @@ static cudaError_t launch_pass(const CandExtParams &X, int sm_count, cudaStream_
 // the warp's own shared accumulators of that label.  A term rint(fr * 2^52) enters as four 16-bit pieces of its two's
 // complement and a sign count, so 32 of them sum exactly in 32 bits whatever the labels are; the warp's accumulators hold a
 // run of CB_RUN_TILES tiles exactly (l0, l1 < 2^58, counts < 2^27) and are flushed into the (c, g) words when the candidate
-// changes and at the breakdown's run limit.
+// changes and at the breakdown's run limit.  A flush forms the run's signed sum l0 + 2^32 l1 - 2^64 neg (|sum| < 2^123) and
+// adds it in the scoring partials' limb split (add_i128): words 0 and 1 grow by < 2^32 per flush, as the host bounds them.
 struct GroupSmem {
 	unsigned long long l0[CB_WARPS][APO_GROUPS_MAX], l1[CB_WARPS][APO_GROUPS_MAX];   // 2^0 and 2^32 limbs of the sum
 	uint32_t n[CB_WARPS][APO_GROUPS_MAX], good[CB_WARPS][APO_GROUPS_MAX], bad[CB_WARPS][APO_GROUPS_MAX];
@@ -670,11 +671,9 @@ k_cand_groups(const CandGroupParams X, uint32_t tiles_per_cand, uint64_t total_t
 		__syncwarp();
 		for (uint32_t g = lane; g < G; g += 32) {
 			unsigned long long *w = (unsigned long long *)X.words + ((uint64_t)c * G + g) * GR_WORDS;
-			const unsigned long long a0 = A.l0[wp][g], a1 = A.l1[wp][g];
 			const uint32_t neg = A.neg[wp][g], rew = A.rew[wp][g], n = A.n[wp][g], good = A.good[wp][g], bad = A.bad[wp][g];
-			if (a0) atomicAdd(w + 0, a0);
-			if (a1) atomicAdd(w + 1, a1);
-			if (neg) atomicAdd(w + 2, 0ull - (unsigned long long)neg);   // each negative term carries -2^64
+			// each negative term carries -2^64
+			add_i128((long long *)w, (__int128)A.l0[wp][g] + ((__int128)A.l1[wp][g] << 32) - ((__int128)neg << 64));
 			if (rew) atomicAdd(w + 3, (unsigned long long)rew);
 			if (n) atomicAdd(w + GR_TALLY, (unsigned long long)n);
 			if (good) atomicAdd(w + GR_TALLY + 1, (unsigned long long)good);
@@ -734,10 +733,7 @@ k_cand_groups_report(const long long *words, uint64_t n, apo_group_score *out) {
 	R.bad = (uint64_t)w[GR_TALLY + 2];
 	R.goodRate = report_good_rate(R.good, R.bad);
 	R.withReward = (uint64_t)w[3];
-	// l0 and l1 hold sums of unsigned 32-bit limbs: carry them into the signed limbs limbs_to_double reads
-	const __int128 v = ((__int128)w[2] << 64) + ((__int128)(unsigned long long)w[1] << 32) + (__int128)(unsigned long long)w[0];
-	const long long l[3] = {(long long)(v & 0xFFFFFFFF), (long long)((v >> 32) & 0xFFFFFFFF), (long long)(v >> 64)};
-	R.rewardSum = limbs_to_double(l);
+	R.rewardSum = limbs_to_double(w);                                   // the scoring partials' limbs, as k_cand_report reads them
 	R.avgReward = report_avg_reward(R.rewardSum, R.withReward);
 	out[i] = R;
 }
@@ -885,6 +881,37 @@ cudaError_t run_cand_spread_report(const unsigned long long *words, const long l
                                    cudaStream_t st) {
 	if (C == 0) return cudaSuccess;
 	k_cand_spread_report<<<(C + 255) / 256, 256, 0, st>>>(words, partials, C, out);
+	return cudaGetLastError();
+}
+
+// ================================================================ limb carry of the words that accumulate across launches
+// Every flush adds < 2^37 to the unsigned limbs l0 and l1 of a triple (flush_acc128: 32 lanes of < 2^32; add_i128: < 2^32),
+// which every reader takes as signed int64.  One launch adds at most limb_flush_bound flushes into any one candidate's triple:
+// one per warp (the scoring kernels run <= sm_count CTAs of <= 32 warps, the walks <= 64 resident warps per SM) plus the run
+// limit's (the shortest, k_cand_corpus's CC_RUN_TILES, in tiles of CB_TILE evaluations).  The host sums the bound over the
+// launches of a session or host-streaming call and, before it could pass LIMB_FLUSH_MAX, rewrites every triple to its value
+// with l0, l1 < 2^32 (k_carry_limbs): then l0, l1 < 2^32 + LIMB_FLUSH_MAX * 2^37 < 2^63 at every read.
+uint64_t limb_flush_bound(uint64_t count, int sm_count) {
+	const uint64_t tiles = (count + CB_TILE - 1) / CB_TILE;
+	return 64ull * (uint64_t)sm_count + tiles / CC_RUN_TILES + 1;
+}
+
+// one thread per triple: w + r * row_words + first + 4 k for r < rows, k < per_row
+__global__ void __launch_bounds__(256)
+k_carry_limbs(long long *w, uint64_t n, uint32_t row_words, uint32_t first, uint32_t per_row) {
+	const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+	if (i >= n) return;
+	long long *l = w + (i / per_row) * row_words + first + 4 * (i % per_row);
+	const __int128 v = ((__int128)l[2] << 64) + ((__int128)l[1] << 32) + (__int128)l[0];
+	l[0] = (long long)(v & 0xFFFFFFFF);
+	l[1] = (long long)((v >> 32) & 0xFFFFFFFF);
+	l[2] = (long long)(v >> 64);
+}
+
+cudaError_t run_carry_limbs(long long *w, uint64_t rows, uint32_t row_words, uint32_t first, uint32_t per_row, cudaStream_t st) {
+	const uint64_t n = rows * per_row;
+	if (n == 0) return cudaSuccess;
+	k_carry_limbs<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(w, n, row_words, first, per_row);
 	return cudaGetLastError();
 }
 

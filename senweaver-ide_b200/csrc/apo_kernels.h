@@ -394,7 +394,8 @@ cudaError_t run_cand_extremes(const CandExtParams &P, int source, bool recip, in
 
 // ---- per-candidate group scores (csrc/apo_cand.cu): every candidate's evaluations split by the label of their record.
 // Own buffer [C][G][GR_WORDS]: l0, l1, l2, withReward (the scoring partials' layout: the exact sum of rint(fr * 2^52) is
-// l2 * 2^64 + l1 * 2^32 + l0), then total, good, bad and one unused word.
+// l2 * 2^64 + l1 * 2^32 + l0, every flush adding its signed sum's 32-bit limbs to l0 and l1 and the rest to l2, and
+// run_carry_limbs bounding l0 and l1 across launches as it bounds the partials'), then total, good, bad and one unused word.
 constexpr int GR_WORDS = 8;
 constexpr int GR_TALLY = 4;
 struct CandGroupParams {
@@ -421,6 +422,15 @@ cudaError_t run_cand_spread(const CandSpreadParams &P, int source, bool recip, i
 // words: the whole buffer; partials: the scoring call's candidate accumulators (4 words per candidate)
 cudaError_t run_cand_spread_report(const unsigned long long *words, const long long *partials, uint32_t C, struct apo_candidate_spread *out,
                                    cudaStream_t st);
+
+// ---- limb carry (csrc/apo_cand.cu): the (l0, l1, l2) triples that accumulate across the launches of a session or of a
+// host-streaming call (the candidate partials, the breakdown's dimension words, the group words, the per-candidate corpus
+// blocks' reward and dimension words) stay exact while l0 and l1 < 2^63.  limb_flush_bound: the most flushes one launch over
+// `count` evaluations per candidate adds into one candidate's triple; LIMB_FLUSH_MAX: the most flushes a triple takes after
+// run_carry_limbs has rewritten it (every triple w + r * row_words + first + 4 k, r < rows, k < per_row) to l0, l1 < 2^32.
+constexpr uint64_t LIMB_FLUSH_MAX = (1ull << 26) - 1;
+uint64_t limb_flush_bound(uint64_t count, int sm_count);
+cudaError_t run_carry_limbs(long long *w, uint64_t rows, uint32_t row_words, uint32_t first, uint32_t per_row, cudaStream_t st);
 
 int k1_tile_evals(int row, int variant);
 cudaError_t run_reward9(K1Params P, int row, int variant, bool recip, int sm_count, cudaStream_t st);
