@@ -27,6 +27,13 @@ parity block holds n and S1 of every candidate against apo_debug_partials (and m
 the spreads of two of the 8 candidates against the exact model of tests/spread_fixtures.py over the generated rows (every
 field bit for bit), and on the rollout legs R16 and R give the same bytes.
 
+Every leg also times the step with the paired comparison (APO_SCORE_CANDIDATE_PAIRS) in the same alternation, under refs
+shaped like a beam: each candidate names the first candidate of its block of 5, which names none (the refs are uploaded once
+per leg, outside the timing).  Its parity block holds the invariants of tests/pair_fixtures.py on every candidate (n + candOnly
+and n + refOnly against counts[], wins + losses + ties == n, nothing for a candidate without a reference); on the fp32 legs
+also the pairs of two candidates against the exact model of tests/pair_fixtures.py over the generated rows (every field bit
+for bit), and on the rollout legs R16 and R give the same bytes.
+
     python examples/candidates_cost.py [--steps 10] [--legs D,W,Q,T,R16,R,FALL] [--out FILE.json]
 
 Prints one JSON object; the card name and power limit are read in the same run (nvidia-smi query)."""
@@ -149,6 +156,46 @@ def spread_block(eng, last, med, ref_spr):
             "parity_spread": spread_parity(eng, last["spread"], ref_spr)}
 
 
+def beam_refs(C):
+    """each candidate names the first candidate of its block of 5 (a parent and its four children), which names none"""
+    import pair_fixtures as pf
+    return np.array([pf.NONE if c % 5 == 0 else c - c % 5 for c in range(C)], np.uint32)
+
+
+def pair_row(p):
+    return (int(p.ref), int(p.n), int(p.wins), int(p.losses), int(p.ties), int(p.candOnly), int(p.refOnly), p.sum, p.sum_sq,
+            bits(p.meanDiff), bits(p.variance), bits(p.stdDev), bits(p.stdErr))
+
+
+def model_pair(m):
+    return (m["ref"], m["n"], m["wins"], m["losses"], m["ties"], m["candOnly"], m["refOnly"], m["D1"], m["D2"], bits(m["meanDiff"]),
+            bits(m["variance"]), bits(m["stdDev"]), bits(m["stdErr"]))
+
+
+def pairs_parity(res, ref_pair):
+    """the invariants on every candidate against the call's counts; ref_pair: {candidate: model pair}"""
+    import pair_fixtures as pf
+    try:
+        pf.invariants(res.pairs, [int(x) for x in res.counts])
+        every = True
+    except AssertionError:
+        every = False
+    out = {"invariants_every_candidate": every}
+    if ref_pair:
+        ok = {c: pair_row(res.pairs[c]) == model_pair(m) for c, m in ref_pair.items()}
+        out.update({"candidates": list(ok), "per_candidate": ok})
+        every = every and all(ok.values())
+    out["equal"] = every
+    return out
+
+
+def pairs_block(last, med, ref_pair):
+    return {"pairs_ms_median": round(med["pairs"], 3), "pairs_ratio": round(med["pairs"] / med["plain"], 3),
+            "pairs_same_scores": last["pairs"].scores.tobytes() == last["plain"].scores.tobytes()
+                                 and last["pairs"].topk.tobytes() == last["plain"].topk.tobytes(),
+            "parity_pairs": pairs_parity(last["pairs"], ref_pair)}
+
+
 def timed(eng, C, K, steps, score_kw, kinds, sets):
     """median / min of every kind of step, alternating; a group step first uploads its labels (outside the timing)"""
     times = {k: [] for k in kinds}
@@ -178,10 +225,11 @@ def groups_block(last, med, sets, ref_grp):
             "parity_groups": groups_parity(last, sets, ref_grp)}
 
 
-def leg(eng, C, K, steps, score_kw, ref, picks, ref_ext=None, sets=None, ref_grp=None, ref_spr=None):
-    """plain / candidates / extremes / groups / spread steps, alternating (ref None: the breakdown is not timed)"""
+def leg(eng, C, K, steps, score_kw, ref, picks, ref_ext=None, sets=None, ref_grp=None, ref_spr=None, ref_pair=None):
+    """plain / candidates / extremes / groups / spread / pairs steps, alternating (ref None: the breakdown is not timed)"""
     sets = sets or {}
-    kinds = {"plain": {}, "extremes": {"extremes": True}, "spread": {"spread": True}}
+    kinds = {"plain": {}, "extremes": {"extremes": True}, "spread": {"spread": True}, "pairs": {"pairs": True}}
+    eng.candidate_refs_upload(beam_refs(C))
     if ref is not None:
         kinds["candidates"] = {"candidates": True}
     kinds.update({k: {"groups": True} for k in sets})
@@ -194,6 +242,7 @@ def leg(eng, C, K, steps, score_kw, ref, picks, ref_ext=None, sets=None, ref_grp
            "parity_extremes": extremes_parity(last["extremes"], ref_ext)}
     out.update(groups_block(last, med, sets, ref_grp))
     out.update(spread_block(eng, last, med, ref_spr))
+    out.update(pairs_block(last, med, ref_pair))
     if ref is not None:
         r = last["candidates"]
         ok = [same(r.candidates[c], d) for c, d in zip(picks, ref)]
@@ -242,9 +291,10 @@ def parity_block(picks, diffs):
 
 
 def corpus_leg(eng, C, K, steps, score_kw, ref, picks, ref_corpus, sets):
-    """plain / candidates / candidate_corpus / extremes / groups / spread steps, alternating, with the parity blocks"""
+    """plain / candidates / candidate_corpus / extremes / groups / spread / pairs steps, alternating, with the parity blocks"""
     kinds = {"plain": {}, "candidates": {"candidates": True}, "candidate_corpus": {"candidate_corpus": True}, "extremes": {"extremes": True},
-             "spread": {"spread": True}}
+             "spread": {"spread": True}, "pairs": {"pairs": True}}
+    eng.candidate_refs_upload(beam_refs(C))
     kinds.update({k: {"groups": True} for k in sets})
     last, times, med = timed(eng, C, K, steps, score_kw, kinds, sets)
     ok = [same(last["candidates"].candidates[c], d) for c, d in zip(picks, ref)]
@@ -254,6 +304,7 @@ def corpus_leg(eng, C, K, steps, score_kw, ref, picks, ref_corpus, sets):
     seq = [seq_corpus_diff(cc[c], d) for c, d in zip(picks, ref_corpus["seq"])]
     return {**groups_block(last, med, sets, None), "groups_bytes": b"".join(bytes(last[k].groups) for k in sets),
             **spread_block(eng, last, med, None), "spread_bytes": bytes(last["spread"].spread),
+            **pairs_block(last, med, None), "pairs_bytes": bytes(last["pairs"].pairs),
             "plain_ms_median": round(med["plain"], 3), "candidates_ms_median": round(med["candidates"], 3),
             "candidate_corpus_ms_median": round(med["candidate_corpus"], 3),
             "candidates_ratio": round(med["candidates"] / med["plain"], 3),
@@ -281,6 +332,7 @@ def main():
     import extremes_fixtures as xf
     import group_fixtures as gf
     import spread_fixtures as sf
+    import pair_fixtures as pf
     legs = args.legs.split(",")
     out = {"card": card(), "steps": args.steps, "timing": "host clock around each synchronous apo_score call"}
     eng = pkg.Engine(0)
@@ -298,18 +350,24 @@ def main():
                 ref_grp[c] = {k: gf.model(d, lab, G)[0] for k, (lab, G) in sets.items()}
                 ref_spr[c] = sf.model(d)[0]
                 del d
+            refs, ref_pair = beam_refs(C), {}
+            for c in (1, C - 2):                            # a child of candidate 0 and one of the last block's
+                r = int(refs[c])
+                d = np.concatenate([oracle.gen_dims(seed, c, 1, 0, T, 300, nth), oracle.gen_dims(seed, r, 1, 0, T, 300, nth)])
+                ref_pair[c] = pf.model(d, [1, pf.NONE])[0] | {"ref": r}
+                del d
             if "D" in legs:
                 eng.dims_generate(seed, 0, C, 0, T, 300)
-                out["form_d_256x5M"] = leg(eng, C, K, args.steps, {}, ref, picks, ref_ext, sets, ref_grp, ref_spr)
+                out["form_d_256x5M"] = leg(eng, C, K, args.steps, {}, ref, picks, ref_ext, sets, ref_grp, ref_spr, ref_pair)
             if "W" in legs:
                 eng.dims_generate(seed, 0, C, 0, T, 300)
                 eng.set_tuning(pkg.TUNE_NO_TWIN_T)
-                out["form_w_copy_256x5M"] = leg(eng, C, K, args.steps, {}, ref, picks, ref_ext, sets, ref_grp, ref_spr)
+                out["form_w_copy_256x5M"] = leg(eng, C, K, args.steps, {}, ref, picks, ref_ext, sets, ref_grp, ref_spr, ref_pair)
                 eng.set_tuning(0)
             if "Q" in legs or "T" in legs:
                 eng.dims_generate_compact(seed, 0, C, 0, T, 300)
             if "Q" in legs:
-                out["form_q_256x5M"] = leg(eng, C, K, args.steps, {}, ref, picks, ref_ext, sets, ref_grp, ref_spr)
+                out["form_q_256x5M"] = leg(eng, C, K, args.steps, {}, ref, picks, ref_ext, sets, ref_grp, ref_spr, ref_pair)
             if "T" in legs:
                 pc, pd = np.empty((C, T), np.uint32), np.empty((C, T), np.uint16)
                 for c in range(C):
@@ -319,7 +377,7 @@ def main():
                 del pc, pd
                 eng.tuples_upload(tl, th, tbook, book, d2book)
                 del tl, th
-                out["form_t_256x5M"] = leg(eng, C, K, args.steps, {"source": pkg.SRC_TUPLES}, ref, picks, ref_ext, sets, ref_grp, ref_spr)
+                out["form_t_256x5M"] = leg(eng, C, K, args.steps, {"source": pkg.SRC_TUPLES}, ref, picks, ref_ext, sets, ref_grp, ref_spr, ref_pair)
         if {"R16", "R"} & set(legs):
             Cr = 128
             picks_r = [int(x) for x in np.linspace(0, Cr - 1, 8).round()]
@@ -337,10 +395,12 @@ def main():
                 out["r16_r_extremes_equal"] = out["form_r16_128x5M"]["extremes_bytes"] == out["form_r_128x5M"]["extremes_bytes"]
                 out["r16_r_groups_equal"] = out["form_r16_128x5M"]["groups_bytes"] == out["form_r_128x5M"]["groups_bytes"]
                 out["r16_r_spread_equal"] = out["form_r16_128x5M"]["spread_bytes"] == out["form_r_128x5M"]["spread_bytes"]
+                out["r16_r_pairs_equal"] = out["form_r16_128x5M"]["pairs_bytes"] == out["form_r_128x5M"]["pairs_bytes"]
             for k in ("form_r16_128x5M", "form_r_128x5M"):
                 out.get(k, {}).pop("extremes_bytes", None)
                 out.get(k, {}).pop("groups_bytes", None)
                 out.get(k, {}).pop("spread_bytes", None)
+                out.get(k, {}).pop("pairs_bytes", None)
         if "FALL" in legs:
             Cf, Tf = 64, 1_000_000
             d = xf.falling(Tf, 1)
@@ -350,7 +410,9 @@ def main():
             eng.dims_upload(np.repeat(d, Cf, axis=0))
             eng.set_tuning(pkg.TUNE_NO_TWIN)
             out["falling_rows_k1_64x1M"] = leg(eng, Cf, K, args.steps, {}, None, None, {0: m, Cf - 1: m}, sets_f, {0: mg, Cf - 1: mg},
-                                               {0: sf.model(d)[0], Cf - 1: sf.model(d)[0]})
+                                               {0: sf.model(d)[0], Cf - 1: sf.model(d)[0]},
+                                               {c: pf.model(np.concatenate([d, d]), [1, pf.NONE])[0] | {"ref": int(beam_refs(Cf)[c])}
+                                                for c in (1, Cf - 2)})
             eng.set_tuning(0)
     finally:
         eng.close()

@@ -539,6 +539,44 @@ struct apo_candidate_spread {
 	double   mean, rewardSumSq, variance, stdDev, stdErr;
 };                        /* 88 bytes */
 int apo_candidate_spread(apo_engine *e, uint32_t c0, uint32_t n, struct apo_candidate_spread *out);
+/* Paired comparison of every candidate with a reference candidate on the same rollouts: did c beat r on the records both were
+ * scored on, and by more than the noise?  Rewards on one record are correlated (its task is easy or hard for every prompt), so
+ * the noise of the gap, Var(x_c - x_r), is smaller than the spreads' unpaired standard errors say; only sums over both rows at
+ * every position give it.  The caller names one reference per candidate (apo_candidate_refs_upload): refs[c] is a candidate
+ * index < C, or APO_PAIR_NONE.  A scoring call that sets APO_SCORE_CANDIDATE_PAIRS compares each c that has a reference
+ * r = refs[c] with r at every record position the call scored, with x_t = rint(fr_t * 2^52) the int64 term it summed into
+ * scores[] (fr_t bit for bit the finalReward it summed, APO_SCORE_RECIP honoured).  Over the positions where both c and r have
+ * a non-null finalReward, d_t = x_c,t - x_r,t (|d| <= 2^62):
+ *   n = number of such positions; wins / losses / ties: positions with d_t > 0 / < 0 / == 0
+ *   candOnly / refOnly: positions where only c / only r has a non-null finalReward (left out of the sums: why meanDiff
+ *                       differs from scores[c] - scores[r])
+ *   D1 = sum d_t (exact, |D1| < 2^126),  D2 = sum d_t^2 (exact, < 2^192),  M = n * D2 - D1^2 (exact):
+ *   meanDiff = RN(RN(D1) * 2^-52 / (double)n), the sequence scores[c] is; NaN when n == 0
+ *   variance, stdDev, stdErr: the rules of apo_candidate_spread with (n, D1, D2) for (n, S1, S2)
+ * Positions are absolute record positions as for the extremes and group scores: a session covers every window it accumulated
+ * (a window accumulated twice counts twice), the host-streaming calls the positions of their T.  Works wherever
+ * APO_SCORE_CANDIDATE_SPREAD works, combines with the other per-candidate flags in any mix, and leaves every other output as
+ * it is without it.  Refusals, before anything is launched: APO_E_STATE when no refs are uploaded, on a handle with more than
+ * one rank, at a session's finish when an accumulate did not set the flag or the refs were uploaded again after the session
+ * began accumulating them; APO_E_ARG when the refs' C is not the call's C (C_total in a session), or when an accumulate of
+ * candidates [cand_offset, cand_offset + C) holds a candidate whose reference lies outside them. */
+#define APO_SCORE_CANDIDATE_PAIRS 0x100u /* also compare every candidate with its reference (apo_candidate_pairs) */
+#define APO_PAIR_NONE 0xFFFFFFFFu
+/* Holds refs[C] until the next upload, independent of dims / rollouts / corpus loads; C == 0 releases them.  APO_E_ARG (the
+ * previous refs stay) when refs is NULL or an entry is >= C and not APO_PAIR_NONE.  refs[c] == c is allowed: every position
+ * is a tie. */
+int apo_candidate_refs_upload(apo_engine *e, const uint32_t *refs, uint32_t C);
+struct apo_candidate_pair {
+	uint32_t ref, pad;    /* r, or APO_PAIR_NONE: then every count and sum is 0 and every double NaN */
+	uint64_t n, wins, losses, ties, candOnly, refOnly;
+	uint64_t sumLo;       /* D1 as a two's complement 128-bit integer: low word */
+	int64_t  sumHi;       /*                                           high word */
+	uint64_t sumSq[3];    /* D2, unsigned 192-bit, least significant word first */
+	double   meanDiff, variance, stdDev, stdErr;
+};                        /* 128 bytes */
+/* Pairs of candidates [c0, c0 + n) of the last scoring call: APO_E_STATE when that call did not set the flag (or failed),
+ * APO_E_ARG when the range exceeds its C. */
+int apo_candidate_pairs(apo_engine *e, uint32_t c0, uint32_t n, struct apo_candidate_pair *out);
 
 /* ---- multi-GPU: the record axis is sharded across ranks (one process per GPU, or one handle per GPU inside one
  * process); the packed int64 partial vectors of the shards are joined INSIDE the scoring launch: the finalising CTA

@@ -106,6 +106,10 @@ int apo_job_validate(apo_job *j)
 		if (j->buf_bytes && !j->buf) return bad(j, "labels buffer missing");
 		if (j->buf_bytes && (j->G == 0 || j->G > APO_GROUPS_MAX)) return bad(j, "G must be 1..64");
 		break;
+	case APO_JOB_CANDIDATE_REFS_UPLOAD:               /* buf_bytes = 4 C; C == 0 releases them */
+		if (j->buf_bytes && !j->buf) return bad(j, "refs buffer missing");
+		if (j->buf_bytes != 4ull * j->C) return bad(j, "refs byte length is not 4 x C");
+		break;
 	case APO_JOB_TEST_HOOK:
 		break;
 	default:
@@ -157,6 +161,14 @@ int apo_job_validate(apo_job *j)
 		if (!fits(j->C, sizeof(struct apo_candidate_spread), 1, APO_JOB_CANDIDATE_SPREAD_MAX_BYTES))
 			return bad(j, "the per-candidate reward spreads of C candidates exceed 4 GiB");
 	}
+	if (j->flags & APO_SCORE_CANDIDATE_PAIRS) {
+		if (j->kind != APO_JOB_SCORE_RESIDENT && j->kind != APO_JOB_SCORE_HOST && j->kind != APO_JOB_SCORE_HOST_RECORDS &&
+		    j->kind != APO_JOB_SCORE_HOST_TUPLES)
+			return bad(j, "the paired comparisons belong to a scoring call");
+		if (j->C == 0) return bad(j, "C must be > 0 for the paired comparisons");
+		if (!fits(j->C, sizeof(struct apo_candidate_pair), 1, APO_JOB_CANDIDATE_PAIRS_MAX_BYTES))
+			return bad(j, "the paired comparisons of C candidates exceed 4 GiB");
+	}
 	return APO_OK;
 }
 
@@ -174,11 +186,14 @@ int apo_job_prepare(apo_job *j)
 		if (j->flags & APO_SCORE_CANDIDATE_GROUPS) j->candidate_groups = (apo_group_score *)malloc(sizeof(apo_group_score) * (size_t)C * j->G);
 		if (j->flags & APO_SCORE_CANDIDATE_SPREAD)
 			j->candidate_spread = (struct apo_candidate_spread *)malloc(sizeof(struct apo_candidate_spread) * (size_t)C);
+		if (j->flags & APO_SCORE_CANDIDATE_PAIRS)
+			j->candidate_pairs = (struct apo_candidate_pair *)malloc(sizeof(struct apo_candidate_pair) * (size_t)C);
 		if (!j->scores || !j->counts || !j->topk || ((j->flags & APO_SCORE_CANDIDATES) && !j->candidates) ||
 		    ((j->flags & APO_SCORE_CANDIDATE_CORPUS) && !j->candidate_corpus) ||
 		    ((j->flags & APO_SCORE_CANDIDATE_EXTREMES) && !j->candidate_extremes) ||
 		    ((j->flags & APO_SCORE_CANDIDATE_GROUPS) && !j->candidate_groups) ||
-		    ((j->flags & APO_SCORE_CANDIDATE_SPREAD) && !j->candidate_spread)) {
+		    ((j->flags & APO_SCORE_CANDIDATE_SPREAD) && !j->candidate_spread) ||
+		    ((j->flags & APO_SCORE_CANDIDATE_PAIRS) && !j->candidate_pairs)) {
 			apo_job_release(j); j->rc = APO_E_NOMEM; snprintf(j->err, sizeof j->err, "out of host memory"); return APO_E_NOMEM;
 		}
 	} else if (j->kind == APO_JOB_REWARD_BATCH) {
@@ -195,8 +210,10 @@ void apo_job_release(apo_job *j)
 {
 	free(j->scores); free(j->counts); free(j->topk); free(j->dims_out); free(j->masks_out); free(j->finals_out); free(j->candidates);
 	free(j->candidate_corpus); free(j->candidate_extremes); free(j->candidate_groups); free(j->candidate_spread);
+	free(j->candidate_pairs);
 	j->scores = NULL; j->counts = NULL; j->topk = NULL; j->dims_out = NULL; j->masks_out = NULL; j->finals_out = NULL; j->candidates = NULL;
 	j->candidate_corpus = NULL; j->candidate_extremes = NULL; j->candidate_groups = NULL; j->candidate_spread = NULL;
+	j->candidate_pairs = NULL;
 }
 
 static void execute(apo_serial *s, apo_job *j)
@@ -259,6 +276,9 @@ static void execute(apo_serial *s, apo_job *j)
 	case APO_JOB_RECORD_GROUPS_UPLOAD:
 		j->rc = apo_record_groups_upload(e, (const uint8_t *)j->buf, j->buf_bytes, j->G);
 		break;
+	case APO_JOB_CANDIDATE_REFS_UPLOAD:
+		j->rc = apo_candidate_refs_upload(e, (const uint32_t *)j->buf, j->C);
+		break;
 	default:
 		j->rc = APO_E_ARG;
 	}
@@ -267,6 +287,7 @@ static void execute(apo_serial *s, apo_job *j)
 	if (j->rc == APO_OK && j->candidate_extremes) j->rc = apo_candidate_extremes(e, 0, j->C, j->candidate_extremes);
 	if (j->rc == APO_OK && j->candidate_groups) j->rc = apo_candidate_groups(e, 0, j->C, j->G, j->candidate_groups);
 	if (j->rc == APO_OK && j->candidate_spread) j->rc = apo_candidate_spread(e, 0, j->C, j->candidate_spread);
+	if (j->rc == APO_OK && j->candidate_pairs) j->rc = apo_candidate_pairs(e, 0, j->C, j->candidate_pairs);
 	if (j->rc != APO_OK) snprintf(j->err, sizeof j->err, "%s", apo_last_error(e));
 }
 

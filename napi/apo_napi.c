@@ -27,10 +27,11 @@
  *   corpusUploadJson(h, utf8:ArrayBuffer, idxBase)                          -> Promise<number>   (records)
  *   dimsTuples(h, cap?)                                                     -> Promise<number>   (nTuples) resident Form T from the loaded dims
  *   recordGroupsUpload(h, labels:ArrayBuffer u8[T], G)                      -> Promise<void>     the record group of every position
- *   scoreResident(h, {C, K, source, corpus, first, count, candidates, candidateCorpus, candidateExtremes, candidateGroups, candidateSpread}) -> Promise<blocks>   ... scored many times
- *   score(h, dims, C, T, corpus|null, K, candidates?, candidateExtremes?, candidateGroups?, candidateSpread?) -> Promise<blocks>   host streaming, Form D
- *   scoreHostRecords(h, recs, rowBytes, C, T, corpus|null, K, candidates?, candidateCorpus?, candidateExtremes?, candidateGroups?, candidateSpread?) -> Promise<blocks>   host streaming, trace records
- *   scoreHostTuples(h, {tl, th, ...}, C, T, corpus|null, K, candidates?, candidateExtremes?, candidateGroups?, candidateSpread?) -> Promise<blocks>   host streaming, Form T
+ *   candidateRefsUpload(h, refs:ArrayBuffer u32[C])                          -> Promise<void>     the reference of every candidate
+ *   scoreResident(h, {C, K, source, corpus, first, count, candidates, candidateCorpus, candidateExtremes, candidateGroups, candidateSpread, candidatePairs}) -> Promise<blocks>   ... scored many times
+ *   score(h, dims, C, T, corpus|null, K, candidates?, candidateExtremes?, candidateGroups?, candidateSpread?, candidatePairs?) -> Promise<blocks>   host streaming, Form D
+ *   scoreHostRecords(h, recs, rowBytes, C, T, corpus|null, K, candidates?, candidateCorpus?, candidateExtremes?, candidateGroups?, candidateSpread?, candidatePairs?) -> Promise<blocks>   host streaming, trace records
+ *   scoreHostTuples(h, {tl, th, ...}, C, T, corpus|null, K, candidates?, candidateExtremes?, candidateGroups?, candidateSpread?, candidatePairs?) -> Promise<blocks>   host streaming, Form T
  *   candidateGroups is the G the labels were uploaded with (0 / absent: no group scores)
  *   rewardBatch(h, recs:ArrayBuffer apo_record[n])                          -> Promise<{dims,masks,finals}>
  *   commUniqueId() -> ArrayBuffer(128) | null     commInit(h, nranks, rank, id) -> Promise<void>
@@ -43,7 +44,8 @@
  *             extremes),
  *             candidateGroups?:ArrayBuffer apo_group_score[C][G] (only when the call asked for the per-candidate group scores),
  *             candidateSpread?:ArrayBuffer struct apo_candidate_spread[C] (only when the call asked for the per-candidate reward
- *             spreads)}
+ *             spreads),
+ *             candidatePairs?:ArrayBuffer struct apo_candidate_pair[C] (only when the call asked for the paired comparisons)}
  */
 #include <stdint.h>
 #include <stdio.h>
@@ -153,6 +155,8 @@ static napi_value blocks_of(napi_env env, const apo_job *j)
 		napi_set_named_property(env, out, "candidateGroups", v);
 	if (j->candidate_spread && (v = copy_out(env, j->candidate_spread, sizeof(struct apo_candidate_spread) * (size_t)C)))
 		napi_set_named_property(env, out, "candidateSpread", v);
+	if (j->candidate_pairs && (v = copy_out(env, j->candidate_pairs, sizeof(struct apo_candidate_pair) * (size_t)C)))
+		napi_set_named_property(env, out, "candidatePairs", v);
 	return out;
 }
 
@@ -330,6 +334,19 @@ static napi_value RecordGroupsUpload(napi_env env, napi_callback_info info)
 	return submit(env, c, argv[0], c->job.buf ? argv[1] : NULL, NULL, "apo_record_groups_upload");
 }
 
+/* candidateRefsUpload(h, refs): apo_candidate_refs_upload with C = refs.byteLength / 4; an empty buffer releases them */
+static napi_value CandidateRefsUpload(napi_env env, napi_callback_info info)
+{
+	ARGS(2)
+	call_t *c = argc >= 1 ? new_call(env, argv[0], APO_JOB_CANDIDATE_REFS_UPLOAD) : NULL;
+	if (!c) return reject_now(env, "candidateRefsUpload: invalid handle");
+	if (argc < 2 || !get_buffer(env, argv[1], &c->job.buf, &c->job.buf_bytes) || c->job.buf_bytes % 4 || c->job.buf_bytes / 4 > 0xFFFFFFFFull)
+		arg_error(c, "candidateRefsUpload(handle, refs:ArrayBuffer u32[C])");
+	else
+		c->job.C = (uint32_t)(c->job.buf_bytes / 4);
+	return submit(env, c, argv[0], c->job.buf ? argv[1] : NULL, NULL, "apo_candidate_refs_upload");
+}
+
 static int opt_u32(napi_env env, napi_value obj, const char *key, uint32_t *out)
 {
 	bool has = false; napi_value v;
@@ -357,7 +374,7 @@ static int opt_bool_arg(napi_env env, napi_value v, int *out)
 }
 
 /* scoreResident(h, {C, K, source?, corpus?, first?, count?, candidates?, candidateCorpus?, candidateExtremes?, candidateGroups?,
- * candidateSpread?}): scores what dimsUpload / rolloutsUpload / corpusUpload left
+ * candidateSpread?, candidatePairs?}): scores what dimsUpload / rolloutsUpload / corpusUpload left
  * resident — "uploaded once, scored many times" (SURVEY 8b ownership row); nothing crosses PCIe but the result block. */
 static napi_value ScoreResident(napi_env env, napi_callback_info info)
 {
@@ -365,27 +382,29 @@ static napi_value ScoreResident(napi_env env, napi_callback_info info)
 	call_t *c = argc >= 1 ? new_call(env, argv[0], APO_JOB_SCORE_RESIDENT) : NULL;
 	if (!c) return reject_now(env, "scoreResident: invalid handle");
 	napi_valuetype t;
-	uint32_t corpus = 0, cands = 0, ccorp = 0, cext = 0, cspr = 0;
+	uint32_t corpus = 0, cands = 0, ccorp = 0, cext = 0, cspr = 0, cpair = 0;
 	if (argc < 2 || napi_typeof(env, argv[1], &t) != napi_ok || t != napi_object || !opt_u32(env, argv[1], "candidateGroups", &c->job.G) ||
 	    !opt_u32(env, argv[1], "C", &c->job.C) || !opt_u32(env, argv[1], "K", &c->job.K) || !opt_u32(env, argv[1], "source", &c->job.source) ||
 	    !opt_u32(env, argv[1], "corpus", &corpus) || !opt_u64(env, argv[1], "first", &c->job.first) || !opt_u64(env, argv[1], "count", &c->job.count) ||
 	    !opt_u32(env, argv[1], "candidates", &cands) || cands > 1 || !opt_u32(env, argv[1], "candidateCorpus", &ccorp) || ccorp > 1 ||
-	    !opt_u32(env, argv[1], "candidateExtremes", &cext) || cext > 1 || !opt_u32(env, argv[1], "candidateSpread", &cspr) || cspr > 1)
-		arg_error(c, "scoreResident(handle, {C:uint32, K:uint32, source?:0|1|2, corpus?:0|1, first?:uint53, count?:uint53, candidates?:0|1, candidateCorpus?:0|1, candidateExtremes?:0|1, candidateGroups?:G, candidateSpread?:0|1})");
+	    !opt_u32(env, argv[1], "candidateExtremes", &cext) || cext > 1 || !opt_u32(env, argv[1], "candidateSpread", &cspr) || cspr > 1 ||
+	    !opt_u32(env, argv[1], "candidatePairs", &cpair) || cpair > 1)
+		arg_error(c, "scoreResident(handle, {C:uint32, K:uint32, source?:0|1|2, corpus?:0|1, first?:uint53, count?:uint53, candidates?:0|1, candidateCorpus?:0|1, candidateExtremes?:0|1, candidateGroups?:G, candidateSpread?:0|1, candidatePairs?:0|1})");
 	if (c->job.C == 0) arg_error(c, "scoreResident: C (the number of uploaded candidates) is required");
 	if (c->job.K > c->job.C) arg_error(c, "scoreResident: K exceeds C");
 	c->job.flags = (corpus ? APO_SCORE_CORPUS : 0) | (cands ? APO_SCORE_CANDIDATES : 0) | (ccorp ? APO_SCORE_CANDIDATE_CORPUS : 0) |
-	               (cext ? APO_SCORE_CANDIDATE_EXTREMES : 0) | (c->job.G ? APO_SCORE_CANDIDATE_GROUPS : 0) | (cspr ? APO_SCORE_CANDIDATE_SPREAD : 0);
+	               (cext ? APO_SCORE_CANDIDATE_EXTREMES : 0) | (c->job.G ? APO_SCORE_CANDIDATE_GROUPS : 0) | (cspr ? APO_SCORE_CANDIDATE_SPREAD : 0) |
+	               (cpair ? APO_SCORE_CANDIDATE_PAIRS : 0);
 	return submit(env, c, argv[0], NULL, NULL, "apo_score");
 }
 
 static napi_value score_host_common(napi_env env, napi_callback_info info, apo_job_kind kind)
 {
 	const int rec = kind == APO_JOB_SCORE_HOST_RECORDS;
-	ARGS(12)
+	ARGS(13)
 	call_t *c = argc >= 1 ? new_call(env, argv[0], kind) : NULL;
 	if (!c) return reject_now(env, "score: invalid handle");
-	int cands = 0, ccorp = 0, cext = 0, cspr = 0;
+	int cands = 0, ccorp = 0, cext = 0, cspr = 0, cpair = 0;
 	const size_t base = rec ? 3 : 2;              /* index of C */
 	const size_t need = base + 4;                 /* ..., C, T, corpus, K */
 	int ok = argc >= need && get_buffer(env, argv[1], &c->job.buf, &c->job.buf_bytes);
@@ -401,11 +420,12 @@ static napi_value score_host_common(napi_env env, napi_callback_info info, apo_j
 	const size_t ext_at = rec ? need + 2 : need + 1;
 	if (ok && argc > ext_at) ok = opt_bool_arg(env, argv[ext_at], &cext);
 	if (ok && argc > ext_at + 1 && !is_nullish(env, argv[ext_at + 1])) ok = get_u32(env, argv[ext_at + 1], &c->job.G);
-	if (ok && argc > ext_at + 2) ok = opt_bool_arg(env, argv[ext_at + 2], &cspr);     /* the last optional argument */
+	if (ok && argc > ext_at + 2) ok = opt_bool_arg(env, argv[ext_at + 2], &cspr);
+	if (ok && argc > ext_at + 3) ok = opt_bool_arg(env, argv[ext_at + 3], &cpair);    /* the last optional argument */
 	c->job.flags = (cands ? APO_SCORE_CANDIDATES : 0) | (ccorp ? APO_SCORE_CANDIDATE_CORPUS : 0) | (cext ? APO_SCORE_CANDIDATE_EXTREMES : 0) |
-	               (c->job.G ? APO_SCORE_CANDIDATE_GROUPS : 0) | (cspr ? APO_SCORE_CANDIDATE_SPREAD : 0);
-	if (!ok) arg_error(c, rec ? "scoreHostRecords(handle, recs:ArrayBuffer, rowBytes:32|16, C:uint32, T:uint53, corpus:ArrayBuffer|null, K:uint32, candidates?:boolean, candidateCorpus?:boolean, candidateExtremes?:boolean, candidateGroups?:G, candidateSpread?:boolean)"
-	                          : "score(handle, dims:ArrayBuffer, C:uint32, T:uint53, corpus:ArrayBuffer|null, K:uint32, candidates?:boolean, candidateExtremes?:boolean, candidateGroups?:G, candidateSpread?:boolean)");
+	               (c->job.G ? APO_SCORE_CANDIDATE_GROUPS : 0) | (cspr ? APO_SCORE_CANDIDATE_SPREAD : 0) | (cpair ? APO_SCORE_CANDIDATE_PAIRS : 0);
+	if (!ok) arg_error(c, rec ? "scoreHostRecords(handle, recs:ArrayBuffer, rowBytes:32|16, C:uint32, T:uint53, corpus:ArrayBuffer|null, K:uint32, candidates?:boolean, candidateCorpus?:boolean, candidateExtremes?:boolean, candidateGroups?:G, candidateSpread?:boolean, candidatePairs?:boolean)"
+	                          : "score(handle, dims:ArrayBuffer, C:uint32, T:uint53, corpus:ArrayBuffer|null, K:uint32, candidates?:boolean, candidateExtremes?:boolean, candidateGroups?:G, candidateSpread?:boolean, candidatePairs?:boolean)");
 	return submit(env, c, argv[0], c->job.buf ? argv[1] : NULL, corpus, rec ? "apo_score_host_records" : "apo_score_host");
 }
 static napi_value Score(napi_env env, napi_callback_info info) { return score_host_common(env, info, APO_JOB_SCORE_HOST); }
@@ -492,12 +512,12 @@ static napi_value EncodeTuples(napi_env env, napi_callback_info info)
 }
 
 /* scoreHostTuples(h, {tl, th, tbookPc, tbookPd, codebook, d2book, nTuples}, C, T, corpus|null, K, candidates?, candidateExtremes?, candidateGroups?,
- * candidateSpread?) -> Promise<blocks>:
+ * candidateSpread?, candidatePairs?) -> Promise<blocks>:
  * the evaluations travel as 3-byte dictionary indices (Form T) instead of 36-byte fp32 rows; same integers, same result. */
 static napi_value ScoreHostTuples(napi_env env, napi_callback_info info)
 {
 	static const char *names[6] = {"tl", "th", "tbookPc", "tbookPd", "codebook", "d2book"};
-	ARGS(10)
+	ARGS(11)
 	call_t *c = argc >= 1 ? new_call(env, argv[0], APO_JOB_SCORE_HOST_TUPLES) : NULL;
 	if (!c) return reject_now(env, "scoreHostTuples: invalid handle");
 	napi_valuetype t;
@@ -513,14 +533,15 @@ static napi_value ScoreHostTuples(napi_env env, napi_callback_info info)
 		ok = get_buffer(env, argv[4], &c->job.corpus, &c->job.corpus_bytes);
 		corpus = ok ? argv[4] : NULL;
 	}
-	int cands = 0, cext = 0, cspr = 0;
+	int cands = 0, cext = 0, cspr = 0, cpair = 0;
 	if (ok && argc > 6) ok = opt_bool_arg(env, argv[6], &cands);
 	if (ok && argc > 7) ok = opt_bool_arg(env, argv[7], &cext);
 	if (ok && argc > 8 && !is_nullish(env, argv[8])) ok = get_u32(env, argv[8], &c->job.G);
 	if (ok && argc > 9) ok = opt_bool_arg(env, argv[9], &cspr);
+	if (ok && argc > 10) ok = opt_bool_arg(env, argv[10], &cpair);
 	c->job.flags = (cands ? APO_SCORE_CANDIDATES : 0) | (cext ? APO_SCORE_CANDIDATE_EXTREMES : 0) | (c->job.G ? APO_SCORE_CANDIDATE_GROUPS : 0) |
-	               (cspr ? APO_SCORE_CANDIDATE_SPREAD : 0);
-	if (!ok) arg_error(c, "scoreHostTuples(handle, {tl, th, tbookPc, tbookPd, codebook, d2book: ArrayBuffer, nTuples:uint32}, C:uint32, T:uint53, corpus:ArrayBuffer|null, K:uint32, candidates?:boolean, candidateExtremes?:boolean, candidateGroups?:G, candidateSpread?:boolean)");
+	               (cspr ? APO_SCORE_CANDIDATE_SPREAD : 0) | (cpair ? APO_SCORE_CANDIDATE_PAIRS : 0);
+	if (!ok) arg_error(c, "scoreHostTuples(handle, {tl, th, tbookPc, tbookPd, codebook, d2book: ArrayBuffer, nTuples:uint32}, C:uint32, T:uint53, corpus:ArrayBuffer|null, K:uint32, candidates?:boolean, candidateExtremes?:boolean, candidateGroups?:G, candidateSpread?:boolean, candidatePairs?:boolean)");
 	for (int i = 1; i < 6; i++)                                      /* the job reads these on a worker thread: keep them alive */
 		if (arr[i]) napi_create_reference(env, arr[i], 1, &c->keep[c->nkeep++]);
 	return submit(env, c, argv[0], arr[0], corpus, "apo_score_host_tuples");
@@ -601,6 +622,7 @@ NAPI_MODULE_INIT()
 	    {"corpusUploadJson", NULL, CorpusUploadJson, NULL, NULL, NULL, napi_default, NULL},
 	    {"dimsTuples", NULL, DimsTuples, NULL, NULL, NULL, napi_default, NULL},
 	    {"recordGroupsUpload", NULL, RecordGroupsUpload, NULL, NULL, NULL, napi_default, NULL},
+	    {"candidateRefsUpload", NULL, CandidateRefsUpload, NULL, NULL, NULL, napi_default, NULL},
 	    {"scoreResident", NULL, ScoreResident, NULL, NULL, NULL, napi_default, NULL},
 	    {"score", NULL, Score, NULL, NULL, NULL, napi_default, NULL},
 	    {"scoreHostRecords", NULL, ScoreHostRecords, NULL, NULL, NULL, napi_default, NULL},

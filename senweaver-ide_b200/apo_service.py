@@ -22,7 +22,7 @@ import uuid
 
 import numpy as np
 
-from .engine import DIM_NAMES, GROUPS_MAX, MODE_NAMES, SRC_DIMS, SRC_ROLLOUTS, Engine
+from .engine import DIM_NAMES, GROUPS_MAX, MODE_NAMES, PAIR_NONE, SRC_DIMS, SRC_ROLLOUTS, Engine
 from .jsfmt import js_substring, js_to_fixed
 from .trace_collector import TraceCollectorService
 
@@ -264,7 +264,20 @@ class APOService:
         if sp is not None:
             out["rewardStdDev"] = None if sp.n < 2 else float(sp.stdDev)
             out["scoreStdErr"] = None if sp.n < 2 else float(sp.stdErr)
+        pr = res.pairs[c] if getattr(res, "pairs", None) is not None else None
+        if pr is not None:
+            out["vsReference"] = None if pr.ref == PAIR_NONE else {
+                "reference": int(pr.ref), "pairedRollouts": int(pr.n), "wins": int(pr.wins), "losses": int(pr.losses), "ties": int(pr.ties),
+                "meanRewardDiff": None if pr.n == 0 else float(pr.meanDiff), "diffStdErr": None if pr.n < 2 else float(pr.stdErr)}
         return out
+
+    @staticmethod
+    def parentRefs(cands, carried):
+        """refs of a round's candidates for the paired comparison: each child (cands[carried:]) names its parent's index in
+        cands; the beam members carried over (cands[:carried], the seed among them) name none."""
+        index = {x["version"]: i for i, x in enumerate(cands)}
+        return np.array([PAIR_NONE if i < carried else index.get(x.get("parentVersion"), PAIR_NONE) for i, x in enumerate(cands)],
+                        np.uint32)
 
     @staticmethod
     def _checkGroups(groups):
@@ -327,7 +340,7 @@ class APOService:
 
     # ---- beam evaluation: the step the reference delegates to its backend --------------------------------
     def evaluateBeam(self, candidates, dims=None, rollouts=None, reports=False, patterns=False, extremes=False, groups=None,
-                     spread=False):
+                     spread=False, refs=None):
         """Score a beam of VersionedPromptTemplate candidates on their rollout outcomes and keep the
         top `beamWidth` (score desc, ties -> lower index), then apply the APO:1138-1166 update with the
         strict `>` adoption rule (APO:1159).  dims: float32 [C][T][9] (NaN = absent) or rollouts:
@@ -336,7 +349,9 @@ class APOService:
         report (res.candidate_corpus: problem patterns, per-mode tallies, tool totals).  extremes=True also lists every
         candidate's 32 lowest- and highest-reward rollouts (res.extremes).  groups=(labels, names) also splits every candidate's
         rollouts by record group (res.groups [C][G]): labels[t] < len(names) is the group of rollout index t.  spread=True also
-        builds every candidate's reward spread (res.spread: exact sums, variance, standard deviation and standard error).  The
+        builds every candidate's reward spread (res.spread: exact sums, variance, standard deviation and standard error).
+        refs (uint32 [C], a candidate index or PAIR_NONE each) also compares every candidate with its reference on the rollouts
+        both were scored on (res.pairs: wins, losses, ties, the exact paired sums, meanDiff and its standard error).  The
         adoption rule stays the strict `>` on the means."""
         try:
             C = len(candidates)
@@ -353,6 +368,9 @@ class APOService:
                 extra["groups"] = True
             if spread:
                 extra["spread"] = True
+            if refs is not None:
+                self._engine.candidate_refs_upload(refs)
+                extra["pairs"] = True
             if dims is not None:
                 self._engine.dims_upload(np.ascontiguousarray(dims, np.float32))
                 res = self._engine.score(C, K, source=SRC_DIMS, **extra)
@@ -373,7 +391,7 @@ class APOService:
             return None
 
     def runBeamSearch(self, seedPrompt, proposeCandidates, rolloutDims=None, rounds=None, withReports=False, rolloutRecords=None,
-                      withExtremes=False, rolloutGroups=None, withSpread=False):
+                      withExtremes=False, rolloutGroups=None, withSpread=False, withParentComparison=False):
         """Client-side round driver (SURVEY 8f rank 3) around the GPU top-K: each round expands every beam
         member into `branchFactor` children through the caller's `proposeCandidates(parent, n) -> [content]`
         hook (the LLM critique/edit step of APO:918-988 lives there), scores parents + children on
@@ -386,13 +404,17 @@ class APOService:
         caller scored it on; rolloutGroups=(labels, names) (which needs withReports=True too) adds the parent's byGroup, so that
         a label that marks a held-out part of the rollouts shows whether a child improved only where its critique looked;
         withSpread=True (which needs withReports=True too) adds the parent's rewardStdDev / scoreStdErr, so that the critique
-        can tell a lead from the noise of the rollouts.  Returns the final beam state."""
+        can tell a lead from the noise of the rollouts; withParentComparison=True (which needs withReports=True too) adds the
+        parent's vsReference: how it fared against its own parent on the rollouts that scored both (wins, losses, ties, the
+        mean reward difference and its paired standard error).  Returns the final beam state."""
         if (rolloutDims is None) == (rolloutRecords is None):
             raise ValueError("runBeamSearch needs exactly one of rolloutDims / rolloutRecords")
         if withExtremes and not withReports:
             raise ValueError("runBeamSearch: withExtremes needs withReports=True (the lists travel in the candidate reports)")
         if withSpread and not withReports:
             raise ValueError("runBeamSearch: withSpread needs withReports=True (the spreads travel in the candidate reports)")
+        if withParentComparison and not withReports:
+            raise ValueError("runBeamSearch: withParentComparison needs withReports=True (the comparisons travel in the candidate reports)")
         if rolloutGroups is not None:
             if not withReports:
                 raise ValueError("runBeamSearch: rolloutGroups needs withReports=True (the group scores travel in the candidate reports)")
@@ -410,12 +432,13 @@ class APOService:
                     counter += 1
                     cands.append({"version": f"v{counter}", "content": content, "score": None,
                                   "parentVersion": parent["version"], "createdAt": time.time() * 1000.0})
+            refs = self.parentRefs(cands, len(beam)) if withParentComparison else None
             if rolloutRecords is not None:
                 res = self.evaluateBeam(cands, rollouts=rolloutRecords(cands), reports=withReports, patterns=withReports,
-                                        extremes=withExtremes, groups=rolloutGroups, spread=withSpread)
+                                        extremes=withExtremes, groups=rolloutGroups, spread=withSpread, refs=refs)
             else:
                 res = self.evaluateBeam(cands, dims=rolloutDims(cands), reports=withReports, extremes=withExtremes, groups=rolloutGroups,
-                                        spread=withSpread)
+                                        spread=withSpread, refs=refs)
             if res is None:
                 break
             if withReports:

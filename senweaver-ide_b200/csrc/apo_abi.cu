@@ -159,13 +159,14 @@ const struct { const char *env; uint32_t bit; } kTuning[] = {
 
 // The per-candidate passes a scoring call can flag (csrc/apo_cand.cu), with the words of their messages.  tbook: the pass
 // reads every source, Form T through the 4-bit table (apo_engine::tbook).
-enum Pass { PASS_CAND, PASS_CCORP, PASS_EXT, PASS_GRP, PASS_SPREAD, NPASS };
+enum Pass { PASS_CAND, PASS_CCORP, PASS_EXT, PASS_GRP, PASS_SPREAD, PASS_PAIR, NPASS };
 const struct { uint32_t flag; const char *name, *joined, *every; bool tbook; } kPass[NPASS] = {
 	{APO_SCORE_CANDIDATES, "APO_SCORE_CANDIDATES", "the per-candidate breakdown is", "a breakdown", true},
 	{APO_SCORE_CANDIDATE_CORPUS, "APO_SCORE_CANDIDATE_CORPUS", "the per-candidate corpus reports are", "the reports", false},
 	{APO_SCORE_CANDIDATE_EXTREMES, "APO_SCORE_CANDIDATE_EXTREMES", "the per-candidate lists are", "the lists", true},
 	{APO_SCORE_CANDIDATE_GROUPS, "APO_SCORE_CANDIDATE_GROUPS", "the per-candidate group scores are", "the group scores", true},
-	{APO_SCORE_CANDIDATE_SPREAD, "APO_SCORE_CANDIDATE_SPREAD", "the per-candidate spreads are", "the spreads", true}};
+	{APO_SCORE_CANDIDATE_SPREAD, "APO_SCORE_CANDIDATE_SPREAD", "the per-candidate spreads are", "the spreads", true},
+	{APO_SCORE_CANDIDATE_PAIRS, "APO_SCORE_CANDIDATE_PAIRS", "the paired comparisons are", "the pairs", true}};
 
 // one pass's state through a call or session
 struct PassState {
@@ -254,6 +255,11 @@ struct apo_engine {
 	uint32_t grp_rep_G = 0, grp_arm_G = 0; uint64_t grp_arm_gen = 0;
 	DevBuf<unsigned long long> spread_acc;   // spread: [C][SP_WORDS] sums of squares of the call or session
 	DevBuf<struct apo_candidate_spread> spread_rep; // spreads of the last flagged call
+	// references of the paired comparison (apo_candidate_refs_upload): device copy the pass reads, host copy the chunk check reads
+	DevBuf<uint32_t> pair_refs; std::vector<uint32_t> pair_refs_host;
+	uint64_t pair_gen = 0, pair_arm_gen = 0;  // counts uploads: a session's pairs belong to the refs it armed with
+	DevBuf<unsigned long long> pair_acc;     // [C][PR_WORDS] words of the call or session
+	DevBuf<struct apo_candidate_pair> pair_rep;   // pairs of the last flagged call
 };
 
 namespace {
@@ -793,7 +799,8 @@ int launch_score(apo_engine *e, const apo_score_opts *o, const Evals &ev, uint32
 	return APO_OK;
 }
 
-// ---- the per-candidate passes (APO_SCORE_CANDIDATES, _CANDIDATE_CORPUS, _CANDIDATE_EXTREMES, _CANDIDATE_GROUPS, _CANDIDATE_SPREAD)
+// ---- the per-candidate passes (APO_SCORE_CANDIDATES, _CANDIDATE_CORPUS, _CANDIDATE_EXTREMES, _CANDIDATE_GROUPS, _CANDIDATE_SPREAD,
+// _CANDIDATE_PAIRS)
 bool wants(const apo_score_opts *o, int p) { return (o->flags & kPass[p].flag) != 0; }
 
 // a failed call or finish leaves no reports behind
@@ -814,18 +821,32 @@ int labels_check(apo_engine *e, uint64_t end) {
 	return APO_OK;
 }
 
+// the refs are held for the C candidates of the call, and those of candidates [c0, c0 + n) (an accumulate's chunk) lie inside them
+int refs_check(apo_engine *e, uint32_t C, uint32_t c0, uint32_t n) {
+	const std::vector<uint32_t> &r = e->pair_refs_host;
+	if (r.empty()) return fail(e, APO_E_STATE, "APO_SCORE_CANDIDATE_PAIRS: no references uploaded (apo_candidate_refs_upload)");
+	if (r.size() != C) return fail(e, APO_E_ARG, "APO_SCORE_CANDIDATE_PAIRS: the references are for C=%zu candidates, the call scores C=%u", r.size(), C);
+	for (uint32_t c = c0; c < c0 + n; c++)
+		if (r[c] != APO_PAIR_NONE && (r[c] < c0 || r[c] >= c0 + n))
+			return fail(e, APO_E_ARG, "APO_SCORE_CANDIDATE_PAIRS: candidate %u names reference %u outside the candidates [%u,%u) this call loads", c, r[c],
+			            c0, c0 + n);
+	return APO_OK;
+}
+
 // score_check's T for the host-streaming calls (they take no window) and for apo_score_finish (each accumulate checked its own)
 constexpr uint64_t kStreamed = ~0ull, kSession = ~0ull - 1;
 
 // The refusals of the flagged passes, in pass order.  records: the call reads trace records; end: one past the last record
-// position it scores (0: a session's finish; kStreamed: not known yet, the host-streaming calls check the labels themselves).
-int passes_check(apo_engine *e, const apo_score_opts *o, bool records, uint64_t end) {
+// position it scores (0: a session's finish; kStreamed: not known yet, the host-streaming calls check the labels themselves);
+// C: the candidates of the call (C_total in a session), of which it loads [c0, c0 + n).
+int passes_check(apo_engine *e, const apo_score_opts *o, bool records, uint64_t end, uint32_t C, uint32_t c0, uint32_t n) {
 	for (int p = 0; p < NPASS; p++) {
 		if (!wants(o, p)) continue;
 		if (p == PASS_CCORP && !records) return refuse_no_records(e);
 		if (e->nranks > 1)
 			return fail(e, APO_E_STATE, "%s is single-rank only: %s not joined across the %d ranks of this handle", kPass[p].name, kPass[p].joined, e->nranks);
 		if (p == PASS_GRP && end != kStreamed) { const int rc = labels_check(e, end); if (rc) return rc; }
+		if (p == PASS_PAIR) { const int rc = refs_check(e, C, c0, n); if (rc) return rc; }
 	}
 	return APO_OK;
 }
@@ -840,6 +861,7 @@ int pass_reserve(apo_engine *e, int p, uint32_t C) {
 	case PASS_EXT: CK(reserve(e, e->ext_acc, ((uint64_t)C + apo::cand_ext_slots(e->sm_count, C)) * apo::CX_WORDS)); break;
 	case PASS_GRP: CK(reserve(e, e->grp_acc, (uint64_t)(C ? C : 1) * e->grp_G * apo::GR_WORDS)); break;
 	case PASS_SPREAD: CK(reserve(e, e->spread_acc, (uint64_t)(C ? C : 1) * apo::SP_WORDS)); break;
+	case PASS_PAIR: CK(reserve(e, e->pair_acc, (uint64_t)(C ? C : 1) * apo::PR_WORDS)); break;
 	}
 	if (kPass[p].tbook) CK(reserve(e, e->tbook, 8 * 16));
 	return APO_OK;
@@ -857,6 +879,10 @@ int pass_arm(apo_engine *e, int p, uint32_t C) {
 		e->grp_arm_G = e->grp_G; e->grp_arm_gen = e->grp_gen;
 		break;
 	case PASS_SPREAD: CK(cudaMemsetAsync(e->spread_acc.p, 0, (uint64_t)C * apo::SP_WORDS * 8, e->stream)); break;
+	case PASS_PAIR:                                                 // the words then belong to the refs held now
+		CK(cudaMemsetAsync(e->pair_acc.p, 0, (uint64_t)C * apo::PR_WORDS * 8, e->stream));
+		e->pair_arm_gen = e->pair_gen;
+		break;
 	}
 	e->pass[p].armed = true;
 	return APO_OK;
@@ -872,11 +898,12 @@ int upload_tbook(apo_engine *e, const uint32_t *codebook) {
 }
 
 // The flagged passes over ev into candidates [cand_offset, ...), behind its scoring launch.  A pass that an accumulate of the
-// session did not flag, or whose group words belong to labels uploaded since, is left out: apo_score_finish refuses it.
+// session did not flag, or whose group (pair) words belong to labels (refs) uploaded since, is left out: apo_score_finish
+// refuses it.
 int launch_passes(apo_engine *e, const apo_score_opts *o, const Evals &ev, uint32_t cand_offset) {
 	bool run[NPASS], any = false;
 	for (int p = 0; p < NPASS; p++) {
-		run[p] = wants(o, p) && e->pass[p].every && (p != PASS_GRP || e->grp_arm_gen == e->grp_gen);
+		run[p] = wants(o, p) && e->pass[p].every && (p != PASS_GRP || e->grp_arm_gen == e->grp_gen) && (p != PASS_PAIR || e->pair_arm_gen == e->pair_gen);
 		any |= run[p];
 	}
 	if (!any || !ev.count) return APO_OK;
@@ -916,6 +943,11 @@ int launch_passes(apo_engine *e, const apo_score_opts *o, const Evals &ev, uint3
 	if (run[PASS_SPREAD]) {
 		const apo::CandSpreadParams X{S, e->W, e->spread_acc.p + (uint64_t)apo::SP_WORDS * cand_offset};
 		CK(apo::run_cand_spread(X, ev.form, recip, e->sm_count, e->stream));
+		e->timing.launches++;
+	}
+	if (run[PASS_PAIR]) {                                           // refs of this launch's candidates, mapped to its rows by the kernel
+		const apo::CandPairParams X{S, e->W, e->pair_refs.p + cand_offset, cand_offset, e->pair_acc.p + (uint64_t)apo::PR_WORDS * cand_offset};
+		CK(apo::run_cand_pairs(X, ev.form, recip, e->sm_count, e->stream));
 		e->timing.launches++;
 	}
 	return APO_OK;
@@ -968,6 +1000,11 @@ int finish_passes(apo_engine *e, const apo_score_opts *o, uint32_t C) {
 		CK(reserve(e, e->spread_rep, C ? C : 1));
 		const long long *partials = e->partials_src ? e->partials_src : e->acc.p;
 		CK(apo::run_cand_spread_report(e->spread_acc.p, partials, C, e->spread_rep.p, e->stream));
+		e->timing.launches++;
+	}
+	if (wants(o, PASS_PAIR)) {                                      // words + refs -> apo_candidate_pair[C]
+		CK(reserve(e, e->pair_rep, C ? C : 1));
+		CK(apo::run_cand_pair_report(e->pair_acc.p, e->pair_refs.p, C, e->pair_rep.p, e->stream));
 		e->timing.launches++;
 	}
 	uint32_t dom = 0;                                               // k_cand_breakdown's domain word (pageable: the copy waits for the stream)
@@ -1129,7 +1166,7 @@ int score_check(apo_engine *e, const apo_score_opts *o, uint32_t C, uint64_t T, 
 		return rc;
 	}
 	const uint64_t end = T == kStreamed ? kStreamed : T == kSession ? 0 : o->count ? o->first + o->count : T;
-	if ((rc = passes_check(e, o, records, end))) return rc;
+	if ((rc = passes_check(e, o, records, end, C, 0, C))) return rc;
 	CK(cudaSetDevice(e->device));
 	if (T == kSession) return APO_OK;                               // a session's scratch was sized by apo_score_begin
 	if ((rc = ensure_scratch(e, C, o->K))) return rc;
@@ -1722,6 +1759,7 @@ extern "C" void apo_destroy(apo_engine *e) {
 	e->cand_acc.release(); e->cand_rep.release(); e->tbook.release(); e->ccorp_acc.release(); e->ccorp_rep.release(); e->ext_acc.release();
 	e->grp_labels.release(); e->grp_acc.release(); e->grp_rep.release();
 	e->spread_acc.release(); e->spread_rep.release();
+	e->pair_refs.release(); e->pair_acc.release(); e->pair_rep.release();
 	e->tup.release(); e->tups.release(); e->tvals.release();
 	e->win[0].release(); e->win[1].release(); e->batch_in.release(); e->batch_out.release(); e->batch_mask.release();
 	if (e->h_result) cudaFreeHost(e->h_result);
@@ -2145,7 +2183,7 @@ extern "C" int apo_score_accumulate(apo_engine *e, const apo_score_opts *o, uint
 	if (rc) return rc;
 	if ((uint64_t)cand_offset + ev.C > e->score_C) return fail(e, APO_E_ARG, "candidates [%u,%u) exceed C_total=%u", cand_offset, cand_offset + ev.C, e->score_C);
 	if ((rc = check_window(e, o, ev.count))) return rc;
-	if ((rc = passes_check(e, o, ev.records(), o->count ? o->first + o->count : ev.count))) return rc;
+	if ((rc = passes_check(e, o, ev.records(), o->count ? o->first + o->count : ev.count, e->score_C, cand_offset, ev.C))) return rc;
 	CK(cudaSetDevice(e->device));
 	for (int p = 0; p < NPASS; p++)                     // allocates: before route_copy
 		if (wants(o, p) && e->pass[p].every && !e->pass[p].armed && (rc = pass_arm(e, p, e->score_C))) return rc;
@@ -2164,12 +2202,14 @@ extern "C" int apo_score_finish(apo_engine *e, const apo_score_opts *o, double *
 	if (!e->scoring) return fail(e, APO_E_STATE, "apo_score_begin has not been called");
 	int rc = score_check(e, o, e->score_C, kSession, true);      // the accumulate calls refused every other source
 	if (rc) return rc;
-	for (const int p : {PASS_GRP, PASS_CAND, PASS_CCORP, PASS_EXT, PASS_SPREAD}) {
+	for (const int p : {PASS_GRP, PASS_CAND, PASS_CCORP, PASS_EXT, PASS_SPREAD, PASS_PAIR}) {
 		if (!wants(o, p)) continue;
 		if (!e->pass[p].every)
 			return fail(e, APO_E_STATE, "%s: every apo_score_accumulate of the session must set the flag for %s", kPass[p].name, kPass[p].every);
 		if (p == PASS_GRP && e->pass[p].armed && e->grp_arm_gen != e->grp_gen)
 			return fail(e, APO_E_STATE, "APO_SCORE_CANDIDATE_GROUPS: the record groups were uploaded again after the session began to accumulate them");
+		if (p == PASS_PAIR && e->pass[p].armed && e->pair_arm_gen != e->pair_gen)
+			return fail(e, APO_E_STATE, "APO_SCORE_CANDIDATE_PAIRS: the references were uploaded again after the session began to accumulate them");
 	}
 	if ((rc = digest_prepare(e, o)) || (rc = score_arm(e, o, e->score_C, false))) return rc;   // nothing accumulated yet: an empty breakdown
 	return finish_score(e, o, e->score_C, scores, counts, topk, report);
@@ -2317,7 +2357,8 @@ int stream_host(apo_engine *e, const apo_score_opts *o, const HostTensor &h, dou
 	}
 	if ((rc = score_arm(e, o, C, true, (uint64_t)C * T * wire))) return rc;
 	if (h.form == apo::CAND_T) {                                   // the dictionary and its values, once for the whole call
-		if ((wants(o, PASS_CAND) || wants(o, PASS_EXT) || wants(o, PASS_GRP) || wants(o, PASS_SPREAD)) && (rc = upload_tbook(e, h.codebook))) return rc;
+		if ((wants(o, PASS_CAND) || wants(o, PASS_EXT) || wants(o, PASS_GRP) || wants(o, PASS_SPREAD) || wants(o, PASS_PAIR)) && (rc = upload_tbook(e, h.codebook)))
+			return rc;
 		if ((rc = dict_upload(e, e->tups, h.tb_pc, h.tb_pd, h.n_tuples, h.codebook, h.d2book))) return rc;
 		ev.dict = &e->tups; ev.t_once = true;
 		if ((rc = tuple_values(e, e->tups, e->tvals, (o->flags & APO_SCORE_RECIP) != 0))) return rc;
@@ -2698,6 +2739,34 @@ extern "C" int apo_candidate_groups(apo_engine *e, uint32_t c0, uint32_t n, uint
 extern "C" int apo_candidate_spread(apo_engine *e, uint32_t c0, uint32_t n, struct apo_candidate_spread *out) {
 	if (const int rc = report_check(e, PASS_SPREAD, c0, n, out); rc || n == 0) return rc;
 	CK(cudaMemcpyAsync(out, e->spread_rep.p + c0, (uint64_t)n * sizeof(struct apo_candidate_spread), cudaMemcpyDeviceToHost, e->stream));
+	CK(cudaStreamSynchronize(e->stream));
+	return APO_OK;
+}
+
+extern "C" int apo_candidate_refs_upload(apo_engine *e, const uint32_t *refs, uint32_t C) {
+	if (!e) return APO_E_ARG;
+	if (C == 0) {
+		CK(cudaSetDevice(e->device));
+		CK(cudaStreamSynchronize(e->stream));                           // no queued pass still reads them
+		e->pair_refs.release();
+		e->pair_refs_host.clear(); e->pair_gen++;
+		return APO_OK;
+	}
+	if (!refs) return fail(e, APO_E_ARG, "refs is NULL");
+	for (uint32_t c = 0; c < C; c++)                                // from outside the program: the pass loads the rows they name
+		if (refs[c] != APO_PAIR_NONE && refs[c] >= C) return fail(e, APO_E_ARG, "refs[%u]=%u is neither below C=%u nor APO_PAIR_NONE", c, refs[c], C);
+	CK(cudaSetDevice(e->device));
+	e->pair_refs_host.clear(); e->pair_gen++;                       // the previous refs are gone once the buffer is reused
+	CK(reserve(e, e->pair_refs, C));
+	CK(cudaMemcpyAsync(e->pair_refs.p, refs, (uint64_t)C * 4, cudaMemcpyHostToDevice, e->stream));   // after every queued pass that reads them
+	CK(cudaStreamSynchronize(e->stream));
+	e->pair_refs_host.assign(refs, refs + C);
+	return APO_OK;
+}
+
+extern "C" int apo_candidate_pairs(apo_engine *e, uint32_t c0, uint32_t n, struct apo_candidate_pair *out) {
+	if (const int rc = report_check(e, PASS_PAIR, c0, n, out); rc || n == 0) return rc;
+	CK(cudaMemcpyAsync(out, e->pair_rep.p + c0, (uint64_t)n * sizeof(struct apo_candidate_pair), cudaMemcpyDeviceToHost, e->stream));
 	CK(cudaStreamSynchronize(e->stream));
 	return APO_OK;
 }

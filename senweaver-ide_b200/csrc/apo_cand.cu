@@ -17,7 +17,7 @@
 //
 // For record sources a second feature (APO_SCORE_CANDIDATE_CORPUS, k_cand_corpus below) goes further: the whole corpus
 // report of every candidate's records — patterns, per-mode tallies and tool totals included — by the corpus scan's own code.
-// The extremes, the group scores and the reward spread follow.  Every pass is one walk (cand_walk) over the same warp tiles with its own
+// The extremes, the group scores, the reward spread and the paired comparison follow.  Every pass is one walk (cand_walk) over the same warp tiles with its own
 // per-evaluation step and flush, and one launcher sizes every walk's grid (walk_grid).
 #include <cstdlib>
 #include "apo_device.cuh"
@@ -228,16 +228,26 @@ __device__ __forceinline__ void stage_tables(const CandEvals &P, CandSmem &S, do
 __device__ __forceinline__ uint64_t cand_warp() { return (uint64_t)blockIdx.x * CB_WARPS + (threadIdx.x >> 5); }
 
 struct NoSide { __device__ uint32_t operator()(uint64_t) const { return 0u; } };
+// the second row a pass reads per candidate: none (every pass but the paired comparison); U: groups of 32 evaluations a lane
+// keeps in flight over loader L
+struct NoPair {
+	static constexpr bool PAIR = false;
+	template <class L> static constexpr int U = L::U;
+	__device__ uint32_t operator()(uint32_t) const { return 0u; }
+};
 
 // Warp tiles of CB_TILE evaluations run candidate-major (tile = c * tiles_per_cand + j), and every warp walks a contiguous
-// range of them (the range k_cand_extremes_merge inverts).  A lane keeps L::U groups of 32 evaluations in flight, then
+// range of them (the range k_cand_extremes_merge inverts).  A lane keeps U = Pair::U<L> groups of 32 evaluations in flight, then
 // each(c, t, in, R, s) sees them in order: t is the lane's evaluation, in says whether it lies inside the row, and only then
 // do R (its fetch) and s (side(t), fetched with it) hold anything.  A group wholly past the row end ends the tile,
 // warp-uniformly.  flush(c) ends the warp's run of candidate c: when the candidate changes, after every RUN tiles (0: never)
-// and after the last tile.
-template <class L, uint32_t RUN, class Each, class Flush, class Side = NoSide>
+// and after the last tile.  A pass with a second row (Pair::PAIR) names it per candidate, pair(c) (APO_PAIR_NONE: the
+// candidate's tiles are skipped, warp-uniformly, and nothing of them is loaded); that row's evaluation t is fetched in the same
+// in-flight group as the candidate's own, and each(c, t, in, R, Q, s) sees it as Q.
+template <class L, uint32_t RUN, class Each, class Flush, class Side = NoSide, class Pair = NoPair>
 __device__ __forceinline__ void cand_walk(const CandEvals &P, uint32_t tiles_per_cand, uint64_t total_tiles, Each &&each, Flush &&flush,
-                                          Side side = {}) {
+                                          Side side = {}, Pair pair = {}) {
+	constexpr int U = Pair::template U<L>;
 	const int lane = threadIdx.x & 31;
 	const uint64_t nwarps = (uint64_t)gridDim.x * CB_WARPS, gw = cand_warp();
 	const uint64_t lo = total_tiles * gw / nwarps, hi = total_tiles * (gw + 1) / nwarps;
@@ -247,23 +257,32 @@ __device__ __forceinline__ void cand_walk(const CandEvals &P, uint32_t tiles_per
 		const uint32_t c = (uint32_t)(tile / tiles_per_cand), j = (uint32_t)(tile - (uint64_t)c * tiles_per_cand);
 		if (c != cur || (RUN && run == RUN)) { flush(cur); cur = c; run = 0; }
 		run++;
+		uint32_t rc = 0;
+		if constexpr (Pair::PAIR) {
+			rc = pair(c);
+			if (rc == APO_PAIR_NONE) continue;                              // warp-uniform: c is the warp's candidate
+		}
 		const uint64_t t0 = (uint64_t)j * CB_TILE;
-		for (int g0 = 0; g0 < CB_GROUPS; g0 += L::U) {
-			typename L::Raw R[L::U];
-			bool in[L::U];
-			uint32_t s[L::U];
+		for (int g0 = 0; g0 < CB_GROUPS; g0 += U) {
+			typename L::Raw R[U], Q[Pair::PAIR ? U : 1];
+			bool in[U];
+			uint32_t s[U];
 #pragma unroll
-			for (int u = 0; u < L::U; u++) {
+			for (int u = 0; u < U; u++) {
 				const uint64_t t = t0 + (uint64_t)(g0 + u) * 32 + lane;
 				in[u] = t < P.T;
 				s[u] = in[u] ? side(t) : 0u;
-				if (in[u]) L::fetch(P, c, t, R[u]);
+				if (in[u]) {
+					L::fetch(P, c, t, R[u]);
+					if constexpr (Pair::PAIR) L::fetch(P, rc, t, Q[u]);
+				}
 			}
 #pragma unroll
-			for (int u = 0; u < L::U; u++) {
+			for (int u = 0; u < U; u++) {
 				const uint64_t t = t0 + (uint64_t)(g0 + u) * 32 + lane;
 				if (t - lane >= P.T) break;                                 // warp-uniform: the rest of the tile is past the row end
-				each(c, t, in[u], R[u], s[u]);
+				if constexpr (Pair::PAIR) each(c, t, in[u], R[u], Q[u], s[u]);
+				else each(c, t, in[u], R[u], s[u]);
 			}
 		}
 	}
@@ -830,6 +849,36 @@ __device__ __forceinline__ double u256_to_double(const unsigned long long m[4]) 
 	return ldexp(__ull2double_rn(top | (sticky ? 1ull : 0ull)), sh);
 }
 
+// variance, stdDev and stdErr of n terms with the exact sums s1 (|s1| < 2^128) and s2 (< 2^192): M = n * s2 - s1^2 in 256
+// bits, rounded once (the spread's rules, and the paired comparison's with d for x)
+__device__ __forceinline__ void spread_moments(uint64_t n, __int128 s1, const unsigned long long s2[4], double &variance, double &stdDev,
+                                               double &stdErr) {
+	if (n < 2) {
+		variance = stdDev = stdErr = __longlong_as_double(0x7ff8000000000000ll);
+		return;
+	}
+	// M = n * S2 - S1^2, with n * S2 < 2^256 and |S1| < 2^128
+	unsigned long long a[4] = {0ull, 0ull, 0ull, 0ull}, b[4] = {0ull, 0ull, 0ull, 0ull};
+	for (int i = 0; i < 3; i++) u256_add_at(a, (unsigned __int128)n * s2[i], i);
+	const unsigned __int128 u = s1 < 0 ? (unsigned __int128)0 - (unsigned __int128)s1 : (unsigned __int128)s1;
+	const unsigned long long u0 = (unsigned long long)u, u1 = (unsigned long long)(u >> 64);
+	u256_add_at(b, (unsigned __int128)u0 * u0, 0);
+	u256_add_at(b, (unsigned __int128)u0 * u1, 1);
+	u256_add_at(b, (unsigned __int128)u0 * u1, 1);
+	u256_add_at(b, (unsigned __int128)u1 * u1, 2);
+	unsigned long long m[4], borrow = 0ull;
+	for (int i = 0; i < 4; i++) {
+		const unsigned long long d = a[i] - b[i];
+		const unsigned long long nb = (a[i] < b[i] ? 1ull : 0ull) | (d < borrow ? 1ull : 0ull);
+		m[i] = d - borrow;
+		borrow = nb;
+	}
+	const double dn = __ull2double_rn(n);
+	variance = __ddiv_rn(__ddiv_rn(__dmul_rn(u256_to_double(m), 0x1p-104), dn), __ull2double_rn(n - 1));
+	stdDev = __dsqrt_rn(variance);
+	stdErr = __dsqrt_rn(__ddiv_rn(variance, dn));
+}
+
 // one thread per candidate
 __global__ void __launch_bounds__(256)
 k_cand_spread_report(const unsigned long long *words, const long long *partials, uint32_t C, struct apo_candidate_spread *out) {
@@ -849,31 +898,7 @@ k_cand_spread_report(const unsigned long long *words, const long long *partials,
 	R.sumSq[0] = s2[0]; R.sumSq[1] = s2[1]; R.sumSq[2] = s2[2];
 	R.mean = report_avg_reward(limbs_to_double(l), n);                   // the division scores[c] is: same bits
 	R.rewardSumSq = __dmul_rn(u256_to_double(s2), 0x1p-104);
-	const double nan = __longlong_as_double(0x7ff8000000000000ll);
-	if (n < 2) {
-		R.variance = R.stdDev = R.stdErr = nan;
-	} else {
-		// M = n * S2 - S1^2, with n * S2 < 2^256 and |S1| < 2^128
-		unsigned long long a[4] = {0ull, 0ull, 0ull, 0ull}, b[4] = {0ull, 0ull, 0ull, 0ull};
-		for (int i = 0; i < 3; i++) u256_add_at(a, (unsigned __int128)n * s2[i], i);
-		const unsigned __int128 u = s1 < 0 ? (unsigned __int128)0 - (unsigned __int128)s1 : (unsigned __int128)s1;
-		const unsigned long long u0 = (unsigned long long)u, u1 = (unsigned long long)(u >> 64);
-		u256_add_at(b, (unsigned __int128)u0 * u0, 0);
-		u256_add_at(b, (unsigned __int128)u0 * u1, 1);
-		u256_add_at(b, (unsigned __int128)u0 * u1, 1);
-		u256_add_at(b, (unsigned __int128)u1 * u1, 2);
-		unsigned long long m[4], borrow = 0ull;
-		for (int i = 0; i < 4; i++) {
-			const unsigned long long d = a[i] - b[i];
-			const unsigned long long nb = (a[i] < b[i] ? 1ull : 0ull) | (d < borrow ? 1ull : 0ull);
-			m[i] = d - borrow;
-			borrow = nb;
-		}
-		const double dn = __ull2double_rn(n);
-		R.variance = __ddiv_rn(__ddiv_rn(__dmul_rn(u256_to_double(m), 0x1p-104), dn), __ull2double_rn(n - 1));
-		R.stdDev = __dsqrt_rn(R.variance);
-		R.stdErr = __dsqrt_rn(__ddiv_rn(R.variance, dn));
-	}
+	spread_moments(n, s1, s2, R.variance, R.stdDev, R.stdErr);
 	out[c] = R;
 }
 
@@ -881,6 +906,118 @@ cudaError_t run_cand_spread_report(const unsigned long long *words, const long l
                                    cudaStream_t st) {
 	if (C == 0) return cudaSuccess;
 	k_cand_spread_report<<<(C + 255) / 256, 256, 0, st>>>(words, partials, C, out);
+	return cudaGetLastError();
+}
+
+// ================================================================ paired comparison with a reference (APO_SCORE_CANDIDATE_PAIRS)
+//   k_cand_pairs<Loader, TABLE, RECIP>  one pass over the evaluations a scoring call reads, on the shared loaders and walk:
+//                                       the walk fetches the reference's row with the candidate's own, and every lane compares
+//                                       the two terms x = rint(fr * 2^52) the call summed at each position
+//   k_cand_pair_report                  the pass's words -> apo_candidate_pair
+// Per lane and run of at most CB_RUN_TILES tiles (2^21 positions): the five tallies as u32, D1 as a signed 128-bit sum
+// (|d| <= 2^62, so |run| < 2^83) and D2 as an unsigned 192-bit one (d^2 <= 2^124).  A flush reduces the warp's sums, D1
+// sign-extended to 192 bits, and adds them into the candidate's words with carried atomics, exact modulo 2^192 for any
+// number of flushes (|D1| < 2^126 and D2 < 2^192 for any n < 2^64), and the tallies as u64 atomics.  No word takes 32-bit
+// limbs that a reader would need carried, so the host's limb carry (limb_guard) has nothing of this pass to rewrite.
+
+// the row of c's reference in this launch (the host keeps every reference inside the launch's candidates).  Two rows in flight
+// per group: loaders of more than 16 bytes per evaluation (Form D's 36, Form R's 32) keep 2 groups, so that the lane holds the
+// bytes one row holds at their U (Form D at U = 4 and two rows reaches the 128-register bound of two CTAs per SM and spills)
+struct RefRow {
+	static constexpr bool PAIR = true;
+	template <class L> static constexpr int U = sizeof(typename L::Raw) > 16 ? 2 : L::U;
+	const uint32_t *refs;
+	uint32_t base;
+	__device__ uint32_t operator()(uint32_t c) const {
+		const uint32_t r = __ldg(refs + c);
+		return r == APO_PAIR_NONE ? APO_PAIR_NONE : r - base;
+	}
+};
+
+template <class L, int TABLE, bool RECIP>
+__global__ void __launch_bounds__(CB_THREADS, L::MIN_CTAS)
+k_cand_pairs(const CandPairParams X, uint32_t tiles_per_cand, uint64_t total_tiles) {
+	const CandEvals &P = X.src;
+	__shared__ CandSmem S;
+	__shared__ double s_rc[512];                                        // reciprocal of the total weight (div_lut)
+	stage_tables<TABLE, true>(P, S, s_rc);
+	const int lane = threadIdx.x & 31;
+	Acc128 d1;
+	d1.zero();
+	U192 d2{0ull, 0ull, 0ull};
+	uint32_t wins = 0, losses = 0, ties = 0, conly = 0, ronly = 0;
+
+	auto flush = [&](uint32_t c) {
+		U192 s1{d1.lo, (unsigned long long)d1.hi, (unsigned long long)(d1.hi >> 63)}, s2 = d2;
+#pragma unroll
+		for (int o = 16; o > 0; o >>= 1) {                              // exact: 32 lanes of |D1| < 2^83 and D2 < 2^145
+			u192_add(s1, __shfl_xor_sync(FULL, s1.w0, o), __shfl_xor_sync(FULL, s1.w1, o), __shfl_xor_sync(FULL, s1.w2, o));
+			u192_add(s2, __shfl_xor_sync(FULL, s2.w0, o), __shfl_xor_sync(FULL, s2.w1, o), __shfl_xor_sync(FULL, s2.w2, o));
+		}
+		const uint32_t k[5] = {warp_sum_u32(wins), warp_sum_u32(losses), warp_sum_u32(ties), warp_sum_u32(conly), warp_sum_u32(ronly)};
+		if (lane == 0) {
+			unsigned long long *w = X.words + (uint64_t)c * PR_WORDS;
+			if (s1.w0 | s1.w1 | s1.w2) atomic_add_u192(w + PR_D1, s1);
+			if (s2.w0 | s2.w1 | s2.w2) atomic_add_u192(w + PR_D2, s2);
+#pragma unroll
+			for (int i = 0; i < 5; i++)
+				if (k[i]) atomicAdd(w + PR_CNT + i, (unsigned long long)k[i]);
+		}
+		d1.zero();
+		d2 = U192{0ull, 0ull, 0ull};
+		wins = losses = ties = conly = ronly = 0;
+	};
+	auto each = [&](uint32_t, uint64_t, bool in, const typename L::Raw &R, const typename L::Raw &Q, uint32_t) {
+		if (!in) return;
+		CandEval E;
+		L::decode(P, S, R, E);
+		const bool vc = E.valid != 0u;
+		const long long xc = vc ? to_fx(cand_final_reward<RECIP>(E, X.W, S.tw, s_rc)) : 0ll;
+		L::decode(P, S, Q, E);
+		const bool vr = E.valid != 0u;
+		const long long xr = vr ? to_fx(cand_final_reward<RECIP>(E, X.W, S.tw, s_rc)) : 0ll;
+		if (vc && vr) {
+			const long long d = xc - xr;
+			wins += d > 0 ? 1u : 0u;
+			losses += d < 0 ? 1u : 0u;
+			ties += d == 0 ? 1u : 0u;
+			d1.add(d);
+			u192_add_sq(d2, d);
+		} else {
+			conly += vc ? 1u : 0u;
+			ronly += vr ? 1u : 0u;
+		}
+	};
+	cand_walk<L, CB_RUN_TILES>(P, tiles_per_cand, total_tiles, each, flush, NoSide{}, RefRow{X.refs, X.base});
+}
+
+// one thread per candidate
+__global__ void __launch_bounds__(256)
+k_cand_pair_report(const unsigned long long *words, const uint32_t *refs, uint32_t C, struct apo_candidate_pair *out) {
+	const uint32_t c = blockIdx.x * blockDim.x + threadIdx.x;
+	if (c >= C) return;
+	const unsigned long long *w = words + (uint64_t)c * PR_WORDS;
+	struct apo_candidate_pair R;
+	R.ref = refs[c];
+	R.pad = 0u;
+	R.wins = w[PR_CNT]; R.losses = w[PR_CNT + 1]; R.ties = w[PR_CNT + 2]; R.candOnly = w[PR_CNT + 3]; R.refOnly = w[PR_CNT + 4];
+	const uint64_t n = R.wins + R.losses + R.ties;
+	R.n = n;
+	const __int128 s1 = (__int128)(((unsigned __int128)w[PR_D1 + 1] << 64) | w[PR_D1]);   // word 2 is the sign extension
+	R.sumLo = w[PR_D1];
+	R.sumHi = (int64_t)w[PR_D1 + 1];
+	const unsigned long long s2[4] = {w[PR_D2], w[PR_D2 + 1], w[PR_D2 + 2], 0ull};
+	R.sumSq[0] = s2[0]; R.sumSq[1] = s2[1]; R.sumSq[2] = s2[2];
+	const long long l[4] = {(long long)(s1 & 0xFFFFFFFF), (long long)((s1 >> 32) & 0xFFFFFFFF), (long long)(s1 >> 64), 0ll};
+	R.meanDiff = report_avg_reward(limbs_to_double(l), n);               // the rounding sequence of scores[c]
+	spread_moments(n, s1, s2, R.variance, R.stdDev, R.stdErr);
+	out[c] = R;
+}
+
+cudaError_t run_cand_pair_report(const unsigned long long *words, const uint32_t *refs, uint32_t C, struct apo_candidate_pair *out,
+                                 cudaStream_t st) {
+	if (C == 0) return cudaSuccess;
+	k_cand_pair_report<<<(C + 255) / 256, 256, 0, st>>>(words, refs, C, out);
 	return cudaGetLastError();
 }
 
@@ -928,6 +1065,10 @@ template <class L, int TABLE, bool RECIP>
 static cudaError_t launch_pass(const CandSpreadParams &X, int sm_count, cudaStream_t st) {
 	return launch_walk(k_cand_spread<L, TABLE, RECIP>, X, sm_count, st);
 }
+template <class L, int TABLE, bool RECIP>
+static cudaError_t launch_pass(const CandPairParams &X, int sm_count, cudaStream_t st) {
+	return launch_walk(k_cand_pairs<L, TABLE, RECIP>, X, sm_count, st);
+}
 
 // the loader of each source and the table it stages; RECIP: the division of the passes that divide (div_lut)
 template <bool RECIP, class X>
@@ -953,6 +1094,9 @@ cudaError_t run_cand_groups(const CandGroupParams &X, int source, bool recip, in
 	return recip ? by_source<true>(X, source, sm_count, st) : by_source<false>(X, source, sm_count, st);
 }
 cudaError_t run_cand_spread(const CandSpreadParams &X, int source, bool recip, int sm_count, cudaStream_t st) {
+	return recip ? by_source<true>(X, source, sm_count, st) : by_source<false>(X, source, sm_count, st);
+}
+cudaError_t run_cand_pairs(const CandPairParams &X, int source, bool recip, int sm_count, cudaStream_t st) {
 	return recip ? by_source<true>(X, source, sm_count, st) : by_source<false>(X, source, sm_count, st);
 }
 

@@ -423,6 +423,24 @@ cudaError_t run_cand_spread(const CandSpreadParams &P, int source, bool recip, i
 cudaError_t run_cand_spread_report(const unsigned long long *words, const long long *partials, uint32_t C, struct apo_candidate_spread *out,
                                    cudaStream_t st);
 
+// ---- per-candidate paired comparison (csrc/apo_cand.cu): every candidate against its reference on the same record positions.
+// Own buffer [C][PR_WORDS]: D1 = sum d (192-bit two's complement), D2 = sum d^2 (unsigned 192-bit), each least significant
+// word first, then wins, losses, ties, candOnly, refOnly.  Every word takes whole 64-bit adds (carried atomics for the sums):
+// nothing accumulates in 32-bit limbs, so the pair words need no limb carry.
+constexpr int PR_WORDS = 11;
+constexpr int PR_D1 = 0, PR_D2 = 3, PR_CNT = 6;
+struct CandPairParams {
+	CandEvals src;
+	Weights W;
+	const uint32_t *refs;           // [C] reference of candidate 0 of this launch onwards: an absolute index, or APO_PAIR_NONE
+	uint32_t base;                  // absolute index of candidate 0 of this launch: the row of refs[c] is refs[c] - base
+	unsigned long long *words;      // [C][PR_WORDS] of candidate 0 of this launch
+};
+cudaError_t run_cand_pairs(const CandPairParams &P, int source, bool recip, int sm_count, cudaStream_t st);
+// words / refs: the whole buffers of C candidates
+cudaError_t run_cand_pair_report(const unsigned long long *words, const uint32_t *refs, uint32_t C, struct apo_candidate_pair *out,
+                                 cudaStream_t st);
+
 // ---- limb carry (csrc/apo_cand.cu): the (l0, l1, l2) triples that accumulate across the launches of a session or of a
 // host-streaming call (the candidate partials, the breakdown's dimension words, the group words, the per-candidate corpus
 // blocks' reward and dimension words) stay exact while l0 and l1 < 2^63.  limb_flush_bound: the most flushes one launch over

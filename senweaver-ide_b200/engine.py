@@ -26,6 +26,8 @@ EXTREMES_N = 32
 SCORE_CANDIDATE_GROUPS = 0x40
 GROUPS_MAX = 64
 SCORE_CANDIDATE_SPREAD = 0x80
+SCORE_CANDIDATE_PAIRS = 0x100
+PAIR_NONE = 0xFFFFFFFF
 TUNE_NO_FUSE, TUNE_FORCE_FUSE, TUNE_NO_STAGING, TUNE_NCCL_JOIN, TUNE_NO_TWIN = 0x1, 0x2, 0x4, 0x8, 0x10
 TUNE_NO_TWIN_T, TUNE_TWIN_T, TUNE_NO_TWIN_T2, TUNE_NO_TWIN_H = 0x20, 0x40, 0x80, 0x100
 TUNE_NO_CORPUS_DIGEST = 0x200
@@ -114,6 +116,29 @@ class CandidateSpread(C.Structure):
         return int(self.sumSq[0]) | (int(self.sumSq[1]) << 64) | (int(self.sumSq[2]) << 128)
 
 
+class CandidatePair(C.Structure):
+    """struct apo_candidate_pair: one candidate compared with its reference on the record positions both were scored on.
+    ref (PAIR_NONE: no reference, every count 0, every double NaN); n positions where both have a finalReward, with wins /
+    losses / ties as d = x_c - x_r > 0 / < 0 / == 0 of the terms x = rint(fr * 2^52); candOnly / refOnly positions where only
+    one of them has a finalReward (left out of the sums); the exact integers D1 = sum d (two's complement 128-bit: sumLo,
+    sumHi) and D2 = sum d^2 (unsigned 192-bit, sumSq least significant word first); meanDiff (NaN when n == 0), the unbiased
+    variance, stdDev and stdErr of the paired differences, each rounded as the header states (NaN when n < 2)."""
+    _fields_ = [("ref", C.c_uint32), ("pad", C.c_uint32), ("n", C.c_uint64), ("wins", C.c_uint64), ("losses", C.c_uint64),
+                ("ties", C.c_uint64), ("candOnly", C.c_uint64), ("refOnly", C.c_uint64), ("sumLo", C.c_uint64), ("sumHi", C.c_int64),
+                ("sumSq", C.c_uint64 * 3), ("meanDiff", C.c_double), ("variance", C.c_double), ("stdDev", C.c_double),
+                ("stdErr", C.c_double)]
+
+    @property
+    def sum(self) -> int:
+        """D1 as a Python int"""
+        return (int(self.sumHi) << 64) | int(self.sumLo)
+
+    @property
+    def sum_sq(self) -> int:
+        """D2 as a Python int"""
+        return int(self.sumSq[0]) | (int(self.sumSq[1]) << 64) | (int(self.sumSq[2]) << 128)
+
+
 class Timing(C.Structure):
     _fields_ = [("reward_ms", C.c_float), ("corpus_ms", C.c_float), ("allreduce_ms", C.c_float),
                 ("finalize_ms", C.c_float), ("total_ms", C.c_float), ("launches", C.c_uint32), ("pad", C.c_uint32),
@@ -143,7 +168,7 @@ ABI_SYMBOLS = (
     "apo_dims_compact_download", "apo_dims_codebook", "apo_packed_encode_host", "apo_score_host_packed", "apo_dims_packed_download", "apo_dims_d2book",
     "apo_tuple_encode_host", "apo_score_host_tuples", "apo_tuples_upload", "apo_dims_tuples", "apo_tuples_download", "apo_tuples_book",
     "apo_host_alloc", "apo_host_free",
-    "apo_last_timing", "apo_debug_partials", "apo_debug_twin_t_list", "apo_debug_twin_h", "apo_debug_corpus_digest", "apo_candidate_reports", "apo_candidate_corpus_reports", "apo_candidate_extremes", "apo_record_groups_upload", "apo_candidate_groups", "apo_candidate_spread", "apo_comm_unique_id", "apo_comm_init", "apo_comm_destroy", "apo_comm_join_mode",
+    "apo_last_timing", "apo_debug_partials", "apo_debug_twin_t_list", "apo_debug_twin_h", "apo_debug_corpus_digest", "apo_candidate_reports", "apo_candidate_corpus_reports", "apo_candidate_extremes", "apo_record_groups_upload", "apo_candidate_groups", "apo_candidate_spread", "apo_candidate_refs_upload", "apo_candidate_pairs", "apo_comm_unique_id", "apo_comm_init", "apo_comm_destroy", "apo_comm_join_mode",
 )
 
 
@@ -237,6 +262,8 @@ def load_library() -> C.CDLL:
     L.apo_record_groups_upload.argtypes = [vp, vp, u64, u32]
     L.apo_candidate_groups.argtypes = [vp, u32, u32, u32, vp]
     L.apo_candidate_spread.argtypes = [vp, u32, u32, vp]
+    L.apo_candidate_refs_upload.argtypes = [vp, vp, u32]
+    L.apo_candidate_pairs.argtypes = [vp, u32, u32, vp]
     L.apo_comm_unique_id.argtypes = [vp]
     L.apo_comm_init.argtypes = [vp, i32, i32, vp]
     L.apo_comm_destroy.argtypes = [vp]
@@ -303,16 +330,17 @@ def records_from_json(text: str | bytes) -> np.ndarray:
 
 
 class ScoreResult:
-    __slots__ = ("scores", "counts", "topk", "report", "timing", "candidates", "candidate_corpus", "extremes", "groups", "spread")
+    __slots__ = ("scores", "counts", "topk", "report", "timing", "candidates", "candidate_corpus", "extremes", "groups", "spread", "pairs")
 
     def __init__(self, scores, counts, topk, report, timing, candidates=None, candidate_corpus=None, extremes=None, groups=None,
-                 spread=None):
+                 spread=None, pairs=None):
         self.scores, self.counts, self.topk, self.report, self.timing = scores, counts, topk, report, timing
         self.candidates = candidates        # CandidateReport array [C] when the call asked for the breakdown, else None
         self.candidate_corpus = candidate_corpus   # CorpusReport array [C] when the call asked for the per-candidate corpus reports
         self.extremes = extremes            # CandidateExtremes array [C] when the call asked for the per-candidate extremes
         self.groups = groups                # GroupScore array [C][G] when the call asked for the per-candidate group scores
         self.spread = spread                # CandidateSpread array [C] when the call asked for the per-candidate reward spread
+        self.pairs = pairs                  # CandidatePair array [C] when the call asked for the paired comparisons
 
 
 class Engine:
@@ -454,12 +482,12 @@ class Engine:
 
     def score_host_records(self, recs: np.ndarray, K: int, corpus: bool = False, recip: bool = False, variant: int = 0,
                            candidates: bool = False, candidate_corpus: bool = False, extremes: bool = False,
-                           groups: bool = False, spread: bool = False) -> ScoreResult:
+                           groups: bool = False, spread: bool = False, pairs: bool = False) -> ScoreResult:
         """recs: C-contiguous [C][T] of RECORD_DTYPE (32 B) or RECORD16_DTYPE (16 B) in host memory."""
         assert recs.flags.c_contiguous and recs.ndim == 2 and recs.dtype.itemsize in (32, 16)
         Cn, T = recs.shape
         o = self._opts(K, SRC_ROLLOUTS, corpus, recip, variant, 0, 0, candidates=candidates, candidate_corpus=candidate_corpus,
-                       extremes=extremes, groups=groups, spread=spread)
+                       extremes=extremes, groups=groups, spread=spread, pairs=pairs)
         scores = np.empty(Cn, np.float64)
         counts = np.empty(Cn, np.uint64)
         topk = np.empty(K, np.int32)
@@ -467,15 +495,15 @@ class Engine:
         self._ck(self._L.apo_score_host_records(self._h, C.byref(o), _p(recs), recs.dtype.itemsize, Cn, T, _p(scores), _p(counts),
                                                 _p(topk), C.byref(rep) if rep is not None else None))
         return ScoreResult(scores, counts, topk, rep, self.last_timing(), self._cands(Cn, candidates),
-                           self._ccorp(Cn, candidate_corpus), self._ext(Cn, extremes), self._grp(Cn, groups), self._spr(Cn, spread))
+                           self._ccorp(Cn, candidate_corpus), self._ext(Cn, extremes), self._grp(Cn, groups), self._spr(Cn, spread), self._pairs(Cn, pairs))
 
     # -- scoring
     def _opts(self, K, source, corpus, recip, variant, first, count, timing=False, candidates=False,
-              candidate_corpus=False, extremes=False, groups=False, spread=False) -> ScoreOpts:
+              candidate_corpus=False, extremes=False, groups=False, spread=False, pairs=False) -> ScoreOpts:
         return ScoreOpts(K, source, (SCORE_CORPUS if corpus else 0) | (SCORE_RECIP if recip else 0) | (SCORE_TIMING if timing else 0)
                          | (SCORE_CANDIDATES if candidates else 0) | (SCORE_CANDIDATE_CORPUS if candidate_corpus else 0)
                          | (SCORE_CANDIDATE_EXTREMES if extremes else 0) | (SCORE_CANDIDATE_GROUPS if groups else 0)
-                         | (SCORE_CANDIDATE_SPREAD if spread else 0),
+                         | (SCORE_CANDIDATE_SPREAD if spread else 0) | (SCORE_CANDIDATE_PAIRS if pairs else 0),
                          variant, first, count)
 
     def _cands(self, Cn: int, wanted: bool):
@@ -492,6 +520,22 @@ class Engine:
 
     def _spr(self, Cn: int, wanted: bool):
         return self.candidate_spread(0, Cn) if wanted else None
+
+    def _pairs(self, Cn: int, wanted: bool):
+        return self.candidate_pairs(0, Cn) if wanted else None
+
+    def candidate_refs_upload(self, refs):
+        """apo_candidate_refs_upload: refs uint32 [C], the reference of every candidate (an index < C, or PAIR_NONE); an empty
+        array releases them.  Scoring calls of C candidates with pairs=True then compare every candidate with its reference."""
+        refs = np.ascontiguousarray(refs, np.uint32)
+        self._ck(self._L.apo_candidate_refs_upload(self._h, _p(refs) if refs.size else None, refs.size))
+
+    def candidate_pairs(self, c0: int, n: int):
+        """apo_candidate_pairs: CandidatePair[n] of candidates [c0, c0+n) from the last scoring call, which must have set
+        pairs=True (ApoError APO_E_STATE otherwise)."""
+        out = (CandidatePair * n)()
+        self._ck(self._L.apo_candidate_pairs(self._h, c0, n, out if n else None))
+        return out
 
     def record_groups_upload(self, labels, G: int = 0):
         """apo_record_groups_upload: labels uint8 [T], the group of every record position (< G <= GROUPS_MAX); an empty
@@ -540,8 +584,8 @@ class Engine:
 
     def score(self, Cn: int, K: int, source: int = SRC_DIMS, corpus: bool = False, recip: bool = False,
               variant: int = 0, first: int = 0, count: int = 0, timing: bool = False, candidates: bool = False,
-              candidate_corpus: bool = False, extremes: bool = False, groups: bool = False, spread: bool = False) -> ScoreResult:
-        o = self._opts(K, source, corpus, recip, variant, first, count, timing, candidates, candidate_corpus, extremes, groups, spread)
+              candidate_corpus: bool = False, extremes: bool = False, groups: bool = False, spread: bool = False, pairs: bool = False) -> ScoreResult:
+        o = self._opts(K, source, corpus, recip, variant, first, count, timing, candidates, candidate_corpus, extremes, groups, spread, pairs)
         scores = np.empty(Cn, np.float64)
         counts = np.empty(Cn, np.uint64)
         topk = np.empty(K, np.int32)
@@ -553,7 +597,7 @@ class Engine:
             self._ck(rc)
         L.apo_last_timing(self._h, C.byref(t))
         return ScoreResult(scores, counts, topk, rep, t, self._cands(Cn, candidates), self._ccorp(Cn, candidate_corpus),
-                           self._ext(Cn, extremes), self._grp(Cn, groups), self._spr(Cn, spread))
+                           self._ext(Cn, extremes), self._grp(Cn, groups), self._spr(Cn, spread), self._pairs(Cn, pairs))
 
     # chunked form: begin / accumulate (per candidate chunk or record window) / finish
     def score_begin(self, C_total: int):
@@ -561,15 +605,15 @@ class Engine:
 
     def score_accumulate(self, cand_offset: int = 0, source: int = SRC_DIMS, recip: bool = False, variant: int = 0,
                          first: int = 0, count: int = 0, candidates: bool = False, candidate_corpus: bool = False,
-                         extremes: bool = False, groups: bool = False, spread: bool = False):
+                         extremes: bool = False, groups: bool = False, spread: bool = False, pairs: bool = False):
         o = self._opts(0, source, False, recip, variant, first, count, candidates=candidates, candidate_corpus=candidate_corpus,
-                       extremes=extremes, groups=groups, spread=spread)
+                       extremes=extremes, groups=groups, spread=spread, pairs=pairs)
         self._ck(self._L.apo_score_accumulate(self._h, C.byref(o), cand_offset))
 
     def score_finish(self, C_total: int, K: int, corpus: bool = False, candidates: bool = False,
-                     candidate_corpus: bool = False, extremes: bool = False, groups: bool = False, spread: bool = False) -> ScoreResult:
+                     candidate_corpus: bool = False, extremes: bool = False, groups: bool = False, spread: bool = False, pairs: bool = False) -> ScoreResult:
         o = self._opts(K, SRC_DIMS, corpus, False, 0, 0, 0, candidates=candidates, candidate_corpus=candidate_corpus, extremes=extremes,
-                       groups=groups, spread=spread)
+                       groups=groups, spread=spread, pairs=pairs)
         scores = np.empty(C_total, np.float64)
         counts = np.empty(C_total, np.uint64)
         topk = np.empty(K, np.int32)
@@ -578,14 +622,14 @@ class Engine:
                                           C.byref(rep) if rep is not None else None))
         return ScoreResult(scores, counts, topk, rep, self.last_timing(), self._cands(C_total, candidates),
                            self._ccorp(C_total, candidate_corpus), self._ext(C_total, extremes), self._grp(C_total, groups),
-                           self._spr(C_total, spread))
+                           self._spr(C_total, spread), self._pairs(C_total, pairs))
 
     def score_host(self, dims: np.ndarray, K: int, corpus: bool = False, recip: bool = False, variant: int = 0,
-                   candidates: bool = False, extremes: bool = False, groups: bool = False, spread: bool = False) -> ScoreResult:
+                   candidates: bool = False, extremes: bool = False, groups: bool = False, spread: bool = False, pairs: bool = False) -> ScoreResult:
         """dims: C-contiguous float32 [C][T][9] in (preferably pinned) host memory."""
         assert dims.dtype == np.float32 and dims.flags.c_contiguous and dims.ndim == 3 and dims.shape[2] == NDIM
         Cn, T, _ = dims.shape
-        o = self._opts(K, SRC_DIMS, corpus, recip, variant, 0, 0, candidates=candidates, extremes=extremes, groups=groups, spread=spread)
+        o = self._opts(K, SRC_DIMS, corpus, recip, variant, 0, 0, candidates=candidates, extremes=extremes, groups=groups, spread=spread, pairs=pairs)
         scores = np.empty(Cn, np.float64)
         counts = np.empty(Cn, np.uint64)
         topk = np.empty(K, np.int32)
@@ -593,7 +637,7 @@ class Engine:
         self._ck(self._L.apo_score_host(self._h, C.byref(o), _p(dims), Cn, T, _p(scores), _p(counts), _p(topk),
                                         C.byref(rep) if rep is not None else None))
         return ScoreResult(scores, counts, topk, rep, self.last_timing(), self._cands(Cn, candidates), extremes=self._ext(Cn, extremes),
-                           groups=self._grp(Cn, groups), spread=self._spr(Cn, spread))
+                           groups=self._grp(Cn, groups), spread=self._spr(Cn, spread), pairs=self._pairs(Cn, pairs))
 
     # -- Form Q in host memory (compact wire format)
     def dims_codebook(self) -> np.ndarray:
@@ -609,13 +653,13 @@ class Engine:
 
     def score_host_compact(self, q8: np.ndarray, d2: np.ndarray, li: np.ndarray, codebook: np.ndarray, K: int, corpus: bool = False,
                            recip: bool = False, candidates: bool = False, extremes: bool = False,
-                          groups: bool = False, spread: bool = False) -> ScoreResult:
+                          groups: bool = False, spread: bool = False, pairs: bool = False) -> ScoreResult:
         """q8 uint64 [C][T], d2 float32 [C][T], li uint16 [C][T] in (preferably pinned) host memory + the uint32[2048] codebook."""
         assert q8.dtype == np.uint64 and d2.dtype == np.float32 and li.dtype == np.uint16 and q8.shape == d2.shape == li.shape and q8.ndim == 2
         assert q8.flags.c_contiguous and d2.flags.c_contiguous and li.flags.c_contiguous
         codebook = np.ascontiguousarray(codebook, np.uint32)
         Cn, T = q8.shape
-        o = self._opts(K, SRC_DIMS, corpus, recip, 0, 0, 0, candidates=candidates, extremes=extremes, groups=groups, spread=spread)
+        o = self._opts(K, SRC_DIMS, corpus, recip, 0, 0, 0, candidates=candidates, extremes=extremes, groups=groups, spread=spread, pairs=pairs)
         scores = np.empty(Cn, np.float64)
         counts = np.empty(Cn, np.uint64)
         topk = np.empty(K, np.int32)
@@ -623,7 +667,7 @@ class Engine:
         self._ck(self._L.apo_score_host_compact(self._h, C.byref(o), _p(q8), _p(d2), _p(li), _p(codebook), Cn, T, _p(scores), _p(counts),
                                                 _p(topk), C.byref(rep) if rep is not None else None))
         return ScoreResult(scores, counts, topk, rep, self.last_timing(), self._cands(Cn, candidates), extremes=self._ext(Cn, extremes),
-                           groups=self._grp(Cn, groups), spread=self._spr(Cn, spread))
+                           groups=self._grp(Cn, groups), spread=self._spr(Cn, spread), pairs=self._pairs(Cn, pairs))
 
     def dims_d2book(self) -> np.ndarray:
         out = np.empty(4096, np.uint32)
@@ -638,13 +682,13 @@ class Engine:
 
     def score_host_packed(self, pc: np.ndarray, pd: np.ndarray, codebook: np.ndarray, d2book: np.ndarray, K: int, corpus: bool = False,
                           recip: bool = False, candidates: bool = False, extremes: bool = False,
-                          groups: bool = False, spread: bool = False) -> ScoreResult:
+                          groups: bool = False, spread: bool = False, pairs: bool = False) -> ScoreResult:
         """Form P: pc uint32 [C][T] (eight 4-bit codes), pd uint16 [C][T] (tool_success_rate index) + the two codebooks."""
         assert pc.dtype == np.uint32 and pd.dtype == np.uint16 and pc.shape == pd.shape and pc.ndim == 2 and pc.flags.c_contiguous and pd.flags.c_contiguous
         codebook, d2book = np.ascontiguousarray(codebook, np.uint32), np.ascontiguousarray(d2book, np.uint32)
         assert codebook.size == 2048 and d2book.size == 4096
         Cn, T = pc.shape
-        o = self._opts(K, SRC_DIMS, corpus, recip, 0, 0, 0, candidates=candidates, extremes=extremes, groups=groups, spread=spread)
+        o = self._opts(K, SRC_DIMS, corpus, recip, 0, 0, 0, candidates=candidates, extremes=extremes, groups=groups, spread=spread, pairs=pairs)
         scores = np.empty(Cn, np.float64)
         counts = np.empty(Cn, np.uint64)
         topk = np.empty(K, np.int32)
@@ -652,7 +696,7 @@ class Engine:
         self._ck(self._L.apo_score_host_packed(self._h, C.byref(o), _p(pc), _p(pd), _p(codebook), _p(d2book), Cn, T, _p(scores), _p(counts),
                                                _p(topk), C.byref(rep) if rep is not None else None))
         return ScoreResult(scores, counts, topk, rep, self.last_timing(), self._cands(Cn, candidates), extremes=self._ext(Cn, extremes),
-                           groups=self._grp(Cn, groups), spread=self._spr(Cn, spread))
+                           groups=self._grp(Cn, groups), spread=self._spr(Cn, spread), pairs=self._pairs(Cn, pairs))
 
     @staticmethod
     def _tuple_args(tl, th, tbook, codebook, d2book):
@@ -665,12 +709,12 @@ class Engine:
 
     def score_host_tuples(self, tl: np.ndarray, th: np.ndarray, tbook, codebook: np.ndarray, d2book: np.ndarray, K: int, corpus: bool = False,
                           recip: bool = False, candidates: bool = False, extremes: bool = False,
-                          groups: bool = False, spread: bool = False) -> ScoreResult:
+                          groups: bool = False, spread: bool = False, pairs: bool = False) -> ScoreResult:
         """Form T: tl uint16 [C][T] + th uint8 [C][T] (24-bit dictionary indices), tbook = (pc uint32 [n], pd uint16 [n]) the distinct
         evaluations as Form P pairs, + the two codebooks of Form P."""
         tb_pc, tb_pd, codebook, d2book = self._tuple_args(tl, th, tbook, codebook, d2book)
         Cn, T = tl.shape
-        o = self._opts(K, SRC_DIMS, corpus, recip, 0, 0, 0, candidates=candidates, extremes=extremes, groups=groups, spread=spread)
+        o = self._opts(K, SRC_DIMS, corpus, recip, 0, 0, 0, candidates=candidates, extremes=extremes, groups=groups, spread=spread, pairs=pairs)
         scores = np.empty(Cn, np.float64)
         counts = np.empty(Cn, np.uint64)
         topk = np.empty(K, np.int32)
@@ -678,7 +722,7 @@ class Engine:
         self._ck(self._L.apo_score_host_tuples(self._h, C.byref(o), _p(tl), _p(th), _p(tb_pc), _p(tb_pd), tb_pc.size, _p(codebook), _p(d2book), Cn, T,
                                                _p(scores), _p(counts), _p(topk), C.byref(rep) if rep is not None else None))
         return ScoreResult(scores, counts, topk, rep, self.last_timing(), self._cands(Cn, candidates), extremes=self._ext(Cn, extremes),
-                           groups=self._grp(Cn, groups), spread=self._spr(Cn, spread))
+                           groups=self._grp(Cn, groups), spread=self._spr(Cn, spread), pairs=self._pairs(Cn, pairs))
 
     def tuples_upload(self, tl: np.ndarray, th: np.ndarray, tbook, codebook: np.ndarray, d2book: np.ndarray):
         """Make a Form T tensor resident: score(C, K, source=SRC_TUPLES) then reads 3 B per evaluation."""

@@ -21,7 +21,8 @@ import { VSBuffer } from '../../../../base/common/buffer.js';
 import { ApoResidentQuery, ApoScoreBlocks, ApoTupleBuffers, IApoScoringService } from '../common/apoScoringService.js';
 
 type Blocks = { scores: ArrayBuffer; counts: ArrayBuffer; topk: ArrayBuffer; report: ArrayBuffer; candidates?: ArrayBuffer; candidateCorpus?: ArrayBuffer;
-	candidateExtremes?: ArrayBuffer; candidateGroups?: ArrayBuffer; candidateSpread?: ArrayBuffer };
+	candidateExtremes?: ArrayBuffer; candidateGroups?: ArrayBuffer; candidateSpread?: ArrayBuffer;
+	candidatePairs?: ArrayBuffer };
 
 interface ApoAddon {
 	create(device: number): unknown | null;             // null when no H100 / library: never throws
@@ -32,15 +33,19 @@ interface ApoAddon {
 	corpusUploadJson(handle: unknown, utf8: ArrayBuffer, idxBase: number): Promise<number>;
 	dimsTuples(handle: unknown, cap?: number): Promise<number>;
 	recordGroupsUpload(handle: unknown, labels: ArrayBuffer, G: number): Promise<void>;
+	candidateRefsUpload(handle: unknown, refs: ArrayBuffer): Promise<void>;
 	scoreResident(handle: unknown, query: ApoResidentQuery): Promise<Blocks>;
 	score(handle: unknown, dims: ArrayBuffer, C: number, T: number, corpus: ArrayBuffer | null, K: number, candidates?: boolean,
-		candidateExtremes?: boolean, candidateGroups?: number, candidateSpread?: boolean): Promise<Blocks>;
+		candidateExtremes?: boolean, candidateGroups?: number, candidateSpread?: boolean,
+		candidatePairs?: boolean): Promise<Blocks>;
 	scoreHostRecords(handle: unknown, records: ArrayBuffer, rowBytes: number, C: number, T: number, corpus: ArrayBuffer | null, K: number,
-		candidates?: boolean, candidateCorpus?: boolean, candidateExtremes?: boolean, candidateGroups?: number, candidateSpread?: boolean): Promise<Blocks>;
+		candidates?: boolean, candidateCorpus?: boolean, candidateExtremes?: boolean, candidateGroups?: number, candidateSpread?: boolean,
+		candidatePairs?: boolean): Promise<Blocks>;
 	/** Form D -> Form T on worker threads of the addon (no GPU): 3 bytes per evaluation instead of 36; null = not categorical. */
 	encodeTuples(dims: ArrayBuffer, C: number, T: number, nthreads?: number): Promise<ApoTuples | null>;
 	scoreHostTuples(handle: unknown, tuples: ApoTuples, C: number, T: number, corpus: ArrayBuffer | null, K: number, candidates?: boolean,
-		candidateExtremes?: boolean, candidateGroups?: number, candidateSpread?: boolean): Promise<Blocks>;
+		candidateExtremes?: boolean, candidateGroups?: number, candidateSpread?: boolean,
+		candidatePairs?: boolean): Promise<Blocks>;
 	rewardBatch(handle: unknown, records: ArrayBuffer): Promise<{ dims: ArrayBuffer; masks: ArrayBuffer; finals: ArrayBuffer }>;
 	recordsFromJson(utf8: ArrayBuffer): ArrayBuffer | null;
 }
@@ -65,6 +70,7 @@ function wrapBlocks(r: Blocks): ApoScoreBlocks {
 	if (r.candidateExtremes) { out.candidateExtremes = VSBuffer.wrap(new Uint8Array(r.candidateExtremes)); }     // struct apo_candidate_extremes[C]
 	if (r.candidateGroups) { out.candidateGroups = VSBuffer.wrap(new Uint8Array(r.candidateGroups)); }     // apo_group_score[C][G]
 	if (r.candidateSpread) { out.candidateSpread = VSBuffer.wrap(new Uint8Array(r.candidateSpread)); }     // struct apo_candidate_spread[C]
+	if (r.candidatePairs) { out.candidatePairs = VSBuffer.wrap(new Uint8Array(r.candidatePairs)); }     // struct apo_candidate_pair[C]
 	return out;
 }
 
@@ -177,15 +183,19 @@ export class ApoScoringMainService implements IApoScoringService {
 		return (await this._need()).recordGroupsUpload(this._handle, ab(labels), G);
 	}
 
+	async candidateRefsUpload(refs: VSBuffer): Promise<void> {
+		return (await this._need()).candidateRefsUpload(this._handle, ab(refs));
+	}
+
 	async scoreResident(query: ApoResidentQuery): Promise<ApoScoreBlocks> {
 		return wrapBlocks(await (await this._need()).scoreResident(this._handle, query));
 	}
 
 	// ---- one-shot path ------------------------------------------------------------------------
 	async score(dims: VSBuffer, C: number, T: number, corpus: VSBuffer | undefined, K: number, candidates?: boolean,
-		candidateExtremes?: boolean, candidateGroups?: number, candidateSpread?: boolean): Promise<ApoScoreBlocks> {
+		candidateExtremes?: boolean, candidateGroups?: number, candidateSpread?: boolean, candidatePairs?: boolean): Promise<ApoScoreBlocks> {
 		return wrapBlocks(await (await this._need()).score(this._handle, ab(dims), C, T, corpus ? ab(corpus) : null, K, !!candidates,
-			!!candidateExtremes, candidateGroups ?? 0, !!candidateSpread));
+			!!candidateExtremes, candidateGroups ?? 0, !!candidateSpread, !!candidatePairs));
 	}
 
 	/** fp32 evaluations -> Form T (3 bytes per evaluation + the dictionary of distinct evaluations); undefined when the tensor is not
@@ -201,16 +211,16 @@ export class ApoScoringMainService implements IApoScoringService {
 
 	/** Same result as score() on the tensor the tuples were encoded from; 12x fewer bytes over IPC and PCIe. */
 	async scoreTuples(t: ApoTupleBuffers, C: number, T: number, corpus: VSBuffer | undefined, K: number, candidates?: boolean,
-		candidateExtremes?: boolean, candidateGroups?: number, candidateSpread?: boolean): Promise<ApoScoreBlocks> {
+		candidateExtremes?: boolean, candidateGroups?: number, candidateSpread?: boolean, candidatePairs?: boolean): Promise<ApoScoreBlocks> {
 		const raw: ApoTuples = { tl: ab(t.tl), th: ab(t.th), tbookPc: ab(t.tbookPc), tbookPd: ab(t.tbookPd), codebook: ab(t.codebook), d2book: ab(t.d2book), nTuples: t.nTuples };
 		return wrapBlocks(await (await this._need()).scoreHostTuples(this._handle, raw, C, T, corpus ? ab(corpus) : null, K, !!candidates,
-			!!candidateExtremes, candidateGroups ?? 0, !!candidateSpread));
+			!!candidateExtremes, candidateGroups ?? 0, !!candidateSpread, !!candidatePairs));
 	}
 
 	async scoreHostRecords(records: VSBuffer, rowBytes: 32 | 16, C: number, T: number, corpus: VSBuffer | undefined, K: number,
 		candidates?: boolean, candidateCorpus?: boolean, candidateExtremes?: boolean, candidateGroups?: number,
-		candidateSpread?: boolean): Promise<ApoScoreBlocks> {
+		candidateSpread?: boolean, candidatePairs?: boolean): Promise<ApoScoreBlocks> {
 		return wrapBlocks(await (await this._need()).scoreHostRecords(this._handle, ab(records), rowBytes, C, T, corpus ? ab(corpus) : null, K, !!candidates,
-			!!candidateCorpus, !!candidateExtremes, candidateGroups ?? 0, !!candidateSpread));
+			!!candidateCorpus, !!candidateExtremes, candidateGroups ?? 0, !!candidateSpread, !!candidatePairs));
 	}
 }

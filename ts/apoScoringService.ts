@@ -29,6 +29,7 @@ export interface ApoScoreBlocks {
 	candidateExtremes?: VSBuffer;   // struct apo_candidate_extremes[C] (1032 bytes each, decodeCandidateExtremes); only when asked for
 	candidateGroups?: VSBuffer;   // apo_group_score[C][G] (56 bytes each, decodeCandidateGroups); only when asked for
 	candidateSpread?: VSBuffer;   // struct apo_candidate_spread[C] (88 bytes each, decodeCandidateSpread); only when asked for
+	candidatePairs?: VSBuffer;   // struct apo_candidate_pair[C] (128 bytes each, decodeCandidatePairs); only when asked for
 }
 
 /** Form T of a float32[C][T][9] tensor (include/apo_b200.h): tl uint16[C][T] | th uint8[C][T] = the 24-bit dictionary index of every
@@ -49,6 +50,7 @@ export interface ApoResidentQuery {
 	candidateExtremes?: 0 | 1;   // also list every candidate's 32 lowest- and highest-reward rollouts (ApoScoreBlocks.candidateExtremes)
 	candidateGroups?: number;   // G of the uploaded record groups: also split every candidate's rollouts by group (ApoScoreBlocks.candidateGroups)
 	candidateSpread?: 0 | 1;   // also build every candidate's reward spread (ApoScoreBlocks.candidateSpread)
+	candidatePairs?: 0 | 1;   // also compare every candidate with its candidateRefsUpload reference (ApoScoreBlocks.candidatePairs)
 	first?: number;         // window [first, first + count) of the trace axis; count 0 = to the end
 	count?: number;
 }
@@ -80,6 +82,10 @@ export interface IApoScoringService {
 	/** One uint8 label per rollout index, each < G <= 64 (a chat mode, a task category, a held-out split): calls that pass
 	 *  candidateGroups = G then split every candidate's rollouts by these groups.  An empty buffer releases them. */
 	recordGroupsUpload(labels: VSBuffer, G: number): Promise<void>;
+	/** One uint32 per candidate: the index of its reference (its parent), or 0xFFFFFFFF for none.  Calls of C candidates that
+	 *  pass candidatePairs then compare every candidate with its reference on the rollouts both were scored on.  An empty buffer
+	 *  releases them. */
+	candidateRefsUpload(refs: VSBuffer): Promise<void>;
 	scoreResident(query: ApoResidentQuery): Promise<ApoScoreBlocks>;
 
 	// ---- one-shot path: host buffers streamed through the device, nothing stays resident
@@ -87,18 +93,19 @@ export interface IApoScoringService {
 	 *  candidates: also return the per-candidate breakdown (ApoScoreBlocks.candidates), here and on the other one-shot calls;
 	 *  candidateExtremes: also return every candidate's 32 lowest- and highest-reward rollouts (ApoScoreBlocks.candidateExtremes);
 	 *  candidateGroups: the G of recordGroupsUpload, also return every candidate's scores per record group (ApoScoreBlocks.candidateGroups);
-	 *  candidateSpread: also return every candidate's reward spread (ApoScoreBlocks.candidateSpread). */
+	 *  candidateSpread: also return every candidate's reward spread (ApoScoreBlocks.candidateSpread);
+	 *  candidatePairs: also compare every candidate with its reference (ApoScoreBlocks.candidatePairs). */
 	score(dims: VSBuffer, C: number, T: number, corpus: VSBuffer | undefined, K: number, candidates?: boolean,
-		candidateExtremes?: boolean, candidateGroups?: number, candidateSpread?: boolean): Promise<ApoScoreBlocks>;
+		candidateExtremes?: boolean, candidateGroups?: number, candidateSpread?: boolean, candidatePairs?: boolean): Promise<ApoScoreBlocks>;
 	/** [C][T] trace records (the IDE's own representation): 2.2x fewer PCIe bytes than fp32 dims with 16-byte rows.
 	 *  candidateCorpus: also return the corpus report of every candidate's records (ApoScoreBlocks.candidateCorpus). */
 	scoreHostRecords(records: VSBuffer, rowBytes: 32 | 16, C: number, T: number, corpus: VSBuffer | undefined, K: number, candidates?: boolean,
-		candidateCorpus?: boolean, candidateExtremes?: boolean, candidateGroups?: number, candidateSpread?: boolean): Promise<ApoScoreBlocks>;
+		candidateCorpus?: boolean, candidateExtremes?: boolean, candidateGroups?: number, candidateSpread?: boolean, candidatePairs?: boolean): Promise<ApoScoreBlocks>;
 	/** fp32 evaluations -> Form T (include/apo_b200.h): a 24-bit dictionary index per evaluation (3 bytes instead of 36) + the
 	 *  dictionary of distinct evaluations.  For evaluations that are scored more than once, kept, or moved between processes. */
 	encodeTuples(dims: VSBuffer, C: number, T: number): Promise<ApoTupleBuffers | undefined>;
 	scoreTuples(tuples: ApoTupleBuffers, C: number, T: number, corpus: VSBuffer | undefined, K: number, candidates?: boolean,
-		candidateExtremes?: boolean, candidateGroups?: number, candidateSpread?: boolean): Promise<ApoScoreBlocks>;
+		candidateExtremes?: boolean, candidateGroups?: number, candidateSpread?: boolean, candidatePairs?: boolean): Promise<ApoScoreBlocks>;
 }
 
 export const IApoScoringService = createDecorator<IApoScoringService>('senweaverApoScoringService');
@@ -121,16 +128,22 @@ export class ApoScoringService implements IApoScoringService {
 	corpusUploadJson(persisted: string, idxBase?: number) { return this._proxy.corpusUploadJson(persisted, idxBase); }
 	dimsTuples(cap?: number) { return this._proxy.dimsTuples(cap); }
 	recordGroupsUpload(labels: VSBuffer, G: number) { return this._proxy.recordGroupsUpload(labels, G); }
+	candidateRefsUpload(refs: VSBuffer) { return this._proxy.candidateRefsUpload(refs); }
 	scoreResident(query: ApoResidentQuery) { return this._proxy.scoreResident(query); }
-	// A call without group scores or spreads sends the channel the same arguments as before those options existed.
+	// A call without group scores, spreads or pairs sends the channel the same arguments as before those options existed.
 	score(dims: VSBuffer, C: number, T: number, corpus: VSBuffer | undefined, K: number, candidates?: boolean, candidateExtremes?: boolean,
-		candidateGroups?: number, candidateSpread?: boolean) {
+		candidateGroups?: number, candidateSpread?: boolean, candidatePairs?: boolean) {
+		if (candidatePairs) { return this._proxy.score(dims, C, T, corpus, K, candidates, candidateExtremes, candidateGroups ?? 0, !!candidateSpread, true); }
 		if (candidateSpread) { return this._proxy.score(dims, C, T, corpus, K, candidates, candidateExtremes, candidateGroups ?? 0, true); }
 		if (candidateGroups) { return this._proxy.score(dims, C, T, corpus, K, candidates, candidateExtremes, candidateGroups); }
 		return this._proxy.score(dims, C, T, corpus, K, candidates, candidateExtremes);
 	}
 	scoreHostRecords(records: VSBuffer, rowBytes: 32 | 16, C: number, T: number, corpus: VSBuffer | undefined, K: number, candidates?: boolean,
-		candidateCorpus?: boolean, candidateExtremes?: boolean, candidateGroups?: number, candidateSpread?: boolean) {
+		candidateCorpus?: boolean, candidateExtremes?: boolean, candidateGroups?: number, candidateSpread?: boolean, candidatePairs?: boolean) {
+		if (candidatePairs) {
+			return this._proxy.scoreHostRecords(records, rowBytes, C, T, corpus, K, candidates, candidateCorpus, candidateExtremes, candidateGroups ?? 0,
+				!!candidateSpread, true);
+		}
 		if (candidateSpread) {
 			return this._proxy.scoreHostRecords(records, rowBytes, C, T, corpus, K, candidates, candidateCorpus, candidateExtremes, candidateGroups ?? 0, true);
 		}
@@ -139,7 +152,10 @@ export class ApoScoringService implements IApoScoringService {
 	}
 	encodeTuples(dims: VSBuffer, C: number, T: number) { return this._proxy.encodeTuples(dims, C, T); }
 	scoreTuples(tuples: ApoTupleBuffers, C: number, T: number, corpus: VSBuffer | undefined, K: number, candidates?: boolean,
-		candidateExtremes?: boolean, candidateGroups?: number, candidateSpread?: boolean) {
+		candidateExtremes?: boolean, candidateGroups?: number, candidateSpread?: boolean, candidatePairs?: boolean) {
+		if (candidatePairs) {
+			return this._proxy.scoreTuples(tuples, C, T, corpus, K, candidates, candidateExtremes, candidateGroups ?? 0, !!candidateSpread, true);
+		}
 		if (candidateSpread) { return this._proxy.scoreTuples(tuples, C, T, corpus, K, candidates, candidateExtremes, candidateGroups ?? 0, true); }
 		if (candidateGroups) { return this._proxy.scoreTuples(tuples, C, T, corpus, K, candidates, candidateExtremes, candidateGroups); }
 		return this._proxy.scoreTuples(tuples, C, T, corpus, K, candidates, candidateExtremes);

@@ -23,8 +23,13 @@
  *  candidate's exact reward sums and the variance, standard deviation and standard error of its mean: the scale against which
  *  the gap between two candidates' scores can be read.
  *
+ *  And the decoder of the paired comparisons (ApoScoreBlocks.candidatePairs): struct apo_candidate_pair[C], each candidate
+ *  against its reference on the rollouts both were scored on: wins, losses, ties, the exact paired sums and the mean reward
+ *  difference with its standard error.
+ *
  *  The byte offsets below are pinned to the C structs by tests/test_napi_candidates.py, tests/test_candidate_corpus_cpu.py,
- *  tests/test_napi_candidate_extremes.py, tests/test_candidate_groups_cpu.py and tests/test_candidate_spread_cpu.py.
+ *  tests/test_napi_candidate_extremes.py, tests/test_candidate_groups_cpu.py, tests/test_candidate_spread_cpu.py and
+ *  tests/test_candidate_pairs_cpu.py.
  *--------------------------------------------------------------------------------------------*/
 import { VSBuffer } from '../../../../base/common/buffer.js';
 import { CorpusReportNumbers, DIM_NAMES, decodeCorpusReport } from './traceRecordCodec.js';
@@ -207,6 +212,58 @@ export function decodeCandidateSpread(buf: VSBuffer, C: number): CandidateSpread
 			candidate: c, n, sum: (v.getBigInt64(OFF_SPR_SUM_HI, true) << 64n) | v.getBigUint64(OFF_SPR_SUM_LO, true), sumSq,
 			mean: n === 0 ? null : f(OFF_SPR_MEAN), rewardSumSq: f(OFF_SPR_REWARD_SUM_SQ),
 			variance: n < 2 ? null : f(OFF_SPR_VARIANCE), stdDev: n < 2 ? null : f(OFF_SPR_STD_DEV), stdErr: n < 2 ? null : f(OFF_SPR_STD_ERR),
+		};
+	});
+}
+
+const CANDIDATE_PAIR_BYTES = 128;        // sizeof(struct apo_candidate_pair)
+const PAIR_NONE = 0xFFFFFFFF;
+const OFF_PR_REF = 0;
+const OFF_PR_N = 8;
+const OFF_PR_WINS = 16;
+const OFF_PR_LOSSES = 24;
+const OFF_PR_TIES = 32;
+const OFF_PR_CAND_ONLY = 40;
+const OFF_PR_REF_ONLY = 48;
+const OFF_PR_SUM_LO = 56;
+const OFF_PR_SUM_HI = 64;
+const OFF_PR_SUM_SQ = 72;
+const OFF_PR_MEAN_DIFF = 96;
+const OFF_PR_VARIANCE = 104;
+const OFF_PR_STD_DEV = 112;
+const OFF_PR_STD_ERR = 120;
+
+export interface CandidatePair {
+	candidate: number;
+	reference: number | null;  // null: the candidate had no reference
+	n: number;                 // positions where both have a reward
+	wins: number; losses: number; ties: number;
+	candOnly: number;          // positions where only the candidate has a reward
+	refOnly: number;           // positions where only the reference has a reward
+	sum: bigint;               // exact sum of d = rint(fr_c * 2^52) - rint(fr_r * 2^52) over the n positions
+	sumSq: bigint;             // exact sum of d^2
+	meanDiff: number | null;   // mean reward difference; null when n == 0
+	variance: number | null;   // sample variance of the differences; null when n < 2
+	stdDev: number | null;
+	stdErr: number | null;     // standard error of meanDiff
+}
+
+/** The paired comparisons of a candidatePairs block (ApoScoreBlocks.candidatePairs) of C candidates. */
+export function decodeCandidatePairs(buf: VSBuffer, C: number): CandidatePair[] {
+	if (C < 0 || C * CANDIDATE_PAIR_BYTES > buf.byteLength) { throw new RangeError(`${C} candidate pairs do not fit the block`); }
+	return Array.from({ length: C }, (_, c) => {
+		const v = new DataView(buf.buffer.buffer, buf.buffer.byteOffset + c * CANDIDATE_PAIR_BYTES, CANDIDATE_PAIR_BYTES);
+		const ref = v.getUint32(OFF_PR_REF, true);
+		const n = u64(v, OFF_PR_N);
+		const f = (o: number) => v.getFloat64(o, true);
+		const sumSq = v.getBigUint64(OFF_PR_SUM_SQ, true) | (v.getBigUint64(OFF_PR_SUM_SQ + 8, true) << 64n) |
+			(v.getBigUint64(OFF_PR_SUM_SQ + 16, true) << 128n);
+		return {
+			candidate: c, reference: ref === PAIR_NONE ? null : ref, n, wins: u64(v, OFF_PR_WINS), losses: u64(v, OFF_PR_LOSSES),
+			ties: u64(v, OFF_PR_TIES), candOnly: u64(v, OFF_PR_CAND_ONLY), refOnly: u64(v, OFF_PR_REF_ONLY),
+			sum: (v.getBigInt64(OFF_PR_SUM_HI, true) << 64n) | v.getBigUint64(OFF_PR_SUM_LO, true), sumSq,
+			meanDiff: n === 0 ? null : f(OFF_PR_MEAN_DIFF),
+			variance: n < 2 ? null : f(OFF_PR_VARIANCE), stdDev: n < 2 ? null : f(OFF_PR_STD_DEV), stdErr: n < 2 ? null : f(OFF_PR_STD_ERR),
 		};
 	});
 }
