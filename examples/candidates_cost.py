@@ -34,6 +34,12 @@ and n + refOnly against counts[], wins + losses + ties == n, nothing for a candi
 also the pairs of two candidates against the exact model of tests/pair_fixtures.py over the generated rows (every field bit
 for bit), and on the rollout legs R16 and R give the same bytes.
 
+Every leg also times the paired comparison per record group (APO_SCORE_CANDIDATE_GROUP_PAIRS) under the same refs and each of
+the groups steps' label planes (gp_<plane>), in the same alternation.  Its parity block holds, on every candidate, the
+invariants of tests/group_pair_fixtures.py against the pairs step's pairs (summed over the labels every integer field, the
+same ref in every group); on the fp32 legs also two candidates' groups against the exact model of that module over the
+generated rows, and on the rollout legs R16 and R give the same bytes.
+
     python examples/candidates_cost.py [--steps 10] [--legs D,W,Q,T,R16,R,FALL] [--out FILE.json]
 
 Prints one JSON object; the card name and power limit are read in the same run (nvidia-smi query)."""
@@ -196,6 +202,31 @@ def pairs_block(last, med, ref_pair):
             "parity_pairs": pairs_parity(last["pairs"], ref_pair)}
 
 
+def group_pairs_parity(last, gsets, ref_gpair):
+    """the invariants on every candidate against the pairs step's pairs (the same refs and rows); ref_gpair: {candidate: {set
+    name: model row [G]}}"""
+    import group_pair_fixtures as gpf
+    out = {}
+    for k, (lab, G) in gsets.items():
+        try:
+            gpf.invariants(last[k].group_pairs, last["pairs"].pairs, G)
+            every = True
+        except AssertionError:
+            every = False
+        ok = {c: [pair_row(x) for x in last[k].group_pairs[c]] == [model_pair(m) for m in rows[k[3:]]] for c, rows in (ref_gpair or {}).items()}
+        out[k] = {"invariants_every_candidate": every, "per_candidate": ok, "equal": every and all(ok.values())}
+    return {"sets": out, "equal": all(v["equal"] for v in out.values())}
+
+
+def group_pairs_block(last, med, gsets, ref_gpair):
+    return {"group_pairs_ms_median": {k: round(med[k], 3) for k in gsets},
+            "group_pairs_ratio": {k: round(med[k] / med["plain"], 3) for k in gsets},
+            "group_pairs_vs_pairs": {k: round(med[k] / med["pairs"], 3) for k in gsets},
+            "group_pairs_same_scores": all(last[k].scores.tobytes() == last["plain"].scores.tobytes()
+                                           and last[k].topk.tobytes() == last["plain"].topk.tobytes() for k in gsets),
+            "parity_group_pairs": group_pairs_parity(last, gsets, ref_gpair)}
+
+
 def timed(eng, C, K, steps, score_kw, kinds, sets):
     """median / min of every kind of step, alternating; a group step first uploads its labels (outside the timing)"""
     times = {k: [] for k in kinds}
@@ -225,15 +256,18 @@ def groups_block(last, med, sets, ref_grp):
             "parity_groups": groups_parity(last, sets, ref_grp)}
 
 
-def leg(eng, C, K, steps, score_kw, ref, picks, ref_ext=None, sets=None, ref_grp=None, ref_spr=None, ref_pair=None):
-    """plain / candidates / extremes / groups / spread / pairs steps, alternating (ref None: the breakdown is not timed)"""
+def leg(eng, C, K, steps, score_kw, ref, picks, ref_ext=None, sets=None, ref_grp=None, ref_spr=None, ref_pair=None, ref_gpair=None):
+    """plain / candidates / extremes / groups / spread / pairs / group_pairs steps, alternating (ref None: the breakdown is not
+    timed)"""
     sets = sets or {}
+    gsets = {f"gp_{k}": v for k, v in sets.items()}                 # the per-group pairs under each label plane
     kinds = {"plain": {}, "extremes": {"extremes": True}, "spread": {"spread": True}, "pairs": {"pairs": True}}
     eng.candidate_refs_upload(beam_refs(C))
     if ref is not None:
         kinds["candidates"] = {"candidates": True}
     kinds.update({k: {"groups": True} for k in sets})
-    last, times, med = timed(eng, C, K, steps, score_kw, kinds, sets)
+    kinds.update({k: {"group_pairs": True} for k in gsets})
+    last, times, med = timed(eng, C, K, steps, score_kw, kinds, {**sets, **gsets})
     out = {"plain_ms_median": round(med["plain"], 3), "extremes_ms_median": round(med["extremes"], 3),
            "extremes_ratio": round(med["extremes"] / med["plain"], 3), "min_ms": {k: round(min(v) * 1e3, 3) for k, v in times.items()},
            "launches": {k: int(r.timing.launches) for k, r in last.items()},
@@ -243,6 +277,7 @@ def leg(eng, C, K, steps, score_kw, ref, picks, ref_ext=None, sets=None, ref_grp
     out.update(groups_block(last, med, sets, ref_grp))
     out.update(spread_block(eng, last, med, ref_spr))
     out.update(pairs_block(last, med, ref_pair))
+    out.update(group_pairs_block(last, med, gsets, ref_gpair))
     if ref is not None:
         r = last["candidates"]
         ok = [same(r.candidates[c], d) for c, d in zip(picks, ref)]
@@ -291,12 +326,15 @@ def parity_block(picks, diffs):
 
 
 def corpus_leg(eng, C, K, steps, score_kw, ref, picks, ref_corpus, sets):
-    """plain / candidates / candidate_corpus / extremes / groups / spread / pairs steps, alternating, with the parity blocks"""
+    """plain / candidates / candidate_corpus / extremes / groups / spread / pairs / group_pairs steps, alternating, with the
+    parity blocks"""
     kinds = {"plain": {}, "candidates": {"candidates": True}, "candidate_corpus": {"candidate_corpus": True}, "extremes": {"extremes": True},
              "spread": {"spread": True}, "pairs": {"pairs": True}}
+    gsets = {f"gp_{k}": v for k, v in sets.items()}
     eng.candidate_refs_upload(beam_refs(C))
     kinds.update({k: {"groups": True} for k in sets})
-    last, times, med = timed(eng, C, K, steps, score_kw, kinds, sets)
+    kinds.update({k: {"group_pairs": True} for k in gsets})
+    last, times, med = timed(eng, C, K, steps, score_kw, kinds, {**sets, **gsets})
     ok = [same(last["candidates"].candidates[c], d) for c, d in zip(picks, ref)]
     import exact_report as xr
     cc = last["candidate_corpus"].candidate_corpus
@@ -305,6 +343,7 @@ def corpus_leg(eng, C, K, steps, score_kw, ref, picks, ref_corpus, sets):
     return {**groups_block(last, med, sets, None), "groups_bytes": b"".join(bytes(last[k].groups) for k in sets),
             **spread_block(eng, last, med, None), "spread_bytes": bytes(last["spread"].spread),
             **pairs_block(last, med, None), "pairs_bytes": bytes(last["pairs"].pairs),
+            **group_pairs_block(last, med, gsets, None), "group_pairs_bytes": b"".join(bytes(last[k].group_pairs) for k in gsets),
             "plain_ms_median": round(med["plain"], 3), "candidates_ms_median": round(med["candidates"], 3),
             "candidate_corpus_ms_median": round(med["candidate_corpus"], 3),
             "candidates_ratio": round(med["candidates"] / med["plain"], 3),
@@ -333,6 +372,7 @@ def main():
     import group_fixtures as gf
     import spread_fixtures as sf
     import pair_fixtures as pf
+    import group_pair_fixtures as gpf
     legs = args.legs.split(",")
     out = {"card": card(), "steps": args.steps, "timing": "host clock around each synchronous apo_score call"}
     eng = pkg.Engine(0)
@@ -350,24 +390,25 @@ def main():
                 ref_grp[c] = {k: gf.model(d, lab, G)[0] for k, (lab, G) in sets.items()}
                 ref_spr[c] = sf.model(d)[0]
                 del d
-            refs, ref_pair = beam_refs(C), {}
+            refs, ref_pair, ref_gpair = beam_refs(C), {}, {}
             for c in (1, C - 2):                            # a child of candidate 0 and one of the last block's
                 r = int(refs[c])
                 d = np.concatenate([oracle.gen_dims(seed, c, 1, 0, T, 300, nth), oracle.gen_dims(seed, r, 1, 0, T, 300, nth)])
                 ref_pair[c] = pf.model(d, [1, pf.NONE])[0] | {"ref": r}
+                ref_gpair[c] = {k: [m | {"ref": r} for m in gpf.model(d, [1, pf.NONE], lab, G)[0]] for k, (lab, G) in sets.items()}
                 del d
             if "D" in legs:
                 eng.dims_generate(seed, 0, C, 0, T, 300)
-                out["form_d_256x5M"] = leg(eng, C, K, args.steps, {}, ref, picks, ref_ext, sets, ref_grp, ref_spr, ref_pair)
+                out["form_d_256x5M"] = leg(eng, C, K, args.steps, {}, ref, picks, ref_ext, sets, ref_grp, ref_spr, ref_pair, ref_gpair)
             if "W" in legs:
                 eng.dims_generate(seed, 0, C, 0, T, 300)
                 eng.set_tuning(pkg.TUNE_NO_TWIN_T)
-                out["form_w_copy_256x5M"] = leg(eng, C, K, args.steps, {}, ref, picks, ref_ext, sets, ref_grp, ref_spr, ref_pair)
+                out["form_w_copy_256x5M"] = leg(eng, C, K, args.steps, {}, ref, picks, ref_ext, sets, ref_grp, ref_spr, ref_pair, ref_gpair)
                 eng.set_tuning(0)
             if "Q" in legs or "T" in legs:
                 eng.dims_generate_compact(seed, 0, C, 0, T, 300)
             if "Q" in legs:
-                out["form_q_256x5M"] = leg(eng, C, K, args.steps, {}, ref, picks, ref_ext, sets, ref_grp, ref_spr, ref_pair)
+                out["form_q_256x5M"] = leg(eng, C, K, args.steps, {}, ref, picks, ref_ext, sets, ref_grp, ref_spr, ref_pair, ref_gpair)
             if "T" in legs:
                 pc, pd = np.empty((C, T), np.uint32), np.empty((C, T), np.uint16)
                 for c in range(C):
@@ -377,7 +418,7 @@ def main():
                 del pc, pd
                 eng.tuples_upload(tl, th, tbook, book, d2book)
                 del tl, th
-                out["form_t_256x5M"] = leg(eng, C, K, args.steps, {"source": pkg.SRC_TUPLES}, ref, picks, ref_ext, sets, ref_grp, ref_spr, ref_pair)
+                out["form_t_256x5M"] = leg(eng, C, K, args.steps, {"source": pkg.SRC_TUPLES}, ref, picks, ref_ext, sets, ref_grp, ref_spr, ref_pair, ref_gpair)
         if {"R16", "R"} & set(legs):
             Cr = 128
             picks_r = [int(x) for x in np.linspace(0, Cr - 1, 8).round()]
@@ -396,11 +437,13 @@ def main():
                 out["r16_r_groups_equal"] = out["form_r16_128x5M"]["groups_bytes"] == out["form_r_128x5M"]["groups_bytes"]
                 out["r16_r_spread_equal"] = out["form_r16_128x5M"]["spread_bytes"] == out["form_r_128x5M"]["spread_bytes"]
                 out["r16_r_pairs_equal"] = out["form_r16_128x5M"]["pairs_bytes"] == out["form_r_128x5M"]["pairs_bytes"]
+                out["r16_r_group_pairs_equal"] = out["form_r16_128x5M"]["group_pairs_bytes"] == out["form_r_128x5M"]["group_pairs_bytes"]
             for k in ("form_r16_128x5M", "form_r_128x5M"):
                 out.get(k, {}).pop("extremes_bytes", None)
                 out.get(k, {}).pop("groups_bytes", None)
                 out.get(k, {}).pop("spread_bytes", None)
                 out.get(k, {}).pop("pairs_bytes", None)
+                out.get(k, {}).pop("group_pairs_bytes", None)
         if "FALL" in legs:
             Cf, Tf = 64, 1_000_000
             d = xf.falling(Tf, 1)

@@ -577,6 +577,22 @@ struct apo_candidate_pair {
 /* Pairs of candidates [c0, c0 + n) of the last scoring call: APO_E_STATE when that call did not set the flag (or failed),
  * APO_E_ARG when the range exceeds its C. */
 int apo_candidate_pairs(apo_engine *e, uint32_t c0, uint32_t n, struct apo_candidate_pair *out);
+/* The paired comparison per record group: did c beat its reference on the held-out records (or any other split the labels
+ * name), and by more than the paired noise there?  A scoring call that sets APO_SCORE_CANDIDATE_GROUP_PAIRS builds, for every
+ * candidate c and label g < G, the fields of apo_candidate_pair restricted to the record positions t with labels[t] == g
+ * (labels from apo_record_groups_upload, r = refs[c] from apo_candidate_refs_upload): n / wins / losses / ties over the
+ * positions where both rows have a finalReward, candOnly / refOnly over those where one has, D1 and D2 exact, the doubles by
+ * the pairs' rules, ref = r; a candidate with APO_PAIR_NONE has every count and sum 0 and every double NaN in every group.
+ * Summed over g, every integer field is the one apo_candidate_pairs gives.  Positions are absolute as for the group scores and
+ * pairs.  Works wherever APO_SCORE_CANDIDATE_PAIRS works, needs neither GROUPS nor PAIRS set, combines with every other
+ * per-candidate flag and leaves every other output as it is.  Refusals, before anything is launched: those of both passes
+ * (APO_E_STATE: no labels or no refs held, more than one rank, at a session's finish an accumulate without the flag or labels
+ * or refs uploaded again after the session began accumulating them; APO_E_ARG: a scored position at or past the labels' T,
+ * the refs' C not the call's C, an accumulated chunk holding a candidate whose reference lies outside it). */
+#define APO_SCORE_CANDIDATE_GROUP_PAIRS 0x200u /* also compare every candidate with its reference per record group */
+/* out[n][G]: pairs of candidates [c0, c0 + n) of the last scoring call per label.  APO_E_STATE when that call did not set the
+ * flag (or failed); APO_E_ARG when G is not the G it split by, or the range exceeds its C. */
+int apo_candidate_group_pairs(apo_engine *e, uint32_t c0, uint32_t n, uint32_t G, struct apo_candidate_pair *out);
 
 /* ---- multi-GPU: the record axis is sharded across ranks (one process per GPU, or one handle per GPU inside one
  * process); the packed int64 partial vectors of the shards are joined INSIDE the scoring launch: the finalising CTA

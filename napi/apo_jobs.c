@@ -169,6 +169,15 @@ int apo_job_validate(apo_job *j)
 		if (!fits(j->C, sizeof(struct apo_candidate_pair), 1, APO_JOB_CANDIDATE_PAIRS_MAX_BYTES))
 			return bad(j, "the paired comparisons of C candidates exceed 4 GiB");
 	}
+	if (j->flags & APO_SCORE_CANDIDATE_GROUP_PAIRS) {
+		if (j->kind != APO_JOB_SCORE_RESIDENT && j->kind != APO_JOB_SCORE_HOST && j->kind != APO_JOB_SCORE_HOST_RECORDS &&
+		    j->kind != APO_JOB_SCORE_HOST_TUPLES)
+			return bad(j, "the paired comparisons per record group belong to a scoring call");
+		if (j->C == 0) return bad(j, "C must be > 0 for the paired comparisons per record group");
+		if (j->G == 0 || j->G > APO_GROUPS_MAX) return bad(j, "G must be 1..64 for the paired comparisons per record group");
+		if (!fits(j->C, j->G, sizeof(struct apo_candidate_pair), APO_JOB_CANDIDATE_GROUP_PAIRS_MAX_BYTES))
+			return bad(j, "the paired comparisons per record group of C candidates and G groups exceed 4 GiB");
+	}
 	return APO_OK;
 }
 
@@ -188,12 +197,15 @@ int apo_job_prepare(apo_job *j)
 			j->candidate_spread = (struct apo_candidate_spread *)malloc(sizeof(struct apo_candidate_spread) * (size_t)C);
 		if (j->flags & APO_SCORE_CANDIDATE_PAIRS)
 			j->candidate_pairs = (struct apo_candidate_pair *)malloc(sizeof(struct apo_candidate_pair) * (size_t)C);
+		if (j->flags & APO_SCORE_CANDIDATE_GROUP_PAIRS)
+			j->candidate_group_pairs = (struct apo_candidate_pair *)malloc(sizeof(struct apo_candidate_pair) * (size_t)C * j->G);
 		if (!j->scores || !j->counts || !j->topk || ((j->flags & APO_SCORE_CANDIDATES) && !j->candidates) ||
 		    ((j->flags & APO_SCORE_CANDIDATE_CORPUS) && !j->candidate_corpus) ||
 		    ((j->flags & APO_SCORE_CANDIDATE_EXTREMES) && !j->candidate_extremes) ||
 		    ((j->flags & APO_SCORE_CANDIDATE_GROUPS) && !j->candidate_groups) ||
 		    ((j->flags & APO_SCORE_CANDIDATE_SPREAD) && !j->candidate_spread) ||
-		    ((j->flags & APO_SCORE_CANDIDATE_PAIRS) && !j->candidate_pairs)) {
+		    ((j->flags & APO_SCORE_CANDIDATE_PAIRS) && !j->candidate_pairs) ||
+		    ((j->flags & APO_SCORE_CANDIDATE_GROUP_PAIRS) && !j->candidate_group_pairs)) {
 			apo_job_release(j); j->rc = APO_E_NOMEM; snprintf(j->err, sizeof j->err, "out of host memory"); return APO_E_NOMEM;
 		}
 	} else if (j->kind == APO_JOB_REWARD_BATCH) {
@@ -210,10 +222,10 @@ void apo_job_release(apo_job *j)
 {
 	free(j->scores); free(j->counts); free(j->topk); free(j->dims_out); free(j->masks_out); free(j->finals_out); free(j->candidates);
 	free(j->candidate_corpus); free(j->candidate_extremes); free(j->candidate_groups); free(j->candidate_spread);
-	free(j->candidate_pairs);
+	free(j->candidate_pairs); free(j->candidate_group_pairs);
 	j->scores = NULL; j->counts = NULL; j->topk = NULL; j->dims_out = NULL; j->masks_out = NULL; j->finals_out = NULL; j->candidates = NULL;
 	j->candidate_corpus = NULL; j->candidate_extremes = NULL; j->candidate_groups = NULL; j->candidate_spread = NULL;
-	j->candidate_pairs = NULL;
+	j->candidate_pairs = NULL; j->candidate_group_pairs = NULL;
 }
 
 static void execute(apo_serial *s, apo_job *j)
@@ -288,6 +300,7 @@ static void execute(apo_serial *s, apo_job *j)
 	if (j->rc == APO_OK && j->candidate_groups) j->rc = apo_candidate_groups(e, 0, j->C, j->G, j->candidate_groups);
 	if (j->rc == APO_OK && j->candidate_spread) j->rc = apo_candidate_spread(e, 0, j->C, j->candidate_spread);
 	if (j->rc == APO_OK && j->candidate_pairs) j->rc = apo_candidate_pairs(e, 0, j->C, j->candidate_pairs);
+	if (j->rc == APO_OK && j->candidate_group_pairs) j->rc = apo_candidate_group_pairs(e, 0, j->C, j->G, j->candidate_group_pairs);
 	if (j->rc != APO_OK) snprintf(j->err, sizeof j->err, "%s", apo_last_error(e));
 }
 

@@ -43,10 +43,10 @@ typedef enum {
 	APO_JOB_ROLLOUTS_UPLOAD,       /* rolloutsUpload(handle, recs, rowBytes 32|16, C, T)         */
 	APO_JOB_CORPUS_UPLOAD,         /* corpusUpload(handle, recs apo_record[T], idxBase)          */
 	APO_JOB_CORPUS_UPLOAD_JSON,    /* corpusUploadJson(handle, utf8, idxBase)                    */
-	APO_JOB_SCORE_RESIDENT,        /* scoreResident(handle, {K, source, corpus, first, count, candidates, candidateCorpus, candidateExtremes, candidateGroups, candidateSpread, candidatePairs}) */
-	APO_JOB_SCORE_HOST,            /* score(handle, dims, C, T, corpus|null, K, candidates?, candidateExtremes?, candidateGroups?, candidateSpread?, candidatePairs?) */
-	APO_JOB_SCORE_HOST_RECORDS,    /* scoreHostRecords(handle, recs, rowBytes, C, T, corpus|null, K, candidates?, candidateCorpus?, candidateExtremes?, candidateGroups?, candidateSpread?, candidatePairs?) */
-	APO_JOB_SCORE_HOST_TUPLES,     /* scoreHostTuples(handle, {tl, th, tbookPc, tbookPd, codebook, d2book}, C, T, corpus|null, K, candidates?, candidateExtremes?, candidateGroups?, candidateSpread?, candidatePairs?) */
+	APO_JOB_SCORE_RESIDENT,        /* scoreResident(handle, {K, source, corpus, first, count, candidates, candidateCorpus, candidateExtremes, candidateGroups, candidateSpread, candidatePairs, candidateGroupPairs}) */
+	APO_JOB_SCORE_HOST,            /* score(handle, dims, C, T, corpus|null, K, candidates?, candidateExtremes?, candidateGroups?, candidateSpread?, candidatePairs?, candidateGroupPairs?) */
+	APO_JOB_SCORE_HOST_RECORDS,    /* scoreHostRecords(handle, recs, rowBytes, C, T, corpus|null, K, candidates?, candidateCorpus?, candidateExtremes?, candidateGroups?, candidateSpread?, candidatePairs?, candidateGroupPairs?) */
+	APO_JOB_SCORE_HOST_TUPLES,     /* scoreHostTuples(handle, {tl, th, tbookPc, tbookPd, codebook, d2book}, C, T, corpus|null, K, candidates?, candidateExtremes?, candidateGroups?, candidateSpread?, candidatePairs?, candidateGroupPairs?) */
 	APO_JOB_REWARD_BATCH,          /* rewardBatch(handle, recs apo_record[n])                    */
 	APO_JOB_COMM_INIT,             /* commInit(handle, nranks, rank, id[128])                    */
 	APO_JOB_TEST_HOOK,             /* tests: calls hook(hook_arg) in its turn                    */
@@ -78,6 +78,7 @@ typedef struct apo_job {
 	apo_group_score *candidate_groups;            /* [C][G], only when flags has APO_SCORE_CANDIDATE_GROUPS (apo_candidate_groups) */
 	struct apo_candidate_spread *candidate_spread;   /* [C], only when flags has APO_SCORE_CANDIDATE_SPREAD (apo_candidate_spread) */
 	struct apo_candidate_pair *candidate_pairs;      /* [C], only when flags has APO_SCORE_CANDIDATE_PAIRS (apo_candidate_pairs) */
+	struct apo_candidate_pair *candidate_group_pairs;   /* [C][G], only when flags has APO_SCORE_CANDIDATE_GROUP_PAIRS (apo_candidate_group_pairs) */
 	double *dims_out; uint32_t *masks_out; double *finals_out; uint64_t n_out;
 	int rc; char err[256];
 } apo_job;
@@ -98,6 +99,9 @@ typedef struct apo_job {
 #define APO_JOB_CANDIDATE_SPREAD_MAX_BYTES (1ull << 32)
 /* Same cap for the paired comparisons (C x sizeof(struct apo_candidate_pair) = 128 B).  They belong to every scoring job. */
 #define APO_JOB_CANDIDATE_PAIRS_MAX_BYTES (1ull << 32)
+/* Same cap for the paired comparisons per record group (C x G x sizeof(struct apo_candidate_pair) = 128 B each).  They belong
+ * to every scoring job and split by the job's G. */
+#define APO_JOB_CANDIDATE_GROUP_PAIRS_MAX_BYTES (1ull << 32)
 
 /* Shape / size / overflow checks that need no engine; 0 = fine, else APO_E_ARG with the reason in j->err.
  * Everything that arrives from the renderer over IPC passes through here before a pointer is dereferenced. */

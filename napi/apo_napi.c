@@ -28,11 +28,12 @@
  *   dimsTuples(h, cap?)                                                     -> Promise<number>   (nTuples) resident Form T from the loaded dims
  *   recordGroupsUpload(h, labels:ArrayBuffer u8[T], G)                      -> Promise<void>     the record group of every position
  *   candidateRefsUpload(h, refs:ArrayBuffer u32[C])                          -> Promise<void>     the reference of every candidate
- *   scoreResident(h, {C, K, source, corpus, first, count, candidates, candidateCorpus, candidateExtremes, candidateGroups, candidateSpread, candidatePairs}) -> Promise<blocks>   ... scored many times
- *   score(h, dims, C, T, corpus|null, K, candidates?, candidateExtremes?, candidateGroups?, candidateSpread?, candidatePairs?) -> Promise<blocks>   host streaming, Form D
- *   scoreHostRecords(h, recs, rowBytes, C, T, corpus|null, K, candidates?, candidateCorpus?, candidateExtremes?, candidateGroups?, candidateSpread?, candidatePairs?) -> Promise<blocks>   host streaming, trace records
- *   scoreHostTuples(h, {tl, th, ...}, C, T, corpus|null, K, candidates?, candidateExtremes?, candidateGroups?, candidateSpread?, candidatePairs?) -> Promise<blocks>   host streaming, Form T
- *   candidateGroups is the G the labels were uploaded with (0 / absent: no group scores)
+ *   scoreResident(h, {C, K, source, corpus, first, count, candidates, candidateCorpus, candidateExtremes, candidateGroups, candidateSpread, candidatePairs, candidateGroupPairs}) -> Promise<blocks>   ... scored many times
+ *   score(h, dims, C, T, corpus|null, K, candidates?, candidateExtremes?, candidateGroups?, candidateSpread?, candidatePairs?, candidateGroupPairs?) -> Promise<blocks>   host streaming, Form D
+ *   scoreHostRecords(h, recs, rowBytes, C, T, corpus|null, K, candidates?, candidateCorpus?, candidateExtremes?, candidateGroups?, candidateSpread?, candidatePairs?, candidateGroupPairs?) -> Promise<blocks>   host streaming, trace records
+ *   scoreHostTuples(h, {tl, th, ...}, C, T, corpus|null, K, candidates?, candidateExtremes?, candidateGroups?, candidateSpread?, candidatePairs?, candidateGroupPairs?) -> Promise<blocks>   host streaming, Form T
+ *   candidateGroups is the G the labels were uploaded with (0 / absent: no group scores); so is candidateGroupPairs (0 / absent:
+ *   no paired comparisons per record group); a call that names both names one G
  *   rewardBatch(h, recs:ArrayBuffer apo_record[n])                          -> Promise<{dims,masks,finals}>
  *   commUniqueId() -> ArrayBuffer(128) | null     commInit(h, nranks, rank, id) -> Promise<void>
  *   recordsFromJson(utf8) -> ArrayBuffer | null   allocPinned(bytes) -> ArrayBuffer | null      (host-only helpers)
@@ -45,7 +46,9 @@
  *             candidateGroups?:ArrayBuffer apo_group_score[C][G] (only when the call asked for the per-candidate group scores),
  *             candidateSpread?:ArrayBuffer struct apo_candidate_spread[C] (only when the call asked for the per-candidate reward
  *             spreads),
- *             candidatePairs?:ArrayBuffer struct apo_candidate_pair[C] (only when the call asked for the paired comparisons)}
+ *             candidatePairs?:ArrayBuffer struct apo_candidate_pair[C] (only when the call asked for the paired comparisons),
+ *             candidateGroupPairs?:ArrayBuffer struct apo_candidate_pair[C][G] (only when the call asked for the paired comparisons
+ *             per record group)}
  */
 #include <stdint.h>
 #include <stdio.h>
@@ -157,6 +160,8 @@ static napi_value blocks_of(napi_env env, const apo_job *j)
 		napi_set_named_property(env, out, "candidateSpread", v);
 	if (j->candidate_pairs && (v = copy_out(env, j->candidate_pairs, sizeof(struct apo_candidate_pair) * (size_t)C)))
 		napi_set_named_property(env, out, "candidatePairs", v);
+	if (j->candidate_group_pairs && (v = copy_out(env, j->candidate_group_pairs, sizeof(struct apo_candidate_pair) * (size_t)C * j->G)))
+		napi_set_named_property(env, out, "candidateGroupPairs", v);
 	return out;
 }
 
@@ -373,8 +378,12 @@ static int opt_bool_arg(napi_env env, napi_value v, int *out)
 	return 1;
 }
 
+/* candidateGroups (g) and candidateGroupPairs (gp) both name the G the labels were uploaded with, and the job holds one G:
+ * 0 when a call names a different G for each, else the one it names (0: neither) */
+static uint32_t one_G(uint32_t g, uint32_t gp) { return g && gp && g != gp ? 0u : g ? g : gp; }
+
 /* scoreResident(h, {C, K, source?, corpus?, first?, count?, candidates?, candidateCorpus?, candidateExtremes?, candidateGroups?,
- * candidateSpread?, candidatePairs?}): scores what dimsUpload / rolloutsUpload / corpusUpload left
+ * candidateSpread?, candidatePairs?, candidateGroupPairs?}): scores what dimsUpload / rolloutsUpload / corpusUpload left
  * resident — "uploaded once, scored many times" (SURVEY 8b ownership row); nothing crosses PCIe but the result block. */
 static napi_value ScoreResident(napi_env env, napi_callback_info info)
 {
@@ -382,29 +391,32 @@ static napi_value ScoreResident(napi_env env, napi_callback_info info)
 	call_t *c = argc >= 1 ? new_call(env, argv[0], APO_JOB_SCORE_RESIDENT) : NULL;
 	if (!c) return reject_now(env, "scoreResident: invalid handle");
 	napi_valuetype t;
-	uint32_t corpus = 0, cands = 0, ccorp = 0, cext = 0, cspr = 0, cpair = 0;
-	if (argc < 2 || napi_typeof(env, argv[1], &t) != napi_ok || t != napi_object || !opt_u32(env, argv[1], "candidateGroups", &c->job.G) ||
+	uint32_t corpus = 0, cands = 0, ccorp = 0, cext = 0, cspr = 0, cpair = 0, g = 0, gp = 0;
+	if (argc < 2 || napi_typeof(env, argv[1], &t) != napi_ok || t != napi_object || !opt_u32(env, argv[1], "candidateGroups", &g) ||
+	    !opt_u32(env, argv[1], "candidateGroupPairs", &gp) || ((g || gp) && !one_G(g, gp)) ||
 	    !opt_u32(env, argv[1], "C", &c->job.C) || !opt_u32(env, argv[1], "K", &c->job.K) || !opt_u32(env, argv[1], "source", &c->job.source) ||
 	    !opt_u32(env, argv[1], "corpus", &corpus) || !opt_u64(env, argv[1], "first", &c->job.first) || !opt_u64(env, argv[1], "count", &c->job.count) ||
 	    !opt_u32(env, argv[1], "candidates", &cands) || cands > 1 || !opt_u32(env, argv[1], "candidateCorpus", &ccorp) || ccorp > 1 ||
 	    !opt_u32(env, argv[1], "candidateExtremes", &cext) || cext > 1 || !opt_u32(env, argv[1], "candidateSpread", &cspr) || cspr > 1 ||
 	    !opt_u32(env, argv[1], "candidatePairs", &cpair) || cpair > 1)
-		arg_error(c, "scoreResident(handle, {C:uint32, K:uint32, source?:0|1|2, corpus?:0|1, first?:uint53, count?:uint53, candidates?:0|1, candidateCorpus?:0|1, candidateExtremes?:0|1, candidateGroups?:G, candidateSpread?:0|1, candidatePairs?:0|1})");
+		arg_error(c, "scoreResident(handle, {C:uint32, K:uint32, source?:0|1|2, corpus?:0|1, first?:uint53, count?:uint53, candidates?:0|1, candidateCorpus?:0|1, candidateExtremes?:0|1, candidateGroups?:G, candidateSpread?:0|1, candidatePairs?:0|1, candidateGroupPairs?:G (the same G as candidateGroups)})");
+	c->job.G = one_G(g, gp);
 	if (c->job.C == 0) arg_error(c, "scoreResident: C (the number of uploaded candidates) is required");
 	if (c->job.K > c->job.C) arg_error(c, "scoreResident: K exceeds C");
 	c->job.flags = (corpus ? APO_SCORE_CORPUS : 0) | (cands ? APO_SCORE_CANDIDATES : 0) | (ccorp ? APO_SCORE_CANDIDATE_CORPUS : 0) |
-	               (cext ? APO_SCORE_CANDIDATE_EXTREMES : 0) | (c->job.G ? APO_SCORE_CANDIDATE_GROUPS : 0) | (cspr ? APO_SCORE_CANDIDATE_SPREAD : 0) |
-	               (cpair ? APO_SCORE_CANDIDATE_PAIRS : 0);
+	               (cext ? APO_SCORE_CANDIDATE_EXTREMES : 0) | (g ? APO_SCORE_CANDIDATE_GROUPS : 0) | (cspr ? APO_SCORE_CANDIDATE_SPREAD : 0) |
+	               (cpair ? APO_SCORE_CANDIDATE_PAIRS : 0) | (gp ? APO_SCORE_CANDIDATE_GROUP_PAIRS : 0);
 	return submit(env, c, argv[0], NULL, NULL, "apo_score");
 }
 
 static napi_value score_host_common(napi_env env, napi_callback_info info, apo_job_kind kind)
 {
 	const int rec = kind == APO_JOB_SCORE_HOST_RECORDS;
-	ARGS(13)
+	ARGS(14)
 	call_t *c = argc >= 1 ? new_call(env, argv[0], kind) : NULL;
 	if (!c) return reject_now(env, "score: invalid handle");
 	int cands = 0, ccorp = 0, cext = 0, cspr = 0, cpair = 0;
+	uint32_t g = 0, gp = 0;
 	const size_t base = rec ? 3 : 2;              /* index of C */
 	const size_t need = base + 4;                 /* ..., C, T, corpus, K */
 	int ok = argc >= need && get_buffer(env, argv[1], &c->job.buf, &c->job.buf_bytes);
@@ -419,13 +431,17 @@ static napi_value score_host_common(napi_env env, napi_callback_info info, apo_j
 	if (ok && rec && argc > need + 1) ok = opt_bool_arg(env, argv[need + 1], &ccorp);     /* trace records only */
 	const size_t ext_at = rec ? need + 2 : need + 1;
 	if (ok && argc > ext_at) ok = opt_bool_arg(env, argv[ext_at], &cext);
-	if (ok && argc > ext_at + 1 && !is_nullish(env, argv[ext_at + 1])) ok = get_u32(env, argv[ext_at + 1], &c->job.G);
+	if (ok && argc > ext_at + 1 && !is_nullish(env, argv[ext_at + 1])) ok = get_u32(env, argv[ext_at + 1], &g);
 	if (ok && argc > ext_at + 2) ok = opt_bool_arg(env, argv[ext_at + 2], &cspr);
-	if (ok && argc > ext_at + 3) ok = opt_bool_arg(env, argv[ext_at + 3], &cpair);    /* the last optional argument */
+	if (ok && argc > ext_at + 3) ok = opt_bool_arg(env, argv[ext_at + 3], &cpair);
+	if (ok && argc > ext_at + 4 && !is_nullish(env, argv[ext_at + 4])) ok = get_u32(env, argv[ext_at + 4], &gp);   /* the last optional argument */
+	if (ok && (g || gp)) ok = one_G(g, gp) != 0;
+	c->job.G = one_G(g, gp);
 	c->job.flags = (cands ? APO_SCORE_CANDIDATES : 0) | (ccorp ? APO_SCORE_CANDIDATE_CORPUS : 0) | (cext ? APO_SCORE_CANDIDATE_EXTREMES : 0) |
-	               (c->job.G ? APO_SCORE_CANDIDATE_GROUPS : 0) | (cspr ? APO_SCORE_CANDIDATE_SPREAD : 0) | (cpair ? APO_SCORE_CANDIDATE_PAIRS : 0);
-	if (!ok) arg_error(c, rec ? "scoreHostRecords(handle, recs:ArrayBuffer, rowBytes:32|16, C:uint32, T:uint53, corpus:ArrayBuffer|null, K:uint32, candidates?:boolean, candidateCorpus?:boolean, candidateExtremes?:boolean, candidateGroups?:G, candidateSpread?:boolean, candidatePairs?:boolean)"
-	                          : "score(handle, dims:ArrayBuffer, C:uint32, T:uint53, corpus:ArrayBuffer|null, K:uint32, candidates?:boolean, candidateExtremes?:boolean, candidateGroups?:G, candidateSpread?:boolean, candidatePairs?:boolean)");
+	               (g ? APO_SCORE_CANDIDATE_GROUPS : 0) | (cspr ? APO_SCORE_CANDIDATE_SPREAD : 0) | (cpair ? APO_SCORE_CANDIDATE_PAIRS : 0) |
+	               (gp ? APO_SCORE_CANDIDATE_GROUP_PAIRS : 0);
+	if (!ok) arg_error(c, rec ? "scoreHostRecords(handle, recs:ArrayBuffer, rowBytes:32|16, C:uint32, T:uint53, corpus:ArrayBuffer|null, K:uint32, candidates?:boolean, candidateCorpus?:boolean, candidateExtremes?:boolean, candidateGroups?:G, candidateSpread?:boolean, candidatePairs?:boolean, candidateGroupPairs?:G)"
+	                          : "score(handle, dims:ArrayBuffer, C:uint32, T:uint53, corpus:ArrayBuffer|null, K:uint32, candidates?:boolean, candidateExtremes?:boolean, candidateGroups?:G, candidateSpread?:boolean, candidatePairs?:boolean, candidateGroupPairs?:G)");
 	return submit(env, c, argv[0], c->job.buf ? argv[1] : NULL, corpus, rec ? "apo_score_host_records" : "apo_score_host");
 }
 static napi_value Score(napi_env env, napi_callback_info info) { return score_host_common(env, info, APO_JOB_SCORE_HOST); }
@@ -512,12 +528,12 @@ static napi_value EncodeTuples(napi_env env, napi_callback_info info)
 }
 
 /* scoreHostTuples(h, {tl, th, tbookPc, tbookPd, codebook, d2book, nTuples}, C, T, corpus|null, K, candidates?, candidateExtremes?, candidateGroups?,
- * candidateSpread?, candidatePairs?) -> Promise<blocks>:
+ * candidateSpread?, candidatePairs?, candidateGroupPairs?) -> Promise<blocks>:
  * the evaluations travel as 3-byte dictionary indices (Form T) instead of 36-byte fp32 rows; same integers, same result. */
 static napi_value ScoreHostTuples(napi_env env, napi_callback_info info)
 {
 	static const char *names[6] = {"tl", "th", "tbookPc", "tbookPd", "codebook", "d2book"};
-	ARGS(11)
+	ARGS(12)
 	call_t *c = argc >= 1 ? new_call(env, argv[0], APO_JOB_SCORE_HOST_TUPLES) : NULL;
 	if (!c) return reject_now(env, "scoreHostTuples: invalid handle");
 	napi_valuetype t;
@@ -534,14 +550,18 @@ static napi_value ScoreHostTuples(napi_env env, napi_callback_info info)
 		corpus = ok ? argv[4] : NULL;
 	}
 	int cands = 0, cext = 0, cspr = 0, cpair = 0;
+	uint32_t g = 0, gp = 0;
 	if (ok && argc > 6) ok = opt_bool_arg(env, argv[6], &cands);
 	if (ok && argc > 7) ok = opt_bool_arg(env, argv[7], &cext);
-	if (ok && argc > 8 && !is_nullish(env, argv[8])) ok = get_u32(env, argv[8], &c->job.G);
+	if (ok && argc > 8 && !is_nullish(env, argv[8])) ok = get_u32(env, argv[8], &g);
 	if (ok && argc > 9) ok = opt_bool_arg(env, argv[9], &cspr);
 	if (ok && argc > 10) ok = opt_bool_arg(env, argv[10], &cpair);
-	c->job.flags = (cands ? APO_SCORE_CANDIDATES : 0) | (cext ? APO_SCORE_CANDIDATE_EXTREMES : 0) | (c->job.G ? APO_SCORE_CANDIDATE_GROUPS : 0) |
-	               (cspr ? APO_SCORE_CANDIDATE_SPREAD : 0) | (cpair ? APO_SCORE_CANDIDATE_PAIRS : 0);
-	if (!ok) arg_error(c, "scoreHostTuples(handle, {tl, th, tbookPc, tbookPd, codebook, d2book: ArrayBuffer, nTuples:uint32}, C:uint32, T:uint53, corpus:ArrayBuffer|null, K:uint32, candidates?:boolean, candidateExtremes?:boolean, candidateGroups?:G, candidateSpread?:boolean, candidatePairs?:boolean)");
+	if (ok && argc > 11 && !is_nullish(env, argv[11])) ok = get_u32(env, argv[11], &gp);
+	if (ok && (g || gp)) ok = one_G(g, gp) != 0;
+	c->job.G = one_G(g, gp);
+	c->job.flags = (cands ? APO_SCORE_CANDIDATES : 0) | (cext ? APO_SCORE_CANDIDATE_EXTREMES : 0) | (g ? APO_SCORE_CANDIDATE_GROUPS : 0) |
+	               (cspr ? APO_SCORE_CANDIDATE_SPREAD : 0) | (cpair ? APO_SCORE_CANDIDATE_PAIRS : 0) | (gp ? APO_SCORE_CANDIDATE_GROUP_PAIRS : 0);
+	if (!ok) arg_error(c, "scoreHostTuples(handle, {tl, th, tbookPc, tbookPd, codebook, d2book: ArrayBuffer, nTuples:uint32}, C:uint32, T:uint53, corpus:ArrayBuffer|null, K:uint32, candidates?:boolean, candidateExtremes?:boolean, candidateGroups?:G, candidateSpread?:boolean, candidatePairs?:boolean, candidateGroupPairs?:G)");
 	for (int i = 1; i < 6; i++)                                      /* the job reads these on a worker thread: keep them alive */
 		if (arr[i]) napi_create_reference(env, arr[i], 1, &c->keep[c->nkeep++]);
 	return submit(env, c, argv[0], arr[0], corpus, "apo_score_host_tuples");

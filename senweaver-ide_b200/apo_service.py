@@ -266,10 +266,18 @@ class APOService:
             out["scoreStdErr"] = None if sp.n < 2 else float(sp.stdErr)
         pr = res.pairs[c] if getattr(res, "pairs", None) is not None else None
         if pr is not None:
-            out["vsReference"] = None if pr.ref == PAIR_NONE else {
-                "reference": int(pr.ref), "pairedRollouts": int(pr.n), "wins": int(pr.wins), "losses": int(pr.losses), "ties": int(pr.ties),
-                "meanRewardDiff": None if pr.n == 0 else float(pr.meanDiff), "diffStdErr": None if pr.n < 2 else float(pr.stdErr)}
+            out["vsReference"] = None if pr.ref == PAIR_NONE else self._vsReference(pr)
+        gp = res.group_pairs[c] if getattr(res, "group_pairs", None) is not None else None
+        if gp is not None:
+            names = groupNames if groupNames is not None else (self._groupNames or [str(g) for g in range(len(gp))])
+            out["vsReferenceByGroup"] = None if gp[0].ref == PAIR_NONE else {names[g]: self._vsReference(x) for g, x in enumerate(gp)}
         return out
+
+    @staticmethod
+    def _vsReference(pr):
+        """the vsReference dict of one apo_candidate_pair (whole record axis or one group)"""
+        return {"reference": int(pr.ref), "pairedRollouts": int(pr.n), "wins": int(pr.wins), "losses": int(pr.losses), "ties": int(pr.ties),
+                "meanRewardDiff": None if pr.n == 0 else float(pr.meanDiff), "diffStdErr": None if pr.n < 2 else float(pr.stdErr)}
 
     @staticmethod
     def parentRefs(cands, carried):
@@ -340,7 +348,7 @@ class APOService:
 
     # ---- beam evaluation: the step the reference delegates to its backend --------------------------------
     def evaluateBeam(self, candidates, dims=None, rollouts=None, reports=False, patterns=False, extremes=False, groups=None,
-                     spread=False, refs=None):
+                     spread=False, refs=None, groupPairs=False):
         """Score a beam of VersionedPromptTemplate candidates on their rollout outcomes and keep the
         top `beamWidth` (score desc, ties -> lower index), then apply the APO:1138-1166 update with the
         strict `>` adoption rule (APO:1159).  dims: float32 [C][T][9] (NaN = absent) or rollouts:
@@ -351,8 +359,11 @@ class APOService:
         rollouts by record group (res.groups [C][G]): labels[t] < len(names) is the group of rollout index t.  spread=True also
         builds every candidate's reward spread (res.spread: exact sums, variance, standard deviation and standard error).
         refs (uint32 [C], a candidate index or PAIR_NONE each) also compares every candidate with its reference on the rollouts
-        both were scored on (res.pairs: wins, losses, ties, the exact paired sums, meanDiff and its standard error).  The
+        both were scored on (res.pairs: wins, losses, ties, the exact paired sums, meanDiff and its standard error).
+        groupPairs=True (which needs groups and refs) also makes that comparison per record group (res.group_pairs [C][G]).  The
         adoption rule stays the strict `>` on the means."""
+        if groupPairs and (groups is None or refs is None):
+            raise ValueError("evaluateBeam: groupPairs needs groups and refs (the comparison is split by the groups' labels)")
         try:
             C = len(candidates)
             K = min(self._config["beamWidth"], C)
@@ -371,6 +382,8 @@ class APOService:
             if refs is not None:
                 self._engine.candidate_refs_upload(refs)
                 extra["pairs"] = True
+            if groupPairs:
+                extra["group_pairs"] = True
             if dims is not None:
                 self._engine.dims_upload(np.ascontiguousarray(dims, np.float32))
                 res = self._engine.score(C, K, source=SRC_DIMS, **extra)
@@ -391,7 +404,7 @@ class APOService:
             return None
 
     def runBeamSearch(self, seedPrompt, proposeCandidates, rolloutDims=None, rounds=None, withReports=False, rolloutRecords=None,
-                      withExtremes=False, rolloutGroups=None, withSpread=False, withParentComparison=False):
+                      withExtremes=False, rolloutGroups=None, withSpread=False, withParentComparison=False, withGroupComparison=False):
         """Client-side round driver (SURVEY 8f rank 3) around the GPU top-K: each round expands every beam
         member into `branchFactor` children through the caller's `proposeCandidates(parent, n) -> [content]`
         hook (the LLM critique/edit step of APO:918-988 lives there), scores parents + children on
@@ -406,7 +419,10 @@ class APOService:
         withSpread=True (which needs withReports=True too) adds the parent's rewardStdDev / scoreStdErr, so that the critique
         can tell a lead from the noise of the rollouts; withParentComparison=True (which needs withReports=True too) adds the
         parent's vsReference: how it fared against its own parent on the rollouts that scored both (wins, losses, ties, the
-        mean reward difference and its paired standard error).  Returns the final beam state."""
+        mean reward difference and its paired standard error); withGroupComparison=True (which needs withReports=True,
+        rolloutGroups and withParentComparison=True) adds the parent's vsReferenceByGroup: that comparison on each group's
+        rollouts, so that the critique sees whether the parent beat its own parent on the held-out ones by more than the paired
+        noise there.  Returns the final beam state."""
         if (rolloutDims is None) == (rolloutRecords is None):
             raise ValueError("runBeamSearch needs exactly one of rolloutDims / rolloutRecords")
         if withExtremes and not withReports:
@@ -419,6 +435,8 @@ class APOService:
             if not withReports:
                 raise ValueError("runBeamSearch: rolloutGroups needs withReports=True (the group scores travel in the candidate reports)")
             rolloutGroups = self._checkGroups(rolloutGroups)
+        if withGroupComparison and not (withReports and rolloutGroups is not None and withParentComparison):
+            raise ValueError("runBeamSearch: withGroupComparison needs withReports=True, rolloutGroups and withParentComparison=True")
         rounds = rounds or self._config["beamRounds"]
         beam = [{"version": "v0", "content": seedPrompt, "score": None, "createdAt": time.time() * 1000.0}]
         counter = 0
@@ -435,10 +453,11 @@ class APOService:
             refs = self.parentRefs(cands, len(beam)) if withParentComparison else None
             if rolloutRecords is not None:
                 res = self.evaluateBeam(cands, rollouts=rolloutRecords(cands), reports=withReports, patterns=withReports,
-                                        extremes=withExtremes, groups=rolloutGroups, spread=withSpread, refs=refs)
+                                        extremes=withExtremes, groups=rolloutGroups, spread=withSpread, refs=refs,
+                                        groupPairs=withGroupComparison)
             else:
                 res = self.evaluateBeam(cands, dims=rolloutDims(cands), reports=withReports, extremes=withExtremes, groups=rolloutGroups,
-                                        spread=withSpread, refs=refs)
+                                        spread=withSpread, refs=refs, groupPairs=withGroupComparison)
             if res is None:
                 break
             if withReports:

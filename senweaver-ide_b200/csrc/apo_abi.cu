@@ -159,14 +159,15 @@ const struct { const char *env; uint32_t bit; } kTuning[] = {
 
 // The per-candidate passes a scoring call can flag (csrc/apo_cand.cu), with the words of their messages.  tbook: the pass
 // reads every source, Form T through the 4-bit table (apo_engine::tbook).
-enum Pass { PASS_CAND, PASS_CCORP, PASS_EXT, PASS_GRP, PASS_SPREAD, PASS_PAIR, NPASS };
+enum Pass { PASS_CAND, PASS_CCORP, PASS_EXT, PASS_GRP, PASS_SPREAD, PASS_PAIR, PASS_GPAIR, NPASS };
 const struct { uint32_t flag; const char *name, *joined, *every; bool tbook; } kPass[NPASS] = {
 	{APO_SCORE_CANDIDATES, "APO_SCORE_CANDIDATES", "the per-candidate breakdown is", "a breakdown", true},
 	{APO_SCORE_CANDIDATE_CORPUS, "APO_SCORE_CANDIDATE_CORPUS", "the per-candidate corpus reports are", "the reports", false},
 	{APO_SCORE_CANDIDATE_EXTREMES, "APO_SCORE_CANDIDATE_EXTREMES", "the per-candidate lists are", "the lists", true},
 	{APO_SCORE_CANDIDATE_GROUPS, "APO_SCORE_CANDIDATE_GROUPS", "the per-candidate group scores are", "the group scores", true},
 	{APO_SCORE_CANDIDATE_SPREAD, "APO_SCORE_CANDIDATE_SPREAD", "the per-candidate spreads are", "the spreads", true},
-	{APO_SCORE_CANDIDATE_PAIRS, "APO_SCORE_CANDIDATE_PAIRS", "the paired comparisons are", "the pairs", true}};
+	{APO_SCORE_CANDIDATE_PAIRS, "APO_SCORE_CANDIDATE_PAIRS", "the paired comparisons are", "the pairs", true},
+	{APO_SCORE_CANDIDATE_GROUP_PAIRS, "APO_SCORE_CANDIDATE_GROUP_PAIRS", "the per-group paired comparisons are", "the group pairs", true}};
 
 // one pass's state through a call or session
 struct PassState {
@@ -260,6 +261,9 @@ struct apo_engine {
 	uint64_t pair_gen = 0, pair_arm_gen = 0;  // counts uploads: a session's pairs belong to the refs it armed with
 	DevBuf<unsigned long long> pair_acc;     // [C][PR_WORDS] words of the call or session
 	DevBuf<struct apo_candidate_pair> pair_rep;   // pairs of the last flagged call
+	DevBuf<unsigned long long> gpair_acc;    // per-group pairs: [C][G][PR_WORDS] words of the call or session
+	DevBuf<struct apo_candidate_pair> gpair_rep;  // [C][G] pairs of the last flagged call
+	uint32_t gpair_rep_G = 0, gpair_arm_G = 0; uint64_t gpair_arm_grp_gen = 0, gpair_arm_pair_gen = 0;
 };
 
 namespace {
@@ -813,22 +817,22 @@ int refuse_no_records(apo_engine *e) {
 }
 
 // the labels cover the record positions below end (0: not known here, a session's finish)
-int labels_check(apo_engine *e, uint64_t end) {
-	if (e->grp_T == 0) return fail(e, APO_E_STATE, "APO_SCORE_CANDIDATE_GROUPS: no record groups uploaded (apo_record_groups_upload)");
+int labels_check(apo_engine *e, uint64_t end, int p = PASS_GRP) {
+	if (e->grp_T == 0) return fail(e, APO_E_STATE, "%s: no record groups uploaded (apo_record_groups_upload)", kPass[p].name);
 	if (end > e->grp_T)
-		return fail(e, APO_E_ARG, "APO_SCORE_CANDIDATE_GROUPS: record position %llu is past the %llu labels uploaded", (unsigned long long)end - 1,
+		return fail(e, APO_E_ARG, "%s: record position %llu is past the %llu labels uploaded", kPass[p].name, (unsigned long long)end - 1,
 		            (unsigned long long)e->grp_T);
 	return APO_OK;
 }
 
 // the refs are held for the C candidates of the call, and those of candidates [c0, c0 + n) (an accumulate's chunk) lie inside them
-int refs_check(apo_engine *e, uint32_t C, uint32_t c0, uint32_t n) {
+int refs_check(apo_engine *e, uint32_t C, uint32_t c0, uint32_t n, int p = PASS_PAIR) {
 	const std::vector<uint32_t> &r = e->pair_refs_host;
-	if (r.empty()) return fail(e, APO_E_STATE, "APO_SCORE_CANDIDATE_PAIRS: no references uploaded (apo_candidate_refs_upload)");
-	if (r.size() != C) return fail(e, APO_E_ARG, "APO_SCORE_CANDIDATE_PAIRS: the references are for C=%zu candidates, the call scores C=%u", r.size(), C);
+	if (r.empty()) return fail(e, APO_E_STATE, "%s: no references uploaded (apo_candidate_refs_upload)", kPass[p].name);
+	if (r.size() != C) return fail(e, APO_E_ARG, "%s: the references are for C=%zu candidates, the call scores C=%u", kPass[p].name, r.size(), C);
 	for (uint32_t c = c0; c < c0 + n; c++)
 		if (r[c] != APO_PAIR_NONE && (r[c] < c0 || r[c] >= c0 + n))
-			return fail(e, APO_E_ARG, "APO_SCORE_CANDIDATE_PAIRS: candidate %u names reference %u outside the candidates [%u,%u) this call loads", c, r[c],
+			return fail(e, APO_E_ARG, "%s: candidate %u names reference %u outside the candidates [%u,%u) this call loads", kPass[p].name, c, r[c],
 			            c0, c0 + n);
 	return APO_OK;
 }
@@ -847,6 +851,10 @@ int passes_check(apo_engine *e, const apo_score_opts *o, bool records, uint64_t 
 			return fail(e, APO_E_STATE, "%s is single-rank only: %s not joined across the %d ranks of this handle", kPass[p].name, kPass[p].joined, e->nranks);
 		if (p == PASS_GRP && end != kStreamed) { const int rc = labels_check(e, end); if (rc) return rc; }
 		if (p == PASS_PAIR) { const int rc = refs_check(e, C, c0, n); if (rc) return rc; }
+		if (p == PASS_GPAIR) {                                          // the refusals of both passes it joins
+			int rc = end != kStreamed ? labels_check(e, end, p) : APO_OK;
+			if (rc || (rc = refs_check(e, C, c0, n, p))) return rc;
+		}
 	}
 	return APO_OK;
 }
@@ -862,6 +870,7 @@ int pass_reserve(apo_engine *e, int p, uint32_t C) {
 	case PASS_GRP: CK(reserve(e, e->grp_acc, (uint64_t)(C ? C : 1) * e->grp_G * apo::GR_WORDS)); break;
 	case PASS_SPREAD: CK(reserve(e, e->spread_acc, (uint64_t)(C ? C : 1) * apo::SP_WORDS)); break;
 	case PASS_PAIR: CK(reserve(e, e->pair_acc, (uint64_t)(C ? C : 1) * apo::PR_WORDS)); break;
+	case PASS_GPAIR: CK(reserve(e, e->gpair_acc, (uint64_t)(C ? C : 1) * e->grp_G * apo::PR_WORDS)); break;
 	}
 	if (kPass[p].tbook) CK(reserve(e, e->tbook, 8 * 16));
 	return APO_OK;
@@ -883,6 +892,10 @@ int pass_arm(apo_engine *e, int p, uint32_t C) {
 		CK(cudaMemsetAsync(e->pair_acc.p, 0, (uint64_t)C * apo::PR_WORDS * 8, e->stream));
 		e->pair_arm_gen = e->pair_gen;
 		break;
+	case PASS_GPAIR:                                                // the words then belong to the labels and refs held now
+		CK(cudaMemsetAsync(e->gpair_acc.p, 0, (uint64_t)C * e->grp_G * apo::PR_WORDS * 8, e->stream));
+		e->gpair_arm_G = e->grp_G; e->gpair_arm_grp_gen = e->grp_gen; e->gpair_arm_pair_gen = e->pair_gen;
+		break;
 	}
 	e->pass[p].armed = true;
 	return APO_OK;
@@ -898,12 +911,13 @@ int upload_tbook(apo_engine *e, const uint32_t *codebook) {
 }
 
 // The flagged passes over ev into candidates [cand_offset, ...), behind its scoring launch.  A pass that an accumulate of the
-// session did not flag, or whose group (pair) words belong to labels (refs) uploaded since, is left out: apo_score_finish
-// refuses it.
+// session did not flag, or whose group (pair, group pair) words belong to labels (refs, either) uploaded since, is left out:
+// apo_score_finish refuses it.
 int launch_passes(apo_engine *e, const apo_score_opts *o, const Evals &ev, uint32_t cand_offset) {
 	bool run[NPASS], any = false;
 	for (int p = 0; p < NPASS; p++) {
-		run[p] = wants(o, p) && e->pass[p].every && (p != PASS_GRP || e->grp_arm_gen == e->grp_gen) && (p != PASS_PAIR || e->pair_arm_gen == e->pair_gen);
+		run[p] = wants(o, p) && e->pass[p].every && (p != PASS_GRP || e->grp_arm_gen == e->grp_gen) && (p != PASS_PAIR || e->pair_arm_gen == e->pair_gen) &&
+		         (p != PASS_GPAIR || (e->gpair_arm_grp_gen == e->grp_gen && e->gpair_arm_pair_gen == e->pair_gen));
 		any |= run[p];
 	}
 	if (!any || !ev.count) return APO_OK;
@@ -948,6 +962,13 @@ int launch_passes(apo_engine *e, const apo_score_opts *o, const Evals &ev, uint3
 	if (run[PASS_PAIR]) {                                           // refs of this launch's candidates, mapped to its rows by the kernel
 		const apo::CandPairParams X{S, e->W, e->pair_refs.p + cand_offset, cand_offset, e->pair_acc.p + (uint64_t)apo::PR_WORDS * cand_offset};
 		CK(apo::run_cand_pairs(X, ev.form, recip, e->sm_count, e->stream));
+		e->timing.launches++;
+	}
+	if (run[PASS_GPAIR]) {
+		const uint32_t G = e->gpair_arm_G;
+		const apo::CandGroupPairParams X{S, e->W, e->grp_labels.p, G, e->pair_refs.p + cand_offset, cand_offset,
+		                                 e->gpair_acc.p + (uint64_t)cand_offset * G * apo::PR_WORDS};
+		CK(apo::run_cand_group_pairs(X, ev.form, recip, e->sm_count, e->stream));
 		e->timing.launches++;
 	}
 	return APO_OK;
@@ -1007,6 +1028,11 @@ int finish_passes(apo_engine *e, const apo_score_opts *o, uint32_t C) {
 		CK(apo::run_cand_pair_report(e->pair_acc.p, e->pair_refs.p, C, e->pair_rep.p, e->stream));
 		e->timing.launches++;
 	}
+	if (wants(o, PASS_GPAIR)) {                                     // words + refs -> apo_candidate_pair[C][G]
+		CK(reserve(e, e->gpair_rep, (uint64_t)(C ? C : 1) * e->gpair_arm_G));
+		CK(apo::run_cand_group_pairs_report(e->gpair_acc.p, e->pair_refs.p, C, e->gpair_arm_G, e->gpair_rep.p, e->stream));
+		e->timing.launches++;
+	}
 	uint32_t dom = 0;                                               // k_cand_breakdown's domain word (pageable: the copy waits for the stream)
 	if (wants(o, PASS_CAND)) CK(cudaMemcpyAsync(&dom, e->cand_acc.p + cand_words(C) - 1, 4, cudaMemcpyDeviceToHost, e->stream));
 	CK(cudaStreamSynchronize(e->stream));
@@ -1016,15 +1042,18 @@ int finish_passes(apo_engine *e, const apo_score_opts *o, uint32_t C) {
 	for (int p = 0; p < NPASS; p++)
 		if (wants(o, p)) { e->pass[p].C = C; e->pass[p].ready = true; }
 	if (wants(o, PASS_GRP)) e->grp_rep_G = e->grp_arm_G;
+	if (wants(o, PASS_GPAIR)) e->gpair_rep_G = e->gpair_arm_G;
 	return APO_OK;
 }
 
-// The refusals every report getter makes, in order: the last scoring call set the pass's flag (the groups: and split by G),
+// The refusals every report getter makes, in order: the last scoring call set the pass's flag (the groups and group pairs:
+// and split by G),
 // [c0, c0 + n) lies inside its candidates, and a range that is not empty has an out; then the device is current.
 int report_check(apo_engine *e, int p, uint32_t c0, uint32_t n, const void *out, uint32_t G = 0) {
 	if (!e) return APO_E_ARG;
 	if (!e->pass[p].ready) return fail(e, APO_E_STATE, "the last scoring call did not set %s", kPass[p].name);
 	if (p == PASS_GRP && G != e->grp_rep_G) return fail(e, APO_E_ARG, "G=%u is not the G=%u the last scoring call split by", G, e->grp_rep_G);
+	if (p == PASS_GPAIR && G != e->gpair_rep_G) return fail(e, APO_E_ARG, "G=%u is not the G=%u the last scoring call split by", G, e->gpair_rep_G);
 	const uint32_t C = e->pass[p].C;
 	if ((uint64_t)c0 + n > C) return fail(e, APO_E_ARG, "candidates [%u,%llu) exceed C=%u", c0, (unsigned long long)c0 + n, C);
 	if (n == 0) return APO_OK;
@@ -1760,6 +1789,7 @@ extern "C" void apo_destroy(apo_engine *e) {
 	e->grp_labels.release(); e->grp_acc.release(); e->grp_rep.release();
 	e->spread_acc.release(); e->spread_rep.release();
 	e->pair_refs.release(); e->pair_acc.release(); e->pair_rep.release();
+	e->gpair_acc.release(); e->gpair_rep.release();
 	e->tup.release(); e->tups.release(); e->tvals.release();
 	e->win[0].release(); e->win[1].release(); e->batch_in.release(); e->batch_out.release(); e->batch_mask.release();
 	if (e->h_result) cudaFreeHost(e->h_result);
@@ -2202,7 +2232,7 @@ extern "C" int apo_score_finish(apo_engine *e, const apo_score_opts *o, double *
 	if (!e->scoring) return fail(e, APO_E_STATE, "apo_score_begin has not been called");
 	int rc = score_check(e, o, e->score_C, kSession, true);      // the accumulate calls refused every other source
 	if (rc) return rc;
-	for (const int p : {PASS_GRP, PASS_CAND, PASS_CCORP, PASS_EXT, PASS_SPREAD, PASS_PAIR}) {
+	for (const int p : {PASS_GRP, PASS_CAND, PASS_CCORP, PASS_EXT, PASS_SPREAD, PASS_PAIR, PASS_GPAIR}) {
 		if (!wants(o, p)) continue;
 		if (!e->pass[p].every)
 			return fail(e, APO_E_STATE, "%s: every apo_score_accumulate of the session must set the flag for %s", kPass[p].name, kPass[p].every);
@@ -2210,6 +2240,8 @@ extern "C" int apo_score_finish(apo_engine *e, const apo_score_opts *o, double *
 			return fail(e, APO_E_STATE, "APO_SCORE_CANDIDATE_GROUPS: the record groups were uploaded again after the session began to accumulate them");
 		if (p == PASS_PAIR && e->pass[p].armed && e->pair_arm_gen != e->pair_gen)
 			return fail(e, APO_E_STATE, "APO_SCORE_CANDIDATE_PAIRS: the references were uploaded again after the session began to accumulate them");
+		if (p == PASS_GPAIR && e->pass[p].armed && (e->gpair_arm_grp_gen != e->grp_gen || e->gpair_arm_pair_gen != e->pair_gen))
+			return fail(e, APO_E_STATE, "APO_SCORE_CANDIDATE_GROUP_PAIRS: the record groups or the references were uploaded again after the session began to accumulate them");
 	}
 	if ((rc = digest_prepare(e, o)) || (rc = score_arm(e, o, e->score_C, false))) return rc;   // nothing accumulated yet: an empty breakdown
 	return finish_score(e, o, e->score_C, scores, counts, topk, report);
@@ -2322,7 +2354,8 @@ int stream_host(apo_engine *e, const apo_score_opts *o, const HostTensor &h, dou
 	}
 	Evals ev;
 	ev.form = h.form; ev.C = C; ev.variant = (int)o->variant;
-	if ((rc = score_check(e, o, C, kStreamed, ev.records())) || (wants(o, PASS_GRP) && (rc = labels_check(e, T))) || (rc = digest_prepare(e, o))) return rc;
+	if ((rc = score_check(e, o, C, kStreamed, ev.records())) || (wants(o, PASS_GRP) && (rc = labels_check(e, T))) ||
+	    (wants(o, PASS_GPAIR) && (rc = labels_check(e, T, PASS_GPAIR))) || (rc = digest_prepare(e, o))) return rc;
 	if (h.form == apo::CAND_Q) {                                   // Form Q / P: K1q's tables of this call's codebook
 		if ((rc = load_qtables(e, e->qt_stream, h.codebook))) return rc;
 		ev.qt = &e->qt_stream;
@@ -2357,7 +2390,8 @@ int stream_host(apo_engine *e, const apo_score_opts *o, const HostTensor &h, dou
 	}
 	if ((rc = score_arm(e, o, C, true, (uint64_t)C * T * wire))) return rc;
 	if (h.form == apo::CAND_T) {                                   // the dictionary and its values, once for the whole call
-		if ((wants(o, PASS_CAND) || wants(o, PASS_EXT) || wants(o, PASS_GRP) || wants(o, PASS_SPREAD) || wants(o, PASS_PAIR)) && (rc = upload_tbook(e, h.codebook)))
+		if ((wants(o, PASS_CAND) || wants(o, PASS_EXT) || wants(o, PASS_GRP) || wants(o, PASS_SPREAD) || wants(o, PASS_PAIR) || wants(o, PASS_GPAIR)) &&
+		    (rc = upload_tbook(e, h.codebook)))
 			return rc;
 		if ((rc = dict_upload(e, e->tups, h.tb_pc, h.tb_pd, h.n_tuples, h.codebook, h.d2book))) return rc;
 		ev.dict = &e->tups; ev.t_once = true;
@@ -2767,6 +2801,13 @@ extern "C" int apo_candidate_refs_upload(apo_engine *e, const uint32_t *refs, ui
 extern "C" int apo_candidate_pairs(apo_engine *e, uint32_t c0, uint32_t n, struct apo_candidate_pair *out) {
 	if (const int rc = report_check(e, PASS_PAIR, c0, n, out); rc || n == 0) return rc;
 	CK(cudaMemcpyAsync(out, e->pair_rep.p + c0, (uint64_t)n * sizeof(struct apo_candidate_pair), cudaMemcpyDeviceToHost, e->stream));
+	CK(cudaStreamSynchronize(e->stream));
+	return APO_OK;
+}
+
+extern "C" int apo_candidate_group_pairs(apo_engine *e, uint32_t c0, uint32_t n, uint32_t G, struct apo_candidate_pair *out) {
+	if (const int rc = report_check(e, PASS_GPAIR, c0, n, out, G); rc || n == 0) return rc;
+	CK(cudaMemcpyAsync(out, e->gpair_rep.p + (uint64_t)c0 * G, (uint64_t)n * G * sizeof(struct apo_candidate_pair), cudaMemcpyDeviceToHost, e->stream));
 	CK(cudaStreamSynchronize(e->stream));
 	return APO_OK;
 }

@@ -17,8 +17,10 @@
 //
 // For record sources a second feature (APO_SCORE_CANDIDATE_CORPUS, k_cand_corpus below) goes further: the whole corpus
 // report of every candidate's records — patterns, per-mode tallies and tool totals included — by the corpus scan's own code.
-// The extremes, the group scores, the reward spread and the paired comparison follow.  Every pass is one walk (cand_walk) over the same warp tiles with its own
-// per-evaluation step and flush, and one launcher sizes every walk's grid (walk_grid).
+// The extremes, the group scores, the reward spread, the paired comparison and its split by record group follow.  Every pass
+// is one walk (cand_walk) over the same warp tiles with its own per-evaluation step and flush, and one launcher sizes every
+// walk's grid (walk_grid).
+#include <atomic>
 #include <cstdlib>
 #include "apo_device.cuh"
 #include "apo_format.h"
@@ -292,18 +294,18 @@ __device__ __forceinline__ void cand_walk(const CandEvals &P, uint32_t tiles_per
 // APO_K1_GRID caps the grids of the per-candidate passes as it caps the scoring kernels' (tuning and tests only, read once)
 static uint64_t cand_env_grid() { static const int g = [] { const char *s = getenv("APO_K1_GRID"); return s ? atoi(s) : 0; }(); return g > 0 ? (uint64_t)g : 0; }
 
-// The tiles of a launch over P and the grid of a walk kernel for them: as many CTAs as the SMs hold at once, no more than the
-// tiles need, at most APO_K1_GRID.  grid = 0: nothing to walk.
+// The tiles of a launch over P and the grid of a walk kernel for them: as many CTAs as the SMs hold at once (with smem bytes
+// of dynamic shared memory each), no more than the tiles need, at most APO_K1_GRID.  grid = 0: nothing to walk.
 struct Walk { uint32_t tiles_per_cand; uint64_t total_tiles, grid; };
 
 template <class K>
-static cudaError_t walk_grid(K *kernel, const CandEvals &P, int sm_count, Walk &w) {
+static cudaError_t walk_grid(K *kernel, const CandEvals &P, int sm_count, Walk &w, size_t smem = 0) {
 	w.tiles_per_cand = (uint32_t)((P.T + CB_TILE - 1) / CB_TILE);
 	w.total_tiles = (uint64_t)w.tiles_per_cand * P.C;
 	w.grid = 0;
 	if (w.total_tiles == 0) return cudaSuccess;
 	int per_sm = 0;
-	const cudaError_t err = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, CB_THREADS, 0);
+	const cudaError_t err = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, CB_THREADS, smem);
 	if (err != cudaSuccess) return err;
 	w.grid = (uint64_t)sm_count * (uint64_t)(per_sm > 0 ? per_sm : 1);
 	const uint64_t need = (w.total_tiles + CB_WARPS - 1) / CB_WARPS;
@@ -314,11 +316,11 @@ static cudaError_t walk_grid(K *kernel, const CandEvals &P, int sm_count, Walk &
 
 // a pass that is its walk kernel alone
 template <class X>
-static cudaError_t launch_walk(void (*kernel)(X, uint32_t, uint64_t), const X &x, int sm_count, cudaStream_t st) {
+static cudaError_t launch_walk(void (*kernel)(X, uint32_t, uint64_t), const X &x, int sm_count, cudaStream_t st, size_t smem = 0) {
 	Walk w;
-	const cudaError_t err = walk_grid(kernel, x.src, sm_count, w);
+	const cudaError_t err = walk_grid(kernel, x.src, sm_count, w, smem);
 	if (err != cudaSuccess || w.grid == 0) return err;
-	kernel<<<(unsigned)w.grid, CB_THREADS, 0, st>>>(x, w.tiles_per_cand, w.total_tiles);
+	kernel<<<(unsigned)w.grid, CB_THREADS, smem, st>>>(x, w.tiles_per_cand, w.total_tiles);
 	return cudaGetLastError();
 }
 
@@ -991,14 +993,10 @@ k_cand_pairs(const CandPairParams X, uint32_t tiles_per_cand, uint64_t total_til
 	cand_walk<L, CB_RUN_TILES>(P, tiles_per_cand, total_tiles, each, flush, NoSide{}, RefRow{X.refs, X.base});
 }
 
-// one thread per candidate
-__global__ void __launch_bounds__(256)
-k_cand_pair_report(const unsigned long long *words, const uint32_t *refs, uint32_t C, struct apo_candidate_pair *out) {
-	const uint32_t c = blockIdx.x * blockDim.x + threadIdx.x;
-	if (c >= C) return;
-	const unsigned long long *w = words + (uint64_t)c * PR_WORDS;
+// one comparison's words (PR_WORDS) and reference -> apo_candidate_pair, for the whole record axis or one group of it
+__device__ __forceinline__ void pair_report(const unsigned long long *w, uint32_t ref, struct apo_candidate_pair *out) {
 	struct apo_candidate_pair R;
-	R.ref = refs[c];
+	R.ref = ref;
 	R.pad = 0u;
 	R.wins = w[PR_CNT]; R.losses = w[PR_CNT + 1]; R.ties = w[PR_CNT + 2]; R.candOnly = w[PR_CNT + 3]; R.refOnly = w[PR_CNT + 4];
 	const uint64_t n = R.wins + R.losses + R.ties;
@@ -1011,13 +1009,140 @@ k_cand_pair_report(const unsigned long long *words, const uint32_t *refs, uint32
 	const long long l[4] = {(long long)(s1 & 0xFFFFFFFF), (long long)((s1 >> 32) & 0xFFFFFFFF), (long long)(s1 >> 64), 0ll};
 	R.meanDiff = report_avg_reward(limbs_to_double(l), n);               // the rounding sequence of scores[c]
 	spread_moments(n, s1, s2, R.variance, R.stdDev, R.stdErr);
-	out[c] = R;
+	*out = R;
+}
+
+// one thread per candidate
+__global__ void __launch_bounds__(256)
+k_cand_pair_report(const unsigned long long *words, const uint32_t *refs, uint32_t C, struct apo_candidate_pair *out) {
+	const uint32_t c = blockIdx.x * blockDim.x + threadIdx.x;
+	if (c >= C) return;
+	pair_report(words + (uint64_t)c * PR_WORDS, refs[c], out + c);
 }
 
 cudaError_t run_cand_pair_report(const unsigned long long *words, const uint32_t *refs, uint32_t C, struct apo_candidate_pair *out,
                                  cudaStream_t st) {
 	if (C == 0) return cudaSuccess;
 	k_cand_pair_report<<<(C + 255) / 256, 256, 0, st>>>(words, refs, C, out);
+	return cudaGetLastError();
+}
+
+// ================================================================ paired comparison per record group (APO_SCORE_CANDIDATE_GROUP_PAIRS)
+//   k_cand_group_pairs<Loader, TABLE, RECIP>  the paired comparison's pass split as the group scores split: the walk fetches
+//                                             the reference's row and the position's label with the candidate's own row
+//   k_cand_group_pairs_report                 words -> apo_candidate_pair[C][G] by the pair report's code (pair_report)
+// A group of 32 positions is aggregated per label before it touches memory, as in k_cand_groups: the lanes that share a
+// label (all 32 on the fast path, __match_any_sync otherwise; a lane alone in its label skips the reductions) reduce d as four
+// 16-bit pieces of its two's complement, d^2 (< 2^124) as eight 16-bit pieces, every piece summing to < 2^21, and the five
+// tallies in 6-bit fields of one word.  The lowest lane of the label adds them into the warp's accumulators of that label: D1
+// as limbs of weight 2^0 and 2^32, each negative d carrying -2^64 (the negative d are the losses, so the losses count them),
+// D2 as four limbs of weight 2^0, 2^32, 2^64 and 2^96.  Every limb grows by < 2^38 per group of 32, so by < 2^59 over a run of
+// CB_RUN_TILES tiles (2^21 groups) whatever the labels.  A flush (candidate change, run limit, end of the range) forms every
+// label's run D1 (signed) and D2 as 192-bit integers and adds them into the (c, g) words with the pairs' carried atomics: exact
+// modulo 2^192 for any number of flushes.  No word takes 32-bit limbs, so limb_guard has nothing of this pass to rewrite.
+// The accumulators are dynamic shared memory sized by G (gp_bytes): at G = 64 they and the staged tables pass the 48 KB a
+// kernel may hold without opting in.
+constexpr int GP_LIMBS = 6;                          // u64 per label and warp: D1 at 2^0, 2^32; D2 at 2^0, 2^32, 2^64, 2^96
+constexpr int GP_TALLIES = 5;                        // u32 per label and warp: wins, losses, ties, candOnly, refOnly (PR_CNT order)
+constexpr size_t gp_bytes(uint32_t G) { return (size_t)CB_WARPS * G * (GP_LIMBS * 8 + GP_TALLIES * 4); }
+
+template <class L, int TABLE, bool RECIP>
+__global__ void __launch_bounds__(CB_THREADS, L::MIN_CTAS)
+k_cand_group_pairs(const CandGroupPairParams X, uint32_t tiles_per_cand, uint64_t total_tiles) {
+	const CandEvals &P = X.src;
+	__shared__ CandSmem S;
+	__shared__ double s_rc[512];                                        // reciprocal of the total weight (div_lut)
+	extern __shared__ unsigned long long gp_acc[];                      // [GP_LIMBS][CB_WARPS][G] u64, then [GP_TALLIES][CB_WARPS][G] u32
+	const int lane = threadIdx.x & 31, wp = threadIdx.x >> 5;
+	const uint32_t G = X.G, WG = CB_WARPS * G;
+	unsigned long long *limb = gp_acc + wp * G;                         // limb k of label l: limb[k * WG + l]
+	uint32_t *tally = reinterpret_cast<uint32_t *>(gp_acc + GP_LIMBS * WG) + wp * G;
+	for (uint32_t g = lane; g < G; g += 32) {
+		for (int k = 0; k < GP_LIMBS; k++) limb[k * WG + g] = 0ull;
+		for (int k = 0; k < GP_TALLIES; k++) tally[k * WG + g] = 0u;
+	}
+	stage_tables<TABLE, true>(P, S, s_rc);
+	const uint8_t *labels = X.labels + P.idx_base;
+
+	auto flush = [&](uint32_t c) {
+		__syncwarp();
+		for (uint32_t g = lane; g < G; g += 32) {
+			unsigned long long *w = X.words + ((uint64_t)c * G + g) * PR_WORDS;
+			const __int128 d1 = (__int128)limb[g] + ((__int128)limb[WG + g] << 32) - ((__int128)tally[WG + g] << 64);   // |d1| < 2^92
+			const U192 s1{(unsigned long long)d1, (unsigned long long)(d1 >> 64), (unsigned long long)(d1 >> 127)};
+			const unsigned __int128 lo = (unsigned __int128)limb[2 * WG + g] + ((unsigned __int128)limb[3 * WG + g] << 32);
+			const unsigned __int128 hi = (unsigned __int128)limb[4 * WG + g] + ((unsigned __int128)limb[5 * WG + g] << 32) + (lo >> 64);
+			const U192 s2{(unsigned long long)lo, (unsigned long long)hi, (unsigned long long)(hi >> 64)};
+			if (s1.w0 | s1.w1 | s1.w2) atomic_add_u192(w + PR_D1, s1);
+			if (s2.w0 | s2.w1 | s2.w2) atomic_add_u192(w + PR_D2, s2);
+			for (int k = 0; k < GP_TALLIES; k++) {
+				if (const uint32_t v = tally[k * WG + g]) atomicAdd(w + PR_CNT + k, (unsigned long long)v);
+				tally[k * WG + g] = 0u;
+			}
+			for (int k = 0; k < GP_LIMBS; k++) limb[k * WG + g] = 0ull;
+		}
+		__syncwarp();
+	};
+	// l: the label, fetched with the evaluations (past the row end: label 0, nothing added)
+	auto each = [&](uint32_t, uint64_t, bool in, const typename L::Raw &R, const typename L::Raw &Q, uint32_t l) {
+		unsigned long long u = 0ull, q0 = 0ull, q1 = 0ull;              // d as two's complement, d^2 as two words
+		uint32_t pk = 0u;                                                // the tallies, 6 bits each in PR_CNT order
+		if (in) {
+			CandEval E;
+			L::decode(P, S, R, E);
+			const bool vc = E.valid != 0u;
+			const long long xc = vc ? to_fx(cand_final_reward<RECIP>(E, X.W, S.tw, s_rc)) : 0ll;
+			L::decode(P, S, Q, E);
+			const bool vr = E.valid != 0u;
+			const long long xr = vr ? to_fx(cand_final_reward<RECIP>(E, X.W, S.tw, s_rc)) : 0ll;
+			if (vc && vr) {
+				const long long d = xc - xr;
+				pk = 1u << (d > 0 ? 0 : d < 0 ? 6 : 12);
+				u = (unsigned long long)d;
+				const unsigned long long a = d < 0 ? 0ull - u : u;
+				asm("mul.lo.u64 %0, %2, %2;\n\tmul.hi.u64 %1, %2, %2;" : "=l"(q0), "=l"(q1) : "l"(a));
+			} else {
+				pk = ((vc ? 1u : 0u) << 18) | ((vr ? 1u : 0u) << 24);
+			}
+		}
+		const uint32_t peers = __all_sync(FULL, l == __shfl_sync(FULL, l, 0)) ? FULL : __match_any_sync(FULL, l);
+		uint32_t p[13];                                                  // d: p[0..3], d^2: p[4..11], tallies: p[12]
+#pragma unroll
+		for (int k = 0; k < 4; k++) {
+			p[k] = (uint32_t)(u >> (16 * k)) & 0xFFFFu;
+			p[4 + k] = (uint32_t)(q0 >> (16 * k)) & 0xFFFFu;
+			p[8 + k] = (uint32_t)(q1 >> (16 * k)) & 0xFFFFu;
+		}
+		p[12] = pk;
+		if (peers != (1u << lane)) {                                    // a label of its own needs no reduction
+#pragma unroll
+			for (int k = 0; k < 13; k++) p[k] = __reduce_add_sync(peers, p[k]);
+		}
+		if (lane == __ffs((int)peers) - 1) {                          // the lowest lane of the label: one writer per label
+#pragma unroll
+			for (int k = 0; k < GP_LIMBS; k++) limb[k * WG + l] += (unsigned long long)p[2 * k] + ((unsigned long long)p[2 * k + 1] << 16);
+#pragma unroll
+			for (int k = 0; k < GP_TALLIES; k++) tally[k * WG + l] += (p[12] >> (6 * k)) & 63u;
+		}
+		__syncwarp();                                                   // the next group's writer of a label may be another lane
+	};
+	cand_walk<L, CB_RUN_TILES>(P, tiles_per_cand, total_tiles, each, flush, [&](uint64_t t) { return (uint32_t)__ldg(labels + t); },
+	                           RefRow{X.refs, X.base});
+}
+
+// one thread per (c, g)
+__global__ void __launch_bounds__(256)
+k_cand_group_pairs_report(const unsigned long long *words, const uint32_t *refs, uint32_t G, uint64_t n, struct apo_candidate_pair *out) {
+	const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+	if (i >= n) return;
+	pair_report(words + i * PR_WORDS, refs[i / G], out + i);
+}
+
+cudaError_t run_cand_group_pairs_report(const unsigned long long *words, const uint32_t *refs, uint32_t C, uint32_t G,
+                                        struct apo_candidate_pair *out, cudaStream_t st) {
+	const uint64_t n = (uint64_t)C * G;
+	if (n == 0) return cudaSuccess;
+	k_cand_group_pairs_report<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(words, refs, G, n, out);
 	return cudaGetLastError();
 }
 
@@ -1069,6 +1194,21 @@ template <class L, int TABLE, bool RECIP>
 static cudaError_t launch_pass(const CandPairParams &X, int sm_count, cudaStream_t st) {
 	return launch_walk(k_cand_pairs<L, TABLE, RECIP>, X, sm_count, st);
 }
+template <class L, int TABLE, bool RECIP>
+static cudaError_t launch_pass(const CandGroupPairParams &X, int sm_count, cudaStream_t st) {
+	// the opt-in past 48 KB belongs to the current device's context: set once per device (ordinals past 63 set it every launch)
+	static std::atomic<uint64_t> opted{0ull};
+	int dev = 0;
+	cudaError_t err = cudaGetDevice(&dev);
+	if (err != cudaSuccess) return err;
+	const uint64_t bit = dev >= 0 && dev < 64 ? 1ull << dev : 0ull;
+	if (!bit || !(opted.load() & bit)) {
+		err = cudaFuncSetAttribute(k_cand_group_pairs<L, TABLE, RECIP>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)gp_bytes(APO_GROUPS_MAX));
+		if (err != cudaSuccess) return err;
+		opted.fetch_or(bit);
+	}
+	return launch_walk(k_cand_group_pairs<L, TABLE, RECIP>, X, sm_count, st, gp_bytes(X.G));
+}
 
 // the loader of each source and the table it stages; RECIP: the division of the passes that divide (div_lut)
 template <bool RECIP, class X>
@@ -1097,6 +1237,9 @@ cudaError_t run_cand_spread(const CandSpreadParams &X, int source, bool recip, i
 	return recip ? by_source<true>(X, source, sm_count, st) : by_source<false>(X, source, sm_count, st);
 }
 cudaError_t run_cand_pairs(const CandPairParams &X, int source, bool recip, int sm_count, cudaStream_t st) {
+	return recip ? by_source<true>(X, source, sm_count, st) : by_source<false>(X, source, sm_count, st);
+}
+cudaError_t run_cand_group_pairs(const CandGroupPairParams &X, int source, bool recip, int sm_count, cudaStream_t st) {
 	return recip ? by_source<true>(X, source, sm_count, st) : by_source<false>(X, source, sm_count, st);
 }
 

@@ -441,6 +441,22 @@ cudaError_t run_cand_pairs(const CandPairParams &P, int source, bool recip, int 
 cudaError_t run_cand_pair_report(const unsigned long long *words, const uint32_t *refs, uint32_t C, struct apo_candidate_pair *out,
                                  cudaStream_t st);
 
+// ---- per-candidate paired comparison per record group (csrc/apo_cand.cu): the paired comparison restricted to the record
+// positions of each label.  Own buffer [C][G][PR_WORDS], each (c, g) in the pair words' layout; no limb carry, as for them.
+struct CandGroupPairParams {
+	CandEvals src;
+	Weights W;
+	const uint8_t *labels;          // [labels T] group of every record position (src.idx_base + t)
+	uint32_t G;                     // 1..APO_GROUPS_MAX
+	const uint32_t *refs;           // as CandPairParams
+	uint32_t base;
+	unsigned long long *words;      // [C][G][PR_WORDS] of candidate 0 of this launch
+};
+cudaError_t run_cand_group_pairs(const CandGroupPairParams &P, int source, bool recip, int sm_count, cudaStream_t st);
+// words / refs: the whole buffers of C candidates
+cudaError_t run_cand_group_pairs_report(const unsigned long long *words, const uint32_t *refs, uint32_t C, uint32_t G,
+                                        struct apo_candidate_pair *out, cudaStream_t st);
+
 // ---- limb carry (csrc/apo_cand.cu): the (l0, l1, l2) triples that accumulate across the launches of a session or of a
 // host-streaming call (the candidate partials, the breakdown's dimension words, the group words, the per-candidate corpus
 // blocks' reward and dimension words) stay exact while l0 and l1 < 2^63.  limb_flush_bound: the most flushes one launch over

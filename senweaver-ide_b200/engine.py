@@ -27,6 +27,7 @@ SCORE_CANDIDATE_GROUPS = 0x40
 GROUPS_MAX = 64
 SCORE_CANDIDATE_SPREAD = 0x80
 SCORE_CANDIDATE_PAIRS = 0x100
+SCORE_CANDIDATE_GROUP_PAIRS = 0x200
 PAIR_NONE = 0xFFFFFFFF
 TUNE_NO_FUSE, TUNE_FORCE_FUSE, TUNE_NO_STAGING, TUNE_NCCL_JOIN, TUNE_NO_TWIN = 0x1, 0x2, 0x4, 0x8, 0x10
 TUNE_NO_TWIN_T, TUNE_TWIN_T, TUNE_NO_TWIN_T2, TUNE_NO_TWIN_H = 0x20, 0x40, 0x80, 0x100
@@ -168,7 +169,7 @@ ABI_SYMBOLS = (
     "apo_dims_compact_download", "apo_dims_codebook", "apo_packed_encode_host", "apo_score_host_packed", "apo_dims_packed_download", "apo_dims_d2book",
     "apo_tuple_encode_host", "apo_score_host_tuples", "apo_tuples_upload", "apo_dims_tuples", "apo_tuples_download", "apo_tuples_book",
     "apo_host_alloc", "apo_host_free",
-    "apo_last_timing", "apo_debug_partials", "apo_debug_twin_t_list", "apo_debug_twin_h", "apo_debug_corpus_digest", "apo_candidate_reports", "apo_candidate_corpus_reports", "apo_candidate_extremes", "apo_record_groups_upload", "apo_candidate_groups", "apo_candidate_spread", "apo_candidate_refs_upload", "apo_candidate_pairs", "apo_comm_unique_id", "apo_comm_init", "apo_comm_destroy", "apo_comm_join_mode",
+    "apo_last_timing", "apo_debug_partials", "apo_debug_twin_t_list", "apo_debug_twin_h", "apo_debug_corpus_digest", "apo_candidate_reports", "apo_candidate_corpus_reports", "apo_candidate_extremes", "apo_record_groups_upload", "apo_candidate_groups", "apo_candidate_spread", "apo_candidate_refs_upload", "apo_candidate_pairs", "apo_candidate_group_pairs", "apo_comm_unique_id", "apo_comm_init", "apo_comm_destroy", "apo_comm_join_mode",
 )
 
 
@@ -264,6 +265,7 @@ def load_library() -> C.CDLL:
     L.apo_candidate_spread.argtypes = [vp, u32, u32, vp]
     L.apo_candidate_refs_upload.argtypes = [vp, vp, u32]
     L.apo_candidate_pairs.argtypes = [vp, u32, u32, vp]
+    L.apo_candidate_group_pairs.argtypes = [vp, u32, u32, u32, vp]
     L.apo_comm_unique_id.argtypes = [vp]
     L.apo_comm_init.argtypes = [vp, i32, i32, vp]
     L.apo_comm_destroy.argtypes = [vp]
@@ -330,10 +332,10 @@ def records_from_json(text: str | bytes) -> np.ndarray:
 
 
 class ScoreResult:
-    __slots__ = ("scores", "counts", "topk", "report", "timing", "candidates", "candidate_corpus", "extremes", "groups", "spread", "pairs")
+    __slots__ = ("scores", "counts", "topk", "report", "timing", "candidates", "candidate_corpus", "extremes", "groups", "spread", "pairs", "group_pairs")
 
     def __init__(self, scores, counts, topk, report, timing, candidates=None, candidate_corpus=None, extremes=None, groups=None,
-                 spread=None, pairs=None):
+                 spread=None, pairs=None, group_pairs=None):
         self.scores, self.counts, self.topk, self.report, self.timing = scores, counts, topk, report, timing
         self.candidates = candidates        # CandidateReport array [C] when the call asked for the breakdown, else None
         self.candidate_corpus = candidate_corpus   # CorpusReport array [C] when the call asked for the per-candidate corpus reports
@@ -341,6 +343,7 @@ class ScoreResult:
         self.groups = groups                # GroupScore array [C][G] when the call asked for the per-candidate group scores
         self.spread = spread                # CandidateSpread array [C] when the call asked for the per-candidate reward spread
         self.pairs = pairs                  # CandidatePair array [C] when the call asked for the paired comparisons
+        self.group_pairs = group_pairs      # CandidatePair array [C][G] when the call asked for the per-group paired comparisons
 
 
 class Engine:
@@ -482,12 +485,12 @@ class Engine:
 
     def score_host_records(self, recs: np.ndarray, K: int, corpus: bool = False, recip: bool = False, variant: int = 0,
                            candidates: bool = False, candidate_corpus: bool = False, extremes: bool = False,
-                           groups: bool = False, spread: bool = False, pairs: bool = False) -> ScoreResult:
+                           groups: bool = False, spread: bool = False, pairs: bool = False, group_pairs: bool = False) -> ScoreResult:
         """recs: C-contiguous [C][T] of RECORD_DTYPE (32 B) or RECORD16_DTYPE (16 B) in host memory."""
         assert recs.flags.c_contiguous and recs.ndim == 2 and recs.dtype.itemsize in (32, 16)
         Cn, T = recs.shape
         o = self._opts(K, SRC_ROLLOUTS, corpus, recip, variant, 0, 0, candidates=candidates, candidate_corpus=candidate_corpus,
-                       extremes=extremes, groups=groups, spread=spread, pairs=pairs)
+                       extremes=extremes, groups=groups, spread=spread, pairs=pairs, group_pairs=group_pairs)
         scores = np.empty(Cn, np.float64)
         counts = np.empty(Cn, np.uint64)
         topk = np.empty(K, np.int32)
@@ -495,15 +498,16 @@ class Engine:
         self._ck(self._L.apo_score_host_records(self._h, C.byref(o), _p(recs), recs.dtype.itemsize, Cn, T, _p(scores), _p(counts),
                                                 _p(topk), C.byref(rep) if rep is not None else None))
         return ScoreResult(scores, counts, topk, rep, self.last_timing(), self._cands(Cn, candidates),
-                           self._ccorp(Cn, candidate_corpus), self._ext(Cn, extremes), self._grp(Cn, groups), self._spr(Cn, spread), self._pairs(Cn, pairs))
+                           self._ccorp(Cn, candidate_corpus), self._ext(Cn, extremes), self._grp(Cn, groups), self._spr(Cn, spread), self._pairs(Cn, pairs), self._gpairs(Cn, group_pairs))
 
     # -- scoring
     def _opts(self, K, source, corpus, recip, variant, first, count, timing=False, candidates=False,
-              candidate_corpus=False, extremes=False, groups=False, spread=False, pairs=False) -> ScoreOpts:
+              candidate_corpus=False, extremes=False, groups=False, spread=False, pairs=False, group_pairs=False) -> ScoreOpts:
         return ScoreOpts(K, source, (SCORE_CORPUS if corpus else 0) | (SCORE_RECIP if recip else 0) | (SCORE_TIMING if timing else 0)
                          | (SCORE_CANDIDATES if candidates else 0) | (SCORE_CANDIDATE_CORPUS if candidate_corpus else 0)
                          | (SCORE_CANDIDATE_EXTREMES if extremes else 0) | (SCORE_CANDIDATE_GROUPS if groups else 0)
-                         | (SCORE_CANDIDATE_SPREAD if spread else 0) | (SCORE_CANDIDATE_PAIRS if pairs else 0),
+                         | (SCORE_CANDIDATE_SPREAD if spread else 0) | (SCORE_CANDIDATE_PAIRS if pairs else 0)
+                         | (SCORE_CANDIDATE_GROUP_PAIRS if group_pairs else 0),
                          variant, first, count)
 
     def _cands(self, Cn: int, wanted: bool):
@@ -524,6 +528,9 @@ class Engine:
     def _pairs(self, Cn: int, wanted: bool):
         return self.candidate_pairs(0, Cn) if wanted else None
 
+    def _gpairs(self, Cn: int, wanted: bool):
+        return self.candidate_group_pairs(0, Cn) if wanted else None
+
     def candidate_refs_upload(self, refs):
         """apo_candidate_refs_upload: refs uint32 [C], the reference of every candidate (an index < C, or PAIR_NONE); an empty
         array releases them.  Scoring calls of C candidates with pairs=True then compare every candidate with its reference."""
@@ -535,6 +542,15 @@ class Engine:
         pairs=True (ApoError APO_E_STATE otherwise)."""
         out = (CandidatePair * n)()
         self._ck(self._L.apo_candidate_pairs(self._h, c0, n, out if n else None))
+        return out
+
+    def candidate_group_pairs(self, c0: int, n: int, G: int | None = None):
+        """apo_candidate_group_pairs: CandidatePair [n][G] of candidates [c0, c0+n) from the last scoring call, which must have
+        set group_pairs=True (ApoError APO_E_STATE otherwise): the paired comparison restricted to the record positions of
+        each label.  G defaults to the G of the labels held."""
+        G = self._groups_G if G is None else G
+        out = ((CandidatePair * max(G, 1)) * n)()
+        self._ck(self._L.apo_candidate_group_pairs(self._h, c0, n, G, out if n else None))
         return out
 
     def record_groups_upload(self, labels, G: int = 0):
@@ -584,8 +600,8 @@ class Engine:
 
     def score(self, Cn: int, K: int, source: int = SRC_DIMS, corpus: bool = False, recip: bool = False,
               variant: int = 0, first: int = 0, count: int = 0, timing: bool = False, candidates: bool = False,
-              candidate_corpus: bool = False, extremes: bool = False, groups: bool = False, spread: bool = False, pairs: bool = False) -> ScoreResult:
-        o = self._opts(K, source, corpus, recip, variant, first, count, timing, candidates, candidate_corpus, extremes, groups, spread, pairs)
+              candidate_corpus: bool = False, extremes: bool = False, groups: bool = False, spread: bool = False, pairs: bool = False, group_pairs: bool = False) -> ScoreResult:
+        o = self._opts(K, source, corpus, recip, variant, first, count, timing, candidates, candidate_corpus, extremes, groups, spread, pairs, group_pairs)
         scores = np.empty(Cn, np.float64)
         counts = np.empty(Cn, np.uint64)
         topk = np.empty(K, np.int32)
@@ -597,7 +613,7 @@ class Engine:
             self._ck(rc)
         L.apo_last_timing(self._h, C.byref(t))
         return ScoreResult(scores, counts, topk, rep, t, self._cands(Cn, candidates), self._ccorp(Cn, candidate_corpus),
-                           self._ext(Cn, extremes), self._grp(Cn, groups), self._spr(Cn, spread), self._pairs(Cn, pairs))
+                           self._ext(Cn, extremes), self._grp(Cn, groups), self._spr(Cn, spread), self._pairs(Cn, pairs), self._gpairs(Cn, group_pairs))
 
     # chunked form: begin / accumulate (per candidate chunk or record window) / finish
     def score_begin(self, C_total: int):
@@ -605,15 +621,15 @@ class Engine:
 
     def score_accumulate(self, cand_offset: int = 0, source: int = SRC_DIMS, recip: bool = False, variant: int = 0,
                          first: int = 0, count: int = 0, candidates: bool = False, candidate_corpus: bool = False,
-                         extremes: bool = False, groups: bool = False, spread: bool = False, pairs: bool = False):
+                         extremes: bool = False, groups: bool = False, spread: bool = False, pairs: bool = False, group_pairs: bool = False):
         o = self._opts(0, source, False, recip, variant, first, count, candidates=candidates, candidate_corpus=candidate_corpus,
-                       extremes=extremes, groups=groups, spread=spread, pairs=pairs)
+                       extremes=extremes, groups=groups, spread=spread, pairs=pairs, group_pairs=group_pairs)
         self._ck(self._L.apo_score_accumulate(self._h, C.byref(o), cand_offset))
 
     def score_finish(self, C_total: int, K: int, corpus: bool = False, candidates: bool = False,
-                     candidate_corpus: bool = False, extremes: bool = False, groups: bool = False, spread: bool = False, pairs: bool = False) -> ScoreResult:
+                     candidate_corpus: bool = False, extremes: bool = False, groups: bool = False, spread: bool = False, pairs: bool = False, group_pairs: bool = False) -> ScoreResult:
         o = self._opts(K, SRC_DIMS, corpus, False, 0, 0, 0, candidates=candidates, candidate_corpus=candidate_corpus, extremes=extremes,
-                       groups=groups, spread=spread, pairs=pairs)
+                       groups=groups, spread=spread, pairs=pairs, group_pairs=group_pairs)
         scores = np.empty(C_total, np.float64)
         counts = np.empty(C_total, np.uint64)
         topk = np.empty(K, np.int32)
@@ -622,14 +638,14 @@ class Engine:
                                           C.byref(rep) if rep is not None else None))
         return ScoreResult(scores, counts, topk, rep, self.last_timing(), self._cands(C_total, candidates),
                            self._ccorp(C_total, candidate_corpus), self._ext(C_total, extremes), self._grp(C_total, groups),
-                           self._spr(C_total, spread), self._pairs(C_total, pairs))
+                           self._spr(C_total, spread), self._pairs(C_total, pairs), self._gpairs(C_total, group_pairs))
 
     def score_host(self, dims: np.ndarray, K: int, corpus: bool = False, recip: bool = False, variant: int = 0,
-                   candidates: bool = False, extremes: bool = False, groups: bool = False, spread: bool = False, pairs: bool = False) -> ScoreResult:
+                   candidates: bool = False, extremes: bool = False, groups: bool = False, spread: bool = False, pairs: bool = False, group_pairs: bool = False) -> ScoreResult:
         """dims: C-contiguous float32 [C][T][9] in (preferably pinned) host memory."""
         assert dims.dtype == np.float32 and dims.flags.c_contiguous and dims.ndim == 3 and dims.shape[2] == NDIM
         Cn, T, _ = dims.shape
-        o = self._opts(K, SRC_DIMS, corpus, recip, variant, 0, 0, candidates=candidates, extremes=extremes, groups=groups, spread=spread, pairs=pairs)
+        o = self._opts(K, SRC_DIMS, corpus, recip, variant, 0, 0, candidates=candidates, extremes=extremes, groups=groups, spread=spread, pairs=pairs, group_pairs=group_pairs)
         scores = np.empty(Cn, np.float64)
         counts = np.empty(Cn, np.uint64)
         topk = np.empty(K, np.int32)
@@ -637,7 +653,7 @@ class Engine:
         self._ck(self._L.apo_score_host(self._h, C.byref(o), _p(dims), Cn, T, _p(scores), _p(counts), _p(topk),
                                         C.byref(rep) if rep is not None else None))
         return ScoreResult(scores, counts, topk, rep, self.last_timing(), self._cands(Cn, candidates), extremes=self._ext(Cn, extremes),
-                           groups=self._grp(Cn, groups), spread=self._spr(Cn, spread), pairs=self._pairs(Cn, pairs))
+                           groups=self._grp(Cn, groups), spread=self._spr(Cn, spread), pairs=self._pairs(Cn, pairs), group_pairs=self._gpairs(Cn, group_pairs))
 
     # -- Form Q in host memory (compact wire format)
     def dims_codebook(self) -> np.ndarray:
@@ -653,13 +669,13 @@ class Engine:
 
     def score_host_compact(self, q8: np.ndarray, d2: np.ndarray, li: np.ndarray, codebook: np.ndarray, K: int, corpus: bool = False,
                            recip: bool = False, candidates: bool = False, extremes: bool = False,
-                          groups: bool = False, spread: bool = False, pairs: bool = False) -> ScoreResult:
+                          groups: bool = False, spread: bool = False, pairs: bool = False, group_pairs: bool = False) -> ScoreResult:
         """q8 uint64 [C][T], d2 float32 [C][T], li uint16 [C][T] in (preferably pinned) host memory + the uint32[2048] codebook."""
         assert q8.dtype == np.uint64 and d2.dtype == np.float32 and li.dtype == np.uint16 and q8.shape == d2.shape == li.shape and q8.ndim == 2
         assert q8.flags.c_contiguous and d2.flags.c_contiguous and li.flags.c_contiguous
         codebook = np.ascontiguousarray(codebook, np.uint32)
         Cn, T = q8.shape
-        o = self._opts(K, SRC_DIMS, corpus, recip, 0, 0, 0, candidates=candidates, extremes=extremes, groups=groups, spread=spread, pairs=pairs)
+        o = self._opts(K, SRC_DIMS, corpus, recip, 0, 0, 0, candidates=candidates, extremes=extremes, groups=groups, spread=spread, pairs=pairs, group_pairs=group_pairs)
         scores = np.empty(Cn, np.float64)
         counts = np.empty(Cn, np.uint64)
         topk = np.empty(K, np.int32)
@@ -667,7 +683,7 @@ class Engine:
         self._ck(self._L.apo_score_host_compact(self._h, C.byref(o), _p(q8), _p(d2), _p(li), _p(codebook), Cn, T, _p(scores), _p(counts),
                                                 _p(topk), C.byref(rep) if rep is not None else None))
         return ScoreResult(scores, counts, topk, rep, self.last_timing(), self._cands(Cn, candidates), extremes=self._ext(Cn, extremes),
-                           groups=self._grp(Cn, groups), spread=self._spr(Cn, spread), pairs=self._pairs(Cn, pairs))
+                           groups=self._grp(Cn, groups), spread=self._spr(Cn, spread), pairs=self._pairs(Cn, pairs), group_pairs=self._gpairs(Cn, group_pairs))
 
     def dims_d2book(self) -> np.ndarray:
         out = np.empty(4096, np.uint32)
@@ -682,13 +698,13 @@ class Engine:
 
     def score_host_packed(self, pc: np.ndarray, pd: np.ndarray, codebook: np.ndarray, d2book: np.ndarray, K: int, corpus: bool = False,
                           recip: bool = False, candidates: bool = False, extremes: bool = False,
-                          groups: bool = False, spread: bool = False, pairs: bool = False) -> ScoreResult:
+                          groups: bool = False, spread: bool = False, pairs: bool = False, group_pairs: bool = False) -> ScoreResult:
         """Form P: pc uint32 [C][T] (eight 4-bit codes), pd uint16 [C][T] (tool_success_rate index) + the two codebooks."""
         assert pc.dtype == np.uint32 and pd.dtype == np.uint16 and pc.shape == pd.shape and pc.ndim == 2 and pc.flags.c_contiguous and pd.flags.c_contiguous
         codebook, d2book = np.ascontiguousarray(codebook, np.uint32), np.ascontiguousarray(d2book, np.uint32)
         assert codebook.size == 2048 and d2book.size == 4096
         Cn, T = pc.shape
-        o = self._opts(K, SRC_DIMS, corpus, recip, 0, 0, 0, candidates=candidates, extremes=extremes, groups=groups, spread=spread, pairs=pairs)
+        o = self._opts(K, SRC_DIMS, corpus, recip, 0, 0, 0, candidates=candidates, extremes=extremes, groups=groups, spread=spread, pairs=pairs, group_pairs=group_pairs)
         scores = np.empty(Cn, np.float64)
         counts = np.empty(Cn, np.uint64)
         topk = np.empty(K, np.int32)
@@ -696,7 +712,7 @@ class Engine:
         self._ck(self._L.apo_score_host_packed(self._h, C.byref(o), _p(pc), _p(pd), _p(codebook), _p(d2book), Cn, T, _p(scores), _p(counts),
                                                _p(topk), C.byref(rep) if rep is not None else None))
         return ScoreResult(scores, counts, topk, rep, self.last_timing(), self._cands(Cn, candidates), extremes=self._ext(Cn, extremes),
-                           groups=self._grp(Cn, groups), spread=self._spr(Cn, spread), pairs=self._pairs(Cn, pairs))
+                           groups=self._grp(Cn, groups), spread=self._spr(Cn, spread), pairs=self._pairs(Cn, pairs), group_pairs=self._gpairs(Cn, group_pairs))
 
     @staticmethod
     def _tuple_args(tl, th, tbook, codebook, d2book):
@@ -709,12 +725,12 @@ class Engine:
 
     def score_host_tuples(self, tl: np.ndarray, th: np.ndarray, tbook, codebook: np.ndarray, d2book: np.ndarray, K: int, corpus: bool = False,
                           recip: bool = False, candidates: bool = False, extremes: bool = False,
-                          groups: bool = False, spread: bool = False, pairs: bool = False) -> ScoreResult:
+                          groups: bool = False, spread: bool = False, pairs: bool = False, group_pairs: bool = False) -> ScoreResult:
         """Form T: tl uint16 [C][T] + th uint8 [C][T] (24-bit dictionary indices), tbook = (pc uint32 [n], pd uint16 [n]) the distinct
         evaluations as Form P pairs, + the two codebooks of Form P."""
         tb_pc, tb_pd, codebook, d2book = self._tuple_args(tl, th, tbook, codebook, d2book)
         Cn, T = tl.shape
-        o = self._opts(K, SRC_DIMS, corpus, recip, 0, 0, 0, candidates=candidates, extremes=extremes, groups=groups, spread=spread, pairs=pairs)
+        o = self._opts(K, SRC_DIMS, corpus, recip, 0, 0, 0, candidates=candidates, extremes=extremes, groups=groups, spread=spread, pairs=pairs, group_pairs=group_pairs)
         scores = np.empty(Cn, np.float64)
         counts = np.empty(Cn, np.uint64)
         topk = np.empty(K, np.int32)
@@ -722,7 +738,7 @@ class Engine:
         self._ck(self._L.apo_score_host_tuples(self._h, C.byref(o), _p(tl), _p(th), _p(tb_pc), _p(tb_pd), tb_pc.size, _p(codebook), _p(d2book), Cn, T,
                                                _p(scores), _p(counts), _p(topk), C.byref(rep) if rep is not None else None))
         return ScoreResult(scores, counts, topk, rep, self.last_timing(), self._cands(Cn, candidates), extremes=self._ext(Cn, extremes),
-                           groups=self._grp(Cn, groups), spread=self._spr(Cn, spread), pairs=self._pairs(Cn, pairs))
+                           groups=self._grp(Cn, groups), spread=self._spr(Cn, spread), pairs=self._pairs(Cn, pairs), group_pairs=self._gpairs(Cn, group_pairs))
 
     def tuples_upload(self, tl: np.ndarray, th: np.ndarray, tbook, codebook: np.ndarray, d2book: np.ndarray):
         """Make a Form T tensor resident: score(C, K, source=SRC_TUPLES) then reads 3 B per evaluation."""

@@ -22,7 +22,7 @@ import { ApoResidentQuery, ApoScoreBlocks, ApoTupleBuffers, IApoScoringService }
 
 type Blocks = { scores: ArrayBuffer; counts: ArrayBuffer; topk: ArrayBuffer; report: ArrayBuffer; candidates?: ArrayBuffer; candidateCorpus?: ArrayBuffer;
 	candidateExtremes?: ArrayBuffer; candidateGroups?: ArrayBuffer; candidateSpread?: ArrayBuffer;
-	candidatePairs?: ArrayBuffer };
+	candidatePairs?: ArrayBuffer; candidateGroupPairs?: ArrayBuffer };
 
 interface ApoAddon {
 	create(device: number): unknown | null;             // null when no H100 / library: never throws
@@ -37,15 +37,15 @@ interface ApoAddon {
 	scoreResident(handle: unknown, query: ApoResidentQuery): Promise<Blocks>;
 	score(handle: unknown, dims: ArrayBuffer, C: number, T: number, corpus: ArrayBuffer | null, K: number, candidates?: boolean,
 		candidateExtremes?: boolean, candidateGroups?: number, candidateSpread?: boolean,
-		candidatePairs?: boolean): Promise<Blocks>;
+		candidatePairs?: boolean, candidateGroupPairs?: number): Promise<Blocks>;
 	scoreHostRecords(handle: unknown, records: ArrayBuffer, rowBytes: number, C: number, T: number, corpus: ArrayBuffer | null, K: number,
 		candidates?: boolean, candidateCorpus?: boolean, candidateExtremes?: boolean, candidateGroups?: number, candidateSpread?: boolean,
-		candidatePairs?: boolean): Promise<Blocks>;
+		candidatePairs?: boolean, candidateGroupPairs?: number): Promise<Blocks>;
 	/** Form D -> Form T on worker threads of the addon (no GPU): 3 bytes per evaluation instead of 36; null = not categorical. */
 	encodeTuples(dims: ArrayBuffer, C: number, T: number, nthreads?: number): Promise<ApoTuples | null>;
 	scoreHostTuples(handle: unknown, tuples: ApoTuples, C: number, T: number, corpus: ArrayBuffer | null, K: number, candidates?: boolean,
 		candidateExtremes?: boolean, candidateGroups?: number, candidateSpread?: boolean,
-		candidatePairs?: boolean): Promise<Blocks>;
+		candidatePairs?: boolean, candidateGroupPairs?: number): Promise<Blocks>;
 	rewardBatch(handle: unknown, records: ArrayBuffer): Promise<{ dims: ArrayBuffer; masks: ArrayBuffer; finals: ArrayBuffer }>;
 	recordsFromJson(utf8: ArrayBuffer): ArrayBuffer | null;
 }
@@ -71,6 +71,7 @@ function wrapBlocks(r: Blocks): ApoScoreBlocks {
 	if (r.candidateGroups) { out.candidateGroups = VSBuffer.wrap(new Uint8Array(r.candidateGroups)); }     // apo_group_score[C][G]
 	if (r.candidateSpread) { out.candidateSpread = VSBuffer.wrap(new Uint8Array(r.candidateSpread)); }     // struct apo_candidate_spread[C]
 	if (r.candidatePairs) { out.candidatePairs = VSBuffer.wrap(new Uint8Array(r.candidatePairs)); }     // struct apo_candidate_pair[C]
+	if (r.candidateGroupPairs) { out.candidateGroupPairs = VSBuffer.wrap(new Uint8Array(r.candidateGroupPairs)); }     // struct apo_candidate_pair[C][G]
 	return out;
 }
 
@@ -193,9 +194,11 @@ export class ApoScoringMainService implements IApoScoringService {
 
 	// ---- one-shot path ------------------------------------------------------------------------
 	async score(dims: VSBuffer, C: number, T: number, corpus: VSBuffer | undefined, K: number, candidates?: boolean,
-		candidateExtremes?: boolean, candidateGroups?: number, candidateSpread?: boolean, candidatePairs?: boolean): Promise<ApoScoreBlocks> {
+		candidateExtremes?: boolean, candidateGroups?: number, candidateSpread?: boolean, candidatePairs?: boolean,
+		candidateGroupPairs?: number): Promise<ApoScoreBlocks> {
 		return wrapBlocks(await (await this._need()).score(this._handle, ab(dims), C, T, corpus ? ab(corpus) : null, K, !!candidates,
-			!!candidateExtremes, candidateGroups ?? 0, !!candidateSpread, !!candidatePairs));
+			!!candidateExtremes, candidateGroups ?? 0, !!candidateSpread, !!candidatePairs,
+			candidateGroupPairs ?? 0));
 	}
 
 	/** fp32 evaluations -> Form T (3 bytes per evaluation + the dictionary of distinct evaluations); undefined when the tensor is not
@@ -211,16 +214,19 @@ export class ApoScoringMainService implements IApoScoringService {
 
 	/** Same result as score() on the tensor the tuples were encoded from; 12x fewer bytes over IPC and PCIe. */
 	async scoreTuples(t: ApoTupleBuffers, C: number, T: number, corpus: VSBuffer | undefined, K: number, candidates?: boolean,
-		candidateExtremes?: boolean, candidateGroups?: number, candidateSpread?: boolean, candidatePairs?: boolean): Promise<ApoScoreBlocks> {
+		candidateExtremes?: boolean, candidateGroups?: number, candidateSpread?: boolean, candidatePairs?: boolean,
+		candidateGroupPairs?: number): Promise<ApoScoreBlocks> {
 		const raw: ApoTuples = { tl: ab(t.tl), th: ab(t.th), tbookPc: ab(t.tbookPc), tbookPd: ab(t.tbookPd), codebook: ab(t.codebook), d2book: ab(t.d2book), nTuples: t.nTuples };
 		return wrapBlocks(await (await this._need()).scoreHostTuples(this._handle, raw, C, T, corpus ? ab(corpus) : null, K, !!candidates,
-			!!candidateExtremes, candidateGroups ?? 0, !!candidateSpread, !!candidatePairs));
+			!!candidateExtremes, candidateGroups ?? 0, !!candidateSpread, !!candidatePairs,
+			candidateGroupPairs ?? 0));
 	}
 
 	async scoreHostRecords(records: VSBuffer, rowBytes: 32 | 16, C: number, T: number, corpus: VSBuffer | undefined, K: number,
 		candidates?: boolean, candidateCorpus?: boolean, candidateExtremes?: boolean, candidateGroups?: number,
-		candidateSpread?: boolean, candidatePairs?: boolean): Promise<ApoScoreBlocks> {
+		candidateSpread?: boolean, candidatePairs?: boolean, candidateGroupPairs?: number): Promise<ApoScoreBlocks> {
 		return wrapBlocks(await (await this._need()).scoreHostRecords(this._handle, ab(records), rowBytes, C, T, corpus ? ab(corpus) : null, K, !!candidates,
-			!!candidateCorpus, !!candidateExtremes, candidateGroups ?? 0, !!candidateSpread, !!candidatePairs));
+			!!candidateCorpus, !!candidateExtremes, candidateGroups ?? 0, !!candidateSpread, !!candidatePairs,
+			candidateGroupPairs ?? 0));
 	}
 }

@@ -30,6 +30,7 @@ export interface ApoScoreBlocks {
 	candidateGroups?: VSBuffer;   // apo_group_score[C][G] (56 bytes each, decodeCandidateGroups); only when asked for
 	candidateSpread?: VSBuffer;   // struct apo_candidate_spread[C] (88 bytes each, decodeCandidateSpread); only when asked for
 	candidatePairs?: VSBuffer;   // struct apo_candidate_pair[C] (128 bytes each, decodeCandidatePairs); only when asked for
+	candidateGroupPairs?: VSBuffer;   // struct apo_candidate_pair[C][G] (128 bytes each, decodeCandidateGroupPairs); only when asked for
 }
 
 /** Form T of a float32[C][T][9] tensor (include/apo_b200.h): tl uint16[C][T] | th uint8[C][T] = the 24-bit dictionary index of every
@@ -51,6 +52,7 @@ export interface ApoResidentQuery {
 	candidateGroups?: number;   // G of the uploaded record groups: also split every candidate's rollouts by group (ApoScoreBlocks.candidateGroups)
 	candidateSpread?: 0 | 1;   // also build every candidate's reward spread (ApoScoreBlocks.candidateSpread)
 	candidatePairs?: 0 | 1;   // also compare every candidate with its candidateRefsUpload reference (ApoScoreBlocks.candidatePairs)
+	candidateGroupPairs?: number;   // G of the uploaded record groups: also make that comparison per group (ApoScoreBlocks.candidateGroupPairs)
 	first?: number;         // window [first, first + count) of the trace axis; count 0 = to the end
 	count?: number;
 }
@@ -94,18 +96,22 @@ export interface IApoScoringService {
 	 *  candidateExtremes: also return every candidate's 32 lowest- and highest-reward rollouts (ApoScoreBlocks.candidateExtremes);
 	 *  candidateGroups: the G of recordGroupsUpload, also return every candidate's scores per record group (ApoScoreBlocks.candidateGroups);
 	 *  candidateSpread: also return every candidate's reward spread (ApoScoreBlocks.candidateSpread);
-	 *  candidatePairs: also compare every candidate with its reference (ApoScoreBlocks.candidatePairs). */
+	 *  candidatePairs: also compare every candidate with its reference (ApoScoreBlocks.candidatePairs);
+	 *  candidateGroupPairs: the G of recordGroupsUpload, also make that comparison per record group (ApoScoreBlocks.candidateGroupPairs). */
 	score(dims: VSBuffer, C: number, T: number, corpus: VSBuffer | undefined, K: number, candidates?: boolean,
-		candidateExtremes?: boolean, candidateGroups?: number, candidateSpread?: boolean, candidatePairs?: boolean): Promise<ApoScoreBlocks>;
+		candidateExtremes?: boolean, candidateGroups?: number, candidateSpread?: boolean, candidatePairs?: boolean,
+		candidateGroupPairs?: number): Promise<ApoScoreBlocks>;
 	/** [C][T] trace records (the IDE's own representation): 2.2x fewer PCIe bytes than fp32 dims with 16-byte rows.
 	 *  candidateCorpus: also return the corpus report of every candidate's records (ApoScoreBlocks.candidateCorpus). */
 	scoreHostRecords(records: VSBuffer, rowBytes: 32 | 16, C: number, T: number, corpus: VSBuffer | undefined, K: number, candidates?: boolean,
-		candidateCorpus?: boolean, candidateExtremes?: boolean, candidateGroups?: number, candidateSpread?: boolean, candidatePairs?: boolean): Promise<ApoScoreBlocks>;
+		candidateCorpus?: boolean, candidateExtremes?: boolean, candidateGroups?: number, candidateSpread?: boolean, candidatePairs?: boolean,
+		candidateGroupPairs?: number): Promise<ApoScoreBlocks>;
 	/** fp32 evaluations -> Form T (include/apo_b200.h): a 24-bit dictionary index per evaluation (3 bytes instead of 36) + the
 	 *  dictionary of distinct evaluations.  For evaluations that are scored more than once, kept, or moved between processes. */
 	encodeTuples(dims: VSBuffer, C: number, T: number): Promise<ApoTupleBuffers | undefined>;
 	scoreTuples(tuples: ApoTupleBuffers, C: number, T: number, corpus: VSBuffer | undefined, K: number, candidates?: boolean,
-		candidateExtremes?: boolean, candidateGroups?: number, candidateSpread?: boolean, candidatePairs?: boolean): Promise<ApoScoreBlocks>;
+		candidateExtremes?: boolean, candidateGroups?: number, candidateSpread?: boolean, candidatePairs?: boolean,
+		candidateGroupPairs?: number): Promise<ApoScoreBlocks>;
 }
 
 export const IApoScoringService = createDecorator<IApoScoringService>('senweaverApoScoringService');
@@ -130,16 +136,25 @@ export class ApoScoringService implements IApoScoringService {
 	recordGroupsUpload(labels: VSBuffer, G: number) { return this._proxy.recordGroupsUpload(labels, G); }
 	candidateRefsUpload(refs: VSBuffer) { return this._proxy.candidateRefsUpload(refs); }
 	scoreResident(query: ApoResidentQuery) { return this._proxy.scoreResident(query); }
-	// A call without group scores, spreads or pairs sends the channel the same arguments as before those options existed.
+	// A call without group scores, spreads, pairs or group pairs sends the channel the same arguments as before those options existed.
 	score(dims: VSBuffer, C: number, T: number, corpus: VSBuffer | undefined, K: number, candidates?: boolean, candidateExtremes?: boolean,
-		candidateGroups?: number, candidateSpread?: boolean, candidatePairs?: boolean) {
+		candidateGroups?: number, candidateSpread?: boolean, candidatePairs?: boolean, candidateGroupPairs?: number) {
+		if (candidateGroupPairs) {
+			return this._proxy.score(dims, C, T, corpus, K, candidates, candidateExtremes, candidateGroups ?? 0, !!candidateSpread, !!candidatePairs,
+				candidateGroupPairs);
+		}
 		if (candidatePairs) { return this._proxy.score(dims, C, T, corpus, K, candidates, candidateExtremes, candidateGroups ?? 0, !!candidateSpread, true); }
 		if (candidateSpread) { return this._proxy.score(dims, C, T, corpus, K, candidates, candidateExtremes, candidateGroups ?? 0, true); }
 		if (candidateGroups) { return this._proxy.score(dims, C, T, corpus, K, candidates, candidateExtremes, candidateGroups); }
 		return this._proxy.score(dims, C, T, corpus, K, candidates, candidateExtremes);
 	}
 	scoreHostRecords(records: VSBuffer, rowBytes: 32 | 16, C: number, T: number, corpus: VSBuffer | undefined, K: number, candidates?: boolean,
-		candidateCorpus?: boolean, candidateExtremes?: boolean, candidateGroups?: number, candidateSpread?: boolean, candidatePairs?: boolean) {
+		candidateCorpus?: boolean, candidateExtremes?: boolean, candidateGroups?: number, candidateSpread?: boolean, candidatePairs?: boolean,
+		candidateGroupPairs?: number) {
+		if (candidateGroupPairs) {
+			return this._proxy.scoreHostRecords(records, rowBytes, C, T, corpus, K, candidates, candidateCorpus, candidateExtremes, candidateGroups ?? 0,
+				!!candidateSpread, !!candidatePairs, candidateGroupPairs);
+		}
 		if (candidatePairs) {
 			return this._proxy.scoreHostRecords(records, rowBytes, C, T, corpus, K, candidates, candidateCorpus, candidateExtremes, candidateGroups ?? 0,
 				!!candidateSpread, true);
@@ -152,7 +167,11 @@ export class ApoScoringService implements IApoScoringService {
 	}
 	encodeTuples(dims: VSBuffer, C: number, T: number) { return this._proxy.encodeTuples(dims, C, T); }
 	scoreTuples(tuples: ApoTupleBuffers, C: number, T: number, corpus: VSBuffer | undefined, K: number, candidates?: boolean,
-		candidateExtremes?: boolean, candidateGroups?: number, candidateSpread?: boolean, candidatePairs?: boolean) {
+		candidateExtremes?: boolean, candidateGroups?: number, candidateSpread?: boolean, candidatePairs?: boolean, candidateGroupPairs?: number) {
+		if (candidateGroupPairs) {
+			return this._proxy.scoreTuples(tuples, C, T, corpus, K, candidates, candidateExtremes, candidateGroups ?? 0, !!candidateSpread, !!candidatePairs,
+				candidateGroupPairs);
+		}
 		if (candidatePairs) {
 			return this._proxy.scoreTuples(tuples, C, T, corpus, K, candidates, candidateExtremes, candidateGroups ?? 0, !!candidateSpread, true);
 		}

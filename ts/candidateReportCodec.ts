@@ -25,7 +25,8 @@
  *
  *  And the decoder of the paired comparisons (ApoScoreBlocks.candidatePairs): struct apo_candidate_pair[C], each candidate
  *  against its reference on the rollouts both were scored on: wins, losses, ties, the exact paired sums and the mean reward
- *  difference with its standard error.
+ *  difference with its standard error.  decodeCandidateGroupPairs reads the same record per (candidate, group) of a
+ *  candidateGroupPairs block (struct apo_candidate_pair[C][G]): that comparison on the rollouts of each record group.
  *
  *  The byte offsets below are pinned to the C structs by tests/test_napi_candidates.py, tests/test_candidate_corpus_cpu.py,
  *  tests/test_napi_candidate_extremes.py, tests/test_candidate_groups_cpu.py, tests/test_candidate_spread_cpu.py and
@@ -251,19 +252,31 @@ export interface CandidatePair {
 /** The paired comparisons of a candidatePairs block (ApoScoreBlocks.candidatePairs) of C candidates. */
 export function decodeCandidatePairs(buf: VSBuffer, C: number): CandidatePair[] {
 	if (C < 0 || C * CANDIDATE_PAIR_BYTES > buf.byteLength) { throw new RangeError(`${C} candidate pairs do not fit the block`); }
-	return Array.from({ length: C }, (_, c) => {
-		const v = new DataView(buf.buffer.buffer, buf.buffer.byteOffset + c * CANDIDATE_PAIR_BYTES, CANDIDATE_PAIR_BYTES);
-		const ref = v.getUint32(OFF_PR_REF, true);
-		const n = u64(v, OFF_PR_N);
-		const f = (o: number) => v.getFloat64(o, true);
-		const sumSq = v.getBigUint64(OFF_PR_SUM_SQ, true) | (v.getBigUint64(OFF_PR_SUM_SQ + 8, true) << 64n) |
-			(v.getBigUint64(OFF_PR_SUM_SQ + 16, true) << 128n);
-		return {
-			candidate: c, reference: ref === PAIR_NONE ? null : ref, n, wins: u64(v, OFF_PR_WINS), losses: u64(v, OFF_PR_LOSSES),
-			ties: u64(v, OFF_PR_TIES), candOnly: u64(v, OFF_PR_CAND_ONLY), refOnly: u64(v, OFF_PR_REF_ONLY),
-			sum: (v.getBigInt64(OFF_PR_SUM_HI, true) << 64n) | v.getBigUint64(OFF_PR_SUM_LO, true), sumSq,
-			meanDiff: n === 0 ? null : f(OFF_PR_MEAN_DIFF),
-			variance: n < 2 ? null : f(OFF_PR_VARIANCE), stdDev: n < 2 ? null : f(OFF_PR_STD_DEV), stdErr: n < 2 ? null : f(OFF_PR_STD_ERR),
-		};
-	});
+	return Array.from({ length: C }, (_, c) => decodePair(buf, c * CANDIDATE_PAIR_BYTES, c));
+}
+
+/** The paired comparisons per record group of a candidateGroupPairs block (ApoScoreBlocks.candidateGroupPairs) of C candidates
+ *  and G groups: out[c][g] is candidate c against its reference on the rollouts of group g. */
+export function decodeCandidateGroupPairs(buf: VSBuffer, C: number, G: number): CandidatePair[][] {
+	if (C < 0 || G < 1 || C * G * CANDIDATE_PAIR_BYTES > buf.byteLength) {
+		throw new RangeError(`${C} x ${G} candidate group pairs do not fit the block`);
+	}
+	return Array.from({ length: C }, (_, c) => Array.from({ length: G }, (_, g) => decodePair(buf, (c * G + g) * CANDIDATE_PAIR_BYTES, c)));
+}
+
+/** One struct apo_candidate_pair at byte offset off of the block: candidate c against its reference. */
+function decodePair(buf: VSBuffer, off: number, c: number): CandidatePair {
+	const v = new DataView(buf.buffer.buffer, buf.buffer.byteOffset + off, CANDIDATE_PAIR_BYTES);
+	const ref = v.getUint32(OFF_PR_REF, true);
+	const n = u64(v, OFF_PR_N);
+	const f = (o: number) => v.getFloat64(o, true);
+	const sumSq = v.getBigUint64(OFF_PR_SUM_SQ, true) | (v.getBigUint64(OFF_PR_SUM_SQ + 8, true) << 64n) |
+		(v.getBigUint64(OFF_PR_SUM_SQ + 16, true) << 128n);
+	return {
+		candidate: c, reference: ref === PAIR_NONE ? null : ref, n, wins: u64(v, OFF_PR_WINS), losses: u64(v, OFF_PR_LOSSES),
+		ties: u64(v, OFF_PR_TIES), candOnly: u64(v, OFF_PR_CAND_ONLY), refOnly: u64(v, OFF_PR_REF_ONLY),
+		sum: (v.getBigInt64(OFF_PR_SUM_HI, true) << 64n) | v.getBigUint64(OFF_PR_SUM_LO, true), sumSq,
+		meanDiff: n === 0 ? null : f(OFF_PR_MEAN_DIFF),
+		variance: n < 2 ? null : f(OFF_PR_VARIANCE), stdDev: n < 2 ? null : f(OFF_PR_STD_DEV), stdErr: n < 2 ? null : f(OFF_PR_STD_ERR),
+	};
 }
