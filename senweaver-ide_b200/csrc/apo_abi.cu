@@ -764,7 +764,7 @@ int launch_score(apo_engine *e, const apo_score_opts *o, const Evals &ev, uint32
 		P.pairs = t->hp.p; P.off = t->ho.p; P.C = ev.C; P.nnz = t->hn; P.acc = acc; P.tval = t->vals.val[recip].p;
 		if (fused) {                                          // the digest pass (fused->T > 0: the corpus words) and the tail
 			P.corpus_on = 1; P.cd.k2 = *fused;
-			if (fused->T) { P.cd.ent = e->digest.ent.p; P.cd.n = e->digest.misc.p + 2; P.cd.fixed = e->digest.fixed.p; }
+			if (fused->T) { P.cd.ent = e->digest.ent.p; P.cd.n = e->digest.misc.p + 2; P.cd.fixed = e->digest.fixed.p; P.cd_n = e->digest.n; }
 		}
 		CK(apo::run_reward9th(P, e->sm_count, e->stream));
 	} else if (ev.read == Evals::K1t2) {

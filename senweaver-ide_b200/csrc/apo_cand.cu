@@ -510,7 +510,8 @@ k_cand_corpus_report(const long long *blk, long long *scratch, apo_corpus_report
 	FinalizeParams F{};
 	F.nranks = 1;
 	F.report = out + c;
-	build_report(F, corp);
+	__shared__ long long s_corp[CORP_EX];
+	build_report(F, corp, s_corp);
 }
 
 cudaError_t run_cand_corpus_report(long long *blk, uint32_t C, apo_corpus_report *out, cudaStream_t st) {

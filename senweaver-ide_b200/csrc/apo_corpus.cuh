@@ -8,6 +8,31 @@
 
 namespace apo {
 
+// Phase stamps of K1h (k_reward9th), in a build with -DAPO_K1H_DIAG only (examples/flagship_launch.py): %globaltimer of every
+// CTA at its entry, the end of its pairs (the last stream warp), the end of its digest share, its ticket, and in the
+// finalising CTA the start and end of finalize_block and the end of the publish.  Nothing in a product build.
+enum { KH_ST_ENTRY, KH_ST_PAIRS, KH_ST_DIGEST, KH_ST_TICKET, KH_ST_FIN0, KH_ST_FIN1, KH_ST_PUBLISH, KH_STAMPS = 8 };
+#ifdef APO_K1H_DIAG
+constexpr uint32_t KH_STAMP_WORDS = 256 * KH_STAMPS;
+static __device__ unsigned long long g_kh_stamp[KH_STAMP_WORDS];
+__device__ __forceinline__ unsigned long long kh_now() {
+	unsigned long long t;
+	asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+	return t;
+}
+// by thread 0 of the CTA
+__device__ __forceinline__ void kh_stamp(int k) {
+	if (threadIdx.x == 0 && blockIdx.x < 256) g_kh_stamp[blockIdx.x * KH_STAMPS + k] = kh_now();
+}
+// by lane 0 of every warp that calls it: the latest
+__device__ __forceinline__ void kh_stamp_max(int k) {
+	if ((threadIdx.x & 31) == 0 && blockIdx.x < 256) atomicMax(&g_kh_stamp[blockIdx.x * KH_STAMPS + k], kh_now());
+}
+#else
+__device__ __forceinline__ void kh_stamp(int) {}
+__device__ __forceinline__ void kh_stamp_max(int) {}
+#endif
+
 // First-three-examples slots hold INVERTED record indices (key = ~index, 0 = empty), so that zero-filled memory is
 // an armed slot set (one memset arms accumulators, slots and ticket).  Smallest index == largest key.
 __device__ __forceinline__ void ex_insert(unsigned long long *slots, unsigned long long key) {
@@ -292,6 +317,7 @@ __device__ __forceinline__ void corpus_tail(const K2Params &P, const unsigned lo
 		const unsigned int ticket = atomicAdd(P.ticket, 1u);
 		*s_last = (ticket == gridDim.x - 1);
 		if (*s_last) __threadfence();                             // acquire side: the other CTAs' flushes are visible from here on
+		kh_stamp(KH_ST_TICKET);
 	}
 	__syncthreads();
 	if (!*s_last) return;
@@ -335,63 +361,126 @@ static __device__ __noinline__ void cd_census_flush(const uint32_t *s_lo, const 
 // One call's corpus words from the digest: each CTA takes a contiguous share of the entries and runs, per entry, what
 // scan_record runs per record (key_ws, key_reward), times the entry's count; CTA 0 adds the fixed words and seeds its example
 // slots; then the tail of the stand-alone scan (ticket, examples, the last CTA finalises when the call asks for it).  Run by
-// the stand-alone k_corpus_digest and, after its pairs, by every CTA of K1h (k_reward9th) on whole rows of the Form T copy.
-// Block-wide; every thread of every CTA of the launch must enter.  Works for any blockDim.x that is a multiple of 32 (<= 1024).
-// P.fixed == NULL: no corpus words (a call without a corpus report), only the tail.
-static __device__ __noinline__ void corpus_digest_block(const CorpusDigestParams &P) {
-	__shared__ unsigned long long s_ex[APO_NPAT * 3];
-	__shared__ double s_cat[CAT_WORDS];
-	__shared__ double2 s_lut[512];
-	__shared__ uint32_t s_lo[CD_CENSUS + 1], s_hi[CD_CENSUS + 1];   // + the counted records
-	__shared__ unsigned long long s_part[32][6];                   // per warp: the limb sums of the reward and of d2
-	__shared__ bool s_last;
-	const int tid = threadIdx.x, lane = tid & 31;
+// the stand-alone k_corpus_digest on every warp of its CTAs (corpus_digest_block) and by K1h (k_reward9th) on one warp of
+// every CTA while the other warps stream the pairs (cd_warp, then cd_tail).  P.fixed == NULL: no corpus words (a call
+// without a corpus report), only the tail.
+struct CdShared {
+	unsigned long long ex[APO_NPAT * 3];
+	double cat[CAT_WORDS];
+	double2 lut[512];
+	uint32_t lo[CD_CENSUS + 1], hi[CD_CENSUS + 1];   // + the counted records
+	unsigned long long part[32][6];                  // per warp that ran entries: the limb sums of the reward and of d2
+	bool last;
+};
+// one instance per CTA, shared by the parts below
+__device__ __forceinline__ CdShared &cd_shared() {
+	__shared__ CdShared s;
+	return s;
+}
+
+// the CTA's examples, census counters and tables, by threads t = 0 .. nt - 1 of the caller's group (the caller syncs the group)
+__device__ __forceinline__ void cd_setup(const CorpusDigestParams &P, CdShared &S, int t, int nt) {
 	const K2Params &K = P.k2;
 	long long *corp = K.acc + (uint64_t)ACC_PER_CAND * K.C;
-	if (tid < APO_NPAT * 3) s_ex[tid] = blockIdx.x == 0 && P.fixed ? (unsigned long long)P.fixed[CD_FIXED + tid] : 0ull;
-	if (tid <= CD_CENSUS) { s_lo[tid] = 0u; s_hi[tid] = 0u; }
-	for (int i = tid; i < CAT_WORDS; i += blockDim.x) s_cat[i] = K.lut[1024 + i];
-	for (int i = tid; i < 512; i += blockDim.x) s_lut[i] = make_double2(K.lut[i], K.lut[512 + i]);
-	if (blockIdx.x == 0 && P.fixed && tid < CD_FIXED && P.fixed[tid]) atomicAdd((unsigned long long *)corp + CORP_TALLY + tid, (unsigned long long)P.fixed[tid]);
-	__syncthreads();
-	const double w2 = K.W.w[2];
-	const uint64_t n = P.fixed ? *P.n : 0, lo = n * blockIdx.x / gridDim.x, hi = n * (blockIdx.x + 1ull) / gridDim.x;
+	for (int i = t; i < APO_NPAT * 3; i += nt) S.ex[i] = blockIdx.x == 0 && P.fixed ? (unsigned long long)P.fixed[CD_FIXED + i] : 0ull;
+	for (int i = t; i <= CD_CENSUS; i += nt) { S.lo[i] = 0u; S.hi[i] = 0u; }
+	for (int i = t; i < CAT_WORDS; i += nt) S.cat[i] = K.lut[1024 + i];
+	for (int i = t; i < 512; i += nt) S.lut[i] = make_double2(K.lut[i], K.lut[512 + i]);
+	if (blockIdx.x == 0 && P.fixed)
+		for (int i = t; i < CD_FIXED; i += nt)
+			if (P.fixed[i]) atomicAdd((unsigned long long *)corp + CORP_TALLY + i, (unsigned long long)P.fixed[i]);
+}
+
+constexpr int CD_UNROLL = 4;   // entries in flight per lane
+
+// One warp's entries i = first + lane, first + lane + stride, ... below hi into the census counters; its limb sums go to
+// S.part[row].  Full-warp collective.
+static __device__ __noinline__ void cd_entries(const CorpusDigestParams &P, CdShared &S, uint64_t first, uint64_t stride, uint64_t hi,
+                                               int row) {
+	const int lane = threadIdx.x & 31;
+	const double w2 = P.k2.W.w[2];
 	Acc128 R, D2; R.zero(); D2.zero();
-	for (uint64_t i = lo + tid; i < hi; i += blockDim.x) {
-		const ulonglong2 e = P.ent[i];
-		const CatIdx ix = cd_key(e);
-		const unsigned long long c = e.y >> CD_COUNT_SHIFT;
-		double ws;
-		const uint32_t mask = key_ws(ix, w2, s_cat, ws);
-		long long fx;
-		if (key_reward<false>(ws, mask, s_lut, fx)) {             // TCS:784 totalWeight > 0
-			acc_add_mul(R, c, fx);
-			acc_add_mul(D2, c, to_fx(ix.d2));                     // +0.0 when not pushed
-			auto add = [&](int j) { cd_add(&s_lo[j], &s_hi[j], c); };
-			add(CD_CENSUS);
-			add(cd_census(0, (int)ix.i01));
-			if (ix.i3 < 4u) { add(cd_census(3, (int)ix.i3)); add(cd_census(4, (int)ix.i4)); }
-			if (ix.i5 < 4u) add(cd_census(5, (int)ix.i5));
-			if (ix.i6 < 6u) add(cd_census(6, (int)ix.i6));
-			if (ix.i7 < 4u) add(cd_census(7, (int)ix.i7));
-			if (ix.i8 < 4u) add(cd_census(8, (int)ix.i8));
+	for (uint64_t i0 = first + lane; i0 < hi; i0 += CD_UNROLL * stride) {
+		ulonglong2 e[CD_UNROLL];
+#pragma unroll
+		for (int u = 0; u < CD_UNROLL; u++) {
+			const uint64_t i = i0 + u * stride;
+			e[u] = i < hi ? P.ent[i] : make_ulonglong2(0ull, 0ull);
+		}
+#pragma unroll 1
+		for (int u = 0; u < CD_UNROLL; u++) {
+			if (i0 + u * stride >= hi) break;
+			const CatIdx ix = cd_key(e[u]);
+			const unsigned long long c = e[u].y >> CD_COUNT_SHIFT;
+			double ws;
+			const uint32_t mask = key_ws(ix, w2, S.cat, ws);
+			long long fx;
+			if (key_reward<false>(ws, mask, S.lut, fx)) {             // TCS:784 totalWeight > 0
+				acc_add_mul(R, c, fx);
+				acc_add_mul(D2, c, to_fx(ix.d2));                     // +0.0 when not pushed
+				auto add = [&](int j) { cd_add(&S.lo[j], &S.hi[j], c); };
+				add(CD_CENSUS);
+				add(cd_census(0, (int)ix.i01));
+				if (ix.i3 < 4u) { add(cd_census(3, (int)ix.i3)); add(cd_census(4, (int)ix.i4)); }
+				if (ix.i5 < 4u) add(cd_census(5, (int)ix.i5));
+				if (ix.i6 < 6u) add(cd_census(6, (int)ix.i6));
+				if (ix.i7 < 4u) add(cd_census(7, (int)ix.i7));
+				if (ix.i8 < 4u) add(cd_census(8, (int)ix.i8));
+			}
 		}
 	}
-	// the limbs are summed over the block first: one global atomic per limb and CTA (K1h runs this in 32 warps of every SM's
-	// CTA, and thousands of warps adding into the same six words serialise in L2)
 	const unsigned long long v[6] = {warp_sum_u64(R.lo & 0xffffffffull), warp_sum_u64(R.lo >> 32), warp_sum_u64((unsigned long long)R.hi),
 	                                 warp_sum_u64(D2.lo & 0xffffffffull), warp_sum_u64(D2.lo >> 32), warp_sum_u64((unsigned long long)D2.hi)};
 	if (lane == 0)
-		for (int k = 0; k < 6; k++) s_part[tid >> 5][k] = v[k];
-	__syncthreads();
-	if (tid >= 32 && tid < 38) {                                   // limb sums as flush_acc128 adds them (the high limb wraps as a signed sum)
-		const int k = tid - 32;
+		for (int k = 0; k < 6; k++) S.part[row][k] = v[k];
+}
+
+// After every warp that ran entries has written its row of S.part (rows [0, nrows)) and its census adds, and the caller has
+// synced them: `who` 0 turns the census into dimension sums, 1..6 add one limb each, summed over the rows (the limbs are summed
+// over the CTA first: one global atomic per limb and CTA, thousands of warps adding into the same six words serialise in L2;
+// the high limb wraps as a signed sum, as flush_acc128 adds it).
+__device__ __forceinline__ void cd_flush(const CorpusDigestParams &P, const CdShared &S, int nrows, int who) {
+	long long *corp = P.k2.acc + (uint64_t)ACC_PER_CAND * P.k2.C;
+	if (who == 0) cd_census_flush(S.lo, S.hi, corp);
+	else if (who >= 1 && who <= 6) {
+		const int k = who - 1;
 		unsigned long long sum = 0;
-		for (int w = 0; w < (int)(blockDim.x >> 5); w++) sum += s_part[w][k];
+		for (int w = 0; w < nrows; w++) sum += S.part[w][k];
 		if (sum) atomicAdd((unsigned long long *)corp + (k < 3 ? CORP_REWARD + k : CORP_DIM + 4 * 2 + k - 3), sum);
 	}
-	if (tid == 0) cd_census_flush(s_lo, s_hi, corp);
-	corpus_tail(K, s_ex, &s_last, reinterpret_cast<unsigned long long *>(s_lut), 1024u);   // the LUT (8 KB) is done with: scratch of the tail
+}
+
+// The tail after the pass: ticket, examples, the last CTA finalises.  Block-wide; its first barrier orders the pass's adds
+// before the ticket.
+__device__ __forceinline__ void cd_tail(const CorpusDigestParams &P, CdShared &S) {
+	corpus_tail(P.k2, S.ex, &S.last, reinterpret_cast<unsigned long long *>(S.lut), 1024u);   // the LUT (8 KB) is done with: scratch of the tail
+}
+
+// The whole pass on one warp of the CTA (K1h): set-up, this CTA's share of the entries, the flush.  The caller then runs cd_tail
+// on every thread of the CTA.
+static __device__ __noinline__ void cd_warp(const CorpusDigestParams &P) {
+	CdShared &S = cd_shared();
+	const int lane = threadIdx.x & 31;
+	cd_setup(P, S, lane, 32);
+	__syncwarp();
+	const uint64_t n = P.fixed ? *P.n : 0, lo = n * blockIdx.x / gridDim.x, hi = n * (blockIdx.x + 1ull) / gridDim.x;
+	cd_entries(P, S, lo, 32, hi, 0);
+	__syncwarp();
+	cd_flush(P, S, 1, lane);
+}
+
+// The pass on every warp of the CTA (the stand-alone k_corpus_digest), then the tail.  Block-wide; every thread of every CTA
+// of the launch must enter.  Works for any blockDim.x that is a multiple of 32 (<= 1024).
+static __device__ __noinline__ void corpus_digest_block(const CorpusDigestParams &P) {
+	CdShared &S = cd_shared();
+	const int tid = threadIdx.x;
+	cd_setup(P, S, tid, blockDim.x);
+	__syncthreads();
+	const uint64_t n = P.fixed ? *P.n : 0, lo = n * blockIdx.x / gridDim.x, hi = n * (blockIdx.x + 1ull) / gridDim.x;
+	cd_entries(P, S, lo + (tid & ~31), blockDim.x, hi, tid >> 5);
+	__syncthreads();
+	cd_flush(P, S, blockDim.x >> 5, tid == 0 ? 0 : tid >= 32 && tid < 38 ? tid - 31 : -1);
+	cd_tail(P, S);
 }
 
 __device__ __forceinline__ unsigned long long score_key(double s) {
@@ -424,42 +513,47 @@ __device__ __forceinline__ apo_dimstat report_dimstat(const long long l[4]) {
 	return D;
 }
 
-// APO:498-625 / TCS:596-626 from the joined corpus block.  Block-wide: thread 0 the tallies, threads 1..9 one
-// dimension each, threads 10..15 one pattern each (a single thread walking all of it costs ~10 us of serial latency).
-static __device__ void build_report(const FinalizeParams &F, const long long *corp_g) {
+// APO:498-625 / TCS:596-626 from the joined corpus block.  Block-wide: the block's words below CORP_EX are staged into s_corp
+// (shared memory the caller lends, CORP_EX words) with one coalesced pass (a single thread loading them one by one between its
+// stores to the report pays a round trip to L2 per word), then thread 0 the tallies, threads 1..9 one dimension each, threads
+// 10..15 one pattern each.
+static __device__ void build_report(const FinalizeParams &F, const long long *corp_g, long long *s_corp) {
+	const long long *corp = s_corp;
 	apo_corpus_report &R = *F.report;
 	const int tid = threadIdx.x;
+	for (int i = tid; i < CORP_EX; i += blockDim.x) s_corp[i] = __ldcg(corp_g + i);
+	__syncthreads();
 	if (tid == 0) {
-		R.total = (uint64_t)__ldcg(corp_g + CORP_NREC);
-		const uint64_t good = (uint64_t)__ldcg(corp_g + CORP_TALLY), bad = (uint64_t)__ldcg(corp_g + CORP_TALLY + 1);
-		R.good = good; R.bad = bad; R.none = (uint64_t)__ldcg(corp_g + CORP_TALLY + 2);
+		R.total = (uint64_t)corp[CORP_NREC];
+		const uint64_t good = (uint64_t)corp[CORP_TALLY], bad = (uint64_t)corp[CORP_TALLY + 1];
+		R.good = good; R.bad = bad; R.none = (uint64_t)corp[CORP_TALLY + 2];
 		R.goodRate = report_good_rate(good, bad);                                                // APO:546-547
 		for (int m = 0; m < APO_NMODE; m++) {
 			uint64_t v[3];
-			for (int k = 0; k < 3; k++) { v[k] = (uint64_t)__ldcg(corp_g + CORP_MODE + 3 * m + k); R.byMode[m][k] = v[k]; }
+			for (int k = 0; k < 3; k++) { v[k] = (uint64_t)corp[CORP_MODE + 3 * m + k]; R.byMode[m][k] = v[k]; }
 			R.byModeGoodRate[m] = report_good_rate(v[1], v[2]);                                  // APO:541-544
 		}
 		long long l[4];
-		for (int q = 0; q < 4; q++) l[q] = __ldcg(corp_g + CORP_REWARD + q);
+		for (int q = 0; q < 4; q++) l[q] = corp[CORP_REWARD + q];
 		const uint64_t nrew = (uint64_t)l[3];
 		const double rsum = limbs_to_double(l);
 		R.withReward = nrew; R.rewardSum = rsum;
 		R.avgReward = report_avg_reward(rsum, nrew);
-		const uint64_t tc = (uint64_t)__ldcg(corp_g + CORP_TOOL), ts = (uint64_t)__ldcg(corp_g + CORP_TOOL + 1);
-		R.toolCalls = tc; R.toolSucc = ts; R.toolFail = (uint64_t)__ldcg(corp_g + CORP_TOOL + 2);
+		const uint64_t tc = (uint64_t)corp[CORP_TOOL], ts = (uint64_t)corp[CORP_TOOL + 1];
+		R.toolCalls = tc; R.toolSucc = ts; R.toolFail = (uint64_t)corp[CORP_TOOL + 2];
 		R.toolSuccessRate = tc > 0 ? __ddiv_rn((double)ts, (double)tc)                          // TCS:624
 		                           : __longlong_as_double(0x7ff8000000000000ll);
 	} else if (tid <= APO_NDIM) {
 		const int i = tid - 1;
 		long long l[4];
-		for (int q = 0; q < 4; q++) l[q] = __ldcg(corp_g + CORP_DIM + 4 * i + q);
+		for (int q = 0; q < 4; q++) l[q] = corp[CORP_DIM + 4 * i + q];
 		R.dim[i] = report_dimstat(l);
 	} else if (tid <= APO_NDIM + APO_NPAT) {
 		const int p = tid - 1 - APO_NDIM;
 		const uint64_t minc[APO_NPAT] = {2, 2, 3, 2, 2, 2};                                      // APO:645,671,695,715,736,756
-		const uint64_t bad = (uint64_t)__ldcg(corp_g + CORP_TALLY + 1);
+		const uint64_t bad = (uint64_t)corp[CORP_TALLY + 1];
 		apo_pattern Q;
-		Q.count = bad == 0 ? 0 : (uint64_t)__ldcg(corp_g + CORP_PAT + p);                       // APO:641
+		Q.count = bad == 0 ? 0 : (uint64_t)corp[CORP_PAT + p];                                  // APO:641
 		Q.flag = Q.count >= minc[p] ? 1 : 0;
 		uint8_t sev = 1;
 		if (p == 0 || p == 1) sev = Q.count >= 5 ? 2 : 1;                                    // APO:650,676
@@ -482,7 +576,7 @@ static __device__ void build_report(const FinalizeParams &F, const long long *co
 // Block-wide; every thread of the calling block must enter.  Works for any blockDim.x
 // that is a multiple of 32 (<= 1024).
 static __device__ __noinline__ void finalize_block(const FinalizeParams &F, unsigned long long *s_scratch, uint32_t scratch_keys) {
-	__shared__ unsigned int s_hist[256];
+	__shared__ __align__(8) unsigned int s_hist[256];          // also the report's stage (build_report), before the top-K
 	__shared__ unsigned long long s_prefix;
 	__shared__ unsigned int s_need, s_base_gt, s_base_eq, s_warp_gt[32], s_warp_eq[32];
 	const int tid = threadIdx.x, nth = blockDim.x, lane = tid & 31, warp = tid >> 5, nwarp = nth >> 5;
@@ -501,7 +595,8 @@ static __device__ __noinline__ void finalize_block(const FinalizeParams &F, unsi
 		F.keys[c] = score_key(s);
 		if (C <= scratch_keys) s_scratch[c] = score_key(s);
 	}
-	if (F.with_corpus) build_report(F, acc + (uint64_t)ACC_PER_CAND * C);
+	static_assert(CORP_EX * sizeof(long long) <= sizeof(s_hist), "the report's stage fits the histogram");
+	if (F.with_corpus) build_report(F, acc + (uint64_t)ACC_PER_CAND * C, reinterpret_cast<long long *>(s_hist));
 	__syncthreads();
 	const uint32_t K = F.K < C ? F.K : C;
 	if (K == 0) return;
@@ -689,9 +784,11 @@ static __device__ void finalize_and_publish(const FinalizeParams &F0, unsigned l
 		F.acc = F.join.joined;
 	} else if (threadIdx.x == 0) { meta->status = 0u; meta->pad = 0u; meta->join_wait_us = 0.f; meta->join_reduce_us = 0.f; }
 	const unsigned long long tf0 = globaltimer_ns();
+	kh_stamp(KH_ST_FIN0);
 	if (ok) finalize_block(F, s_scratch, scratch_keys);
 	__syncthreads();
 	const unsigned long long tf1 = globaltimer_ns();
+	kh_stamp(KH_ST_FIN1);
 	if (threadIdx.x == 0) { meta->finalize_us = (float)((tf1 - tf0) * 1e-3); meta->publish_us = 0.f; meta->entered_us = 0.f; meta->pad2 = 0u; }
 	if (F.host_out) {
 		__syncthreads();
@@ -712,6 +809,7 @@ static __device__ void finalize_and_publish(const FinalizeParams &F0, unsigned l
 		// the timer of this last step lands in the host copy only (the device block was already copied out)
 		reinterpret_cast<ResultMeta *>(F.host_out + F.meta_off)->publish_us = (float)((globaltimer_ns() - tf1) * 1e-3);
 	}
+	kh_stamp(KH_ST_PUBLISH);
 }
 
 }  // namespace apo

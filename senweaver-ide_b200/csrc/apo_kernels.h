@@ -283,6 +283,7 @@ struct KhParams {
 	const long long *tval;            // [n_tuples + 1] the table in entry order
 	int corpus_on;                    // every CTA then runs the digest pass over its share of cd's entries and the tail
 	CorpusDigestParams cd;            // (cd.fixed NULL: the tail alone, for a call without a corpus report)
+	uint64_t cd_n;                    // the digest's entry count as the host holds it (0 with cd.fixed NULL): picks each CTA's pass
 };
 cudaError_t run_reward9th(const KhParams &P, int sm_count, cudaStream_t st);
 // The counts of rows [0, R) of tl / th [R][tpitch] (evaluations t < T) into cnt [R][npitch] (npitch a multiple of 32, zeroed

@@ -365,19 +365,39 @@ cudaError_t run_reward9t2(Kt2Params P, int sm_count, cudaStream_t st) {
 }
 
 // =================================================================== K1h: whole rows of the Form T copy from its counts
-// Each CTA takes a contiguous range of the pair array (the rows' pairs back to back), finds its first row by a binary search
-// of the offsets and walks the rows the range covers; every warp flushes once per row.  Per pair: one 8-byte load, the
-// entry's table value through the read-only path (a row's entries ascend, so a warp's gathers land in neighbouring sectors)
-// and the exact 128-bit count * value.
+// Each CTA takes a contiguous range of the pair array (the rows' pairs back to back), finds its first row by a search of the
+// offsets and walks the rows the range covers; every warp flushes once per row.  Per pair: one 8-byte load, the entry's table
+// value through the read-only path (a row's entries ascend, so a warp's gathers land in neighbouring sectors) and the exact
+// 128-bit count * value.  With the corpus report the CTA's last warp runs its share of the digest pass meanwhile (cd_warp), so
+// only the ticket and the finalisation follow the stream.  One warp takes ~90 ns per digest entry where the CTA's stream takes
+// ~0.45 ns per pair (H100, DESIGN §8).  A CTA with fewer than KH_PAIRS_PER_ENTRY pairs per entry of its digest share (small C
+// or T), whose lone digest warp would outlast its stream by more than the block-wide pass costs after it, streams on all 32
+// warps and then runs the pass block-wide, as the stand-alone k_corpus_digest does.  The flagship has ~215 pairs per entry.
 constexpr int KH_THREADS = 1024;
 constexpr int KH_UNROLL = 8;                      // pairs in flight per thread
+constexpr uint64_t KH_PAIRS_PER_ENTRY = 128;
 
-// the rows of pairs [lo, hi) of one CTA
+#ifdef APO_K1H_DIAG
+// examples/flagship_launch.py: the phases of every CTA as %globaltimer stamps (kh_stamp, apo_corpus.cuh), and with
+// APO_K1H_DIAG=1 the stream alone: the gather replaced by a constant (its sums are not the table's)
+extern "C" int apo_diag_k1h_stamps(unsigned long long *out, uint32_t n) {
+	cudaError_t err = cudaMemcpyFromSymbol(out, g_kh_stamp, sizeof(unsigned long long) * (n < KH_STAMP_WORDS ? n : KH_STAMP_WORDS));
+	void *p = nullptr;
+	if (err == cudaSuccess) err = cudaGetSymbolAddress(&p, g_kh_stamp);
+	if (err == cudaSuccess) err = cudaMemset(p, 0, sizeof(g_kh_stamp));
+	return (int)err;
+}
+#endif
+
+// the rows of pairs [lo, hi) of one CTA, streamed by its first NT threads
+template <int NT, int DIAG>
 __device__ __forceinline__ void kh_rows(const KhParams &P, uint64_t lo, uint64_t hi, int tid, int lane) {
-	uint32_t a = 0, b = P.C;                                       // off[a] <= lo < off[b]
+	uint32_t a = 0, b = P.C;                                       // off[a] <= lo < off[b]: 32 offsets per step, not 2
 	while (b - a > 1) {
-		const uint32_t m = (a + b) / 2;
-		if (P.off[m] <= lo) a = m; else b = m;
+		const uint32_t step = (b - a + 31) / 32, i = a + (uint32_t)lane * step;
+		const unsigned le = __ballot_sync(0xffffffffu, i < b && P.off[i] <= lo);     // lane 0 (off[a]) always; the rest ascend
+		a += (31u - __clz(le)) * step;
+		b = min(a + step, b);
 	}
 	for (uint32_t c = a; c < P.C; c++) {
 		const uint64_t r0 = P.off[c], r1 = P.off[c + 1];
@@ -385,19 +405,20 @@ __device__ __forceinline__ void kh_rows(const KhParams &P, uint64_t lo, uint64_t
 		const uint64_t s = max(lo, r0), t = min(hi, r1);
 		Acc128 acc; acc.zero();
 		unsigned long long cnt = 0;
-		for (uint64_t p = s + tid; p < t; p += (uint64_t)KH_THREADS * KH_UNROLL) {
+		for (uint64_t p = s + tid; p < t; p += (uint64_t)NT * KH_UNROLL) {
 			unsigned long long w[KH_UNROLL];
 #pragma unroll
 			for (int u = 0; u < KH_UNROLL; u++) {
-				const uint64_t q = p + (uint64_t)u * KH_THREADS;
+				const uint64_t q = p + (uint64_t)u * NT;
 				if (q < t) { const uint2 v = ld_stream8(P.pairs + q); w[u] = (unsigned long long)v.x | ((unsigned long long)v.y << 32); }
 				else w[u] = 0;                                        // entry 0, count 0: adds nothing
 			}
 #pragma unroll
 			for (int u = 0; u < KH_UNROLL; u++) {
 				const unsigned long long n = w[u] >> KH_COUNT_SHIFT;
+				const uint32_t entry = (uint32_t)(w[u] & ((1u << KH_COUNT_SHIFT) - 1u));
 				int k;
-				const long long v = kt_split(__ldg(P.tval + (uint32_t)(w[u] & ((1u << KH_COUNT_SHIFT) - 1u))), k);
+				const long long v = kt_split(DIAG ? (1ll << KT_VALID_SHIFT) + entry : __ldg(P.tval + entry), k);
 				acc_add_mul(acc, n, v);
 				cnt += k ? n : 0ull;
 			}
@@ -410,12 +431,31 @@ __device__ __forceinline__ void kh_rows(const KhParams &P, uint64_t lo, uint64_t
 	}
 }
 
+template <int DIAG>
 __global__ void __launch_bounds__(KH_THREADS, 1)
 k_reward9th(const __grid_constant__ KhParams P) {      // grid constant: the digest pass reads P.cd in place, no per-thread copy
 	const int tid = threadIdx.x, lane = tid & 31;
+	kh_stamp(KH_ST_ENTRY);
 	const uint64_t lo = P.nnz * blockIdx.x / gridDim.x, hi = P.nnz * (blockIdx.x + 1ull) / gridDim.x;
-	if (lo < hi) kh_rows(P, lo, hi, tid, lane);
-	if (P.corpus_on) corpus_digest_block(P.cd);                       // every CTA, with or without pairs: block-wide
+	if (!P.corpus_on) {
+		if (lo < hi) kh_rows<KH_THREADS, DIAG>(P, lo, hi, tid, lane);
+		return;
+	}
+	const uint64_t share = P.cd_n * (blockIdx.x + 1ull) / gridDim.x - P.cd_n * blockIdx.x / gridDim.x;   // block-uniform
+	if (hi - lo < KH_PAIRS_PER_ENTRY * share) {                        // the digest share outlasts the pairs: all warps on both
+		if (lo < hi) kh_rows<KH_THREADS, DIAG>(P, lo, hi, tid, lane);
+		kh_stamp_max(KH_ST_PAIRS);
+		corpus_digest_block(P.cd);
+		return;
+	}
+	if (tid >= KH_THREADS - 32) {                                      // the last warp: this CTA's share of the digest
+		cd_warp(P.cd);
+		kh_stamp_max(KH_ST_DIGEST);
+	} else {
+		if (lo < hi) kh_rows<KH_THREADS - 32, DIAG>(P, lo, hi, tid, lane);
+		kh_stamp_max(KH_ST_PAIRS);
+	}
+	cd_tail(P.cd, cd_shared());                                        // every CTA, with or without pairs: block-wide
 }
 
 cudaError_t run_reward9th(const KhParams &P, int sm_count, cudaStream_t st) {
@@ -425,7 +465,13 @@ cudaError_t run_reward9th(const KhParams &P, int sm_count, cudaStream_t st) {
 	const uint64_t need = (P.nnz + KH_THREADS - 1) / KH_THREADS;
 	if ((uint64_t)grid > need) grid = (int)need;
 	if (grid < 1) grid = 1;                                                  // no pairs: one CTA for the corpus words and the tail
-	k_reward9th<<<grid, KH_THREADS, 0, st>>>(P);
+#ifdef APO_K1H_DIAG
+	if (const char *d = getenv("APO_K1H_DIAG"); d && atoi(d) == 1) {       // read per launch: one process alternates the variants
+		k_reward9th<1><<<grid, KH_THREADS, 0, st>>>(P);
+		return cudaGetLastError();
+	}
+#endif
+	k_reward9th<0><<<grid, KH_THREADS, 0, st>>>(P);
 	return cudaGetLastError();
 }
 
